@@ -425,9 +425,9 @@ constexpr size_t kSmemSlack = 1024 + 256;           // 1024-byte alignment of th
 size_t umma_stage_bytes(int nch) { return ((size_t)umma::kBlockM + 2 * 32 * (size_t)nch) * umma::kKB * 4; }     // A + B_hi + B_lo
 int umma_stages(int nch) { return (int)std::min<size_t>(6, (kSmemMax - kSmemSlack) / umma_stage_bytes(nch)); }
 size_t umma_smem(int nch, int stages) { return (size_t)stages * umma_stage_bytes(nch) + kSmemSlack; }
-// weight-gradient GEMM: two Bᵀ copies (hi, lo) of 32*nch rows x 128 bytes, then the ring of raw [A | B] k-blocks
-size_t dw_fixed_bytes(int nch) { return (size_t)2 * 32 * nch * 128; }
-size_t dw_stage_bytes(int nch) { return (size_t)32 * (128 + 32 * nch) * 4; }
+// weight-gradient GEMM: two buffers of two Bᵀ copies (hi, lo) of 32*nch rows x 128 bytes, then the ring of raw [A | B] k-blocks
+size_t dw_fixed_bytes(int nch) { return (size_t)2 * 2 * 32 * nch * 128; }
+size_t dw_stage_bytes(int nch) { return (size_t)32 * (umma::kDwAPitch + 32 * nch) * 4; }
 int dw_stages(int nch) { return (int)std::min<size_t>(6, (kSmemMax - kSmemSlack - dw_fixed_bytes(nch)) / dw_stage_bytes(nch)); }
 
 bool umma_supported(const ctr_handle* h) {
@@ -469,7 +469,9 @@ int umma_init(ctr_handle* h) {
     u.nch_h0 = (h->H0p + 31) / 32; u.nch_h1 = (h->H1p + 31) / 32; u.nch_dx = (u.bn_dx + 31) / 32;
     u.stages_h0 = umma_stages(u.nch_h0); u.stages_h1 = umma_stages(u.nch_h1); u.stages_dx = umma_stages(u.nch_dx);
     u.dw_stages0 = dw_stages(u.nch_h0); u.dw_stages1 = dw_stages(u.nch_h1);
-    if (std::min({u.stages_h0, u.stages_h1, u.stages_dx, u.dw_stages0, u.dw_stages1}) < 2)
+    // k_umma_dw frees a raw slot as soon as it is transposed, so its producer refills even a single slot while the
+    // wgmmas run; k_umma_gemm holds a slot until its wgmma group retires and needs two
+    if (std::min({u.stages_h0, u.stages_h1, u.stages_dx}) < 2 || std::min(u.dw_stages0, u.dw_stages1) < 1)
         return set_err(h, CTR_EINVAL, "wgmma GEMM: tile does not fit shared memory");
     for (int i = 0; i < 2; i++) {
         RET(dalloc(h, &u.Wt0[i], (size_t)h->H0p * h->Kp)); RET(dalloc(h, &u.Wt1[i], (size_t)h->H1p * h->H0p));
@@ -484,9 +486,9 @@ int umma_init(ctr_handle* h) {
     RET(make_map(h, &u.mA_dZ1, h->dZ1, h->Bmax, h->H1p, h->H1p, umma::kBlockM));
     RET(make_map(h, &u.mA_dZ0, h->dZ0, h->Bmax, h->H0p, h->H0p, umma::kBlockM));
     // weight-gradient operands: rows limited to the training batch so that TMA zero-fills the K tail; unswizzled
-    // {width, 32 samples} boxes (the A operand: 128 columns starting at the CTA's row block of C)
-    RET(make_map(h, &u.mK_X0, h->X0, c.batch, h->Kp, h->Kp, 32, CU_TENSOR_MAP_SWIZZLE_NONE, umma::kBlockM));
-    RET(make_map(h, &u.mK_H0d, h->H0d, c.batch, h->H0p, h->H0p, 32, CU_TENSOR_MAP_SWIZZLE_NONE, umma::kBlockM));
+    // {width, 32 samples} boxes (the A operand: kDwAPitch columns starting at the CTA's row block of C)
+    RET(make_map(h, &u.mK_X0, h->X0, c.batch, h->Kp, h->Kp, 32, CU_TENSOR_MAP_SWIZZLE_NONE, umma::kDwAPitch));
+    RET(make_map(h, &u.mK_H0d, h->H0d, c.batch, h->H0p, h->H0p, 32, CU_TENSOR_MAP_SWIZZLE_NONE, umma::kDwAPitch));
     RET(make_map(h, &u.mK_dZ0, h->dZ0, c.batch, h->H0p, h->H0p, 32, CU_TENSOR_MAP_SWIZZLE_NONE, 32 * u.nch_h0));
     RET(make_map(h, &u.mK_dZ1, h->dZ1, c.batch, h->H1p, h->H1p, 32, CU_TENSOR_MAP_SWIZZLE_NONE, 32 * u.nch_h1));
     CU(h, allow_smem_gemm<umma::UEPI_SIGMOID_DROP>(u.nch_h0)); CU(h, allow_smem_gemm<umma::UEPI_SIGMOID_DROP>(u.nch_h1));
