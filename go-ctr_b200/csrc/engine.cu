@@ -10,6 +10,7 @@
 #include "idmap.cuh"
 #include "item2vec.cuh"
 #include "mlp64.cuh"
+#include "knn.cuh"
 #include "comm.cuh"
 
 #include <nvtx3/nvToolsExt.h>
@@ -170,8 +171,9 @@ struct ctr_handle {
     unsigned long long idm_cap[2] = {0, 0}; int64_t idm_n[2] = {0, 0};
     long long *k_keys = nullptr, *k_host = nullptr; int* k_flags = nullptr;   // staging for ctr_batch_predict_keys (device, pinned host)
 
-    // grow-only device scratch of the host-buffer entry points (gather / window / id lookup): no cudaMalloc on the serving path
-    void* scratch[3] = {nullptr, nullptr, nullptr}; size_t scratch_cap[3] = {0, 0, 0};
+    // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search):
+    // no cudaMalloc on the serving path
+    void* scratch[4] = {nullptr, nullptr, nullptr, nullptr}; size_t scratch_cap[4] = {0, 0, 0, 0};
 
     Comm comm;
 };
@@ -989,6 +991,41 @@ static void i2v_build_paths(const std::vector<int64_t>& cnt, int V, int max_dept
     }
 }
 
+// ---- ctr_knn_search (knn.cuh) ----------------------------------------------------------------------------------------
+namespace {
+struct KnnArgs {
+    const double* qvec; const int* qrow; const int* excl; int nq, k; long rows_per_slice; int slices;
+    double* sl_sim; int* sl_row;
+};
+template <int QT, bool ROWQ>
+void knn_scan_launch(ctr_handle* h, const KnnArgs& a, size_t smem) {
+    const int T = CTR_TABLE_ITEM_EMB;
+    dim3 grid((a.nq + QT - 1) / QT, a.slices);
+    knn::k_knn_scan<QT, ROWQ><<<grid, knn::kThreads, smem, h->stream>>>(h->tab[T], h->tab_ld[T], (long)h->tab_rows[T], h->tab_width[T],
+                                                                       a.qvec, a.qrow, a.excl, a.nq, a.k, a.rows_per_slice, a.sl_sim, a.sl_row);
+}
+template <int QT, bool ROWQ>
+int knn_scan_occupancy(size_t smem) {
+    cudaFuncSetAttribute(knn::k_knn_scan<QT, ROWQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int n = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, knn::k_knn_scan<QT, ROWQ>, knn::kThreads, smem);
+    return std::max(n, 1);
+}
+// QT in {1, 2, 4, 8, 16}: the query-tile width the scan kernel was instantiated for
+template <bool ROWQ>
+int knn_scan_dispatch(ctr_handle* h, int QT, KnnArgs a, bool occupancy_only, size_t smem, int* occ) {
+    switch (QT) {
+        case 1:  if (occupancy_only) *occ = knn_scan_occupancy<1, ROWQ>(smem);  else knn_scan_launch<1, ROWQ>(h, a, smem);  break;
+        case 2:  if (occupancy_only) *occ = knn_scan_occupancy<2, ROWQ>(smem);  else knn_scan_launch<2, ROWQ>(h, a, smem);  break;
+        case 4:  if (occupancy_only) *occ = knn_scan_occupancy<4, ROWQ>(smem);  else knn_scan_launch<4, ROWQ>(h, a, smem);  break;
+        case 8:  if (occupancy_only) *occ = knn_scan_occupancy<8, ROWQ>(smem);  else knn_scan_launch<8, ROWQ>(h, a, smem);  break;
+        default: if (occupancy_only) *occ = knn_scan_occupancy<16, ROWQ>(smem); else knn_scan_launch<16, ROWQ>(h, a, smem); break;
+    }
+    return CTR_OK;
+}
+
+}  // namespace
+
 // =====================================================================================================
 extern "C" {
 
@@ -1073,7 +1110,7 @@ void ctr_destroy(ctr_handle* h) {
                     (void*)h->dUb, (void*)h->dIt, (void*)h->keys, (void*)h->keys2, (void*)h->pos, (void*)h->pos2, h->sort_tmp,
                     (void*)h->d_cost, (void*)h->s_user, (void*)h->s_item, (void*)h->s_hist, (void*)h->s_label, (void*)h->dXd, (void*)h->dYd, (void*)h->hot_acc, (void*)h->emb_m, (void*)h->emb_v})
         if (p) cudaFree(p);
-    for (int i = 0; i < 3; i++) if (h->scratch[i]) cudaFree(h->scratch[i]);
+    for (int i = 0; i < 4; i++) if (h->scratch[i]) cudaFree(h->scratch[i]);
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 2; i++) { if (h->ev_copied[i]) cudaEventDestroy(h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy(h->ev_consumed[i]); }
@@ -1892,6 +1929,79 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
     { cudaError_t e = auc_run(h->stream, pred, y, (long)n, auc); if (e != cudaSuccess) return set_err(h, CTR_ECUDA, "auc: %s", cudaGetErrorString(e)); return CTR_OK; }
+}
+
+int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
+                   int32_t* out_rows, double* out_sim, int32_t* out_count) {
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    if (k < 1 || k > knn::kMaxK || nq < 1 || (!queries && !query_rows) || !out_rows || !out_sim || !out_count)
+        return set_err(h, CTR_EINVAL, "bad knn arguments (k in [1, %d], nq >= 1, queries or query_rows, non-null outputs)", knn::kMaxK);
+    std::lock_guard<std::mutex> lk(h->mu);
+    const int T = CTR_TABLE_ITEM_EMB;
+    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+    if (h->tab_sharded[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB is row-sharded over %d ranks: search needs the whole table on one device", h->comm.world);
+    const int64_t N = h->tab_rows[T];
+    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+    const bool by_row = queries == nullptr;
+    if (query_rows) for (int64_t i = 0; i < nq; i++) {
+        const int32_t r = query_rows[i];
+        if (by_row && (r < 0 || r >= N)) return set_err(h, CTR_ENOTFOUND, "%d is not found in searcher", r);     // search.go:75-77
+        if (!by_row && (r < -1 || r >= N)) return set_err(h, CTR_EINVAL, "excluded row %d of query %lld outside [-1, %lld)", r, (long long)i, (long long)N);
+    }
+    CU(h, cudaSetDevice(h->dev));
+    const int D = h->tab_width[T], Dp = (D + 3) & ~3;
+    // query tile: as wide as the batch needs, narrower when k's lists would not fit shared memory
+    int QT = 16;
+    while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
+    const size_t smem = knn::kTileBytes + knn::smem_bytes(QT, Dp, k), msmem = knn::smem_bytes(1, 0, k);
+    int occ = 1;
+    if (by_row) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
+    // row slices: enough CTAs to fill the GPU with the least idle tail (whole waves of resident CTAs); queries are
+    // chunked so that the slices' lists stay within 256 MB of scratch
+    const long steps = (long)((N + knn::kStep - 1) / knn::kStep);
+    const long wave = (long)h->num_sms * occ;
+    int64_t chunk = std::min<int64_t>(nq, 1024);
+    int slices = 1;
+    for (;;) {
+        const long tiles = (long)((chunk + QT - 1) / QT);
+        double best = -1;
+        for (long m = 1; m <= 8; m++) {
+            const long s = std::max<long>(1, std::min<long>({(m * wave + tiles - 1) / tiles, steps, 4096}));
+            const double w = (double)(s * tiles) / wave, eff = w / std::ceil(w);
+            if (eff > best + 0.02) { best = eff; slices = (int)s; }
+        }
+        if (chunk == 1 || (size_t)chunk * slices * k * 12 <= ((size_t)256 << 20)) break;
+        chunk = (chunk + 1) / 2;
+    }
+    const long rps = (steps + slices - 1) / slices * knn::kStep;
+    slices = (int)((N + rps - 1) / rps);
+
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t b_q = al((size_t)chunk * D * 8), b_r = al((size_t)chunk * 4), b_ls = al((size_t)chunk * slices * k * 8),
+                 b_lr = al((size_t)chunk * slices * k * 4), b_os = al((size_t)chunk * k * 8), b_or = al((size_t)chunk * k * 4), b_oc = al((size_t)chunk * 4);
+    char* base = nullptr;
+    RET(scratch_get(h, 3, b_q + b_r + b_ls + b_lr + b_os + b_or + b_oc, (void**)&base));
+    double* d_q = (double*)base; int* d_r = (int*)(base + b_q);
+    double* d_ls = (double*)(base + b_q + b_r); int* d_lr = (int*)(base + b_q + b_r + b_ls);
+    double* d_os = (double*)(base + b_q + b_r + b_ls + b_lr); int* d_or = (int*)(base + b_q + b_r + b_ls + b_lr + b_os);
+    int* d_oc = (int*)(base + b_q + b_r + b_ls + b_lr + b_os + b_or);
+
+    for (int64_t s = 0; s < nq; s += chunk) {
+        const int n = (int)std::min<int64_t>(chunk, nq - s);
+        if (!by_row) CU(h, cudaMemcpyAsync(d_q, queries + s * D, (size_t)n * D * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+        if (query_rows) CU(h, cudaMemcpyAsync(d_r, query_rows + s, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+        const KnnArgs a{by_row ? nullptr : d_q, by_row ? d_r : nullptr, (!by_row && query_rows) ? d_r : nullptr, n, k, rps, slices, d_ls, d_lr};
+        RET(launch(h, "knn_scan", [&] {
+            int unused = 0;
+            if (by_row) knn_scan_dispatch<true>(h, QT, a, false, smem, &unused); else knn_scan_dispatch<false>(h, QT, a, false, smem, &unused);
+        }));
+        RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, d_or, d_os, d_oc); }));
+        CU(h, cudaMemcpyAsync(out_rows + s * k, d_or, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_sim + s * k, d_os, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_count + s, d_oc, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+    }
+    return CTR_OK;
 }
 
 int ctr_i2v_paths(const int64_t* count, int32_t V, int32_t max_depth, int64_t* path_off, int32_t* path_node, uint8_t* path_code, int64_t cap) {

@@ -11,14 +11,14 @@ from . import build as _build
 
 __all__ = ["Engine", "Config", "MLPClassifier", "MlpConfig", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
-           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND"]
+           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE"]
 
 MODEL_YOUTUBE, MODEL_DIN_COS, MODEL_DIN_EUC = 0, 1, 2
 TABLE_USER_FEAT, TABLE_ITEM_FEAT, TABLE_ITEM_EMB = 0, 1, 2
 TABLE_FROZEN, TABLE_SGD, TABLE_SGD_DETERMINISTIC, TABLE_ADAM = 0, 1, 2, 3
 GEMM_AUTO, GEMM_FP32, GEMM_TCGEN05_3XTF32 = 0, 1, 2
 IDMAP_USER, IDMAP_ITEM = 0, 1
-ENOTFOUND = 7
+EINVAL, ESTATE, ENOTFOUND = 1, 5, 7
 
 # every symbol include/ctr_b200.h declares (tests check the .so exports all of them)
 EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy", "ctr_last_error",
@@ -27,7 +27,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_create", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params"]
 
@@ -346,6 +346,26 @@ class Engine:
         auc = C.c_double(0)
         self._ck(self.L.ctr_roc_auc(self.h, pp, tp, C.c_int64(p.size), C.byref(auc)))
         return auc.value
+
+    def knn_search(self, k, queries=None, rows=None):
+        """search.Searcher on ITEM_EMB (ctr_knn_search): queries [nq, D] float64 vectors (rows: optional row to exclude
+        per query, -1 = none), or queries=None and rows = the query rows.  Returns (rows [nq, k] int32, sims [nq, k]
+        float64, counts [nq] int32); positions past a query's count hold row -1 and similarity 0."""
+        qp = rp = None
+        if queries is not None:
+            q = np.ascontiguousarray(queries, np.float64)
+            q = q.reshape(1, -1) if q.ndim == 1 else q
+            nq, qp = q.shape[0], q.ctypes.data_as(C.POINTER(C.c_double))
+        if rows is not None:
+            r, rp = _i(np.atleast_1d(rows))
+            nq = r.size if queries is None else nq
+            assert r.size == nq
+        if qp is None and rp is None:
+            raise ValueError("knn_search needs queries or rows")
+        out_r = np.empty((nq, k), np.int32); out_s = np.empty((nq, k), np.float64); cnt = np.empty(nq, np.int32)
+        self._ck(self.L.ctr_knn_search(self.h, qp, rp, C.c_int64(nq), C.c_int32(k), out_r.ctypes.data_as(_ip),
+                                       out_s.ctypes.data_as(C.POINTER(C.c_double)), cnt.ctypes.data_as(_ip)))
+        return out_r, out_s, cnt
 
 
 MLP_ACT = {"relu": 0, "logistic": 1, "identity": 2}

@@ -6,6 +6,8 @@
     vector.Save(f, dic, mat, ...)  word2vec text format           model/modelutil/vector/vector.go:40-67
     emb.Load(r) / parse / parseLine → []Embedding{Word,Dim,Vector,Norm}   emb/embedding.go:73-131
 
+    search.New(embs...) / SearchInternal / SearchVector → Neighbors        search/search.go:53-134
+
 The channel carries one WORD per message (cpsutil.ReadWord, cpsutil.go:46-53); ids are assigned by first
 appearance (dictionary.Add, dictionary.go:70-81)."""
 import ctypes as C
@@ -15,7 +17,7 @@ import numpy as np
 from . import engine as _e
 
 __all__ = ["i2v_paths", "I2vConfig", "I2vStats", "i2v_default_config", "i2v_train_ids", "i2v_train_dist", "TrainEmbedding", "EmbeddingModel",
-           "Embedding", "SaveVectors", "LoadVectors", "ParseLine"]
+           "Embedding", "SaveVectors", "LoadVectors", "ParseLine", "Neighbor", "Searcher", "neighbors_from_result"]
 
 
 class I2vConfig(C.Structure):
@@ -159,3 +161,76 @@ def SaveVectors(f, words, mat):
         raise ValueError("different for length of dic and row of matrix: %d, %d" % (len(words), mat.shape[0]))
     for w, row in zip(words, mat):
         f.write("%s " % w + "".join("%f " % float(v) for v in row) + "\n")
+
+
+# ---- search.Searcher: top-k cosine neighbours, scanned on the device (ctr_knn_search) ---------------------------
+class Neighbor:
+    """search.Neighbor (search.go:27-32); compares by value like the reference's reflect.DeepEqual."""
+    __slots__ = ("Word", "Rank", "Similarity")
+
+    def __init__(self, Word, Rank, Similarity):
+        self.Word, self.Rank, self.Similarity = Word, int(Rank), float(Similarity)
+
+    def __eq__(self, o):
+        return isinstance(o, Neighbor) and (self.Word, self.Rank, self.Similarity) == (o.Word, o.Rank, o.Similarity)
+
+    def __repr__(self):
+        return "Neighbor(%r, %d, %r)" % (self.Word, self.Rank, self.Similarity)
+
+
+def neighbors_from_result(words, rows, sims, count, k):
+    """One query's device result (rows, sims, true count) as the reference's Neighbors list.  When fewer than k items
+    qualify, search.go:126-133 sets k to the index of the LAST empty slot, i.e. k-1, and returns neighbors[:k-1]:
+    the qualifying items followed by zero Neighbor{} values, k-1 entries in all.  This mirror keeps that shape."""
+    out = [Neighbor(words[int(rows[i])], i + 1, float(sims[i])) for i in range(int(count))]
+    if count < k:
+        out += [Neighbor("", 0, 0.0) for _ in range(k - 1 - int(count))]
+    return out
+
+
+class Searcher:
+    """search.Searcher (search.go:53-134) over an ITEM_EMB table in HBM.  Similarities are bit-identical to search.go
+    run on the table's float32 values widened to float64; vectors loaded from text are rounded to float32 when
+    uploaded, so on those inputs parity holds up to that rounding.  Equal similarities rank by row ascending."""
+
+    def __init__(self, engine, words, vectors=None):
+        self.engine, self.words = engine, list(words)
+        self.rows = {}
+        for i, w in enumerate(self.words):
+            if w in self.rows:                 # item2vec dictionaries never repeat a word; Search would ignore both
+                raise ValueError("duplicate word %r in searcher" % w)
+            self.rows[w] = i
+        self.vectors = vectors                 # float64 [N, dim] of New(); None for a live table (from_engine)
+
+    @classmethod
+    def New(cls, *embs):
+        """search.New(embs...): validates (equal dims, emb.Embeddings.Validate), then uploads the vectors as float32
+        ITEM_EMB into an engine with D = dim and no feature tables."""
+        if embs and any(e.Dim != embs[0].Dim for e in embs):
+            raise ValueError("dimension for all vectors must be the same: %d" % embs[0].Dim)
+        if not embs:
+            raise ValueError("searcher needs at least one embedding")
+        dim = embs[0].Dim
+        vec = np.stack([e.Vector for e in embs]).astype(np.float64)
+        eng = _e.Engine(_e.default_config(_e.MODEL_DIN_COS, uP=0, cF=0, S=1, D=dim, batch=1, pred_batch=1))
+        eng.table_upload(_e.TABLE_ITEM_EMB, vec.astype(np.float32))
+        return cls(eng, [e.Word for e in embs], vec)
+
+    @classmethod
+    def from_engine(cls, eng, words):
+        """Searches eng's live ITEM_EMB (row i is words[i]) without copying it; SearchInternal then queries by row."""
+        return cls(eng, words)
+
+    def SearchInternal(self, word, k):
+        row = self.rows.get(word)
+        if row is None:
+            raise ValueError("%s is not found in searcher" % word)         # search.go:75-77
+        if self.vectors is not None:           # the word's own float64 vector, its row excluded (search.go:79)
+            r, s, c = self.engine.knn_search(k, queries=self.vectors[row:row + 1], rows=[row])
+        else:
+            r, s, c = self.engine.knn_search(k, rows=[row])
+        return neighbors_from_result(self.words, r[0], s[0], c[0], k)
+
+    def SearchVector(self, query, k):
+        r, s, c = self.engine.knn_search(k, queries=np.asarray(query, np.float64).reshape(1, -1))
+        return neighbors_from_result(self.words, r[0], s[0], c[0], k)

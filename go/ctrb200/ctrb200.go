@@ -163,6 +163,38 @@ func (e *Engine) BatchPredict(sampleKeys []rcmd.Sample) ([]float32, error) {
 	return y, e.err(rc)
 }
 
+// Search is search.Searcher (feature/embedding/search/search.go:66-134) over the ITEM_EMB table on the device: the k
+// rows most cosine-similar to each query. queries holds nq float64 vectors of the table's width (SearchVector; rows,
+// if not nil, names a row to exclude per query, -1 for none), or is nil and rows holds the query rows (SearchInternal,
+// with the word→row map on the Go side). outRows / sims are [nq*k] in rank order; counts[i] is the true number of
+// results of query i, the positions past it hold row -1 and similarity 0.
+func (e *Engine) Search(queries []float64, rows []int32, k int) (outRows []int32, sims []float64, counts []int32, err error) {
+	nq := len(rows)
+	var qp *C.double
+	var rp *C.int32_t
+	if len(queries) > 0 {
+		nq = len(queries) / int(e.cfg.D)
+		if rows != nil && len(rows) != nq {
+			return nil, nil, nil, fmt.Errorf("ctrb200: len(rows) must equal the number of queries")
+		}
+		qp = (*C.double)(unsafe.Pointer(&queries[0]))
+	}
+	if len(rows) > 0 {
+		rp = i32(rows)
+	}
+	if nq == 0 || k < 1 {
+		return nil, nil, nil, fmt.Errorf("ctrb200: Search needs at least one query and k >= 1")
+	}
+	outRows = make([]int32, nq*k)
+	sims = make([]float64, nq*k)
+	counts = make([]int32, nq)
+	rc := C.ctr_knn_search(e.h, qp, rp, C.int64_t(nq), C.int32_t(k), i32(outRows), (*C.double)(unsafe.Pointer(&sims[0])), i32(counts))
+	if err = e.err(rc); err != nil {
+		return nil, nil, nil, err
+	}
+	return outRows, sims, counts, nil
+}
+
 // SaveCheckpoint / LoadCheckpoint: binary snapshot of weights, Adam moments, step counter and tables.
 func (e *Engine) SaveCheckpoint(path string) error {
 	cs := C.CString(path)

@@ -234,6 +234,20 @@ int ctr_checkpoint_load(ctr_handle* h, const char* path);
  * scores grouped, trapezoid. Sorted on the device. */
 int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, double* auc);
 
+/* search.Searcher (feature/embedding/search/search.go:66-134): the k items of ITEM_EMB most cosine-similar to each
+ * query, on the device.  queries == NULL: search by row — query i is ITEM_EMB row query_rows[i] widened to float64 and
+ * excluded from its own result (SearchInternal, with the word→row map on the caller's side); a row outside [0, rows)
+ * is CTR_ENOTFOUND ("<row> is not found in searcher").  queries != NULL: search by the float64 vectors queries [nq, D]
+ * (SearchVector); query_rows may then be NULL or name a row to exclude per query (-1 = none).
+ * Similarities are bit-identical to search.go on the widened float32 table: Norm and Cosine in float64, sequential
+ * sums, dot / |q| / |v|; only similarities > 0 qualify.  Results come in rank order: similarity descending, equal
+ * similarities by row ascending.  out_rows / out_sim are [nq, k]; out_count[i] is the true number of results of query i,
+ * positions at or past it hold row -1 and similarity 0.  k in [1, 1024].  Needs only ITEM_EMB (a handle with
+ * uP = cF = 0 is enough); a row-sharded ITEM_EMB (world > 1, large table) is CTR_ESTATE, a replicated one is searched
+ * locally.  Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
+int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
+                   int32_t* out_rows, double* out_sim, int32_t* out_count);
+
 /* ---- item2vec (BASELINE config 5; SURVEY.md §8f row f1) ------------------------------------------------
  * embedding.TrainEmbedding(ch, window, dim, iter) (feature/embedding/wordemb.go:9-32): SkipGram +
  * HierarchicalSoftmax word2vec over the users' item sequences; its output is the ITEM_EMB table the hot
