@@ -344,7 +344,7 @@ int attn_forward(ctr_handle* h, const RowSrc& r, int B) {
     if (r.world > 1)        // row-sharded tables: the owner's HBM is read over NVLink (comm_check vetted the dims)
         return launch(h, "attn_fwd_peer", [&] { dispatch_fwd_idx<true>(h, r, B); });
     if (vec_ok(h, r) && idx_fwd_ok(h, r, B))
-        return launch(h, "attn_fwd_vec", [&] { dispatch_fwd_idx<false>(h, r, B); });
+        return launch(h, "attn_fwd_idx", [&] { dispatch_fwd_idx<false>(h, r, B); });
     if (vec_ok(h, r)) {
         return launch(h, "attn_fwd_vec", [&] {
             switch (h->cfg.D / 4) {           // float4 per row
@@ -362,7 +362,7 @@ int attn_backward(ctr_handle* h, const RowSrc& r, const BwdOut& o, int B) {
     if (r.world > 1)
         return launch(h, "attn_bwd_peer", [&] { dispatch_bwd_idx<true>(h, r, o, B); });
     if (vec_ok(h, r) && idx_bwd_ok(h, r, B))
-        return launch(h, "attn_bwd_vec", [&] { dispatch_bwd_idx<false>(h, r, o, B); });
+        return launch(h, "attn_bwd_idx", [&] { dispatch_bwd_idx<false>(h, r, o, B); });
     if (vec_ok(h, r)) {
         return launch(h, "attn_bwd_vec", [&] {
             switch (h->cfg.D / 4) {

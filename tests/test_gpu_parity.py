@@ -23,14 +23,21 @@ SHAPES = {"ref": (52, 10, 16, 53), "ns": (52, 50, 64, 53), "odd": (5, 3, 7, 5), 
 MODELS = [g.MODEL_YOUTUBE, g.MODEL_DIN_COS, g.MODEL_DIN_EUC]
 
 
-def setup(model, shape, B, seed=0, U=97, I=211, **kw):
-    uP, S, D, cF = SHAPES[shape]
+def setup(model, shape, B, seed=0, U=97, I=211, H0=200, H1=80, hot_rows=0, **kw):
+    """shape: a SHAPES name or a (uP, S, D, cF) tuple.  A zero-width feature table is not uploaded.  hot_rows: the
+    replicated hot-row count of the fused SGD scatter (cfg.reserved[0]: 0 = auto, < 0 = off)."""
+    uP, S, D, cF = SHAPES[shape] if isinstance(shape, str) else shape
     rng = np.random.default_rng(seed)
-    cfg = g.engine.default_config(model, uP=uP, S=S, D=D, cF=cF, batch=B, pred_batch=B, seed=seed + 5, **kw)
+    cfg = g.engine.default_config(model, uP=uP, S=S, D=D, cF=cF, H0=H0, H1=H1, batch=B, pred_batch=B, seed=seed + 5, **kw)
+    cfg.reserved[0] = hot_rows
     eng = g.Engine(cfg)
     uf, itf, emb = make_tables(rng, U, I, uP, cF, D)
-    eng.table_upload(g.TABLE_USER_FEAT, uf); eng.table_upload(g.TABLE_ITEM_FEAT, itf); eng.table_upload(g.TABLE_ITEM_EMB, emb)
-    ocfg = orc.make_cfg(model, uP, S, D, cF, 200, 80, cfg.dropout0, cfg.dropout1)
+    if uP:
+        eng.table_upload(g.TABLE_USER_FEAT, uf)
+    if cF:
+        eng.table_upload(g.TABLE_ITEM_FEAT, itf)
+    eng.table_upload(g.TABLE_ITEM_EMB, emb)
+    ocfg = orc.make_cfg(model, uP, S, D, cF, H0, H1, cfg.dropout0, cfg.dropout1)
     W = scaled_init(orc, ocfg, seed + 1)
     eng.set_weights(*W)
     batch = make_batch(rng, U, I, B, S)

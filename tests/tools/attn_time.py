@@ -33,10 +33,12 @@ def main():
     prof = {k: round(ms / n, 4) for k, (ms, n) in eng.profile_dump().items()}
     rows = sum(int((b[2] >= 0).sum()) + B for b in batches) / len(batches)
     fwd_b = rows * D * 4 + B * ((S + 2) * 4 + (uP + cF) * 4); bwd_b = 2 * rows * D * 4
+    # D=64, S=50 from row ids takes the index-route kernels (k_attn_fwd_idx / k_attn_bwd_idx)
+    fwd_ms, bwd_ms = prof.get("attn_fwd_idx", 1), prof.get("attn_bwd_idx", 1)
     out = {"rows": I, "zipf": zipf, "hot": hot, "ms": prof, "sum_ms": round(sum(prof.values()), 4),
-           "fwd_GBs": round(fwd_b / prof.get("attn_fwd_vec", 1) / 1e6), "bwd_GBs": round(bwd_b / prof.get("attn_bwd_vec", 1) / 1e6),
+           "fwd_GBs": round(fwd_b / fwd_ms / 1e6), "bwd_GBs": round(bwd_b / bwd_ms / 1e6),
            # fraction of the H100 SXM data sheet's 3.35 TB/s HBM3 bandwidth
-           "pair_frac_of_3350": round((fwd_b + bwd_b) / (prof.get("attn_fwd_vec", 1) + prof.get("attn_bwd_vec", 1)) / 1e6 / 3350.0, 4)}
+           "pair_frac_of_3350": round((fwd_b + bwd_b) / (fwd_ms + bwd_ms) / 1e6 / 3350.0, 4)}
     print(json.dumps(out))
 
 
