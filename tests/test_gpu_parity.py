@@ -23,12 +23,14 @@ SHAPES = {"ref": (52, 10, 16, 53), "ns": (52, 50, 64, 53), "odd": (5, 3, 7, 5), 
 MODELS = [g.MODEL_YOUTUBE, g.MODEL_DIN_COS, g.MODEL_DIN_EUC]
 
 
-def setup(model, shape, B, seed=0, U=97, I=211, H0=200, H1=80, hot_rows=0, **kw):
+def setup(model, shape, B, seed=0, U=97, I=211, H0=200, H1=80, hot_rows=0, pred_batch=None, **kw):
     """shape: a SHAPES name or a (uP, S, D, cF) tuple.  A zero-width feature table is not uploaded.  hot_rows: the
-    replicated hot-row count of the fused SGD scatter (cfg.reserved[0]: 0 = auto, < 0 = off)."""
+    replicated hot-row count of the fused SGD scatter (cfg.reserved[0]: 0 = auto, < 0 = off).  pred_batch defaults
+    to the training batch B."""
     uP, S, D, cF = SHAPES[shape] if isinstance(shape, str) else shape
     rng = np.random.default_rng(seed)
-    cfg = g.engine.default_config(model, uP=uP, S=S, D=D, cF=cF, H0=H0, H1=H1, batch=B, pred_batch=B, seed=seed + 5, **kw)
+    cfg = g.engine.default_config(model, uP=uP, S=S, D=D, cF=cF, H0=H0, H1=H1, batch=B, pred_batch=pred_batch or B,
+                                  seed=seed + 5, **kw)
     cfg.reserved[0] = hot_rows
     eng = g.Engine(cfg)
     uf, itf, emb = make_tables(rng, U, I, uP, cF, D)

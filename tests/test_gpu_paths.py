@@ -61,13 +61,14 @@ def edges(batch):
     return batch
 
 
-def oracle(model, dims, H0, H1, W, tabs, batch, training=False, seed=0, drop=(0.0, 0.0)):
+def oracle(model, dims, H0, H1, W, tabs, batch, training=False, seed=0, drop=(0.0, 0.0), step=0):
+    """The oracle's forward and backward of one batch; `step` is the handle's step counter (the dropout stream)."""
     uP, S, D, cF = dims
     (uf, itf, emb), (ur, ir, hist, y) = tabs, batch
     o = orc.make_cfg(model, uP, S, D, cF, H0, H1, *drop)
     ws = orc.Workspace(o, len(y))
     p, z = orc.forward(o, W, orc.gather_rows(uf, itf, emb, ur, ir, hist), orc.make_ranges(uP, S, D, cF),
-                       training=training, seed=seed, step=0, ws=ws)
+                       training=training, seed=seed, step=step, ws=ws)
     ref = orc.backward(o, W, ws, y)
     ref.update(p=p, logit=z)
     return ref
