@@ -15,7 +15,7 @@
 //                         shared-memory slots (cp.async), see the comments at the kernels;
 //   k_attn_{fwd,bwd}_vec  the same lane mapping for the dense-X compatibility route and S > 64;
 //   k_attn_{fwd,bwd}_gen  any D <= 256, unaligned sources (the reference test's D = 7), scalar loads.
-// Set CTR_ATTN_OLD=1 to route index-mode batches through the *_vec kernels (A/B checks).
+// _vec and _idx share their per-row math (attn_gate, bwd_coef, sum_subgroups); _gen keeps exact sqrtf / division.
 #pragma once
 #include "common.cuh"
 
@@ -45,8 +45,9 @@ struct HistIdx {
 // one history slot: pointer to the row (nullptr = zeros) and its table row id (-1 in dense mode)
 struct RowRef { const float* p; int idx; };
 
-__device__ __forceinline__ RowRef ub_ref(const RowSrc& r, const Dims& d, const HistIdx& hi,
-                                         bool use_hi, int b, int s) {
+// history ids come from hi when it holds them (index mode, S <= 64), else from r.hist
+__device__ __forceinline__ RowRef ub_ref(const RowSrc& r, const Dims& d, const HistIdx& hi, int b, int s) {
+    const bool use_hi = (!r.dense) && d.S <= 64;
     // every lane of the warp reaches the shuffle inside hi.get()
     int sidx = use_hi ? hi.get(s < d.S ? s : 0) : -1;
     RowRef o; o.p = nullptr; o.idx = -1;
@@ -55,10 +56,6 @@ __device__ __forceinline__ RowRef ub_ref(const RowSrc& r, const Dims& d, const H
     int idx = use_hi ? sidx : __ldg(r.hist + (long)b * d.S + s);
     if (row_ok(idx, r.n_emb)) { o.p = emb_row(r, idx); o.idx = idx; }
     return o;
-}
-__device__ __forceinline__ const float* ub_ptr(const RowSrc& r, const Dims& d, const HistIdx& hi,
-                                               bool use_hi, int b, int s) {
-    return ub_ref(r, d, hi, use_hi, b, s).p;
 }
 
 // MUFU-based reciprocal / sigmoid / sqrt for the attention gate, flush-to-zero forms (no denormal fix-up code
@@ -82,27 +79,70 @@ __device__ __forceinline__ float gate_cos(float dot, float nx2, float ny, float 
 }
 
 // -------------------------------------------------------------------------------------------------
-// forward, vector path.  Writes the MLP input row X0[b] = [uProfile | pooled | item | ctx | 0-pad].
-// A row of D = 4*LPR*VPL floats is covered by LPR lanes holding VPL float4 each (column block q of
-// lane l = (q*LPR + l)*4, so every load instruction of the group is one contiguous LPR*16-byte
-// segment); a warp therefore carries 32/LPR rows per instruction group and the scalar gate math is
-// amortised over them.
+// Per-row math of the _vec and _idx kernels.  A row of D = 4*LPR*VPL floats is covered by LPR lanes
+// holding VPL float4 each (column block q of lane l = (q*LPR + l)*4, so every load instruction of the
+// group is one contiguous LPR*16-byte segment); a warp therefore carries 32/LPR rows per instruction
+// group and the scalar gate math is amortised over them.
 // -------------------------------------------------------------------------------------------------
-// MODEL is a template parameter (no per-row branches); NT threads per block with at least MINB blocks
-// per SM: the micro-benchmark (tests/cuda/gather_probe.cu) shows occupancy, not software pipelining,
-// is what hides the gate's MUFU/shuffle latency — 32 warps/SM at <= 64 registers reach ~5.9 TB/s.
-template <int LPR, int VPL, int UNR, int MODEL, int NT, int MINB>
-__global__ void __launch_bounds__(NT, MINB)
+// 128 threads per block with at least 8 blocks per SM: the micro-benchmark (tests/cuda/gather_probe.cu)
+// shows occupancy, not software pipelining, is what hides the gate's MUFU/shuffle latency — 32 warps/SM
+// at <= 64 registers reach ~5.9 TB/s.
+constexpr int kAttnThreads = 128, kAttnMinBlocks = 8;
+
+// attention gate a of history row s, u, against the item row v (ny = |v|); att[s] reads as 0 beyond S.  MODEL is a
+// template parameter (no per-row branches); mean pooling has a = 1.
+template <int LPR, int VPL, int MODEL>
+__device__ __forceinline__ float attn_gate(const float4 (&u)[VPL], const float4 (&v)[VPL], float ny, const float* __restrict__ att,
+                                           int s, int S) {
+    float a = 1.0f;
+    if (MODEL == MODEL_DIN_COS) {
+        float dot = 0.0f, nx2 = 0.0f;
+#pragma unroll
+        for (int q = 0; q < VPL; q++) { dot += dot4(u[q], v[q]); nx2 += dot4(u[q], u[q]); }
+        dot = group_sum<LPR>(dot); nx2 = group_sum<LPR>(nx2);
+        const float cs = dot * frcp(fsqrt_pos(nx2) * ny + 1e-8f);
+        a = sigmoid_fast((cs + 1.0f) * 0.5f * (s < S ? __ldg(att + s) : 0.0f));
+    } else if (MODEL == MODEL_DIN_EUC) {
+        float d2 = 0.0f;
+#pragma unroll
+        for (int q = 0; q < VPL; q++) {
+            const float4 e = make_float4(u[q].x - v[q].x, u[q].y - v[q].y, u[q].z - v[q].z, u[q].w - v[q].w);
+            d2 += dot4(e, e);
+        }
+        a = sigmoid_fast((1.0f - fsqrt_pos(group_sum<LPR>(d2))) * (s < S ? __ldg(att + s) : 0.0f));
+    }
+    return a;
+}
+
+// x[q] += the same lane's x[q] in the other 32/LPR - 1 sub-groups of the warp
+template <int LPR, int VPL>
+__device__ __forceinline__ void sum_subgroups(float4 (&x)[VPL]) {
+#pragma unroll
+    for (int q = 0; q < VPL; q++) {
+#pragma unroll
+        for (int o = LPR; o < 32; o <<= 1) {
+            x[q].x += __shfl_xor_sync(0xffffffffu, x[q].x, o);
+            x[q].y += __shfl_xor_sync(0xffffffffu, x[q].y, o);
+            x[q].z += __shfl_xor_sync(0xffffffffu, x[q].z, o);
+            x[q].w += __shfl_xor_sync(0xffffffffu, x[q].w, o);
+        }
+    }
+}
+
+// -------------------------------------------------------------------------------------------------
+// forward, vector path.  Writes the MLP input row X0[b] = [uProfile | pooled | item | ctx | 0-pad].
+// -------------------------------------------------------------------------------------------------
+template <int LPR, int VPL, int MODEL>
+__global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks)
 k_attn_fwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
                float* __restrict__ X0, long ldx0, int Kp, int B) {
     extern __shared__ __align__(16) float smem[];
-    constexpr int RPW = 32 / LPR;
+    constexpr int RPW = 32 / LPR, NT = kAttnThreads;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int lir = lane % LPR, sub = lane / LPR;
     const int nwarps = gridDim.x * (NT / 32);
     float* row = smem + (long)wib * Kp;
     const float invS = 1.0f / (float)d.S;
-    const bool use_hi = (!r.dense) && d.S <= 64;
     // 128-bit copies of the dense per-sample features when every offset is 16-byte aligned
     const bool feat4 = (!r.dense) && (d.uP % 4 == 0) && (d.D % 2 == 0) && (r.ldu % 4 == 0) && (r.ldi % 4 == 0);
     const int nu4 = (d.uP + 3) / 4, nc4 = (d.cF + 3) / 4;
@@ -130,48 +170,17 @@ k_attn_fwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
         float4 acc[VPL];
 #pragma unroll
         for (int q = 0; q < VPL; q++) acc[q] = zero4();
-        for (int s0 = 0; s0 < d.S; s0 += UNR * RPW) {
-            float4 u[UNR][VPL];
+        for (int s0 = 0; s0 < d.S; s0 += RPW) {
+            const int s = s0 + sub;
+            const float* p = ub_ref(r, d, hi, b, s).p;
+            float4 u[VPL];
 #pragma unroll
-            for (int j = 0; j < UNR; j++) {               // UNR*VPL independent 128-bit loads in flight
-                const float* p = ub_ptr(r, d, hi, use_hi, b, s0 + j * RPW + sub);
+            for (int q = 0; q < VPL; q++) u[q] = p ? ldg4_stream(p + (q * LPR + lir) * 4) : zero4();
+            const float a = attn_gate<LPR, VPL, MODEL>(u, v, ny, att, s, d.S);
 #pragma unroll
-                for (int q = 0; q < VPL; q++) u[j][q] = p ? ldg4_stream(p + (q * LPR + lir) * 4) : zero4();
-            }
-#pragma unroll
-            for (int j = 0; j < UNR; j++) {
-                const int s = s0 + j * RPW + sub;
-                float a = 1.0f;
-                if (MODEL == MODEL_DIN_COS) {
-                    float dot = 0.0f, nx2 = 0.0f;
-#pragma unroll
-                    for (int q = 0; q < VPL; q++) { dot += dot4(u[j][q], v[q]); nx2 += dot4(u[j][q], u[j][q]); }
-                    dot = group_sum<LPR>(dot); nx2 = group_sum<LPR>(nx2);
-                    const float cs = dot * frcp(fsqrt_pos(nx2) * ny + 1e-8f);
-                    a = sigmoid_fast((cs + 1.0f) * 0.5f * (s < d.S ? __ldg(att + s) : 0.0f));
-                } else if (MODEL == MODEL_DIN_EUC) {
-                    float d2 = 0.0f;
-#pragma unroll
-                    for (int q = 0; q < VPL; q++) {
-                        const float4 e = make_float4(u[j][q].x - v[q].x, u[j][q].y - v[q].y, u[j][q].z - v[q].z, u[j][q].w - v[q].w);
-                        d2 += dot4(e, e);
-                    }
-                    a = sigmoid_fast((1.0f - fsqrt_pos(group_sum<LPR>(d2))) * (s < d.S ? __ldg(att + s) : 0.0f));
-                }
-#pragma unroll
-                for (int q = 0; q < VPL; q++) acc[q] = fma4(a, u[j][q], acc[q]);   // slots beyond S / missing rows carry u == 0
-            }
+            for (int q = 0; q < VPL; q++) acc[q] = fma4(a, u[q], acc[q]);   // slots beyond S / missing rows carry u == 0
         }
-#pragma unroll
-        for (int q = 0; q < VPL; q++) {
-#pragma unroll
-            for (int o = LPR; o < 32; o <<= 1) {
-                acc[q].x += __shfl_xor_sync(0xffffffffu, acc[q].x, o);
-                acc[q].y += __shfl_xor_sync(0xffffffffu, acc[q].y, o);
-                acc[q].z += __shfl_xor_sync(0xffffffffu, acc[q].z, o);
-                acc[q].w += __shfl_xor_sync(0xffffffffu, acc[q].w, o);
-            }
-        }
+        sum_subgroups<LPR, VPL>(acc);
         // assemble the concat row in shared memory, then one coalesced 128-bit store pass
         if (sub == 0) {
 #pragma unroll
@@ -209,7 +218,7 @@ __device__ __forceinline__ float4 ld4_peer(const float* p) {
 }
 template <bool PEER>
 __device__ __forceinline__ float* emb_ptr(const RowSrc& r, int idx) {
-    return PEER ? r.peer_emb[idx & r.wmask] + (long)(idx >> r.wshift) * r.lde : const_cast<float*>(r.emb) + (long)idx * r.lde;
+    return PEER ? shard_row(r, r.peer_emb, idx, r.lde) : const_cast<float*>(r.emb) + (long)idx * r.lde;
 }
 // read side of a sharded table: the replicated hot rows are local
 template <bool PEER>
@@ -222,10 +231,10 @@ __device__ __forceinline__ const float* emb_src(const RowSrc& r, int idx) {
 // this process (CUDA IPC): the gather reads the owner's HBM directly over NVLink — the transfer is the load itself, so
 // it overlaps the gate math of the other warps tile by tile — and keeps each fetched row in rows_cache for the
 // backward, so a row crosses NVLink once per step.
-template <int LPR, int VPL, int MODEL, bool PEER, int NT, int MINB>
-__global__ void __launch_bounds__(NT, MINB)
+template <int LPR, int VPL, int MODEL, bool PEER>
+__global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks)
 k_attn_fwd_idx(RowSrc r, Dims d, const float* __restrict__ att, float* __restrict__ X0, long ldx0, int Kp, int B) {
-    constexpr int RPW = 32 / LPR, DD = 4 * LPR * VPL;
+    constexpr int RPW = 32 / LPR, DD = 4 * LPR * VPL, NT = kAttnThreads;
     __shared__ __align__(16) float4 s_feat[NT];      // lane-private: this lane's feature chunk of the current sample
     __shared__ __align__(16) int4 s_ids[NT];         // lane-private: {hist id lane, hist id lane+32, item row, feature row} of the next sample
     const int lane = threadIdx.x & 31, lir = lane % LPR, sub = lane / LPR;
@@ -299,23 +308,7 @@ k_attn_fwd_idx(RowSrc r, Dims d, const float* __restrict__ att, float* __restric
         }
         for (int s0 = 0;;) {
             const int s = s0 + sub;
-            float a = 1.0f;
-            if (MODEL == MODEL_DIN_COS) {
-                float dot = 0.0f, nx2 = 0.0f;
-#pragma unroll
-                for (int q = 0; q < VPL; q++) { dot += dot4(u[q], v[q]); nx2 += dot4(u[q], u[q]); }
-                dot = group_sum<LPR>(dot); nx2 = group_sum<LPR>(nx2);
-                const float cs = dot * frcp(fsqrt_pos(nx2) * ny + 1e-8f);
-                a = sigmoid_fast((cs + 1.0f) * 0.5f * (s < d.S ? __ldg(att + s) : 0.0f));
-            } else if (MODEL == MODEL_DIN_EUC) {
-                float d2 = 0.0f;
-#pragma unroll
-                for (int q = 0; q < VPL; q++) {
-                    const float4 e = make_float4(u[q].x - v[q].x, u[q].y - v[q].y, u[q].z - v[q].z, u[q].w - v[q].w);
-                    d2 += dot4(e, e);
-                }
-                a = sigmoid_fast((1.0f - fsqrt_pos(group_sum<LPR>(d2))) * (s < d.S ? __ldg(att + s) : 0.0f));
-            }
+            const float a = attn_gate<LPR, VPL, MODEL>(u, v, ny, att, s, d.S);
 #pragma unroll
             for (int q = 0; q < VPL; q++) acc[q] = fma4(a, u[q], acc[q]);      // slots beyond S / missing rows carry u == 0
             if (PEER && cache_b && row >= 0) {
@@ -327,16 +320,7 @@ k_attn_fwd_idx(RowSrc r, Dims d, const float* __restrict__ att, float* __restric
             if (s0 >= d.S) break;
             load_rows(u, s0);
         }
-#pragma unroll
-        for (int q = 0; q < VPL; q++) {
-#pragma unroll
-            for (int o = LPR; o < 32; o <<= 1) {
-                acc[q].x += __shfl_xor_sync(0xffffffffu, acc[q].x, o);
-                acc[q].y += __shfl_xor_sync(0xffffffffu, acc[q].y, o);
-                acc[q].z += __shfl_xor_sync(0xffffffffu, acc[q].z, o);
-                acc[q].w += __shfl_xor_sync(0xffffffffu, acc[q].w, o);
-            }
-        }
+        sum_subgroups<LPR, VPL>(acc);
         float* xr = X0 + (long)b * ldx0;
         if (sub == 0) {
 #pragma unroll
@@ -368,7 +352,6 @@ k_attn_fwd_gen(RowSrc r, Dims d, int model, const float* __restrict__ att,
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nwarps = gridDim.x * (blockDim.x >> 5);
     const float invS = 1.0f / (float)d.S;
-    HistIdx hi; hi.i0 = hi.i1 = -1;
     for (int b = blockIdx.x * (blockDim.x >> 5) + wib; b < B; b += nwarps) {
         const float* ip = src_it(r, d, b);
         float vv[kGenAcc], acc[kGenAcc];
@@ -381,7 +364,7 @@ k_attn_fwd_gen(RowSrc r, Dims d, int model, const float* __restrict__ att,
         }
         const float ny = sqrtf(warp_sum(ny2));
         for (int s = 0; s < d.S; s++) {
-            const float* up = ub_ptr(r, d, hi, false, b, s);
+            const float* up = src_ub(r, d, b, s);
             float uu[kGenAcc]; float dot = 0.0f, nx2 = 0.0f, d2 = 0.0f;
 #pragma unroll
             for (int j = 0; j < kGenAcc; j++) {
@@ -449,12 +432,63 @@ __device__ __forceinline__ float* scatter_dst(const RowSrc& r, const Dims& d, co
     return o.scatter_base + (long)idx * r.lde;
 }
 
-template <int LPR, int VPL, int UNR, int MODEL, int NT, int MINB>
-__global__ void __launch_bounds__(NT, MINB)
+// Backward coefficients of history row s (u) for the lanes of its group: du = c1*g + c2*v + c3*u and
+// dv += c4*u - kv*v, where kv is added to kvsum.  The group's lane 0 (lead) adds d att_s to sdatt[s] while
+// s < S.  u is in registers; g and v are accessors q → float4 of this lane's chunk q, so that a kernel may
+// keep them in shared memory.  ny = |v|, rny = 1/|v| (0 for v = 0).
+struct DuCoef { float c1, c2, c3, c4; };
+template <int LPR, int VPL, int MODEL, typename GF, typename VF>
+__device__ __forceinline__ DuCoef bwd_coef(const float4 (&u)[VPL], GF g, VF v, float ny, float rny, float invS,
+                                           const float* __restrict__ att, int s, int S, bool lead, float* sdatt, float& kvsum) {
+    DuCoef c{invS, 0.0f, 0.0f, 0.0f};
+    if (MODEL != MODEL_YOUTUBE) {
+        const float att_s = s < S ? __ldg(att + s) : 0.0f;
+        float gu = 0.0f, dot = 0.0f, nx2 = 0.0f;
+#pragma unroll
+        for (int q = 0; q < VPL; q++) {
+            const float4 gq = g(q), vq = v(q);
+            gu += dot4(gq, u[q]);
+            if (MODEL == MODEL_DIN_COS) { dot += dot4(u[q], vq); nx2 += dot4(u[q], u[q]); }
+            else {
+                const float4 e = make_float4(u[q].x - vq.x, u[q].y - vq.y, u[q].z - vq.z, u[q].w - vq.w);
+                nx2 += dot4(e, e);
+            }
+        }
+        gu = group_sum<LPR>(gu); nx2 = group_sum<LPR>(nx2);
+        if (MODEL == MODEL_DIN_COS) {
+            dot = group_sum<LPR>(dot);
+            const float nx = fsqrt_pos(nx2);
+            const float iden = frcp(nx * ny + 1e-8f);
+            const float cs = dot * iden;
+            const float w = (cs + 1.0f) * 0.5f;
+            const float a = sigmoid_fast(w * att_s);
+            const float dz = gu * invS * a * (1.0f - a);
+            if (lead && s < S) atomicAdd(&sdatt[s], dz * w);
+            const float cc = 0.5f * dz * att_s;
+            c.c1 = a * invS; c.c2 = cc * iden; c.c4 = c.c2;
+            c.c3 = nx2 > 1e-30f ? -cc * cs * ny * iden * rsqrt_ftz(nx2) : 0.0f;   // -cc*cos*|v|/(|u| den)
+            kvsum += cc * cs * nx * iden * rny;                                 //  cc*cos*|u|/(|v| den)
+        } else {
+            const float dist = fsqrt_pos(nx2);
+            const float w = 1.0f - dist;
+            const float a = sigmoid_fast(w * att_s);
+            const float dz = gu * invS * a * (1.0f - a);
+            if (lead && s < S) atomicAdd(&sdatt[s], dz * w);
+            const float k = nx2 > 1e-30f ? dz * att_s * rsqrt_ftz(nx2) : 0.0f;  // dw/dist
+            c.c1 = a * invS; c.c3 = -k; c.c2 = k;      // du = c1 g - k (u - v)
+            c.c4 = s < S ? k : 0.0f;                   // dv += k (u - v)
+            kvsum += c.c4;
+        }
+    }
+    return c;
+}
+
+template <int LPR, int VPL, int MODEL>
+__global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks)
 k_attn_bwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
                const float* __restrict__ dX, long lddx, BwdOut o, int B) {
     extern __shared__ __align__(16) float smem[];     // datt partials [S]
-    constexpr int RPW = 32 / LPR;
+    constexpr int RPW = 32 / LPR, NT = kAttnThreads;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int lir = lane % LPR, sub = lane / LPR;
     const int gwarp = blockIdx.x * (NT / 32) + wib;
@@ -462,7 +496,6 @@ k_attn_bwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
     const int rep = o.hot_reps > 0 ? gwarp % o.hot_reps : 0;
     const float invS = 1.0f / (float)d.S;
     const float sc = o.sgd ? o.neg_lr : 1.0f;         // fused SGD: gradients leave pre-scaled by -lr
-    const bool use_hi = (!r.dense) && d.S <= 64;
     for (int j = threadIdx.x; j < d.S; j += NT) smem[j] = 0.0f;
     __syncthreads();
 
@@ -482,87 +515,32 @@ k_attn_bwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
         const float ny = fsqrt_pos(ny2);
         const float rny = ny2 > 1e-30f ? rsqrt_ftz(ny2) : 0.0f;
         float kvsum = 0.0f;                               // coefficient of -v in dv
-        for (int s0 = 0; s0 < d.S; s0 += UNR * RPW) {
-            float4 u[UNR][VPL]; int idx[UNR]; bool have[UNR];
+        for (int s0 = 0; s0 < d.S; s0 += RPW) {
+            const int s = s0 + sub;
+            const RowRef rr = ub_ref(r, d, hi, b, s);
+            float4 u[VPL];
 #pragma unroll
-            for (int j = 0; j < UNR; j++) {
-                const RowRef rr = ub_ref(r, d, hi, use_hi, b, s0 + j * RPW + sub);
-                idx[j] = rr.idx; have[j] = rr.p != nullptr;
+            for (int q = 0; q < VPL; q++) u[q] = rr.p ? *reinterpret_cast<const float4*>(rr.p + (q * LPR + lir) * 4) : zero4();
+            const DuCoef c = bwd_coef<LPR, VPL, MODEL>(u, [&](int q) { return g[q]; }, [&](int q) { return v[q]; }, ny, rny, invS,
+                                                       att, s, d.S, lir == 0, smem, kvsum);
+            if (s < d.S) {
+                const float e1 = c.c1 * sc, e2 = c.c2 * sc, e3 = c.c3 * sc;
+                float* dst = (o.sgd && rr.p) ? scatter_dst(r, d, o, rr.idx, rep) : nullptr;
 #pragma unroll
-                for (int q = 0; q < VPL; q++) u[j][q] = rr.p ? *reinterpret_cast<const float4*>(rr.p + (q * LPR + lir) * 4) : zero4();
-            }
-#pragma unroll
-            for (int j = 0; j < UNR; j++) {
-                const int s = s0 + j * RPW + sub;
-                // du = c1*g + c2*v + c3*u ; dv += c4*u - (kv coefficient)*v
-                float c1 = invS, c2 = 0.0f, c3 = 0.0f, c4 = 0.0f;
-                if (MODEL != MODEL_YOUTUBE) {
-                    const float att_s = s < d.S ? __ldg(att + s) : 0.0f;
-                    float gu = 0.0f, dot = 0.0f, nx2 = 0.0f;
-#pragma unroll
-                    for (int q = 0; q < VPL; q++) {
-                        gu += dot4(g[q], u[j][q]);
-                        if (MODEL == MODEL_DIN_COS) { dot += dot4(u[j][q], v[q]); nx2 += dot4(u[j][q], u[j][q]); }
-                        else {
-                            const float4 e = make_float4(u[j][q].x - v[q].x, u[j][q].y - v[q].y, u[j][q].z - v[q].z, u[j][q].w - v[q].w);
-                            nx2 += dot4(e, e);
-                        }
-                    }
-                    gu = group_sum<LPR>(gu); nx2 = group_sum<LPR>(nx2);
-                    if (MODEL == MODEL_DIN_COS) {
-                        dot = group_sum<LPR>(dot);
-                        const float nx = fsqrt_pos(nx2);
-                        const float iden = frcp(nx * ny + 1e-8f);
-                        const float cs = dot * iden;
-                        const float w = (cs + 1.0f) * 0.5f;
-                        const float a = sigmoid_fast(w * att_s);
-                        const float dz = gu * invS * a * (1.0f - a);
-                        if (lir == 0 && s < d.S) atomicAdd(&smem[s], dz * w);
-                        const float cc = 0.5f * dz * att_s;
-                        c1 = a * invS; c2 = cc * iden; c4 = c2;
-                        c3 = nx2 > 1e-30f ? -cc * cs * ny * iden * rsqrt_ftz(nx2) : 0.0f;     // -cc*cos*|v|/(|u| den)
-                        kvsum += cc * cs * nx * iden * rny;                               //  cc*cos*|u|/(|v| den)
-                    } else {
-                        const float dist = fsqrt_pos(nx2);
-                        const float w = 1.0f - dist;
-                        const float a = sigmoid_fast(w * att_s);
-                        const float dz = gu * invS * a * (1.0f - a);
-                        if (lir == 0 && s < d.S) atomicAdd(&smem[s], dz * w);
-                        const float k = nx2 > 1e-30f ? dz * att_s * rsqrt_ftz(nx2) : 0.0f;    // dw/dist
-                        c1 = a * invS; c3 = -k; c2 = k;      // du = c1 g - k (u - v)
-                        c4 = s < d.S ? k : 0.0f;             // dv += k (u - v)
-                        kvsum += c4;
-                    }
-                }
-                if (s < d.S) {
-                    const float e1 = c1 * sc, e2 = c2 * sc, e3 = c3 * sc;
-                    float* dst = (o.sgd && have[j]) ? scatter_dst(r, d, o, idx[j], rep) : nullptr;
-#pragma unroll
-                    for (int q = 0; q < VPL; q++) {
-                        const float4 uu = u[j][q];
-                        float4 du;
-                        du.x = fmaf(e3, uu.x, fmaf(e2, v[q].x, e1 * g[q].x)); du.y = fmaf(e3, uu.y, fmaf(e2, v[q].y, e1 * g[q].y));
-                        du.z = fmaf(e3, uu.z, fmaf(e2, v[q].z, e1 * g[q].z)); du.w = fmaf(e3, uu.w, fmaf(e2, v[q].w, e1 * g[q].w));
-                        dvu[q] = fma4(c4, uu, dvu[q]);
-                        if (o.dUb) *reinterpret_cast<float4*>(o.dUb + ((long)b * d.S + s) * d.D + (q * LPR + lir) * 4) = du;
-                        if (dst) red_add4(dst + (q * LPR + lir) * 4, du);
-                    }
+                for (int q = 0; q < VPL; q++) {
+                    float4 du;
+                    du.x = fmaf(e3, u[q].x, fmaf(e2, v[q].x, e1 * g[q].x)); du.y = fmaf(e3, u[q].y, fmaf(e2, v[q].y, e1 * g[q].y));
+                    du.z = fmaf(e3, u[q].z, fmaf(e2, v[q].z, e1 * g[q].z)); du.w = fmaf(e3, u[q].w, fmaf(e2, v[q].w, e1 * g[q].w));
+                    dvu[q] = fma4(c.c4, u[q], dvu[q]);
+                    if (o.dUb) *reinterpret_cast<float4*>(o.dUb + ((long)b * d.S + s) * d.D + (q * LPR + lir) * 4) = du;
+                    if (dst) red_add4(dst + (q * LPR + lir) * 4, du);
                 }
             }
         }
         // dv = gi + sum_subgroups(dvu) - (sum kv) * v
 #pragma unroll
         for (int of = LPR; of < 32; of <<= 1) kvsum += __shfl_xor_sync(0xffffffffu, kvsum, of);
-#pragma unroll
-        for (int q = 0; q < VPL; q++) {
-#pragma unroll
-            for (int of = LPR; of < 32; of <<= 1) {
-                dvu[q].x += __shfl_xor_sync(0xffffffffu, dvu[q].x, of);
-                dvu[q].y += __shfl_xor_sync(0xffffffffu, dvu[q].y, of);
-                dvu[q].z += __shfl_xor_sync(0xffffffffu, dvu[q].z, of);
-                dvu[q].w += __shfl_xor_sync(0xffffffffu, dvu[q].w, of);
-            }
-        }
+        sum_subgroups<LPR, VPL>(dvu);
         if (sub == 0) {
             float* dst = (o.sgd && ip) ? scatter_dst(r, d, o, r.item_row[b], rep) : nullptr;
 #pragma unroll
@@ -593,11 +571,11 @@ k_attn_bwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
 // PEER (row-sharded tables over NVLink, see k_attn_fwd_idx): rows are re-read from rows_cache (what the forward
 // fetched — the gradient is taken at the step-start table values, and nothing crosses NVLink twice), and each row
 // gradient leaves as red.global.add.v4.f32 straight into the OWNER's table over NVLink, pre-scaled by -lr/world.
-template <int LPR, int VPL, int MODEL, bool FUSED, bool PEER, int NT, int MINB>
-__global__ void __launch_bounds__(NT, MINB)
+template <int LPR, int VPL, int MODEL, bool FUSED, bool PEER>
+__global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks)
 k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
                const float* __restrict__ dX, long lddx, BwdOut o, int B) {
-    constexpr int RPW = 32 / LPR, CH = LPR * VPL;
+    constexpr int RPW = 32 / LPR, CH = LPR * VPL, NT = kAttnThreads;
     __shared__ float s_datt[64];
     __shared__ __align__(16) int4 s_ids[NT];
     __shared__ __align__(16) float4 s_g[NT / 32][CH], s_v[NT / 32][CH];
@@ -607,7 +585,7 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
     const int rep = o.hot_reps > 0 ? gwarp % o.hot_reps : 0;
     const float invS = 1.0f / (float)d.S;
     const float sc = FUSED ? o.neg_lr : 1.0f;         // fused SGD: gradients leave pre-scaled by -lr
-    if (threadIdx.x < 64) s_datt[threadIdx.x] = 0.0f;
+    if (MODEL != MODEL_YOUTUBE && threadIdx.x < 64) s_datt[threadIdx.x] = 0.0f;     // mean pooling has no att
     int* my_ids = reinterpret_cast<int*>(&s_ids[threadIdx.x]);
     *reinterpret_cast<int4*>(my_ids) = make_int4(-1, -1, -1, -1);
     __syncthreads();
@@ -622,6 +600,8 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
     };
     const float4* gs = s_g[wib];
     const float4* vs = s_v[wib];
+    auto g_of = [&](int q) { return gs[q * LPR + lir]; };       // this lane's chunk q of g / v
+    auto v_of = [&](int q) { return vs[q * LPR + lir]; };
     int b = gwarp;
     if (b < B) fetch_ids(b);
     while (b < B) {
@@ -651,65 +631,25 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
         __syncwarp();
         float ny2 = 0.0f;
 #pragma unroll
-        for (int q = 0; q < VPL; q++) { const float4 t = vs[q * LPR + lir]; ny2 += dot4(t, t); dvu[q] = zero4(); }
+        for (int q = 0; q < VPL; q++) { const float4 t = v_of(q); ny2 += dot4(t, t); dvu[q] = zero4(); }
         ny2 = group_sum<LPR>(ny2);
         const float ny = fsqrt_pos(ny2), rny = ny2 > 1e-30f ? rsqrt_ftz(ny2) : 0.0f;
         float kvsum = 0.0f;                               // coefficient of -v in dv
         for (int s0 = 0;;) {
             const int s = s0 + sub;
-            // du = c1*g + c2*v + c3*u ; dv += c4*u - (kv coefficient)*v
-            float c1 = invS, c2 = 0.0f, c3 = 0.0f, c4 = 0.0f;
-            if (MODEL != MODEL_YOUTUBE) {
-                const float att_s = s < d.S ? __ldg(att + s) : 0.0f;
-                float gu = 0.0f, dot = 0.0f, nx2 = 0.0f;
-#pragma unroll
-                for (int q = 0; q < VPL; q++) {
-                    const float4 gq = gs[q * LPR + lir], vq = vs[q * LPR + lir];
-                    gu += dot4(gq, u[q]);
-                    if (MODEL == MODEL_DIN_COS) { dot += dot4(u[q], vq); nx2 += dot4(u[q], u[q]); }
-                    else {
-                        const float4 e = make_float4(u[q].x - vq.x, u[q].y - vq.y, u[q].z - vq.z, u[q].w - vq.w);
-                        nx2 += dot4(e, e);
-                    }
-                }
-                gu = group_sum<LPR>(gu); nx2 = group_sum<LPR>(nx2);
-                if (MODEL == MODEL_DIN_COS) {
-                    dot = group_sum<LPR>(dot);
-                    const float nx = fsqrt_pos(nx2);
-                    const float iden = frcp(nx * ny + 1e-8f);
-                    const float cs = dot * iden;
-                    const float w = (cs + 1.0f) * 0.5f;
-                    const float a = sigmoid_fast(w * att_s);
-                    const float dz = gu * invS * a * (1.0f - a);
-                    if (lir == 0 && s < d.S) atomicAdd(&s_datt[s], dz * w);
-                    const float cc = 0.5f * dz * att_s;
-                    c1 = a * invS; c2 = cc * iden; c4 = c2;
-                    c3 = nx2 > 1e-30f ? -cc * cs * ny * iden * rsqrt_ftz(nx2) : 0.0f;   // -cc*cos*|v|/(|u| den)
-                    kvsum += cc * cs * nx * iden * rny;                               //  cc*cos*|u|/(|v| den)
-                } else {
-                    const float dist = fsqrt_pos(nx2);
-                    const float w = 1.0f - dist;
-                    const float a = sigmoid_fast(w * att_s);
-                    const float dz = gu * invS * a * (1.0f - a);
-                    if (lir == 0 && s < d.S) atomicAdd(&s_datt[s], dz * w);
-                    const float k = nx2 > 1e-30f ? dz * att_s * rsqrt_ftz(nx2) : 0.0f;  // dw/dist
-                    c1 = a * invS; c3 = -k; c2 = k;      // du = c1 g - k (u - v)
-                    c4 = s < d.S ? k : 0.0f;             // dv += k (u - v)
-                    kvsum += c4;
-                }
-            }
+            const DuCoef c = bwd_coef<LPR, VPL, MODEL>(u, g_of, v_of, ny, rny, invS, att, s, d.S, lir == 0, s_datt, kvsum);
             if (s < d.S) {
-                const float e1 = c1 * sc, e2 = c2 * sc, e3 = c3 * sc;
+                const float e1 = c.c1 * sc, e2 = c.c2 * sc, e3 = c.c3 * sc;
                 float* dst = nullptr;
                 if (FUSED) { if (row >= 0) dst = ((PEER && row >= o.hot_rows) ? emb_ptr<true>(r, row) : scatter_dst(r, d, o, row, rep)) + lir * 4; }
                 else if (o.dUb) dst = o.dUb + ((long)b * d.S + s) * d.D + lir * 4;
 #pragma unroll
                 for (int q = 0; q < VPL; q++) {
-                    const float4 gq = gs[q * LPR + lir], vq = vs[q * LPR + lir];
+                    const float4 gq = g_of(q), vq = v_of(q);
                     float4 du;
                     du.x = fmaf(e3, u[q].x, fmaf(e2, vq.x, e1 * gq.x)); du.y = fmaf(e3, u[q].y, fmaf(e2, vq.y, e1 * gq.y));
                     du.z = fmaf(e3, u[q].z, fmaf(e2, vq.z, e1 * gq.z)); du.w = fmaf(e3, u[q].w, fmaf(e2, vq.w, e1 * gq.w));
-                    dvu[q] = fma4(c4, u[q], dvu[q]);
+                    dvu[q] = fma4(c.c4, u[q], dvu[q]);
                     if (dst) { if (FUSED) red_add4(dst + q * LPR * 4, du); else *reinterpret_cast<float4*>(dst + q * LPR * 4) = du; }
                 }
             }
@@ -720,16 +660,7 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
         // dv = gi + sum_subgroups(dvu) - (sum kv) * v
 #pragma unroll
         for (int of = LPR; of < 32; of <<= 1) kvsum += __shfl_xor_sync(0xffffffffu, kvsum, of);
-#pragma unroll
-        for (int q = 0; q < VPL; q++) {
-#pragma unroll
-            for (int of = LPR; of < 32; of <<= 1) {
-                dvu[q].x += __shfl_xor_sync(0xffffffffu, dvu[q].x, of);
-                dvu[q].y += __shfl_xor_sync(0xffffffffu, dvu[q].y, of);
-                dvu[q].z += __shfl_xor_sync(0xffffffffu, dvu[q].z, of);
-                dvu[q].w += __shfl_xor_sync(0xffffffffu, dvu[q].w, of);
-            }
-        }
+        sum_subgroups<LPR, VPL>(dvu);
         if (sub == 0) {
             float* dst = nullptr;
             if (FUSED) { if (id.z >= 0) dst = ((PEER && id.z >= o.hot_rows) ? emb_ptr<true>(r, id.z) : scatter_dst(r, d, o, id.z, rep)) + lir * 4; }
@@ -737,7 +668,7 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
 #pragma unroll
             for (int q = 0; q < VPL; q++) {
                 const float4 gi = ldg4(dX + (long)b * lddx + d.D + (q * LPR + lir) * 4);
-                const float4 vq = vs[q * LPR + lir];
+                const float4 vq = v_of(q);
                 float4 dv;
                 dv.x = (gi.x + dvu[q].x - kvsum * vq.x) * sc; dv.y = (gi.y + dvu[q].y - kvsum * vq.y) * sc;
                 dv.z = (gi.z + dvu[q].z - kvsum * vq.z) * sc; dv.w = (gi.w + dvu[q].w - kvsum * vq.w) * sc;
@@ -817,7 +748,6 @@ k_attn_bwd_gen(RowSrc r, Dims d, int model, const float* __restrict__ att,
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nwarps = gridDim.x * (blockDim.x >> 5);
     const float invS = 1.0f / (float)d.S;
-    HistIdx hi; hi.i0 = hi.i1 = -1;
     for (int j = threadIdx.x; j < d.S; j += blockDim.x) smem[j] = 0.0f;
     __syncthreads();
     for (int b = blockIdx.x * (blockDim.x >> 5) + wib; b < B; b += nwarps) {
@@ -834,7 +764,7 @@ k_attn_bwd_gen(RowSrc r, Dims d, int model, const float* __restrict__ att,
         }
         const float ny = sqrtf(warp_sum(ny2));
         for (int s = 0; s < d.S; s++) {
-            const float* up = ub_ptr(r, d, hi, false, b, s);
+            const float* up = src_ub(r, d, b, s);
             float uu[kGenAcc], du[kGenAcc];
             float dot = 0.0f, nx2 = 0.0f, d2 = 0.0f, gu = 0.0f;
 #pragma unroll
@@ -911,13 +841,12 @@ __global__ void __launch_bounds__(256)
 k_gather_rows(RowSrc r, Dims d, float* __restrict__ X, long ldx, int B) {
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nwarps = gridDim.x * (blockDim.x >> 5);
-    HistIdx hi; hi.i0 = hi.i1 = -1;
     for (int b = blockIdx.x * (blockDim.x >> 5) + wib; b < B; b += nwarps) {
         float* x = X + (long)b * ldx;
         const float* pu = src_up(r, b);
         for (int j = lane; j < d.uP; j += 32) x[j] = pu ? __ldg(pu + j) : 0.0f;
         for (int s = 0; s < d.S; s++) {
-            const float* up = ub_ptr(r, d, hi, false, b, s);
+            const float* up = src_ub(r, d, b, s);
             for (int j = lane; j < d.D; j += 32) x[d.uP + (long)s * d.D + j] = up ? __ldg(up + j) : 0.0f;
         }
         const float* ip = src_it(r, d, b);
@@ -945,6 +874,18 @@ __global__ void k_scatter_keys(const int* __restrict__ hist, const int* __restri
     }
 }
 
+// element k of the gradient sum of the segment of equal keys that starts at i, in double, in ascending p
+__device__ __forceinline__ double segment_sum(const unsigned* __restrict__ keys, const unsigned* __restrict__ pos, long n, long i,
+                                              unsigned key, const float* __restrict__ dUb, const float* __restrict__ dIt, int S, int D, int k) {
+    double acc = 0.0;
+    for (long j = i; j < n && keys[j] == key; j++) {
+        unsigned p = pos[j];
+        int b = (int)(p / (unsigned)(S + 1)), sl = (int)(p % (unsigned)(S + 1));
+        if (k < D) acc += (double)(sl < S ? dUb[((long)b * S + sl) * D + k] : dIt[(long)b * D + k]);
+    }
+    return acc;
+}
+
 __global__ void __launch_bounds__(256)
 k_segment_sgd(const unsigned* __restrict__ keys, const unsigned* __restrict__ pos, long n,
               const float* __restrict__ dUb, const float* __restrict__ dIt, int S, int D,
@@ -958,12 +899,7 @@ k_segment_sgd(const unsigned* __restrict__ keys, const unsigned* __restrict__ po
         if (i > 0 && keys[i - 1] == key) continue;        // not a segment head
         for (int k0 = 0; k0 < D; k0 += 32) {
             int k = k0 + lane;
-            double acc = 0.0;
-            for (long j = i; j < n && keys[j] == key; j++) {
-                unsigned p = pos[j];
-                int b = (int)(p / (unsigned)(S + 1)), sl = (int)(p % (unsigned)(S + 1));
-                if (k < D) acc += (double)(sl < S ? dUb[((long)b * S + sl) * D + k] : dIt[(long)b * D + k]);
-            }
+            const double acc = segment_sum(keys, pos, n, i, key, dUb, dIt, S, D, k);
             if (k < D) {
                 float* e = emb + (long)key * lde + k;
                 *e = (float)((double)*e - (double)lr * acc);
@@ -996,12 +932,7 @@ k_segment_adam(const unsigned* __restrict__ keys, const unsigned* __restrict__ p
         if (i > 0 && keys[i - 1] == key) continue;        // not a segment head
         for (int k0 = 0; k0 < D; k0 += 32) {
             int k = k0 + lane;
-            double acc = 0.0;
-            for (long j = i; j < n && keys[j] == key; j++) {
-                unsigned p = pos[j];
-                int b = (int)(p / (unsigned)(S + 1)), sl = (int)(p % (unsigned)(S + 1));
-                if (k < D) acc += (double)(sl < S ? dUb[((long)b * S + sl) * D + k] : dIt[(long)b * D + k]);
-            }
+            const double acc = segment_sum(keys, pos, n, i, key, dUb, dIt, S, D, k);
             if (k < D) {
                 const long o = (long)key * lde + k;
                 float ww = emb[o], mm = mo[o], vv = vo[o];

@@ -185,8 +185,7 @@ int comm_check(ctr_handle* h) {
     if (!h->tab[CTR_TABLE_ITEM_EMB] || h->tab_width[CTR_TABLE_ITEM_EMB] != c.D) return set_err(h, CTR_ESTATE, "ITEM_EMB shard not uploaded");
     if (c.uP > 0 && !h->tab[CTR_TABLE_USER_FEAT]) return set_err(h, CTR_ESTATE, "USER_FEAT not uploaded");
     if (c.cF > 0 && !h->tab[CTR_TABLE_ITEM_FEAT]) return set_err(h, CTR_ESTATE, "ITEM_FEAT not uploaded");
-    const int lpr = c.D / 4;
-    if (c.D % 4 || lpr < 4 || lpr > 32 || (lpr & (lpr - 1)) || c.S > 64 || c.uP % 4 || (h->Kp - 2 * c.D) / 4 > 32)
+    if (!attn_idx_shape_ok(h, true))
         return set_err(h, CTR_EINVAL, "row-sharded tables need D in {16,32,64,128}, S <= 64, uP %% 4 == 0 and uP + cF <= 128");
     return CTR_OK;
 }

@@ -124,18 +124,23 @@ struct RowSrc {
 struct Dims { int uP, S, D, cF, in; };
 
 __device__ __forceinline__ bool row_ok(int idx, int n) { return (unsigned)idx < (unsigned)n; }
+// address of row idx of a row-sharded table whose shards are mapped at peer[0, world)
+template <typename T>
+__device__ __forceinline__ T* shard_row(const RowSrc& r, T* const* peer, int idx, long ld) {
+    return peer[idx & r.wmask] + (long)(idx >> r.wshift) * ld;
+}
 // address of ITEM_EMB row idx (must be valid)
 __device__ __forceinline__ const float* emb_row(const RowSrc& r, int idx) {
-    return r.world > 1 ? r.peer_emb[idx & r.wmask] + (long)(idx >> r.wshift) * r.lde : r.emb + (long)idx * r.lde;
+    return r.world > 1 ? shard_row(r, r.peer_emb, idx, r.lde) : r.emb + (long)idx * r.lde;
 }
 __device__ __forceinline__ const float* ifeat_row(const RowSrc& r, int idx) {
-    return r.ifeat_sharded ? r.peer_ifeat[idx & r.wmask] + (long)(idx >> r.wshift) * r.ldi : r.ifeat + (long)idx * r.ldi;
+    return r.ifeat_sharded ? shard_row(r, r.peer_ifeat, idx, r.ldi) : r.ifeat + (long)idx * r.ldi;
 }
 
 __device__ __forceinline__ const float* src_ub(const RowSrc& r, const Dims& d, int b, int s) {
     if (b >= r.nvalid) return nullptr;
     if (r.dense) return r.X + (long)b * r.ldx + r.ub0 + (long)s * d.D;
-    int idx = r.hist[(long)b * d.S + s];
+    int idx = __ldg(r.hist + (long)b * d.S + s);
     return row_ok(idx, r.n_emb) ? emb_row(r, idx) : nullptr;
 }
 __device__ __forceinline__ const float* src_it(const RowSrc& r, const Dims& d, int b) {

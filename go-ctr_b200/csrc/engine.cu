@@ -30,6 +30,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 using namespace ctr;
@@ -240,140 +241,129 @@ int grid_for_warps(const ctr_handle* h, int B) {
     return std::max(1, std::min(blocks, h->num_sms * 8));
 }
 
-bool vec_ok(const ctr_handle* h, const RowSrc& r) {
-    int D = h->cfg.D;
-    if (D % 4) return false;
-    int lpr = D / 4;
-    if (lpr < 4 || lpr > 32 || (lpr & (lpr - 1))) return false;      // D in {16,32,64,128}; others use the generic kernels
-    if (r.dense) return (r.ldx % 4 == 0) && (r.ub0 % 4 == 0) && (r.it0 % 4 == 0) && (((uintptr_t)r.X) % 16 == 0);
-    return r.lde % 4 == 0;
+// Attention kernel families (attn.cuh), in the order attn_path prefers them.  _peer is the _idx kernels' PEER
+// instantiation for row-sharded tables.
+enum AttnFamily { ATTN_PEER, ATTN_IDX, ATTN_VEC, ATTN_GEN };
+const char* const kAttnKey[2][4] = {       // profile / NVTX keys: [backward][family]
+    {"attn_fwd_peer", "attn_fwd_idx", "attn_fwd_vec", "attn_fwd_gen"},
+    {"attn_bwd_peer", "attn_bwd_idx", "attn_bwd_vec", "attn_bwd_gen"}};
+struct AttnPath { AttnFamily fwd, bwd; };
+
+// the lane maps of the _vec / _idx kernels (kLanes) cover D in {16, 32, 64, 128}
+bool attn_lanes_ok(int D) { return D == 16 || D == 32 || D == 64 || D == 128; }
+// The _idx kernels also need S <= 64 (two history ids per lane), and the _idx forward uP % 4 == 0 and (Kp - 2D)/4 <= 32
+// (one 16-byte feature chunk per lane).  Row-sharded tables run only on the _idx kernels: comm_check rejects other shapes.
+bool attn_idx_shape_ok(const ctr_handle* h, bool fwd) {
+    const ctr_config& c = h->cfg;
+    return attn_lanes_ok(c.D) && c.S <= 64 && (!fwd || (c.uP % 4 == 0 && (h->Kp - 2 * c.D) / 4 <= 32));
+}
+AttnPath attn_path(const ctr_handle* h, const RowSrc& r) {
+    if (r.world > 1) return {ATTN_PEER, ATTN_PEER};        // comm_check vetted the dims
+    const bool aligned = r.dense ? (r.ldx % 4 == 0) && (r.ub0 % 4 == 0) && (r.it0 % 4 == 0) && (((uintptr_t)r.X) % 16 == 0)
+                                 : r.lde % 4 == 0;
+    if (!attn_lanes_ok(h->cfg.D) || !aligned) return {ATTN_GEN, ATTN_GEN};
+    if (r.dense || !attn_idx_shape_ok(h, false)) return {ATTN_VEC, ATTN_VEC};
+    // the forward also moves the dense features in 16-byte chunks
+    const bool idx_fwd = attn_idx_shape_ok(h, true) && r.ldu % 4 == 0 && r.ldi % 4 == 0 && r.ufeat && r.ifeat;
+    return {idx_fwd ? ATTN_IDX : ATTN_VEC, ATTN_IDX};
 }
 
-// Lane mapping of the vector attention kernels for a row of D floats: LPR lanes x VPL float4 each, one
-// load group in flight per warp, 128-thread blocks at >= 6-8 blocks/SM: the gather is latency bound, so occupancy
-// rather than deeper per-warp unrolling keeps enough loads in flight (tests/cuda/gather_probe.cu, bwd_probe.cu).
+// Lane map of the _vec / _idx kernels for a row of D = 4·LPR·VPL floats: LPR lanes x VPL float4 each, one load group in
+// flight per warp, 128-thread blocks at 8 blocks/SM: the gather is latency bound, so occupancy rather than deeper
+// per-warp unrolling keeps enough loads in flight (tests/cuda/gather_probe.cu, bwd_probe.cu).
+struct Lanes { int lpr, vpl; };
+constexpr Lanes kLanes[2][2][4] = {        // [backward][PEER][D = 16, 32, 64, 128]
+    // forward.  PEER, D = 64: over NVLink the request size matters more than the shuffle count, so 8 lanes x 2 float4
+    // (128-byte contiguous segments per load instruction) rather than 4 x 4 (64-byte segments)
+    {{{4, 1}, {4, 2}, {4, 4}, {8, 4}}, {{4, 1}, {4, 2}, {8, 2}, {8, 4}}},
+    // backward.  D = 64: 8 x 2 (128-byte contiguous red.add / load segments per row) rather than 4 x 4, although the
+    // latter executes a third fewer instructions (tests/cuda/bwd_probe.cu compares them)
+    {{{4, 1}, {4, 2}, {8, 2}, {16, 2}}, {{4, 1}, {4, 2}, {8, 2}, {16, 2}}},
+};
+template <int LPR_, int VPL_> struct LaneMap { static constexpr int LPR = LPR_, VPL = VPL_; };
+template <bool BWD, bool PEER, int I> using lanes_at = LaneMap<kLanes[BWD][PEER][I].lpr, kLanes[BWD][PEER][I].vpl>;
+
+// f(LaneMap) for D in {16, 32, 64, 128}
+template <bool BWD, bool PEER, typename F>
+void with_lanes(int D, F&& f) {
+    switch (D) {
+        case 16: f(lanes_at<BWD, PEER, 0>{}); break;
+        case 32: f(lanes_at<BWD, PEER, 1>{}); break;
+        case 64: f(lanes_at<BWD, PEER, 2>{}); break;
+        default: f(lanes_at<BWD, PEER, 3>{}); break;
+    }
+}
+// f(std::integral_constant<int, MODEL>)
+template <typename F>
+void with_model(int model, F&& f) {
+    switch (model) {
+        case CTR_MODEL_YOUTUBE: f(std::integral_constant<int, MODEL_YOUTUBE>{}); break;
+        case CTR_MODEL_DIN_COS: f(std::integral_constant<int, MODEL_DIN_COS>{}); break;
+        default:                f(std::integral_constant<int, MODEL_DIN_EUC>{}); break;
+    }
+}
+
 int grid_attn(const ctr_handle* h, int B) {
     int blocks = (B + 3) / 4;
     return std::max(1, std::min(blocks, h->num_sms * 16));     // two waves of 8 resident blocks
 }
-template <int LPR, int VPL, int MINB>
-void launch_fwd_vec(ctr_handle* h, const RowSrc& r, int B) {
-    size_t smem = (size_t)4 * h->Kp * sizeof(float);
-    const int g = grid_attn(h, B);
-    switch (h->cfg.model) {
-        case CTR_MODEL_YOUTUBE: k_attn_fwd_vec<LPR, VPL, 1, MODEL_YOUTUBE, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-        case CTR_MODEL_DIN_COS: k_attn_fwd_vec<LPR, VPL, 1, MODEL_DIN_COS, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-        default:                k_attn_fwd_vec<LPR, VPL, 1, MODEL_DIN_EUC, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-    }
-}
-template <int LPR, int VPL, int MINB>
-void launch_bwd_vec(ctr_handle* h, const RowSrc& r, const BwdOut& o, int B) {
-    size_t smem = (size_t)std::max(h->cfg.S, 1) * sizeof(float);
-    const int g = grid_attn(h, B);
-    switch (h->cfg.model) {
-        case CTR_MODEL_YOUTUBE: k_attn_bwd_vec<LPR, VPL, 1, MODEL_YOUTUBE, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->dX, h->lddx, o, B); break;
-        case CTR_MODEL_DIN_COS: k_attn_bwd_vec<LPR, VPL, 1, MODEL_DIN_COS, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->dX, h->lddx, o, B); break;
-        default:                k_attn_bwd_vec<LPR, VPL, 1, MODEL_DIN_EUC, 128, MINB><<<g, 128, smem, h->stream>>>(r, dims_of(h), h->W[3], h->dX, h->lddx, o, B); break;
-    }
-}
-
-// index-mode fast kernels (k_attn_fwd_idx / k_attn_bwd_idx): conditions beyond vec_ok
-bool idx_fwd_ok(const ctr_handle* h, const RowSrc& r, int B) {
-    static const bool off = getenv("CTR_ATTN_OLD") != nullptr;
-    const ctr_config& c = h->cfg;
-    return !off && !r.dense && c.S <= 64 && c.uP % 4 == 0 && r.ldu % 4 == 0 && r.ldi % 4 == 0 && (h->Kp - 2 * c.D) / 4 <= 32 &&
-           r.ufeat && r.ifeat;
-}
-bool idx_bwd_ok(const ctr_handle* h, const RowSrc& r, int B) {
-    static const bool off = getenv("CTR_ATTN_OLD") != nullptr;
-    return !off && !r.dense && h->cfg.S <= 64;
-}
-template <int LPR, int VPL, int MINB, bool PEER>
-void launch_fwd_idx(ctr_handle* h, const RowSrc& r, int B) {
-    const int g = grid_attn(h, B);
-    switch (h->cfg.model) {
-        case CTR_MODEL_YOUTUBE: k_attn_fwd_idx<LPR, VPL, MODEL_YOUTUBE, PEER, 128, MINB><<<g, 128, 0, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-        case CTR_MODEL_DIN_COS: k_attn_fwd_idx<LPR, VPL, MODEL_DIN_COS, PEER, 128, MINB><<<g, 128, 0, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-        default:                k_attn_fwd_idx<LPR, VPL, MODEL_DIN_EUC, PEER, 128, MINB><<<g, 128, 0, h->stream>>>(r, dims_of(h), h->W[3], h->X0, h->Kp, h->Kp, B); break;
-    }
-}
-template <int LPR, int VPL, int MINB, bool PEER>
-void launch_bwd_idx(ctr_handle* h, const RowSrc& r, const BwdOut& o, int B) {
-    const int g = grid_attn(h, B);
-#define BWD_CASE(M) { if (o.sgd) k_attn_bwd_idx<LPR, VPL, M, true, PEER, 128, MINB><<<g, 128, 0, h->stream>>>(r, dims_of(h), h->W[3], h->dX, h->lddx, o, B); \
-                      else       k_attn_bwd_idx<LPR, VPL, M, false, PEER, 128, MINB><<<g, 128, 0, h->stream>>>(r, dims_of(h), h->W[3], h->dX, h->lddx, o, B); }
-    switch (h->cfg.model) {
-        case CTR_MODEL_YOUTUBE: BWD_CASE(MODEL_YOUTUBE) break;
-        case CTR_MODEL_DIN_COS: BWD_CASE(MODEL_DIN_COS) break;
-        default:                BWD_CASE(MODEL_DIN_EUC) break;
-    }
-#undef BWD_CASE
-}
-template <bool PEER>
-void dispatch_fwd_idx(ctr_handle* h, const RowSrc& r, int B) {
-    if (PEER && h->cfg.D == 64) {
-        // over NVLink the request size matters more than the shuffle count: 8 lanes x 2 float4 (128-byte contiguous
-        // segments per load instruction) by default, the local kernels' 4 x 4 mapping (64-byte segments) or 16 x 1
-        // (256-byte) on request (tests/tools/shard_time.py compares them).  CTR_PEER_FWD_MAP: 0 = 4x4, 2 = 16x1.
-        static const int map = getenv("CTR_PEER_FWD_MAP") ? atoi(getenv("CTR_PEER_FWD_MAP")) : 1;
-        if (map == 1) { launch_fwd_idx<8, 2, 8, PEER>(h, r, B); return; }
-        if (map == 2) { launch_fwd_idx<16, 1, 8, PEER>(h, r, B); return; }
-    }
-    switch (h->cfg.D / 4) {
-        case 4: launch_fwd_idx<4, 1, 8, PEER>(h, r, B); break;    case 8: launch_fwd_idx<4, 2, 8, PEER>(h, r, B); break;
-        case 16: launch_fwd_idx<4, 4, 8, PEER>(h, r, B); break;
-        default: launch_fwd_idx<8, 4, 8, PEER>(h, r, B); break;
-    }
-}
-template <bool PEER>
-void dispatch_bwd_idx(ctr_handle* h, const RowSrc& r, const BwdOut& o, int B) {
-    if (PEER && h->cfg.D == 64) {
-        static const int map = getenv("CTR_PEER_BWD_MAP") ? atoi(getenv("CTR_PEER_BWD_MAP")) : 0;
-        if (map == 2) { launch_bwd_idx<16, 1, 8, PEER>(h, r, o, B); return; }
-    }
-    switch (h->cfg.D / 4) {
-        case 4: launch_bwd_idx<4, 1, 8, PEER>(h, r, o, B); break;    case 8: launch_bwd_idx<4, 2, 8, PEER>(h, r, o, B); break;
-        // D = 64: 8 lanes x 2 float4 (128-byte contiguous red.add / load segments per row) rather than 4 x 4 (64-byte
-        // segments), although the latter executes a third fewer instructions (tests/cuda/bwd_probe.cu compares them)
-        case 16: launch_bwd_idx<8, 2, 8, PEER>(h, r, o, B); break;
-        default: launch_bwd_idx<16, 2, 8, PEER>(h, r, o, B); break;
-    }
-}
 
 int attn_forward(ctr_handle* h, const RowSrc& r, int B) {
-    if (r.world > 1)        // row-sharded tables: the owner's HBM is read over NVLink (comm_check vetted the dims)
-        return launch(h, "attn_fwd_peer", [&] { dispatch_fwd_idx<true>(h, r, B); });
-    if (vec_ok(h, r) && idx_fwd_ok(h, r, B))
-        return launch(h, "attn_fwd_idx", [&] { dispatch_fwd_idx<false>(h, r, B); });
-    if (vec_ok(h, r)) {
-        return launch(h, "attn_fwd_vec", [&] {
-            switch (h->cfg.D / 4) {           // float4 per row
-                case 4: launch_fwd_vec<4, 1, 8>(h, r, B); break;    case 8: launch_fwd_vec<4, 2, 8>(h, r, B); break;
-                case 16: launch_fwd_vec<4, 4, 8>(h, r, B); break;   default: launch_fwd_vec<8, 4, 8>(h, r, B); break;
-            }
+    const AttnFamily f = attn_path(h, r).fwd;
+    return launch(h, kAttnKey[0][f], [&] {
+        const Dims d = dims_of(h);
+        const int g = grid_attn(h, B);
+        if (f == ATTN_GEN) {
+            k_attn_fwd_gen<<<grid_for_warps(h, B), 256, 0, h->stream>>>(r, d, h->cfg.model, h->W[3], h->X0, h->Kp, h->Kp, B);
+            return;
+        }
+        with_model(h->cfg.model, [&](auto m) {
+            constexpr int M = decltype(m)::value;
+            auto idx = [&](auto peer) {
+                constexpr bool P = decltype(peer)::value;
+                with_lanes<false, P>(h->cfg.D, [&](auto l) {
+                    using L = decltype(l);
+                    k_attn_fwd_idx<L::LPR, L::VPL, M, P><<<g, kAttnThreads, 0, h->stream>>>(r, d, h->W[3], h->X0, h->Kp, h->Kp, B);
+                });
+            };
+            if (f == ATTN_PEER) idx(std::true_type{});
+            else if (f == ATTN_IDX) idx(std::false_type{});
+            else with_lanes<false, false>(h->cfg.D, [&](auto l) {
+                using L = decltype(l);
+                const size_t smem = (size_t)(kAttnThreads / 32) * h->Kp * sizeof(float);
+                k_attn_fwd_vec<L::LPR, L::VPL, M><<<g, kAttnThreads, smem, h->stream>>>(r, d, h->W[3], h->X0, h->Kp, h->Kp, B);
+            });
         });
-    }
-    return launch(h, "attn_fwd_gen", [&] {
-        k_attn_fwd_gen<<<grid_for_warps(h, B), 256, 0, h->stream>>>(r, dims_of(h), h->cfg.model, h->W[3], h->X0, h->Kp, h->Kp, B);
     });
 }
 
 int attn_backward(ctr_handle* h, const RowSrc& r, const BwdOut& o, int B) {
-    if (r.world > 1)
-        return launch(h, "attn_bwd_peer", [&] { dispatch_bwd_idx<true>(h, r, o, B); });
-    if (vec_ok(h, r) && idx_bwd_ok(h, r, B))
-        return launch(h, "attn_bwd_idx", [&] { dispatch_bwd_idx<false>(h, r, o, B); });
-    if (vec_ok(h, r)) {
-        return launch(h, "attn_bwd_vec", [&] {
-            switch (h->cfg.D / 4) {
-                case 4: launch_bwd_vec<4, 1, 8>(h, r, o, B); break;    case 8: launch_bwd_vec<4, 2, 8>(h, r, o, B); break;
-                case 16: launch_bwd_vec<8, 2, 8>(h, r, o, B); break;   default: launch_bwd_vec<16, 2, 8>(h, r, o, B); break;
-            }
+    const AttnFamily f = attn_path(h, r).bwd;
+    return launch(h, kAttnKey[1][f], [&] {
+        const Dims d = dims_of(h);
+        const int g = grid_attn(h, B);
+        const size_t datt_smem = (size_t)std::max(h->cfg.S, 1) * sizeof(float);
+        if (f == ATTN_GEN) {
+            k_attn_bwd_gen<<<grid_for_warps(h, B), 256, datt_smem, h->stream>>>(r, d, h->cfg.model, h->W[3], h->dX, h->lddx, o, B);
+            return;
+        }
+        with_model(h->cfg.model, [&](auto m) {
+            constexpr int M = decltype(m)::value;
+            auto idx = [&](auto peer) {
+                constexpr bool P = decltype(peer)::value;
+                with_lanes<true, P>(h->cfg.D, [&](auto l) {
+                    using L = decltype(l);
+                    if (o.sgd) k_attn_bwd_idx<L::LPR, L::VPL, M, true, P><<<g, kAttnThreads, 0, h->stream>>>(r, d, h->W[3], h->dX, h->lddx, o, B);
+                    else       k_attn_bwd_idx<L::LPR, L::VPL, M, false, P><<<g, kAttnThreads, 0, h->stream>>>(r, d, h->W[3], h->dX, h->lddx, o, B);
+                });
+            };
+            if (f == ATTN_PEER) idx(std::true_type{});
+            else if (f == ATTN_IDX) idx(std::false_type{});
+            else with_lanes<true, false>(h->cfg.D, [&](auto l) {
+                using L = decltype(l);
+                k_attn_bwd_vec<L::LPR, L::VPL, M><<<g, kAttnThreads, datt_smem, h->stream>>>(r, d, h->W[3], h->dX, h->lddx, o, B);
+            });
         });
-    }
-    return launch(h, "attn_bwd_gen", [&] {
-        size_t smem = (size_t)std::max(h->cfg.S, 1) * sizeof(float);
-        k_attn_bwd_gen<<<grid_for_warps(h, B), 256, smem, h->stream>>>(r, dims_of(h), h->cfg.model, h->W[3], h->dX, h->lddx, o, B);
     });
 }
 
@@ -541,8 +531,7 @@ int umma_dw(ctr_handle* h, const char* name, int nch, const CUtensorMap& mA, con
 // the weight-gradient GEMMs run on the tensor cores when the padded widths fit 8 column chunks and the batch
 // is the configured training batch (the TMA maps zero-fill rows beyond it)
 bool use_umma_dw(const ctr_handle* h, int B) {
-    static const bool off = getenv("CTR_DW_FP32") != nullptr;
-    return B == h->cfg.batch && h->Kp <= 256 && h->H0p <= 256 && h->H1p <= 256 && !off;
+    return B == h->cfg.batch && h->Kp <= 256 && h->H0p <= 256 && h->H1p <= 256;
 }
 
 bool use_umma(const ctr_handle* h) {
@@ -676,8 +665,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
         a.p = h->P; a.logit = h->Z; a.dZ1 = bwd ? h->dZ1 : nullptr; a.lddz = h->H1p; a.dW2 = h->G[2]; a.cost_sum = h->d_cost;
         // few, long-lived blocks: every block ends with H1 same-address atomics (dW2) and one on the cost — with one block per
         // 64 rows those serialised in L2 (~27 cycles each per address) and cost more than the 50 MB the kernel streams
-        static const int hb = getenv("CTR_HEAD_BLOCKS") ? atoi(getenv("CTR_HEAD_BLOCKS")) : 2;
-        const int hgrid = std::max(1, std::min((B + 63) / 64, h->num_sms * std::max(1, hb)));
+        const int hgrid = std::max(1, std::min((B + 63) / 64, h->num_sms * 2));
         RET(launch(h, bwd ? "head_fwd_bwd" : "head_fwd", [&] { k_head<<<hgrid, 256, 0, h->stream>>>(a); }));
     }
     if (!bwd) return CTR_OK;
@@ -731,7 +719,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
         // replicated table: the all-reduced sum is the global-batch gradient the row solver consumes)
         bo.neg_lr = (adam_rows ? 1.0f : -c.table_lr) * o.grad_scale;
         bo.scatter_base = o.table_grad ? o.table_grad : h->tab[CTR_TABLE_ITEM_EMB];
-        const bool hot = bo.sgd && vec_ok(h, r) && !o.comm;
+        const bool hot = bo.sgd && attn_path(h, r).bwd != ATTN_GEN && !o.comm;
         if (hot) { RET(ensure_hot(h)); bo.hot_acc = h->hot_acc; bo.hot_rows = h->hot_rows; bo.hot_reps = h->hot_reps; }
         const bool peer_hot = o.peer && bo.sgd && h->comm.hot_k > 0;
         if (peer_hot) { bo.hot_acc = h->comm.hot_acc; bo.hot_rows = h->comm.hot_k; bo.hot_reps = h->comm.hot_reps; }
@@ -2228,8 +2216,7 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
             I2vArgs a{}; a.doc = d_doc; a.nd = nd; a.z = d_z; a.poff = d_poff; a.pnode = d_pnode; a.pcode = d_pcode; a.syn0 = d_syn0; a.syn1 = d_syn1;
             a.D = D; a.W = W; a.lr_tab = d_lr; a.upd = c.update_lr_batch; a.seed = c.seed; a.iter = it; a.counters = d_ctr;
             a.node_scale = d_nsc; a.word_scale = d_wsc;
-            static const bool no_hot = getenv("CTR_I2V_NO_HOT") != nullptr;
-            a.hot_n = no_hot ? 0 : std::min(kI2vHot, n_inner); a.hot_base = n_inner - a.hot_n;      // the last nodes created = the top of the tree
+            a.hot_n = std::min(kI2vHot, n_inner); a.hot_base = n_inner - a.hot_n;      // the last nodes created = the top of the tree
             const size_t sm = (size_t)std::max(a.hot_n, 1) * D * sizeof(float);
             CI(cudaEventRecord(e0, st));
             for (long p0 = 0; p0 < std::max<long>(nd_max_global, 1); p0 += seg) {
