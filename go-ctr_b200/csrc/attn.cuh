@@ -14,7 +14,8 @@
 //                         fast path — next-sample ids and the dense features travel through lane-private
 //                         shared-memory slots (cp.async), see the comments at the kernels;
 //   k_attn_{fwd,bwd}_vec  the same lane mapping for the dense-X compatibility route and S > 64;
-//   k_attn_{fwd,bwd}_gen  any D <= 256, unaligned sources (the reference test's D = 7), scalar loads.
+//   k_attn_{fwd,bwd}_gen  any D <= 256, unaligned sources (the reference test's D = 7), scalar loads;
+//   k_attn_fwd_user       one user against a run of consecutive items (ctr_recommend_topk), history in shared memory.
 // _vec and _idx share their per-row math (attn_gate, bwd_coef, sum_subgroups); _gen keeps exact sqrtf / division.
 #pragma once
 #include "common.cuh"
@@ -337,6 +338,81 @@ k_attn_fwd_idx(RowSrc r, Dims d, const float* __restrict__ att, float* __restric
         }
         if (bn >= B) break;
         b = bn;
+    }
+}
+
+// -------------------------------------------------------------------------------------------------
+// forward, one user against a run of consecutive items (ctr_recommend_topk): X0[b] is the MLP input row of the sample
+// (user, item i0 + b, hist[0, S)) for b < B; every item i0 + b must be a row of ITEM_EMB.  Each CTA stages the user's
+// S history rows (zeros for missing slots) in shared memory once; a warp then reads only its item's ITEM_EMB and
+// ITEM_FEAT rows.  Same lane map and per-row math as k_attn_fwd_idx / _vec (attn_gate, fma4 in s0 order,
+// sum_subgroups), so every row is bit-identical to the row they write for the same sample.  The profile row and the
+// zero pad are the same for every item: each warp writes them once into its staging row.
+// Dynamic shared memory: user_smem_floats(S, D, Kp) floats.  Two blocks fewer per SM than the gather kernels (80
+// registers): the history comes from shared memory, so fewer loads need to be in flight, and the cosine gate at D >= 64
+// fits without spills.
+// -------------------------------------------------------------------------------------------------
+__host__ __device__ inline size_t user_smem_floats(int S, int D, int Kp) { return (size_t)S * D + (size_t)(kAttnThreads / 32) * Kp; }
+
+template <int LPR, int VPL, int MODEL>
+__global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks - 2)
+k_attn_fwd_user(RowSrc r, Dims d, const float* __restrict__ att, int user, const int* __restrict__ hist, int i0,
+                float* __restrict__ X0, long ldx0, int Kp, int B) {
+    extern __shared__ __align__(16) float smem[];
+    constexpr int RPW = 32 / LPR, DD = 4 * LPR * VPL, NT = kAttnThreads;
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int lir = lane % LPR, sub = lane / LPR;
+    const int nwarps = gridDim.x * (NT / 32);
+    float4* s_hist = reinterpret_cast<float4*>(smem);                 // [S][DD/4]
+    float* row = smem + (long)d.S * DD + (long)wib * Kp;              // this warp's MLP input row
+    for (int i = threadIdx.x; i < d.S * (DD / 4); i += NT) {
+        const int s = i / (DD / 4), c = i - s * (DD / 4);
+        const int idx = __ldg(hist + s);
+        s_hist[i] = row_ok(idx, r.n_emb) ? ldg4(r.emb + (long)idx * r.lde + 4 * c) : zero4();
+    }
+    const float* pu = row_ok(user, r.n_user) ? r.ufeat + (long)user * r.ldu : nullptr;
+    for (int j = lane; j < d.uP; j += 32) row[j] = pu ? __ldg(pu + j) : 0.0f;
+    for (int j = d.in + lane; j < Kp; j += 32) row[j] = 0.0f;
+    __syncthreads();
+    const float invS = 1.0f / (float)d.S;
+
+    for (int b = blockIdx.x * (NT / 32) + wib; b < B; b += nwarps) {
+        const int item = i0 + b;
+        const float* ip = r.emb + (long)item * r.lde;
+        float4 v[VPL];
+        float ny2 = 0.0f;
+#pragma unroll
+        for (int q = 0; q < VPL; q++) { v[q] = ldg4(ip + (q * LPR + lir) * 4); ny2 += dot4(v[q], v[q]); }
+        const float ny = fsqrt_pos(group_sum<LPR>(ny2));
+        float4 acc[VPL];
+#pragma unroll
+        for (int q = 0; q < VPL; q++) acc[q] = zero4();
+        for (int s0 = 0; s0 < d.S; s0 += RPW) {
+            const int s = s0 + sub;
+            float4 u[VPL];
+#pragma unroll
+            for (int q = 0; q < VPL; q++) u[q] = s < d.S ? s_hist[s * (DD / 4) + q * LPR + lir] : zero4();
+            const float a = attn_gate<LPR, VPL, MODEL>(u, v, ny, att, s, d.S);
+#pragma unroll
+            for (int q = 0; q < VPL; q++) acc[q] = fma4(a, u[q], acc[q]);   // slots beyond S / missing rows carry u == 0
+        }
+        sum_subgroups<LPR, VPL>(acc);
+        if (sub == 0) {
+#pragma unroll
+            for (int q = 0; q < VPL; q++) {
+                float* p1 = row + d.uP + (q * LPR + lir) * 4;
+                p1[0] = acc[q].x * invS; p1[1] = acc[q].y * invS; p1[2] = acc[q].z * invS; p1[3] = acc[q].w * invS;
+                float* p2 = p1 + d.D;
+                p2[0] = v[q].x; p2[1] = v[q].y; p2[2] = v[q].z; p2[3] = v[q].w;
+            }
+        }
+        const float* pc = row_ok(item, r.n_ifeat) ? r.ifeat + (long)item * r.ldi : nullptr;
+        for (int j = lane; j < d.cF; j += 32) row[d.uP + 2 * d.D + j] = pc ? __ldg(pc + j) : 0.0f;
+        __syncwarp();
+        float4* dst = reinterpret_cast<float4*>(X0 + (long)b * ldx0);
+        const float4* src4 = reinterpret_cast<const float4*>(row);
+        for (int j = lane; j < Kp / 4; j += 32) dst[j] = src4[j];
+        __syncwarp();
     }
 }
 

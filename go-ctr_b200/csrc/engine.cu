@@ -11,6 +11,7 @@
 #include "item2vec.cuh"
 #include "mlp64.cuh"
 #include "knn.cuh"
+#include "rec.cuh"
 #include "comm.cuh"
 
 #include <nvtx3/nvToolsExt.h>
@@ -172,9 +173,10 @@ struct ctr_handle {
     unsigned long long idm_cap[2] = {0, 0}; int64_t idm_n[2] = {0, 0};
     long long *k_keys = nullptr, *k_host = nullptr; int* k_flags = nullptr;   // staging for ctr_batch_predict_keys (device, pinned host)
 
-    // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search):
-    // no cudaMalloc on the serving path
-    void* scratch[4] = {nullptr, nullptr, nullptr, nullptr}; size_t scratch_cap[4] = {0, 0, 0, 0};
+    // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search;
+    // slot 4: ctr_recommend_topk): no cudaMalloc on the serving path
+    static constexpr int kScratch = 5;
+    void* scratch[kScratch] = {}; size_t scratch_cap[kScratch] = {};
 
     Comm comm;
 };
@@ -333,6 +335,42 @@ int attn_forward(ctr_handle* h, const RowSrc& r, int B) {
                 const size_t smem = (size_t)(kAttnThreads / 32) * h->Kp * sizeof(float);
                 k_attn_fwd_vec<L::LPR, L::VPL, M><<<g, kAttnThreads, smem, h->stream>>>(r, d, h->W[3], h->X0, h->Kp, h->Kp, B);
             });
+        });
+    });
+}
+
+// k_attn_fwd_user (ctr_recommend_topk) runs where the _vec / _idx lane maps cover D, the ITEM_EMB rows are 16-byte
+// aligned and the user's history rows fit the opt-in shared memory; other shapes fill index buffers for attn_forward.
+size_t attn_user_smem(const ctr_handle* h) { return user_smem_floats(h->cfg.S, h->cfg.D, h->Kp) * sizeof(float); }
+bool attn_user_ok(const ctr_handle* h, size_t smem_optin) {
+    return attn_lanes_ok(h->cfg.D) && h->tab_ld[CTR_TABLE_ITEM_EMB] % 4 == 0 && attn_user_smem(h) <= smem_optin;
+}
+// f(kernel) for the handle's model and D
+template <typename F>
+void with_user_kernel(const ctr_handle* h, F&& f) {
+    with_model(h->cfg.model, [&](auto m) {
+        constexpr int M = decltype(m)::value;
+        with_lanes<false, false>(h->cfg.D, [&](auto l) { using L = decltype(l); f(k_attn_fwd_user<L::LPR, L::VPL, M>); });
+    });
+}
+// sets the kernel's dynamic shared-memory limit; returns its resident CTAs per SM
+int attn_user_prepare(const ctr_handle* h) {
+    int occ = 1;
+    const size_t smem = attn_user_smem(h);
+    with_user_kernel(h, [&](auto kern) {
+        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kAttnThreads, smem);
+    });
+    return std::max(occ, 1);
+}
+// X0 rows of the samples (user, item i0 + b, d_hist) for b < B; grid: one wave of resident CTAs, so that each stages
+// the history once
+int attn_forward_user(ctr_handle* h, const RowSrc& r, int user, const int* d_hist, int i0, int B, int grid) {
+    return launch(h, "attn_fwd_user", [&] {
+        const Dims d = dims_of(h);
+        const size_t smem = attn_user_smem(h);
+        with_user_kernel(h, [&](auto kern) {
+            kern<<<std::min(grid, grid_attn(h, B)), kAttnThreads, smem, h->stream>>>(r, d, h->W[3], user, d_hist, i0, h->X0, h->Kp, h->Kp, B);
         });
     });
 }
@@ -543,6 +581,7 @@ bool use_umma(const ctr_handle* h) {
 struct StepOpts {
     bool training = false, update = false;
     bool want_rows = false;              // fill h->dUb / h->dIt
+    bool x0_ready = false;               // h->X0 already holds the MLP input rows (ctr_recommend_topk): no attention forward
     const float* d_label = nullptr;
     // sharded-table step (comm_impl.cuh): rows live in a per-lookup buffer, gradients are scaled to the
     // global mean and the dense gradients are all-reduced before Adam
@@ -634,7 +673,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
     if (B <= 0 || B > h->Bmax) return set_err(h, CTR_EINVAL, "batch %d outside (0, %d]", B, h->Bmax);
     const float d0 = o.training ? c.dropout0 : 0.0f, d1 = o.training ? c.dropout1 : 0.0f;
 
-    RET(attn_forward(h, r, B));
+    if (!o.x0_ready) RET(attn_forward(h, r, B));
     const bool um = use_umma(h);
     if (um) {
         RET(umma_init(h));
@@ -1098,7 +1137,7 @@ void ctr_destroy(ctr_handle* h) {
                     (void*)h->dUb, (void*)h->dIt, (void*)h->keys, (void*)h->keys2, (void*)h->pos, (void*)h->pos2, h->sort_tmp,
                     (void*)h->d_cost, (void*)h->s_user, (void*)h->s_item, (void*)h->s_hist, (void*)h->s_label, (void*)h->dXd, (void*)h->dYd, (void*)h->hot_acc, (void*)h->emb_m, (void*)h->emb_v})
         if (p) cudaFree(p);
-    for (int i = 0; i < 4; i++) if (h->scratch[i]) cudaFree(h->scratch[i]);
+    for (int i = 0; i < ctr_handle::kScratch; i++) if (h->scratch[i]) cudaFree(h->scratch[i]);
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 2; i++) { if (h->ev_copied[i]) cudaEventDestroy(h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy(h->ev_consumed[i]); }
@@ -1940,8 +1979,8 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
     const int D = h->tab_width[T], Dp = (D + 3) & ~3;
     // query tile: as wide as the batch needs, narrower when k's lists would not fit shared memory
     int QT = 16;
-    while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
-    const size_t smem = knn::kTileBytes + knn::smem_bytes(QT, Dp, k), msmem = knn::smem_bytes(1, 0, k);
+    while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
+    const size_t smem = knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k), msmem = knn::smem_bytes<knn::SimKey>(1, 0, k);
     int occ = 1;
     if (by_row) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
     // row slices: enough CTAs to fill the GPU with the least idle tail (whole waves of resident CTAs); queries are
@@ -1983,11 +2022,98 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
             int unused = 0;
             if (by_row) knn_scan_dispatch<true>(h, QT, a, false, smem, &unused); else knn_scan_dispatch<false>(h, QT, a, false, smem, &unused);
         }));
-        RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, d_or, d_os, d_oc); }));
+        RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, d_or, d_os, d_oc); }));
         CU(h, cudaMemcpyAsync(out_rows + s * k, d_or, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_sim + s * k, d_os, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_count + s, d_oc, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaStreamSynchronize(h->stream));
+    }
+    return CTR_OK;
+}
+
+int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k, int32_t exclude_history,
+                       int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count) {
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    if (k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count)
+        return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs)", knn::kMaxK);
+    std::lock_guard<std::mutex> lk(h->mu);
+    const int T = CTR_TABLE_ITEM_EMB;
+    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+    if (h->tab_sharded[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB is row-sharded over %d ranks: recommendation needs the whole table on one device", h->comm.world);
+    RET(check_tables(h));
+    const int64_t N = h->tab_rows[T];
+    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+    CU(h, cudaSetDevice(h->dev));
+    const int S = h->cfg.S, Bc = h->Bmax;
+    int optin = 0;
+    CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
+    const bool user_kernel = attn_user_ok(h, (size_t)optin);
+    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h) : 0;
+    // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
+    const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
+    const int max_slices = (Bc + rps - 1) / rps;
+    const int nex = exclude_history ? S : 0;
+    const size_t ssmem = rec::scan_smem_bytes(k, nex), msmem = knn::smem_bytes<knn::LogitKey>(1, 0, k);
+    CU(h, cudaFuncSetAttribute(rec::k_rec_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+    const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
+
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t gk = (size_t)G * k, sl = (size_t)(1 + max_slices) * k;
+    const size_t b_h = al((size_t)G * S * 4), b_sl = al(sl * 4), b_l = al(gk * 4), b_c = al((size_t)G * 4);
+    char* p = nullptr;
+    RET(scratch_get(h, 4, b_h + 2 * b_sl + 5 * b_l + b_c, (void**)&p));
+    int* d_hist = (int*)p;                 p += b_h;
+    float* d_sl_s = (float*)p;             p += b_sl;      // [0, k): the user's running list, then the chunk's slice lists
+    int* d_sl_r = (int*)p;                 p += b_sl;
+    float* d_ls = (float*)p;               p += b_l;       // [G][k] the users' final lists
+    int* d_lr = (int*)p;                   p += b_l;
+    int* d_or = (int*)p;                   p += b_l;
+    float* d_ol = (float*)p;               p += b_l;
+    float* d_os = (float*)p;               p += b_l;
+    int* d_oc = (int*)p;
+
+    const int nchunks = (int)((N + Bc - 1) / Bc);
+    for (int64_t g0 = 0; g0 < nu; g0 += G) {
+        const int ng = (int)std::min<int64_t>(G, nu - g0);
+        if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + g0 * S, (size_t)ng * S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+        for (int j = 0; j < ng; j++) {
+            const int user = user_rows[g0 + j];
+            const int* uh = d_hist + (size_t)j * S;
+            for (int c = 0; c < nchunks; c++) {
+                const int i0 = c * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
+                StepOpts o;
+                RowSrc r;
+                if (user_kernel) {
+                    r = idx_src(h, nullptr, nullptr, nullptr, nb);
+                    RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
+                    o.x0_ready = true;
+                } else {
+                    const int fg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)nb * std::max(S, 1) + 255) / 256, (int64_t)h->num_sms * 8));
+                    RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
+                    r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+                }
+                RET(step_core(h, r, nb, o));
+                const int slices = (nb + rps - 1) / rps;
+                const bool first = c == 0, last = c == nchunks - 1;
+                RET(launch(h, "rec_topk", [&] {
+                    rec::k_rec_scan<<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, rps, uh, nex, k, first ? nullptr : d_sl_s,
+                                                                                first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
+                }));
+                // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
+                RET(launch(h, "rec_merge", [&] {
+                    knn::k_knn_merge<knn::LogitKey><<<1, knn::kThreads, msmem, h->stream>>>(
+                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, first ? slices : slices + 1, k,
+                        last ? d_lr + (size_t)j * k : d_sl_r, last ? d_ls + (size_t)j * k : d_sl_s, nullptr);
+                }));
+            }
+        }
+        const long n = (long)ng * k;
+        RET(launch(h, "rec_finish", [&] { rec::k_rec_finish<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
+        CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_count + g0, d_oc, (size_t)ng * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));          // d_hist and the result buffers are reused by the next group
     }
     return CTR_OK;
 }

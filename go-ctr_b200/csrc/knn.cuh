@@ -15,6 +15,9 @@
 // query the CTA keeps a sorted top-k list and a candidate buffer in shared memory; a candidate enters the buffer only
 // if it beats the list's current k-th entry, and after every step one warp per query inserts the buffered candidates.
 // k_knn_merge: one CTA per query streams the slices' lists through the same list/buffer and writes the final top-k.
+//
+// The list/buffer machinery is shared with the recommendation top-k (rec.cuh): a Key type names the score type and the
+// rule a score must meet to enter a list.
 #pragma once
 #include "common.cuh"
 #include <climits>
@@ -26,33 +29,53 @@ constexpr int kThreads = 128;
 constexpr int kRows = 2;                      // rows per thread and step
 constexpr int kStep = kThreads * kRows;       // rows per step == candidate buffer capacity per query
 constexpr int kMaxK = 1024;
-constexpr int kEmptyRow = INT_MAX;            // list entries start as (0, kEmptyRow): any similarity > 0 beats them
+constexpr int kEmptyRow = INT_MAX;            // list entries start as (Key::empty(), kEmptyRow): every qualifying score beats them
 constexpr int kChunk = 32;                    // columns of a step's rows staged in shared memory at a time
 constexpr int kTileLd = kChunk + 4;           // padded row pitch: the per-thread float4 reads are conflict-free
 constexpr size_t kTileBytes = (size_t)kStep * kTileLd * 4;
 
-__device__ __forceinline__ bool better(double s1, int r1, double s2, int r2) { return s1 > s2 || (s1 == s2 && r1 < r2); }
+// list order: score descending, then row ascending (a total order: NaN never enters a list)
+template <typename T>
+__device__ __forceinline__ bool better(T s1, int r1, T s2, int r2) { return s1 > s2 || (s1 == s2 && r1 < r2); }
+
+// search.Searcher: cosine similarities, only those > 0 qualify (search.go)
+struct SimKey {
+    using T = double;
+    __device__ static double empty() { return 0.0; }
+    __device__ static bool qualifies(double s) { return s > 0.0; }
+};
+// recommendation (rec.cuh): pre-sigmoid logits, any that is not NaN qualifies; (-inf, kEmptyRow) loses to (-inf, row)
+struct LogitKey {
+    using T = float;
+    __device__ static float empty() { return -__int_as_float(0x7f800000); }
+    __device__ static bool qualifies(float s) { return s == s; }
+};
 
 // shared-memory layout of QT queries' top-k state
+template <class K>
 struct Smem {
-    double* q;      // [QT][Dp] query tile (scan only)
-    double* ls;     // [QT][k] list similarities, sorted best first
-    double* bs;     // [QT][kStep] candidate buffer
+    using T = typename K::T;
+    double* q;      // [QT][Dp] query tile (search scan only)
+    double* qn;     // [QT] query norms
+    T* ls;          // [QT][k] list scores, sorted best first
+    T* bs;          // [QT][kStep] candidate buffer
     int* lr;        // [QT][k] list rows
     int* br;        // [QT][kStep]
     int* bn;        // [QT] buffered candidates
-    double* qn;     // [QT] query norms
     int* ex;        // [QT] excluded row (-1: none)
 };
+template <class K>
 __host__ __device__ inline size_t smem_bytes(int QT, int Dp, int k) {
-    return (size_t)QT * ((size_t)Dp * 8 + (size_t)k * 12 + (size_t)kStep * 12 + 16);
+    return (size_t)QT * ((size_t)Dp * 8 + ((size_t)k + kStep) * (sizeof(typename K::T) + 4) + 16);
 }
-__device__ inline Smem carve(char* p, int QT, int Dp, int k) {
-    Smem s;
+template <class K>
+__device__ inline Smem<K> carve(char* p, int QT, int Dp, int k) {
+    using T = typename K::T;
+    Smem<K> s;
     s.q = (double*)p;   p += (size_t)QT * Dp * 8;
-    s.ls = (double*)p;  p += (size_t)QT * k * 8;
-    s.bs = (double*)p;  p += (size_t)QT * kStep * 8;
     s.qn = (double*)p;  p += (size_t)QT * 8;
+    s.ls = (T*)p;       p += (size_t)QT * k * sizeof(T);
+    s.bs = (T*)p;       p += (size_t)QT * kStep * sizeof(T);
     s.lr = (int*)p;     p += (size_t)QT * k * 4;
     s.br = (int*)p;     p += (size_t)QT * kStep * 4;
     s.bn = (int*)p;     p += (size_t)QT * 4;
@@ -62,16 +85,17 @@ __device__ inline Smem carve(char* p, int QT, int Dp, int k) {
 
 // one warp inserts n buffered candidates into a sorted list of k entries (insertion order does not matter: the order
 // is total).  Candidates that no longer beat the k-th entry are dropped.
-__device__ void warp_insert(double* ls, int* lr, int k, const double* bs, const int* br, int n, int lane) {
+template <typename T>
+__device__ void warp_insert(T* ls, int* lr, int k, const T* bs, const int* br, int n, int lane) {
     for (int c = 0; c < n; c++) {
-        const double s = bs[c]; const int r = br[c];
+        const T s = bs[c]; const int r = br[c];
         if (!better(s, r, ls[k - 1], lr[k - 1])) continue;          // uniform: every lane reads the same entries
         int cnt = 0;
         for (int i = lane; i < k; i += 32) cnt += better(ls[i], lr[i], s, r) ? 1 : 0;
         const int pos = __reduce_add_sync(0xffffffffu, cnt);       // entries better than the candidate: a prefix
         for (int top = k - 2; top >= pos; top -= 32) {              // shift [pos, k-1) up by one, top chunk first
             const int i = top - lane;
-            double vs = 0; int vr = 0;
+            T vs = 0; int vr = 0;
             if (i >= pos) { vs = ls[i]; vr = lr[i]; }
             __syncwarp();
             if (i >= pos) { ls[i + 1] = vs; lr[i + 1] = vr; }
@@ -83,8 +107,8 @@ __device__ void warp_insert(double* ls, int* lr, int k, const double* bs, const 
 }
 
 // after a step: warp w inserts the buffers of queries w, w + nwarps, ...  Call between two __syncthreads().
-template <int QT>
-__device__ __forceinline__ void flush(const Smem& sm, int k) {
+template <int QT, class K>
+__device__ __forceinline__ void flush(const Smem<K>& sm, int k) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int q = warp; q < QT; q += kThreads / 32) {
         const int n = sm.bn[q];
@@ -94,8 +118,9 @@ __device__ __forceinline__ void flush(const Smem& sm, int k) {
     }
 }
 
-__device__ __forceinline__ void offer(const Smem& sm, int q, int k, double s, int row) {
-    if (s > 0.0 && better(s, row, sm.ls[(size_t)q * k + k - 1], sm.lr[(size_t)q * k + k - 1])) {
+template <class K>
+__device__ __forceinline__ void offer(const Smem<K>& sm, int q, int k, typename K::T s, int row) {
+    if (K::qualifies(s) && better(s, row, sm.ls[(size_t)q * k + k - 1], sm.lr[(size_t)q * k + k - 1])) {
         const int i = atomicAdd(&sm.bn[q], 1);
         sm.bs[(size_t)q * kStep + i] = s; sm.br[(size_t)q * kStep + i] = row;
     }
@@ -111,7 +136,7 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__
     extern __shared__ __align__(16) char smem_raw[];
     const int Dp = (D + 3) & ~3;
     float* tile = (float*)smem_raw;           // [kStep][kTileLd]: the step's rows, kChunk columns at a time
-    const Smem sm = carve(smem_raw + kTileBytes, QT, Dp, k);
+    const Smem<SimKey> sm = carve<SimKey>(smem_raw + kTileBytes, QT, Dp, k);
     const int q0 = blockIdx.x * QT;
     const int slice = blockIdx.y, slices = gridDim.y;
 
@@ -121,7 +146,7 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__
         if (g < nq && d < D) v = ROWQ ? (double)tab[(size_t)qrow[g] * ld + d] : qvec[(size_t)g * D + d];
         sm.q[i] = v;
     }
-    for (int i = threadIdx.x; i < QT * k; i += kThreads) { sm.ls[i] = 0.0; sm.lr[i] = kEmptyRow; }
+    for (int i = threadIdx.x; i < QT * k; i += kThreads) { sm.ls[i] = SimKey::empty(); sm.lr[i] = kEmptyRow; }
     if (threadIdx.x < QT) {
         const int g = q0 + threadIdx.x;
         sm.bn[threadIdx.x] = 0;
@@ -206,18 +231,21 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__
     }
 }
 
-// one CTA per query: the top-k of the slices' lists.  Positions past the count hold row -1 and similarity 0.
-__global__ void __launch_bounds__(kThreads) k_knn_merge(const double* __restrict__ in_sim, const int* __restrict__ in_row,
-                                                         int slices, int k, int32_t* __restrict__ out_row,
-                                                         double* __restrict__ out_sim, int32_t* __restrict__ out_count) {
+// one CTA per query: the top-k of `slices` lists of k entries.  Positions past the count hold row -1 and score 0.
+// out_count == nullptr: the list is written as it stands, empty entries included, to be merged again; it may then
+// overwrite the first input list (every input is read before the first write).
+template <class K>
+__global__ void __launch_bounds__(kThreads) k_knn_merge(const typename K::T* in_sim, const int* in_row, int slices, int k,
+                                                         int32_t* out_row, typename K::T* out_sim, int32_t* __restrict__ out_count) {
+    using T = typename K::T;
     extern __shared__ __align__(16) char smem_raw[];
-    const Smem sm = carve(smem_raw, 1, 0, k);
+    const Smem<K> sm = carve<K>(smem_raw, 1, 0, k);
     const int g = blockIdx.x;
-    for (int i = threadIdx.x; i < k; i += kThreads) { sm.ls[i] = 0.0; sm.lr[i] = kEmptyRow; }
+    for (int i = threadIdx.x; i < k; i += kThreads) { sm.ls[i] = K::empty(); sm.lr[i] = kEmptyRow; }
     if (threadIdx.x == 0) sm.bn[0] = 0;
     __syncthreads();
     const long n = (long)slices * k;
-    const double* is = in_sim + (size_t)g * n;
+    const T* is = in_sim + (size_t)g * n;
     const int* ir = in_row + (size_t)g * n;
     for (long base = 0; base < n; base += kStep) {
 #pragma unroll
@@ -229,11 +257,15 @@ __global__ void __launch_bounds__(kThreads) k_knn_merge(const double* __restrict
         flush<1>(sm, k);
         __syncthreads();
     }
+    if (!out_count) {
+        for (int i = threadIdx.x; i < k; i += kThreads) { out_row[(size_t)g * k + i] = sm.lr[i]; out_sim[(size_t)g * k + i] = sm.ls[i]; }
+        return;
+    }
     int cnt = 0;
     for (int i = threadIdx.x; i < k; i += kThreads) {
-        const bool v = sm.ls[i] > 0.0;
+        const bool v = sm.lr[i] != kEmptyRow;
         out_row[(size_t)g * k + i] = v ? sm.lr[i] : -1;
-        out_sim[(size_t)g * k + i] = v ? sm.ls[i] : 0.0;
+        out_sim[(size_t)g * k + i] = v ? sm.ls[i] : T(0);
         cnt += v ? 1 : 0;
     }
     cnt = __reduce_add_sync(0xffffffffu, cnt);

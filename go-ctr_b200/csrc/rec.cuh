@@ -1,0 +1,101 @@
+// rec.cuh — top-k recommendation over the whole item table (ctr_recommend_topk): the default recall the reference leaves
+// as a todo (recommend/api.go:115-118).  DESIGN.md §1a row f6.
+//
+// One user's items are scored chunk by chunk by the ordinary forward (k_attn_fwd_user, the MLP GEMMs, k_head), which
+// leaves the chunk's logits in h->Z.  The selection keeps the first k items under (logit descending, row ascending) in
+// knn.cuh's list/buffer machinery with LogitKey: a NaN logit never qualifies, and the rows of the user's exclusion list
+// are skipped.  The order is total, so the result depends neither on the chunk size nor on the slicing.
+//   k_rec_scan:   grid = slices of the chunk; each CTA writes the top-k of its slice as it stands (empty entries included)
+//   k_knn_merge<LogitKey>: merges the user's running list with the slices' lists
+//   k_rec_finish: the users' lists → rows (-1 past the count), logits and scores (0 past the count), counts
+#pragma once
+#include "knn.cuh"
+
+namespace ctr {
+namespace rec {
+
+using knn::LogitKey;
+using knn::kEmptyRow;
+using knn::kStep;
+using knn::kThreads;
+
+// dynamic shared memory of k_rec_scan: the list/buffer state plus the exclusion rows that fall into the slice
+__host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<LogitKey>(1, 0, k) + (size_t)nex * 4 + 16; }
+
+// z[b] is the logit of row row0 + b, b < n.  excl[0, nex): rows that must not be returned (duplicates and rows outside
+// the table are harmless).  run_s / run_r: the user's running list over the earlier chunks (nullptr for the first): only
+// rows that beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row
+// lies in an earlier chunk, so the fillers are told apart by row and written back as empty entries.
+// Out: per slice the top-k list, [slices][k].
+__global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__ z, int n, int row0, int rows_per_slice,
+                                                        const int* __restrict__ excl, int nex, int k,
+                                                        const float* run_s, const int* run_r,
+                                                        float* __restrict__ out_s, int* __restrict__ out_row) {
+    extern __shared__ __align__(16) char smem_raw[];
+    const knn::Smem<LogitKey> sm = knn::carve<LogitKey>(smem_raw, 1, 0, k);
+    int* ex = reinterpret_cast<int*>(smem_raw + knn::smem_bytes<LogitKey>(1, 0, k));
+    __shared__ int nx;
+    const int r0 = blockIdx.x * rows_per_slice, r1 = min(n, r0 + rows_per_slice);
+    const float t_s = run_r ? run_s[k - 1] : LogitKey::empty();
+    const int t_r = run_r ? run_r[k - 1] : kEmptyRow;
+    for (int i = threadIdx.x; i < k; i += kThreads) { sm.ls[i] = t_s; sm.lr[i] = t_r; }
+    if (threadIdx.x == 0) { sm.bn[0] = 0; nx = 0; }
+    __syncthreads();
+    for (int i = threadIdx.x; i < nex; i += kThreads) {       // usually none of the user's rows fall into this slice
+        const int e = __ldg(excl + i);
+        const long b = (long)e - row0;
+        if (b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+    }
+    __syncthreads();
+    const int m = nx;
+    for (int base = r0; base < r1; base += kStep) {
+#pragma unroll
+        for (int r = 0; r < knn::kRows; r++) {
+            const int b = base + threadIdx.x + r * kThreads;
+            if (b >= r1) continue;
+            const int row = row0 + b;
+            bool skip = false;
+            for (int e = 0; e < m; e++) skip |= ex[e] == row;
+            if (!skip) knn::offer(sm, 0, k, __ldg(z + b), row);
+        }
+        __syncthreads();
+        knn::flush<1>(sm, k);
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < k; i += kThreads) {
+        const bool filler = sm.lr[i] == t_r;
+        out_s[(size_t)blockIdx.x * k + i] = filler ? LogitKey::empty() : sm.ls[i];
+        out_row[(size_t)blockIdx.x * k + i] = filler ? kEmptyRow : sm.lr[i];
+    }
+}
+
+// n = users * k list entries.  The score is sigmoid32 of the logit, the function k_head applies: bit-identical to the
+// score ctr_predict_idx returns for the same sample.
+__global__ void k_rec_finish(const float* __restrict__ ls, const int* __restrict__ lr, int k, long n,
+                             int32_t* __restrict__ out_row, float* __restrict__ out_logit, float* __restrict__ out_score,
+                             int32_t* __restrict__ out_count) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long j = i / k;
+    const int p = (int)(i - j * k);
+    const bool v = lr[i] != kEmptyRow;
+    out_row[i] = v ? lr[i] : -1;
+    out_logit[i] = v ? ls[i] : 0.0f;
+    out_score[i] = v ? sigmoid32(ls[i]) : 0.0f;
+    // valid entries are a prefix of the sorted list
+    if (v && (p == k - 1 || lr[i + 1] == kEmptyRow)) out_count[j] = p + 1;
+    if (!v && p == 0) out_count[j] = 0;
+}
+
+// the fallback route: index buffers of B samples (user, item row0 + b, hist) for the ordinary attention kernels
+__global__ void k_rec_fill_idx(int user, const int* __restrict__ hist, int S, int row0, int B, int* __restrict__ d_user,
+                               int* __restrict__ d_item, int* __restrict__ d_hist) {
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < (long)B * S; i += (long)gridDim.x * blockDim.x) {
+        const int b = (int)(i / S), s = (int)(i - (long)b * S);
+        d_hist[i] = __ldg(hist + s);
+        if (s == 0) { d_user[b] = user; d_item[b] = row0 + b; }
+    }
+}
+
+}  // namespace rec
+}  // namespace ctr

@@ -27,7 +27,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_create", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params"]
 
@@ -366,6 +366,19 @@ class Engine:
         self._ck(self.L.ctr_knn_search(self.h, qp, rp, C.c_int64(nq), C.c_int32(k), out_r.ctypes.data_as(_ip),
                                        out_s.ctypes.data_as(C.POINTER(C.c_double)), cnt.ctypes.data_as(_ip)))
         return out_r, out_s, cnt
+
+    def recommend_topk(self, user_rows, hist, k, exclude_history=True):
+        """Top-k recommendation over every ITEM_EMB row (ctr_recommend_topk): user_rows [nu], hist [nu, S] (-1 padded).
+        Returns (rows [nu, k] int32, scores [nu, k] float32, logits [nu, k] float32, counts [nu] int32), best first
+        (logit descending, then row ascending); positions past a user's count hold row -1, score 0 and logit 0."""
+        u, up = _i(np.atleast_1d(user_rows))
+        hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
+        out_r = np.empty((u.size, k), np.int32); out_s = np.empty((u.size, k), np.float32)
+        out_l = np.empty((u.size, k), np.float32); cnt = np.empty(u.size, np.int32)
+        self._ck(self.L.ctr_recommend_topk(self.h, up, hp, C.c_int64(u.size), C.c_int32(k), C.c_int32(int(bool(exclude_history))),
+                                           out_r.ctypes.data_as(_ip), out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(_fp),
+                                           cnt.ctypes.data_as(_ip)))
+        return out_r, out_s, out_l, cnt
 
 
 MLP_ACT = {"relu": 0, "logistic": 1, "identity": 2}

@@ -43,8 +43,30 @@ def Rank(recSys, userId, itemIds, now=None):
     return [ItemScore(int(it), float(y[k, 0])) for k, it in enumerate(itemIds)]
 
 
+def Recommend(recSys, userId, k, now=None, exclude_history=True):
+    """What recommend/api.go's empty-itemIdList branch would return (api.go:115-118, "todo: some default recall
+    algorithm"): the k best items of the whole table for one user at the current time, best first, as [ItemScore].
+    Every ITEM_EMB row is scored with the trained model (ctr_recommend_topk); the user's history is windowed from the
+    device ubcache at `now` (empty without one, as in BatchPredict); exclude_history drops the items of that window.
+    An unknown user raises CtrError with code ENOTFOUND, as BatchPredict does for an unresolvable first key."""
+    ts = int(time.time()) if now is None else int(now)
+    row = int(recSys.idmap_lookup(_e.IDMAP_USER, [int(userId)])[0])
+    if row < 0:
+        raise _e.CtrError(_e.ENOTFOUND, "user %d is not found" % int(userId))
+    try:
+        hist = recSys.ubcache_window([row], [ts])
+    except _e.CtrError as err:          # ESTATE: no ubcache uploaded
+        if err.code != _e.ESTATE:
+            raise
+        hist = np.full((1, recSys.cfg.S), -1, np.int32)
+    rows, scores, _, cnt = recSys.recommend_topk([row], hist, k, exclude_history=exclude_history)
+    item_ids = recSys.item_ids
+    return [ItemScore(int(item_ids[rows[0, i]]), float(scores[0, i])) for i in range(int(cnt[0]))]
+
+
 def load_id_maps(recSys, user_ids, item_ids):
     """user_ids[r] / item_ids[r] = external id of table row r (what the Go side's string-keyed caches hold,
-    rcmd.go:472-505)."""
+    rcmd.go:472-505).  The item ids stay on the engine (item_ids) to map Recommend's rows back to ids."""
     recSys.idmap_build(_e.IDMAP_USER, user_ids)
     recSys.idmap_build(_e.IDMAP_ITEM, item_ids)
+    recSys.item_ids = np.array(item_ids, np.int64)

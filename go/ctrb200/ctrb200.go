@@ -195,6 +195,31 @@ func (e *Engine) Search(queries []float64, rows []int32, k int) (outRows []int32
 	return outRows, sims, counts, nil
 }
 
+// Recommend is the default recall recommend/api.go:115-118 leaves as a todo: for each user row, every ITEM_EMB row is
+// scored with the trained model as the sample (userRows[j], item, histRows[j*S:(j+1)*S]) and the k best are returned,
+// logit descending then row ascending. excludeHistory drops the items of the user's valid history rows. outRows /
+// scores / logits are [nu*k]; counts[j] is the true number of results of user j, the positions past it hold row -1,
+// score 0 and logit 0.
+func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory bool) (outRows []int32, scores, logits []float32, counts []int32, err error) {
+	nu := len(userRows)
+	if nu == 0 || k < 1 || len(histRows) != nu*int(e.cfg.S) {
+		return nil, nil, nil, nil, fmt.Errorf("ctrb200: Recommend needs at least one user, k >= 1 and S history rows per user")
+	}
+	ex := C.int32_t(0)
+	if excludeHistory {
+		ex = 1
+	}
+	outRows = make([]int32, nu*k)
+	scores = make([]float32, nu*k)
+	logits = make([]float32, nu*k)
+	counts = make([]int32, nu)
+	rc := C.ctr_recommend_topk(e.h, i32(userRows), i32(histRows), C.int64_t(nu), C.int32_t(k), ex, i32(outRows), f32(scores), f32(logits), i32(counts))
+	if err = e.err(rc); err != nil {
+		return nil, nil, nil, nil, err
+	}
+	return outRows, scores, logits, counts, nil
+}
+
 // SaveCheckpoint / LoadCheckpoint: binary snapshot of weights, Adam moments, step counter and tables.
 func (e *Engine) SaveCheckpoint(path string) error {
 	cs := C.CString(path)

@@ -248,6 +248,27 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count);
 
+/* Recommendation without a candidate list (recommend/api.go:115-118 "todo: some default recall algorithm"): for each
+ * of nu users, score EVERY row of ITEM_EMB as the sample (user_rows[j], item, hist_rows[j]) with the model's forward
+ * pass (dropout off, exactly what ctr_predict_idx computes for that triple) and return the k best.
+ *   Candidates: the ITEM_EMB rows [0, I).  An item's features are ITEM_FEAT row `item`, zeros when that row is missing.
+ *     A user row or history row outside its table reads as a missing row, as in the other _idx entry points.
+ *     hist_rows is [nu, S], -1 padded.
+ *   Order: pre-sigmoid logit descending, then row ascending.  The sigmoid is monotone, so this is also a top-k by score,
+ *     but it does not collapse where the score saturates at 1 (logit > 15).  out_scores[j, i] is sigmoid(logit)
+ *     exactly as ctr_predict_idx returns it; out_logits (may be NULL) the logit.
+ *   Exclusions: an item whose logit is NaN is never returned; with exclude_history != 0 neither is an item that appears
+ *     among the user's valid hist_rows.
+ *   out_rows / out_scores / out_logits are [nu, k]; out_count[j] is the true number of results of user j, positions at
+ *     or past it hold row -1, score 0 and logit 0.
+ *   k in [1, 1024]; nu >= 1.  Missing tables, or no ITEM_EMB, is CTR_ESTATE; so is a row-sharded ITEM_EMB (world > 1,
+ *     large table) — a replicated one is served locally.
+ *   Items are scored in chunks of max(batch, pred_batch) rows, in the activation buffers the handle already has: a large
+ *     catalogue wants a large pred_batch.  Only nu·k results cross PCIe.
+ *   Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
+int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k,
+                       int32_t exclude_history, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count);
+
 /* ---- item2vec (BASELINE config 5; SURVEY.md §8f row f1) ------------------------------------------------
  * embedding.TrainEmbedding(ch, window, dim, iter) (feature/embedding/wordemb.go:9-32): SkipGram +
  * HierarchicalSoftmax word2vec over the users' item sequences; its output is the ITEM_EMB table the hot
