@@ -78,6 +78,32 @@ def test_marshal_schema_matches_reference_json():
     assert "att0" not in json.loads(y.Marshal())                             # dnn.go:38-47
 
 
+def test_idmap_hash_restatement_and_its_inverse():
+    """tests/util.py restates idmap.cuh's idmap_hash in numpy and inverts it, so that test_gpu_keys.py can build ids
+    that start their probe at chosen slots.  Checked here against a plain-integer transcription of the device function."""
+    import numpy as np
+    from tests.util import INT64_MAX, INT64_MIN, idmap_capacity, idmap_hash, idmap_unhash, ids_probing_from
+
+    M = (1 << 64) - 1
+
+    def fmix64(k):                       # idmap_hash, line for line
+        k ^= k >> 33; k = k * 0xff51afd7ed558ccd & M; k ^= k >> 33; k = k * 0xc4ceb9fe1a85ec53 & M; k ^= k >> 33
+        return k
+
+    rng = np.random.default_rng(5)
+    ids = np.concatenate([[0, -1, 1, INT64_MAX, INT64_MIN, INT64_MIN + 1], rng.integers(INT64_MIN, INT64_MAX, 2000, dtype=np.int64)])
+    assert idmap_hash(ids).tolist() == [fmix64(int(v) & M) for v in ids]
+    assert (idmap_unhash(idmap_hash(ids)) == ids).all()
+    h = np.concatenate([np.array([0, 1, 1 << 63, M], np.uint64), rng.integers(0, 2**64, 2000, dtype=np.uint64)])
+    assert (idmap_hash(idmap_unhash(h)) == h).all()
+    assert [idmap_capacity(n) for n in (1, 32, 33, 64, 65, 100_000)] == [64, 64, 128, 128, 256, 262_144]
+    for cap in (64, 128, 262_144):
+        slots = np.concatenate([np.full(20, cap - 1), np.arange(20), rng.integers(0, cap, 20)])
+        got = ids_probing_from(rng, slots, cap, avoid=[0, -1])
+        assert ((idmap_hash(got) & np.uint64(cap - 1)) == slots.astype(np.uint64)).all()
+        assert np.unique(got).size == got.size and not np.isin(got, [INT64_MIN, 0, -1]).any()
+
+
 def test_item2vec_host_plan_matches_the_reference_huffman_procedure():
     """ctr_i2v_paths (host-only part of the item2vec trainer) == dictionary.HuffnamTree + Node.GetPath as the
     oracle restates them (huffman.go:23-57, node.go:26-43), including ties and never-seen words."""
