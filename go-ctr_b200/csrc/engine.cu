@@ -16,6 +16,7 @@
 
 #include <nvtx3/nvToolsExt.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -165,8 +166,11 @@ struct ctr_handle {
         int dw_stages0 = 0, dw_stages1 = 0;
     } um;
 
-    // device-side ubcache (ubcache.cuh)
+    // device-side ubcache (ubcache.cuh); ub_cap_* are the allocated sizes
     long long *ub_off = nullptr, *ub_ts = nullptr; int* ub_items = nullptr; int64_t ub_users = 0, ub_n = 0;
+    size_t ub_cap_off = 0, ub_cap_n = 0;
+    // the spare CSR an append / set writes before the two are swapped
+    long long *ubx_off = nullptr, *ubx_ts = nullptr; int* ubx_items = nullptr; size_t ubx_cap_off = 0, ubx_cap_n = 0;
 
     // device id maps (idmap.cuh): [CTR_IDMAP_USER, CTR_IDMAP_ITEM]
     unsigned long long* idm_keys[2] = {nullptr, nullptr}; int* idm_vals[2] = {nullptr, nullptr};
@@ -174,8 +178,8 @@ struct ctr_handle {
     long long *k_keys = nullptr, *k_host = nullptr; int* k_flags = nullptr;   // staging for ctr_batch_predict_keys (device, pinned host)
 
     // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search;
-    // slot 4: ctr_recommend_topk): no cudaMalloc on the serving path
-    static constexpr int kScratch = 5;
+    // slot 4: ctr_recommend_topk; slot 5: ubcache append / set): no cudaMalloc on the serving path
+    static constexpr int kScratch = 6;
     void* scratch[kScratch] = {}; size_t scratch_cap[kScratch] = {};
 
     Comm comm;
@@ -1053,6 +1057,174 @@ int knn_scan_dispatch(ctr_handle* h, int QT, KnnArgs a, bool occupancy_only, siz
 
 }  // namespace
 
+// ---- live ubcache updates (ctr_ubcache_append / ctr_ubcache_set; kernels in ubcache.cuh)
+namespace {
+// bits needed to hold every value in [0, v]
+int bits_for(unsigned long long v) { return v ? 64 - __builtin_clzll(v) : 0; }
+
+// user rows an append / set may name: below the cache's user count, USER_FEAT's rows or the user id map's size
+int64_t ub_row_bound(const ctr_handle* h) {
+    return std::max({h->ub_off ? h->ub_users : (int64_t)0, h->tab_rows[CTR_TABLE_USER_FEAT], h->idm_keys[CTR_IDMAP_USER] ? h->idm_n[CTR_IDMAP_USER] : (int64_t)0});
+}
+
+// device workspace of one update, carved from scratch slot 5 (pass base = nullptr to size it)
+struct Carve {
+    char* base; size_t used = 0;
+    template <typename T> T* take(size_t n) { T* p = (T*)(base + used); used += (std::max<size_t>(n, 1) * sizeof(T) + 255) & ~(size_t)255; return p; }
+};
+
+// The batch of an append or set, as the touched users' segments (ubcache.cuh): T touched users, tuser / bb / bcnt / ob /
+// oe [T], dcum [T+1], and the batch events bts / bit they index.
+struct UbBatch {
+    int T = 0; int64_t grow = 0;                      // grow: dcum[T], the change of the event count
+    int *tuser = nullptr, *bb = nullptr, *bcnt = nullptr, *bit = nullptr;
+    long long *ob = nullptr, *oe = nullptr, *dcum = nullptr, *bts = nullptr;
+};
+
+// the stored cache's user and event counts (0, 0 when none was uploaded)
+void ub_stored(const ctr_handle* h, long long* n_users, long long* n) {
+    *n_users = h->ub_off ? h->ub_users : 0; *n = h->ub_off ? h->ub_n : 0;
+}
+
+// append: the batch to the device, sorted by (user, ts desc, arrival desc) with CUB radix sort, run-length encoded by user
+int ub_batch_append(ctr_handle* h, const int32_t* user_rows, const int64_t* ts, const int32_t* item_rows, int64_t m,
+                    int32_t max_row, int64_t tmin, int64_t tmax, UbBatch* ub) {
+    long long U, n; ub_stored(h, &U, &n);
+    const int ubits = bits_for((unsigned long long)max_row), tbits = bits_for((unsigned long long)tmax - (unsigned long long)tmin);
+    const bool two_pass = ubits + tbits > 64;
+    size_t tmp = 0, t1 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, t1, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, (int)m, 0, 64, h->stream); tmp = std::max(tmp, t1);
+    cub::DeviceRadixSort::SortPairs(nullptr, t1, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, (int)m, 0, 32, h->stream); tmp = std::max(tmp, t1);
+    cub::DeviceRunLengthEncode::Encode(nullptr, t1, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)m, h->stream); tmp = std::max(tmp, t1);
+    cub::DeviceScan::ExclusiveSum(nullptr, t1, (int*)nullptr, (int*)nullptr, (int)m, h->stream); tmp = std::max(tmp, t1);
+    cub::DeviceScan::ExclusiveSum(nullptr, t1, (long long*)nullptr, (long long*)nullptr, (int)m + 1, h->stream); tmp = std::max(tmp, t1);
+    auto carve = [&](char* base, UbBatch& b, int*& du, long long*& dts, int*& dit, unsigned long long*& ka, unsigned long long*& kb,
+                     int*& ia, int*& ib, int*& nruns, long long*& delta, void*& ctmp) {
+        Carve c{base};
+        du = c.take<int>(m); dts = c.take<long long>(m); dit = c.take<int>(m);
+        ka = c.take<unsigned long long>(m); kb = c.take<unsigned long long>(m); ia = c.take<int>(m); ib = c.take<int>(m);
+        b.tuser = c.take<int>(m); b.bts = c.take<long long>(m); b.bit = c.take<int>(m);
+        b.bb = c.take<int>(m); b.bcnt = c.take<int>(m); b.ob = c.take<long long>(m); b.oe = c.take<long long>(m);
+        b.dcum = c.take<long long>(m + 1); delta = c.take<long long>(m + 1); nruns = c.take<int>(1);
+        ctmp = c.take<char>(tmp);
+        return c.used;
+    };
+    int *du, *dit, *ia, *ib, *nruns; long long *dts, *delta; unsigned long long *ka, *kb; void* ctmp; char* ws = nullptr;
+    RET(scratch_get(h, 5, carve(nullptr, *ub, du, dts, dit, ka, kb, ia, ib, nruns, delta, ctmp), (void**)&ws));
+    carve(ws, *ub, du, dts, dit, ka, kb, ia, ib, nruns, delta, ctmp);
+    int* bu = ia;                                       // the sorted users reuse the first index buffer once it is read
+    CU(h, cudaMemcpyAsync(du, user_rows, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(dts, ts, sizeof(long long) * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(dit, item_rows, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((m + 255) / 256, (int64_t)h->num_sms * 8));
+    RET(launch(h, "ubcache_sort_keys", [&] { k_ub_sort_keys<<<grid, 256, 0, h->stream>>>(du, dts, m, tbits, tmax, two_pass, ka, ia); }));
+    int* idx = ib;
+    RET(launch(h, "ubcache_sort", [&] {
+        cub::DeviceRadixSort::SortPairs(ctmp, tmp, ka, kb, ia, ib, (int)m, 0, std::max(1, two_pass ? tbits : ubits + tbits), h->stream);
+    }));
+    if (two_pass) {                                      // then by user row, stably
+        RET(launch(h, "ubcache_user_keys", [&] { k_ub_user_keys<<<grid, 256, 0, h->stream>>>(du, ib, m, (unsigned*)ka); }));
+        RET(launch(h, "ubcache_sort", [&] {
+            cub::DeviceRadixSort::SortPairs(ctmp, tmp, (unsigned*)ka, (unsigned*)kb, ib, ia, (int)m, 0, std::max(1, ubits), h->stream);
+        }));
+        idx = ia; bu = ib;
+    }
+    RET(launch(h, "ubcache_gather", [&] { k_ub_gather_batch<<<grid, 256, 0, h->stream>>>(idx, du, dts, dit, m, bu, ub->bts, ub->bit); }));
+    RET(launch(h, "ubcache_rle", [&] { cub::DeviceRunLengthEncode::Encode(ctmp, tmp, bu, ub->tuser, ub->bcnt, nruns, (int)m, h->stream); }));
+    int T = 0;
+    CU(h, cudaMemcpyAsync(&T, nruns, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    ub->T = T; ub->grow = m;
+    RET(launch(h, "ubcache_scan", [&] { cub::DeviceScan::ExclusiveSum(ctmp, tmp, ub->bcnt, ub->bb, T, h->stream); }));
+    RET(launch(h, "ubcache_touched", [&] {
+        k_ub_touched<<<(T + 256) / 256, 256, 0, h->stream>>>(ub->tuser, nullptr, nullptr, T, h->ub_off, U, n, ub->bb, ub->bcnt, ub->ob, ub->oe, delta);
+    }));
+    return launch(h, "ubcache_scan", [&] { cub::DeviceScan::ExclusiveSum(ctmp, tmp, delta, ub->dcum, T + 1, h->stream); });
+}
+
+// set: the n_set sequences to the device, their users sorted (radix sort of (row, entry)); each touched user's new
+// events stay where the caller put them
+int ub_batch_set(ctr_handle* h, const int32_t* user_rows, const int64_t* offsets, const int64_t* ts, const int32_t* item_rows,
+                 int64_t ns, int64_t m, int32_t max_row, UbBatch* ub) {
+    long long U, n; ub_stored(h, &U, &n);
+    const int ubits = bits_for((unsigned long long)max_row);
+    size_t tmp = 0, t1 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, t1, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, (int)ns, 0, 32, h->stream); tmp = std::max(tmp, t1);
+    cub::DeviceScan::ExclusiveSum(nullptr, t1, (long long*)nullptr, (long long*)nullptr, (int)ns + 1, h->stream); tmp = std::max(tmp, t1);
+    auto carve = [&](char* base, UbBatch& b, int*& du, long long*& soff, int*& iota, int*& perm, long long*& delta, void*& ctmp) {
+        Carve c{base};
+        du = c.take<int>(ns); soff = c.take<long long>(ns + 1); iota = c.take<int>(ns); perm = c.take<int>(ns);
+        b.bts = c.take<long long>(m); b.bit = c.take<int>(m);
+        b.tuser = c.take<int>(ns); b.bb = c.take<int>(ns); b.bcnt = c.take<int>(ns); b.ob = c.take<long long>(ns); b.oe = c.take<long long>(ns);
+        b.dcum = c.take<long long>(ns + 1); delta = c.take<long long>(ns + 1);
+        ctmp = c.take<char>(tmp);
+        return c.used;
+    };
+    int *du, *iota, *perm; long long *soff, *delta; void* ctmp; char* ws = nullptr;
+    RET(scratch_get(h, 5, carve(nullptr, *ub, du, soff, iota, perm, delta, ctmp), (void**)&ws));
+    carve(ws, *ub, du, soff, iota, perm, delta, ctmp);
+    std::vector<int> seq((size_t)ns);
+    for (int64_t i = 0; i < ns; i++) seq[(size_t)i] = (int)i;
+    CU(h, cudaMemcpyAsync(du, user_rows, sizeof(int) * (size_t)ns, cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(soff, offsets, sizeof(long long) * (size_t)(ns + 1), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(iota, seq.data(), sizeof(int) * (size_t)ns, cudaMemcpyHostToDevice, h->stream));
+    if (m > 0) {
+        CU(h, cudaMemcpyAsync(ub->bts, ts, sizeof(long long) * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+        CU(h, cudaMemcpyAsync(ub->bit, item_rows, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice, h->stream));
+    }
+    RET(launch(h, "ubcache_sort", [&] {
+        cub::DeviceRadixSort::SortPairs(ctmp, tmp, (unsigned*)du, (unsigned*)ub->tuser, iota, perm, (int)ns, 0, std::max(1, ubits), h->stream);
+    }));
+    const int T = (int)ns;
+    RET(launch(h, "ubcache_touched", [&] {
+        k_ub_touched<<<(T + 256) / 256, 256, 0, h->stream>>>(ub->tuser, perm, soff, T, h->ub_off, U, n, ub->bb, ub->bcnt, ub->ob, ub->oe, delta);
+    }));
+    RET(launch(h, "ubcache_scan", [&] { cub::DeviceScan::ExclusiveSum(ctmp, tmp, delta, ub->dcum, T + 1, h->stream); }));
+    long long grow = 0;
+    CU(h, cudaMemcpyAsync(&grow, ub->dcum + T, sizeof grow, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    ub->T = T; ub->grow = grow;
+    return CTR_OK;
+}
+
+// the rewrite: offsets, stored events and new events into the spare CSR, then the swap
+int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users) {
+    long long U, n; ub_stored(h, &U, &n);
+    const int64_t n_new = n + ub.grow;
+    // The spare may still be read by work enqueued before the last swap: on the engine stream that is ordered before
+    // this call's kernels; the window stream of ctr_train_keys is drained here.
+    if (h->win_stream) CU(h, cudaStreamSynchronize(h->win_stream));
+    if (h->ubx_cap_off < (size_t)new_users + 1) {
+        if (h->ubx_off) { CU(h, cudaFree(h->ubx_off)); h->ubx_off = nullptr; h->ubx_cap_off = 0; }
+        const size_t cap = (size_t)new_users + 1 + (size_t)new_users / 8;      // slack, so steady growth rarely reallocates
+        RET(dalloc(h, &h->ubx_off, cap, false)); h->ubx_cap_off = cap;
+    }
+    if (h->ubx_cap_n < (size_t)n_new) {
+        for (void* p : {(void*)h->ubx_ts, (void*)h->ubx_items}) if (p) CU(h, cudaFree(p));
+        h->ubx_ts = nullptr; h->ubx_items = nullptr; h->ubx_cap_n = 0;
+        const size_t cap = (size_t)n_new + (size_t)n_new / 8;
+        RET(dalloc(h, &h->ubx_ts, cap, false)); RET(dalloc(h, &h->ubx_items, cap, false)); h->ubx_cap_n = cap;
+    }
+    RET(launch(h, "ubcache_offsets", [&] {
+        k_ub_offsets<<<(int)((new_users + kUbTile) / kUbTile), 256, 0, h->stream>>>(h->ub_off, U, n, ub.tuser, ub.T, ub.dcum, new_users, h->ubx_off);
+    }));
+    if (n > 0) RET(launch(h, "ubcache_move_stored", [&] {
+        const int grid = (int)((n + kUbTile - 1) / kUbTile);
+        if (replace) k_ub_move_stored<true><<<grid, 256, 0, h->stream>>>(h->ub_ts, h->ub_items, n, ub.ob, ub.oe, ub.dcum, ub.T, ub.bb, ub.bcnt, ub.bts, h->ubx_ts, h->ubx_items);
+        else k_ub_move_stored<false><<<grid, 256, 0, h->stream>>>(h->ub_ts, h->ub_items, n, ub.ob, ub.oe, ub.dcum, ub.T, ub.bb, ub.bcnt, ub.bts, h->ubx_ts, h->ubx_items);
+    }));
+    if (ub.T > 0) RET(launch(h, "ubcache_place_new", [&] {
+        const int grid = grid_for_warps(h, ub.T);
+        if (replace) k_ub_place_new<true><<<grid, 256, 0, h->stream>>>(h->ub_ts, ub.ob, ub.oe, ub.dcum, ub.T, ub.bb, ub.bcnt, ub.bts, ub.bit, h->ubx_ts, h->ubx_items);
+        else k_ub_place_new<false><<<grid, 256, 0, h->stream>>>(h->ub_ts, ub.ob, ub.oe, ub.dcum, ub.T, ub.bb, ub.bcnt, ub.bts, ub.bit, h->ubx_ts, h->ubx_items);
+    }));
+    std::swap(h->ub_off, h->ubx_off); std::swap(h->ub_ts, h->ubx_ts); std::swap(h->ub_items, h->ubx_items);
+    std::swap(h->ub_cap_off, h->ubx_cap_off); std::swap(h->ub_cap_n, h->ubx_cap_n);
+    h->ub_users = new_users; h->ub_n = n_new;
+    return CTR_OK;
+}
+}  // namespace
+
 // =====================================================================================================
 extern "C" {
 
@@ -1127,7 +1299,7 @@ void ctr_destroy(ctr_handle* h) {
     if (h->stream) cudaStreamSynchronize(h->stream);
     comm_destroy(h);
     for (int i = 0; i < 3; i++) table_free(h, i);
-    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items}) if (p) cudaFree(p);
+    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items, (void*)h->ubx_off, (void*)h->ubx_ts, (void*)h->ubx_items}) if (p) cudaFree(p);
     for (void* p : {(void*)h->idm_keys[0], (void*)h->idm_keys[1], (void*)h->idm_vals[0], (void*)h->idm_vals[1], (void*)h->k_keys, (void*)h->k_flags}) if (p) cudaFree(p);
     if (h->k_host) cudaFreeHost(h->k_host);
     for (int i = 0; i < 2; i++) for (float* p : {h->um.Wt0[i], h->um.Wt1[i], h->um.W1s[i], h->um.W0s[i]}) if (p) cudaFree(p);
@@ -1695,9 +1867,10 @@ int ctr_ubcache_upload(ctr_handle* h, const int64_t* offsets, const int64_t* ts,
     if (offsets[0] != 0 || offsets[n_users] != n) return set_err(h, CTR_EINVAL, "ubcache offsets must run from 0 to n");
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
-    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items}) if (p) cudaFree(p);
-    h->ub_off = h->ub_ts = nullptr; h->ub_items = nullptr;
+    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items}) if (p) cudaFree(p);      // the spare (ubx_*) is kept
+    h->ub_off = h->ub_ts = nullptr; h->ub_items = nullptr; h->ub_cap_off = h->ub_cap_n = 0;
     RET(dalloc(h, &h->ub_off, (size_t)n_users + 1, false)); RET(dalloc(h, &h->ub_ts, (size_t)n, false)); RET(dalloc(h, &h->ub_items, (size_t)n, false));
+    h->ub_cap_off = (size_t)n_users + 1; h->ub_cap_n = (size_t)n;
     CU(h, cudaMemcpyAsync(h->ub_off, offsets, sizeof(int64_t) * (size_t)(n_users + 1), cudaMemcpyHostToDevice, h->stream));
     if (n > 0) {
         CU(h, cudaMemcpyAsync(h->ub_ts, ts, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
@@ -1734,6 +1907,63 @@ int ctr_ubcache_window(ctr_handle* h, const int32_t* user_row, const int64_t* ma
                              cudaStreamSynchronize(h->stream) != cudaSuccess)) rc = set_err(h, CTR_ECUDA, "ubcache window copy: %s", cudaGetErrorString(cudaGetLastError()));
     }
     return rc;
+}
+
+int ctr_ubcache_append(ctr_handle* h, const int32_t* user_rows, const int64_t* ts, const int32_t* item_rows, int64_t n) {
+    if (!h || n < 0 || n > INT32_MAX || (n > 0 && (!user_rows || !ts || !item_rows))) return set_err(h, CTR_EINVAL, "bad ubcache append arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (n == 0) return CTR_OK;
+    const int64_t bound = ub_row_bound(h);
+    int32_t max_row = 0; int64_t tmin = INT64_MAX, tmax = INT64_MIN;
+    for (int64_t i = 0; i < n; i++) {
+        if (user_rows[i] < 0 || user_rows[i] >= bound)
+            return set_err(h, CTR_EINVAL, "ubcache append: user row %d of event %lld outside [0, %lld)", user_rows[i], (long long)i, (long long)bound);
+        max_row = std::max(max_row, user_rows[i]); tmin = std::min(tmin, ts[i]); tmax = std::max(tmax, ts[i]);
+    }
+    CU(h, cudaSetDevice(h->dev));
+    UbBatch ub;
+    RET(ub_batch_append(h, user_rows, ts, item_rows, n, max_row, tmin, tmax, &ub));
+    return ub_rewrite(h, ub, false, std::max<int64_t>(h->ub_off ? h->ub_users : 0, (int64_t)max_row + 1));
+}
+
+int ctr_ubcache_set(ctr_handle* h, const int32_t* user_rows, const int64_t* offsets, const int64_t* ts, const int32_t* item_rows, int64_t n_set, int64_t n) {
+    if (!h || n_set < 0 || n < 0 || n_set > INT32_MAX || n > INT32_MAX || (n_set > 0 && (!user_rows || !offsets)) || (n > 0 && (!ts || !item_rows)))
+        return set_err(h, CTR_EINVAL, "bad ubcache set arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (n_set == 0) return n == 0 ? CTR_OK : set_err(h, CTR_EINVAL, "ubcache set: %lld events for no user", (long long)n);
+    if (offsets[0] != 0 || offsets[n_set] != n) return set_err(h, CTR_EINVAL, "ubcache set: offsets must run from 0 to n");
+    const int64_t bound = ub_row_bound(h);
+    int32_t max_row = 0;
+    for (int64_t k = 0; k < n_set; k++) {
+        if (user_rows[k] < 0 || user_rows[k] >= bound)
+            return set_err(h, CTR_EINVAL, "ubcache set: user row %d outside [0, %lld)", user_rows[k], (long long)bound);
+        if (offsets[k + 1] < offsets[k] || offsets[k + 1] > n) return set_err(h, CTR_EINVAL, "ubcache set: offsets must not decrease nor pass n (entry %lld)", (long long)k);
+        for (int64_t e = offsets[k] + 1; e < offsets[k + 1]; e++)
+            if (ts[e] > ts[e - 1]) return set_err(h, CTR_EINVAL, "ubcache set: the sequence of user row %d is not time-descending", user_rows[k]);
+        max_row = std::max(max_row, user_rows[k]);
+    }
+    std::vector<int32_t> sorted(user_rows, user_rows + n_set);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return set_err(h, CTR_EINVAL, "ubcache set: user row %d appears twice", *std::adjacent_find(sorted.begin(), sorted.end()));
+    CU(h, cudaSetDevice(h->dev));
+    UbBatch ub;
+    RET(ub_batch_set(h, user_rows, offsets, ts, item_rows, n_set, n, max_row, &ub));
+    return ub_rewrite(h, ub, true, std::max<int64_t>(h->ub_off ? h->ub_users : 0, (int64_t)max_row + 1));
+}
+
+int ctr_ubcache_download(ctr_handle* h, int64_t* offsets, int64_t* ts, int32_t* item_rows, int64_t cap_users, int64_t cap_events, int64_t* n_users, int64_t* n) {
+    if (!h || !n_users || !n) return set_err(h, CTR_EINVAL, "bad ubcache download arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->ub_off) return set_err(h, CTR_ESTATE, "ubcache not uploaded");
+    *n_users = h->ub_users; *n = h->ub_n;
+    if ((offsets && cap_users < h->ub_users) || ((ts || item_rows) && cap_events < h->ub_n))
+        return set_err(h, CTR_EINVAL, "ubcache download: the cache holds %lld users and %lld events", (long long)h->ub_users, (long long)h->ub_n);
+    CU(h, cudaSetDevice(h->dev));
+    if (offsets) CU(h, cudaMemcpyAsync(offsets, h->ub_off, sizeof(int64_t) * (size_t)(h->ub_users + 1), cudaMemcpyDeviceToHost, h->stream));
+    if (ts && h->ub_n) CU(h, cudaMemcpyAsync(ts, h->ub_ts, sizeof(int64_t) * (size_t)h->ub_n, cudaMemcpyDeviceToHost, h->stream));
+    if (item_rows && h->ub_n) CU(h, cudaMemcpyAsync(item_rows, h->ub_items, sizeof(int32_t) * (size_t)h->ub_n, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return CTR_OK;
 }
 
 // ---- sparse ids, serving keys, checkpoint (rows f3 / f4) -------------------------------------------------

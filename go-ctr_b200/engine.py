@@ -26,7 +26,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_gather_rows", "ctr_train_dense", "ctr_predict_dense", "ctr_train_step_idx", "ctr_train_idx", "ctr_train_keys", "ctr_predict_idx",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
-           "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
+           "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_create", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params"]
@@ -315,6 +315,28 @@ class Engine:
         out = np.empty((u.size, self.cfg.S), np.int32)
         self._ck(self.L.ctr_ubcache_window(self.h, up, t.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int32(u.size), out.ctypes.data_as(_ip)))
         return out
+
+    def ubcache_append(self, user_rows, ts, item_rows):
+        """Appends events to the device ubcache (ctr_ubcache_append): equal timestamps keep the most recent arrival first."""
+        u, up = _i(user_rows); t = np.ascontiguousarray(ts, np.int64); it, ip = _i(item_rows)
+        assert u.size == t.size == it.size
+        self._ck(self.L.ctr_ubcache_append(self.h, up, t.ctypes.data_as(_lp), ip, C.c_int64(u.size)))
+
+    def ubcache_set(self, user_rows, offsets, ts, item_rows):
+        """Replaces the whole sequences of distinct users (ctr_ubcache_set); user_rows[k]'s events are
+        [offsets[k], offsets[k+1]) of ts / item_rows, time-descending.  An empty sequence deletes the user's history."""
+        u, up = _i(user_rows); off = np.ascontiguousarray(offsets, np.int64); t = np.ascontiguousarray(ts, np.int64); it, ip = _i(item_rows)
+        assert off.size == u.size + 1 and t.size == it.size
+        self._ck(self.L.ctr_ubcache_set(self.h, up, off.ctypes.data_as(_lp), t.ctypes.data_as(_lp), ip, C.c_int64(u.size), C.c_int64(t.size)))
+
+    def ubcache_download(self):
+        """The live ubcache as (offsets [n_users+1], ts [n], item_rows [n])."""
+        nu = C.c_int64(0); n = C.c_int64(0)
+        self._ck(self.L.ctr_ubcache_download(self.h, None, None, None, C.c_int64(0), C.c_int64(0), C.byref(nu), C.byref(n)))
+        off = np.empty(nu.value + 1, np.int64); t = np.empty(n.value, np.int64); it = np.empty(n.value, np.int32)
+        self._ck(self.L.ctr_ubcache_download(self.h, off.ctypes.data_as(_lp), t.ctypes.data_as(_lp), it.ctypes.data_as(_ip),
+                                             C.c_int64(nu.value), C.c_int64(n.value), C.byref(nu), C.byref(n)))
+        return off, t, it
 
     def idmap_build(self, which, ids):
         a = np.ascontiguousarray(ids, np.int64)

@@ -64,6 +64,69 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     return [ItemScore(int(item_ids[rows[0, i]]), float(scores[0, i])) for i in range(int(cnt[0]))]
 
 
+class UserBehaviorCache:
+    """feature/ubcache's UserBehaviorCache (cache.go:16-55) over the engine's device ubcache, keyed by external ids
+    through the engine's id maps (load_id_maps).  Every change is applied in HBM, so the next Rank / BatchPredict /
+    Recommend / train_keys sees it.  An item id the item map does not hold is stored as row -1 and reads as a zero row
+    in its history slot, as in the reference.  Sequences are TimeSeq's: timestamps descending."""
+
+    def __init__(self, engine):
+        self.e = engine
+
+    def _user_rows(self, user_ids):
+        return self.e.idmap_lookup(_e.IDMAP_USER, np.asarray(user_ids, np.int64))
+
+    def _item_rows(self, item_ids):
+        item_ids = np.asarray(item_ids, np.int64)
+        return self.e.idmap_lookup(_e.IDMAP_ITEM, item_ids) if item_ids.size else np.zeros(0, np.int32)
+
+    def Set(self, userId, ts, itemIds):
+        """cache.go:28-33: replace one user's whole sequence."""
+        self.BatchSet({userId: (ts, itemIds)})
+
+    def BatchSet(self, ub):
+        """cache.go:36-41: replace the sequences of every user in {userId: (ts, itemIds)}.  A user id the user map does
+        not hold raises CtrError(ENOTFOUND) before anything changes."""
+        if not ub:
+            return
+        users = list(ub)
+        rows = self._user_rows(users)
+        if (rows < 0).any():
+            raise _e.CtrError(_e.ENOTFOUND, "user %d is not found" % int(users[int(np.flatnonzero(rows < 0)[0])]))
+        ts = [np.asarray(ub[u][0], np.int64).ravel() for u in users]
+        items = [np.asarray(ub[u][1], np.int64).ravel() for u in users]
+        if any(t.size != i.size for t, i in zip(ts, items)):
+            raise ValueError("every sequence needs one timestamp per item")
+        off = np.concatenate([[0], np.cumsum([t.size for t in ts])]).astype(np.int64)
+        all_ts = np.concatenate(ts) if ts else np.zeros(0, np.int64)
+        self.e.ubcache_set(rows, off, all_ts, self._item_rows(np.concatenate(items)))
+
+    def Delete(self, userId):
+        """cache.go:44-48: the user's history becomes empty.  Like Go's delete, an unknown user is a no-op."""
+        row = int(self._user_rows([userId])[0])
+        if row >= 0:
+            self.e.ubcache_set([row], [0, 0], np.zeros(0, np.int64), np.zeros(0, np.int32))
+
+    def Clear(self):
+        """cache.go:51-55: every user's history becomes empty (an upload of an empty cache)."""
+        self.e.ubcache_upload([0, 0], np.zeros(0, np.int64), np.zeros(0, np.int32))
+
+    def Append(self, userIds, itemIds, ts):
+        """Online learning's write path: append events (userIds[i] clicked itemIds[i] at ts[i]) to their users'
+        sequences.  Among equal timestamps the latest arrival comes first.  Events of user ids the user map does not
+        hold are dropped; returns how many."""
+        u = np.asarray(userIds, np.int64).ravel(); it = np.asarray(itemIds, np.int64).ravel(); t = np.asarray(ts, np.int64).ravel()
+        if not u.size == it.size == t.size:
+            raise ValueError("userIds, itemIds and ts must have one entry per event")
+        if u.size == 0:
+            return 0
+        rows = self._user_rows(u)
+        keep = rows >= 0
+        if keep.any():
+            self.e.ubcache_append(rows[keep], t[keep], self._item_rows(it[keep]))
+        return int((~keep).sum())
+
+
 def load_id_maps(recSys, user_ids, item_ids):
     """user_ids[r] / item_ids[r] = external id of table row r (what the Go side's string-keyed caches hold,
     rcmd.go:472-505).  The item ids stay on the engine (item_ids) to map Recommend's rows back to ids."""

@@ -151,6 +151,50 @@ func (e *Engine) UploadUserBehavior(offsets, ts []int64, itemRows []int32) error
 	return e.err(C.ctr_ubcache_upload(e.h, i64(offsets), i64(ts), i32(itemRows), C.int64_t(len(offsets)-1), C.int64_t(len(ts))))
 }
 
+// i64n / i32n are i64 / i32 for slices that may be empty (NULL then).
+func i64n(p []int64) *C.int64_t {
+	if len(p) == 0 {
+		return nil
+	}
+	return i64(p)
+}
+
+func i32n(p []int32) *C.int32_t {
+	if len(p) == 0 {
+		return nil
+	}
+	return i32(p)
+}
+
+// AppendUserBehavior appends events (userRows[i] acted on itemRows[i] at ts[i]) to the device ubcache, creating it if
+// none was uploaded.  Sequences stay time-descending; equal timestamps keep the most recent arrival first.
+func (e *Engine) AppendUserBehavior(userRows []int32, ts []int64, itemRows []int32) error {
+	if len(ts) != len(userRows) || len(itemRows) != len(userRows) {
+		return fmt.Errorf("AppendUserBehavior: %d users, %d timestamps, %d items", len(userRows), len(ts), len(itemRows))
+	}
+	return e.err(C.ctr_ubcache_append(e.h, i32n(userRows), i64n(ts), i32n(itemRows), C.int64_t(len(userRows))))
+}
+
+// SetUserBehavior is UserBehaviorCache.BatchSet (cache.go:36-41) at row level: userRows[k]'s whole sequence becomes
+// [offsets[k], offsets[k+1]) of ts / itemRows (time-descending); an empty sequence is Delete (cache.go:44-48).
+func (e *Engine) SetUserBehavior(userRows []int32, offsets, ts []int64, itemRows []int32) error {
+	if len(offsets) != len(userRows)+1 || len(itemRows) != len(ts) {
+		return fmt.Errorf("SetUserBehavior: %d users, %d offsets, %d timestamps, %d items", len(userRows), len(offsets), len(ts), len(itemRows))
+	}
+	return e.err(C.ctr_ubcache_set(e.h, i32n(userRows), i64(offsets), i64n(ts), i32n(itemRows), C.int64_t(len(userRows)), C.int64_t(len(ts))))
+}
+
+// DownloadUserBehavior returns the live device ubcache as the CSR UploadUserBehavior takes.
+func (e *Engine) DownloadUserBehavior() (offsets, ts []int64, itemRows []int32, err error) {
+	var nu, n C.int64_t
+	if err = e.err(C.ctr_ubcache_download(e.h, nil, nil, nil, 0, 0, &nu, &n)); err != nil {
+		return
+	}
+	offsets, ts, itemRows = make([]int64, int(nu)+1), make([]int64, int(n)), make([]int32, int(n))
+	err = e.err(C.ctr_ubcache_download(e.h, i64(offsets), i64n(ts), i32n(itemRows), nu, n, &nu, &n))
+	return
+}
+
 // BatchPredict is recommend.BatchPredict (rcmd.go:277-337) over sample keys, entirely on the device.
 func (e *Engine) BatchPredict(sampleKeys []rcmd.Sample) ([]float32, error) {
 	n := len(sampleKeys)

@@ -202,6 +202,31 @@ int ctr_ubcache_upload(ctr_handle* h, const int64_t* offsets, const int64_t* ts,
 int ctr_ubcache_window(ctr_handle* h, const int32_t* user_row, const int64_t* max_ts, int32_t B, int32_t* hist_rows);
 int ctr_ubcache_window_dev(ctr_handle* h, const int32_t* d_user_row, const int64_t* d_max_ts, int32_t B, int32_t* d_hist_rows);
 
+/* The live cache: UserBehaviorCache.Set / BatchSet / Delete (cache.go:27-48) and online appends, applied in HBM so the
+ * next window / ctr_batch_predict_keys / ctr_recommend_topk / ctr_train_keys sees them without a re-upload.
+ * append: n events (user_rows[i], ts[i], item_rows[i]) go into their users' sequences; the cache is created if none was
+ *   uploaded.  Every sequence stays time-descending, and equal timestamps are ordered most recent ARRIVAL first: an
+ *   appended event comes before the stored events with the same ts, and among one call's events of one user with the
+ *   same ts, the later in the call comes first.  This decides which items a window whose maxTs falls on a tied run
+ *   returns.
+ * set: replaces the whole sequences of n_set distinct users; user k's events are [offsets[k], offsets[k+1]) of ts /
+ *   item_rows [n] (offsets [n_set+1] from 0 to n), non-increasing in ts.  An empty sequence is Delete: that user then
+ *   windows to an empty history, as an unknown user does.  Clear (cache.go:51-55) is ctr_ubcache_upload of an empty
+ *   cache (offsets {0, 0}).
+ * Item rows are stored as given (-1 or out of range reads as a zero row, as with upload).  A user row must lie in
+ * [0, max(cache users, USER_FEAT rows, user id map size)); the cache's user count grows to the largest row + 1.
+ * Everything is validated on the host before any device work (CTR_EINVAL), and a failed call leaves the cache as it
+ * was.  One call rewrites the CSR into a spare buffer and swaps the two (O(stored events + users) of HBM traffic), on
+ * the engine stream.  With world > 1 each rank's cache is its own; these calls are not collective.
+ * download: the live cache back to the host.  *n_users and *n are always written; offsets [n_users+1] is written when
+ *   non-NULL and cap_users >= n_users, ts / item_rows [n] when non-NULL and cap_events >= n; a non-NULL array that is
+ *   too small is CTR_EINVAL, no cache is CTR_ESTATE. */
+int ctr_ubcache_append(ctr_handle* h, const int32_t* user_rows, const int64_t* ts, const int32_t* item_rows, int64_t n);
+int ctr_ubcache_set(ctr_handle* h, const int32_t* user_rows, const int64_t* offsets, const int64_t* ts,
+                    const int32_t* item_rows, int64_t n_set, int64_t n);
+int ctr_ubcache_download(ctr_handle* h, int64_t* offsets, int64_t* ts, int32_t* item_rows,
+                         int64_t cap_users, int64_t cap_events, int64_t* n_users, int64_t* n);
+
 /* ---- sparse ids, serving keys, checkpoint (SURVEY.md §8f rows f3, f4) ------------------------------------
  * The reference keys its caches by the decimal string of a Go int (rcmd.go:472,483,502,519); the engine's
  * tables are dense.  ctr_idmap_build puts `ids[i] → row i` into a device hash table (which: CTR_IDMAP_*);
