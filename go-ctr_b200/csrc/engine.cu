@@ -2646,18 +2646,20 @@ int ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, i
 // ---- model/mlp: the float64 MLP classifier (row a11) ---------------------------------------------------------
 struct ctr_mlp {
     ctr_mlp_config cfg{};
+    ctr_mlp_options opts{};
     Mlp64Dims d{};
     long np = 0;
     int dev = 0, num_sms = 132;
     cudaStream_t stream = nullptr;
     mutable std::string err;
     std::mutex mu;
-    double *params = nullptr, *grads = nullptr, *ms = nullptr, *vs = nullptr;
+    double *params = nullptr, *grads = nullptr, *ms = nullptr, *vs = nullptr;     // sgd keeps its velocities in ms
     double *act[kMlpMaxLayers] = {}, *del[kMlpMaxLayers] = {};       // [rows_cap, units[l]]
     long rows_cap = 0;
     double *X64 = nullptr; float* Y32 = nullptr; long* idx = nullptr; size_t x_cap = 0, y_cap = 0, idx_cap = 0;
     double* scal = nullptr;                                           // [0] batch loss, [1] epoch accumulator
     double adam_calls = 0;                                            // AdamOptimizer64.t
+    double t = 0;                                                     // BaseMultilayerPerceptron64.t: samples since initialize (:412,814)
     bool fitted = false;
 };
 namespace {
@@ -2707,6 +2709,11 @@ void mlp_forward(ctr_mlp* m, const long* idx, long row0, int rows) {
 }
 }  // namespace
 
+void ctr_mlp_options_default(ctr_mlp_options* o) {
+    memset(o, 0, sizeof *o);
+    o->solver = CTR_MLP_SOLVER_ADAM; o->lr_schedule = CTR_MLP_LR_CONSTANT; o->nesterov = 1;     // :229-256
+    o->power_t = 0.5; o->momentum = 0.9; o->weight_decay = 0.0;
+}
 void ctr_mlp_config_default(ctr_mlp_config* c, int32_t n_features) {
     memset(c, 0, sizeof *c);
     c->n_layers = 3; c->units[0] = n_features; c->units[1] = 100; c->units[2] = 1;      // HiddenLayerSizes {100}, basemlp64.go:239
@@ -2716,21 +2723,39 @@ void ctr_mlp_config_default(ctr_mlp_config* c, int32_t n_features) {
 }
 const char* ctr_mlp_last_error(const ctr_mlp* m) { return m ? m->err.c_str() : g_create_error.c_str(); }
 
-int ctr_mlp_create(const ctr_mlp_config* cfg, ctr_mlp** out) {
+int ctr_mlp_create(const ctr_mlp_config* cfg, ctr_mlp** out) { return ctr_mlp_create_ex(cfg, nullptr, out); }
+
+int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out) {
     if (!cfg || !out) return mlp_err(nullptr, CTR_EINVAL, "null argument");
     *out = nullptr;
     const ctr_mlp_config& c = *cfg;
     if (c.n_layers < 2 || c.n_layers > kMlpMaxLayers) return mlp_err(nullptr, CTR_EINVAL, "n_layers must be in [2, %d]", kMlpMaxLayers);
     for (int i = 0; i < c.n_layers; i++) if (c.units[i] < 1) return mlp_err(nullptr, CTR_EINVAL, "layer %d has %d units", i, c.units[i]);
     if (c.units[c.n_layers - 1] != 1) return mlp_err(nullptr, CTR_EINVAL, "binary classifier: one output unit (basemlp64.go:423-425)");
-    if (c.hidden_act < CTR_MLP_RELU || c.hidden_act > CTR_MLP_IDENTITY || c.max_iter < 1) return mlp_err(nullptr, CTR_EINVAL, "bad activation / max_iter");
+    if (c.hidden_act < CTR_MLP_RELU || c.hidden_act > CTR_MLP_TANH || c.max_iter < 1) return mlp_err(nullptr, CTR_EINVAL, "bad activation / max_iter");
+    ctr_mlp_options o;
+    ctr_mlp_options_default(&o);
+    if (opts) o = *opts;
+    else if (c.adaptive) o.lr_schedule = CTR_MLP_LR_ADAPTIVE;
+    if (o.solver != CTR_MLP_SOLVER_ADAM && o.solver != CTR_MLP_SOLVER_SGD)
+        return mlp_err(nullptr, CTR_EINVAL, "solver %d: adam (%d) or sgd (%d); lbfgs is not built", o.solver, CTR_MLP_SOLVER_ADAM, CTR_MLP_SOLVER_SGD);
+    if (o.lr_schedule < CTR_MLP_LR_CONSTANT || o.lr_schedule > CTR_MLP_LR_ADAPTIVE)
+        return mlp_err(nullptr, CTR_EINVAL, "lr_schedule %d: constant (0), invscaling (1) or adaptive (2)", o.lr_schedule);
+    if (c.adaptive && o.lr_schedule != CTR_MLP_LR_ADAPTIVE)
+        return mlp_err(nullptr, CTR_EINVAL, "cfg.adaptive is set but the options' lr_schedule is %d, not adaptive", o.lr_schedule);
+    if (!(o.momentum >= 0.0 && o.momentum <= 1.0)) return mlp_err(nullptr, CTR_EINVAL, "momentum %g must be in [0, 1] (basemlp64.go:635)", o.momentum);
+    if (!(o.weight_decay >= 0.0 && o.weight_decay < 1.0)) return mlp_err(nullptr, CTR_EINVAL, "weight_decay %g must be in [0, 1)", o.weight_decay);
+    if (!std::isfinite(o.power_t)) return mlp_err(nullptr, CTR_EINVAL, "power_t must be finite");
+    if (o.nesterov != 0 && o.nesterov != 1) return mlp_err(nullptr, CTR_EINVAL, "nesterov must be 0 or 1");
+    if (o.reserved0) return mlp_err(nullptr, CTR_EINVAL, "ctr_mlp_options.reserved0 must be 0");
+    for (double r : o.reserved) if (r != 0.0) return mlp_err(nullptr, CTR_EINVAL, "ctr_mlp_options.reserved must be 0");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return mlp_err(nullptr, CTR_ENODEV, "no CUDA device: this engine has no CPU fallback"); }
     if (c.device < 0 || c.device >= ndev) return mlp_err(nullptr, CTR_ENODEV, "device %d of %d", c.device, ndev);
     cudaDeviceProp prop{}; cudaGetDeviceProperties(&prop, c.device);
     if (prop.major != 9) return mlp_err(nullptr, CTR_ENODEV, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
     ctr_mlp* m = new ctr_mlp();
-    m->cfg = c; m->dev = c.device; m->num_sms = prop.multiProcessorCount;
+    m->cfg = c; m->opts = o; m->dev = c.device; m->num_sms = prop.multiProcessorCount;
     m->d.n_layers = c.n_layers; m->d.hidden_act = c.hidden_act;
     long off = 0;
     for (int l = 0; l < c.n_layers; l++) { m->d.units[l] = c.units[l]; if (l + 1 < c.n_layers) { m->d.off[l] = off; off += (long)(1 + c.units[l]) * c.units[l + 1]; } }
@@ -2802,10 +2827,14 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
         }
         MCU(m, cudaMemcpyAsync(m->params, p.data(), sizeof(double) * (size_t)m->np, cudaMemcpyHostToDevice, m->stream));
         MCU(m, cudaStreamSynchronize(m->stream));
+        m->t = 0;                                                        // :412
     }
-    MCU(m, cudaMemsetAsync(m->ms, 0, sizeof(double) * (size_t)m->np, m->stream));        // a fresh optimizer per fit (:541-556)
+    const ctr_mlp_options& o = m->opts;
+    const bool sgd = o.solver == CTR_MLP_SOLVER_SGD;
+    MCU(m, cudaMemsetAsync(m->ms, 0, sizeof(double) * (size_t)m->np, m->stream));        // a fresh optimizer per fit (:731-752)
     MCU(m, cudaMemsetAsync(m->vs, 0, sizeof(double) * (size_t)m->np, m->stream));
     m->adam_calls = 0;
+    double sgd_lr = c.lr_init;                                           // SGDOptimizer64.LearningRate
     std::vector<long> idx((size_t)n);
     for (int64_t i = 0; i < n; i++) idx[(size_t)i] = i;
     double lr_init = c.lr_init, lr_last = c.lr_init, best = INFINITY;
@@ -2820,6 +2849,8 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
         for (long b0 = 0; b0 < n; b0 += bs) {                            // :791-808
             const int rows = (int)std::min<long>(bs, n - b0);
             const long* bi = m->idx + b0;
+            if (o.weight_decay > 0.0)                                    // backprop :342-346
+                k_mlp64_decay<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->np, 1.0 - o.weight_decay);
             mlp_forward(m, bi, 0, rows);
             k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], m->Y32, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
             for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
@@ -2827,8 +2858,12 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
                     m->params, m->grads, m->d, l, m->X64, nin, bi, l == 0 ? nullptr : m->act[l], m->del[l + 1], rows, c.alpha);
                 if (l >= 1) k_mlp64_delta<<<mlp_grid(m, (long)rows * m->d.units[l]), 256, 0, m->stream>>>(m->params, m->d, l, m->act[l], m->del[l + 1], m->del[l], rows);
             }
-            k_mlp64_adam<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->vs, m->np, m->adam_calls, lr_init, c.beta1, c.beta2, c.eps);
-            m->adam_calls += 1;
+            if (sgd) {
+                k_mlp64_sgd<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->np, sgd_lr, o.momentum, o.nesterov);
+            } else {
+                k_mlp64_adam<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->vs, m->np, m->adam_calls, lr_init, c.beta1, c.beta2, c.eps);
+                m->adam_calls += 1;
+            }
         }
         it++;
         double sc[2] = {0, 0};
@@ -2836,17 +2871,21 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
         MCU(m, cudaStreamSynchronize(m->stream));
         MCU(m, cudaGetLastError());
         const double loss = sc[1] / (double)n;                           // :810-811
+        m->t += (double)n;                                               // :814
         if (loss_curve) loss_curve[it - 1] = loss;
-        {   // the learning rate the optimizer last used (:1088): decides "adaptive" stopping (:1059-1064)
+        if (!sgd) {   // the learning rate the optimizer last used (:1088): decides "adaptive" stopping (:1059-1064)
             const double e = m->adam_calls * (double)m->np;
             lr_last = lr_init * std::sqrt(1.0 - std::pow(c.beta2, e)) / (1.0 - std::pow(c.beta1, e));
         }
         if (loss > best - c.tol) no_improve++; else no_improve = 0;      // :886-892
         if (loss < best) best = loss;
+        if (sgd && o.lr_schedule == CTR_MLP_LR_INVSCALING)               // iterationEnds :999-1003 (Adam's is a no-op, :1053)
+            sgd_lr = c.lr_init / std::pow(m->t + 1.0, o.power_t);
         if (no_improve > c.n_iter_no_change) {                           // :826-840
-            if (!c.adaptive) break;                                      // triggerStopping :1053-1058
-            if (lr_last <= 1e-6) break;
-            lr_init *= .8;
+            if (o.lr_schedule != CTR_MLP_LR_ADAPTIVE) break;             // triggerStopping :1005-1011, :1054-1060
+            if ((sgd ? sgd_lr : lr_last) <= 1e-6) break;                 // :1012-1017, :1061-1066
+            if (sgd) sgd_lr *= .8;                                       // :1018 — the current rate
+            else lr_init *= .8;                                          // :1067 — the base rate
             no_improve = 0;
         }
     }

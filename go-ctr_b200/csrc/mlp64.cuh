@@ -3,10 +3,11 @@
 // nn/neural_network/basemlp64.go `BaseMultilayerPerceptron64`: fit :484, fitStochastic :729, backprop :340,
 // forwardPass :259, AdamOptimizer64.updateParams :1075).
 //
-// One hidden layer or more, biases, relu / logistic hidden activation, logistic output + binary_log_loss with the
+// One hidden layer or more, biases, relu / logistic / identity / tanh hidden activation, logistic output + binary_log_loss with the
 // probabilities clipped to (nextafter(0,1), nextafter(1,0)) (:180-195), L2 term alpha/(2n)·Σw² in the loss (:361) and
 // alpha/n·w in the coefficient gradients (:327), Adam whose beta powers advance once per parameter ELEMENT
-// (:1082-1090 — the bias correction is gone within the first call), minibatches of 200 visited through a per-epoch
+// (:1082-1090 — the bias correction is gone within the first call) or SGD with momentum / Nesterov (:1024-1039),
+// weight decay of the whole packed vector before every minibatch (:342-346), minibatches of 200 visited through a per-epoch
 // shuffle (:788), tol / n_iter_no_change stopping (:826-840,886-890).
 //
 // All arithmetic is float64 (the reference's: gonum Dgemm).  A step is ~17 MFLOP — launch-latency, not throughput,
@@ -20,7 +21,7 @@
 namespace ctr {
 
 constexpr int kMlpMaxLayers = 8;
-enum { MLP_ACT_RELU = 0, MLP_ACT_LOGISTIC = 1, MLP_ACT_IDENTITY = 2 };
+enum { MLP_ACT_RELU = 0, MLP_ACT_LOGISTIC = 1, MLP_ACT_IDENTITY = 2, MLP_ACT_TANH = 3 };
 
 struct Mlp64Dims {
     int n_layers;                    // len(layerUnits) = hidden layers + 2
@@ -46,6 +47,7 @@ k_mlp64_layer(const double* __restrict__ params, Mlp64Dims d, int l, const doubl
         z += b[j];                                                              // addIntercepts64 :205
         if (last || d.hidden_act == MLP_ACT_LOGISTIC) z = 1.0 / (1.0 + exp(-z));   // :82-88, out_activation :423-425
         else if (d.hidden_act == MLP_ACT_RELU) z = z < 0.0 ? 0.0 : z;             // :96-104
+        else if (d.hidden_act == MLP_ACT_TANH) z = tanh(-z);                       // :88-94 — the argument is negated
         out[t] = z;
     }
 }
@@ -111,7 +113,9 @@ k_mlp64_grads(const double* __restrict__ params, double* __restrict__ grads, Mlp
     }
 }
 
-// delta of hidden layer l from delta of layer l+1 (:388-396): (delta_{l+1} · Wᵀ) ⊙ act'(z)
+// delta of hidden layer l from delta of layer l+1 (:388-396): (delta_{l+1} · Wᵀ) ⊙ act'(z).  For tanh the factor is
+// 1 − a² (:131-138), the derivative of tanh(z) although the forward pass computed tanh(−z): every layer below an odd
+// number of tanh layers receives the negated data gradient, as in the reference.
 __global__ void __launch_bounds__(256)
 k_mlp64_delta(const double* __restrict__ params, Mlp64Dims d, int l, const double* __restrict__ act, const double* __restrict__ dnext,
               double* __restrict__ dcur, int m) {
@@ -124,6 +128,7 @@ k_mlp64_delta(const double* __restrict__ params, Mlp64Dims d, int l, const doubl
         const double z = act[t];
         if (d.hidden_act == MLP_ACT_RELU) { if (z == 0.0) s = 0.0; }                   // :140-148
         else if (d.hidden_act == MLP_ACT_LOGISTIC) s *= z * (1.0 - z);                 // :124-131
+        else if (d.hidden_act == MLP_ACT_TANH) s *= 1.0 - z * z;                       // :131-138
         dcur[t] = s;
     }
 }
@@ -143,6 +148,26 @@ k_mlp64_adam(double* __restrict__ params, const double* __restrict__ grads, doub
         const double lr = lr_init * sqrt(1.0 - b2t) / (1.0 - b1t);
         params[i] += -lr * m / (sqrt(v) + eps);
     }
+}
+
+// SGDOptimizer64.updateParams (:1024-1039): u = momentum·v − lr·g, v = u; p += momentum·v − lr·g (Nesterov) or u.
+// vel is zero at the start of every fit (the optimizer is rebuilt per fit, :731-752).
+__global__ void __launch_bounds__(256)
+k_mlp64_sgd(double* __restrict__ params, const double* __restrict__ grads, double* __restrict__ vel, long np,
+            double lr, double momentum, int nesterov) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < np; i += (long)gridDim.x * blockDim.x) {
+        const double g = grads[i];
+        const double u = momentum * vel[i] - lr * g;
+        vel[i] = u;
+        params[i] += nesterov ? momentum * u - lr * g : u;
+    }
+}
+
+// weight decay at the top of backprop (:342-346): every packed element, intercepts included, times (1 − weight_decay),
+// before the forward pass of the minibatch; keep = 1 − weight_decay is rounded once on the host as in the reference
+__global__ void __launch_bounds__(256)
+k_mlp64_decay(double* __restrict__ params, long np, double keep) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < np; i += (long)gridDim.x * blockDim.x) params[i] *= keep;
 }
 
 __global__ void __launch_bounds__(256)

@@ -9,7 +9,7 @@ import numpy as np
 
 from . import build as _build
 
-__all__ = ["Engine", "Config", "MLPClassifier", "MlpConfig", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
+__all__ = ["Engine", "Config", "MLPClassifier", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
            "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE"]
 
@@ -28,7 +28,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
-           "ctr_mlp_config_default", "ctr_mlp_create", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
+           "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params"]
 
 
@@ -52,6 +52,11 @@ class MlpConfig(C.Structure):
                 ("n_iter_no_change", C.c_int32), ("shuffle", C.c_int32), ("adaptive", C.c_int32), ("warm_start", C.c_int32), ("seed", C.c_uint32),
                 ("device", C.c_int32), ("alpha", C.c_double), ("lr_init", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
                 ("eps", C.c_double), ("tol", C.c_double)]
+
+
+class MlpOptions(C.Structure):
+    _fields_ = [("solver", C.c_int32), ("lr_schedule", C.c_int32), ("nesterov", C.c_int32), ("reserved0", C.c_int32),
+                ("power_t", C.c_double), ("momentum", C.c_double), ("weight_decay", C.c_double), ("reserved", C.c_double * 5)]
 
 
 class StepStats(C.Structure):
@@ -87,6 +92,7 @@ def load_library():
     L.ctr_mlp_destroy.argtypes = [C.c_void_p]
     L.ctr_mlp_destroy.restype = None
     L.ctr_mlp_config_default.restype = None
+    L.ctr_mlp_options_default.restype = None
     _lib = L
     return L
 
@@ -403,16 +409,46 @@ class Engine:
         return out_r, out_s, out_l, cnt
 
 
-MLP_ACT = {"relu": 0, "logistic": 1, "identity": 2}
+MLP_ACT = {"relu": 0, "logistic": 1, "identity": 2, "tanh": 3}
+MLP_SOLVER = {"adam": 0, "sgd": 1}
+MLP_LR = {"constant": 0, "invscaling": 1, "adaptive": 2}
 
 
 class MLPClassifier:
-    """nn.MLPClassifier on the device (float64): NewMLPClassifier(hidden, activation, "adam", alpha) with
-    NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:81-90, basemlp64.go:227-256)."""
+    """nn.MLPClassifier on the device (float64): NewMLPClassifier(hidden, activation, solver, alpha) with
+    NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:81-90, basemlp64.go:227-256).
+
+    `adaptive=True` is `learning_rate="adaptive"`; naming another schedule beside it raises.  solver "lbfgs",
+    early_stopping and batch_normalize are not built and raise instead of being ignored."""
 
     def __init__(self, n_features, hidden=(100,), activation="relu", alpha=1e-4, batch=200, max_iter=200, lr_init=1e-3,
-                 adaptive=False, shuffle=True, seed=0, tol=1e-4, n_iter_no_change=10, warm_start=False, device=0):
+                 adaptive=False, shuffle=True, seed=0, tol=1e-4, n_iter_no_change=10, warm_start=False, device=0,
+                 solver="adam", learning_rate=None, power_t=0.5, momentum=0.9, nesterovs_momentum=True, weight_decay=0.0,
+                 early_stopping=False, batch_normalize=False):
+        if solver == "lbfgs":
+            raise ValueError("solver 'lbfgs' is not built: the reference runs gonum's optimize.Minimize (basemlp64.go:675-727), "
+                             "which is not part of the reference tree and cannot be restated or checked")
+        if early_stopping:
+            raise ValueError("early_stopping is not built: the reference scores raw probabilities by exact-equality accuracy "
+                             "(basemlp64.go:933-938, 1143-1155) and then restores a best-parameter copy it never wrote (:850-853)")
+        if batch_normalize:
+            raise ValueError("batch_normalize is not built: the reference normalises activations in training only (:347-351), never in predict (:897-915)")
+        if solver not in MLP_SOLVER:
+            raise ValueError("solver must be one of %s, got %r" % (sorted(MLP_SOLVER), solver))
+        if activation not in MLP_ACT:
+            raise ValueError("activation must be one of %s, got %r" % (sorted(MLP_ACT), activation))
+        if learning_rate is None:
+            learning_rate = "adaptive" if adaptive else "constant"
+        elif adaptive and learning_rate != "adaptive":
+            raise ValueError("adaptive=True contradicts learning_rate=%r" % (learning_rate,))
+        if learning_rate not in MLP_LR:
+            raise ValueError("learning_rate must be one of %s, got %r" % (sorted(MLP_LR), learning_rate))
         self.L = load_library()
+        opts = MlpOptions()
+        self.L.ctr_mlp_options_default(C.byref(opts))
+        opts.solver = MLP_SOLVER[solver]; opts.lr_schedule = MLP_LR[learning_rate]; opts.nesterov = int(bool(nesterovs_momentum))
+        opts.power_t = power_t; opts.momentum = momentum; opts.weight_decay = weight_decay
+        self.opts = opts
         cfg = MlpConfig()
         self.L.ctr_mlp_config_default(C.byref(cfg), C.c_int32(n_features))
         units = [n_features, *hidden, 1]
@@ -420,11 +456,11 @@ class MLPClassifier:
         for i, u in enumerate(units):
             cfg.units[i] = u
         cfg.hidden_act = MLP_ACT[activation]; cfg.alpha = alpha; cfg.batch = batch; cfg.max_iter = max_iter; cfg.lr_init = lr_init
-        cfg.adaptive = int(adaptive); cfg.shuffle = int(shuffle); cfg.seed = seed; cfg.tol = tol; cfg.n_iter_no_change = n_iter_no_change
+        cfg.adaptive = int(learning_rate == "adaptive"); cfg.shuffle = int(shuffle); cfg.seed = seed; cfg.tol = tol; cfg.n_iter_no_change = n_iter_no_change
         cfg.warm_start = int(warm_start); cfg.device = device
         self.cfg = cfg
         self.h = C.c_void_p()
-        rc = self.L.ctr_mlp_create(C.byref(cfg), C.byref(self.h))
+        rc = self.L.ctr_mlp_create_ex(C.byref(cfg), C.byref(opts), C.byref(self.h))
         if rc != 0:
             raise CtrError(rc, self.L.ctr_mlp_last_error(None).decode())
         self.n_iter = 0; self.loss_curve = np.zeros(0)

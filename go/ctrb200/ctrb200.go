@@ -409,14 +409,31 @@ func NewEngineWith(kind Kind, uP, S, D, cF, batchSize, predBatchSize, tableOpt i
 // ---- model/mlp: drop-in for mlp.SimpleMlpFitWrap / SimpleMlpPredWrap (model/mlp/mlp.go:11-65) -----------------
 
 // MlpFitWrap satisfies recommend.Fitter like mlp.SimpleMlpFitWrap{Model: nn.NewMLPClassifier([]int{100}, "relu",
-// "adam", 1e-4)} (main.go:42-52): float32 TrainSample in, float64 training on the device.
+// "adam", 1e-4)} (main.go:42-52): float32 TrainSample in, float64 training on the device.  The fields after Seed
+// carry the names of BaseMultilayerPerceptron64's (basemlp64.go:25-50); a zero value means the reference default,
+// and pointer fields exist where zero is itself a meaningful setting.  Fit returns an error for what the engine
+// does not build (solver "lbfgs", EarlyStopping, BatchNormalize) instead of training something else.
 type MlpFitWrap struct {
 	Hidden      []int   // HiddenLayerSizes, default {100}
-	Activation  int     // C.CTR_MLP_RELU (default) | CTR_MLP_LOGISTIC | CTR_MLP_IDENTITY
+	Activation  int     // C.CTR_MLP_RELU (default) | CTR_MLP_LOGISTIC | CTR_MLP_IDENTITY | CTR_MLP_TANH
 	Alpha       float64 // 1e-4
 	MaxIter     int     // 200
 	Adaptive    bool    // LearningRate == "adaptive"
 	Seed        uint32
+
+	Solver            string   // "adam" (default) | "sgd"
+	LearningRate      string   // "constant" (default, or "adaptive" when Adaptive) | "invscaling" | "adaptive"
+	LearningRateInit  float64  // 1e-3
+	PowerT            float64  // .5 (invscaling)
+	Momentum          *float64 // .9 (sgd), in [0, 1]
+	NesterovsMomentum *bool    // true (sgd)
+	WeightDecay       float64  // 0, in [0, 1)
+	BatchSize         int      // 200; clipped to the sample count
+	Tol               float64  // 1e-4
+	NIterNoChange     int      // 10
+	Shuffle           *bool    // true
+	EarlyStopping     bool     // not built: an error
+	BatchNormalize    bool     // not built: an error
 }
 
 // MlpPredWrap satisfies recommend.PredictAbstract like mlp.SimpleMlpPredWrap.
@@ -446,9 +463,66 @@ func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, e
 		cfg.adaptive = 1
 	}
 	cfg.seed = C.uint32_t(f.Seed)
+	if f.LearningRateInit != 0 {
+		cfg.lr_init = C.double(f.LearningRateInit)
+	}
+	if f.BatchSize != 0 {
+		cfg.batch = C.int32_t(f.BatchSize)
+	}
+	if f.Tol != 0 {
+		cfg.tol = C.double(f.Tol)
+	}
+	if f.NIterNoChange != 0 {
+		cfg.n_iter_no_change = C.int32_t(f.NIterNoChange)
+	}
+	if f.Shuffle != nil && !*f.Shuffle {
+		cfg.shuffle = 0
+	}
+	var opts C.ctr_mlp_options
+	C.ctr_mlp_options_default(&opts)
+	switch f.Solver {
+	case "", "adam":
+	case "sgd":
+		opts.solver = C.CTR_MLP_SOLVER_SGD
+	case "lbfgs":
+		return nil, fmt.Errorf("MlpFitWrap: solver lbfgs is not built: the reference runs gonum's optimize.Minimize (basemlp64.go:675-727), which cannot be restated here")
+	default:
+		return nil, fmt.Errorf("MlpFitWrap: solver %q is not one of adam, sgd", f.Solver)
+	}
+	switch f.LearningRate {
+	case "":
+		if f.Adaptive {
+			opts.lr_schedule = C.CTR_MLP_LR_ADAPTIVE
+		}
+	case "constant":
+		opts.lr_schedule = C.CTR_MLP_LR_CONSTANT
+	case "invscaling":
+		opts.lr_schedule = C.CTR_MLP_LR_INVSCALING
+	case "adaptive":
+		opts.lr_schedule = C.CTR_MLP_LR_ADAPTIVE
+		cfg.adaptive = 1
+	default:
+		return nil, fmt.Errorf("MlpFitWrap: learning rate %q is not one of constant, invscaling, adaptive", f.LearningRate)
+	}
+	if f.EarlyStopping {
+		return nil, fmt.Errorf("MlpFitWrap: EarlyStopping is not built: the reference scores raw probabilities by exact-equality accuracy (basemlp64.go:933-938) and restores a best-parameter copy it never wrote (:850-853)")
+	}
+	if f.BatchNormalize {
+		return nil, fmt.Errorf("MlpFitWrap: BatchNormalize is not built: the reference normalises in training only, never in predict (:347-351, :897-915)")
+	}
+	if f.PowerT != 0 {
+		opts.power_t = C.double(f.PowerT)
+	}
+	if f.Momentum != nil {
+		opts.momentum = C.double(*f.Momentum)
+	}
+	if f.NesterovsMomentum != nil && !*f.NesterovsMomentum {
+		opts.nesterov = 0
+	}
+	opts.weight_decay = C.double(f.WeightDecay)
 	var m *C.ctr_mlp
-	if rc := C.ctr_mlp_create(&cfg, &m); rc != C.CTR_OK {
-		return nil, fmt.Errorf("ctr_mlp_create: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(nil)))
+	if rc := C.ctr_mlp_create_ex(&cfg, &opts, &m); rc != C.CTR_OK {
+		return nil, fmt.Errorf("ctr_mlp_create_ex: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(nil)))
 	}
 	var iters C.int32_t
 	if rc := C.ctr_mlp_fit(m, f32(trainSample.X), f32(trainSample.Y), C.int64_t(trainSample.Rows), C.int32_t(trainSample.XCols), &iters, nil); rc != C.CTR_OK {

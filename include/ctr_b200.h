@@ -343,12 +343,14 @@ int  ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, 
  * a11) — main.go:42-52 → model/mlp/mlp.go:45-65 (SimpleMlpFitWrap.Fit / SimpleMlpPredWrap.Predict: float32 samples →
  * float64 → nn.MLPClassifier) → nn/neural_network/basemlp64.go.  Float64 arithmetic on the device; packed parameter
  * vector in the reference's layout (basemlp64.go:459-463: per layer [intercepts | coefs row-major]). -------------- */
-enum { CTR_MLP_RELU = 0, CTR_MLP_LOGISTIC = 1, CTR_MLP_IDENTITY = 2 };
+enum { CTR_MLP_RELU = 0, CTR_MLP_LOGISTIC = 1, CTR_MLP_IDENTITY = 2, CTR_MLP_TANH = 3 };
+enum { CTR_MLP_SOLVER_ADAM = 0, CTR_MLP_SOLVER_SGD = 1 };                              /* Solver "adam" | "sgd" */
+enum { CTR_MLP_LR_CONSTANT = 0, CTR_MLP_LR_INVSCALING = 1, CTR_MLP_LR_ADAPTIVE = 2 };  /* LearningRate */
 typedef struct ctr_mlp ctr_mlp;
 typedef struct {
     int32_t n_layers;                 /* len(layerUnits): hidden layers + 2 (basemlp64.go:495-497) */
     int32_t units[8];                 /* [nFeatures, HiddenLayerSizes..., 1] */
-    int32_t hidden_act;               /* Activation "relu" (:229) | "logistic" | "identity"; the output is logistic (:423-425) */
+    int32_t hidden_act;               /* Activation "relu" (:229) | "logistic" | "identity" | "tanh"; the output is logistic (:423-425) */
     int32_t batch, max_iter, n_iter_no_change;   /* BatchSize 200, MaxIter 200, NIterNoChange 10 (:233,238,254) */
     int32_t shuffle, adaptive;        /* Shuffle true (:241); LearningRate == "adaptive" */
     int32_t warm_start;               /* WarmStart (:245): keep the current parameters instead of re-initialising */
@@ -358,10 +360,29 @@ typedef struct {
 } ctr_mlp_config;
 void ctr_mlp_config_default(ctr_mlp_config* cfg, int32_t n_features);      /* NewBaseMultilayerPerceptron64, :227-256 */
 int  ctr_mlp_create(const ctr_mlp_config* cfg, ctr_mlp** out);             /* nn.NewMLPClassifier */
+/* The solver surface of BaseMultilayerPerceptron64 beyond ctr_mlp_config (basemlp64.go:25-50).  "lbfgs",
+ * EarlyStopping and BatchNormalize are not built; callers must reject them rather than drop them. */
+typedef struct {
+    int32_t solver;                   /* CTR_MLP_SOLVER_*: "adam" (:1075-1091) or "sgd" (SGDOptimizer64, :987-1039) */
+    int32_t lr_schedule;              /* CTR_MLP_LR_*: "constant"; "invscaling": lr = lr_init / (t+1)^power_t at every epoch
+                                       * end, t = samples seen since the last cold initialise (:999-1003, :814) — sgd only,
+                                       * Adam treats it as "constant" (:1053); "adaptive" (:1005-1023, :1054-1073) */
+    int32_t nesterov;                 /* NesterovsMomentum (sgd) */
+    int32_t reserved0;                /* 0 */
+    double power_t;                   /* PowerT .5 */
+    double momentum;                  /* Momentum .9, in [0, 1] (sgd) */
+    double weight_decay;              /* WeightDecay 0, in [0, 1): packed parameters *= (1 − wd) before every minibatch (:342-346) */
+    double reserved[5];               /* 0 */
+} ctr_mlp_options;
+void ctr_mlp_options_default(ctr_mlp_options* opts);                       /* adam, constant, .5, .9, Nesterov, 0 */
+/* ctr_mlp_create(cfg, out) == ctr_mlp_create_ex(cfg, NULL, out): default options, lr_schedule adaptive iff cfg->adaptive.
+ * cfg->adaptive together with a non-adaptive opts->lr_schedule is CTR_EINVAL. */
+int  ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out);
 void ctr_mlp_destroy(ctr_mlp* m);
 const char* ctr_mlp_last_error(const ctr_mlp* m);
 /* SimpleMlpFitWrap.Fit (mlp.go:45-65): X [n, xcols] float32, Y [n] float32 in {0,1} → fit (basemlp64.go:484-567 →
- * fitStochastic :729-857, solver adam).  *n_iter = epochs run (NIter); loss_curve (may be NULL) receives max_iter
+ * fitStochastic :729-857, solver adam or sgd).  The sample count t of "invscaling" carries over warm-start fits
+ * (and ctr_mlp_set_params) and restarts at 0 whenever the parameters are initialised.  *n_iter = epochs run (NIter); loss_curve (may be NULL) receives max_iter
  * per-epoch losses at most. */
 int  ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, int32_t* n_iter, double* loss_curve);
 /* SimpleMlpPredWrap.Predict (mlp.go:15-39): probabilities as float32 [n] (the 64-bit class returns them raw,
