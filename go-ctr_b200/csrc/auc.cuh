@@ -4,6 +4,7 @@
 // SURVEY.md §8(f) row f4 (on-device eval).  CUB does the sort/scans; the curve logic is below.
 #pragma once
 #include "common.cuh"
+#include "owner.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -42,44 +43,39 @@ __global__ void k_auc_area(const unsigned* __restrict__ keys, const int* __restr
 
 // pred_h / y_h are host pointers; returns cudaSuccess and *auc (NaN when one class is absent)
 inline cudaError_t auc_run(cudaStream_t st, const float* pred_h, const float* y_h, long n, double* auc) {
-    float *d_pred = nullptr, *d_y = nullptr; unsigned *k0 = nullptr, *k1 = nullptr; int *f0 = nullptr, *f1 = nullptr, *tp = nullptr, *head = nullptr;
-    double* d_area = nullptr; void* tmp = nullptr;
-    cudaError_t e = cudaSuccess;
-#define AUC_TRY(x) do { e = (x); if (e != cudaSuccess) goto done; } while (0)
-    {
-        AUC_TRY(cudaMalloc(&d_pred, n * sizeof(float))); AUC_TRY(cudaMalloc(&d_y, n * sizeof(float)));
-        AUC_TRY(cudaMalloc(&k0, n * sizeof(unsigned))); AUC_TRY(cudaMalloc(&k1, n * sizeof(unsigned)));
-        AUC_TRY(cudaMalloc(&f0, n * sizeof(int))); AUC_TRY(cudaMalloc(&f1, n * sizeof(int)));
-        AUC_TRY(cudaMalloc(&tp, n * sizeof(int))); AUC_TRY(cudaMalloc(&head, n * sizeof(int)));
-        AUC_TRY(cudaMalloc(&d_area, sizeof(double)));
-        AUC_TRY(cudaMemcpyAsync(d_pred, pred_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
-        AUC_TRY(cudaMemcpyAsync(d_y, y_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
-        AUC_TRY(cudaMemsetAsync(d_area, 0, sizeof(double), st));
-        size_t b0 = 0, b1 = 0, b2 = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, b0, k0, k1, f0, f1, (int)n, 0, 32, st);
-        cub::DeviceScan::InclusiveSum(nullptr, b1, f1, tp, (int)n, st);
-        cub::DeviceScan::InclusiveScan(nullptr, b2, head, head, MaxOp(), (int)n, st);
-        size_t bytes = b0 > b1 ? b0 : b1; bytes = bytes > b2 ? bytes : b2;
-        AUC_TRY(cudaMalloc(&tmp, bytes ? bytes : 1));
-        int grid = (int)((n + 255) / 256); if (grid > 132 * 8) grid = 132 * 8;
-        k_auc_keys<<<grid, 256, 0, st>>>(d_pred, d_y, n, k0, f0);
-        AUC_TRY(cub::DeviceRadixSort::SortPairs(tmp, bytes, k0, k1, f0, f1, (int)n, 0, 32, st));
-        AUC_TRY(cub::DeviceScan::InclusiveSum(tmp, bytes, f1, tp, (int)n, st));
-        k_auc_heads<<<grid, 256, 0, st>>>(k1, n, head);
-        AUC_TRY(cub::DeviceScan::InclusiveScan(tmp, bytes, head, head, MaxOp(), (int)n, st));
-        k_auc_area<<<grid, 256, 0, st>>>(k1, tp, head, n, d_area);
-        double area = 0; int P = 0;
-        AUC_TRY(cudaMemcpyAsync(&area, d_area, sizeof(double), cudaMemcpyDeviceToHost, st));
-        AUC_TRY(cudaMemcpyAsync(&P, tp + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-        AUC_TRY(cudaStreamSynchronize(st));
-        AUC_TRY(cudaGetLastError());
-        double N = (double)n - (double)P;
-        *auc = (P > 0 && N > 0) ? area / ((double)P * N) : nan("");
-    }
-done:
+    DevBuf<float> d_pred, d_y; DevBuf<unsigned> k0, k1; DevBuf<int> f0, f1, tp, head;
+    DevBuf<double> d_area; DevBuf<unsigned char> tmp;
+#define AUC_TRY(x) do { const cudaError_t e_ = (x); if (e_ != cudaSuccess) return e_; } while (0)
+    AUC_TRY(d_pred.alloc(n)); AUC_TRY(d_y.alloc(n));
+    AUC_TRY(k0.alloc(n)); AUC_TRY(k1.alloc(n));
+    AUC_TRY(f0.alloc(n)); AUC_TRY(f1.alloc(n));
+    AUC_TRY(tp.alloc(n)); AUC_TRY(head.alloc(n));
+    AUC_TRY(d_area.alloc(1));
+    AUC_TRY(cudaMemcpyAsync(d_pred, pred_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
+    AUC_TRY(cudaMemcpyAsync(d_y, y_h, n * sizeof(float), cudaMemcpyHostToDevice, st));
+    AUC_TRY(cudaMemsetAsync(d_area, 0, sizeof(double), st));
+    size_t b0 = 0, b1 = 0, b2 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, b0, k0.get(), k1.get(), f0.get(), f1.get(), (int)n, 0, 32, st);
+    cub::DeviceScan::InclusiveSum(nullptr, b1, f1.get(), tp.get(), (int)n, st);
+    cub::DeviceScan::InclusiveScan(nullptr, b2, head.get(), head.get(), MaxOp(), (int)n, st);
+    size_t bytes = b0 > b1 ? b0 : b1; bytes = bytes > b2 ? bytes : b2;
+    AUC_TRY(tmp.alloc(bytes ? bytes : 1));
+    int grid = (int)((n + 255) / 256); if (grid > 132 * 8) grid = 132 * 8;
+    k_auc_keys<<<grid, 256, 0, st>>>(d_pred, d_y, n, k0, f0);
+    AUC_TRY(cub::DeviceRadixSort::SortPairs(tmp, bytes, k0.get(), k1.get(), f0.get(), f1.get(), (int)n, 0, 32, st));
+    AUC_TRY(cub::DeviceScan::InclusiveSum(tmp, bytes, f1.get(), tp.get(), (int)n, st));
+    k_auc_heads<<<grid, 256, 0, st>>>(k1, n, head);
+    AUC_TRY(cub::DeviceScan::InclusiveScan(tmp, bytes, head.get(), head.get(), MaxOp(), (int)n, st));
+    k_auc_area<<<grid, 256, 0, st>>>(k1, tp, head, n, d_area);
+    double area = 0; int P = 0;
+    AUC_TRY(cudaMemcpyAsync(&area, d_area, sizeof(double), cudaMemcpyDeviceToHost, st));
+    AUC_TRY(cudaMemcpyAsync(&P, tp + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+    AUC_TRY(cudaStreamSynchronize(st));
+    AUC_TRY(cudaGetLastError());
 #undef AUC_TRY
-    for (void* p : {(void*)d_pred, (void*)d_y, (void*)k0, (void*)k1, (void*)f0, (void*)f1, (void*)tp, (void*)head, (void*)d_area, tmp}) if (p) cudaFree(p);
-    return e;
+    double N = (double)n - (double)P;
+    *auc = (P > 0 && N > 0) ? area / ((double)P * N) : nan("");
+    return cudaSuccess;
 }
 
 }  // namespace ctr

@@ -22,6 +22,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "owner.cuh"
 #include "vmm.cuh"
 
 struct ctr_handle;
@@ -37,7 +38,7 @@ struct Comm {
     bool ready = false;
     // placement of ITEM_EMB under world > 1 (ITEM_FEAT: ctr_handle::tab_sharded)
     bool replicate = false;
-    float* table_grad = nullptr; size_t table_grad_n = 0;     // replicated placement: summed row gradients [rows, ld]
+    DevBuf<float> table_grad;                         // replicated placement: summed row gradients [rows, ld]
     // ---- row-sharded placement: peer mappings
     int wshift = 0;                                   // log2(world)
     float* peer_emb[kMaxPeers] = {};                  // rank j's ITEM_EMB shard ([j == rank] = the local table)
@@ -48,13 +49,13 @@ struct Comm {
     int lsock = -1; unsigned long long job_hash = 0;  // descriptor socket of this rank (abstract UDS named after the NCCL id)
     unsigned char* peer_arena[kMaxPeers] = {};
     unsigned long long epoch = 0;                     // barrier generation (same sequence on every rank)
-    int* h_err = nullptr; int* d_err = nullptr;       // pinned + mapped: set by a barrier that timed out
-    float* rows_cache = nullptr; size_t rows_cache_cap = 0;   // [Bmax, S+1, D] rows fetched by the forward
-    void* d_xchg = nullptr;                           // device staging of the handle all-gather
+    PinnedBuf<int> h_err; int* d_err = nullptr;       // pinned + mapped: set by a barrier that timed out
+    DevBuf<float> rows_cache;                         // [Bmax, S+1, D] rows fetched by the forward
+    DevBuf<unsigned char> d_xchg;                     // device staging of the handle all-gather
     // replicated hot rows of a sharded ITEM_EMB: rows [0, hot_k) live on every rank (hot_tab), their -lr/world scaled
     // gradient sums (hot_sum) are all-reduced with the dense gradients — a Zipf-popular row is neither pulled over
     // NVLink by every sample nor hammered by every rank's red.add
-    int hot_k = 0; float* hot_tab = nullptr; float* hot_sum = nullptr; float* hot_acc = nullptr; int hot_reps = 0;
+    int hot_k = 0; DevBuf<float> hot_tab, hot_sum, hot_acc; int hot_reps = 0;
 };
 
 }  // namespace ctr

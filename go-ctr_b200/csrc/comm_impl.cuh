@@ -99,8 +99,8 @@ int comm_publish(ctr_handle* h) {
     PubRec rec{};
     for (int k = 0; k < 3; k++) if (mine[k] && mine[k]->live) { rec.bytes[k] = mine[k]->bytes; rec.has[k] = 1; }
     if (!rec.has[0] || !rec.has[2]) return set_err(h, CTR_ESTATE, "row-sharded ITEM_EMB is not in shareable memory (upload the table after ctr_create with world > 1)");
-    if (!cm.d_xchg) CU(h, cudaMalloc(&cm.d_xchg, 256 * (size_t)(kMaxPeers + 1)));
-    PubRec* d_send = (PubRec*)cm.d_xchg; PubRec* d_recv = d_send + 1;
+    if (!cm.d_xchg) RET(dalloc(h, cm.d_xchg, 256 * (size_t)(kMaxPeers + 1), false));
+    PubRec* d_send = (PubRec*)cm.d_xchg.get(); PubRec* d_recv = d_send + 1;
     std::vector<PubRec> all((size_t)W);
     CU(h, cudaMemcpyAsync(d_send, &rec, sizeof rec, cudaMemcpyHostToDevice, h->stream));
     NC(h, g_nccl.AllGather(d_send, d_recv, sizeof(PubRec), kNcclChar, cm.nccl, h->stream));
@@ -155,13 +155,13 @@ int comm_hot_setup(ctr_handle* h) {
     if (want == 0) want = 32768;
     if (want < 0) want = 0;
     want = (int)std::min<int64_t>(want, h->tab_rows[CTR_TABLE_ITEM_EMB]);
-    for (float** p : {&cm.hot_tab, &cm.hot_sum, &cm.hot_acc}) if (*p) { cudaFree(*p); *p = nullptr; }
+    cm.hot_tab.reset(); cm.hot_sum.reset(); cm.hot_acc.reset();
     cm.hot_k = want; cm.hot_reps = 0;
     if (want == 0) return CTR_OK;
     if (h->tab_ld[CTR_TABLE_ITEM_EMB] != D) return set_err(h, CTR_EINVAL, "replicated hot rows need D %% 4 == 0");
-    RET(dalloc(h, &cm.hot_tab, (size_t)want * D, false)); RET(dalloc(h, &cm.hot_sum, (size_t)want * D));
+    RET(dalloc(h, cm.hot_tab, (size_t)want * D, false)); RET(dalloc(h, cm.hot_sum, (size_t)want * D));
     cm.hot_reps = (int)std::min<size_t>(16, std::max<size_t>(1, ((size_t)64 << 20) / ((size_t)want * D * sizeof(float))));
-    RET(dalloc(h, &cm.hot_acc, (size_t)cm.hot_reps * want * D));
+    RET(dalloc(h, cm.hot_acc, (size_t)cm.hot_reps * want * D));
     RowSrc r{}; r.lde = D; r.wmask = cm.world - 1; r.wshift = cm.wshift; r.world = cm.world;
     for (int j = 0; j < cm.world; j++) r.peer_emb[j] = cm.peer_emb[j];
     RET(launch(h, "hot_rows_pull", [&] { k_hot_pull<<<h->num_sms * 4, 256, 0, h->stream>>>(r, cm.hot_tab, want, D); }));
@@ -193,15 +193,7 @@ int comm_check(ctr_handle* h) {
 int comm_ensure(ctr_handle* h, bool want_cache) {
     Comm& cm = h->comm;
     if (cm.published_gen != h->tab_gen) RET(comm_publish(h));
-    if (want_cache) {
-        const size_t need = (size_t)h->Bmax * (h->cfg.S + 1) * h->cfg.D;
-        if (cm.rows_cache_cap < need) {
-            if (cm.rows_cache) cudaFree(cm.rows_cache);
-            cm.rows_cache = nullptr; cm.rows_cache_cap = 0;
-            RET(dalloc(h, &cm.rows_cache, need, false));
-            cm.rows_cache_cap = need;
-        }
-    }
+    if (want_cache) RET(reserve(h, cm.rows_cache, (size_t)h->Bmax * (h->cfg.S + 1) * h->cfg.D, false));
     return CTR_OK;
 }
 
@@ -211,7 +203,7 @@ RowSrc comm_src(ctr_handle* h, const int* d_user, const int* d_item, const int* 
     r.world = cm.world; r.wmask = cm.world - 1; r.wshift = cm.wshift;
     r.ifeat_sharded = h->tab_sharded[CTR_TABLE_ITEM_FEAT] ? 1 : 0;
     for (int j = 0; j < cm.world; j++) { r.peer_emb[j] = cm.peer_emb[j]; r.peer_ifeat[j] = cm.peer_ifeat[j]; }
-    r.rows_cache = cache ? cm.rows_cache : nullptr;
+    r.rows_cache = cache ? cm.rows_cache.get() : nullptr;
     r.hot_k = cm.hot_k; r.hot_tab = cm.hot_tab;
     return r;
 }
@@ -222,7 +214,7 @@ RowSrc comm_src(ctr_handle* h, const int* d_user, const int* d_item, const int* 
 static int comm_max_i64(ctr_handle* h, int64_t* v) {
     Comm& cm = h->comm;
     if (!cm.ready) return set_err(h, CTR_ESTATE, "world=%d but ctr_comm_init was not called", cm.world);
-    if (!cm.d_xchg) CU(h, cudaMalloc(&cm.d_xchg, 256 * (size_t)(kMaxPeers + 1)));
+    if (!cm.d_xchg) RET(dalloc(h, cm.d_xchg, 256 * (size_t)(kMaxPeers + 1), false));
     CU(h, cudaMemcpyAsync(cm.d_xchg, v, sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
     NC(h, g_nccl.AllReduce(cm.d_xchg, cm.d_xchg, 1, kNcclInt64, kNcclMax, cm.nccl, h->stream));
     CU(h, cudaMemcpyAsync(v, cm.d_xchg, sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
@@ -312,7 +304,7 @@ static int comm_init(ctr_handle* h, const void* id, int32_t id_bytes) {
     if (cm.lsock < 0) return set_err(h, CTR_ECOMM, "cannot listen on the descriptor socket %s", name);
     timeval tv{60, 0};                                  // a rank that died must not hang the others in accept()
     setsockopt(cm.lsock, SOL_SOCKET, SO_RCVTIMEO, &tv, sizeof tv);
-    CU(h, cudaHostAlloc(&cm.h_err, sizeof(int), cudaHostAllocMapped));
+    CU(h, cm.h_err.alloc(1, cudaHostAllocMapped));
     *cm.h_err = 0;
     CU(h, cudaHostGetDevicePointer(&cm.d_err, cm.h_err, 0));
     cm.ready = true;
@@ -322,12 +314,9 @@ static int comm_init(ctr_handle* h, const void* id, int32_t id_bytes) {
 static void comm_destroy(ctr_handle* h) {
     Comm& cm = h->comm;
     comm_close_peers(h);
-    for (void* p : {(void*)cm.table_grad, (void*)cm.rows_cache, cm.d_xchg, (void*)cm.hot_tab, (void*)cm.hot_sum, (void*)cm.hot_acc}) if (p) cudaFree(p);
-    cm.hot_tab = cm.hot_sum = cm.hot_acc = nullptr; cm.hot_k = 0;
     vmm_free(&cm.arena_vmm);
+    cm.arena = nullptr;
     if (cm.lsock >= 0) { close(cm.lsock); cm.lsock = -1; }
-    if (cm.h_err) cudaFreeHost(cm.h_err);
-    cm.table_grad = nullptr; cm.rows_cache = nullptr; cm.arena = nullptr; cm.d_xchg = nullptr; cm.h_err = nullptr; cm.d_err = nullptr;
     if (cm.nccl && g_nccl.CommDestroy) g_nccl.CommDestroy(cm.nccl);
     cm.nccl = nullptr; cm.ready = false;
 }

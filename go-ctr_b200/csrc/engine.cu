@@ -29,6 +29,7 @@
 #include <condition_variable>
 #include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -110,47 +111,47 @@ struct ctr_handle {
     uint64_t tab_gen = 1;                 // bumped whenever an ITEM_* table is (re)allocated: peers must re-map it
 
     // learnables, padded storage: W0 [Kp,H0p] W1 [H0p,H1p] W2 [H1p] att [Sp]; grads / Adam moments alike
-    float *W[4] = {}, *G[4] = {}, *Mo[4] = {}, *Vo[4] = {};
-    float* Gflat = nullptr; size_t Gflat_n = 0;    // the four gradient tensors live in one buffer (one all-reduce, one memset)
+    DevBuf<float> W[4], Mo[4], Vo[4];
+    float* G[4] = {};                     // views into Gflat
+    DevBuf<float> Gflat; size_t Gflat_n = 0;       // the four gradient tensors live in one buffer (one all-reduce, one memset)
     size_t wsize[4] = {};
     uint32_t step = 0;                    // optimiser steps taken (Adam t = step+1; dropout stream = step*4+layer)
 
     // activations
-    float *X0 = nullptr, *H0d = nullptr, *H1d = nullptr, *P = nullptr, *Z = nullptr;
-    float *dZ1 = nullptr, *dZ0 = nullptr, *dX = nullptr;
-    float *dUb = nullptr, *dIt = nullptr;         // row-gradient buffers (deterministic / debug)
-    size_t dUb_cap = 0;
-    unsigned *keys = nullptr, *keys2 = nullptr, *pos = nullptr, *pos2 = nullptr;
-    void* sort_tmp = nullptr; size_t sort_tmp_bytes = 0; size_t keys_cap = 0;
-    double* d_cost = nullptr;
-    float* hot_acc = nullptr; int hot_rows = 0, hot_reps = 0;
-    float *emb_m = nullptr, *emb_v = nullptr;      // CTR_TABLE_ADAM: first / second moments of ITEM_EMB, same layout as the table
+    DevBuf<float> X0, H0d, H1d, P, Z;
+    DevBuf<float> dZ1, dZ0, dX;
+    DevBuf<float> dUb, dIt;               // row-gradient buffers (deterministic / debug)
+    DevBuf<unsigned> keys, keys2, pos, pos2;
+    DevBuf<unsigned char> sort_tmp;
+    DevBuf<double> d_cost;
+    DevBuf<float> hot_acc; int hot_rows = 0, hot_reps = 0;
+    DevBuf<float> emb_m, emb_v;           // CTR_TABLE_ADAM: first / second moments of ITEM_EMB, same layout as the table
     // staging for host-pointer entry points
-    int *s_user = nullptr, *s_item = nullptr, *s_hist = nullptr; float* s_label = nullptr;
+    DevBuf<int> s_user, s_item, s_hist; DevBuf<float> s_label;
     // epoch entry points (ctr_train_idx / ctr_train_keys): pinned host ring (filled by the copy pool from the caller's
     // pageable buffers) → device slots on a copy stream, overlapping the compute of the previous batch
     static constexpr int kPin = 3;
-    unsigned char* feed_pin[kPin] = {}; unsigned char* feed_dev[2] = {}; size_t feed_bytes = 0;
-    cudaEvent_t pin_free[kPin] = {};
-    CopyPool* pool = nullptr;
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
-    double* d_costs = nullptr; size_t d_costs_cap = 0;
+    PinnedBuf<unsigned char> feed_pin[kPin]; DevBuf<unsigned char> feed_dev[2]; size_t feed_bytes = 0;
+    Event pin_free[kPin];
+    std::unique_ptr<CopyPool> pool;
+    Stream copy_stream;
+    Event ev_copied[2], ev_consumed[2];
+    DevBuf<double> d_costs;
     // ctr_train_keys: resolved + compacted samples resident in HBM
-    int *kt_user = nullptr, *kt_item = nullptr; long long* kt_ts = nullptr; float* kt_label = nullptr; size_t kt_cap = 0;
-    int *kt_flag = nullptr, *kt_pos = nullptr; void* kt_scan_tmp = nullptr; size_t kt_scan_bytes = 0; size_t kt_chunk = 0;
-    unsigned long long* kt_count = nullptr;
+    DevBuf<int> kt_user, kt_item; DevBuf<long long> kt_ts; DevBuf<float> kt_label;
+    DevBuf<int> kt_flag, kt_pos; DevBuf<unsigned char> kt_scan_tmp;
+    DevBuf<unsigned long long> kt_count;
     static constexpr int kCnt = 8;                       // pinned ring of survivor counts read back chunk by chunk
-    unsigned long long* kt_count_host = nullptr; cudaEvent_t kt_counted[kCnt] = {};
+    PinnedBuf<unsigned long long> kt_count_host; Event kt_counted[kCnt];
     // history windows of batch b+1 are cut on their own stream while batch b trains (two buffers)
-    cudaStream_t win_stream = nullptr; int* kt_hist[2] = {}; cudaEvent_t kt_win[2] = {}, kt_used[2] = {};
+    Stream win_stream; DevBuf<int> kt_hist[2]; Event kt_win[2], kt_used[2];
     // dense-X residency
-    float* dXd = nullptr; float* dYd = nullptr; size_t dXd_cap = 0, dYd_cap = 0;
+    DevBuf<float> dXd, dYd;
 
     int64_t launches = 0;
     bool profiling = false;
     std::map<std::string, Prof> prof;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    Event ev0, ev1;
 
     // wgmma GEMM engine (umma_gemm.cuh): pre-split K-major weight operands + TMA descriptors
     struct Umma {
@@ -159,28 +160,27 @@ struct ctr_handle {
         int nch_h0 = 0, nch_h1 = 0, nch_dx = 0;                            // 32-column chunks of the H0p / H1p / dX-wide tiles
         int stages_h0 = 0, stages_h1 = 0, stages_dx = 0;
         int bn_dx = 0;
-        float *Wt0[2] = {}, *Wt1[2] = {}, *W1s[2] = {}, *W0s[2] = {};     // [hi, lo]
+        DevBuf<float> Wt0[2], Wt1[2], W1s[2], W0s[2];                       // [hi, lo]
         CUtensorMap mA_X0, mA_H0d, mA_dZ1, mA_dZ0;
         CUtensorMap mB_Wt0[2], mB_Wt1[2], mB_W1s[2], mB_W0s[2];
         CUtensorMap mK_X0, mK_H0d, mK_dZ0, mK_dZ1;      // {width, 32 samples} boxes over [batch, width] for the weight-gradient GEMMs
         int dw_stages0 = 0, dw_stages1 = 0;
     } um;
 
-    // device-side ubcache (ubcache.cuh); ub_cap_* are the allocated sizes
-    long long *ub_off = nullptr, *ub_ts = nullptr; int* ub_items = nullptr; int64_t ub_users = 0, ub_n = 0;
-    size_t ub_cap_off = 0, ub_cap_n = 0;
+    // device-side ubcache (ubcache.cuh)
+    DevBuf<long long> ub_off, ub_ts; DevBuf<int> ub_items; int64_t ub_users = 0, ub_n = 0;
     // the spare CSR an append / set writes before the two are swapped
-    long long *ubx_off = nullptr, *ubx_ts = nullptr; int* ubx_items = nullptr; size_t ubx_cap_off = 0, ubx_cap_n = 0;
+    DevBuf<long long> ubx_off, ubx_ts; DevBuf<int> ubx_items;
 
     // device id maps (idmap.cuh): [CTR_IDMAP_USER, CTR_IDMAP_ITEM]
-    unsigned long long* idm_keys[2] = {nullptr, nullptr}; int* idm_vals[2] = {nullptr, nullptr};
-    unsigned long long idm_cap[2] = {0, 0}; int64_t idm_n[2] = {0, 0};
-    long long *k_keys = nullptr, *k_host = nullptr; int* k_flags = nullptr;   // staging for ctr_batch_predict_keys (device, pinned host)
+    DevBuf<unsigned long long> idm_keys[2]; DevBuf<int> idm_vals[2];
+    int64_t idm_n[2] = {0, 0};              // the tables hold idm_keys[i].size() slots (a power of two)
+    DevBuf<long long> k_keys; PinnedBuf<unsigned char> k_host; DevBuf<int> k_flags;   // staging for ctr_batch_predict_keys (device, pinned host)
 
     // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search;
     // slot 4: ctr_recommend_topk; slot 5: ubcache append / set): no cudaMalloc on the serving path
     static constexpr int kScratch = 6;
-    void* scratch[kScratch] = {}; size_t scratch_cap[kScratch] = {};
+    DevBuf<unsigned char> scratch[kScratch];
 
     Comm comm;
 };
@@ -221,21 +221,23 @@ int launch(ctr_handle* h, const char* name, F&& f) {
     return CTR_OK;
 }
 
+// (re)allocates b for n elements (at least one), freeing its old allocation first; zeroed on the engine stream
 template <typename T>
-int dalloc(ctr_handle* h, T** p, size_t n, bool zero = true) {
-    CU(h, cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)));
-    if (zero) CU(h, cudaMemsetAsync(*p, 0, std::max<size_t>(n, 1) * sizeof(T), h->stream));
+int dalloc(ctr_handle* h, DevBuf<T>& b, size_t n, bool zero = true) {
+    CU(h, b.alloc(std::max<size_t>(n, 1)));
+    if (zero) CU(h, cudaMemsetAsync(b, 0, b.size() * sizeof(T), h->stream));
     return CTR_OK;
 }
+// grow-only: reallocates b (old allocation freed first) only when it holds fewer than n elements
+template <typename T>
+int reserve(ctr_handle* h, DevBuf<T>& b, size_t n, bool zero = true) {
+    return b.size() >= n ? CTR_OK : dalloc(h, b, n, zero);
+}
 
-// device scratch slot `i` with at least `bytes` (contents undefined); grows geometrically, freed with the handle
+// device scratch slot `i` with at least `bytes` (contents undefined); grows to exactly the request, freed with the handle
 int scratch_get(ctr_handle* h, int i, size_t bytes, void** out) {
-    if (h->scratch_cap[i] < bytes) {
-        if (h->scratch[i]) { cudaStreamSynchronize(h->stream); cudaFree(h->scratch[i]); h->scratch[i] = nullptr; h->scratch_cap[i] = 0; }
-        const size_t cap = std::max(bytes, h->scratch_cap[i] * 2);
-        CU(h, cudaMalloc(&h->scratch[i], cap));
-        h->scratch_cap[i] = cap;
-    }
+    if (h->scratch[i] && h->scratch[i].size() < bytes) cudaStreamSynchronize(h->stream);   // queued work may still read it
+    RET(reserve(h, h->scratch[i], bytes, false));
     *out = h->scratch[i];
     return CTR_OK;
 }
@@ -508,8 +510,11 @@ int umma_init(ctr_handle* h) {
     if (std::min({u.stages_h0, u.stages_h1, u.stages_dx}) < 2 || std::min(u.dw_stages0, u.dw_stages1) < 1)
         return set_err(h, CTR_EINVAL, "wgmma GEMM: tile does not fit shared memory");
     for (int i = 0; i < 2; i++) {
-        RET(dalloc(h, &u.Wt0[i], (size_t)h->H0p * h->Kp)); RET(dalloc(h, &u.Wt1[i], (size_t)h->H1p * h->H0p));
-        RET(dalloc(h, &u.W1s[i], (size_t)h->H0p * h->H1p)); RET(dalloc(h, &u.W0s[i], (size_t)u.bn_dx * h->H0p));
+        // allocated once per handle (the maps hold their addresses): a retry after a failed init keeps the live copies
+        if (!u.Wt0[i]) RET(dalloc(h, u.Wt0[i], (size_t)h->H0p * h->Kp));
+        if (!u.Wt1[i]) RET(dalloc(h, u.Wt1[i], (size_t)h->H1p * h->H0p));
+        if (!u.W1s[i]) RET(dalloc(h, u.W1s[i], (size_t)h->H0p * h->H1p));
+        if (!u.W0s[i]) RET(dalloc(h, u.W0s[i], (size_t)u.bn_dx * h->H0p));
         RET(make_map(h, &u.mB_Wt0[i], u.Wt0[i], h->H0p, h->Kp, h->Kp, 32 * u.nch_h0));
         RET(make_map(h, &u.mB_Wt1[i], u.Wt1[i], h->H1p, h->H0p, h->H0p, 32 * u.nch_h1));
         RET(make_map(h, &u.mB_W1s[i], u.W1s[i], h->H0p, h->H1p, h->H1p, 32 * u.nch_h0));
@@ -597,15 +602,8 @@ struct StepOpts {
 };
 
 int ensure_rowgrad_buffers(ctr_handle* h, int B) {
-    size_t need = (size_t)B * h->cfg.S * h->cfg.D;
-    if (h->dUb_cap >= need && h->dUb) return CTR_OK;
-    if (h->dUb) cudaFree(h->dUb);
-    if (h->dIt) cudaFree(h->dIt);
-    h->dUb = h->dIt = nullptr;
-    RET(dalloc(h, &h->dUb, need));
-    RET(dalloc(h, &h->dIt, (size_t)B * h->cfg.D));
-    h->dUb_cap = need;
-    return CTR_OK;
+    RET(reserve(h, h->dUb, (size_t)B * h->cfg.S * h->cfg.D));
+    return reserve(h, h->dIt, (size_t)B * h->cfg.D);
 }
 
 // Replica accumulators for the popular rows of ITEM_EMB (rows [0, hot_rows), see k_attn_bwd_vec).
@@ -618,41 +616,42 @@ int ensure_hot(ctr_handle* h) {
     if (want < 0) want = 0;
     want = (int)std::min<int64_t>(want, rows);
     if (h->hot_acc && h->hot_rows == want) return CTR_OK;
-    if (h->hot_acc) { cudaFree(h->hot_acc); h->hot_acc = nullptr; }
+    h->hot_acc.reset();
     h->hot_rows = want; h->hot_reps = 0;
     if (want == 0) return CTR_OK;
     const size_t row_bytes = (size_t)h->cfg.D * sizeof(float);
     int reps = (int)std::min<size_t>(32, std::max<size_t>(1, ((size_t)64 << 20) / ((size_t)want * row_bytes)));
     h->hot_reps = reps;
-    return dalloc(h, &h->hot_acc, (size_t)reps * want * h->cfg.D);
+    return dalloc(h, h->hot_acc, (size_t)reps * want * h->cfg.D);
 }
 
 // CTR_TABLE_ADAM: moments of the embedding rows (zero-initialised, like the solver's, model.go:88)
 int ensure_moments(ctr_handle* h) {
     if (h->emb_m) return CTR_OK;
     const size_t n = (size_t)std::max<int64_t>(h->tab_local_rows[CTR_TABLE_ITEM_EMB], 1) * h->tab_ld[CTR_TABLE_ITEM_EMB];
-    RET(dalloc(h, &h->emb_m, n)); RET(dalloc(h, &h->emb_v, n));
+    DevBuf<float> m, v;                  // both or neither
+    RET(dalloc(h, m, n)); RET(dalloc(h, v, n));
+    h->emb_m = std::move(m); h->emb_v = std::move(v);
     return CTR_OK;
 }
 
 int deterministic_table_update(ctr_handle* h, const RowSrc& r, int B, int adam_batch) {
     const int S = h->cfg.S, D = h->cfg.D;
     size_t n = (size_t)B * (S + 1);
-    if (h->keys_cap < n) {
-        for (void* p : {(void*)h->keys, (void*)h->keys2, (void*)h->pos, (void*)h->pos2, h->sort_tmp}) if (p) cudaFree(p);
-        h->keys = h->keys2 = h->pos = h->pos2 = nullptr; h->sort_tmp = nullptr;
-        RET(dalloc(h, &h->keys, n, false)); RET(dalloc(h, &h->keys2, n, false));
-        RET(dalloc(h, &h->pos, n, false)); RET(dalloc(h, &h->pos2, n, false));
+    if (!h->sort_tmp || h->keys.size() < n) {           // sort_tmp is allocated last: it exists only with the other four
+        h->sort_tmp.reset();
+        RET(dalloc(h, h->keys, n, false)); RET(dalloc(h, h->keys2, n, false));
+        RET(dalloc(h, h->pos, n, false)); RET(dalloc(h, h->pos2, n, false));
         size_t bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, bytes, h->keys, h->keys2, h->pos, h->pos2, (int)n, 0, 32, h->stream);
-        CU(h, cudaMalloc(&h->sort_tmp, bytes));
-        h->sort_tmp_bytes = bytes; h->keys_cap = n;
+        cub::DeviceRadixSort::SortPairs(nullptr, bytes, h->keys.get(), h->keys2.get(), h->pos.get(), h->pos2.get(), (int)n, 0, 32, h->stream);
+        RET(dalloc(h, h->sort_tmp, bytes, false));
     }
+    size_t bytes = h->sort_tmp.size();
     RET(launch(h, "scatter_keys", [&] {
         k_scatter_keys<<<std::min<int>((int)((n + 255) / 256), h->num_sms * 8), 256, 0, h->stream>>>(r.hist, r.item_row, S, B, r.nvalid, r.n_emb, h->keys, h->pos);
     }));
     RET(launch(h, "cub_radix_sort_pairs", [&] {
-        cub::DeviceRadixSort::SortPairs(h->sort_tmp, h->sort_tmp_bytes, h->keys, h->keys2, h->pos, h->pos2, (int)n, 0, 32, h->stream);
+        cub::DeviceRadixSort::SortPairs(h->sort_tmp, bytes, h->keys.get(), h->keys2.get(), h->pos.get(), h->pos2.get(), (int)n, 0, 32, h->stream);
     }));
     if (h->cfg.table_opt == CTR_TABLE_ADAM) {
         RET(ensure_moments(h));
@@ -705,7 +704,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
     {
         HeadArgs a{}; a.H1d = h->H1d; a.ldh = h->H1p; a.H1 = c.H1; a.H1p = h->H1p; a.w2 = h->W[2];
         a.y = bwd ? o.d_label : nullptr; a.B = B; a.nvalid = r.nvalid; a.drop_p = d1;
-        a.p = h->P; a.logit = h->Z; a.dZ1 = bwd ? h->dZ1 : nullptr; a.lddz = h->H1p; a.dW2 = h->G[2]; a.cost_sum = h->d_cost;
+        a.p = h->P; a.logit = h->Z; a.dZ1 = bwd ? h->dZ1.get() : nullptr; a.lddz = h->H1p; a.dW2 = h->G[2]; a.cost_sum = h->d_cost;
         // few, long-lived blocks: every block ends with H1 same-address atomics (dW2) and one on the cost — with one block per
         // 64 rows those serialised in L2 (~27 cycles each per address) and cost more than the 50 MB the kernel streams
         const int hgrid = std::max(1, std::min((B + 63) / 64, h->num_sms * 2));
@@ -756,7 +755,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
         if (adam_rows && o.peer) return set_err(h, CTR_ESTATE, "CTR_TABLE_ADAM is not available with row-sharded tables (use CTR_TABLE_SGD, or a replicated table)");
         const bool buffers = o.want_rows || (learn_rows && sorted_rows && !fused_only);
         if (buffers) RET(ensure_rowgrad_buffers(h, B));
-        BwdOut bo{}; bo.datt = h->G[3]; bo.dUb = buffers ? h->dUb : nullptr; bo.dIt = buffers ? h->dIt : nullptr;
+        BwdOut bo{}; bo.datt = h->G[3]; bo.dUb = buffers ? h->dUb.get() : nullptr; bo.dIt = buffers ? h->dIt.get() : nullptr;
         bo.sgd = (learn_rows && (c.table_opt == CTR_TABLE_SGD || fused_only)) ? 1 : 0;
         // what leaves the kernel: -lr/world * gradient (SGD: added straight into rows), or 1/world * gradient (Adam on a
         // replicated table: the all-reduced sum is the global-batch gradient the row solver consumes)
@@ -783,7 +782,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
     if (o.update) {
         const bool tg = o.table_grad && c.table_opt != CTR_TABLE_FROZEN;
         const bool ph = o.peer && c.table_opt != CTR_TABLE_FROZEN && h->comm.hot_k > 0;
-        if (o.comm || o.table_grad) RET(comm_allreduce_grads(h, tg ? o.table_grad : ph ? h->comm.hot_sum : nullptr, tg ? o.table_grad_n : ph ? (size_t)h->comm.hot_k * c.D : 0));
+        if (o.comm || o.table_grad) RET(comm_allreduce_grads(h, tg ? o.table_grad : ph ? h->comm.hot_sum.get() : nullptr, tg ? o.table_grad_n : ph ? (size_t)h->comm.hot_k * c.D : 0));
         if (ph)
             RET(launch(h, "hot_rows_apply", [&] {
                 k_apply_table_grad<<<h->num_sms * 8, 256, 0, h->stream>>>(h->comm.hot_tab, h->comm.hot_sum, (long)h->comm.hot_k * c.D / 4);
@@ -873,8 +872,8 @@ int table_alloc(ctr_handle* h, int which, int64_t nrows, int32_t width) {
     h->tab_sharded[which] = shard;
     if (which == CTR_TABLE_ITEM_EMB) {
         h->comm.replicate = h->comm.world > 1 && !shard;
-        if (h->hot_acc) { cudaFree(h->hot_acc); h->hot_acc = nullptr; h->hot_rows = 0; }
-        for (float** p : {&h->emb_m, &h->emb_v}) if (*p) { cudaFree(*p); *p = nullptr; }       // a new table starts a new solver state
+        if (h->hot_acc) { h->hot_acc.reset(); h->hot_rows = 0; }
+        h->emb_m.reset(); h->emb_v.reset();                       // a new table starts a new solver state
     }
     if (which != CTR_TABLE_USER_FEAT) h->tab_gen++;           // peers hold mappings of the old allocation
     return CTR_OK;
@@ -938,10 +937,10 @@ int dense_src(ctr_handle* h, const int32_t ranges[8], int32_t xcols, RowSrc* out
 
 int upload_dense(ctr_handle* h, const float* X, const float* Y, int64_t n, int32_t xcols) {
     size_t need = (size_t)n * xcols;
-    if (h->dXd_cap < need) { if (h->dXd) cudaFree(h->dXd); h->dXd = nullptr; CU(h, cudaMalloc(&h->dXd, need * sizeof(float))); h->dXd_cap = need; }
+    RET(reserve(h, h->dXd, need, false));
     CU(h, cudaMemcpyAsync(h->dXd, X, need * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     if (Y) {
-        if (h->dYd_cap < (size_t)n) { if (h->dYd) cudaFree(h->dYd); h->dYd = nullptr; CU(h, cudaMalloc(&h->dYd, (size_t)n * sizeof(float))); h->dYd_cap = (size_t)n; }
+        RET(reserve(h, h->dYd, (size_t)n, false));
         CU(h, cudaMemcpyAsync(h->dYd, Y, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     }
     return CTR_OK;
@@ -1194,17 +1193,10 @@ int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users
     // The spare may still be read by work enqueued before the last swap: on the engine stream that is ordered before
     // this call's kernels; the window stream of ctr_train_keys is drained here.
     if (h->win_stream) CU(h, cudaStreamSynchronize(h->win_stream));
-    if (h->ubx_cap_off < (size_t)new_users + 1) {
-        if (h->ubx_off) { CU(h, cudaFree(h->ubx_off)); h->ubx_off = nullptr; h->ubx_cap_off = 0; }
-        const size_t cap = (size_t)new_users + 1 + (size_t)new_users / 8;      // slack, so steady growth rarely reallocates
-        RET(dalloc(h, &h->ubx_off, cap, false)); h->ubx_cap_off = cap;
-    }
-    if (h->ubx_cap_n < (size_t)n_new) {
-        for (void* p : {(void*)h->ubx_ts, (void*)h->ubx_items}) if (p) CU(h, cudaFree(p));
-        h->ubx_ts = nullptr; h->ubx_items = nullptr; h->ubx_cap_n = 0;
-        const size_t cap = (size_t)n_new + (size_t)n_new / 8;
-        RET(dalloc(h, &h->ubx_ts, cap, false)); RET(dalloc(h, &h->ubx_items, cap, false)); h->ubx_cap_n = cap;
-    }
+    // 1/8 slack, so steady growth rarely reallocates
+    if (h->ubx_off.size() < (size_t)new_users + 1) RET(dalloc(h, h->ubx_off, (size_t)new_users + 1 + (size_t)new_users / 8, false));
+    if (h->ubx_ts.size() < (size_t)n_new) RET(dalloc(h, h->ubx_ts, (size_t)n_new + (size_t)n_new / 8, false));
+    if (h->ubx_items.size() < (size_t)n_new) RET(dalloc(h, h->ubx_items, (size_t)n_new + (size_t)n_new / 8, false));
     RET(launch(h, "ubcache_offsets", [&] {
         k_ub_offsets<<<(int)((new_users + kUbTile) / kUbTile), 256, 0, h->stream>>>(h->ub_off, U, n, ub.tuser, ub.T, ub.dcum, new_users, h->ubx_off);
     }));
@@ -1219,7 +1211,6 @@ int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users
         else k_ub_place_new<false><<<grid, 256, 0, h->stream>>>(h->ub_ts, ub.ob, ub.oe, ub.dcum, ub.T, ub.bb, ub.bcnt, ub.bts, ub.bit, h->ubx_ts, h->ubx_items);
     }));
     std::swap(h->ub_off, h->ubx_off); std::swap(h->ub_ts, h->ubx_ts); std::swap(h->ub_items, h->ubx_items);
-    std::swap(h->ub_cap_off, h->ubx_cap_off); std::swap(h->ub_cap_n, h->ubx_cap_n);
     h->ub_users = new_users; h->ub_n = n_new;
     return CTR_OK;
 }
@@ -1269,22 +1260,22 @@ int ctr_create(const ctr_config* cfg, ctr_handle** out) {
 #define RC(x) do { int r_ = (x); if (r_ != CTR_OK) { g_create_error = h->err; ctr_destroy(h); return r_; } } while (0)
     CUC(cudaSetDevice(h->dev));
     CUC(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true;
-    CUC(cudaEventCreate(&h->ev0)); CUC(cudaEventCreate(&h->ev1));
+    CUC(h->ev0.create(cudaEventDefault)); CUC(h->ev1.create(cudaEventDefault));
     h->in = c.uP + 2 * c.D + c.cF;                      // din.go:187
     h->Kp = round_up(h->in, 32); h->H0p = round_up(c.H0, 32); h->H1p = round_up(c.H1, 32); h->Sp = round_up(c.S, 4);
     h->lddx = round_up(2 * c.D, 4);
     h->Bmax = std::max(c.batch, c.pred_batch);
     h->wsize[0] = (size_t)h->Kp * h->H0p; h->wsize[1] = (size_t)h->H0p * h->H1p; h->wsize[2] = h->H1p; h->wsize[3] = h->Sp;
     h->Gflat_n = h->wsize[0] + h->wsize[1] + h->wsize[2] + h->wsize[3];
-    RC(dalloc(h, &h->Gflat, h->Gflat_n));
+    RC(dalloc(h, h->Gflat, h->Gflat_n));
     for (size_t i = 0, off = 0; i < 4; off += h->wsize[i], i++) h->G[i] = h->Gflat + off;
-    for (int i = 0; i < 4; i++) { RC(dalloc(h, &h->W[i], h->wsize[i])); RC(dalloc(h, &h->Mo[i], h->wsize[i])); RC(dalloc(h, &h->Vo[i], h->wsize[i])); }
+    for (int i = 0; i < 4; i++) { RC(dalloc(h, h->W[i], h->wsize[i])); RC(dalloc(h, h->Mo[i], h->wsize[i])); RC(dalloc(h, h->Vo[i], h->wsize[i])); }
     const size_t B = h->Bmax;
-    RC(dalloc(h, &h->X0, B * h->Kp)); RC(dalloc(h, &h->H0d, B * h->H0p)); RC(dalloc(h, &h->H1d, B * h->H1p));
-    RC(dalloc(h, &h->P, B)); RC(dalloc(h, &h->Z, B));
-    RC(dalloc(h, &h->dZ1, B * h->H1p)); RC(dalloc(h, &h->dZ0, B * h->H0p)); RC(dalloc(h, &h->dX, B * h->lddx));
-    RC(dalloc(h, &h->d_cost, 1));
-    RC(dalloc(h, &h->s_user, B)); RC(dalloc(h, &h->s_item, B)); RC(dalloc(h, &h->s_hist, B * c.S)); RC(dalloc(h, &h->s_label, B));
+    RC(dalloc(h, h->X0, B * h->Kp)); RC(dalloc(h, h->H0d, B * h->H0p)); RC(dalloc(h, h->H1d, B * h->H1p));
+    RC(dalloc(h, h->P, B)); RC(dalloc(h, h->Z, B));
+    RC(dalloc(h, h->dZ1, B * h->H1p)); RC(dalloc(h, h->dZ0, B * h->H0p)); RC(dalloc(h, h->dX, B * h->lddx));
+    RC(dalloc(h, h->d_cost, 1));
+    RC(dalloc(h, h->s_user, B)); RC(dalloc(h, h->s_item, B)); RC(dalloc(h, h->s_hist, B * c.S)); RC(dalloc(h, h->s_label, B));
     RC(ctr_init_weights(h, c.seed));
     CUC(cudaStreamSynchronize(h->stream));
 #undef CUC
@@ -1293,35 +1284,14 @@ int ctr_create(const ctr_config* cfg, ctr_handle** out) {
     return CTR_OK;
 }
 
+// the device buffers, events and library-created streams are members: they free themselves at `delete h`, with this
+// handle's device current
 void ctr_destroy(ctr_handle* h) {
     if (!h) return;
     cudaSetDevice(h->dev);
     if (h->stream) cudaStreamSynchronize(h->stream);
     comm_destroy(h);
     for (int i = 0; i < 3; i++) table_free(h, i);
-    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items, (void*)h->ubx_off, (void*)h->ubx_ts, (void*)h->ubx_items}) if (p) cudaFree(p);
-    for (void* p : {(void*)h->idm_keys[0], (void*)h->idm_keys[1], (void*)h->idm_vals[0], (void*)h->idm_vals[1], (void*)h->k_keys, (void*)h->k_flags}) if (p) cudaFree(p);
-    if (h->k_host) cudaFreeHost(h->k_host);
-    for (int i = 0; i < 2; i++) for (float* p : {h->um.Wt0[i], h->um.Wt1[i], h->um.W1s[i], h->um.W0s[i]}) if (p) cudaFree(p);
-    for (int i = 0; i < 4; i++) for (float* p : {h->W[i], h->Mo[i], h->Vo[i]}) if (p) cudaFree(p);
-    if (h->Gflat) cudaFree(h->Gflat);
-    for (void* p : {(void*)h->X0, (void*)h->H0d, (void*)h->H1d, (void*)h->P, (void*)h->Z, (void*)h->dZ1, (void*)h->dZ0, (void*)h->dX,
-                    (void*)h->dUb, (void*)h->dIt, (void*)h->keys, (void*)h->keys2, (void*)h->pos, (void*)h->pos2, h->sort_tmp,
-                    (void*)h->d_cost, (void*)h->s_user, (void*)h->s_item, (void*)h->s_hist, (void*)h->s_label, (void*)h->dXd, (void*)h->dYd, (void*)h->hot_acc, (void*)h->emb_m, (void*)h->emb_v})
-        if (p) cudaFree(p);
-    for (int i = 0; i < ctr_handle::kScratch; i++) if (h->scratch[i]) cudaFree(h->scratch[i]);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    for (int i = 0; i < 2; i++) { if (h->ev_copied[i]) cudaEventDestroy(h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy(h->ev_consumed[i]); }
-    for (void* p : {(void*)h->feed_dev[0], (void*)h->feed_dev[1], (void*)h->d_costs, (void*)h->kt_user, (void*)h->kt_item, (void*)h->kt_ts, (void*)h->kt_label,
-                    (void*)h->kt_flag, (void*)h->kt_pos, h->kt_scan_tmp, (void*)h->kt_count}) if (p) cudaFree(p);
-    for (int i = 0; i < ctr_handle::kPin; i++) { if (h->feed_pin[i]) cudaFreeHost(h->feed_pin[i]); if (h->pin_free[i]) cudaEventDestroy(h->pin_free[i]); }
-    if (h->kt_count_host) cudaFreeHost(h->kt_count_host);
-    for (int i = 0; i < 2; i++) { if (h->kt_hist[i]) cudaFree(h->kt_hist[i]); if (h->kt_win[i]) cudaEventDestroy(h->kt_win[i]); if (h->kt_used[i]) cudaEventDestroy(h->kt_used[i]); }
-    if (h->win_stream) cudaStreamDestroy(h->win_stream);
-    for (int i = 0; i < ctr_handle::kCnt; i++) if (h->kt_counted[i]) cudaEventDestroy(h->kt_counted[i]);
-    delete h->pool; h->pool = nullptr;
-    if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -1507,11 +1477,7 @@ int train_opts(ctr_handle* h, const float* d_label, int B, StepOpts* out) {
     if (h->comm.world > 1) {
         Comm& cm = h->comm;
         const size_t n = (size_t)h->tab_rows[CTR_TABLE_ITEM_EMB] * h->tab_ld[CTR_TABLE_ITEM_EMB];
-        if (cm.table_grad_n != n) {
-            if (cm.table_grad) cudaFree(cm.table_grad);
-            cm.table_grad = nullptr; cm.table_grad_n = 0;
-            RET(dalloc(h, &cm.table_grad, n)); cm.table_grad_n = n;
-        }
+        if (cm.table_grad.size() != n) RET(dalloc(h, cm.table_grad, n));        // reallocated on any size change
         o.table_grad = cm.table_grad; o.table_grad_n = n; o.grad_scale = 1.0f / (float)cm.world; o.adam_batch = B * cm.world;
     }
     *out = o;
@@ -1553,28 +1519,29 @@ int ctr_train_step_idx(ctr_handle* h, const int32_t* user_row, const int32_t* it
 }
 
 namespace {
-// lazily creates the pinned ring, the two device slots and the copy stream; slot size fits one idx batch
+// lazily creates the pinned ring, the two device slots and the copy stream; slot size fits one idx batch.  Built
+// into locals and moved into the handle once all of it exists.
 int feed_init(ctr_handle* h) {
     if (h->copy_stream) return CTR_OK;
     const size_t B = (size_t)h->Bmax;
-    h->feed_bytes = (B * (size_t)(h->cfg.S + 3) * 4 + 255) & ~(size_t)255;      // [user | item | hist | label] — also fits [uid | iid | ts | label] chunks
-    h->feed_bytes = std::max(h->feed_bytes, (size_t)B * 28 + 256);
-    CU(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+    size_t bytes = (B * (size_t)(h->cfg.S + 3) * 4 + 255) & ~(size_t)255;      // [user | item | hist | label] — also fits [uid | iid | ts | label] chunks
+    bytes = std::max(bytes, (size_t)B * 28 + 256);
+    Stream copy; Event copied[2], consumed[2], pin_free[ctr_handle::kPin];
+    DevBuf<unsigned char> dev[2]; PinnedBuf<unsigned char> pin[ctr_handle::kPin];
+    CU(h, copy.create());
     for (int i = 0; i < 2; i++) {
-        CU(h, cudaEventCreateWithFlags(&h->ev_copied[i], cudaEventDisableTiming)); CU(h, cudaEventCreateWithFlags(&h->ev_consumed[i], cudaEventDisableTiming));
-        CU(h, cudaMalloc(&h->feed_dev[i], h->feed_bytes));
+        CU(h, copied[i].create(cudaEventDisableTiming)); CU(h, consumed[i].create(cudaEventDisableTiming));
+        CU(h, dev[i].alloc(bytes));
     }
     for (int i = 0; i < ctr_handle::kPin; i++) {
-        CU(h, cudaHostAlloc(&h->feed_pin[i], h->feed_bytes, cudaHostAllocDefault));
-        CU(h, cudaEventCreateWithFlags(&h->pin_free[i], cudaEventDisableTiming));
+        CU(h, pin[i].alloc(bytes));
+        CU(h, pin_free[i].create(cudaEventDisableTiming));
     }
-    h->pool = new CopyPool(7);          // 7 workers + the caller: 8 memcpy streams, so a 14 MB batch is staged in parallel with the step
-    return CTR_OK;
-}
-int costs_reserve(ctr_handle* h, size_t nb) {
-    if (h->d_costs_cap >= nb) return CTR_OK;
-    if (h->d_costs) cudaFree(h->d_costs);
-    h->d_costs = nullptr; RET(dalloc(h, &h->d_costs, nb)); h->d_costs_cap = nb;
+    for (int i = 0; i < 2; i++) { h->ev_copied[i] = std::move(copied[i]); h->ev_consumed[i] = std::move(consumed[i]); h->feed_dev[i] = std::move(dev[i]); }
+    for (int i = 0; i < ctr_handle::kPin; i++) { h->feed_pin[i] = std::move(pin[i]); h->pin_free[i] = std::move(pin_free[i]); }
+    h->feed_bytes = bytes;
+    h->pool = std::make_unique<CopyPool>(7);          // 7 workers + the caller: 8 memcpy streams, so a 14 MB batch is staged in parallel with the step
+    h->copy_stream = std::move(copy);
     return CTR_OK;
 }
 }  // namespace
@@ -1588,7 +1555,7 @@ int ctr_train_idx(ctr_handle* h, const int32_t* user_row, const int32_t* item_ro
     const int B = h->cfg.batch, S = h->cfg.S;
     const int64_t nb = (n + B - 1) / B;                      // model.go:96-99
     RET(feed_init(h));
-    RET(costs_reserve(h, (size_t)nb));
+    RET(reserve(h, h->d_costs, (size_t)nb));
     const size_t o_item = (size_t)B * 4, o_hist = (size_t)B * 8, o_label = (size_t)B * (S + 2) * 4;
     CU(h, cudaStreamSynchronize(h->stream));                 // a device slot may still be in use by an earlier call
     for (int64_t b = 0; b < nb; b++) {
@@ -1636,38 +1603,38 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
     RET(feed_init(h));
     // ---- resident sample arrays (+B slack so a padded tail never indexes past the end)
     const size_t cap = (size_t)n + (size_t)B;
-    if (h->kt_cap < cap) {
-        for (void* p : {(void*)h->kt_user, (void*)h->kt_item, (void*)h->kt_ts, (void*)h->kt_label}) if (p) cudaFree(p);
-        h->kt_user = h->kt_item = nullptr; h->kt_ts = nullptr; h->kt_label = nullptr; h->kt_cap = 0;
-        RET(dalloc(h, &h->kt_user, cap)); RET(dalloc(h, &h->kt_item, cap)); RET(dalloc(h, &h->kt_ts, cap)); RET(dalloc(h, &h->kt_label, cap));
-        h->kt_cap = cap;
-    }
+    RET(reserve(h, h->kt_user, cap)); RET(reserve(h, h->kt_item, cap)); RET(reserve(h, h->kt_ts, cap)); RET(reserve(h, h->kt_label, cap));
     // One GPU: the first epoch STREAMS — small chunks, and the steps over the samples already resident are queued while
     // the host stages the next chunk (the survivor count of chunk c-1 comes back through a pinned ring).  Several ranks:
     // every step is collective, so the ranks first agree on the batch count (resolve everything, then train).
     const bool streaming = epochs > 0 && h->comm.world == 1;
     const size_t chunk = std::min<size_t>((size_t)n, streaming ? std::min<size_t>(h->feed_bytes / 28, (size_t)2 * B) : h->feed_bytes / 28);   // keys per staging slot
-    if (h->kt_chunk < chunk) {
-        for (void* p : {(void*)h->kt_flag, (void*)h->kt_pos, h->kt_scan_tmp}) if (p) cudaFree(p);
-        h->kt_flag = h->kt_pos = nullptr; h->kt_scan_tmp = nullptr;
-        RET(dalloc(h, &h->kt_flag, chunk + 1)); RET(dalloc(h, &h->kt_pos, chunk + 1));
-        cub::DeviceScan::ExclusiveSum(nullptr, h->kt_scan_bytes, h->kt_flag, h->kt_pos, (int)(chunk + 1), h->stream);
-        CU(h, cudaMalloc(&h->kt_scan_tmp, h->kt_scan_bytes));
-        h->kt_chunk = chunk;
+    if (!h->kt_scan_tmp || h->kt_flag.size() < chunk + 1) {     // kt_scan_tmp is allocated last: it exists only with the other two
+        h->kt_scan_tmp.reset();
+        RET(dalloc(h, h->kt_flag, chunk + 1)); RET(dalloc(h, h->kt_pos, chunk + 1));
+        size_t bytes = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, bytes, h->kt_flag.get(), h->kt_pos.get(), (int)(chunk + 1), h->stream);
+        RET(dalloc(h, h->kt_scan_tmp, bytes, false));
     }
-    if (!h->kt_count) RET(dalloc(h, &h->kt_count, 1));
-    if (!h->kt_count_host) {
-        CU(h, cudaHostAlloc(&h->kt_count_host, sizeof(unsigned long long) * ctr_handle::kCnt, cudaHostAllocDefault));
-        for (int i = 0; i < ctr_handle::kCnt; i++) CU(h, cudaEventCreateWithFlags(&h->kt_counted[i], cudaEventDisableTiming));
+    if (!h->kt_count) RET(dalloc(h, h->kt_count, 1));
+    if (!h->kt_count_host) {            // the count ring and its events, moved into the handle together
+        PinnedBuf<unsigned long long> ring; Event counted[ctr_handle::kCnt];
+        CU(h, ring.alloc(ctr_handle::kCnt));
+        for (int i = 0; i < ctr_handle::kCnt; i++) CU(h, counted[i].create(cudaEventDisableTiming));
+        for (int i = 0; i < ctr_handle::kCnt; i++) h->kt_counted[i] = std::move(counted[i]);
+        h->kt_count_host = std::move(ring);
     }
     CU(h, cudaMemsetAsync(h->kt_count, 0, sizeof(unsigned long long), h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
-    if (!h->win_stream) {
-        CU(h, cudaStreamCreateWithFlags(&h->win_stream, cudaStreamNonBlocking));
+    if (!h->win_stream) {               // the window stream, its two buffers and their events, moved in together
+        Stream ws; DevBuf<int> hist[2]; Event win[2], used[2];
+        CU(h, ws.create());
         for (int i = 0; i < 2; i++) {
-            RET(dalloc(h, &h->kt_hist[i], (size_t)h->Bmax * S, false));
-            CU(h, cudaEventCreateWithFlags(&h->kt_win[i], cudaEventDisableTiming)); CU(h, cudaEventCreateWithFlags(&h->kt_used[i], cudaEventDisableTiming));
+            RET(dalloc(h, hist[i], (size_t)h->Bmax * S, false));
+            CU(h, win[i].create(cudaEventDisableTiming)); CU(h, used[i].create(cudaEventDisableTiming));
         }
+        for (int i = 0; i < 2; i++) { h->kt_hist[i] = std::move(hist[i]); h->kt_win[i] = std::move(win[i]); h->kt_used[i] = std::move(used[i]); }
+        h->win_stream = std::move(ws);
     }
     // one step of model.Train's loop over the resident samples [b*B, b*B + B) of which `have` exist so far.  The batch's
     // history windows (GetUserBehavior at the sample's timestamp) are cut on the window stream into one of two buffers,
@@ -1709,15 +1676,15 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
         h->pool->copy(pin + m * 16, ts + start, m * 8); h->pool->copy(pin + m * 24, label + start, m * 4);
         CU(h, cudaMemcpyAsync(h->feed_dev[slot], pin, m * 28, cudaMemcpyHostToDevice, rs));     // after resolve(c-2), which read this slot (stream order)
         CU(h, cudaEventRecord(h->pin_free[ps], rs));
-        const long long* dk = (const long long*)h->feed_dev[slot];
+        const long long* dk = (const long long*)h->feed_dev[slot].get();
         const int grid = (int)std::max<size_t>(1, std::min<size_t>((m + 255) / 256, (size_t)h->num_sms * 8));
         RET(launch(h, "keys_rows", [&] {
-            k_keys_rows<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_cap[0] - 1, h->idm_keys[1], h->idm_vals[1], h->idm_cap[1] - 1,
+            k_keys_rows<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
                                              dk, dk + m, (long)m, h->kt_flag);
         }));
-        RET(launch(h, "cub_exclusive_scan", [&] { cub::DeviceScan::ExclusiveSum(h->kt_scan_tmp, h->kt_scan_bytes, h->kt_flag, h->kt_pos, (int)(m + 1), rs); }));
+        RET(launch(h, "cub_exclusive_scan", [&] { size_t tb = h->kt_scan_tmp.size(); cub::DeviceScan::ExclusiveSum(h->kt_scan_tmp, tb, h->kt_flag.get(), h->kt_pos.get(), (int)(m + 1), rs); }));
         RET(launch(h, "keys_compact", [&] {
-            k_keys_compact<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_cap[0] - 1, h->idm_keys[1], h->idm_vals[1], h->idm_cap[1] - 1,
+            k_keys_compact<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
                                                 dk, dk + m, dk + 2 * m, (const float*)(dk + 3 * m), (long)m, h->kt_flag, h->kt_pos, h->kt_count,
                                                 h->kt_user, h->kt_item, h->kt_ts, h->kt_label);
         }));
@@ -1867,10 +1834,8 @@ int ctr_ubcache_upload(ctr_handle* h, const int64_t* offsets, const int64_t* ts,
     if (offsets[0] != 0 || offsets[n_users] != n) return set_err(h, CTR_EINVAL, "ubcache offsets must run from 0 to n");
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
-    for (void* p : {(void*)h->ub_off, (void*)h->ub_ts, (void*)h->ub_items}) if (p) cudaFree(p);      // the spare (ubx_*) is kept
-    h->ub_off = h->ub_ts = nullptr; h->ub_items = nullptr; h->ub_cap_off = h->ub_cap_n = 0;
-    RET(dalloc(h, &h->ub_off, (size_t)n_users + 1, false)); RET(dalloc(h, &h->ub_ts, (size_t)n, false)); RET(dalloc(h, &h->ub_items, (size_t)n, false));
-    h->ub_cap_off = (size_t)n_users + 1; h->ub_cap_n = (size_t)n;
+    h->ub_off.reset(); h->ub_ts.reset(); h->ub_items.reset();      // all three freed first; the spare (ubx_*) is kept
+    RET(dalloc(h, h->ub_off, (size_t)n_users + 1, false)); RET(dalloc(h, h->ub_ts, (size_t)n, false)); RET(dalloc(h, h->ub_items, (size_t)n, false));
     CU(h, cudaMemcpyAsync(h->ub_off, offsets, sizeof(int64_t) * (size_t)(n_users + 1), cudaMemcpyHostToDevice, h->stream));
     if (n > 0) {
         CU(h, cudaMemcpyAsync(h->ub_ts, ts, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
@@ -1971,14 +1936,13 @@ int ctr_idmap_build(ctr_handle* h, int which, const int64_t* ids, int64_t n) {
     if (!h || !ids || which < 0 || which > 1 || n < 1 || n > 0x7fffffff) return set_err(h, CTR_EINVAL, "bad idmap arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
-    for (void* p : {(void*)h->idm_keys[which], (void*)h->idm_vals[which]}) if (p) cudaFree(p);
-    h->idm_keys[which] = nullptr; h->idm_vals[which] = nullptr; h->idm_n[which] = 0;
+    h->idm_keys[which].reset(); h->idm_vals[which].reset(); h->idm_n[which] = 0;
     unsigned long long cap = 64;
     while (cap < 2ull * (unsigned long long)n) cap <<= 1;                 // load factor <= 0.5
-    RET(dalloc(h, &h->idm_keys[which], (size_t)cap, false)); RET(dalloc(h, &h->idm_vals[which], (size_t)cap, false));
-    if (!h->k_flags) RET(dalloc(h, &h->k_flags, 1));
-    long long* d_ids = nullptr;
-    CU(h, cudaMalloc(&d_ids, sizeof(long long) * (size_t)n));
+    RET(dalloc(h, h->idm_keys[which], (size_t)cap, false)); RET(dalloc(h, h->idm_vals[which], (size_t)cap, false));
+    if (!h->k_flags) RET(dalloc(h, h->k_flags, 1));
+    DevBuf<long long> d_ids;
+    CU(h, d_ids.alloc((size_t)n));
     int flags = 0, rc = CTR_OK;
     cudaMemcpyAsync(d_ids, ids, sizeof(long long) * (size_t)n, cudaMemcpyHostToDevice, h->stream);
     cudaMemsetAsync(h->k_flags, 0, sizeof(int), h->stream);
@@ -1988,13 +1952,12 @@ int ctr_idmap_build(ctr_handle* h, int which, const int64_t* ids, int64_t n) {
     });
     if (rc == CTR_OK && (cudaMemcpyAsync(&flags, h->k_flags, sizeof(int), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
                          cudaStreamSynchronize(h->stream) != cudaSuccess)) rc = set_err(h, CTR_ECUDA, "idmap build: %s", cudaGetErrorString(cudaGetLastError()));
-    cudaFree(d_ids);
     RET(rc);
     if (flags) {
-        cudaFree(h->idm_keys[which]); cudaFree(h->idm_vals[which]); h->idm_keys[which] = nullptr; h->idm_vals[which] = nullptr;
+        h->idm_keys[which].reset(); h->idm_vals[which].reset();
         return set_err(h, CTR_EINVAL, flags & 2 ? "idmap: id INT64_MIN is reserved" : "idmap: duplicate ids");
     }
-    h->idm_cap[which] = cap; h->idm_n[which] = n;
+    h->idm_n[which] = n;
     return CTR_OK;
 }
 
@@ -2004,7 +1967,7 @@ int ctr_idmap_lookup_dev(ctr_handle* h, int which, const int64_t* d_ids, int64_t
     CU(h, cudaSetDevice(h->dev));
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, h->num_sms * 8));
     return launch(h, "idmap_lookup", [&] {
-        k_idmap_lookup<<<grid, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], h->idm_cap[which] - 1, (const long long*)d_ids, (long)n, d_rows);
+        k_idmap_lookup<<<grid, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, (const long long*)d_ids, (long)n, d_rows);
     });
 }
 
@@ -2030,11 +1993,13 @@ int ctr_batch_predict_keys(ctr_handle* h, const int64_t* user_ids, const int64_t
     CU(h, cudaSetDevice(h->dev));
     if (!h->idm_keys[0] || !h->idm_keys[1]) return set_err(h, CTR_ESTATE, "batch predict needs both id maps (ctr_idmap_build)");
     const int B = h->cfg.pred_batch, S = h->cfg.S;
-    if (!h->k_keys) {       // device + pinned staging: [user ids | item ids | ts] and {first user row}
-        RET(dalloc(h, &h->k_keys, (size_t)3 * B, false));
-        CU(h, cudaMallocHost(&h->k_host, sizeof(long long) * (size_t)3 * B + sizeof(float) * (size_t)B + 16));
+    if (!h->k_keys) {       // device + pinned staging: [user ids | item ids | ts] and {first user row}, moved in together
+        DevBuf<long long> keys; PinnedBuf<unsigned char> host;
+        RET(dalloc(h, keys, (size_t)3 * B, false));
+        CU(h, host.alloc(sizeof(long long) * (size_t)3 * B + sizeof(float) * (size_t)B + 16));
+        h->k_host = std::move(host); h->k_keys = std::move(keys);
     }
-    long long* hk = h->k_host;
+    long long* hk = (long long*)h->k_host.get();
     float* hs = (float*)(hk + (size_t)3 * B);
     int* hfirst = (int*)(hs + B);
     for (int64_t s = 0; s < n; s += B) {
@@ -2044,7 +2009,7 @@ int ctr_batch_predict_keys(ctr_handle* h, const int64_t* user_ids, const int64_t
         memcpy(hk + 2 * (size_t)nb, ts + s, sizeof(long long) * (size_t)nb);
         CU(h, cudaMemcpyAsync(h->k_keys, hk, sizeof(long long) * (size_t)3 * nb, cudaMemcpyHostToDevice, h->stream));
         RET(launch(h, "keys_resolve", [&] {
-            k_keys_resolve<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_cap[0] - 1, h->idm_keys[1], h->idm_vals[1], h->idm_cap[1] - 1,
+            k_keys_resolve<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
                                                                     h->ub_off, h->ub_ts, h->ub_items, (long)h->ub_users, h->k_keys, nb, S, h->s_user, h->s_item, h->s_hist);
         }));
         if (s == 0) CU(h, cudaMemcpyAsync(hfirst, h->s_user, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
@@ -2110,8 +2075,8 @@ int ctr_checkpoint_save(ctr_handle* h, const char* path) {
     CU(h, cudaStreamSynchronize(h->stream));
     FILE* f = fopen(path, "wb");
     if (!f) return set_err(h, CTR_EIO, "checkpoint: cannot open %s for writing", path);
-    float* bounce = nullptr;
-    if (cudaMallocHost(&bounce, kCkptChunk) != cudaSuccess) { fclose(f); return set_err(h, CTR_ENOMEM, "checkpoint bounce buffer"); }
+    PinnedBuf<float> bounce;
+    if (bounce.alloc(kCkptChunk / sizeof(float)) != cudaSuccess) { fclose(f); return set_err(h, CTR_ENOMEM, "checkpoint bounce buffer"); }
     const ctr_config& c = h->cfg;
     CkptHeader hd{};
     memcpy(hd.magic, "CTRB200", 8);
@@ -2122,14 +2087,13 @@ int ctr_checkpoint_save(ctr_handle* h, const char* path) {
     int rc = fwrite(&hd, sizeof hd, 1, f) == 1 ? CTR_OK : set_err(h, CTR_EIO, "checkpoint: short write");
     for (int i = 0; i < 4 && rc == CTR_OK; i++) {
         int64_t rows; int width; long ld; dense_shape(h, i, &rows, &width, &ld);
-        for (float* src : {h->W[i], h->Mo[i], h->Vo[i]}) if (rc == CTR_OK) rc = ckpt_write_2d(h, f, src, ld, rows, width, bounce);
+        for (float* src : {h->W[i].get(), h->Mo[i].get(), h->Vo[i].get()}) if (rc == CTR_OK) rc = ckpt_write_2d(h, f, src, ld, rows, width, bounce);
     }
     for (int t = 0; t < 3 && rc == CTR_OK; t++)
         if (h->tab[t]) rc = ckpt_write_2d(h, f, h->tab[t], h->tab_ld[t], h->tab_local_rows[t], h->tab_width[t], bounce);
     if (hd.has_moments)
-        for (float* src : {h->emb_m, h->emb_v})
+        for (float* src : {h->emb_m.get(), h->emb_v.get()})
             if (rc == CTR_OK) rc = ckpt_write_2d(h, f, src, h->tab_ld[CTR_TABLE_ITEM_EMB], h->tab_local_rows[CTR_TABLE_ITEM_EMB], h->tab_width[CTR_TABLE_ITEM_EMB], bounce);
-    cudaFreeHost(bounce);
     if (fclose(f) != 0 && rc == CTR_OK) rc = set_err(h, CTR_EIO, "checkpoint: close failed");
     return rc;
 }
@@ -2147,11 +2111,11 @@ int ctr_checkpoint_load(ctr_handle* h, const char* path) {
     else if (hd.model != c.model || hd.uP != c.uP || hd.S != c.S || hd.D != c.D || hd.cF != c.cF || hd.H0 != c.H0 || hd.H1 != c.H1)
         rc = set_err(h, CTR_EINVAL, "checkpoint: model dims differ from this handle");
     else if (hd.rank != h->comm.rank || hd.world != h->comm.world) rc = set_err(h, CTR_EINVAL, "checkpoint: written by rank %d/%d, this handle is %d/%d", hd.rank, hd.world, h->comm.rank, h->comm.world);
-    float* bounce = nullptr;
-    if (rc == CTR_OK && cudaMallocHost(&bounce, kCkptChunk) != cudaSuccess) rc = set_err(h, CTR_ENOMEM, "checkpoint bounce buffer");
+    PinnedBuf<float> bounce;
+    if (rc == CTR_OK && bounce.alloc(kCkptChunk / sizeof(float)) != cudaSuccess) rc = set_err(h, CTR_ENOMEM, "checkpoint bounce buffer");
     for (int i = 0; i < 4 && rc == CTR_OK; i++) {
         int64_t rows; int width; long ld; dense_shape(h, i, &rows, &width, &ld);
-        for (float* dst : {h->W[i], h->Mo[i], h->Vo[i]}) if (rc == CTR_OK) rc = ckpt_read_2d(h, f, dst, ld, rows, width, bounce);
+        for (float* dst : {h->W[i].get(), h->Mo[i].get(), h->Vo[i].get()}) if (rc == CTR_OK) rc = ckpt_read_2d(h, f, dst, ld, rows, width, bounce);
     }
     for (int t = 0; t < 3 && rc == CTR_OK; t++) {
         if (!hd.has_table[t]) continue;
@@ -2167,15 +2131,14 @@ int ctr_checkpoint_load(ctr_handle* h, const char* path) {
         if (t == CTR_TABLE_ITEM_EMB) h->comm.replicate = h->comm.world > 1 && hd.replicated == 1;
         if (t != CTR_TABLE_USER_FEAT) h->tab_gen++;
         rc = ckpt_read_2d(h, f, h->tab[t], ld, hd.tab_local_rows[t], hd.tab_width[t], bounce);
-        if (t == CTR_TABLE_ITEM_EMB && h->hot_acc) { cudaFree(h->hot_acc); h->hot_acc = nullptr; h->hot_rows = 0; }
+        if (t == CTR_TABLE_ITEM_EMB && h->hot_acc) { h->hot_acc.reset(); h->hot_rows = 0; }
     }
-    for (float** p : {&h->emb_m, &h->emb_v}) if (*p) { cudaFree(*p); *p = nullptr; }
+    h->emb_m.reset(); h->emb_v.reset();
     if (rc == CTR_OK && hd.has_moments) {
         rc = ensure_moments(h);
-        for (float* dst : {h->emb_m, h->emb_v})
+        for (float* dst : {h->emb_m.get(), h->emb_v.get()})
             if (rc == CTR_OK) rc = ckpt_read_2d(h, f, dst, h->tab_ld[CTR_TABLE_ITEM_EMB], h->tab_local_rows[CTR_TABLE_ITEM_EMB], h->tab_width[CTR_TABLE_ITEM_EMB], bounce);
     }
-    if (bounce) cudaFreeHost(bounce);
     fclose(f);
     if (rc == CTR_OK) { h->step = hd.step; h->um.dirty = true; cudaStreamSynchronize(h->stream); }
     return rc;
@@ -2373,9 +2336,9 @@ namespace {
 cudaError_t big_copy(void* dst, const void* src, size_t bytes, bool to_device, cudaStream_t st) {
     const size_t kChunk = (size_t)32 << 20;
     if (bytes < ((size_t)8 << 20)) { cudaError_t e = cudaMemcpyAsync(dst, src, bytes, to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost, st); return e != cudaSuccess ? e : cudaStreamSynchronize(st); }
-    unsigned char* pin[2] = {nullptr, nullptr}; cudaEvent_t ev[2] = {nullptr, nullptr};
+    PinnedBuf<unsigned char> pin[2]; Event ev[2];
     cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) { e = cudaHostAlloc(&pin[i], kChunk, cudaHostAllocDefault); if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming); }
+    for (int i = 0; i < 2 && e == cudaSuccess; i++) { e = pin[i].alloc(kChunk); if (e == cudaSuccess) e = ev[i].create(cudaEventDisableTiming); }
     if (e == cudaSuccess) {
         CopyPool pool(7);
         const size_t nchunks = (bytes + kChunk - 1) / kChunk;
@@ -2403,7 +2366,6 @@ cudaError_t big_copy(void* dst, const void* src, size_t bytes, bool to_device, c
             }
         }
     }
-    for (int i = 0; i < 2; i++) { if (pin[i]) cudaFreeHost(pin[i]); if (ev[i]) cudaEventDestroy(ev[i]); }
     return e;
 }
 
@@ -2426,198 +2388,184 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     const int world = dist ? dist->world : 1;
     const bool seq = c.reserved[0] == 1;
     if (seq && world > 1) return set_err(nullptr, CTR_EINVAL, "the sequential float64 mode is single-GPU");
-#define CI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = set_err(nullptr, CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); goto done; } } while (0)
-#define CN(call) do { int r_ = (call); if (r_ != 0) { rc = set_err(nullptr, CTR_ECOMM, "%s: %s", #call, g_nccl.GetErrorString(r_)); goto done; } } while (0)
-    int rc = CTR_OK;
-    int *d_tok = nullptr, *d_doc = nullptr, *d_pnode = nullptr, *d_sid = nullptr, *d_sid2 = nullptr, *d_parent = nullptr, *d_bad = nullptr;
-    unsigned long long *d_cnt64 = nullptr, *d_skey = nullptr, *d_skey2 = nullptr, *d_ctr = nullptr, *d_misc = nullptr;
-    unsigned char *d_keep = nullptr, *d_pcode = nullptr, *d_code = nullptr;
-    long long *d_poff = nullptr, *d_nval = nullptr; long* d_nd = nullptr;
-    double* d_z = nullptr; float *d_syn0 = nullptr, *d_syn1 = nullptr, *d_lr = nullptr, *d_nsc = nullptr, *d_wsc = nullptr;
-    void* d_tmp = nullptr; size_t tmp_bytes = 0;
-    cudaStream_t st = nullptr; cudaEvent_t e0 = nullptr, e1 = nullptr;
+#define CI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return set_err(nullptr, CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
+#define CN(call) do { int r_ = (call); if (r_ != 0) return set_err(nullptr, CTR_ECOMM, "%s: %s", #call, g_nccl.GetErrorString(r_)); } while (0)
+    // declared first, destroyed last: every buffer below is freed before the stream and the events
+    Stream st; Event e0, e1;
+    DevBuf<int> d_tok, d_doc, d_pnode, d_sid, d_sid2, d_parent, d_bad;
+    DevBuf<unsigned long long> d_cnt64, d_skey, d_skey2, d_ctr, d_misc;
+    DevBuf<unsigned char> d_keep, d_pcode, d_code, d_tmp;
+    DevBuf<long long> d_poff, d_nval; DevBuf<long> d_nd;
+    DevBuf<double> d_z; DevBuf<float> d_syn0, d_syn1, d_lr, d_nsc, d_wsc;
+    size_t tmp_bytes = 0;
     float ms_total = 0; int launches = 0; unsigned long long hc[3] = {0, 0, 0};
+    CI(cudaSetDevice(c.device));
+    cudaDeviceProp prop{}; CI(cudaGetDeviceProperties(&prop, c.device));
+    if (prop.major != 9) return set_err(nullptr, CTR_ENODEV, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
+    const int G = prop.multiProcessorCount * 8;
+    CI(st.create()); CI(e0.create(cudaEventDefault)); CI(e1.create(cudaEventDefault));
+    // ---- dictionary counts over the whole stream (dictionary.go:70-81), on the device
+    CI(d_tok.alloc((size_t)n)); CI(d_doc.alloc((size_t)n)); CI(d_keep.alloc((size_t)n));
+    CI(d_cnt64.alloc((size_t)V)); CI(d_bad.alloc(1)); CI(d_nd.alloc(1));
+    CI(d_misc.alloc(4));
+    CI(big_copy(d_tok, tokens, sizeof(int) * (size_t)n, true, st));
+    CI(cudaMemsetAsync(d_cnt64, 0, sizeof(unsigned long long) * (size_t)V, st)); CI(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+    k_i2v_count<<<G, 256, 0, st>>>(d_tok, (long)n, V, d_cnt64, d_bad); launches++;
+    unsigned long long n_global = (unsigned long long)n;
+    long nd_max_global = 0;
+    if (world > 1) {
+        CN(g_nccl.AllReduce(d_cnt64, d_cnt64, (size_t)V, kNcclUint64, kNcclSum, dist->nccl, st));
+        CI(cudaMemcpyAsync(d_misc, &n_global, sizeof n_global, cudaMemcpyHostToDevice, st));
+        CN(g_nccl.AllReduce(d_misc, d_misc, 1, kNcclUint64, kNcclSum, dist->nccl, st));
+        CI(cudaMemcpyAsync(&n_global, d_misc, sizeof n_global, cudaMemcpyDeviceToHost, st));
+    }
+    // ---- the training document: words rarer than MinCount are dropped (memory.go:53-62), order kept
+    k_i2v_keep<<<G, 256, 0, st>>>(d_tok, (long)n, d_cnt64, c.min_count, d_keep); launches++;
+    cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_tok.get(), d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st);
     {
-        CI(cudaSetDevice(c.device));
-        cudaDeviceProp prop{}; CI(cudaGetDeviceProperties(&prop, c.device));
-        if (prop.major != 9) { rc = set_err(nullptr, CTR_ENODEV, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor); goto done; }
-        const int G = prop.multiProcessorCount * 8;
-        CI(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); CI(cudaEventCreate(&e0)); CI(cudaEventCreate(&e1));
-        // ---- dictionary counts over the whole stream (dictionary.go:70-81), on the device
-        CI(cudaMalloc(&d_tok, sizeof(int) * (size_t)n)); CI(cudaMalloc(&d_doc, sizeof(int) * (size_t)n)); CI(cudaMalloc(&d_keep, (size_t)n));
-        CI(cudaMalloc(&d_cnt64, sizeof(unsigned long long) * (size_t)V)); CI(cudaMalloc(&d_bad, sizeof(int))); CI(cudaMalloc(&d_nd, sizeof(long)));
-        CI(cudaMalloc(&d_misc, 4 * sizeof(unsigned long long)));
-        CI(big_copy(d_tok, tokens, sizeof(int) * (size_t)n, true, st));
-        CI(cudaMemsetAsync(d_cnt64, 0, sizeof(unsigned long long) * (size_t)V, st)); CI(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-        k_i2v_count<<<G, 256, 0, st>>>(d_tok, (long)n, V, d_cnt64, d_bad); launches++;
-        unsigned long long n_global = (unsigned long long)n;
-        long nd_max_global = 0;
-        if (world > 1) {
-            CN(g_nccl.AllReduce(d_cnt64, d_cnt64, (size_t)V, kNcclUint64, kNcclSum, dist->nccl, st));
-            CI(cudaMemcpyAsync(d_misc, &n_global, sizeof n_global, cudaMemcpyHostToDevice, st));
-            CN(g_nccl.AllReduce(d_misc, d_misc, 1, kNcclUint64, kNcclSum, dist->nccl, st));
-            CI(cudaMemcpyAsync(&n_global, d_misc, sizeof n_global, cudaMemcpyDeviceToHost, st));
-        }
-        // ---- the training document: words rarer than MinCount are dropped (memory.go:53-62), order kept
-        k_i2v_keep<<<G, 256, 0, st>>>(d_tok, (long)n, d_cnt64, c.min_count, d_keep); launches++;
-        cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_tok, d_keep, d_doc, d_nd, (int)n, st);
-        {
-            size_t b2 = 0, b3 = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, b2, d_skey, d_skey2, d_sid, d_sid2, V, 0, 64, st);
-            cub::DeviceScan::ExclusiveSum(nullptr, b3, d_poff, d_poff, V + 1, st);
-            tmp_bytes = std::max(tmp_bytes, std::max(b2, b3));
-        }
-        CI(cudaMalloc(&d_tmp, tmp_bytes));
-        { size_t tb = tmp_bytes; cub::DeviceSelect::Flagged(d_tmp, tb, d_tok, d_keep, d_doc, d_nd, (int)n, st); launches++; }
-        long nd = 0; int bad = 0;
-        CI(cudaMemcpyAsync(&nd, d_nd, sizeof nd, cudaMemcpyDeviceToHost, st)); CI(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
-        CI(cudaStreamSynchronize(st));
-        if (bad) { rc = set_err(nullptr, CTR_EINVAL, "a token lies outside [0, vocab)"); goto done; }
-        nd_max_global = nd;
-        if (world > 1) {
-            unsigned long long v = (unsigned long long)nd;
-            CI(cudaMemcpyAsync(d_misc, &v, sizeof v, cudaMemcpyHostToDevice, st));
-            CN(g_nccl.AllReduce(d_misc, d_misc, 1, kNcclUint64, kNcclMax, dist->nccl, st));
-            CI(cudaMemcpyAsync(&v, d_misc, sizeof v, cudaMemcpyDeviceToHost, st)); CI(cudaStreamSynchronize(st));
-            nd_max_global = (long)v;
-        }
-        // concurrency: (centre, context) pairs in flight ~ vocabulary / 4, at most the whole machine
-        const int rpw = 32 / (D / 4);
-        const long max_warps = (long)prop.multiProcessorCount * 8 * 8;
-        const long warps = std::max<long>(1, std::min<long>(std::min<long>(max_warps, (std::max<long>(nd, 1) + 63) / 64), std::max<long>(1, (long)V / 4 / rpw)));
-        const int grid = (int)((warps + 7) / 8);
-        const double Ceff = (double)grid * 8 * rpw;
-        // ---- per-word tables + count-sorted leaves (stable: ties stay in id order, like the reference's sort)
-        CI(cudaMalloc(&d_z, sizeof(double) * (size_t)V)); CI(cudaMalloc(&d_wsc, sizeof(float) * (size_t)V));
-        CI(cudaMalloc(&d_skey, sizeof(unsigned long long) * (size_t)V)); CI(cudaMalloc(&d_skey2, sizeof(unsigned long long) * (size_t)V));
-        CI(cudaMalloc(&d_sid, sizeof(int) * (size_t)V)); CI(cudaMalloc(&d_sid2, sizeof(int) * (size_t)V));
-        k_i2v_word_tables<<<G, 256, 0, st>>>(d_cnt64, V, (double)c.subsample, Ceff, (double)n_global, d_z, d_wsc, d_skey, d_sid); launches++;
-        { size_t tb = tmp_bytes; cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_skey, d_skey2, d_sid, d_sid2, V, 0, 64, st); launches++; }
-        std::vector<int64_t> cnt((size_t)V); std::vector<int> leaves((size_t)V);
-        CI(cudaMemcpyAsync(cnt.data(), d_cnt64, sizeof(int64_t) * (size_t)V, cudaMemcpyDeviceToHost, st));
-        CI(cudaMemcpyAsync(leaves.data(), d_sid2, sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, st));
-        CI(cudaStreamSynchronize(st));
-        // ---- host: the Huffman merge (huffman.go:23-57), O(V)
-        std::vector<int> parent; std::vector<unsigned char> code; std::vector<long long> node_val;
-        const int n_inner = i2v_huffman_sorted(cnt.data(), leaves.data(), V, parent, code, node_val);
-        if (n_inner < 1) { rc = set_err(nullptr, CTR_EINVAL, "item2vec needs at least two distinct words in the stream"); goto done; }
-        // ---- paths (node.go:26-43) on the device
-        CI(cudaMalloc(&d_parent, sizeof(int) * parent.size())); CI(cudaMalloc(&d_code, code.size())); CI(cudaMalloc(&d_nval, sizeof(long long) * node_val.size()));
-        CI(cudaMalloc(&d_poff, sizeof(long long) * ((size_t)V + 1))); CI(cudaMalloc(&d_nsc, sizeof(float) * node_val.size()));
-        CI(cudaMemcpyAsync(d_parent, parent.data(), sizeof(int) * parent.size(), cudaMemcpyHostToDevice, st));
-        CI(cudaMemcpyAsync(d_code, code.data(), code.size(), cudaMemcpyHostToDevice, st));
-        CI(cudaMemcpyAsync(d_nval, node_val.data(), sizeof(long long) * node_val.size(), cudaMemcpyHostToDevice, st));
-        CI(cudaMemsetAsync(d_poff, 0, sizeof(long long) * ((size_t)V + 1), st));
-        k_i2v_paths<<<G, 256, 0, st>>>(d_parent, d_code, d_cnt64, V, c.max_depth, 0, d_poff, nullptr, nullptr); launches++;
-        { size_t tb = tmp_bytes; cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_poff, d_poff, V + 1, st); launches++; }
-        long long nsteps = 0;
-        CI(cudaMemcpyAsync(&nsteps, d_poff + V, sizeof nsteps, cudaMemcpyDeviceToHost, st)); CI(cudaStreamSynchronize(st));
-        CI(cudaMalloc(&d_pnode, sizeof(int) * (size_t)std::max<long long>(nsteps, 1))); CI(cudaMalloc(&d_pcode, (size_t)std::max<long long>(nsteps, 1)));
-        k_i2v_paths<<<G, 256, 0, st>>>(d_parent, d_code, d_cnt64, V, c.max_depth, 1, d_poff, d_pnode, d_pcode); launches++;
-        k_i2v_node_scale<<<G, 256, 0, st>>>(d_nval, V - 1, Ceff, (double)n_global, d_nsc); launches++;
-        CI(cudaMalloc(&d_ctr, 3 * sizeof(unsigned long long))); CI(cudaMemsetAsync(d_ctr, 0, 3 * sizeof(unsigned long long), st));
-        if (seq) {
-            // sequential float64 parity mode (item2vec.cuh): one warp, the reference's single-goroutine order
-            double *d64_0 = nullptr, *d64_1 = nullptr, *d_lut64 = nullptr; float* d_out32 = nullptr;
-            std::vector<double> lut64(1000);
-            for (int i = 0; i < 1000; i++) { double e = std::exp(((double)i / 1000.0 * 2.0 - 1.0) * 6.0); lut64[(size_t)i] = e / (e + 1.0); }   // sigmoid_table.go:28-45
-            cudaError_t e1_ = cudaMalloc(&d64_0, sizeof(double) * (size_t)V * D), e2_ = cudaMalloc(&d64_1, sizeof(double) * (size_t)std::max(V - 1, 1) * D),
-                        e3_ = cudaMalloc(&d_lut64, sizeof(double) * 1000), e4_ = cudaMalloc(&d_out32, sizeof(float) * (size_t)V * D);
-            if (e1_ != cudaSuccess || e2_ != cudaSuccess || e3_ != cudaSuccess || e4_ != cudaSuccess) rc = set_err(nullptr, CTR_ENOMEM, "item2vec float64 tables");
-            if (rc == CTR_OK) {
-                cudaMemcpyAsync(d_lut64, lut64.data(), sizeof(double) * 1000, cudaMemcpyHostToDevice, st);
-                cudaMemsetAsync(d64_1, 0, sizeof(double) * (size_t)std::max(V - 1, 1) * D, st);
-                k_i2v_init64<<<G, 256, 0, st>>>(d64_0, (long)V * D, D, c.seed); launches++;
-                I2vSeqArgs sa{}; sa.doc = d_doc; sa.nd = nd; sa.n_stream = (long)n; sa.z = d_z; sa.poff = d_poff; sa.pnode = d_pnode; sa.pcode = d_pcode;
-                sa.syn0 = d64_0; sa.syn1 = d64_1; sa.lut = d_lut64; sa.D = D; sa.W = W; sa.upd = c.update_lr_batch; sa.iters = c.iter;
-                sa.init_lr = (double)c.init_lr; sa.min_lr = (double)c.min_lr; sa.seed = c.seed; sa.counters = d_ctr;
-                cudaEventRecord(e0, st);
-                k_i2v_seq_f64<<<1, 32, 0, st>>>(sa); launches++;
-                cudaEventRecord(e1, st);
-                k_f64_to_f32_i2v<<<G, 256, 0, st>>>(d64_0, d_out32, (long)V * D); launches++;
-                cudaMemcpyAsync(emb_out, d_out32, sizeof(float) * (size_t)V * D, cudaMemcpyDeviceToHost, st);
-                cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st);
-                if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = set_err(nullptr, CTR_ECUDA, "item2vec sequential mode: %s", cudaGetErrorString(cudaGetLastError()));
-                else {
-                    cudaEventElapsedTime(&ms_total, e0, e1);
-                    if (stats) {
-                        stats->doc_len = nd; stats->trained_positions = (int64_t)hc[0]; stats->pairs = (int64_t)hc[1]; stats->node_visits = (int64_t)hc[2];
-                        stats->algorithmic_bytes = 2.0 * D * 8.0 * ((double)hc[1] + (double)hc[2]); stats->ms_device = ms_total; stats->launches = launches;
-                    }
-                }
-            }
-            for (void* p : {(void*)d64_0, (void*)d64_1, (void*)d_lut64, (void*)d_out32}) if (p) cudaFree(p);
-            goto done;
-        }
-        // ---- vector tables: syn0 = (U-0.5)/dim (word2vec.go:103-111), inner nodes zero (huffman.go:40)
-        std::vector<float> lut(1000);
-        for (int i = 0; i < 1000; i++) { double e = std::exp(((double)i / 1000.0 * 2.0 - 1.0) * 6.0); lut[(size_t)i] = (float)(e / (e + 1.0)); }
-        CI(cudaMemcpyToSymbolAsync(c_i2v_lut, lut.data(), sizeof(float) * 1000, 0, cudaMemcpyHostToDevice, st));
-        CI(cudaMalloc(&d_syn0, sizeof(float) * (size_t)V * D)); CI(cudaMalloc(&d_syn1, sizeof(float) * (size_t)(V - 1) * D));
-        CI(cudaMemsetAsync(d_syn1, 0, sizeof(float) * (size_t)(V - 1) * D, st));
-        k_i2v_init<<<G, 256, 0, st>>>(d_syn0, (long)V * D, D, c.seed); launches++;
-        const long nchunks = nd_max_global / c.update_lr_batch + 2;
-        CI(cudaMalloc(&d_lr, sizeof(float) * (size_t)nchunks));
-        std::vector<float> lr_tab((size_t)nchunks);
-        double lr = c.init_lr;                                                           // w.currentlr persists across iterations
-        // segments: one per iteration on a single GPU; every sync_every positions when replicas have to be averaged
-        const long seg = (world > 1 && dist->sync_every > 0) ? dist->sync_every : std::max<long>(nd_max_global, 1);
-        for (int it = 0; it < c.iter; it++) {
-            for (long k = 0; k < nchunks; k++) {                                         // observe(), word2vec.go:223-233 (positions of all ranks advance together)
-                lr_tab[(size_t)k] = (float)lr;
-                const double seen = (double)(k + 1) * c.update_lr_batch * world;
-                if ((double)(k + 1) * c.update_lr_batch <= (double)nd_max_global) lr = lr < (double)c.min_lr ? (double)c.min_lr : (double)c.init_lr * (1.0 - seen / (double)n_global);
-            }
-            CI(cudaMemcpyAsync(d_lr, lr_tab.data(), sizeof(float) * (size_t)nchunks, cudaMemcpyHostToDevice, st));
-            I2vArgs a{}; a.doc = d_doc; a.nd = nd; a.z = d_z; a.poff = d_poff; a.pnode = d_pnode; a.pcode = d_pcode; a.syn0 = d_syn0; a.syn1 = d_syn1;
-            a.D = D; a.W = W; a.lr_tab = d_lr; a.upd = c.update_lr_batch; a.seed = c.seed; a.iter = it; a.counters = d_ctr;
-            a.node_scale = d_nsc; a.word_scale = d_wsc;
-            a.hot_n = std::min(kI2vHot, n_inner); a.hot_base = n_inner - a.hot_n;      // the last nodes created = the top of the tree
-            const size_t sm = (size_t)std::max(a.hot_n, 1) * D * sizeof(float);
-            CI(cudaEventRecord(e0, st));
-            for (long p0 = 0; p0 < std::max<long>(nd_max_global, 1); p0 += seg) {
-                a.pos_begin = p0; a.pos_end = std::min<long>(nd, p0 + seg);
-                if (a.pos_end > a.pos_begin) {
-                    switch (D / 4) {
-                        case 1: k_i2v_skipgram_hs<1><<<grid, 256, sm, st>>>(a); break;   case 2: k_i2v_skipgram_hs<2><<<grid, 256, sm, st>>>(a); break;
-                        case 4: k_i2v_skipgram_hs<4><<<grid, 256, sm, st>>>(a); break;   case 8: k_i2v_skipgram_hs<8><<<grid, 256, sm, st>>>(a); break;
-                        case 16: k_i2v_skipgram_hs<16><<<grid, 256, sm, st>>>(a); break; default: k_i2v_skipgram_hs<32><<<grid, 256, sm, st>>>(a); break;
-                    }
-                    launches++;
-                }
-                if (world > 1) {      // model averaging: every replica continues from the mean of all replicas
-                    CN(g_nccl.GroupStart());
-                    CN(g_nccl.AllReduce(d_syn0, d_syn0, (size_t)V * D, kNcclFloat32, kNcclSum, dist->nccl, st));
-                    CN(g_nccl.AllReduce(d_syn1, d_syn1, (size_t)(V - 1) * D, kNcclFloat32, kNcclSum, dist->nccl, st));
-                    CN(g_nccl.GroupEnd());
-                    k_i2v_scale<<<G, 256, 0, st>>>(d_syn0, (long)V * D, 1.0f / (float)world);
-                    k_i2v_scale<<<G, 256, 0, st>>>(d_syn1, (long)(V - 1) * D, 1.0f / (float)world);
-                    launches += 3;
-                }
-            }
-            CI(cudaGetLastError());
-            CI(cudaEventRecord(e1, st)); CI(cudaStreamSynchronize(st));                   // lr_tab is reused by the next iteration
-            float ms = 0; CI(cudaEventElapsedTime(&ms, e0, e1)); ms_total += ms;
-        }
-        CI(cudaStreamSynchronize(st));
-        if (emb_out) CI(big_copy(emb_out, d_syn0, sizeof(float) * (size_t)V * D, false, st));
-        CI(cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
-        CI(cudaStreamSynchronize(st));
+        size_t b2 = 0, b3 = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, b2, d_skey.get(), d_skey2.get(), d_sid.get(), d_sid2.get(), V, 0, 64, st);
+        cub::DeviceScan::ExclusiveSum(nullptr, b3, d_poff.get(), d_poff.get(), V + 1, st);
+        tmp_bytes = std::max(tmp_bytes, std::max(b2, b3));
+    }
+    CI(d_tmp.alloc(tmp_bytes));
+    { size_t tb = tmp_bytes; cub::DeviceSelect::Flagged(d_tmp, tb, d_tok.get(), d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st); launches++; }
+    long nd = 0; int bad = 0;
+    CI(cudaMemcpyAsync(&nd, d_nd, sizeof nd, cudaMemcpyDeviceToHost, st)); CI(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+    CI(cudaStreamSynchronize(st));
+    if (bad) return set_err(nullptr, CTR_EINVAL, "a token lies outside [0, vocab)");
+    nd_max_global = nd;
+    if (world > 1) {
+        unsigned long long v = (unsigned long long)nd;
+        CI(cudaMemcpyAsync(d_misc, &v, sizeof v, cudaMemcpyHostToDevice, st));
+        CN(g_nccl.AllReduce(d_misc, d_misc, 1, kNcclUint64, kNcclMax, dist->nccl, st));
+        CI(cudaMemcpyAsync(&v, d_misc, sizeof v, cudaMemcpyDeviceToHost, st)); CI(cudaStreamSynchronize(st));
+        nd_max_global = (long)v;
+    }
+    // concurrency: (centre, context) pairs in flight ~ vocabulary / 4, at most the whole machine
+    const int rpw = 32 / (D / 4);
+    const long max_warps = (long)prop.multiProcessorCount * 8 * 8;
+    const long warps = std::max<long>(1, std::min<long>(std::min<long>(max_warps, (std::max<long>(nd, 1) + 63) / 64), std::max<long>(1, (long)V / 4 / rpw)));
+    const int grid = (int)((warps + 7) / 8);
+    const double Ceff = (double)grid * 8 * rpw;
+    // ---- per-word tables + count-sorted leaves (stable: ties stay in id order, like the reference's sort)
+    CI(d_z.alloc((size_t)V)); CI(d_wsc.alloc((size_t)V));
+    CI(d_skey.alloc((size_t)V)); CI(d_skey2.alloc((size_t)V));
+    CI(d_sid.alloc((size_t)V)); CI(d_sid2.alloc((size_t)V));
+    k_i2v_word_tables<<<G, 256, 0, st>>>(d_cnt64, V, (double)c.subsample, Ceff, (double)n_global, d_z, d_wsc, d_skey, d_sid); launches++;
+    { size_t tb = tmp_bytes; cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_skey.get(), d_skey2.get(), d_sid.get(), d_sid2.get(), V, 0, 64, st); launches++; }
+    std::vector<int64_t> cnt((size_t)V); std::vector<int> leaves((size_t)V);
+    CI(cudaMemcpyAsync(cnt.data(), d_cnt64, sizeof(int64_t) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    CI(cudaMemcpyAsync(leaves.data(), d_sid2, sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    CI(cudaStreamSynchronize(st));
+    // ---- host: the Huffman merge (huffman.go:23-57), O(V)
+    std::vector<int> parent; std::vector<unsigned char> code; std::vector<long long> node_val;
+    const int n_inner = i2v_huffman_sorted(cnt.data(), leaves.data(), V, parent, code, node_val);
+    if (n_inner < 1) return set_err(nullptr, CTR_EINVAL, "item2vec needs at least two distinct words in the stream");
+    // ---- paths (node.go:26-43) on the device
+    CI(d_parent.alloc(parent.size())); CI(d_code.alloc(code.size())); CI(d_nval.alloc(node_val.size()));
+    CI(d_poff.alloc((size_t)V + 1)); CI(d_nsc.alloc(node_val.size()));
+    CI(cudaMemcpyAsync(d_parent, parent.data(), sizeof(int) * parent.size(), cudaMemcpyHostToDevice, st));
+    CI(cudaMemcpyAsync(d_code, code.data(), code.size(), cudaMemcpyHostToDevice, st));
+    CI(cudaMemcpyAsync(d_nval, node_val.data(), sizeof(long long) * node_val.size(), cudaMemcpyHostToDevice, st));
+    CI(cudaMemsetAsync(d_poff, 0, sizeof(long long) * ((size_t)V + 1), st));
+    k_i2v_paths<<<G, 256, 0, st>>>(d_parent, d_code, d_cnt64, V, c.max_depth, 0, d_poff, nullptr, nullptr); launches++;
+    { size_t tb = tmp_bytes; cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_poff.get(), d_poff.get(), V + 1, st); launches++; }
+    long long nsteps = 0;
+    CI(cudaMemcpyAsync(&nsteps, d_poff + V, sizeof nsteps, cudaMemcpyDeviceToHost, st)); CI(cudaStreamSynchronize(st));
+    CI(d_pnode.alloc((size_t)std::max<long long>(nsteps, 1))); CI(d_pcode.alloc((size_t)std::max<long long>(nsteps, 1)));
+    k_i2v_paths<<<G, 256, 0, st>>>(d_parent, d_code, d_cnt64, V, c.max_depth, 1, d_poff, d_pnode, d_pcode); launches++;
+    k_i2v_node_scale<<<G, 256, 0, st>>>(d_nval, V - 1, Ceff, (double)n_global, d_nsc); launches++;
+    CI(d_ctr.alloc(3)); CI(cudaMemsetAsync(d_ctr, 0, 3 * sizeof(unsigned long long), st));
+    if (seq) {
+        // sequential float64 parity mode (item2vec.cuh): one warp, the reference's single-goroutine order
+        DevBuf<double> d64_0, d64_1, d_lut64; DevBuf<float> d_out32;
+        std::vector<double> lut64(1000);
+        for (int i = 0; i < 1000; i++) { double e = std::exp(((double)i / 1000.0 * 2.0 - 1.0) * 6.0); lut64[(size_t)i] = e / (e + 1.0); }   // sigmoid_table.go:28-45
+        cudaError_t e1_ = d64_0.alloc((size_t)V * D), e2_ = d64_1.alloc((size_t)std::max(V - 1, 1) * D),
+                    e3_ = d_lut64.alloc(1000), e4_ = d_out32.alloc((size_t)V * D);
+        if (e1_ != cudaSuccess || e2_ != cudaSuccess || e3_ != cudaSuccess || e4_ != cudaSuccess) return set_err(nullptr, CTR_ENOMEM, "item2vec float64 tables");
+        cudaMemcpyAsync(d_lut64, lut64.data(), sizeof(double) * 1000, cudaMemcpyHostToDevice, st);
+        cudaMemsetAsync(d64_1, 0, sizeof(double) * (size_t)std::max(V - 1, 1) * D, st);
+        k_i2v_init64<<<G, 256, 0, st>>>(d64_0, (long)V * D, D, c.seed); launches++;
+        I2vSeqArgs sa{}; sa.doc = d_doc; sa.nd = nd; sa.n_stream = (long)n; sa.z = d_z; sa.poff = d_poff; sa.pnode = d_pnode; sa.pcode = d_pcode;
+        sa.syn0 = d64_0; sa.syn1 = d64_1; sa.lut = d_lut64; sa.D = D; sa.W = W; sa.upd = c.update_lr_batch; sa.iters = c.iter;
+        sa.init_lr = (double)c.init_lr; sa.min_lr = (double)c.min_lr; sa.seed = c.seed; sa.counters = d_ctr;
+        cudaEventRecord(e0, st);
+        k_i2v_seq_f64<<<1, 32, 0, st>>>(sa); launches++;
+        cudaEventRecord(e1, st);
+        k_f64_to_f32_i2v<<<G, 256, 0, st>>>(d64_0, d_out32, (long)V * D); launches++;
+        cudaMemcpyAsync(emb_out, d_out32, sizeof(float) * (size_t)V * D, cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st);
+        if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return set_err(nullptr, CTR_ECUDA, "item2vec sequential mode: %s", cudaGetErrorString(cudaGetLastError()));
+        cudaEventElapsedTime(&ms_total, e0, e1);
         if (stats) {
             stats->doc_len = nd; stats->trained_positions = (int64_t)hc[0]; stats->pairs = (int64_t)hc[1]; stats->node_visits = (int64_t)hc[2];
-            stats->algorithmic_bytes = 2.0 * D * 4.0 * ((double)hc[1] + (double)hc[2]); stats->ms_device = ms_total; stats->launches = launches;
+            stats->algorithmic_bytes = 2.0 * D * 8.0 * ((double)hc[1] + (double)hc[2]); stats->ms_device = ms_total; stats->launches = launches;
         }
+        return CTR_OK;
     }
-done:
+    // ---- vector tables: syn0 = (U-0.5)/dim (word2vec.go:103-111), inner nodes zero (huffman.go:40)
+    std::vector<float> lut(1000);
+    for (int i = 0; i < 1000; i++) { double e = std::exp(((double)i / 1000.0 * 2.0 - 1.0) * 6.0); lut[(size_t)i] = (float)(e / (e + 1.0)); }
+    CI(cudaMemcpyToSymbolAsync(c_i2v_lut, lut.data(), sizeof(float) * 1000, 0, cudaMemcpyHostToDevice, st));
+    CI(d_syn0.alloc((size_t)V * D)); CI(d_syn1.alloc((size_t)(V - 1) * D));
+    CI(cudaMemsetAsync(d_syn1, 0, sizeof(float) * (size_t)(V - 1) * D, st));
+    k_i2v_init<<<G, 256, 0, st>>>(d_syn0, (long)V * D, D, c.seed); launches++;
+    const long nchunks = nd_max_global / c.update_lr_batch + 2;
+    CI(d_lr.alloc((size_t)nchunks));
+    std::vector<float> lr_tab((size_t)nchunks);
+    double lr = c.init_lr;                                                           // w.currentlr persists across iterations
+    // segments: one per iteration on a single GPU; every sync_every positions when replicas have to be averaged
+    const long seg = (world > 1 && dist->sync_every > 0) ? dist->sync_every : std::max<long>(nd_max_global, 1);
+    for (int it = 0; it < c.iter; it++) {
+        for (long k = 0; k < nchunks; k++) {                                         // observe(), word2vec.go:223-233 (positions of all ranks advance together)
+            lr_tab[(size_t)k] = (float)lr;
+            const double seen = (double)(k + 1) * c.update_lr_batch * world;
+            if ((double)(k + 1) * c.update_lr_batch <= (double)nd_max_global) lr = lr < (double)c.min_lr ? (double)c.min_lr : (double)c.init_lr * (1.0 - seen / (double)n_global);
+        }
+        CI(cudaMemcpyAsync(d_lr, lr_tab.data(), sizeof(float) * (size_t)nchunks, cudaMemcpyHostToDevice, st));
+        I2vArgs a{}; a.doc = d_doc; a.nd = nd; a.z = d_z; a.poff = d_poff; a.pnode = d_pnode; a.pcode = d_pcode; a.syn0 = d_syn0; a.syn1 = d_syn1;
+        a.D = D; a.W = W; a.lr_tab = d_lr; a.upd = c.update_lr_batch; a.seed = c.seed; a.iter = it; a.counters = d_ctr;
+        a.node_scale = d_nsc; a.word_scale = d_wsc;
+        a.hot_n = std::min(kI2vHot, n_inner); a.hot_base = n_inner - a.hot_n;      // the last nodes created = the top of the tree
+        const size_t sm = (size_t)std::max(a.hot_n, 1) * D * sizeof(float);
+        CI(cudaEventRecord(e0, st));
+        for (long p0 = 0; p0 < std::max<long>(nd_max_global, 1); p0 += seg) {
+            a.pos_begin = p0; a.pos_end = std::min<long>(nd, p0 + seg);
+            if (a.pos_end > a.pos_begin) {
+                switch (D / 4) {
+                    case 1: k_i2v_skipgram_hs<1><<<grid, 256, sm, st>>>(a); break;   case 2: k_i2v_skipgram_hs<2><<<grid, 256, sm, st>>>(a); break;
+                    case 4: k_i2v_skipgram_hs<4><<<grid, 256, sm, st>>>(a); break;   case 8: k_i2v_skipgram_hs<8><<<grid, 256, sm, st>>>(a); break;
+                    case 16: k_i2v_skipgram_hs<16><<<grid, 256, sm, st>>>(a); break; default: k_i2v_skipgram_hs<32><<<grid, 256, sm, st>>>(a); break;
+                }
+                launches++;
+            }
+            if (world > 1) {      // model averaging: every replica continues from the mean of all replicas
+                CN(g_nccl.GroupStart());
+                CN(g_nccl.AllReduce(d_syn0, d_syn0, (size_t)V * D, kNcclFloat32, kNcclSum, dist->nccl, st));
+                CN(g_nccl.AllReduce(d_syn1, d_syn1, (size_t)(V - 1) * D, kNcclFloat32, kNcclSum, dist->nccl, st));
+                CN(g_nccl.GroupEnd());
+                k_i2v_scale<<<G, 256, 0, st>>>(d_syn0, (long)V * D, 1.0f / (float)world);
+                k_i2v_scale<<<G, 256, 0, st>>>(d_syn1, (long)(V - 1) * D, 1.0f / (float)world);
+                launches += 3;
+            }
+        }
+        CI(cudaGetLastError());
+        CI(cudaEventRecord(e1, st)); CI(cudaStreamSynchronize(st));                   // lr_tab is reused by the next iteration
+        float ms = 0; CI(cudaEventElapsedTime(&ms, e0, e1)); ms_total += ms;
+    }
+    CI(cudaStreamSynchronize(st));
+    if (emb_out) CI(big_copy(emb_out, d_syn0, sizeof(float) * (size_t)V * D, false, st));
+    CI(cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
+    CI(cudaStreamSynchronize(st));
+    if (stats) {
+        stats->doc_len = nd; stats->trained_positions = (int64_t)hc[0]; stats->pairs = (int64_t)hc[1]; stats->node_visits = (int64_t)hc[2];
+        stats->algorithmic_bytes = 2.0 * D * 4.0 * ((double)hc[1] + (double)hc[2]); stats->ms_device = ms_total; stats->launches = launches;
+    }
 #undef CI
 #undef CN
-    for (void* p : {(void*)d_tok, (void*)d_doc, (void*)d_keep, (void*)d_cnt64, (void*)d_bad, (void*)d_nd, (void*)d_misc, (void*)d_z, (void*)d_wsc, (void*)d_skey, (void*)d_skey2,
-                    (void*)d_sid, (void*)d_sid2, (void*)d_parent, (void*)d_code, (void*)d_nval, (void*)d_poff, (void*)d_nsc, (void*)d_pnode, (void*)d_pcode, (void*)d_ctr,
-                    (void*)d_syn0, (void*)d_syn1, (void*)d_lr, d_tmp}) if (p) cudaFree(p);
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    if (st) cudaStreamDestroy(st);
-    return rc;
+    return CTR_OK;
 }
 }  // namespace
 
@@ -2650,14 +2598,13 @@ struct ctr_mlp {
     Mlp64Dims d{};
     long np = 0;
     int dev = 0, num_sms = 132;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     mutable std::string err;
     std::mutex mu;
-    double *params = nullptr, *grads = nullptr, *ms = nullptr, *vs = nullptr;     // sgd keeps its velocities in ms
-    double *act[kMlpMaxLayers] = {}, *del[kMlpMaxLayers] = {};       // [rows_cap, units[l]]
-    long rows_cap = 0;
-    double *X64 = nullptr; float* Y32 = nullptr; long* idx = nullptr; size_t x_cap = 0, y_cap = 0, idx_cap = 0;
-    double* scal = nullptr;                                           // [0] batch loss, [1] epoch accumulator
+    DevBuf<double> params, grads, ms, vs;                             // sgd keeps its velocities in ms
+    DevBuf<double> act[kMlpMaxLayers], del[kMlpMaxLayers];           // [rows, units[l]]
+    DevBuf<double> X64; DevBuf<float> Y32; DevBuf<long> idx;
+    DevBuf<double> scal;                                              // [0] batch loss, [1] epoch accumulator
     double adam_calls = 0;                                            // AdamOptimizer64.t
     double t = 0;                                                     // BaseMultilayerPerceptron64.t: samples since initialize (:412,814)
     bool fitted = false;
@@ -2671,25 +2618,22 @@ int mlp_err(const ctr_mlp* m, int code, const char* fmt, ...) {
 }
 #define MCU(m, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return mlp_err(m, e_ == cudaErrorMemoryAllocation ? CTR_ENOMEM : CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
 int mlp_grid(const ctr_mlp* m, long work) { return (int)std::max<long>(1, std::min<long>((work + 255) / 256, (long)m->num_sms * 8)); }
+// grow-only; every layer's pair is checked, so a failed growth is redone by the next call
 int mlp_rows(ctr_mlp* m, long rows) {
-    if (m->rows_cap >= rows) return CTR_OK;
     for (int l = 1; l < m->d.n_layers; l++) {
-        if (m->act[l]) cudaFree(m->act[l]);
-        if (m->del[l]) cudaFree(m->del[l]);
-        m->act[l] = m->del[l] = nullptr;
-        MCU(m, cudaMalloc(&m->act[l], sizeof(double) * (size_t)rows * m->d.units[l]));
-        MCU(m, cudaMalloc(&m->del[l], sizeof(double) * (size_t)rows * m->d.units[l]));
+        const size_t n = (size_t)rows * m->d.units[l];
+        if (m->act[l].size() < n) MCU(m, m->act[l].alloc(n));
+        if (m->del[l].size() < n) MCU(m, m->del[l].alloc(n));
     }
-    m->rows_cap = rows;
     return CTR_OK;
 }
 // f32 host matrix → f64 device matrix (mlp.go:47-52 / :17-29), through a bounded f32 staging buffer
 int mlp_upload_x(ctr_mlp* m, const float* X, int64_t n, int nin) {
     const size_t need = (size_t)n * nin;
-    if (m->x_cap < need) { if (m->X64) cudaFree(m->X64); m->X64 = nullptr; MCU(m, cudaMalloc(&m->X64, need * sizeof(double))); m->x_cap = need; }
+    if (m->X64.size() < need) MCU(m, m->X64.alloc(need));
     const size_t chunk = std::min<size_t>(need, (size_t)16 << 20);
-    float* st = nullptr;
-    MCU(m, cudaMalloc(&st, chunk * sizeof(float)));
+    DevBuf<float> st;
+    MCU(m, st.alloc(chunk));
     int rc = CTR_OK;
     for (size_t o = 0; o < need && rc == CTR_OK; o += chunk) {
         const size_t c = std::min(chunk, need - o);
@@ -2697,7 +2641,6 @@ int mlp_upload_x(ctr_mlp* m, const float* X, int64_t n, int nin) {
         k_f32_to_f64<<<mlp_grid(m, (long)c), 256, 0, m->stream>>>(st, m->X64 + o, (long)c);
         if (cudaStreamSynchronize(m->stream) != cudaSuccess) rc = mlp_err(m, CTR_ECUDA, "upload X: %s", cudaGetErrorString(cudaGetLastError()));
     }
-    cudaFree(st);
     return rc;
 }
 // forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads X64 through idx (may be null = identity) from row0
@@ -2705,7 +2648,7 @@ void mlp_forward(ctr_mlp* m, const long* idx, long row0, int rows) {
     const int L = m->d.n_layers, nin = m->d.units[0];
     for (int l = 0; l + 1 < L; l++)
         k_mlp64_layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, m->X64 + (idx ? 0 : row0 * nin), nin, idx,
-                                                                                      l == 0 ? nullptr : m->act[l], m->act[l + 1], rows);
+                                                                                      l == 0 ? nullptr : m->act[l].get(), m->act[l + 1], rows);
 }
 }  // namespace
 
@@ -2760,9 +2703,9 @@ int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ct
     long off = 0;
     for (int l = 0; l < c.n_layers; l++) { m->d.units[l] = c.units[l]; if (l + 1 < c.n_layers) { m->d.off[l] = off; off += (long)(1 + c.units[l]) * c.units[l + 1]; } }
     m->np = off;
-    bool ok = cudaSetDevice(m->dev) == cudaSuccess && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) == cudaSuccess;
-    for (double** p : {&m->params, &m->grads, &m->ms, &m->vs}) ok = ok && cudaMalloc(p, sizeof(double) * (size_t)m->np) == cudaSuccess && cudaMemset(*p, 0, sizeof(double) * (size_t)m->np) == cudaSuccess;
-    ok = ok && cudaMalloc(&m->scal, 2 * sizeof(double)) == cudaSuccess;
+    bool ok = cudaSetDevice(m->dev) == cudaSuccess && m->stream.create() == cudaSuccess;
+    for (DevBuf<double>* p : {&m->params, &m->grads, &m->ms, &m->vs}) ok = ok && p->alloc((size_t)m->np) == cudaSuccess && cudaMemset(*p, 0, sizeof(double) * (size_t)m->np) == cudaSuccess;
+    ok = ok && m->scal.alloc(2) == cudaSuccess;
     if (!ok) { mlp_err(nullptr, CTR_ECUDA, "ctr_mlp_create: %s", cudaGetErrorString(cudaGetLastError())); ctr_mlp_destroy(m); return CTR_ECUDA; }
     *out = m;
     return CTR_OK;
@@ -2772,10 +2715,7 @@ void ctr_mlp_destroy(ctr_mlp* m) {
     if (!m) return;
     cudaSetDevice(m->dev);
     if (m->stream) cudaStreamSynchronize(m->stream);
-    for (void* p : {(void*)m->params, (void*)m->grads, (void*)m->ms, (void*)m->vs, (void*)m->X64, (void*)m->Y32, (void*)m->idx, (void*)m->scal}) if (p) cudaFree(p);
-    for (int l = 0; l < kMlpMaxLayers; l++) { if (m->act[l]) cudaFree(m->act[l]); if (m->del[l]) cudaFree(m->del[l]); }
-    if (m->stream) cudaStreamDestroy(m->stream);
-    delete m;
+    delete m;                                         // the members free themselves, this device current
 }
 
 int ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np) {
@@ -2810,8 +2750,8 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
     long bs = c.batch;
     if (bs <= 0) bs = n < 200 ? n : 200; else if (bs > n) bs = n;                       // basemlp64.go:517-527
     RET(mlp_upload_x(m, X, n, nin));
-    if (m->y_cap < (size_t)n) { if (m->Y32) cudaFree(m->Y32); m->Y32 = nullptr; MCU(m, cudaMalloc(&m->Y32, sizeof(float) * (size_t)n)); m->y_cap = (size_t)n; }
-    if (m->idx_cap < (size_t)n) { if (m->idx) cudaFree(m->idx); m->idx = nullptr; MCU(m, cudaMalloc(&m->idx, sizeof(long) * (size_t)n)); m->idx_cap = (size_t)n; }
+    if (m->Y32.size() < (size_t)n) MCU(m, m->Y32.alloc((size_t)n));
+    if (m->idx.size() < (size_t)n) MCU(m, m->idx.alloc((size_t)n));
     MCU(m, cudaMemcpyAsync(m->Y32, Y, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
     RET(mlp_rows(m, bs));
     if (!c.warm_start || !m->fitted) {
@@ -2855,7 +2795,7 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
             k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], m->Y32, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
             for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
                 k_mlp64_grads<<<mlp_grid(m, (long)(m->d.units[l] + 1) * m->d.units[l + 1]), 256, 0, m->stream>>>(
-                    m->params, m->grads, m->d, l, m->X64, nin, bi, l == 0 ? nullptr : m->act[l], m->del[l + 1], rows, c.alpha);
+                    m->params, m->grads, m->d, l, m->X64, nin, bi, l == 0 ? nullptr : m->act[l].get(), m->del[l + 1], rows, c.alpha);
                 if (l >= 1) k_mlp64_delta<<<mlp_grid(m, (long)rows * m->d.units[l]), 256, 0, m->stream>>>(m->params, m->d, l, m->act[l], m->del[l + 1], m->del[l], rows);
             }
             if (sgd) {
@@ -2904,8 +2844,8 @@ int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float*
     RET(mlp_upload_x(m, X, n, nin));
     const long chunk = 8192;
     RET(mlp_rows(m, std::min<long>(chunk, n)));
-    float* d_out = nullptr;
-    MCU(m, cudaMalloc(&d_out, sizeof(float) * (size_t)std::min<long>(chunk, n)));
+    DevBuf<float> d_out;
+    MCU(m, d_out.alloc((size_t)std::min<long>(chunk, n)));
     int rc = CTR_OK;
     for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predictProbas :897-931: raw probabilities for the f64 class
         const int rows = (int)std::min<long>(chunk, n - r0);
@@ -2914,7 +2854,6 @@ int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float*
         if (cudaMemcpyAsync(out + r0, d_out, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, m->stream) != cudaSuccess ||
             cudaStreamSynchronize(m->stream) != cudaSuccess) rc = mlp_err(m, CTR_ECUDA, "predict: %s", cudaGetErrorString(cudaGetLastError()));
     }
-    cudaFree(d_out);
     return rc;
 }
 
