@@ -82,6 +82,42 @@ def ids_probing_from(rng, slots, cap, avoid=()):
     return out
 
 
+_M0, _M1, _M2 = 0x9E3779B97F4A7C15, 0xD1B54A32D192ED03, 0x632BE59BD9B4E019
+_M3, _M4 = np.uint64(0xBF58476D1CE4E5B9), np.uint64(0x94D049BB133111EB)
+
+
+def mix64(seed, stream, ctr):
+    """The engine's counter RNG (common.cuh mix64, oracle orc_mix64) over an array of uint64 counters."""
+    z = np.asarray(ctr, np.uint64) * np.uint64(_M1) + np.uint64((((seed << 32) | stream) * _M0 + _M2) % (1 << 64))
+    z ^= z >> np.uint64(30); z *= _M3
+    z ^= z >> np.uint64(27); z *= _M4
+    z ^= z >> np.uint64(31)
+    return z
+
+
+def fill_rows(rows, width, seed, stream, dist, scale):
+    """Rows of a table made by ctr_table_fill on one GPU (attn.cuh k_table_fill): element (row, c) draws
+    mix64(seed, stream = table index, row * width + c).  dist 0: U[0, 1) * scale as float32, bit for bit.  dist 1:
+    Box-Muller N(0, 1) * scale in float64 from the device's float32 u1, u2, with r = sqrt(-2 ln u1), which bounds the
+    error of the device's __logf (see fill_normal_tol)."""
+    ctr = np.asarray(rows, np.uint64)[:, None] * np.uint64(width) + np.arange(width, dtype=np.uint64)
+    z = mix64(seed, stream, ctr)
+    if dist == 0:
+        return (z >> np.uint64(40)).astype(np.float32) * np.float32(1.0 / 16777216.0) * np.float32(scale)
+    # the float32 arithmetic of the kernel: 16777217.0f rounds to 2^24, so u1 lies in (0, 1]
+    u1 = ((z >> np.uint64(40)).astype(np.float32) + np.float32(1.0)) * (np.float32(1.0) / np.float32(16777217.0))
+    u2 = ((z >> np.uint64(8)) & np.uint64(0xFFFFFF)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+    r = np.sqrt(-2.0 * np.log(u1.astype(np.float64)))
+    return r * np.cos((np.float32(6.2831853) * u2).astype(np.float64)) * scale, r
+
+
+def fill_normal_tol(r, scale):
+    """Bound on |device - fill_rows| for dist 1: 1e-5 * scale for the float32 rounding and __cosf, plus __logf's absolute
+    error (2^-21.41 on [0.5, 2]) carried through the square root, which grows as r -> 0 (u1 -> 1) and is at most
+    sqrt(2 * 2^-21.41)."""
+    return scale * (1e-5 + 4e-7 / np.maximum(r, 4e-4))
+
+
 def scaled_init(orc, ocfg, seed, s0=0.05, s1=0.05, s2=0.3):
     """N(0,1) init (din.go:187-191) scaled so sigmoids are not saturated and parity is informative."""
     W0, W1, W2, att = orc.init_weights(ocfg, seed)
