@@ -351,12 +351,16 @@ k_attn_fwd_idx(RowSrc r, Dims d, const float* __restrict__ att, float* __restric
 // Dynamic shared memory: user_smem_floats(S, D, Kp) floats.  Two blocks fewer per SM than the gather kernels (80
 // registers): the history comes from shared memory, so fewer loads need to be in flight, and the cosine gate at D >= 64
 // fits without spills.
+// PEER (row-sharded ITEM_EMB): the items are this rank's local rows i0 + b (r.emb is the shard, the hot rows written
+// back), global row (i0 + b)·world + rank; the history rows come through emb_src<PEER> (the hot-row replica, else the
+// owner's HBM over NVLink); the item's ITEM_FEAT row is its local row of a sharded ITEM_FEAT or its global row of a
+// replicated one, missing when the global row is not below n_ifeat.
 // -------------------------------------------------------------------------------------------------
 __host__ __device__ inline size_t user_smem_floats(int S, int D, int Kp) { return (size_t)S * D + (size_t)(kAttnThreads / 32) * Kp; }
 
-template <int LPR, int VPL, int MODEL>
+template <int LPR, int VPL, int MODEL, bool PEER>
 __global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks - 2)
-k_attn_fwd_user(RowSrc r, Dims d, const float* __restrict__ att, int user, const int* __restrict__ hist, int i0,
+k_attn_fwd_user(RowSrc r, Dims d, const float* __restrict__ att, int user, const int* __restrict__ hist, int i0, int rank,
                 float* __restrict__ X0, long ldx0, int Kp, int B) {
     extern __shared__ __align__(16) float smem[];
     constexpr int RPW = 32 / LPR, DD = 4 * LPR * VPL, NT = kAttnThreads;
@@ -368,7 +372,7 @@ k_attn_fwd_user(RowSrc r, Dims d, const float* __restrict__ att, int user, const
     for (int i = threadIdx.x; i < d.S * (DD / 4); i += NT) {
         const int s = i / (DD / 4), c = i - s * (DD / 4);
         const int idx = __ldg(hist + s);
-        s_hist[i] = row_ok(idx, r.n_emb) ? ldg4(r.emb + (long)idx * r.lde + 4 * c) : zero4();
+        s_hist[i] = !row_ok(idx, r.n_emb) ? zero4() : PEER ? ld4_peer(emb_src<PEER>(r, idx) + 4 * c) : ldg4(r.emb + (long)idx * r.lde + 4 * c);
     }
     const float* pu = row_ok(user, r.n_user) ? r.ufeat + (long)user * r.ldu : nullptr;
     for (int j = lane; j < d.uP; j += 32) row[j] = pu ? __ldg(pu + j) : 0.0f;
@@ -406,7 +410,11 @@ k_attn_fwd_user(RowSrc r, Dims d, const float* __restrict__ att, int user, const
                 p2[0] = v[q].x; p2[1] = v[q].y; p2[2] = v[q].z; p2[3] = v[q].w;
             }
         }
-        const float* pc = row_ok(item, r.n_ifeat) ? r.ifeat + (long)item * r.ldi : nullptr;
+        const float* pc;
+        if (PEER) {
+            const int gi = item * r.world + rank;
+            pc = row_ok(gi, r.n_ifeat) ? r.ifeat + (long)(r.ifeat_sharded ? item : gi) * r.ldi : nullptr;
+        } else pc = row_ok(item, r.n_ifeat) ? r.ifeat + (long)item * r.ldi : nullptr;
         for (int j = lane; j < d.cF; j += 32) row[d.uP + 2 * d.D + j] = pc ? __ldg(pc + j) : 0.0f;
         __syncwarp();
         float4* dst = reinterpret_cast<float4*>(X0 + (long)b * ldx0);
@@ -800,6 +808,15 @@ k_hot_writeback(float* __restrict__ shard, long lde, const float* __restrict__ h
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)hot_k * q4; i += (long)gridDim.x * blockDim.x) {
         const int row = (int)(i / q4), c = (int)(i % q4) * 4;
         if (row % world == rank) *reinterpret_cast<float4*>(shard + (long)(row / world) * lde + c) = *reinterpret_cast<const float4*>(hot_tab + (long)row * lde + c);
+    }
+}
+// sharded search by row: out[i] = ITEM_EMB row rows[i] (valid), widened to float64, for the vector instantiation of
+// k_knn_scan (knn.cuh)
+__global__ void __launch_bounds__(256)
+k_gather_rows_f64(RowSrc r, const int* __restrict__ rows, int n, int D, double* __restrict__ out) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)n * D; i += (long)gridDim.x * blockDim.x) {
+        const int q = (int)(i / D), c = (int)(i - (long)q * D);
+        out[i] = (double)emb_src<true>(r, __ldg(rows + q))[c];
     }
 }
 

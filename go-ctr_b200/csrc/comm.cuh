@@ -58,8 +58,22 @@ struct Comm {
     int hot_k = 0; DevBuf<float> hot_tab, hot_sum, hot_acc; int hot_reps = 0;
 };
 
+// the fixed header a collective serving call all-gathers first (comm_agree): the call's shape, a hash of every input
+// array, and this rank's validation verdict
+struct CommHdr {
+    int64_t n;                  // queries / users
+    int32_t k, mode, flag;      // mode: which inputs are given; flag: exclude_history
+    int32_t code;               // CTR_OK or this rank's error code ...
+    uint64_t hash[2];
+    int64_t plan;               // what fixes the number of list all-gathers (queries per chunk / users per group)
+    char msg[208];              // ... and its message
+};
+static_assert(sizeof(CommHdr) == 256, "one all-gather slot of Comm::d_xchg");
+
 }  // namespace ctr
 
+static int comm_agree(ctr_handle* h, ctr::CommHdr hd, int verdict);
+static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, size_t score_bytes, const int* send_r, int* recv_r, size_t n);
 static int comm_allreduce_grads(ctr_handle* h, float* extra, size_t extra_n);
 static int comm_train_step(ctr_handle* h, const int32_t* d_user, const int32_t* d_item, const int32_t* d_hist, const float* d_label, int32_t B, int32_t nvalid);
 static int comm_predict(ctr_handle* h, const int32_t* d_user, const int32_t* d_item, const int32_t* d_hist, int32_t B, float* d_out);

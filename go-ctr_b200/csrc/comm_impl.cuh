@@ -177,12 +177,18 @@ int comm_hot_writeback(ctr_handle* h) {
     });
 }
 
-int comm_check(ctr_handle* h) {
-    const ctr_config& c = h->cfg;
+// what search needs of a sharded handle: the communicator, a supported world and the ITEM_EMB shard
+int comm_check_emb(ctr_handle* h) {
     const Comm& cm = h->comm;
     if (!cm.ready) return set_err(h, CTR_ESTATE, "world=%d but ctr_comm_init was not called", cm.world);
     if (cm.world > kMaxPeers || (cm.world & (cm.world - 1))) return set_err(h, CTR_EINVAL, "row-sharded tables need world in {2, 4, 8} (one NVSwitch box), got %d", cm.world);
-    if (!h->tab[CTR_TABLE_ITEM_EMB] || h->tab_width[CTR_TABLE_ITEM_EMB] != c.D) return set_err(h, CTR_ESTATE, "ITEM_EMB shard not uploaded");
+    if (!h->tab[CTR_TABLE_ITEM_EMB] || h->tab_width[CTR_TABLE_ITEM_EMB] != h->cfg.D) return set_err(h, CTR_ESTATE, "ITEM_EMB shard not uploaded");
+    return CTR_OK;
+}
+
+int comm_check(ctr_handle* h) {
+    const ctr_config& c = h->cfg;
+    RET(comm_check_emb(h));
     if (c.uP > 0 && !h->tab[CTR_TABLE_USER_FEAT]) return set_err(h, CTR_ESTATE, "USER_FEAT not uploaded");
     if (c.cF > 0 && !h->tab[CTR_TABLE_ITEM_FEAT]) return set_err(h, CTR_ESTATE, "ITEM_FEAT not uploaded");
     if (!attn_idx_shape_ok(h, true))
@@ -219,6 +225,65 @@ static int comm_max_i64(ctr_handle* h, int64_t* v) {
     NC(h, g_nccl.AllReduce(cm.d_xchg, cm.d_xchg, 1, kNcclInt64, kNcclMax, cm.nccl, h->stream));
     CU(h, cudaMemcpyAsync(v, cm.d_xchg, sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
+    return CTR_OK;
+}
+
+// 64-bit hash of a caller array (FNV-1a over 8-byte words), for comparing the ranks' arguments of a collective call
+static uint64_t comm_hash(const void* p, size_t bytes) {
+    const unsigned char* b = (const unsigned char*)p;
+    uint64_t hs = 1469598103934665603ull;
+    for (size_t i = 0; i < bytes; i += 8) {
+        uint64_t w = 0;
+        memcpy(&w, b + i, std::min<size_t>(8, bytes - i));
+        hs = (hs ^ w) * 1099511628211ull;
+        hs ^= hs >> 29;
+    }
+    return hs;
+}
+
+// Argument agreement of a collective call (search / recommendation on a row-sharded ITEM_EMB).  Every rank all-gathers
+// its header and its own validation verdict (code, message) before doing anything else, so a rank never leaves the
+// others blocked in NCCL: headers that differ give CTR_EINVAL everywhere, else the verdict of the lowest failing rank,
+// else CTR_EINVAL if the ranks' plans differ (hd.plan is read only when every rank is valid).  A failure after the
+// agreement (out of memory for scratch, a failed publish) still leaves the peers waiting, as in the sharded train step.
+static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
+    Comm& cm = h->comm;
+    if (!cm.ready) return set_err(h, CTR_ESTATE, "world=%d but ctr_comm_init was not called", cm.world);
+    hd.code = verdict;
+    if (verdict != CTR_OK) snprintf(hd.msg, sizeof hd.msg, "%s", h->err.c_str());
+    if (!cm.d_xchg) RET(dalloc(h, cm.d_xchg, 256 * (size_t)(kMaxPeers + 1), false));
+    const int W = cm.world;
+    std::vector<CommHdr> all((size_t)W);
+    CommHdr* d_send = (CommHdr*)cm.d_xchg.get();
+    CU(h, cudaMemcpyAsync(d_send, &hd, sizeof hd, cudaMemcpyHostToDevice, h->stream));
+    NC(h, g_nccl.AllGather(d_send, d_send + 1, sizeof(CommHdr), kNcclChar, cm.nccl, h->stream));
+    CU(h, cudaMemcpyAsync(all.data(), d_send + 1, sizeof(CommHdr) * (size_t)W, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    for (int j = 1; j < W; j++) {
+        const CommHdr& a = all[0]; const CommHdr& b = all[(size_t)j];
+        if (a.n != b.n || a.k != b.k || a.mode != b.mode || a.flag != b.flag || a.hash[0] != b.hash[0] || a.hash[1] != b.hash[1])
+            return set_err(h, CTR_EINVAL, "ranks disagree on the arguments of this collective call: rank %d (n %lld, k %d) differs from rank 0 (n %lld, k %d) — every rank must pass the same arguments",
+                           j, (long long)b.n, b.k, (long long)a.n, a.k);
+    }
+    for (int j = 0; j < W; j++)
+        if (all[(size_t)j].code != CTR_OK) return set_err(h, all[(size_t)j].code, "%s", all[(size_t)j].msg);
+    for (int j = 1; j < W; j++)          // every rank valid: their plans must give the same sequence of all-gathers
+        if (all[(size_t)j].plan != all[0].plan)
+            return set_err(h, CTR_EINVAL, "ranks disagree on the plan of this collective call: rank %d would exchange %lld entries per round, rank 0 %lld",
+                           j, (long long)all[(size_t)j].plan, (long long)all[0].plan);
+    return CTR_OK;
+}
+
+// The ranks' top-k lists, all-gathered on the engine stream (device buffers of the caller's scratch): send_s / send_r
+// hold n entries, recv_s / recv_r receive [world][n].  Every rank's reads of the table are queued before its send, so
+// the gather completes on a rank only after every rank has finished reading.
+static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, size_t score_bytes, const int* send_r, int* recv_r, size_t n) {
+    Comm& cm = h->comm;
+    NC(h, g_nccl.GroupStart());
+    NC(h, g_nccl.AllGather(send_s, recv_s, n * score_bytes, kNcclChar, cm.nccl, h->stream));
+    NC(h, g_nccl.AllGather(send_r, recv_r, n, kNcclInt32, cm.nccl, h->stream));
+    NC(h, g_nccl.GroupEnd());
+    h->launches += 1;
     return CTR_OK;
 }
 

@@ -351,32 +351,35 @@ size_t attn_user_smem(const ctr_handle* h) { return user_smem_floats(h->cfg.S, h
 bool attn_user_ok(const ctr_handle* h, size_t smem_optin) {
     return attn_lanes_ok(h->cfg.D) && h->tab_ld[CTR_TABLE_ITEM_EMB] % 4 == 0 && attn_user_smem(h) <= smem_optin;
 }
-// f(kernel) for the handle's model and D
+// f(kernel) for the handle's model and D; peer: the row-sharded instantiation (same lane map: the same arithmetic)
 template <typename F>
-void with_user_kernel(const ctr_handle* h, F&& f) {
+void with_user_kernel(const ctr_handle* h, bool peer, F&& f) {
     with_model(h->cfg.model, [&](auto m) {
         constexpr int M = decltype(m)::value;
-        with_lanes<false, false>(h->cfg.D, [&](auto l) { using L = decltype(l); f(k_attn_fwd_user<L::LPR, L::VPL, M>); });
+        with_lanes<false, false>(h->cfg.D, [&](auto l) {
+            using L = decltype(l);
+            if (peer) f(k_attn_fwd_user<L::LPR, L::VPL, M, true>); else f(k_attn_fwd_user<L::LPR, L::VPL, M, false>);
+        });
     });
 }
 // sets the kernel's dynamic shared-memory limit; returns its resident CTAs per SM
-int attn_user_prepare(const ctr_handle* h) {
+int attn_user_prepare(const ctr_handle* h, bool peer) {
     int occ = 1;
     const size_t smem = attn_user_smem(h);
-    with_user_kernel(h, [&](auto kern) {
+    with_user_kernel(h, peer, [&](auto kern) {
         cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kAttnThreads, smem);
     });
     return std::max(occ, 1);
 }
-// X0 rows of the samples (user, item i0 + b, d_hist) for b < B; grid: one wave of resident CTAs, so that each stages
-// the history once
+// X0 rows of the samples (user, item i0 + b, d_hist) for b < B (r.world > 1: local rows of this rank's shard); grid:
+// one wave of resident CTAs, so that each stages the history once
 int attn_forward_user(ctr_handle* h, const RowSrc& r, int user, const int* d_hist, int i0, int B, int grid) {
     return launch(h, "attn_fwd_user", [&] {
         const Dims d = dims_of(h);
         const size_t smem = attn_user_smem(h);
-        with_user_kernel(h, [&](auto kern) {
-            kern<<<std::min(grid, grid_attn(h, B)), kAttnThreads, smem, h->stream>>>(r, d, h->W[3], user, d_hist, i0, h->X0, h->Kp, h->Kp, B);
+        with_user_kernel(h, r.world > 1, [&](auto kern) {
+            kern<<<std::min(grid, grid_attn(h, B)), kAttnThreads, smem, h->stream>>>(r, d, h->W[3], user, d_hist, i0, h->comm.rank, h->X0, h->Kp, h->Kp, B);
         });
     });
 }
@@ -1030,9 +1033,11 @@ struct KnnArgs {
 template <int QT, bool ROWQ>
 void knn_scan_launch(ctr_handle* h, const KnnArgs& a, size_t smem) {
     const int T = CTR_TABLE_ITEM_EMB;
+    const bool sh = h->tab_sharded[T];            // this rank's shard: local row l is global row l·world + rank
     dim3 grid((a.nq + QT - 1) / QT, a.slices);
-    knn::k_knn_scan<QT, ROWQ><<<grid, knn::kThreads, smem, h->stream>>>(h->tab[T], h->tab_ld[T], (long)h->tab_rows[T], h->tab_width[T],
-                                                                       a.qvec, a.qrow, a.excl, a.nq, a.k, a.rows_per_slice, a.sl_sim, a.sl_row);
+    knn::k_knn_scan<QT, ROWQ><<<grid, knn::kThreads, smem, h->stream>>>(h->tab[T], h->tab_ld[T], (long)h->tab_local_rows[T], sh ? h->comm.world : 1,
+                                                                       sh ? h->comm.rank : 0, h->tab_width[T], a.qvec, a.qrow, a.excl, a.nq, a.k,
+                                                                       a.rows_per_slice, a.sl_sim, a.sl_row);
 }
 template <int QT, bool ROWQ>
 int knn_scan_occupancy(size_t smem) {
@@ -2154,31 +2159,60 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
-    if (k < 1 || k > knn::kMaxK || nq < 1 || (!queries && !query_rows) || !out_rows || !out_sim || !out_count)
-        return set_err(h, CTR_EINVAL, "bad knn arguments (k in [1, %d], nq >= 1, queries or query_rows, non-null outputs)", knn::kMaxK);
     std::lock_guard<std::mutex> lk(h->mu);
     const int T = CTR_TABLE_ITEM_EMB;
-    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
-    if (h->tab_sharded[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB is row-sharded over %d ranks: search needs the whole table on one device", h->comm.world);
-    const int64_t N = h->tab_rows[T];
-    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+    // a row-sharded ITEM_EMB makes the call collective: every rank scans its shard, the ranks' lists are merged
+    const bool coll = emb_sharded(h);
+    const int W = coll ? h->comm.world : 1;
     const bool by_row = queries == nullptr;
-    if (query_rows) for (int64_t i = 0; i < nq; i++) {
-        const int32_t r = query_rows[i];
-        if (by_row && (r < 0 || r >= N)) return set_err(h, CTR_ENOTFOUND, "%d is not found in searcher", r);     // search.go:75-77
-        if (!by_row && (r < -1 || r >= N)) return set_err(h, CTR_EINVAL, "excluded row %d of query %lld outside [-1, %lld)", r, (long long)i, (long long)N);
+    CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
+    const bool args_ok = !(k < 1 || k > knn::kMaxK || nq < 1 || (!queries && !query_rows) || !out_rows || !out_sim || !out_count);
+    const int verdict = [&]() -> int {
+        if (!args_ok)
+            return set_err(h, CTR_EINVAL, "bad knn arguments (k in [1, %d], nq >= 1, queries or query_rows, non-null outputs)", knn::kMaxK);
+        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+        if (coll) RET(comm_check_emb(h));
+        const int64_t N = h->tab_rows[T];
+        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+        if (query_rows) for (int64_t i = 0; i < nq; i++) {
+            const int32_t r = query_rows[i];
+            if (by_row && (r < 0 || r >= N)) return set_err(h, CTR_ENOTFOUND, "%d is not found in searcher", r);     // search.go:75-77
+            if (!by_row && (r < -1 || r >= N)) return set_err(h, CTR_EINVAL, "excluded row %d of query %lld outside [-1, %lld)", r, (long long)i, (long long)N);
+        }
+        return CTR_OK;
+    }();
+    // the call's header: the arguments are hashed whenever they are well-formed, whatever this rank's state, so a rank
+    // whose state check fails still agrees with the others and its verdict reaches them
+    CommHdr hd{};
+    hd.n = nq; hd.k = k; hd.mode = (queries ? 1 : 0) | (query_rows ? 2 : 0);
+    if (coll && args_ok) {
+        if (queries) hd.hash[0] = comm_hash(queries, (size_t)nq * h->cfg.D * sizeof(double));
+        if (query_rows) hd.hash[1] = comm_hash(query_rows, (size_t)nq * sizeof(int32_t));
     }
-    CU(h, cudaSetDevice(h->dev));
+    if (verdict != CTR_OK) {
+        if (!coll) return verdict;
+        const int rc = comm_agree(h, hd, verdict);
+        return rc != CTR_OK ? rc : verdict;
+    }
+    const int64_t N = h->tab_local_rows[T];   // the rows this rank scans
     const int D = h->tab_width[T], Dp = (D + 3) & ~3;
     // query tile: as wide as the batch needs, narrower when k's lists would not fit shared memory
     int QT = 16;
     while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
     const size_t smem = knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k), msmem = knn::smem_bytes<knn::SimKey>(1, 0, k);
-    int occ = 1;
-    if (by_row) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
+    // Row queries on a shard: the query rows are gathered (hot rows from the replica, the others from their owners)
+    // and widened to float64, then scanned as vector queries that exclude their own row.  A product of two widened
+    // floats is exact in float64, so the unfused sums of the vector instantiation equal the fused ones of ROWQ bit for bit.
+    const bool rowq = by_row && !coll;
+    int occ = 1;      // also sets the instantiation's shared-memory limit
+    if (rowq) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
     // row slices: enough CTAs to fill the GPU with the least idle tail (whole waves of resident CTAs); queries are
-    // chunked so that the slices' lists stay within 256 MB of scratch
-    const long steps = (long)((N + knn::kStep - 1) / knn::kStep);
+    // chunked so that the slices' lists (and on a sharded table the ranks' gathered lists) stay within 256 MB of scratch
+    // On a shard the plan is made for the largest shard (rank 0's), so that every rank picks the same query chunk and
+    // the ranks' all-gathers match.
+    const int64_t Nplan = coll ? (h->tab_rows[T] + W - 1) / W : N;
+    const long steps = std::max<long>(1, (long)((Nplan + knn::kStep - 1) / knn::kStep));
+    const int gw = coll ? W : 0;
     const long wave = (long)h->num_sms * occ;
     int64_t chunk = std::min<int64_t>(nq, 1024);
     int slices = 1;
@@ -2190,32 +2224,56 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
             const double w = (double)(s * tiles) / wave, eff = w / std::ceil(w);
             if (eff > best + 0.02) { best = eff; slices = (int)s; }
         }
-        if (chunk == 1 || (size_t)chunk * slices * k * 12 <= ((size_t)256 << 20)) break;
+        if (chunk == 1 || (size_t)chunk * (slices + gw) * k * 12 <= ((size_t)256 << 20)) break;
         chunk = (chunk + 1) / 2;
     }
     const long rps = (steps + slices - 1) / slices * knn::kStep;
-    slices = (int)((N + rps - 1) / rps);
+    slices = (int)std::max<int64_t>(1, (N + rps - 1) / rps);     // an empty shard still writes (empty) lists
+    if (coll) {
+        hd.plan = chunk;                 // the number of list all-gathers follows from it: checked, not assumed equal
+        RET(comm_agree(h, hd, CTR_OK));
+        RET(comm_ensure(h, false));
+        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
+        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+    }
 
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t b_q = al((size_t)chunk * D * 8), b_r = al((size_t)chunk * 4), b_ls = al((size_t)chunk * slices * k * 8),
-                 b_lr = al((size_t)chunk * slices * k * 4), b_os = al((size_t)chunk * k * 8), b_or = al((size_t)chunk * k * 4), b_oc = al((size_t)chunk * 4);
+                 b_lr = al((size_t)chunk * slices * k * 4), b_os = al((size_t)chunk * k * 8), b_or = al((size_t)chunk * k * 4), b_oc = al((size_t)chunk * 4),
+                 b_gs = al((size_t)chunk * gw * k * 8), b_gr = al((size_t)chunk * gw * k * 4);
     char* base = nullptr;
-    RET(scratch_get(h, 3, b_q + b_r + b_ls + b_lr + b_os + b_or + b_oc, (void**)&base));
+    RET(scratch_get(h, 3, b_q + b_r + b_ls + b_lr + b_os + b_or + b_oc + b_gs + b_gr, (void**)&base));
     double* d_q = (double*)base; int* d_r = (int*)(base + b_q);
     double* d_ls = (double*)(base + b_q + b_r); int* d_lr = (int*)(base + b_q + b_r + b_ls);
     double* d_os = (double*)(base + b_q + b_r + b_ls + b_lr); int* d_or = (int*)(base + b_q + b_r + b_ls + b_lr + b_os);
     int* d_oc = (int*)(base + b_q + b_r + b_ls + b_lr + b_os + b_or);
+    double* d_gs = (double*)(base + b_q + b_r + b_ls + b_lr + b_os + b_or + b_oc);      // [W][n][k] the ranks' lists
+    int* d_gr = (int*)(base + b_q + b_r + b_ls + b_lr + b_os + b_or + b_oc + b_gs);
 
     for (int64_t s = 0; s < nq; s += chunk) {
         const int n = (int)std::min<int64_t>(chunk, nq - s);
         if (!by_row) CU(h, cudaMemcpyAsync(d_q, queries + s * D, (size_t)n * D * sizeof(double), cudaMemcpyHostToDevice, h->stream));
         if (query_rows) CU(h, cudaMemcpyAsync(d_r, query_rows + s, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-        const KnnArgs a{by_row ? nullptr : d_q, by_row ? d_r : nullptr, (!by_row && query_rows) ? d_r : nullptr, n, k, rps, slices, d_ls, d_lr};
+        if (by_row && coll) {
+            const RowSrc src = comm_src(h, nullptr, nullptr, nullptr, 0, false);
+            const int gg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)n * D + 255) / 256, (int64_t)h->num_sms * 4));
+            RET(launch(h, "knn_gather_rows", [&] { k_gather_rows_f64<<<gg, 256, 0, h->stream>>>(src, d_r, n, D, d_q); }));
+        }
+        const KnnArgs a{rowq ? nullptr : d_q, rowq ? d_r : nullptr, (!rowq && query_rows) ? d_r : nullptr, n, k, rps, slices, d_ls, d_lr};
         RET(launch(h, "knn_scan", [&] {
             int unused = 0;
-            if (by_row) knn_scan_dispatch<true>(h, QT, a, false, smem, &unused); else knn_scan_dispatch<false>(h, QT, a, false, smem, &unused);
+            if (rowq) knn_scan_dispatch<true>(h, QT, a, false, smem, &unused); else knn_scan_dispatch<false>(h, QT, a, false, smem, &unused);
         }));
-        RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, d_or, d_os, d_oc); }));
+        const long sk = (long)slices * k;
+        if (!coll) {
+            RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, sk, k, d_or, d_os, d_oc); }));
+        } else {      // this rank's lists, then every rank's: the same total order, so the same result as one whole-table scan
+            RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, sk, k, d_or, d_os, nullptr); }));
+            RET(comm_gather_lists(h, d_os, d_gs, sizeof(double), d_or, d_gr, (size_t)n * k));
+            RET(launch(h, "knn_merge_ranks", [&] {
+                knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_gs, d_gr, W, k, k, (long)n * k, d_or, d_os, d_oc);
+            }));
+        }
         CU(h, cudaMemcpyAsync(out_rows + s * k, d_or, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_sim + s * k, d_os, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_count + s, d_oc, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -2227,21 +2285,47 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
 int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k, int32_t exclude_history,
                        int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
-    if (k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count)
-        return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs)", knn::kMaxK);
     std::lock_guard<std::mutex> lk(h->mu);
     const int T = CTR_TABLE_ITEM_EMB;
-    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
-    if (h->tab_sharded[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB is row-sharded over %d ranks: recommendation needs the whole table on one device", h->comm.world);
-    RET(check_tables(h));
-    const int64_t N = h->tab_rows[T];
-    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
-    CU(h, cudaSetDevice(h->dev));
+    // a row-sharded ITEM_EMB makes the call collective: every rank scores its shard, the ranks' lists are merged
+    const bool coll = emb_sharded(h);
+    const int W = coll ? h->comm.world : 1;
     const int S = h->cfg.S, Bc = h->Bmax;
     int optin = 0;
-    CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
-    const bool user_kernel = attn_user_ok(h, (size_t)optin);
-    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h) : 0;
+    bool user_kernel = false;
+    CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
+    const bool args_ok = !(k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count);
+    const int verdict = [&]() -> int {
+        if (!args_ok)
+            return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs)", knn::kMaxK);
+        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+        RET(coll ? comm_check(h) : check_tables(h));
+        const int64_t N = h->tab_rows[T];
+        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+        CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
+        user_kernel = attn_user_ok(h, (size_t)optin);
+        if (coll && !user_kernel)
+            return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)", S, attn_user_smem(h), optin);
+        return CTR_OK;
+    }();
+    if (!coll) RET(verdict);
+    else {
+        // the arguments are hashed whenever they are well-formed, whatever this rank's state (see ctr_knn_search)
+        CommHdr hd{};
+        hd.n = nu; hd.k = k; hd.flag = exclude_history ? 1 : 0;
+        if (args_ok) {
+            hd.hash[0] = comm_hash(user_rows, (size_t)nu * sizeof(int32_t));
+            hd.hash[1] = comm_hash(hist_rows, (size_t)nu * S * sizeof(int32_t));
+            hd.plan = std::min<int64_t>(nu, 256);      // users per list all-gather (G below)
+        }
+        const int rc = comm_agree(h, hd, verdict);
+        if (rc != CTR_OK || verdict != CTR_OK) return rc != CTR_OK ? rc : verdict;
+        RET(comm_ensure(h, false));
+        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
+        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+    }
+    const int64_t N = h->tab_local_rows[T];   // the items this rank scores
+    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
     // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
     const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     const int max_slices = (Bc + rps - 1) / rps;
@@ -2252,9 +2336,10 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
 
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t gk = (size_t)G * k, sl = (size_t)(1 + max_slices) * k;
-    const size_t b_h = al((size_t)G * S * 4), b_sl = al(sl * 4), b_l = al(gk * 4), b_c = al((size_t)G * 4);
+    const size_t b_h = al((size_t)G * S * 4), b_sl = al(sl * 4), b_l = al(gk * 4), b_c = al((size_t)G * 4),
+                 b_g = coll ? al((size_t)W * gk * 4) : 0;
     char* p = nullptr;
-    RET(scratch_get(h, 4, b_h + 2 * b_sl + 5 * b_l + b_c, (void**)&p));
+    RET(scratch_get(h, 4, b_h + 2 * b_sl + 5 * b_l + b_c + 2 * b_g, (void**)&p));
     int* d_hist = (int*)p;                 p += b_h;
     float* d_sl_s = (float*)p;             p += b_sl;      // [0, k): the user's running list, then the chunk's slice lists
     int* d_sl_r = (int*)p;                 p += b_sl;
@@ -2263,7 +2348,9 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     int* d_or = (int*)p;                   p += b_l;
     float* d_ol = (float*)p;               p += b_l;
     float* d_os = (float*)p;               p += b_l;
-    int* d_oc = (int*)p;
+    int* d_oc = (int*)p;                   p += b_c;
+    float* d_gs = (float*)p;               p += b_g;       // [W][G][k] the ranks' lists of the group
+    int* d_gr = (int*)p;
 
     const int nchunks = (int)((N + Bc - 1) / Bc);
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
@@ -2277,7 +2364,7 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
                 StepOpts o;
                 RowSrc r;
                 if (user_kernel) {
-                    r = idx_src(h, nullptr, nullptr, nullptr, nb);
+                    r = coll ? comm_src(h, nullptr, nullptr, nullptr, nb, false) : idx_src(h, nullptr, nullptr, nullptr, nb);
                     RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
                     o.x0_ready = true;
                 } else {
@@ -2289,18 +2376,29 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
                 const int slices = (nb + rps - 1) / rps;
                 const bool first = c == 0, last = c == nchunks - 1;
                 RET(launch(h, "rec_topk", [&] {
-                    rec::k_rec_scan<<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, rps, uh, nex, k, first ? nullptr : d_sl_s,
-                                                                                first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
+                    rec::k_rec_scan<<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, W, coll ? h->comm.rank : 0, rps, uh, nex, k,
+                                                                                first ? nullptr : d_sl_s, first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
                 }));
                 // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
+                const int ns = first ? slices : slices + 1;
                 RET(launch(h, "rec_merge", [&] {
                     knn::k_knn_merge<knn::LogitKey><<<1, knn::kThreads, msmem, h->stream>>>(
-                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, first ? slices : slices + 1, k,
+                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, ns, k, (long)ns * k, k,
                         last ? d_lr + (size_t)j * k : d_sl_r, last ? d_ls + (size_t)j * k : d_sl_s, nullptr);
                 }));
             }
+            if (nchunks == 0)            // an empty shard contributes an empty list
+                RET(launch(h, "rec_merge", [&] {
+                    knn::k_knn_merge<knn::LogitKey><<<1, knn::kThreads, msmem, h->stream>>>(d_sl_s, d_sl_r, 0, k, 0, 0, d_lr + (size_t)j * k, d_ls + (size_t)j * k, nullptr);
+                }));
         }
         const long n = (long)ng * k;
+        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
+            RET(comm_gather_lists(h, d_ls, d_gs, sizeof(float), d_lr, d_gr, (size_t)n));
+            RET(launch(h, "rec_merge_ranks", [&] {
+                knn::k_knn_merge<knn::LogitKey><<<ng, knn::kThreads, msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, d_lr, d_ls, nullptr);
+            }));
+        }
         RET(launch(h, "rec_finish", [&] { rec::k_rec_finish<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
         CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));

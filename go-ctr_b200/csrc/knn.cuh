@@ -16,6 +16,10 @@
 // if it beats the list's current k-th entry, and after every step one warp per query inserts the buffered candidates.
 // k_knn_merge: one CTA per query streams the slices' lists through the same list/buffer and writes the final top-k.
 //
+// Row-sharded ITEM_EMB (world > 1): the scan walks this rank's shard, whose local row l is global row l·world + rank;
+// exclusion and the tie order use the global row, so every rank's lists hold global rows and merging the ranks' lists
+// with k_knn_merge gives what one scan of the whole table gives.
+//
 // The list/buffer machinery is shared with the recommendation top-k (rec.cuh): a Key type names the score type and the
 // rule a score must meet to enter a list.
 #pragma once
@@ -127,9 +131,10 @@ __device__ __forceinline__ void offer(const Smem<K>& sm, int q, int k, typename 
 }
 
 // ROWQ: query i is table row qrow[i] (excluded from its own result); else the float64 vector qvec[i] (excl may name a
-// row to exclude, -1 = none).  Out: per (query, slice) the sorted top-k list, [nq][slices][k].
+// row to exclude, -1 = none).  tab holds nrows local rows; local row l is global row l·world + rank.  ROWQ reads the
+// query rows from tab and so needs world == 1.  Out: per (query, slice) the sorted top-k list, [nq][slices][k].
 template <int QT, bool ROWQ>
-__global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__ tab, long ld, long nrows, int D,
+__global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__ tab, long ld, long nrows, int world, int rank, int D,
                                                         const double* __restrict__ qvec, const int* __restrict__ qrow,
                                                         const int* __restrict__ excl, int nq, int k, long rows_per_slice,
                                                         double* __restrict__ out_sim, int* __restrict__ out_row) {
@@ -211,11 +216,12 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__
         for (int r = 0; r < kRows; r++) {
             if (!ok[r]) continue;
             const double n2 = __dsqrt_rn(nv[r]);
+            const int grow = (int)row[r] * world + rank;          // global rows fit int32 (checked by the host)
 #pragma unroll
             for (int q = 0; q < QT; q++) {
                 const double n1 = sm.qn[q];
                 const double s = (n1 == 0.0 || n2 == 0.0) ? 0.0 : __ddiv_rn(__ddiv_rn(acc[q][r], n1), n2);
-                if ((int)row[r] != sm.ex[q]) offer(sm, q, k, s, (int)row[r]);
+                if (grow != sm.ex[q]) offer(sm, q, k, s, grow);
             }
         }
         __syncthreads();
@@ -231,12 +237,14 @@ __global__ void __launch_bounds__(kThreads) k_knn_scan(const float* __restrict__
     }
 }
 
-// one CTA per query: the top-k of `slices` lists of k entries.  Positions past the count hold row -1 and score 0.
+// one CTA per query: the top-k of `slices` lists of k entries; list s of query g starts at element g·qstride + s·sstride
+// ([n][slices][k]: qstride = slices·k, sstride = k; the ranks' gathered [world][n][k]: qstride = k, sstride = n·k).
+// Positions past the count hold row -1 and score 0.
 // out_count == nullptr: the list is written as it stands, empty entries included, to be merged again; it may then
 // overwrite the first input list (every input is read before the first write).
 template <class K>
-__global__ void __launch_bounds__(kThreads) k_knn_merge(const typename K::T* in_sim, const int* in_row, int slices, int k,
-                                                         int32_t* out_row, typename K::T* out_sim, int32_t* __restrict__ out_count) {
+__global__ void __launch_bounds__(kThreads) k_knn_merge(const typename K::T* in_sim, const int* in_row, int slices, int k, long qstride,
+                                                         long sstride, int32_t* out_row, typename K::T* out_sim, int32_t* __restrict__ out_count) {
     using T = typename K::T;
     extern __shared__ __align__(16) char smem_raw[];
     const Smem<K> sm = carve<K>(smem_raw, 1, 0, k);
@@ -245,13 +253,16 @@ __global__ void __launch_bounds__(kThreads) k_knn_merge(const typename K::T* in_
     if (threadIdx.x == 0) sm.bn[0] = 0;
     __syncthreads();
     const long n = (long)slices * k;
-    const T* is = in_sim + (size_t)g * n;
-    const int* ir = in_row + (size_t)g * n;
+    const T* is = in_sim + (size_t)g * qstride;
+    const int* ir = in_row + (size_t)g * qstride;
     for (long base = 0; base < n; base += kStep) {
 #pragma unroll
         for (int r = 0; r < kRows; r++) {
             const long i = base + threadIdx.x + r * kThreads;
-            if (i < n) offer(sm, 0, k, is[i], ir[i]);
+            if (i >= n) continue;
+            long o = i;                                   // contiguous lists: no division
+            if (sstride != k) { const long s = i / k; o = s * sstride + (i - s * k); }
+            offer(sm, 0, k, is[o], ir[o]);
         }
         __syncthreads();
         flush<1>(sm, k);

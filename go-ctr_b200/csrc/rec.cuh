@@ -22,12 +22,13 @@ using knn::kThreads;
 // dynamic shared memory of k_rec_scan: the list/buffer state plus the exclusion rows that fall into the slice
 __host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<LogitKey>(1, 0, k) + (size_t)nex * 4 + 16; }
 
-// z[b] is the logit of row row0 + b, b < n.  excl[0, nex): rows that must not be returned (duplicates and rows outside
-// the table are harmless).  run_s / run_r: the user's running list over the earlier chunks (nullptr for the first): only
-// rows that beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row
-// lies in an earlier chunk, so the fillers are told apart by row and written back as empty entries.
-// Out: per slice the top-k list, [slices][k].
-__global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__ z, int n, int row0, int rows_per_slice,
+// z[b] is the logit of local row row0 + b, b < n; local row l is global row l·world + rank (a row-sharded ITEM_EMB; 1
+// and 0 otherwise).  excl[0, nex): global rows that must not be returned (duplicates and rows outside the table are
+// harmless).  run_s / run_r: the user's running list over the earlier chunks (nullptr for the first): only rows that
+// beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row lies in an
+// earlier chunk, so the fillers are told apart by row and written back as empty entries.
+// Out: per slice the top-k list of global rows, [slices][k].
+__global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
                                                         const int* __restrict__ excl, int nex, int k,
                                                         const float* run_s, const int* run_r,
                                                         float* __restrict__ out_s, int* __restrict__ out_row) {
@@ -43,8 +44,8 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__
     __syncthreads();
     for (int i = threadIdx.x; i < nex; i += kThreads) {       // usually none of the user's rows fall into this slice
         const int e = __ldg(excl + i);
-        const long b = (long)e - row0;
-        if (b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+        const long b = (long)(e / world) - row0;
+        if (e >= 0 && e % world == rank && b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
     }
     __syncthreads();
     const int m = nx;
@@ -53,7 +54,7 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__
         for (int r = 0; r < knn::kRows; r++) {
             const int b = base + threadIdx.x + r * kThreads;
             if (b >= r1) continue;
-            const int row = row0 + b;
+            const int row = (row0 + b) * world + rank;
             bool skip = false;
             for (int e = 0; e < m; e++) skip |= ex[e] == row;
             if (!skip) knn::offer(sm, 0, k, __ldg(z + b), row);

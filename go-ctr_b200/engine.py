@@ -378,7 +378,10 @@ class Engine:
     def knn_search(self, k, queries=None, rows=None):
         """search.Searcher on ITEM_EMB (ctr_knn_search): queries [nq, D] float64 vectors (rows: optional row to exclude
         per query, -1 = none), or queries=None and rows = the query rows.  Returns (rows [nq, k] int32, sims [nq, k]
-        float64, counts [nq] int32); positions past a query's count hold row -1 and similarity 0."""
+        float64, counts [nq] int32); positions past a query's count hold row -1 and similarity 0.
+        On a row-sharded ITEM_EMB (world > 1, large table) the call is collective: every rank calls it with the same
+        arguments and receives the same complete result, bit-identical to one GPU holding the whole table; arguments
+        that differ between the ranks raise CTR_EINVAL on every rank.  No sync is needed after training."""
         qp = rp = None
         if queries is not None:
             q = np.ascontiguousarray(queries, np.float64)
@@ -398,7 +401,8 @@ class Engine:
     def recommend_topk(self, user_rows, hist, k, exclude_history=True):
         """Top-k recommendation over every ITEM_EMB row (ctr_recommend_topk): user_rows [nu], hist [nu, S] (-1 padded).
         Returns (rows [nu, k] int32, scores [nu, k] float32, logits [nu, k] float32, counts [nu] int32), best first
-        (logit descending, then row ascending); positions past a user's count hold row -1, score 0 and logit 0."""
+        (logit descending, then row ascending); positions past a user's count hold row -1, score 0 and logit 0.
+        On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search."""
         u, up = _i(np.atleast_1d(user_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
         out_r = np.empty((u.size, k), np.int32); out_s = np.empty((u.size, k), np.float32)

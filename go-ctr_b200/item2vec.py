@@ -191,7 +191,9 @@ def neighbors_from_result(words, rows, sims, count, k):
 class Searcher:
     """search.Searcher (search.go:53-134) over an ITEM_EMB table in HBM.  Similarities are bit-identical to search.go
     run on the table's float32 values widened to float64; vectors loaded from text are rounded to float32 when
-    uploaded, so on those inputs parity holds up to that rounding.  Equal similarities rank by row ascending."""
+    uploaded, so on those inputs parity holds up to that rounding.  Equal similarities rank by row ascending.
+    On an engine whose ITEM_EMB is row-sharded over several GPUs every search is collective: every rank's process
+    makes the same call and receives the same complete result (Engine.knn_search)."""
 
     def __init__(self, engine, words, vectors=None):
         self.engine, self.words = engine, list(words)

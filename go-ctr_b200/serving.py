@@ -48,7 +48,11 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     algorithm"): the k best items of the whole table for one user at the current time, best first, as [ItemScore].
     Every ITEM_EMB row is scored with the trained model (ctr_recommend_topk); the user's history is windowed from the
     device ubcache at `now` (empty without one, as in BatchPredict); exclude_history drops the items of that window.
-    An unknown user raises CtrError with code ENOTFOUND, as BatchPredict does for an unresolvable first key."""
+    An unknown user raises CtrError with code ENOTFOUND, as BatchPredict does for an unresolvable first key.
+    On an engine whose ITEM_EMB is row-sharded over several GPUs the call is collective: every rank's process makes
+    the same call (same user, k, now and history) and receives the same complete result (Engine.recommend_topk).
+    A sharded deployment must pass `now` explicitly, the value broadcast with the request: the default reads each
+    process's own clock, so ranks can window different histories and then all fail with CTR_EINVAL."""
     ts = int(time.time()) if now is None else int(now)
     row = int(recSys.idmap_lookup(_e.IDMAP_USER, [int(userId)])[0])
     if row < 0:

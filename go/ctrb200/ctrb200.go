@@ -212,6 +212,9 @@ func (e *Engine) BatchPredict(sampleKeys []rcmd.Sample) ([]float32, error) {
 // if not nil, names a row to exclude per query, -1 for none), or is nil and rows holds the query rows (SearchInternal,
 // with the word→row map on the Go side). outRows / sims are [nq*k] in rank order; counts[i] is the true number of
 // results of query i, the positions past it hold row -1 and similarity 0.
+// With a row-sharded ITEM_EMB (world > 1, large table) Search is collective: every rank's process calls it with the
+// same arguments and each receives the same complete result, bit-identical to one GPU holding the whole table;
+// arguments that differ between the ranks fail on every rank. No Sync is needed after training.
 func (e *Engine) Search(queries []float64, rows []int32, k int) (outRows []int32, sims []float64, counts []int32, err error) {
 	nq := len(rows)
 	var qp *C.double
@@ -244,6 +247,7 @@ func (e *Engine) Search(queries []float64, rows []int32, k int) (outRows []int32
 // logit descending then row ascending. excludeHistory drops the items of the user's valid history rows. outRows /
 // scores / logits are [nu*k]; counts[j] is the true number of results of user j, the positions past it hold row -1,
 // score 0 and logit 0.
+// With a row-sharded ITEM_EMB (world > 1, large table) Recommend is collective, under the same rule as Search.
 func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory bool) (outRows []int32, scores, logits []float32, counts []int32, err error) {
 	nu := len(userRows)
 	if nu == 0 || k < 1 || len(histRows) != nu*int(e.cfg.S) {

@@ -268,8 +268,16 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
  * sums, dot / |q| / |v|; only similarities > 0 qualify.  Results come in rank order: similarity descending, equal
  * similarities by row ascending.  out_rows / out_sim are [nq, k]; out_count[i] is the true number of results of query i,
  * positions at or past it hold row -1 and similarity 0.  k in [1, 1024].  Needs only ITEM_EMB (a handle with
- * uP = cF = 0 is enough); a row-sharded ITEM_EMB (world > 1, large table) is CTR_ESTATE, a replicated one is searched
- * locally.  Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
+ * uP = cF = 0 is enough).  Runs on the engine stream under the handle's mutex, so it sees every update queued before it.
+ * Row-sharded ITEM_EMB (world > 1, large table): the call is collective — every rank calls it with the same arguments
+ * and receives the same complete result, bit-identical to one GPU holding the whole table.  Row ids stay global; more
+ * than INT32_MAX rows is CTR_ESTATE.  Each rank scans its own shard and the ranks' lists are merged.  The ranks first
+ * exchange their arguments and validation verdicts: arguments that differ are CTR_EINVAL on every rank ("ranks
+ * disagree ..."), otherwise every rank returns the verdict of the lowest failing rank.  A failure after that exchange
+ * (out of device memory, a failed peer mapping) leaves the other ranks waiting, as in the sharded train step.  The call starts with a device
+ * barrier over the ranks and finishes its reads before any rank's next step can change a row, so no ctr_sync or host
+ * barrier is needed between training and this call (unlike ctr_predict_idx on a sharded table).  A replicated ITEM_EMB
+ * is searched locally, by each rank alone. */
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count);
 
@@ -286,8 +294,12 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
  *     among the user's valid hist_rows.
  *   out_rows / out_scores / out_logits are [nu, k]; out_count[j] is the true number of results of user j, positions at
  *     or past it hold row -1, score 0 and logit 0.
- *   k in [1, 1024]; nu >= 1.  Missing tables, or no ITEM_EMB, is CTR_ESTATE; so is a row-sharded ITEM_EMB (world > 1,
- *     large table) — a replicated one is served locally.
+ *   k in [1, 1024]; nu >= 1.  Missing tables, or no ITEM_EMB, is CTR_ESTATE.
+ *   Row-sharded ITEM_EMB (world > 1, large table): collective, under the same rule as ctr_knn_search — every rank calls
+ *     with the same arguments and receives the same complete result, bit-identical to one GPU holding the whole table;
+ *     each rank scores its own shard's items and the ranks' lists are merged; disagreeing arguments are CTR_EINVAL
+ *     everywhere; no ctr_sync or host barrier is needed after training.  It needs D in {16, 32, 64, 128} and the user's
+ *     history rows in shared memory (else CTR_ESTATE).  A replicated ITEM_EMB is served locally, by each rank alone.
  *   Items are scored in chunks of max(batch, pred_batch) rows, in the activation buffers the handle already has: a large
  *     catalogue wants a large pred_batch.  Only nu·k results cross PCIe.
  *   Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
