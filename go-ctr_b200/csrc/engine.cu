@@ -2156,6 +2156,82 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
     { cudaError_t e = auc_run(h->stream, pred, y, (long)n, auc); if (e != cudaSuccess) return set_err(h, CTR_ECUDA, "auc: %s", cudaGetErrorString(e)); return CTR_OK; }
 }
 
+namespace {
+
+// ctr_group_auc on the engine stream: (group, score) order by two stable radix passes, one scan, one reduce-by-key,
+// then the per-group AUCs and their weighted mean on the device (auc.cuh); only the result, and the per-group arrays
+// when asked for, come back
+int gauc_run(ctr_handle* h, const float* pred_h, const float* y_h, const int64_t* group_h, long n, double* gauc,
+             int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+    cudaStream_t st = h->stream;
+    const size_t N = (size_t)n;
+    const int grid = (int)std::min<long>((n + 255) / 256, (long)h->num_sms * 8), gparts = h->num_sms * 2;
+    DevBuf<float> d_pred, d_y; DevBuf<long long> d_group;
+    DevBuf<unsigned> k0, k1; DevBuf<int> i0, i1, d_runs;
+    DevBuf<unsigned long long> g0, g1, v0, v1;
+    DevBuf<GaucScan> scan; DevBuf<GaucAgg> val, agg; DevBuf<GaucPart> part; DevBuf<GaucResult> res;
+    DevBuf<long long> o_group; DevBuf<int> o_n, o_pos; DevBuf<double> o_auc;
+    DevBuf<unsigned char> tmp;
+    CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N)); CU(h, d_group.alloc(N));
+    CU(h, k0.alloc(N)); CU(h, k1.alloc(N)); CU(h, i0.alloc(N)); CU(h, i1.alloc(N));
+    CU(h, g0.alloc(N)); CU(h, g1.alloc(N)); CU(h, v0.alloc(N)); CU(h, v1.alloc(N));
+    CU(h, scan.alloc(N)); CU(h, val.alloc(N)); CU(h, agg.alloc(N));
+    CU(h, d_runs.alloc(1)); CU(h, part.alloc(gparts)); CU(h, res.alloc(1));
+    if (out_group) CU(h, o_group.alloc(N));
+    if (out_n) CU(h, o_n.alloc(N));
+    if (out_pos) CU(h, o_pos.alloc(N));
+    if (out_auc) CU(h, o_auc.alloc(N));
+    unsigned long long* uniq = g0.get();     // free once the group pass has read it
+    size_t b[4] = {0, 0, 0, 0};
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[0], k0.get(), k1.get(), i0.get(), i1.get(), (int)n, 0, 32, st));
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[1], g0.get(), g1.get(), v0.get(), v1.get(), (int)n, 0, 64, st));
+    CU(h, cub::DeviceScan::InclusiveScan(nullptr, b[2], scan.get(), scan.get(), GaucScanOp(), (int)n, st));
+    CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b[3], g1.get(), uniq, val.get(), agg.get(), d_runs.get(), GaucAggOp(), (int)n, st));
+    size_t bytes = std::max(std::max(b[0], b[1]), std::max(b[2], b[3]));
+    CU(h, tmp.alloc(std::max<size_t>(bytes, 1)));
+    CU(h, cudaMemcpyAsync(d_pred, pred_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_y, y_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_group, group_h, N * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    RET(launch(h, "gauc_keys", [&] { k_gauc_keys<<<grid, 256, 0, st>>>(d_pred, n, k0, i0); }));
+    RET(launch(h, "gauc_sort_score", [&] {
+        cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, k0.get(), k1.get(), i0.get(), i1.get(), (int)n, 0, 32, st); }));
+    RET(launch(h, "gauc_gather", [&] { k_gauc_gather<<<grid, 256, 0, st>>>(k1, i1, d_group, d_y, n, g0, v0); }));
+    RET(launch(h, "gauc_sort_group", [&] {
+        cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, g0.get(), g1.get(), v0.get(), v1.get(), (int)n, 0, 64, st); }));
+    RET(launch(h, "gauc_heads", [&] { k_gauc_heads<<<grid, 256, 0, st>>>(g1, v1, n, scan); }));
+    RET(launch(h, "gauc_scan", [&] {
+        cub::DeviceScan::InclusiveScan(tmp.get(), bytes, scan.get(), scan.get(), GaucScanOp(), (int)n, st); }));
+    RET(launch(h, "gauc_terms", [&] { k_gauc_terms<<<grid, 256, 0, st>>>(g1, v1, scan, n, val); }));
+    RET(launch(h, "gauc_reduce", [&] {
+        cub::DeviceReduce::ReduceByKey(tmp.get(), bytes, g1.get(), uniq, val.get(), agg.get(), d_runs.get(), GaucAggOp(), (int)n, st); }));
+    RET(launch(h, "gauc_groups", [&] { k_gauc_groups<<<gparts, 256, 0, st>>>(uniq, agg, d_runs, o_group, o_n, o_pos, o_auc, part); }));
+    RET(launch(h, "gauc_final", [&] { k_gauc_final<<<1, 256, 0, st>>>(part, gparts, d_runs, res); }));
+    GaucResult r{};
+    CU(h, cudaMemcpyAsync(&r, res, sizeof r, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    const size_t R = (size_t)r.groups;
+    if (out_group) CU(h, cudaMemcpyAsync(out_group, o_group, R * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_n) CU(h, cudaMemcpyAsync(out_n, o_n, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_pos) CU(h, cudaMemcpyAsync(out_pos, o_pos, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_auc) CU(h, cudaMemcpyAsync(out_auc, o_auc, R * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *gauc = r.gauc;
+    if (n_groups) *n_groups = r.groups;
+    if (n_used) *n_used = r.used;
+    return CTR_OK;
+}
+
+}  // namespace
+
+int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n, double* gauc,
+                  int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+    if (!h || !pred || !y || !group || !gauc || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad group auc arguments (n must be in [1, 2^31); pred, y, group and gauc non-null)");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return gauc_run(h, pred, y, group, (long)n, gauc, n_groups, n_used, out_group, out_n, out_pos, out_auc);
+}
+
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");

@@ -27,7 +27,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params"]
 
@@ -374,6 +374,27 @@ class Engine:
         auc = C.c_double(0)
         self._ck(self.L.ctr_roc_auc(self.h, pp, tp, C.c_int64(p.size), C.byref(auc)))
         return auc.value
+
+    def group_auc(self, pred, y, group, per_group=False):
+        """Grouped AUC (ctr_group_auc): RocAuc32 within each group (normally the user id), weighted by the groups'
+        sample counts over the groups that hold both classes.  Returns (gauc, n_groups, n_used); with per_group=True
+        also a dict of the ascending group ids and their n, positives and AUC (NaN for a group with one class)."""
+        p, pp = _f(pred); t, tp = _f(y)
+        gr = np.ascontiguousarray(group, np.int64)
+        if not p.size == t.size == gr.size:
+            raise ValueError("pred, y and group differ in length: %d, %d, %d" % (p.size, t.size, gr.size))
+        gauc = C.c_double(0); ng = C.c_int64(0); nu = C.c_int64(0)
+        outs = None
+        if per_group:
+            outs = dict(group=np.empty(p.size, np.int64), n=np.empty(p.size, np.int32), pos=np.empty(p.size, np.int32),
+                        auc=np.empty(p.size, np.float64))
+        ptr = (lambda k, ty: outs[k].ctypes.data_as(C.POINTER(ty))) if outs else (lambda k, ty: None)
+        self._ck(self.L.ctr_group_auc(self.h, pp, tp, gr.ctypes.data_as(_lp), C.c_int64(p.size), C.byref(gauc), C.byref(ng),
+                                      C.byref(nu), ptr("group", C.c_int64), ptr("n", C.c_int32), ptr("pos", C.c_int32),
+                                      ptr("auc", C.c_double)))
+        if outs is None:
+            return gauc.value, ng.value, nu.value
+        return gauc.value, ng.value, nu.value, {k: v[:ng.value].copy() for k, v in outs.items()}
 
     def knn_search(self, k, queries=None, rows=None):
         """search.Searcher on ITEM_EMB (ctr_knn_search): queries [nq, D] float64 vectors (rows: optional row to exclude

@@ -23,7 +23,7 @@ from . import engine as _e
 
 __all__ = ["SampleInfo", "TrainSample", "DinNet", "YoutubeDnn", "NewDinNet", "NewDinNetFromJson",
            "NewYoutubeDnn", "NewYoutubeDnnFromJson", "Train", "InitForwardOnlyVm", "Predict",
-           "DinImpl", "YoutubeDnnImpl", "RocAuc32", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
+           "DinImpl", "YoutubeDnnImpl", "RocAuc32", "GroupAuc32", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
 
 mlp0_1, mlp1_2 = 200, 80          # din.go:17-18
 
@@ -248,3 +248,10 @@ def RocAuc32(pred, y, engine=None):
     """utils.RocAuc32 (util.go:131-148) on the device."""
     eng = engine or _e.Engine(_e.default_config(_e.MODEL_YOUTUBE, batch=1, pred_batch=1))
     return eng.roc_auc(pred, y)
+
+
+def GroupAuc32(pred, y, group, engine=None):
+    """GAUC on the device (ctr_group_auc): RocAuc32 per group (normally the UserId), weighted by the groups' sample
+    counts over the groups that hold both classes — the metric go-ctr's README quotes (README.md:17, 25, 33)."""
+    eng = engine or _e.Engine(_e.default_config(_e.MODEL_YOUTUBE, batch=1, pred_batch=1))
+    return eng.group_auc(pred, y, group)[0]

@@ -207,6 +207,34 @@ func (e *Engine) BatchPredict(sampleKeys []rcmd.Sample) ([]float32, error) {
 	return y, e.err(rc)
 }
 
+// GroupAUC is the GAUC the README quotes (README.md:17, 25, 33): utils.RocAuc32 within each group (normally the
+// sample's UserId), weighted by the groups' sample counts over the groups that hold both classes; NaN when none does.
+// With perGroup, groups holds the distinct ids ascending and n / pos / auc their samples, positives and AUC (NaN for a
+// group with one class), so another weighting is one dot product away.
+func (e *Engine) GroupAUC(pred, y []float32, group []int64, perGroup bool) (gauc float64, usedGroups int64, groups []int64, n, pos []int32, auc []float64, err error) {
+	m := len(pred)
+	if m == 0 || len(y) != m || len(group) != m {
+		return 0, 0, nil, nil, nil, nil, fmt.Errorf("ctrb200: GroupAUC needs equally long, non-empty pred, y and group")
+	}
+	var g C.double
+	var ng, nu C.int64_t
+	var gp *C.int64_t
+	var np, pp *C.int32_t
+	var ap *C.double
+	if perGroup {
+		groups, n, pos, auc = make([]int64, m), make([]int32, m), make([]int32, m), make([]float64, m)
+		gp, np, pp, ap = i64(groups), i32(n), i32(pos), (*C.double)(unsafe.Pointer(&auc[0]))
+	}
+	if err = e.err(C.ctr_group_auc(e.h, f32(pred), f32(y), i64(group), C.int64_t(m), &g, &ng, &nu, gp, np, pp, ap)); err != nil {
+		return 0, 0, nil, nil, nil, nil, err
+	}
+	if perGroup {
+		k := int(ng)
+		groups, n, pos, auc = groups[:k], n[:k], pos[:k], auc[:k]
+	}
+	return float64(g), int64(nu), groups, n, pos, auc, nil
+}
+
 // Search is search.Searcher (feature/embedding/search/search.go:66-134) over the ITEM_EMB table on the device: the k
 // rows most cosine-similar to each query. queries holds nq float64 vectors of the table's width (SearchVector; rows,
 // if not nil, names a row to exclude per query, -1 for none), or is nil and rows holds the query rows (SearchInternal,

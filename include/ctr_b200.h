@@ -259,6 +259,24 @@ int ctr_checkpoint_load(ctr_handle* h, const char* path);
  * scores grouped, trapezoid. Sorted on the device. */
 int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, double* auc);
 
+/* Grouped AUC (GAUC: the metric of the DIN paper and of go-ctr's README.md:17/25/33): samples are grouped by
+ * group[i] (normally the sample's UserId), groups ordered by ascending signed int64.  For group g with n_g samples, P_g
+ * positives and N_g = n_g - P_g negatives, AUC_g is ctr_roc_auc over the group's samples by the same rules (labels
+ * binarised at 0.5, -0 read as +0, scores ordered by the same transform of their float32 bits, equal scores one threshold
+ * group) from integer counts: area2_g = sum (fp_i - fp_{i-1}) (tp_i + tp_{i-1}) over the threshold-group ends in int64,
+ * AUC_g = (double)area2_g / (2.0 * P_g * N_g), NaN when P_g = 0 or N_g = 0.  Whenever 2 P_g N_g < 2^53, AUC_g equals
+ * ctr_roc_auc on that group's samples bit for bit.  A group is used when P_g > 0 and N_g > 0;
+ * *gauc = sum_used n_g AUC_g / sum_used n_g (weighted by impressions), NaN when no group is used.  The sum is
+ * deterministic (identical inputs give identical bits) and compensated.
+ * n in [1, 2^31); pred, y, group and gauc non-NULL, else CTR_EINVAL before any input is read.  n_groups (number of
+ * groups), n_used (used groups) and the out_* arrays may each be NULL.  A non-NULL out_* array has room for n entries;
+ * its first *n_groups entries are written in ascending group order: the group id, n_g, P_g and AUC_g (NaN when unused).
+ * Host buffers; needs no tables (a handle created with batch = pred_batch = 1 is enough).  Runs on the engine stream
+ * under the handle's mutex.  Not collective under world > 1: each rank evaluates the samples it passes. */
+int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n,
+                  double* gauc, int64_t* n_groups, int64_t* n_used,
+                  int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc);
+
 /* search.Searcher (feature/embedding/search/search.go:66-134): the k items of ITEM_EMB most cosine-similar to each
  * query, on the device.  queries == NULL: search by row — query i is ITEM_EMB row query_rows[i] widened to float64 and
  * excluded from its own result (SearchInternal, with the word→row map on the caller's side); a row outside [0, rows)
