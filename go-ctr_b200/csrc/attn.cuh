@@ -928,25 +928,35 @@ k_attn_bwd_gen(RowSrc r, Dims d, int model, const float* __restrict__ att,
 
 // -------------------------------------------------------------------------------------------------
 // recommend.GetSampleVector materialised (rcmd.go:462-536): X[b] = [user | S history rows | item
-// emb | item feat].  Bit-exact copies; one warp per sample.
+// emb | item feat].  Bit-exact copies (widened exactly when T is double); one warp per sample.
+// Output row b holds sample rows(b): RowsAsIs (sample b) for ctr_gather_rows and the MLP's key-fed predict,
+// RowsByIdx (sample idx[b]) for the shuffled minibatches of ctr_mlp_fit_keys.
 // -------------------------------------------------------------------------------------------------
+struct RowsAsIs { __device__ __forceinline__ int operator()(int b) const { return b; } };
+struct RowsByIdx {
+    const long* idx;
+    __device__ __forceinline__ int operator()(int b) const { return (int)__ldg(idx + b); }
+};
+
+template <typename T, typename Rows>
 __global__ void __launch_bounds__(256)
-k_gather_rows(RowSrc r, Dims d, float* __restrict__ X, long ldx, int B) {
+k_gather_rows(RowSrc r, Dims d, T* __restrict__ X, long ldx, int B, Rows rows) {
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nwarps = gridDim.x * (blockDim.x >> 5);
     for (int b = blockIdx.x * (blockDim.x >> 5) + wib; b < B; b += nwarps) {
-        float* x = X + (long)b * ldx;
-        const float* pu = src_up(r, b);
-        for (int j = lane; j < d.uP; j += 32) x[j] = pu ? __ldg(pu + j) : 0.0f;
+        T* x = X + (long)b * ldx;
+        const int sb = rows(b);
+        const float* pu = src_up(r, sb);
+        for (int j = lane; j < d.uP; j += 32) x[j] = pu ? (T)__ldg(pu + j) : (T)0;
         for (int s = 0; s < d.S; s++) {
-            const float* up = src_ub(r, d, b, s);
-            for (int j = lane; j < d.D; j += 32) x[d.uP + (long)s * d.D + j] = up ? __ldg(up + j) : 0.0f;
+            const float* up = src_ub(r, d, sb, s);
+            for (int j = lane; j < d.D; j += 32) x[d.uP + (long)s * d.D + j] = up ? (T)__ldg(up + j) : (T)0;
         }
-        const float* ip = src_it(r, d, b);
-        float* xi = x + d.uP + (long)d.S * d.D;
-        for (int j = lane; j < d.D; j += 32) xi[j] = ip ? __ldg(ip + j) : 0.0f;
-        const float* pc = src_cx(r, b);
-        for (int j = lane; j < d.cF; j += 32) xi[d.D + j] = pc ? __ldg(pc + j) : 0.0f;
+        const float* ip = src_it(r, d, sb);
+        T* xi = x + d.uP + (long)d.S * d.D;
+        for (int j = lane; j < d.D; j += 32) xi[j] = ip ? (T)__ldg(ip + j) : (T)0;
+        const float* pc = src_cx(r, sb);
+        for (int j = lane; j < d.cF; j += 32) xi[d.D + j] = pc ? (T)__ldg(pc + j) : (T)0;
     }
 }
 

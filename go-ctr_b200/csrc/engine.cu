@@ -145,6 +145,8 @@ struct ctr_handle {
     PinnedBuf<unsigned long long> kt_count_host; Event kt_counted[kCnt];
     // history windows of batch b+1 are cut on their own stream while batch b trains (two buffers)
     Stream win_stream; DevBuf<int> kt_hist[2]; Event kt_win[2], kt_used[2];
+    // ctr_mlp_fit_keys: the history window of every survivor [survivors, S], cut once per fit
+    DevBuf<int> kt_hist_all;
     // dense-X residency
     DevBuf<float> dXd, dYd;
 
@@ -1413,7 +1415,7 @@ int ctr_gather_rows(ctr_handle* h, const int32_t* user_row, const int32_t* item_
         rc = stage_idx(h, user_row + s, item_row + s, hist + s * c.S, nullptr, nb);
         if (rc != CTR_OK) break;
         RowSrc r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
-        rc = launch(h, "gather_rows", [&] { k_gather_rows<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), dout, xc, nb); });
+        rc = launch(h, "gather_rows", [&] { k_gather_rows<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), dout, xc, nb, RowsAsIs{}); });
         if (rc != CTR_OK) break;
         if (cudaMemcpyAsync(X + s * xc, dout, (size_t)nb * xc * sizeof(float), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
             cudaStreamSynchronize(h->stream) != cudaSuccess) rc = set_err(h, CTR_ECUDA, "gather D2H: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1549,6 +1551,51 @@ int feed_init(ctr_handle* h) {
     h->copy_stream = std::move(copy);
     return CTR_OK;
 }
+
+// GetSample's assembly over sample keys (ctr_train_keys, ctr_mlp_fit_keys): the resident survivor arrays kt_* for cap
+// samples, the flag / scan buffers of `chunk` keys and the survivor count, zeroed.  feed_init must have run.
+int keys_prepare(ctr_handle* h, size_t cap, size_t chunk) {
+    RET(reserve(h, h->kt_user, cap)); RET(reserve(h, h->kt_item, cap)); RET(reserve(h, h->kt_ts, cap)); RET(reserve(h, h->kt_label, cap));
+    if (!h->kt_scan_tmp || h->kt_flag.size() < chunk + 1) {     // kt_scan_tmp is allocated last: it exists only with the other two
+        h->kt_scan_tmp.reset();
+        RET(dalloc(h, h->kt_flag, chunk + 1)); RET(dalloc(h, h->kt_pos, chunk + 1));
+        size_t bytes = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, bytes, h->kt_flag.get(), h->kt_pos.get(), (int)(chunk + 1), h->stream);
+        RET(dalloc(h, h->kt_scan_tmp, bytes, false));
+    }
+    if (!h->kt_count) RET(dalloc(h, h->kt_count, 1));
+    CU(h, cudaMemsetAsync(h->kt_count, 0, sizeof(unsigned long long), h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return CTR_OK;
+}
+
+// keys [c·chunk, c·chunk + chunk) of n → (user row, item row, ts, label) appended to kt_* after the survivors of the
+// earlier chunks; unresolvable samples dropped, order kept.  Caller memory → pinned ring (host threads) → device slot
+// c & 1 → k_keys_rows, scan, k_keys_compact, count advance, all on stream rs.
+int keys_resolve_chunk(ctr_handle* h, int64_t c, size_t chunk, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
+                       const float* label, int64_t n, cudaStream_t rs) {
+    const int slot = (int)(c & 1), ps = (int)(c % ctr_handle::kPin);
+    const int64_t start = c * (int64_t)chunk; const size_t m = (size_t)std::min<int64_t>((int64_t)chunk, n - start);
+    if (c >= ctr_handle::kPin) CU(h, cudaEventSynchronize(h->pin_free[ps]));
+    unsigned char* pin = h->feed_pin[ps];
+    h->pool->copy(pin, user_ids + start, m * 8); h->pool->copy(pin + m * 8, item_ids + start, m * 8);
+    h->pool->copy(pin + m * 16, ts + start, m * 8); h->pool->copy(pin + m * 24, label + start, m * 4);
+    CU(h, cudaMemcpyAsync(h->feed_dev[slot], pin, m * 28, cudaMemcpyHostToDevice, rs));     // after resolve(c-2), which read this slot (stream order)
+    CU(h, cudaEventRecord(h->pin_free[ps], rs));
+    const long long* dk = (const long long*)h->feed_dev[slot].get();
+    const int grid = (int)std::max<size_t>(1, std::min<size_t>((m + 255) / 256, (size_t)h->num_sms * 8));
+    RET(launch(h, "keys_rows", [&] {
+        k_keys_rows<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
+                                         dk, dk + m, (long)m, h->kt_flag);
+    }));
+    RET(launch(h, "cub_exclusive_scan", [&] { size_t tb = h->kt_scan_tmp.size(); cub::DeviceScan::ExclusiveSum(h->kt_scan_tmp, tb, h->kt_flag.get(), h->kt_pos.get(), (int)(m + 1), rs); }));
+    RET(launch(h, "keys_compact", [&] {
+        k_keys_compact<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
+                                            dk, dk + m, dk + 2 * m, (const float*)(dk + 3 * m), (long)m, h->kt_flag, h->kt_pos, h->kt_count,
+                                            h->kt_user, h->kt_item, h->kt_ts, h->kt_label);
+    }));
+    return launch(h, "keys_advance", [&] { k_keys_advance<<<1, 1, 0, rs>>>(h->kt_pos + m, h->kt_count); });
+}
 }  // namespace
 
 int ctr_train_idx(ctr_handle* h, const int32_t* user_row, const int32_t* item_row, const int32_t* hist, const float* label,
@@ -1606,22 +1653,13 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
     if (!emb_sharded(h)) RET(check_tables(h));
     const int B = h->cfg.batch, S = h->cfg.S;
     RET(feed_init(h));
-    // ---- resident sample arrays (+B slack so a padded tail never indexes past the end)
-    const size_t cap = (size_t)n + (size_t)B;
-    RET(reserve(h, h->kt_user, cap)); RET(reserve(h, h->kt_item, cap)); RET(reserve(h, h->kt_ts, cap)); RET(reserve(h, h->kt_label, cap));
     // One GPU: the first epoch STREAMS — small chunks, and the steps over the samples already resident are queued while
     // the host stages the next chunk (the survivor count of chunk c-1 comes back through a pinned ring).  Several ranks:
     // every step is collective, so the ranks first agree on the batch count (resolve everything, then train).
     const bool streaming = epochs > 0 && h->comm.world == 1;
     const size_t chunk = std::min<size_t>((size_t)n, streaming ? std::min<size_t>(h->feed_bytes / 28, (size_t)2 * B) : h->feed_bytes / 28);   // keys per staging slot
-    if (!h->kt_scan_tmp || h->kt_flag.size() < chunk + 1) {     // kt_scan_tmp is allocated last: it exists only with the other two
-        h->kt_scan_tmp.reset();
-        RET(dalloc(h, h->kt_flag, chunk + 1)); RET(dalloc(h, h->kt_pos, chunk + 1));
-        size_t bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, bytes, h->kt_flag.get(), h->kt_pos.get(), (int)(chunk + 1), h->stream);
-        RET(dalloc(h, h->kt_scan_tmp, bytes, false));
-    }
-    if (!h->kt_count) RET(dalloc(h, h->kt_count, 1));
+    // ---- resident sample arrays (+B slack so a padded tail never indexes past the end)
+    RET(keys_prepare(h, (size_t)n + (size_t)B, chunk));
     if (!h->kt_count_host) {            // the count ring and its events, moved into the handle together
         PinnedBuf<unsigned long long> ring; Event counted[ctr_handle::kCnt];
         CU(h, ring.alloc(ctr_handle::kCnt));
@@ -1629,8 +1667,6 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
         for (int i = 0; i < ctr_handle::kCnt; i++) h->kt_counted[i] = std::move(counted[i]);
         h->kt_count_host = std::move(ring);
     }
-    CU(h, cudaMemsetAsync(h->kt_count, 0, sizeof(unsigned long long), h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
     if (!h->win_stream) {               // the window stream, its two buffers and their events, moved in together
         Stream ws; DevBuf<int> hist[2]; Event win[2], used[2];
         CU(h, ws.create());
@@ -1673,27 +1709,7 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
     int64_t nchunks = ((int64_t)n + (int64_t)chunk - 1) / (int64_t)chunk;
     int64_t queued = 0;                                       // first-epoch batches already on the engine stream (streaming)
     for (int64_t c = 0; c < nchunks; c++) {
-        const int slot = (int)(c & 1), ps = (int)(c % ctr_handle::kPin);
-        const int64_t start = c * (int64_t)chunk; const size_t m = (size_t)std::min<int64_t>((int64_t)chunk, n - start);
-        if (c >= ctr_handle::kPin) CU(h, cudaEventSynchronize(h->pin_free[ps]));
-        unsigned char* pin = h->feed_pin[ps];
-        h->pool->copy(pin, user_ids + start, m * 8); h->pool->copy(pin + m * 8, item_ids + start, m * 8);
-        h->pool->copy(pin + m * 16, ts + start, m * 8); h->pool->copy(pin + m * 24, label + start, m * 4);
-        CU(h, cudaMemcpyAsync(h->feed_dev[slot], pin, m * 28, cudaMemcpyHostToDevice, rs));     // after resolve(c-2), which read this slot (stream order)
-        CU(h, cudaEventRecord(h->pin_free[ps], rs));
-        const long long* dk = (const long long*)h->feed_dev[slot].get();
-        const int grid = (int)std::max<size_t>(1, std::min<size_t>((m + 255) / 256, (size_t)h->num_sms * 8));
-        RET(launch(h, "keys_rows", [&] {
-            k_keys_rows<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
-                                             dk, dk + m, (long)m, h->kt_flag);
-        }));
-        RET(launch(h, "cub_exclusive_scan", [&] { size_t tb = h->kt_scan_tmp.size(); cub::DeviceScan::ExclusiveSum(h->kt_scan_tmp, tb, h->kt_flag.get(), h->kt_pos.get(), (int)(m + 1), rs); }));
-        RET(launch(h, "keys_compact", [&] {
-            k_keys_compact<<<grid, 256, 0, rs>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
-                                                dk, dk + m, dk + 2 * m, (const float*)(dk + 3 * m), (long)m, h->kt_flag, h->kt_pos, h->kt_count,
-                                                h->kt_user, h->kt_item, h->kt_ts, h->kt_label);
-        }));
-        RET(launch(h, "keys_advance", [&] { k_keys_advance<<<1, 1, 0, rs>>>(h->kt_pos + m, h->kt_count); }));
+        RET(keys_resolve_chunk(h, c, chunk, user_ids, item_ids, ts, label, n, rs));
         if (streaming) {
             const int cs = (int)(c % ctr_handle::kCnt);
             CU(h, cudaMemcpyAsync(h->kt_count_host + cs, h->kt_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, rs));
@@ -1992,18 +2008,27 @@ int ctr_idmap_lookup(ctr_handle* h, int which, const int64_t* ids, int64_t n, in
     return rc;
 }
 
+namespace {
+// staging of the key-fed predict calls, moved in together: device [user ids | item ids | ts] of one pred_batch chunk and
+// pinned host [keys | scores | first user row]
+int keys_stage_init(ctr_handle* h) {
+    if (h->k_keys) return CTR_OK;
+    const int B = h->cfg.pred_batch;
+    DevBuf<long long> keys; PinnedBuf<unsigned char> host;
+    RET(dalloc(h, keys, (size_t)3 * B, false));
+    CU(h, host.alloc(sizeof(long long) * (size_t)3 * B + sizeof(float) * (size_t)B + 16));
+    h->k_host = std::move(host); h->k_keys = std::move(keys);
+    return CTR_OK;
+}
+}  // namespace
+
 int ctr_batch_predict_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
     if (!h || !user_ids || !item_ids || !ts || !scores || n < 1) return set_err(h, CTR_EINVAL, "bad batch predict arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
     if (!h->idm_keys[0] || !h->idm_keys[1]) return set_err(h, CTR_ESTATE, "batch predict needs both id maps (ctr_idmap_build)");
     const int B = h->cfg.pred_batch, S = h->cfg.S;
-    if (!h->k_keys) {       // device + pinned staging: [user ids | item ids | ts] and {first user row}, moved in together
-        DevBuf<long long> keys; PinnedBuf<unsigned char> host;
-        RET(dalloc(h, keys, (size_t)3 * B, false));
-        CU(h, host.alloc(sizeof(long long) * (size_t)3 * B + sizeof(float) * (size_t)B + 16));
-        h->k_host = std::move(host); h->k_keys = std::move(keys);
-    }
+    RET(keys_stage_init(h));
     long long* hk = (long long*)h->k_host.get();
     float* hs = (float*)(hk + (size_t)3 * B);
     int* hfirst = (int*)(hs + B);
@@ -2779,7 +2804,10 @@ struct ctr_mlp {
     DevBuf<double> act[kMlpMaxLayers], del[kMlpMaxLayers];           // [rows, units[l]]
     DevBuf<double> X64; DevBuf<float> Y32; DevBuf<long> idx;
     DevBuf<double> scal;                                              // [0] batch loss, [1] epoch accumulator
-    double adam_calls = 0;                                            // AdamOptimizer64.t
+    // key-fed fit / predict: [rows, nin] float64 inputs a feature store gathers (two, so minibatch k+1 is gathered on the
+    // store's stream while k trains); stage_free[s]: the minibatch that last read stage[s] is done; stage_full[s]: gathered
+    DevBuf<double> stage[2]; Event stage_free[2], stage_full[2];
+    double adam_calls = 0;                                           // AdamOptimizer64.t
     double t = 0;                                                     // BaseMultilayerPerceptron64.t: samples since initialize (:412,814)
     bool fitted = false;
 };
@@ -2817,12 +2845,124 @@ int mlp_upload_x(ctr_mlp* m, const float* X, int64_t n, int nin) {
     }
     return rc;
 }
-// forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads X64 through idx (may be null = identity) from row0
-void mlp_forward(ctr_mlp* m, const long* idx, long row0, int rows) {
+// forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads the [*, nin] matrix X through idx (may be null = identity)
+void mlp_forward(ctr_mlp* m, const double* X, const long* idx, int rows) {
     const int L = m->d.n_layers, nin = m->d.units[0];
     for (int l = 0; l + 1 < L; l++)
-        k_mlp64_layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, m->X64 + (idx ? 0 : row0 * nin), nin, idx,
+        k_mlp64_layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, X, nin, idx,
                                                                                       l == 0 ? nullptr : m->act[l].get(), m->act[l + 1], rows);
+}
+// the two [rows, nin] staging buffers and their events of the key-fed entry points (grow-only; events made once)
+int mlp_stage(ctr_mlp* m, long rows) {
+    const size_t n = (size_t)rows * m->d.units[0];
+    for (int s = 0; s < 2; s++) if (m->stage[s].size() < n) MCU(m, m->stage[s].alloc(n));
+    if (!m->stage_full[1]) {
+        Event fr[2], fu[2];
+        for (int s = 0; s < 2; s++) { MCU(m, fr[s].create(cudaEventDisableTiming)); MCU(m, fu[s].create(cudaEventDisableTiming)); }
+        for (int s = 0; s < 2; s++) { m->stage_free[s] = std::move(fr[s]); m->stage_full[s] = std::move(fu[s]); }
+    }
+    return CTR_OK;
+}
+// initialize, basemlp64.go:459-476, unless a warm start keeps the fitted parameters
+int mlp_init_params(ctr_mlp* m) {
+    const ctr_mlp_config& c = m->cfg;
+    if (c.warm_start && m->fitted) return CTR_OK;
+    // every packed element (intercepts too) = U[0,1)·sqrt(f/(fi+fo)), f = 6, or 2 for a logistic hidden activation —
+    // non-negative; counter RNG instead of the reference's time-seeded source
+    std::vector<double> p((size_t)m->np);
+    long pos = 0;
+    for (int l = 0; l + 1 < m->d.n_layers; l++) {
+        const int fi = m->d.units[l], fo = m->d.units[l + 1];
+        const double bound = std::sqrt((c.hidden_act == CTR_MLP_LOGISTIC ? 2.0 : 6.0) / (double)(fi + fo));
+        const long end = pos + (long)(1 + fi) * fo;
+        for (; pos < end; pos++) p[(size_t)pos] = (double)(mix64(c.seed, 7, (uint64_t)pos) >> 11) * (1.0 / 9007199254740992.0) * bound;
+    }
+    MCU(m, cudaMemcpyAsync(m->params, p.data(), sizeof(double) * (size_t)m->np, cudaMemcpyHostToDevice, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    m->t = 0;                                                            // :412
+    return CTR_OK;
+}
+// Layer 0's input of minibatch k (0-based within the epoch), whose samples are bi[0, rows): *X = a [rows, nin] matrix
+// read row by row, or left null to read X64 through bi (ctr_mlp_fit).
+using MlpInput = std::function<int(long k, const long* bi, int rows, const double** X)>;
+// fitStochastic (basemlp64.go:729-857) over n samples with the device labels Y [n], in minibatches of bs: a fresh optimizer,
+// the per-epoch shuffle, the solvers, weight decay, the stopping rules and the t carry.  Only layer 0's input differs
+// between the callers (input may be empty).  m->idx holds n entries and the activations bs rows.
+int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const MlpInput& input, int32_t* n_iter, double* loss_curve) {
+    const ctr_mlp_config& c = m->cfg;
+    const int nin = m->d.units[0];
+    const ctr_mlp_options& o = m->opts;
+    const bool sgd = o.solver == CTR_MLP_SOLVER_SGD;
+    MCU(m, cudaMemsetAsync(m->ms, 0, sizeof(double) * (size_t)m->np, m->stream));        // a fresh optimizer per fit (:731-752)
+    MCU(m, cudaMemsetAsync(m->vs, 0, sizeof(double) * (size_t)m->np, m->stream));
+    m->adam_calls = 0;
+    double sgd_lr = c.lr_init;                                           // SGDOptimizer64.LearningRate
+    std::vector<long> idx((size_t)n);
+    for (long i = 0; i < n; i++) idx[(size_t)i] = i;
+    double lr_init = c.lr_init, lr_last = c.lr_init, best = INFINITY;
+    int no_improve = 0, it = 0;
+    const int L = m->d.n_layers;
+    for (it = 0; it < c.max_iter;) {
+        if (c.shuffle) {                                                 // rand.Shuffle (:788): Fisher–Yates from the top
+            for (long i = n - 1; i > 0; i--) { const long j = (long)(mix64(c.seed, 100u + (uint32_t)it, (uint64_t)i) % (uint64_t)(i + 1)); std::swap(idx[(size_t)i], idx[(size_t)j]); }
+        }
+        MCU(m, cudaMemcpyAsync(m->idx, idx.data(), sizeof(long) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
+        MCU(m, cudaMemsetAsync(m->scal, 0, 2 * sizeof(double), m->stream));
+        for (long b0 = 0; b0 < n; b0 += bs) {                            // :791-808
+            const int rows = (int)std::min<long>(bs, n - b0);
+            const long* bi = m->idx + b0;
+            const double* X0 = nullptr;
+            if (input) RET(input(b0 / bs, bi, rows, &X0));
+            const long* xi = X0 ? nullptr : bi;
+            if (!X0) X0 = m->X64;
+            if (o.weight_decay > 0.0)                                    // backprop :342-346
+                k_mlp64_decay<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->np, 1.0 - o.weight_decay);
+            mlp_forward(m, X0, xi, rows);
+            k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
+            for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
+                k_mlp64_grads<<<mlp_grid(m, (long)(m->d.units[l] + 1) * m->d.units[l + 1]), 256, 0, m->stream>>>(
+                    m->params, m->grads, m->d, l, X0, nin, xi, l == 0 ? nullptr : m->act[l].get(), m->del[l + 1], rows, c.alpha);
+                if (l >= 1) k_mlp64_delta<<<mlp_grid(m, (long)rows * m->d.units[l]), 256, 0, m->stream>>>(m->params, m->d, l, m->act[l], m->del[l + 1], m->del[l], rows);
+            }
+            if (sgd) {
+                k_mlp64_sgd<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->np, sgd_lr, o.momentum, o.nesterov);
+            } else {
+                k_mlp64_adam<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->vs, m->np, m->adam_calls, lr_init, c.beta1, c.beta2, c.eps);
+                m->adam_calls += 1;
+            }
+        }
+        it++;
+        double sc[2] = {0, 0};
+        MCU(m, cudaMemcpyAsync(sc, m->scal, sizeof sc, cudaMemcpyDeviceToHost, m->stream));
+        MCU(m, cudaStreamSynchronize(m->stream));
+        MCU(m, cudaGetLastError());
+        const double loss = sc[1] / (double)n;                           // :810-811
+        m->t += (double)n;                                               // :814
+        if (loss_curve) loss_curve[it - 1] = loss;
+        if (!sgd) {   // the learning rate the optimizer last used (:1088): decides "adaptive" stopping (:1059-1064)
+            const double e = m->adam_calls * (double)m->np;
+            lr_last = lr_init * std::sqrt(1.0 - std::pow(c.beta2, e)) / (1.0 - std::pow(c.beta1, e));
+        }
+        if (loss > best - c.tol) no_improve++; else no_improve = 0;      // :886-892
+        if (loss < best) best = loss;
+        if (sgd && o.lr_schedule == CTR_MLP_LR_INVSCALING)               // iterationEnds :999-1003 (Adam's is a no-op, :1053)
+            sgd_lr = c.lr_init / std::pow(m->t + 1.0, o.power_t);
+        if (no_improve > c.n_iter_no_change) {                           // :826-840
+            if (o.lr_schedule != CTR_MLP_LR_ADAPTIVE) break;             // triggerStopping :1005-1011, :1054-1060
+            if ((sgd ? sgd_lr : lr_last) <= 1e-6) break;                 // :1012-1017, :1061-1066
+            if (sgd) sgd_lr *= .8;                                       // :1018 — the current rate
+            else lr_init *= .8;                                          // :1067 — the base rate
+            no_improve = 0;
+        }
+    }
+    if (n_iter) *n_iter = it;
+    m->fitted = true;
+    return CTR_OK;
+}
+long mlp_batch(const ctr_mlp* m, long n) {
+    long bs = m->cfg.batch;
+    if (bs <= 0) bs = n < 200 ? n : 200; else if (bs > n) bs = n;       // basemlp64.go:517-527
+    return bs;
 }
 }  // namespace
 
@@ -2917,95 +3057,17 @@ int ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np) {
 int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, int32_t* n_iter, double* loss_curve) {
     if (!m || !X || !Y || n < 1) return mlp_err(m, CTR_EINVAL, "bad fit arguments");
     std::lock_guard<std::mutex> lk(m->mu);
-    const ctr_mlp_config& c = m->cfg;
     const int nin = m->d.units[0];
     if (xcols != nin) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, nin);
     MCU(m, cudaSetDevice(m->dev));
-    long bs = c.batch;
-    if (bs <= 0) bs = n < 200 ? n : 200; else if (bs > n) bs = n;                       // basemlp64.go:517-527
+    const long bs = mlp_batch(m, n);
     RET(mlp_upload_x(m, X, n, nin));
     if (m->Y32.size() < (size_t)n) MCU(m, m->Y32.alloc((size_t)n));
     if (m->idx.size() < (size_t)n) MCU(m, m->idx.alloc((size_t)n));
     MCU(m, cudaMemcpyAsync(m->Y32, Y, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
     RET(mlp_rows(m, bs));
-    if (!c.warm_start || !m->fitted) {
-        // initialize, basemlp64.go:459-476: every packed element (intercepts too) = U[0,1)·sqrt(f/(fi+fo)), f = 6, or 2 for a
-        // logistic hidden activation — non-negative; counter RNG instead of the reference's time-seeded source
-        std::vector<double> p((size_t)m->np);
-        long pos = 0;
-        for (int l = 0; l + 1 < m->d.n_layers; l++) {
-            const int fi = m->d.units[l], fo = m->d.units[l + 1];
-            const double bound = std::sqrt((c.hidden_act == CTR_MLP_LOGISTIC ? 2.0 : 6.0) / (double)(fi + fo));
-            const long end = pos + (long)(1 + fi) * fo;
-            for (; pos < end; pos++) p[(size_t)pos] = (double)(mix64(c.seed, 7, (uint64_t)pos) >> 11) * (1.0 / 9007199254740992.0) * bound;
-        }
-        MCU(m, cudaMemcpyAsync(m->params, p.data(), sizeof(double) * (size_t)m->np, cudaMemcpyHostToDevice, m->stream));
-        MCU(m, cudaStreamSynchronize(m->stream));
-        m->t = 0;                                                        // :412
-    }
-    const ctr_mlp_options& o = m->opts;
-    const bool sgd = o.solver == CTR_MLP_SOLVER_SGD;
-    MCU(m, cudaMemsetAsync(m->ms, 0, sizeof(double) * (size_t)m->np, m->stream));        // a fresh optimizer per fit (:731-752)
-    MCU(m, cudaMemsetAsync(m->vs, 0, sizeof(double) * (size_t)m->np, m->stream));
-    m->adam_calls = 0;
-    double sgd_lr = c.lr_init;                                           // SGDOptimizer64.LearningRate
-    std::vector<long> idx((size_t)n);
-    for (int64_t i = 0; i < n; i++) idx[(size_t)i] = i;
-    double lr_init = c.lr_init, lr_last = c.lr_init, best = INFINITY;
-    int no_improve = 0, it = 0;
-    const int L = m->d.n_layers;
-    for (it = 0; it < c.max_iter;) {
-        if (c.shuffle) {                                                 // rand.Shuffle (:788): Fisher–Yates from the top
-            for (long i = n - 1; i > 0; i--) { const long j = (long)(mix64(c.seed, 100u + (uint32_t)it, (uint64_t)i) % (uint64_t)(i + 1)); std::swap(idx[(size_t)i], idx[(size_t)j]); }
-        }
-        MCU(m, cudaMemcpyAsync(m->idx, idx.data(), sizeof(long) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
-        MCU(m, cudaMemsetAsync(m->scal, 0, 2 * sizeof(double), m->stream));
-        for (long b0 = 0; b0 < n; b0 += bs) {                            // :791-808
-            const int rows = (int)std::min<long>(bs, n - b0);
-            const long* bi = m->idx + b0;
-            if (o.weight_decay > 0.0)                                    // backprop :342-346
-                k_mlp64_decay<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->np, 1.0 - o.weight_decay);
-            mlp_forward(m, bi, 0, rows);
-            k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], m->Y32, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
-            for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
-                k_mlp64_grads<<<mlp_grid(m, (long)(m->d.units[l] + 1) * m->d.units[l + 1]), 256, 0, m->stream>>>(
-                    m->params, m->grads, m->d, l, m->X64, nin, bi, l == 0 ? nullptr : m->act[l].get(), m->del[l + 1], rows, c.alpha);
-                if (l >= 1) k_mlp64_delta<<<mlp_grid(m, (long)rows * m->d.units[l]), 256, 0, m->stream>>>(m->params, m->d, l, m->act[l], m->del[l + 1], m->del[l], rows);
-            }
-            if (sgd) {
-                k_mlp64_sgd<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->np, sgd_lr, o.momentum, o.nesterov);
-            } else {
-                k_mlp64_adam<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->grads, m->ms, m->vs, m->np, m->adam_calls, lr_init, c.beta1, c.beta2, c.eps);
-                m->adam_calls += 1;
-            }
-        }
-        it++;
-        double sc[2] = {0, 0};
-        MCU(m, cudaMemcpyAsync(sc, m->scal, sizeof sc, cudaMemcpyDeviceToHost, m->stream));
-        MCU(m, cudaStreamSynchronize(m->stream));
-        MCU(m, cudaGetLastError());
-        const double loss = sc[1] / (double)n;                           // :810-811
-        m->t += (double)n;                                               // :814
-        if (loss_curve) loss_curve[it - 1] = loss;
-        if (!sgd) {   // the learning rate the optimizer last used (:1088): decides "adaptive" stopping (:1059-1064)
-            const double e = m->adam_calls * (double)m->np;
-            lr_last = lr_init * std::sqrt(1.0 - std::pow(c.beta2, e)) / (1.0 - std::pow(c.beta1, e));
-        }
-        if (loss > best - c.tol) no_improve++; else no_improve = 0;      // :886-892
-        if (loss < best) best = loss;
-        if (sgd && o.lr_schedule == CTR_MLP_LR_INVSCALING)               // iterationEnds :999-1003 (Adam's is a no-op, :1053)
-            sgd_lr = c.lr_init / std::pow(m->t + 1.0, o.power_t);
-        if (no_improve > c.n_iter_no_change) {                           // :826-840
-            if (o.lr_schedule != CTR_MLP_LR_ADAPTIVE) break;             // triggerStopping :1005-1011, :1054-1060
-            if ((sgd ? sgd_lr : lr_last) <= 1e-6) break;                 // :1012-1017, :1061-1066
-            if (sgd) sgd_lr *= .8;                                       // :1018 — the current rate
-            else lr_init *= .8;                                          // :1067 — the base rate
-            no_improve = 0;
-        }
-    }
-    if (n_iter) *n_iter = it;
-    m->fitted = true;
-    return CTR_OK;
+    RET(mlp_init_params(m));
+    return mlp_epochs(m, n, bs, m->Y32, MlpInput(), n_iter, loss_curve);
 }
 
 int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float* out) {
@@ -3023,12 +3085,161 @@ int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float*
     int rc = CTR_OK;
     for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predictProbas :897-931: raw probabilities for the f64 class
         const int rows = (int)std::min<long>(chunk, n - r0);
-        mlp_forward(m, nullptr, r0, rows);
+        mlp_forward(m, m->X64 + r0 * nin, nullptr, rows);
         k_f64_to_f32<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], d_out, rows);
         if (cudaMemcpyAsync(out + r0, d_out, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, m->stream) != cudaSuccess ||
             cudaStreamSynchronize(m->stream) != cudaSuccess) rc = mlp_err(m, CTR_ECUDA, "predict: %s", cudaGetErrorString(cudaGetLastError()));
     }
     return rc;
+}
+
+// ---- the MLP fed by sample keys from a feature store (ctr_mlp_fit_keys / ctr_mlp_predict_keys) -------------
+namespace {
+// the refusals shared by both calls; h->mu and m->mu are held, m's device is made current
+int mlp_keys_check(ctr_mlp* m, ctr_handle* h) {
+    const ctr_config& c = h->cfg;
+    const long width = (long)c.uP + (long)c.S * c.D + c.D + c.cF;
+    if (m->dev != h->dev) return mlp_err(m, CTR_EINVAL, "the classifier is on device %d, the feature store on device %d", m->dev, h->dev);
+    if (m->d.units[0] != width)
+        return mlp_err(m, CTR_EINVAL, "the network has %d inputs, the feature store's samples uP + S*D + D + cF = %ld columns", m->d.units[0], width);
+    if (h->comm.world > 1) return mlp_err(m, CTR_ESTATE, "the key-fed MLP needs a single-GPU feature store (world=%d)", h->comm.world);
+    if (!h->idm_keys[0] || !h->idm_keys[1]) return mlp_err(m, CTR_ESTATE, "the key-fed MLP needs both id maps of the feature store (ctr_idmap_build)");
+    RET(check_tables(h));
+    MCU(m, cudaSetDevice(m->dev));
+    return CTR_OK;
+}
+// every exit of a key-fed call: no work of m may still read h's buffers, and the message is readable from both objects
+int mlp_keys_done(ctr_mlp* m, ctr_handle* h, int rc) {
+    if (m->dev == h->dev) {
+        cudaSetDevice(m->dev);
+        const cudaError_t e1 = cudaStreamSynchronize(m->stream), e2 = cudaStreamSynchronize(h->stream);
+        if (rc == CTR_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = mlp_err(m, CTR_ECUDA, "key-fed MLP: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    if (rc != CTR_OK) { if (m->err.empty()) m->err = h->err; else h->err = m->err; }
+    return rc;
+}
+// h's stream has queued what m's stream must see: m's stream waits for it (no host round trip)
+int mlp_after_store(ctr_mlp* m, ctr_handle* h, int slot) {
+    MCU(m, cudaEventRecord(m->stage_full[slot], h->stream));
+    MCU(m, cudaStreamWaitEvent(m->stream, m->stage_full[slot], 0));
+    return CTR_OK;
+}
+
+int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label, int64_t n,
+                 int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    const int S = h->cfg.S;
+    // ---- GetSample's resolution, as in ctr_train_keys: survivors resident in kt_*, input order kept
+    RET(feed_init(h));
+    const size_t chunk = std::min<size_t>((size_t)n, h->feed_bytes / 28);
+    RET(keys_prepare(h, (size_t)n, chunk));
+    cudaStream_t rs = h->copy_stream;
+    const int64_t nchunks = (n + (int64_t)chunk - 1) / (int64_t)chunk;
+    for (int64_t c = 0; c < nchunks; c++) RET(keys_resolve_chunk(h, c, chunk, user_ids, item_ids, ts, label, n, rs));
+    unsigned long long used = 0;
+    CU(h, cudaMemcpyAsync(&used, h->kt_count, sizeof used, cudaMemcpyDeviceToHost, rs));
+    CU(h, cudaStreamSynchronize(rs));
+    if (rows_used) *rows_used = (int64_t)used;
+    if (used == 0) return mlp_err(m, CTR_ENOTFOUND, "no sample resolved: every key has an unknown user or item");
+    const long ns = (long)used;
+    // ---- every survivor's history, GetUserBehavior(uid, S, -1, ts), cut once: h->mu is held, so the cache stays as it is
+    RET(reserve(h, h->kt_hist_all, (size_t)ns * S, false));
+    if (h->ub_off) {
+        RET(launch(h, "ubcache_window", [&] {
+            k_ub_window<<<grid_for_warps(h, (int)ns), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->kt_user, h->kt_ts, (int)ns, S,
+                                                                           (long)h->ub_users, h->kt_hist_all);
+        }));
+    } else CU(h, cudaMemsetAsync(h->kt_hist_all, 0xff, sizeof(int) * (size_t)ns * S, h->stream));   // no UserBehavior provider → empty history
+    // ---- the classifier: minibatch k's rows are gathered on h's stream into stage[k & 1] while minibatch k-1 trains
+    const long bs = mlp_batch(m, ns);
+    if (m->idx.size() < (size_t)ns) MCU(m, m->idx.alloc((size_t)ns));
+    RET(mlp_rows(m, bs));
+    RET(mlp_stage(m, bs));
+    RET(mlp_after_store(m, h, 0));                                     // labels and windows before the first loss
+    RET(mlp_init_params(m));
+    const RowSrc r = idx_src(h, h->kt_user, h->kt_item, h->kt_hist_all, (int)ns);
+    const int nin = m->d.units[0];
+    auto input = [&](long k, const long* bi, int rows, const double** X) -> int {
+        const int s = (int)(k & 1);
+        // stage[(k+1) & 1] was last read by minibatch k-1, the last one queued on m's stream; at k == 0 both buffers are
+        // free once the epoch's index upload is done
+        if (k == 0) MCU(m, cudaEventRecord(m->stage_free[0], m->stream));
+        MCU(m, cudaEventRecord(m->stage_free[(k + 1) & 1], m->stream));
+        MCU(m, cudaStreamWaitEvent(h->stream, m->stage_free[s], 0));
+        RET(launch(h, "mlp_gather", [&] {
+            k_gather_rows<<<grid_for_warps(h, rows), 256, 0, h->stream>>>(r, dims_of(h), m->stage[s].get(), (long)nin, rows, RowsByIdx{bi});
+        }));
+        RET(mlp_after_store(m, h, s));
+        *X = m->stage[s];
+        return CTR_OK;
+    };
+    return mlp_epochs(m, ns, bs, h->kt_label, input, n_iter, loss_curve);
+}
+
+int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
+    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
+    const int B = h->cfg.pred_batch, S = h->cfg.S, nin = m->d.units[0], L = m->d.n_layers;
+    RET(keys_stage_init(h));
+    RET(mlp_rows(m, B));
+    RET(mlp_stage(m, B));
+    DevBuf<float> d_out;
+    MCU(m, d_out.alloc((size_t)B));
+    long long* hk = (long long*)h->k_host.get();
+    float* hs = (float*)(hk + (size_t)3 * B);
+    int* hfirst = (int*)(hs + B);
+    for (int64_t s = 0; s < n; s += B) {
+        const int nb = (int)std::min<int64_t>(B, n - s);
+        memcpy(hk, user_ids + s, sizeof(long long) * (size_t)nb);
+        memcpy(hk + nb, item_ids + s, sizeof(long long) * (size_t)nb);
+        memcpy(hk + 2 * (size_t)nb, ts + s, sizeof(long long) * (size_t)nb);
+        CU(h, cudaMemcpyAsync(h->k_keys, hk, sizeof(long long) * (size_t)3 * nb, cudaMemcpyHostToDevice, h->stream));
+        // BatchPredict's resolution (rcmd.go:277-337): an unknown key → user, item and history rows -1 → an all-zero X row
+        RET(launch(h, "keys_resolve", [&] {
+            k_keys_resolve<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, h->idm_keys[1], h->idm_vals[1], h->idm_keys[1].size() - 1,
+                                                                    h->ub_off, h->ub_ts, h->ub_items, (long)h->ub_users, h->k_keys, nb, S, h->s_user, h->s_item, h->s_hist);
+        }));
+        if (s == 0) CU(h, cudaMemcpyAsync(hfirst, h->s_user, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        const RowSrc r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+        RET(launch(h, "mlp_gather", [&] {
+            k_gather_rows<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), m->stage[0].get(), (long)nin, nb, RowsAsIs{});
+        }));
+        RET(mlp_after_store(m, h, 0));
+        mlp_forward(m, m->stage[0], nullptr, nb);
+        k_f64_to_f32<<<mlp_grid(m, nb), 256, 0, m->stream>>>(m->act[L - 1], d_out, nb);
+        MCU(m, cudaMemcpyAsync(hs, d_out, sizeof(float) * (size_t)nb, cudaMemcpyDeviceToHost, m->stream));
+        MCU(m, cudaStreamSynchronize(m->stream));                      // the next chunk's gather overwrites stage[0]
+        CU(h, cudaStreamSynchronize(h->stream));
+        // rcmd.go:300-303: an unresolvable FIRST key is an error, later ones become zero rows
+        if (s == 0 && *hfirst < 0)
+            return mlp_err(m, CTR_ENOTFOUND, "get sample vector error: user %lld or item %lld has no features", (long long)user_ids[0], (long long)item_ids[0]);
+        memcpy(scores + s, hs, sizeof(float) * (size_t)nb);
+    }
+    return CTR_OK;
+}
+}  // namespace
+
+int ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label,
+                     int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    if (!m) return CTR_EINVAL;
+    if (!h || !user_ids || !item_ids || !ts || !label || n < 1 || n > INT32_MAX)
+        return mlp_err(m, CTR_EINVAL, "bad fit_keys arguments (n in [1, 2^31))");
+    std::lock_guard<std::mutex> lh(h->mu);                           // the feature store first, then the classifier
+    std::lock_guard<std::mutex> lm(m->mu);
+    m->err.clear(); h->err.clear();
+    int rc = mlp_keys_check(m, h);
+    if (rc == CTR_OK) rc = mlp_fit_keys(m, h, user_ids, item_ids, ts, label, n, n_iter, loss_curve, rows_used);
+    return mlp_keys_done(m, h, rc);
+}
+
+int ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
+    if (!m) return CTR_EINVAL;
+    if (!h || !user_ids || !item_ids || !ts || !scores || n < 1) return mlp_err(m, CTR_EINVAL, "bad predict_keys arguments");
+    std::lock_guard<std::mutex> lh(h->mu);
+    std::lock_guard<std::mutex> lm(m->mu);
+    m->err.clear(); h->err.clear();
+    int rc = mlp_keys_check(m, h);
+    if (rc == CTR_OK) rc = mlp_predict_keys(m, h, user_ids, item_ids, ts, n, scores);
+    return mlp_keys_done(m, h, rc);
 }
 
 int ctr_comm_unique_id(void* id_out, int32_t* id_bytes) { return comm_unique_id(id_out, id_bytes); }

@@ -29,7 +29,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
-           "ctr_mlp_get_params", "ctr_mlp_set_params"]
+           "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys"]
 
 
 class CtrError(RuntimeError):
@@ -488,7 +488,7 @@ class MLPClassifier:
         rc = self.L.ctr_mlp_create_ex(C.byref(cfg), C.byref(opts), C.byref(self.h))
         if rc != 0:
             raise CtrError(rc, self.L.ctr_mlp_last_error(None).decode())
-        self.n_iter = 0; self.loss_curve = np.zeros(0)
+        self.n_iter = 0; self.loss_curve = np.zeros(0); self.rows_used = 0
 
     def _ck(self, rc):
         if rc != 0:
@@ -515,6 +515,36 @@ class MLPClassifier:
         Xa, Xp = _f(X)
         out = np.empty(Xa.shape[0], np.float32)
         self._ck(self.L.ctr_mlp_predict(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), out.ctypes.data_as(_fp)))
+        return out
+
+    @staticmethod
+    def _keys(user_ids, item_ids, ts):
+        u = np.ascontiguousarray(user_ids, np.int64); i = np.ascontiguousarray(item_ids, np.int64); t = np.ascontiguousarray(ts, np.int64)
+        if not u.size == i.size == t.size:
+            raise ValueError("user_ids, item_ids and ts differ in length: %d, %d, %d" % (u.size, i.size, t.size))
+        return u, i, t
+
+    def fit_keys(self, engine, user_ids, item_ids, ts, label):
+        """recommend.Train with SimpleMlpFitWrap over sample keys (ctr_mlp_fit_keys): `engine` is the feature store (id
+        maps, tables, optional ubcache).  Keys with an unknown user or item are dropped; sets n_iter, loss_curve and
+        rows_used (the surviving samples).  Bit-identical to fit() on the rows engine.gather_rows builds for the survivors."""
+        u, i, t = self._keys(user_ids, item_ids, ts)
+        y, yp = _f(label)
+        if y.size != u.size:
+            raise ValueError("label has %d entries for %d keys" % (y.size, u.size))
+        it = C.c_int32(0); used = C.c_int64(0); curve = np.zeros(self.cfg.max_iter, np.float64)
+        self._ck(self.L.ctr_mlp_fit_keys(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp), yp,
+                                         C.c_int64(u.size), C.byref(it), curve.ctypes.data_as(C.POINTER(C.c_double)), C.byref(used)))
+        self.n_iter = it.value; self.loss_curve = curve[:it.value]; self.rows_used = used.value
+        return self
+
+    def predict_keys(self, engine, user_ids, item_ids, ts):
+        """recommend.BatchPredict for the MLP over sample keys (ctr_mlp_predict_keys) → float32 [n].  An unknown key
+        scores as an all-zero row, except key 0, which raises CtrError with code ENOTFOUND."""
+        u, i, t = self._keys(user_ids, item_ids, ts)
+        out = np.empty(u.size, np.float32)
+        self._ck(self.L.ctr_mlp_predict_keys(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
+                                             C.c_int64(u.size), out.ctypes.data_as(_fp)))
         return out
 
     def get_params(self):

@@ -220,12 +220,21 @@ class YoutubeDnnImpl(_Impl):
 class SimpleMlpPredWrap:
     """model/mlp/mlp.go:11-39: PredictAbstract over the fitted classifier — float32 X in, float32 [n, 1] out."""
 
-    def __init__(self, pred):
+    def __init__(self, pred, engine=None):
         self.pred = pred
+        self.engine = engine          # the feature store of FitKeys: serves batch_predict_keys
 
     def Predict(self, X):
         X = np.asarray(X, np.float32)
         return self.pred.predict(X).reshape(-1, 1)
+
+    def batch_predict_keys(self, user_ids, item_ids, ts):
+        """Scores sample keys through the bound feature store (ctr_mlp_predict_keys), so serving.BatchPredict and
+        serving.Rank serve the MLP as they serve an engine.  serving.Recommend over the whole item table is not
+        available for the MLP: it needs the engine's own model."""
+        if self.engine is None:
+            raise RuntimeError("this predictor was fitted from dense X: no feature store is bound (use FitKeys)")
+        return self.pred.predict_keys(self.engine, user_ids, item_ids, ts)
 
 
 class SimpleMlpFitWrap:
@@ -242,6 +251,16 @@ class SimpleMlpFitWrap:
         self.Model = _e.MLPClassifier(trainSample.XCols, **self.mlp_kw)
         self.Model.fit(X, Y)
         return SimpleMlpPredWrap(self.Model)
+
+    def FitKeys(self, engine, user_ids, item_ids, ts, label):
+        """rcmd.Train (rcmd.go:197-246) with this fitter, GetSample on the device: `engine` holds the id maps, the tables
+        and optionally the ubcache; the sample width is its uP + S·D + D + cF.  Keys with an unknown user or item are
+        dropped (Model.rows_used counts the rest).  Returns a SimpleMlpPredWrap bound to `engine`, which
+        serving.BatchPredict / serving.Rank accept in place of an engine; serving.Recommend does not serve the MLP."""
+        c = engine.cfg
+        self.Model = _e.MLPClassifier(c.uP + c.S * c.D + c.D + c.cF, **self.mlp_kw)
+        self.Model.fit_keys(engine, user_ids, item_ids, ts, label)
+        return SimpleMlpPredWrap(self.Model, engine)
 
 
 def RocAuc32(pred, y, engine=None):

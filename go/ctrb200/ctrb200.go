@@ -23,6 +23,7 @@ import (
 	"encoding/json"
 	"fmt"
 	"runtime"
+	"time"
 	"unsafe"
 
 	rcmd "github.com/auxten/go-ctr/recommend"
@@ -474,9 +475,10 @@ type MlpPredWrap struct {
 	xcols int
 }
 
-func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, error) {
+// create maps the options onto a classifier of xcols inputs, or refuses what the engine does not build.
+func (f *MlpFitWrap) create(xcols int) (*C.ctr_mlp, error) {
 	var cfg C.ctr_mlp_config
-	C.ctr_mlp_config_default(&cfg, C.int32_t(trainSample.XCols))
+	C.ctr_mlp_config_default(&cfg, C.int32_t(xcols))
 	if len(f.Hidden) > 0 {
 		cfg.n_layers = C.int32_t(len(f.Hidden) + 2)
 		for i, u := range f.Hidden {
@@ -556,6 +558,14 @@ func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, e
 	if rc := C.ctr_mlp_create_ex(&cfg, &opts, &m); rc != C.CTR_OK {
 		return nil, fmt.Errorf("ctr_mlp_create_ex: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(nil)))
 	}
+	return m, nil
+}
+
+func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, error) {
+	m, err := f.create(trainSample.XCols)
+	if err != nil {
+		return nil, err
+	}
 	var iters C.int32_t
 	if rc := C.ctr_mlp_fit(m, f32(trainSample.X), f32(trainSample.Y), C.int64_t(trainSample.Rows), C.int32_t(trainSample.XCols), &iters, nil); rc != C.CTR_OK {
 		err := fmt.Errorf("ctr_mlp_fit: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(m)))
@@ -575,4 +585,71 @@ func (p *MlpPredWrap) Predict(X tensor.Tensor) tensor.Tensor {
 		return nil
 	}
 	return tensor.NewDense(tensor.Float32, tensor.Shape{n, 1}, tensor.WithBacking(y))
+}
+
+// FitKeys is rcmd.Train (rcmd.go:197-246) with this fitter, with GetSample (rcmd.go:339-460) on the device: e is the
+// feature store (id maps, tables, optional ubcache), samples are its keys.  Samples whose user or item is unknown are
+// dropped; rowsUsed counts the rest.  The classifier has e's uP + S·D + D + cF inputs and trains bit for bit as Fit
+// would on the rows GetSample builds.  The options and refusals are Fit's.  The predictor serves keys through e.
+func (f *MlpFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
+	n := len(samples)
+	if n == 0 {
+		return nil, 0, fmt.Errorf("MlpFitWrap.FitKeys: no samples")
+	}
+	xcols := int(e.cfg.uP + e.cfg.S*e.cfg.D + e.cfg.D + e.cfg.cF)
+	m, err := f.create(xcols)
+	if err != nil {
+		return nil, 0, err
+	}
+	u, it, ts, y := make([]int64, n), make([]int64, n), make([]int64, n), make([]float32, n)
+	for i, s := range samples {
+		u[i], it[i], ts[i], y[i] = int64(s.UserId), int64(s.ItemId), s.Timestamp, s.Label
+	}
+	var iters C.int32_t
+	var used C.int64_t
+	if rc := C.ctr_mlp_fit_keys(m, e.h, i64(u), i64(it), i64(ts), f32(y), C.int64_t(n), &iters, nil, &used); rc != C.CTR_OK {
+		err := fmt.Errorf("ctr_mlp_fit_keys: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(m)))
+		C.ctr_mlp_destroy(m)
+		return nil, int64(used), err
+	}
+	p := &MlpPredWrap{m: m, xcols: xcols}
+	runtime.SetFinalizer(p, func(p *MlpPredWrap) { C.ctr_mlp_destroy(p.m) })
+	return p, int64(used), nil
+}
+
+// BatchPredict is recommend.BatchPredict (rcmd.go:277-337) for the MLP over the feature store e: an unknown key scores
+// as an all-zero row, except key 0, which is an error.
+func (p *MlpPredWrap) BatchPredict(e *Engine, sampleKeys []rcmd.Sample) ([]float32, error) {
+	n := len(sampleKeys)
+	if n == 0 {
+		return nil, fmt.Errorf("MlpPredWrap.BatchPredict: no sample keys")
+	}
+	u, it, ts := make([]int64, n), make([]int64, n), make([]int64, n)
+	for i, k := range sampleKeys {
+		u[i], it[i], ts[i] = int64(k.UserId), int64(k.ItemId), k.Timestamp
+	}
+	y := make([]float32, n)
+	if rc := C.ctr_mlp_predict_keys(p.m, e.h, i64(u), i64(it), i64(ts), C.int64_t(n), f32(y)); rc != C.CTR_OK {
+		return nil, fmt.Errorf("ctr_mlp_predict_keys: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+	}
+	return y, nil
+}
+
+// Rank is recommend.Rank (rcmd.go:248-275) for the MLP: itemIds scored for one user at the current time, in the
+// caller's order.
+func (p *MlpPredWrap) Rank(e *Engine, userId int, itemIds []int) ([]rcmd.ItemScore, error) {
+	now := time.Now().Unix()
+	keys := make([]rcmd.Sample, len(itemIds))
+	for i, id := range itemIds {
+		keys[i] = rcmd.Sample{UserId: userId, ItemId: id, Timestamp: now}
+	}
+	y, err := p.BatchPredict(e, keys)
+	if err != nil {
+		return nil, err
+	}
+	out := make([]rcmd.ItemScore, len(itemIds))
+	for i, id := range itemIds {
+		out[i] = rcmd.ItemScore{ItemId: id, Score: y[i]}
+	}
+	return out, nil
 }

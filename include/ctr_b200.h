@@ -418,6 +418,30 @@ int  ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t 
 /* SimpleMlpPredWrap.Predict (mlp.go:15-39): probabilities as float32 [n] (the 64-bit class returns them raw,
  * basemlp64.go:897-931). */
 int  ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float* out);
+/* The classifier fed by sample keys {UserId, ItemId, Timestamp, Label} from a feature store: no X on the host.  The
+ * handle h is used only as the feature store — its id maps, USER_FEAT / ITEM_EMB / ITEM_FEAT tables, optional device
+ * ubcache and uP, S, D, cF; its model kind and dense weights are not used.  m->units[0] must equal uP + S·D + D + cF.
+ * fit: recommend.Train (rcmd.go:197-246) with mlp.SimpleMlpFitWrap — GetSample (rcmd.go:339-460) on the device, then
+ *   ctr_mlp_fit.  Samples resolve as in ctr_train_keys: a key whose user or item is unknown is dropped, order kept; each
+ *   survivor's history is GetUserBehavior(uid, S, -1, ts) from the ubcache (empty without one).  The classifier then
+ *   trains on the survivors exactly as ctr_mlp_fit would on the X ctr_gather_rows builds for them, bit for bit: init
+ *   or warm start, minibatches clipped to the survivor count, the shuffle over the survivors, solvers, weight decay,
+ *   stopping rules and the t carry.  Each minibatch's float64 rows are gathered on the device into a [batch, nin]
+ *   buffer the classifier owns; resident cost is about (S + 7)·4 bytes per survivor instead of nin·8.  *rows_used
+ *   (may be NULL) = survivors; none is CTR_ENOTFOUND with the parameters untouched.  n in [1, 2^31).
+ * predict: recommend.BatchPredict / Rank (rcmd.go:248-337) with model/mlp: keys → probabilities scores [n], in
+ *   chunks of h's pred_batch, history windowed at each key's ts.  An unknown key scores as an all-zero X row, unless
+ *   it is key 0, which fails the call with CTR_ENOTFOUND (rcmd.go:300-303).
+ * Refusals change nothing: CTR_EINVAL for null or short arguments, a width mismatch, or m and h on different devices;
+ * CTR_ESTATE for a missing id map, missing tables, h with world > 1 (sharded feature stores are not served), and
+ * predict before any fit or ctr_mlp_set_params.  The message is readable through both ctr_mlp_last_error(m) and
+ * ctr_last_error(h).
+ * Locking: both calls take h's mutex, then m's.  A caller that holds either object's lock across calls must take
+ * them in the same order. */
+int  ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
+                      const float* label, int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used);
+int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
+                          int64_t n, float* scores);
 /* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the length */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
