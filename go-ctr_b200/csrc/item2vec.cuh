@@ -17,7 +17,12 @@
 // than summed — top Huffman nodes (p = subtree frequency) and very frequent context items are damped,
 // rare nodes and items (C*p < 1) get the exact update.  C itself is kept proportional to the vocabulary
 // (small corpora run almost sequentially).  Deliberate adaptation to 10^3..10^5-way concurrency; quality is
-// checked against the sequential float64 oracle (tests/test_gpu_i2v.py).
+// checked against the sequential float64 oracle (tests/test_gpu_i2v.py), the arithmetic of this kernel against a
+// float64 model of one launch at every vector width (tests/test_gpu_i2v_kernel.py).
+//
+// What one warp sees of its own updates (measured on H100, tests/test_gpu_i2v_kernel.py tier A at D = 128): the
+// contexts of one pass read the same node vectors; a later pass of the same centre reads the red.add of the earlier
+// pass (same thread, same address), except for hot nodes, whose updates wait in shared memory until the next flush.
 #pragma once
 #include "common.cuh"
 
@@ -93,7 +98,9 @@ k_i2v_skipgram_hs(I2vArgs a) {
                     const float f = group_sum<LPR>(dot4(c, nv));
                     if (alive && (f <= -6.0f || f >= 6.0f)) alive = false;      // `return`: the rest of the path is abandoned
                     if (alive) {
-                        const float g = (1.0f - (float)a.pcode[p0 + i] - c_i2v_lut[(int)((f + 6.0f) * (1000.0f / 6.0f / 2.0f))]) * lr;
+                        // clamped: in float32 f = nextafterf(6, 0) rounds f + 6 up to 12 and the product to 1000, one past the table
+                        const int bin = min((int)((f + 6.0f) * (1000.0f / 6.0f / 2.0f)), 999);
+                        const float g = (1.0f - (float)a.pcode[p0 + i] - c_i2v_lut[bin]) * lr;
                         tmp = fma4(g, nv, tmp);
                         const float gs = g * __ldg(a.node_scale + node);
                         const int hs = node - a.hot_base;
@@ -138,9 +145,10 @@ k_i2v_skipgram_hs(I2vArgs a) {
 // would run it (word2vec.go:198-221, model.go:48-78, optimizer.go:107-129), operation for operation: the dot product
 // is accumulated in element order, multiplications and additions are rounded separately (the CPU restatement is
 // built without FMA contraction), the sigmoid comes from the same 1000-entry table.  It exists for PARITY: on the same
-// tokens it reproduces oracle/i2v_oracle.c bit for bit (tests/test_gpu_i2v.py), which pins the device-side dictionary
-// filter, subsampling draws, window draws, Huffman paths, learning-rate schedule and update rule that the parallel
-// kernel above shares.  Throughput is irrelevant here (~10^5 tokens/s).
+// tokens it reproduces oracle/i2v_oracle.c bit for bit (tests/test_gpu_i2v.py), which pins the host plan both kernels
+// are given: the device-side dictionary filter, subsample thresholds, Huffman paths and learning-rate schedule.  The
+// parallel kernel above shares no code with this one below that plan; its own draws, window enumeration and update
+// arithmetic are pinned by tests/test_gpu_i2v_kernel.py.  Throughput is irrelevant here (~10^5 tokens/s).
 // -------------------------------------------------------------------------------------------------------------------
 struct I2vSeqArgs {
     const int* doc; long nd; long n_stream;

@@ -60,8 +60,9 @@ def test_train_embedding_mirror_and_dims():
 def test_sequential_float64_mode_reproduces_the_oracle_bit_for_bit(dim):
     """cfg.reserved[0] = 1: one warp walks the document in order with float64 tables — the reference's algorithm as a
     single goroutine runs it (word2vec.go:198-221, model.go:48-78, optimizer.go:107-129).  Same tokens, same counter-RNG
-    draws: the embeddings equal oracle/i2v_oracle.c's exactly, which pins the MinCount filter, subsampling, window
-    draws, Huffman paths, lr schedule and update rule the parallel kernel shares."""
+    draws: the embeddings equal oracle/i2v_oracle.c's exactly, which pins the MinCount filter, subsample thresholds,
+    Huffman paths and lr schedule of the host plan both kernels are given.  The parallel kernel's own draws, window
+    enumeration and update arithmetic are checked in tests/test_gpu_i2v_kernel.py."""
     rng = np.random.default_rng(12)
     toks, remap, nc, per = planted_corpus(rng, n_clusters=5, per=8, n_users=60, seq=40)
     V = nc * per + 3
