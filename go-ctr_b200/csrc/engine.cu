@@ -16,6 +16,7 @@
 
 #include <nvtx3/nvToolsExt.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
@@ -867,6 +868,15 @@ int table_mem(ctr_handle* h, int which, bool shard, size_t bytes) {
     CU(h, cudaMemsetAsync(h->tab[which], 0, bytes, h->stream));
     return CTR_OK;
 }
+// what new contents of a table reset, whether it was reallocated (table_alloc) or rewritten in place (ctr_item_emb_train)
+void table_new_state(ctr_handle* h, int which) {
+    if (which == CTR_TABLE_ITEM_EMB) {
+        h->comm.replicate = h->comm.world > 1 && !h->tab_sharded[which];
+        if (h->hot_acc) { h->hot_acc.reset(); h->hot_rows = 0; }
+        h->emb_m.reset(); h->emb_v.reset();                       // a new table starts a new solver state
+    }
+    if (which != CTR_TABLE_USER_FEAT) h->tab_gen++;           // peers hold mappings of the old allocation
+}
 int table_alloc(ctr_handle* h, int which, int64_t nrows, int32_t width) {
     const long ld = round_up(width, 4);                       // 16-byte aligned rows for 128-bit loads
     const bool shard = table_sharded(h, which, nrows, width);
@@ -875,12 +885,7 @@ int table_alloc(ctr_handle* h, int which, int64_t nrows, int32_t width) {
     RET(table_mem(h, which, shard, bytes));
     h->tab_ld[which] = ld; h->tab_rows[which] = nrows; h->tab_local_rows[which] = local; h->tab_width[which] = width;
     h->tab_sharded[which] = shard;
-    if (which == CTR_TABLE_ITEM_EMB) {
-        h->comm.replicate = h->comm.world > 1 && !shard;
-        if (h->hot_acc) { h->hot_acc.reset(); h->hot_rows = 0; }
-        h->emb_m.reset(); h->emb_v.reset();                       // a new table starts a new solver state
-    }
-    if (which != CTR_TABLE_USER_FEAT) h->tab_gen++;           // peers hold mappings of the old allocation
+    table_new_state(h, which);
     return CTR_OK;
 }
 
@@ -2576,38 +2581,38 @@ struct I2vDist { int rank = 0, world = 1; void* nccl = nullptr; long sync_every 
 // both vector tables; dictionary counts are all-reduced (identical tree everywhere) and the replicas are averaged
 // every sync_every positions (local SGD / model averaging — the reference's own trainer is Hogwild over goroutines,
 // word2vec.go:165-169; across GPUs the racy shared memory becomes periodic averaging).
-int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, int32_t V, float* emb_out, ctr_i2v_stats* stats, I2vDist* dist) {
-    if (!cfg || !tokens || (!emb_out && !dist) || n < 1 || V < 2 || n > 0x7fffffffLL) return set_err(nullptr, CTR_EINVAL, "bad item2vec arguments");
-    const ctr_i2v_config& c = *cfg;
+int i2v_check_cfg(const ctr_i2v_config& c, const ctr_handle* eh) {
+    if (c.dim < 4 || c.dim > 128 || (c.dim & (c.dim - 1)) || c.window < 1 || c.iter < 1 || c.max_depth < 2 || c.update_lr_batch < 1)
+        return set_err(eh, CTR_EINVAL, "item2vec: dim must be a power of two in [4,128], window/iter >= 1");
+    return CTR_OK;
+}
+
+// The trainer proper, from a device-resident word-id document d_tok [n] (ids in [0, V), corpus order) on stream st:
+// leaves the trained float32 syn0 [V, D] in d_syn0 on the device.  The same document trains the same whether it came
+// from the host (ctr_i2v_train) or was numbered on the device (ctr_item_emb_train).  Errors are reported on eh
+// (nullptr: the stand-alone entry points).
+int i2v_train_dev(const ctr_i2v_config& c, const int* d_tok, int64_t n, int32_t V, int num_sms, cudaStream_t st, DevBuf<float>& d_syn0,
+                  ctr_i2v_stats* stats, I2vDist* dist, const ctr_handle* eh) {
     const int D = c.dim, W = c.window;
-    if (D < 4 || D > 128 || (D & (D - 1)) || W < 1 || c.iter < 1 || c.max_depth < 2 || c.update_lr_batch < 1)
-        return set_err(nullptr, CTR_EINVAL, "item2vec: dim must be a power of two in [4,128], window/iter >= 1");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_err(nullptr, CTR_ENODEV, "no CUDA device: this engine has no CPU fallback"); }
     const int world = dist ? dist->world : 1;
     const bool seq = c.reserved[0] == 1;
-    if (seq && world > 1) return set_err(nullptr, CTR_EINVAL, "the sequential float64 mode is single-GPU");
-#define CI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return set_err(nullptr, CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
-#define CN(call) do { int r_ = (call); if (r_ != 0) return set_err(nullptr, CTR_ECOMM, "%s: %s", #call, g_nccl.GetErrorString(r_)); } while (0)
-    // declared first, destroyed last: every buffer below is freed before the stream and the events
-    Stream st; Event e0, e1;
-    DevBuf<int> d_tok, d_doc, d_pnode, d_sid, d_sid2, d_parent, d_bad;
+#define CI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return set_err(eh, CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
+#define CN(call) do { int r_ = (call); if (r_ != 0) return set_err(eh, CTR_ECOMM, "%s: %s", #call, g_nccl.GetErrorString(r_)); } while (0)
+    // declared first, destroyed last: every buffer below is freed before the events
+    Event e0, e1;
+    DevBuf<int> d_doc, d_pnode, d_sid, d_sid2, d_parent, d_bad;
     DevBuf<unsigned long long> d_cnt64, d_skey, d_skey2, d_ctr, d_misc;
     DevBuf<unsigned char> d_keep, d_pcode, d_code, d_tmp;
     DevBuf<long long> d_poff, d_nval; DevBuf<long> d_nd;
-    DevBuf<double> d_z; DevBuf<float> d_syn0, d_syn1, d_lr, d_nsc, d_wsc;
+    DevBuf<double> d_z; DevBuf<float> d_syn1, d_lr, d_nsc, d_wsc;
     size_t tmp_bytes = 0;
     float ms_total = 0; int launches = 0; unsigned long long hc[3] = {0, 0, 0};
-    CI(cudaSetDevice(c.device));
-    cudaDeviceProp prop{}; CI(cudaGetDeviceProperties(&prop, c.device));
-    if (prop.major != 9) return set_err(nullptr, CTR_ENODEV, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
-    const int G = prop.multiProcessorCount * 8;
-    CI(st.create()); CI(e0.create(cudaEventDefault)); CI(e1.create(cudaEventDefault));
+    const int G = num_sms * 8;
+    CI(e0.create(cudaEventDefault)); CI(e1.create(cudaEventDefault));
     // ---- dictionary counts over the whole stream (dictionary.go:70-81), on the device
-    CI(d_tok.alloc((size_t)n)); CI(d_doc.alloc((size_t)n)); CI(d_keep.alloc((size_t)n));
+    CI(d_doc.alloc((size_t)n)); CI(d_keep.alloc((size_t)n));
     CI(d_cnt64.alloc((size_t)V)); CI(d_bad.alloc(1)); CI(d_nd.alloc(1));
     CI(d_misc.alloc(4));
-    CI(big_copy(d_tok, tokens, sizeof(int) * (size_t)n, true, st));
     CI(cudaMemsetAsync(d_cnt64, 0, sizeof(unsigned long long) * (size_t)V, st)); CI(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
     k_i2v_count<<<G, 256, 0, st>>>(d_tok, (long)n, V, d_cnt64, d_bad); launches++;
     unsigned long long n_global = (unsigned long long)n;
@@ -2620,7 +2625,7 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     }
     // ---- the training document: words rarer than MinCount are dropped (memory.go:53-62), order kept
     k_i2v_keep<<<G, 256, 0, st>>>(d_tok, (long)n, d_cnt64, c.min_count, d_keep); launches++;
-    cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_tok.get(), d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st);
+    cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_tok, d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st);
     {
         size_t b2 = 0, b3 = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, b2, d_skey.get(), d_skey2.get(), d_sid.get(), d_sid2.get(), V, 0, 64, st);
@@ -2628,11 +2633,11 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
         tmp_bytes = std::max(tmp_bytes, std::max(b2, b3));
     }
     CI(d_tmp.alloc(tmp_bytes));
-    { size_t tb = tmp_bytes; cub::DeviceSelect::Flagged(d_tmp, tb, d_tok.get(), d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st); launches++; }
+    { size_t tb = tmp_bytes; cub::DeviceSelect::Flagged(d_tmp, tb, d_tok, d_keep.get(), d_doc.get(), d_nd.get(), (int)n, st); launches++; }
     long nd = 0; int bad = 0;
     CI(cudaMemcpyAsync(&nd, d_nd, sizeof nd, cudaMemcpyDeviceToHost, st)); CI(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
     CI(cudaStreamSynchronize(st));
-    if (bad) return set_err(nullptr, CTR_EINVAL, "a token lies outside [0, vocab)");
+    if (bad) return set_err(eh, CTR_EINVAL, "a token lies outside [0, vocab)");
     nd_max_global = nd;
     if (world > 1) {
         unsigned long long v = (unsigned long long)nd;
@@ -2643,7 +2648,7 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     }
     // concurrency: (centre, context) pairs in flight ~ vocabulary / 4, at most the whole machine
     const int rpw = 32 / (D / 4);
-    const long max_warps = (long)prop.multiProcessorCount * 8 * 8;
+    const long max_warps = (long)num_sms * 8 * 8;
     const long warps = std::max<long>(1, std::min<long>(std::min<long>(max_warps, (std::max<long>(nd, 1) + 63) / 64), std::max<long>(1, (long)V / 4 / rpw)));
     const int grid = (int)((warps + 7) / 8);
     const double Ceff = (double)grid * 8 * rpw;
@@ -2660,7 +2665,7 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     // ---- host: the Huffman merge (huffman.go:23-57), O(V)
     std::vector<int> parent; std::vector<unsigned char> code; std::vector<long long> node_val;
     const int n_inner = i2v_huffman_sorted(cnt.data(), leaves.data(), V, parent, code, node_val);
-    if (n_inner < 1) return set_err(nullptr, CTR_EINVAL, "item2vec needs at least two distinct words in the stream");
+    if (n_inner < 1) return set_err(eh, CTR_EINVAL, "item2vec needs at least two distinct words in the stream");
     // ---- paths (node.go:26-43) on the device
     CI(d_parent.alloc(parent.size())); CI(d_code.alloc(code.size())); CI(d_nval.alloc(node_val.size()));
     CI(d_poff.alloc((size_t)V + 1)); CI(d_nsc.alloc(node_val.size()));
@@ -2678,12 +2683,12 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     CI(d_ctr.alloc(3)); CI(cudaMemsetAsync(d_ctr, 0, 3 * sizeof(unsigned long long), st));
     if (seq) {
         // sequential float64 parity mode (item2vec.cuh): one warp, the reference's single-goroutine order
-        DevBuf<double> d64_0, d64_1, d_lut64; DevBuf<float> d_out32;
+        DevBuf<double> d64_0, d64_1, d_lut64;
         std::vector<double> lut64(1000);
         for (int i = 0; i < 1000; i++) { double e = std::exp(((double)i / 1000.0 * 2.0 - 1.0) * 6.0); lut64[(size_t)i] = e / (e + 1.0); }   // sigmoid_table.go:28-45
         cudaError_t e1_ = d64_0.alloc((size_t)V * D), e2_ = d64_1.alloc((size_t)std::max(V - 1, 1) * D),
-                    e3_ = d_lut64.alloc(1000), e4_ = d_out32.alloc((size_t)V * D);
-        if (e1_ != cudaSuccess || e2_ != cudaSuccess || e3_ != cudaSuccess || e4_ != cudaSuccess) return set_err(nullptr, CTR_ENOMEM, "item2vec float64 tables");
+                    e3_ = d_lut64.alloc(1000), e4_ = d_syn0.alloc((size_t)V * D);
+        if (e1_ != cudaSuccess || e2_ != cudaSuccess || e3_ != cudaSuccess || e4_ != cudaSuccess) return set_err(eh, CTR_ENOMEM, "item2vec float64 tables");
         cudaMemcpyAsync(d_lut64, lut64.data(), sizeof(double) * 1000, cudaMemcpyHostToDevice, st);
         cudaMemsetAsync(d64_1, 0, sizeof(double) * (size_t)std::max(V - 1, 1) * D, st);
         k_i2v_init64<<<G, 256, 0, st>>>(d64_0, (long)V * D, D, c.seed); launches++;
@@ -2693,10 +2698,9 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
         cudaEventRecord(e0, st);
         k_i2v_seq_f64<<<1, 32, 0, st>>>(sa); launches++;
         cudaEventRecord(e1, st);
-        k_f64_to_f32_i2v<<<G, 256, 0, st>>>(d64_0, d_out32, (long)V * D); launches++;
-        cudaMemcpyAsync(emb_out, d_out32, sizeof(float) * (size_t)V * D, cudaMemcpyDeviceToHost, st);
+        k_f64_to_f32_i2v<<<G, 256, 0, st>>>(d64_0, d_syn0, (long)V * D); launches++;
         cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st);
-        if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return set_err(nullptr, CTR_ECUDA, "item2vec sequential mode: %s", cudaGetErrorString(cudaGetLastError()));
+        if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return set_err(eh, CTR_ECUDA, "item2vec sequential mode: %s", cudaGetErrorString(cudaGetLastError()));
         cudaEventElapsedTime(&ms_total, e0, e1);
         if (stats) {
             stats->doc_len = nd; stats->trained_positions = (int64_t)hc[0]; stats->pairs = (int64_t)hc[1]; stats->node_visits = (int64_t)hc[2];
@@ -2754,8 +2758,6 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
         CI(cudaEventRecord(e1, st)); CI(cudaStreamSynchronize(st));                   // lr_tab is reused by the next iteration
         float ms = 0; CI(cudaEventElapsedTime(&ms, e0, e1)); ms_total += ms;
     }
-    CI(cudaStreamSynchronize(st));
-    if (emb_out) CI(big_copy(emb_out, d_syn0, sizeof(float) * (size_t)V * D, false, st));
     CI(cudaMemcpyAsync(hc, d_ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
     CI(cudaStreamSynchronize(st));
     if (stats) {
@@ -2764,6 +2766,30 @@ int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
     }
 #undef CI
 #undef CN
+    return CTR_OK;
+}
+
+// ctr_i2v_train / ctr_i2v_train_dist: the word-id stream from the caller's host memory, the table back to it
+int i2v_train_impl(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, int32_t V, float* emb_out, ctr_i2v_stats* stats, I2vDist* dist) {
+    if (!cfg || !tokens || (!emb_out && !dist) || n < 1 || V < 2 || n > 0x7fffffffLL) return set_err(nullptr, CTR_EINVAL, "bad item2vec arguments");
+    const ctr_i2v_config& c = *cfg;
+    RET(i2v_check_cfg(c, nullptr));
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_err(nullptr, CTR_ENODEV, "no CUDA device: this engine has no CPU fallback"); }
+    if (c.reserved[0] == 1 && dist && dist->world > 1) return set_err(nullptr, CTR_EINVAL, "the sequential float64 mode is single-GPU");
+#define CI(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return set_err(nullptr, CTR_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
+    // declared first, destroyed last: both buffers are freed before the stream
+    Stream st;
+    DevBuf<int> d_tok; DevBuf<float> d_syn0;
+    CI(cudaSetDevice(c.device));
+    cudaDeviceProp prop{}; CI(cudaGetDeviceProperties(&prop, c.device));
+    if (prop.major != 9) return set_err(nullptr, CTR_ENODEV, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
+    CI(st.create());
+    CI(d_tok.alloc((size_t)n));
+    CI(big_copy(d_tok, tokens, sizeof(int) * (size_t)n, true, st));
+    RET(i2v_train_dev(c, d_tok, n, V, prop.multiProcessorCount, st, d_syn0, stats, dist, nullptr));
+    if (emb_out) CI(big_copy(emb_out, d_syn0, sizeof(float) * (size_t)V * c.dim, false, st));
+#undef CI
     return CTR_OK;
 }
 }  // namespace
@@ -2788,6 +2814,102 @@ int ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, i
     const int rc = i2v_train_impl(cfg, tokens_shard, n_shard, V, emb_out, stats, &d);
     g_nccl.CommDestroy(d.nccl);
     return rc;
+}
+
+namespace {
+struct MinPos { __device__ int operator()(int a, int b) const { return a < b ? a : b; } };
+}  // namespace
+
+// recommend.Train's embedding stage (rcmd.go:207-213, 538-545) into the handle's ITEM_EMB: first-appearance numbering of
+// the item-id stream on the device (item2vec.cuh, idmap.cuh), the trainer on that document, one scatter into the rows.
+int ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n, int64_t* vocab_ids, int64_t cap,
+                       int32_t* vocab, ctr_i2v_stats* stats) {
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    if (!cfg || !item_ids || n < 1 || n > 0x7fffffffLL || cap < 0) return set_err(h, CTR_EINVAL, "bad item embedding arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    const ctr_i2v_config& c = *cfg;
+    if (c.dim != h->cfg.D) return set_err(h, CTR_EINVAL, "item2vec dim %d != model dim D=%d", c.dim, h->cfg.D);
+    RET(i2v_check_cfg(c, h));
+    if (!h->idm_keys[CTR_IDMAP_ITEM]) return set_err(h, CTR_ESTATE, "ctr_item_emb_train needs the item id map (ctr_idmap_build)");
+    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_item_emb_train is single-GPU (world = %d)", h->comm.world);
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const long R = (long)h->idm_n[CTR_IDMAP_ITEM];
+    const int G = h->num_sms * 8;
+    // kept to the end: the word-id document, row -> word, the vocabulary's item ids, the trained vectors
+    DevBuf<int> d_doc, d_word_row; DevBuf<long long> d_vocab; DevBuf<float> d_syn0;
+    int V = 0;
+    {
+        DevBuf<long long> d_ids; DevBuf<unsigned> d_first; DevBuf<unsigned long long> d_cnt;
+        CU(h, d_ids.alloc((size_t)n)); CU(h, d_doc.alloc((size_t)n));
+        CU(h, d_first.alloc((size_t)R)); CU(h, d_word_row.alloc((size_t)R)); CU(h, d_cnt.alloc(2));
+        CU(h, big_copy(d_ids, item_ids, sizeof(int64_t) * (size_t)n, true, st));
+        CU(h, cudaMemsetAsync(d_first, 0xff, sizeof(unsigned) * (size_t)R, st));
+        CU(h, cudaMemsetAsync(d_word_row, 0xff, sizeof(int) * (size_t)R, st));
+        CU(h, cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), st));
+        // 1. every token through the item map; first position per row; tokens without an entry counted
+        RET(launch(h, "i2v_dict_resolve", [&] {
+            k_idmap_first_pos<<<G, 256, 0, st>>>(h->idm_keys[CTR_IDMAP_ITEM], h->idm_vals[CTR_IDMAP_ITEM], h->idm_keys[CTR_IDMAP_ITEM].size() - 1,
+                                                 d_ids, (long)n, d_doc, d_first, d_cnt);
+        }));
+        unsigned long long m = 0;
+        CU(h, cudaMemcpyAsync(&m, d_cnt, sizeof m, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+        // 2. the side list: distinct unmapped ids (ascending as uint64) and the first position of each
+        DevBuf<unsigned long long> d_side_id; DevBuf<int> d_side_first, d_word_side;
+        int u = 0;
+        if (m > 0) {
+            DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
+            CU(h, k0.alloc(m)); CU(h, k1.alloc(m)); CU(h, p0.alloc(m)); CU(h, p1.alloc(m)); CU(h, d_u.alloc(1));
+            size_t b1 = 0, b2 = 0;
+            CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b1, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st));
+            CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b2, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st));
+            CU(h, tmp.alloc(std::max(b1, b2)));
+            RET(launch(h, "i2v_dict_side", [&] { k_i2v_dict_side<<<G, 256, 0, st>>>(d_doc, d_ids, (long)n, k0, p0, d_cnt + 1); }));
+            RET(launch(h, "i2v_dict_side", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st); }));
+            RET(launch(h, "i2v_dict_side", [&] { size_t tb = tmp.size(); cub::DeviceReduce::ReduceByKey(tmp.get(), tb, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st); }));
+            CU(h, cudaMemcpyAsync(&u, d_u, sizeof u, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+            CU(h, d_side_id.alloc((size_t)u)); CU(h, d_side_first.alloc((size_t)u)); CU(h, d_word_side.alloc((size_t)u));
+            CU(h, cudaMemcpyAsync(d_side_id, k0, sizeof(unsigned long long) * (size_t)u, cudaMemcpyDeviceToDevice, st));
+            CU(h, cudaMemcpyAsync(d_side_first, p0, sizeof(int) * (size_t)u, cudaMemcpyDeviceToDevice, st));
+        }
+        // 3. rows and side words ordered by first position: the rank is the word id
+        {
+            const long N = R + u;
+            DevBuf<unsigned> rk0, rk1; DevBuf<int> rv0, rv1, d_V; DevBuf<unsigned char> tmp;
+            CU(h, rk0.alloc((size_t)N)); CU(h, rk1.alloc((size_t)N)); CU(h, rv0.alloc((size_t)N)); CU(h, rv1.alloc((size_t)N));
+            CU(h, d_vocab.alloc((size_t)N)); CU(h, d_V.alloc(1));
+            size_t tb = 0;
+            CU(h, cub::DeviceRadixSort::SortPairs(nullptr, tb, rk0.get(), rk1.get(), rv0.get(), rv1.get(), (int)N, 0, 32, st));
+            CU(h, tmp.alloc(tb));
+            RET(launch(h, "i2v_dict_rank", [&] { k_i2v_dict_rank_keys<<<G, 256, 0, st>>>(d_first, R, d_side_first, u, rk0, rv0); }));
+            RET(launch(h, "i2v_dict_rank", [&] { size_t b = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), b, rk0.get(), rk1.get(), rv0.get(), rv1.get(), (int)N, 0, 32, st); }));
+            RET(launch(h, "i2v_dict_rank", [&] { k_i2v_dict_rank<<<G, 256, 0, st>>>(rk1, rv1, N, d_ids, d_word_row, d_word_side, d_vocab, d_V); }));
+            CU(h, cudaMemcpyAsync(&V, d_V, sizeof V, cudaMemcpyDeviceToHost, st));
+        }
+        // 4. the int32 word-id document, in place over the resolved rows
+        RET(launch(h, "i2v_dict_doc", [&] { k_i2v_dict_doc<<<G, 256, 0, st>>>(d_doc, d_ids, (long)n, d_word_row, d_side_id, u, d_word_side); }));
+        CU(h, cudaStreamSynchronize(st));
+    }
+    if (vocab) *vocab = V;
+    if (vocab_ids && cap > 0) {
+        CU(h, cudaMemcpyAsync(vocab_ids, d_vocab, sizeof(int64_t) * (size_t)std::min<int64_t>(cap, V), cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+    }
+    if (V < 2) return set_err(h, CTR_EINVAL, "item2vec needs at least two distinct words in the stream (%d)", V);
+    d_vocab.reset();
+    ctr_i2v_stats s{};
+    RET(i2v_train_dev(c, d_doc, n, V, h->num_sms, st, d_syn0, &s, nullptr, h));
+    d_doc.reset();
+    // ITEM_EMB [R, D]: as ctr_table_upload of the remapped table would leave it
+    const int D = c.dim;
+    float* tab = h->tab[CTR_TABLE_ITEM_EMB];
+    if (tab && h->tab_rows[CTR_TABLE_ITEM_EMB] == R && h->tab_width[CTR_TABLE_ITEM_EMB] == D && !h->tab_sharded[CTR_TABLE_ITEM_EMB]) table_new_state(h, CTR_TABLE_ITEM_EMB);
+    else RET(table_alloc(h, CTR_TABLE_ITEM_EMB, R, D));
+    tab = h->tab[CTR_TABLE_ITEM_EMB];
+    RET(launch(h, "i2v_emb_scatter", [&] { k_i2v_emb_scatter<<<G, 256, 0, st>>>(d_syn0, d_word_row, R, D, tab); }));
+    CU(h, cudaStreamSynchronize(st));
+    if (stats) *stats = s;
+    return CTR_OK;
 }
 
 // ---- model/mlp: the float64 MLP classifier (row a11) ---------------------------------------------------------

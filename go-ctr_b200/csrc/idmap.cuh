@@ -72,6 +72,26 @@ __device__ __forceinline__ int idmap_find(const unsigned long long* __restrict__
     }
 }
 
+// First step of the item2vec dictionary over an item-id stream (ctr_item_emb_train): rows[i] = the row of ids[i], -1
+// when the map has no entry; first_pos[row] = the smallest position of the row's id (first_pos starts at 0xFFFFFFFF);
+// *n_side counts the tokens without an entry.  Positions ascend with the lane, so among the lanes of a warp holding
+// one row the lowest lane carries the minimum, and a plain read skips the atomic once an earlier position is stored.
+__global__ void __launch_bounds__(256)
+k_idmap_first_pos(const unsigned long long* __restrict__ keys, const int* __restrict__ vals, unsigned long long mask,
+                  const long long* __restrict__ ids, long n, int* __restrict__ rows, unsigned* __restrict__ first_pos,
+                  unsigned long long* __restrict__ n_side) {
+    const int lane = threadIdx.x & 31;
+    for (long i0 = blockIdx.x * (long)blockDim.x + threadIdx.x; i0 < ((n + 31) & ~31L); i0 += (long)gridDim.x * blockDim.x) {
+        const bool in = i0 < n;
+        const int row = in ? idmap_find(keys, vals, mask, (unsigned long long)ids[i0]) : -1;
+        if (in) rows[i0] = row;
+        const unsigned side = __ballot_sync(0xffffffffu, in && row < 0);
+        if (lane == 0 && side) atomicAdd(n_side, (unsigned long long)__popc(side));
+        const unsigned peers = __match_any_sync(0xffffffffu, row);
+        if (row >= 0 && lane == __ffs(peers) - 1 && (unsigned)i0 < *(volatile unsigned*)(first_pos + row)) atomicMin(first_pos + row, (unsigned)i0);
+    }
+}
+
 // The whole key → index step of recommend.BatchPredict (rcmd.go:277-337) in one launch, one warp per key:
 // lanes 0/1 resolve the user / item id, the warp then evaluates TimeSeq.Filter (cache.go:71-94) for the
 // user's behaviour CSR (ub_off == nullptr: no UserBehavior provider → empty history) and writes hist [B,S].

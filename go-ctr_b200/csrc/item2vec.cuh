@@ -296,6 +296,79 @@ k_i2v_scale(float* __restrict__ x, long n, float s) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) x[i] *= s;
 }
 
+// -------------------------------------------------------------------------------------------------------------------
+// dictionary.Add's first-appearance numbering over an int64 item-id stream, on the device (ctr_item_emb_train).  The
+// item map resolves most tokens to a row and k_idmap_first_pos (idmap.cuh) keeps each row's first position; the tokens
+// without an entry form the side list, whose distinct ids and first positions come from a sort.  Both sets, ordered by
+// first position, are the vocabulary: a word's rank in that order is its id.
+// -------------------------------------------------------------------------------------------------------------------
+// side list: (id, position) of every token without an item-map entry, in any order (the sort that follows is keyed by id
+// and the reduction takes the minimum position, so the slot order does not reach the result)
+__global__ void __launch_bounds__(256)
+k_i2v_dict_side(const int* __restrict__ rows, const long long* __restrict__ ids, long n, unsigned long long* __restrict__ key,
+                int* __restrict__ pos, unsigned long long* __restrict__ count) {
+    const int lane = threadIdx.x & 31;
+    for (long i0 = blockIdx.x * (long)blockDim.x + threadIdx.x; i0 < ((n + 31) & ~31L); i0 += (long)gridDim.x * blockDim.x) {
+        const bool side = i0 < n && rows[i0] < 0;
+        const unsigned b = __ballot_sync(0xffffffffu, side);
+        if (!b) continue;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(b));
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (side) { const unsigned long long o = base + __popc(b & ((1u << lane) - 1u)); key[o] = (unsigned long long)ids[i0]; pos[o] = (int)i0; }
+    }
+}
+// sort input of the vocabulary: rows [0, R) keyed by their first position (0xFFFFFFFF: the row's id never occurs), then
+// the u side words keyed by theirs; val = row, or -(j+1) for side word j.  Positions are distinct, so the order is total.
+__global__ void __launch_bounds__(256)
+k_i2v_dict_rank_keys(const unsigned* __restrict__ first_pos, long R, const int* __restrict__ side_first, long u,
+                     unsigned* __restrict__ key, int* __restrict__ val) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R + u; i += (long)gridDim.x * blockDim.x) {
+        if (i < R) { key[i] = first_pos[i]; val[i] = (int)i; }
+        else { key[i] = (unsigned)side_first[i - R]; val[i] = -(int)(i - R) - 1; }
+    }
+}
+// after the sort: entry w < V is word w.  Its item id is the token at its first position; *V = the entries before the
+// first 0xFFFFFFFF key.  Rows whose id never occurs keep word_of_row = -1.
+__global__ void __launch_bounds__(256)
+k_i2v_dict_rank(const unsigned* __restrict__ key, const int* __restrict__ val, long N, const long long* __restrict__ ids,
+                int* __restrict__ word_of_row, int* __restrict__ word_of_side, long long* __restrict__ vocab_ids, int* __restrict__ V) {
+    for (long w = blockIdx.x * (long)blockDim.x + threadIdx.x; w < N; w += (long)gridDim.x * blockDim.x) {
+        const unsigned k = key[w];
+        if (k == 0xFFFFFFFFu) continue;
+        const int v = val[w];
+        if (v >= 0) word_of_row[v] = (int)w; else word_of_side[-v - 1] = (int)w;
+        vocab_ids[w] = ids[k];
+        if (w + 1 == N || key[w + 1] == 0xFFFFFFFFu) *V = (int)(w + 1);
+    }
+}
+// the int32 word-id document, in place over rows[]: a mapped token takes its row's word, a side token the word of its id
+// in side_ids (ascending as uint64, distinct)
+__global__ void __launch_bounds__(256)
+k_i2v_dict_doc(int* __restrict__ doc, const long long* __restrict__ ids, long n, const int* __restrict__ word_of_row,
+               const unsigned long long* __restrict__ side_ids, long u, const int* __restrict__ word_of_side) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const int row = doc[i];
+        if (row >= 0) { doc[i] = word_of_row[row]; continue; }
+        const unsigned long long id = (unsigned long long)ids[i];
+        long lo = 0, hi = u;                                   // first side id >= id; the id is in the list
+        while (lo < hi) { const long mid = (lo + hi) >> 1; if (side_ids[mid] < id) lo = mid + 1; else hi = mid; }
+        doc[i] = word_of_side[lo];
+    }
+}
+// ITEM_EMB [R, D] (row stride D: D is a power of two >= 4) from the trained syn0 [V, D]: row r takes its word's vector,
+// or zeros when its id never occurs.  One float4 per thread.
+__global__ void __launch_bounds__(256)
+k_i2v_emb_scatter(const float* __restrict__ syn0, const int* __restrict__ word_of_row, long R, int D, float* __restrict__ tab) {
+    const int q = D / 4;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R * q; i += (long)gridDim.x * blockDim.x) {
+        const long r = i / q; const int c = (int)(i - r * q);
+        const int w = word_of_row[r];
+        const float4 v = w >= 0 ? reinterpret_cast<const float4*>(syn0)[(long)w * q + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+        reinterpret_cast<float4*>(tab)[i] = v;
+    }
+}
+
 // syn0 = (U[0,1) - 0.5) / dim (word2vec.go:103-111) with the counter RNG
 __global__ void k_i2v_init(float* __restrict__ syn0, long n, int D, uint32_t seed) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {

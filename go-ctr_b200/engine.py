@@ -27,7 +27,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys"]
 
@@ -353,6 +353,21 @@ class Engine:
         out = np.empty(a.size, np.int32)
         self._ck(self.L.ctr_idmap_lookup(self.h, C.c_int(which), a.ctypes.data_as(_lp), C.c_int64(a.size), out.ctypes.data_as(_ip)))
         return out
+
+    def item_emb_train(self, item_ids, cfg=None, **kw):
+        """recommend.Train's embedding stage into ITEM_EMB (ctr_item_emb_train): item2vec over the int64 item stream,
+        words numbered by first appearance on the device, row r of ITEM_EMB = the vector of the item the item map sends
+        to r (zeros when it never occurs).  cfg: an item2vec.I2vConfig (default: i2v_default_config(dim=D, **kw)).
+        Returns (vocab_ids [V] int64: the item id of every word in word-id order, I2vStats)."""
+        from .item2vec import I2vStats, i2v_default_config
+        cfg = cfg or i2v_default_config(**{"dim": self.cfg.D, **kw})
+        ids = np.ascontiguousarray(item_ids, np.int64)
+        st = I2vStats(); V = C.c_int32(0)
+        cap = ids.size
+        vocab = np.empty(max(cap, 1), np.int64)
+        self._ck(self.L.ctr_item_emb_train(self.h, C.byref(cfg), ids.ctypes.data_as(_lp), C.c_int64(ids.size), vocab.ctypes.data_as(_lp),
+                                           C.c_int64(cap), C.byref(V), C.byref(st)))
+        return vocab[:V.value].copy(), st
 
     def batch_predict_keys(self, user_ids, item_ids, ts):
         """recommend.BatchPredict (rcmd.go:277-337) over Sample keys."""

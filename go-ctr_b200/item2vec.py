@@ -17,6 +17,7 @@ import numpy as np
 from . import engine as _e
 
 __all__ = ["i2v_paths", "I2vConfig", "I2vStats", "i2v_default_config", "i2v_train_ids", "i2v_train_dist", "TrainEmbedding", "EmbeddingModel",
+           "item_ids_from_seq", "TrainItemEmbedding",
            "Embedding", "SaveVectors", "LoadVectors", "ParseLine", "Neighbor", "Searcher", "neighbors_from_result"]
 
 
@@ -104,6 +105,40 @@ def TrainEmbedding(inputCh, window, dim, iter, **kw):
         toks.append(i)
     emb, st = i2v_train_ids(np.asarray(toks, np.int32), len(id2word), window=window, dim=dim, iter=iter, **kw)
     return EmbeddingModel(id2word, emb, st)
+
+
+_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def item_ids_from_seq(itemSeq):
+    """The int64 item stream of ItemSeqGenerator's messages: ints, or the decimal strings it sends (fmt.Sprintf("%d")).
+    A string that is not the canonical decimal of its value ("007", "+7", " 7") is another word in the reference and
+    raises ValueError rather than merging with the int's word; so does a value outside int64."""
+    out = []
+    for w in itemSeq:
+        if isinstance(w, str):
+            try:
+                v = int(w)
+            except ValueError:
+                raise ValueError("item %r is not a decimal item id" % (w,)) from None
+            if str(v) != w:
+                raise ValueError("item %r is not the canonical decimal of %d: it would be a different word" % (w, v))
+        elif isinstance(w, (int, np.integer)) and not isinstance(w, (bool, np.bool_)):
+            v = int(w)
+        else:
+            raise ValueError("item %r is neither an int nor a decimal string" % (w,))
+        if not _I64_MIN <= v <= _I64_MAX:
+            raise ValueError("item id %d is outside int64" % v)
+        out.append(v)
+    return np.asarray(out, np.int64)
+
+
+def TrainItemEmbedding(engine, itemSeq, window=5, iter=1, **kw):
+    """GetItemEmbeddingModelFromUb (rcmd.go:538-545) + GenEmbeddingMap32 into engine's ITEM_EMB (ctr_item_emb_train):
+    embedding.TrainEmbedding(itemSeq, window, D, iter) with dim = the engine's D.  Row r of ITEM_EMB becomes the vector
+    of the item the engine's item map sends to r, zeros for an item the stream never holds.  Returns (vocab_ids, I2vStats):
+    the item id of every word in word-id order (first appearance)."""
+    return engine.item_emb_train(item_ids_from_seq(itemSeq), window=window, iter=iter, **kw)
 
 
 # ---- the word2vec text format the reference saves / loads its vectors in -------------------------------------

@@ -423,6 +423,27 @@ func (e *Engine) TrainKeys(samples []rcmd.Sample, epochs, earlyStop int) (lastCo
 	return float32(cost), int64(used), e.err(rc)
 }
 
+// TrainItemEmbedding is recommend.Train's embedding stage (GetItemEmbeddingModelFromUb + GenEmbeddingMap32 and the
+// itemEmbeddingMap lookups, rcmd.go:207-213, 502, 519, 538-545) on the device: itemIds is what ItemSeqGenerator yields,
+// as int64, in corpus order.  Words are numbered by first appearance, embedding.TrainEmbedding(itemSeq, window, D, iter)
+// runs on them, and ITEM_EMB row r becomes the vector of the item LoadIDMaps put at row r (zeros when the item never
+// occurs).  No table crosses PCIe.  Returns the item id of every word in word-id order (SaveVectors, Searcher).
+func (e *Engine) TrainItemEmbedding(itemIds []int64, window, iter int) ([]int64, error) {
+	if len(itemIds) == 0 {
+		return nil, fmt.Errorf("TrainItemEmbedding: empty item stream")
+	}
+	var cfg C.ctr_i2v_config
+	C.ctr_i2v_config_default(&cfg)
+	cfg.dim, cfg.window, cfg.iter = e.cfg.D, C.int32_t(window), C.int32_t(iter)
+	vocab := make([]int64, len(itemIds))
+	var v C.int32_t
+	rc := C.ctr_item_emb_train(e.h, &cfg, i64(itemIds), C.int64_t(len(itemIds)), i64(vocab), C.int64_t(len(vocab)), &v, nil)
+	if err := e.err(rc); err != nil {
+		return nil, err
+	}
+	return vocab[:int(v)], nil
+}
+
 // SetTableOptimizer selects how embedding rows learn (engine extension; the reference keeps them frozen,
 // din.go:161-169): C.CTR_TABLE_FROZEN | SGD | SGD_DETERMINISTIC | ADAM.  Call before NewEngine's ctr_create in a
 // custom constructor, or use NewEngineWith.

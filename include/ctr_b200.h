@@ -368,6 +368,34 @@ int  ctr_i2v_train(const ctr_i2v_config* cfg, const int32_t* tokens, int64_t n, 
 int  ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, int64_t n_shard, int32_t vocab,
                         float* emb_out, ctr_i2v_stats* stats, int32_t rank, int32_t world,
                         const void* nccl_id, int32_t id_bytes, int64_t sync_every);
+/* recommend.Train's embedding stage (rcmd.go:207-213, 538-545: GetItemEmbeddingModelFromUb → TrainEmbedding →
+ * GenEmbeddingMap32 → the itemEmbeddingMap lookups) straight into the handle's ITEM_EMB, with no table crossing PCIe.
+ * item_ids [n] is the item stream in corpus order, as ItemSeqGenerator yields it (one item per message, users
+ * concatenated), as int64; every int64 value is a word, INT64_MIN included.  Word ids are assigned on the device by first
+ * appearance (dictionary.Add, dictionary.go:70-81), and the trainer then runs exactly as ctr_i2v_train on that word-id
+ * stream: MinCount filter, Huffman tree over all words, subsampling, lr schedule, and reserved[0] = 1 (sequential
+ * float64 mode) alike.  n in [1, 2^31); the stream needs at least two distinct words.
+ * ITEM_EMB becomes [idmap_n(CTR_IDMAP_ITEM), D]: row r holds the trained vector of the word whose item id the item map
+ * sends to r; rows whose item never occurs are zero (rcmd.go:501-505, 519-521: missing item embedding → zeros); words
+ * below min_count keep their initial vector, as GenEmbeddingMap32 has them; words without an item-map entry shape the
+ * dictionary and the tree but land in no row.  Afterwards the handle is exactly as ctr_table_upload(ITEM_EMB, M) of that
+ * matrix M would leave it: same allocation rules, row-Adam moments and hot-row accumulators reset.  When ITEM_EMB already
+ * has that shape the rows are rewritten in place, otherwise the table is allocated as ctr_table_upload allocates it.
+ * The rows are written only after training has succeeded: a refusal, or any error before that write, leaves ITEM_EMB
+ * and its solver state as they were.
+ * *vocab = V is written when vocab is non-NULL (also when V < 2 is refused); vocab_ids (may be NULL) receives the first
+ * min(cap, V) words' item ids in word-id order (SaveVectors, the word ↔ row bookkeeping of a Searcher).  stats as
+ * ctr_i2v_train fills it.
+ * CTR_EINVAL: null or short arguments, cfg->dim != D, a configuration ctr_i2v_train refuses, n out of range, fewer than
+ * two distinct words.  CTR_ESTATE: no item id map, or world > 1 (the ranks would need a global first-appearance order).
+ * cfg->device is ignored: the handle's device is used.  Runs on the engine stream under the handle's mutex: ordered after
+ * everything queued before it, and everything queued after it sees the new table.  The int64 stream is staged from
+ * pageable memory through pinned bounce buffers.  Peak device memory beside the handle's own buffers, with R item-map
+ * rows, m tokens without an item-map entry and u distinct such ids: at most 12·n + 24·m + 40·(R + u) bytes (+ sort
+ * scratch) while numbering — the whole stream is never sorted, only its m unmapped tokens — then 9·n + 4·R bytes plus
+ * ctr_i2v_train's vocabulary tables while training, and 4·V·D + 4·R bytes next to ITEM_EMB for the final write. */
+int  ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n,
+                        int64_t* vocab_ids, int64_t cap, int32_t* vocab, ctr_i2v_stats* stats);
 
 /* ---- model/mlp: the float64 MLP classifier of the reference's default path (BASELINE configs[0]; SURVEY.md §8a row
  * a11) — main.go:42-52 → model/mlp/mlp.go:45-65 (SimpleMlpFitWrap.Fit / SimpleMlpPredWrap.Predict: float32 samples →
