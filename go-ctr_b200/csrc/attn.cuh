@@ -1083,4 +1083,23 @@ __global__ void k_table_fill(float* __restrict__ t, long ld, long local_rows, in
     }
 }
 
+// ctr_table_write_rows: row rows[i] of t = data[i] ([n, width] compact), bit for bit; mo / vo (ITEM_EMB row-Adam moments,
+// layout of the table) are zeroed on those rows when non-null.  One warp per row.
+__global__ void __launch_bounds__(256)
+k_table_write_rows(float* __restrict__ t, long ld, const int* __restrict__ rows, const float* __restrict__ data, long n, int width,
+                   float* __restrict__ mo, float* __restrict__ vo) {
+    const int lane = threadIdx.x & 31;
+    for (long r = (blockIdx.x * (long)blockDim.x + threadIdx.x) >> 5; r < n; r += ((long)gridDim.x * blockDim.x) >> 5) {
+        const long dst = (long)rows[r] * ld;
+        for (int c = lane; c < width; c += 32) t[dst + c] = data[r * width + c];
+        if (mo) for (long c = lane; c < ld; c += 32) { mo[dst + c] = 0.0f; vo[dst + c] = 0.0f; }
+    }
+}
+// *dup = 1 when the ascending rows hold a value twice
+__global__ void __launch_bounds__(256)
+k_rows_dup(const int* __restrict__ sorted, long n, int* __restrict__ dup) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i + 1 < n; i += (long)gridDim.x * blockDim.x)
+        if (sorted[i] == sorted[i + 1]) *dup = 1;
+}
+
 }  // namespace ctr

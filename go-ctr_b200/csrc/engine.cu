@@ -109,6 +109,7 @@ struct ctr_handle {
     int tab_width[3] = {0, 0, 0};
     bool tab_sharded[3] = {false, false, false};   // world > 1: rows r % world == rank live here, the rest on the peers
     VmmBuf tab_vmm[3];                    // a sharded table lives in shareable (VMM) memory; tab[] points into it
+    GrowBuf<float> tab_mem[3];            // any other table lives in growable memory (ctr_table_write_rows); tab[] points into it
     uint64_t tab_gen = 1;                 // bumped whenever an ITEM_* table is (re)allocated: peers must re-map it
 
     // learnables, padded storage: W0 [Kp,H0p] W1 [H0p,H1p] W2 [H1p] att [Sp]; grads / Adam moments alike
@@ -126,7 +127,7 @@ struct ctr_handle {
     DevBuf<unsigned char> sort_tmp;
     DevBuf<double> d_cost;
     DevBuf<float> hot_acc; int hot_rows = 0, hot_reps = 0;
-    DevBuf<float> emb_m, emb_v;           // CTR_TABLE_ADAM: first / second moments of ITEM_EMB, same layout as the table
+    GrowBuf<float> emb_m, emb_v;          // CTR_TABLE_ADAM: first / second moments of ITEM_EMB, same layout as the table (grown with it)
     // staging for host-pointer entry points
     DevBuf<int> s_user, s_item, s_hist; DevBuf<float> s_label;
     // epoch entry points (ctr_train_idx / ctr_train_keys): pinned host ring (filled by the copy pool from the caller's
@@ -631,12 +632,20 @@ int ensure_hot(ctr_handle* h) {
     return dalloc(h, h->hot_acc, (size_t)reps * want * h->cfg.D);
 }
 
+// maps at least n elements of b (growable memory); the new part is not initialised
+int grow_buf(ctr_handle* h, GrowBuf<float>& b, size_t n) {
+    std::string err;
+    if (!b.grow(std::max<size_t>(n, 1), h->dev, h->stream, &err)) return set_err(h, CTR_ENOMEM, "device memory (%zu bytes): %s", n * sizeof(float), err.c_str());
+    return CTR_OK;
+}
+
 // CTR_TABLE_ADAM: moments of the embedding rows (zero-initialised, like the solver's, model.go:88)
 int ensure_moments(ctr_handle* h) {
     if (h->emb_m) return CTR_OK;
     const size_t n = (size_t)std::max<int64_t>(h->tab_local_rows[CTR_TABLE_ITEM_EMB], 1) * h->tab_ld[CTR_TABLE_ITEM_EMB];
-    DevBuf<float> m, v;                  // both or neither
-    RET(dalloc(h, m, n)); RET(dalloc(h, v, n));
+    GrowBuf<float> m, v;                 // both or neither
+    RET(grow_buf(h, m, n)); RET(grow_buf(h, v, n));
+    CU(h, cudaMemsetAsync(m, 0, n * sizeof(float), h->stream)); CU(h, cudaMemsetAsync(v, 0, n * sizeof(float), h->stream));
     h->emb_m = std::move(m); h->emb_v = std::move(v);
     return CTR_OK;
 }
@@ -854,17 +863,20 @@ bool table_sharded(const ctr_handle* h, int which, int64_t nrows, int32_t width)
 // (re)allocates table `which` for nrows logical rows; decides the placement; leaves the rows zeroed
 void table_free(ctr_handle* h, int which) {
     if (h->tab_vmm[which].live) { cudaStreamSynchronize(h->stream); vmm_free(&h->tab_vmm[which]); }
-    else if (h->tab[which]) cudaFree(h->tab[which]);
+    else h->tab_mem[which].reset();
     h->tab[which] = nullptr;
 }
-// device memory of a table: shareable VMM memory when the table is sharded (peers map it), cudaMalloc otherwise
+// device memory of a table: shareable VMM memory when the table is sharded (peers map it), growable memory otherwise
 int table_mem(ctr_handle* h, int which, bool shard, size_t bytes) {
     table_free(h, which);
     if (shard) {
         std::string err;
         if (!vmm_alloc(bytes, h->dev, &h->tab_vmm[which], &err)) return set_err(h, CTR_ENOMEM, "table %d (%zu bytes): %s", which, bytes, err.c_str());
         h->tab[which] = (float*)h->tab_vmm[which].ptr;
-    } else CU(h, cudaMalloc(&h->tab[which], bytes));
+    } else {
+        RET(grow_buf(h, h->tab_mem[which], bytes / sizeof(float)));
+        h->tab[which] = h->tab_mem[which].get();
+    }
     CU(h, cudaMemsetAsync(h->tab[which], 0, bytes, h->stream));
     return CTR_OK;
 }
@@ -1974,7 +1986,7 @@ int ctr_idmap_build(ctr_handle* h, int which, const int64_t* ids, int64_t n) {
     cudaMemsetAsync(h->k_flags, 0, sizeof(int), h->stream);
     rc = launch(h, "idmap_clear", [&] { k_idmap_clear<<<h->num_sms * 8, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], cap); });
     if (rc == CTR_OK) rc = launch(h, "idmap_insert", [&] {
-        k_idmap_insert<<<h->num_sms * 8, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], cap - 1, d_ids, (long)n, h->k_flags);
+        k_idmap_insert<<<h->num_sms * 8, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], cap - 1, d_ids, (long)n, h->k_flags, 0);
     });
     if (rc == CTR_OK && (cudaMemcpyAsync(&flags, h->k_flags, sizeof(int), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
                          cudaStreamSynchronize(h->stream) != cudaSuccess)) rc = set_err(h, CTR_ECUDA, "idmap build: %s", cudaGetErrorString(cudaGetLastError()));
@@ -2909,6 +2921,182 @@ int ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* 
     RET(launch(h, "i2v_emb_scatter", [&] { k_i2v_emb_scatter<<<G, 256, 0, st>>>(d_syn0, d_word_row, R, D, tab); }));
     CU(h, cudaStreamSynchronize(st));
     if (stats) *stats = s;
+    return CTR_OK;
+}
+
+// ---- live id maps and tables: new users and items on a running handle (row f3) -----------------------------------
+namespace {
+unsigned long long idmap_cap_for(int64_t n) {
+    unsigned long long cap = 64;
+    while (cap < 2ull * (unsigned long long)n) cap <<= 1;                 // load factor <= 0.5, as ctr_idmap_build
+    return cap;
+}
+}  // namespace
+
+// The ids the map lacks get rows idm_n, idm_n + 1, ... in order of first occurrence, numbered as ctr_item_emb_train
+// numbers its side words: the probe (k_idmap_first_pos) marks them, k_i2v_dict_side + a radix sort + ReduceByKey(MinPos)
+// give each distinct one its first position, and a sort by that position is the order.  Only the missing ids are sorted.
+int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows) {
+    if (!h || !ids || which < 0 || which > 1 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad idmap insert arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_idmap_insert is single-GPU (world = %d)", h->comm.world);
+    for (int64_t i = 0; i < n; i++)
+        if ((unsigned long long)ids[i] == kIdEmpty) return set_err(h, CTR_EINVAL, "idmap insert: id INT64_MIN is reserved (position %lld)", (long long)i);
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const int G = h->num_sms * 8;
+    const int64_t R = h->idm_n[which];
+    const bool have = (bool)h->idm_keys[which];
+    long long* d_ids = nullptr; int* d_rows = nullptr; unsigned long long* d_cnt = nullptr;
+    RET(scratch_get(h, 0, sizeof(long long) * (size_t)n, (void**)&d_ids)); RET(scratch_get(h, 1, sizeof(int) * (size_t)n, (void**)&d_rows));
+    RET(scratch_get(h, 2, 2 * sizeof(unsigned long long), (void**)&d_cnt));
+    if (!h->k_flags) RET(dalloc(h, h->k_flags, 1));
+    CU(h, big_copy(d_ids, ids, sizeof(int64_t) * (size_t)n, true, st));
+    CU(h, cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), st));
+    unsigned long long m = (unsigned long long)n;
+    if (have) {
+        RET(launch(h, "idmap_probe", [&] {
+            k_idmap_first_pos<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows, nullptr, d_cnt);
+        }));
+        CU(h, cudaMemcpyAsync(&m, d_cnt, sizeof m, cudaMemcpyDeviceToHost, st));
+    } else CU(h, cudaMemsetAsync(d_rows, 0xff, sizeof(int) * (size_t)n, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (m > 0) {
+        // distinct missing ids and their first positions, then ordered by first position: k1[j] gets row R + j
+        DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
+        CU(h, k0.alloc(m)); CU(h, k1.alloc(m)); CU(h, p0.alloc(m)); CU(h, p1.alloc(m)); CU(h, d_u.alloc(1));
+        size_t b1 = 0, b2 = 0, b3 = 0;
+        CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b1, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st));
+        CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b2, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st));
+        CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b3, p0.get(), p1.get(), k0.get(), k1.get(), (int)m, 0, 32, st));
+        CU(h, tmp.alloc(std::max(b1, std::max(b2, b3))));
+        RET(launch(h, "idmap_number", [&] { k_i2v_dict_side<<<G, 256, 0, st>>>(d_rows, d_ids, (long)n, k0, p0, d_cnt + 1); }));
+        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st); }));
+        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceReduce::ReduceByKey(tmp.get(), tb, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st); }));
+        int u = 0;
+        CU(h, cudaMemcpyAsync(&u, d_u, sizeof u, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+        if (R + u > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "idmap insert: %lld ids + %d new ones exceed INT32_MAX rows", (long long)R, u);
+        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, p0.get(), p1.get(), k0.get(), k1.get(), u, 0, 32, st); }));
+        // a table at the capacity ctr_idmap_build picks for the new count: the old entries rehashed into it, then swapped
+        const unsigned long long cap = idmap_cap_for(R + u), old_cap = have ? h->idm_keys[which].size() : 0;
+        if (cap > old_cap) {
+            DevBuf<unsigned long long> nk; DevBuf<int> nv;
+            RET(dalloc(h, nk, (size_t)cap, false)); RET(dalloc(h, nv, (size_t)cap, false));
+            RET(launch(h, "idmap_clear", [&] { k_idmap_clear<<<G, 256, 0, st>>>(nk, nv, cap); }));
+            if (have) RET(launch(h, "idmap_rehash", [&] { k_idmap_rehash<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], old_cap, nk, nv, cap - 1); }));
+            h->idm_keys[which] = std::move(nk); h->idm_vals[which] = std::move(nv);        // cudaFree of the old table waits for the rehash
+        }
+        RET(launch(h, "idmap_insert", [&] {
+            k_idmap_insert<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, (const long long*)k1.get(), (long)u, h->k_flags, (int)R);
+        }));
+        h->idm_n[which] = R + u;
+        if (rows) RET(launch(h, "idmap_lookup", [&] {
+            k_idmap_lookup<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows);
+        }));
+    }
+    if (rows) CU(h, cudaMemcpyAsync(rows, d_rows, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+
+int ctr_idmap_download(ctr_handle* h, int which, int64_t* ids, int64_t cap, int64_t* n) {
+    if (!h || !n || which < 0 || which > 1) return set_err(h, CTR_EINVAL, "bad idmap download arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_idmap_download is single-GPU (world = %d)", h->comm.world);
+    if (!h->idm_keys[which]) return set_err(h, CTR_ESTATE, "idmap %d not built", which);
+    *n = h->idm_n[which];
+    if (!ids) return CTR_OK;
+    if (cap < h->idm_n[which]) return set_err(h, CTR_EINVAL, "idmap download: the map holds %lld ids", (long long)h->idm_n[which]);
+    CU(h, cudaSetDevice(h->dev));
+    DevBuf<long long> d;
+    CU(h, d.alloc((size_t)h->idm_n[which]));
+    RET(launch(h, "idmap_download", [&] {
+        k_idmap_dump<<<h->num_sms * 8, 256, 0, h->stream>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size(), d);
+    }));
+    CU(h, big_copy(ids, d, sizeof(int64_t) * (size_t)h->idm_n[which], false, h->stream));
+    return CTR_OK;
+}
+
+// Rows are written in place; a row past the end grows the table (and ITEM_EMB's moments) in its growable memory, the
+// gap zeroed.  Validation (ranges on the host, duplicates by a device sort) comes before any write to the table.
+int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const float* data, int64_t n, int32_t width) {
+    if (!h || !rows || !data || which < 0 || which > 2 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad table write arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    const ctr_config& c = h->cfg;
+    const int want = which == CTR_TABLE_USER_FEAT ? c.uP : which == CTR_TABLE_ITEM_FEAT ? c.cF : c.D;
+    if (width != want || width < 1) return set_err(h, CTR_EINVAL, "table %d width %d != model dim %d", which, width, want);
+    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_table_write_rows is single-GPU (world = %d)", h->comm.world);
+    int32_t top = -1;
+    for (int64_t i = 0; i < n; i++) {
+        if (rows[i] < 0 || rows[i] == 0x7fffffff) return set_err(h, CTR_EINVAL, "table write: row %d outside [0, INT32_MAX) at position %lld", rows[i], (long long)i);
+        top = std::max(top, rows[i]);
+    }
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const int G = h->num_sms * 8;
+    DevBuf<int> d_rows;
+    CU(h, d_rows.alloc((size_t)n));
+    CU(h, big_copy(d_rows, rows, sizeof(int32_t) * (size_t)n, true, st));
+    if (n > 1) {
+        DevBuf<int> sorted, d_dup; DevBuf<unsigned char> tmp;
+        CU(h, sorted.alloc((size_t)n)); CU(h, d_dup.alloc(1));
+        int bits = 1; while (bits < 31 && (top >> bits) != 0) bits++;
+        size_t tb = 0;
+        CU(h, cub::DeviceRadixSort::SortKeys(nullptr, tb, d_rows.get(), sorted.get(), (int)n, 0, bits, st));
+        CU(h, tmp.alloc(tb));
+        CU(h, cudaMemsetAsync(d_dup, 0, sizeof(int), st));
+        RET(launch(h, "table_write_check", [&] { size_t b = tmp.size(); cub::DeviceRadixSort::SortKeys(tmp.get(), b, d_rows.get(), sorted.get(), (int)n, 0, bits, st); }));
+        RET(launch(h, "table_write_check", [&] { k_rows_dup<<<G, 256, 0, st>>>(sorted, (long)n, d_dup); }));
+        int dup = 0;
+        CU(h, cudaMemcpyAsync(&dup, d_dup, sizeof dup, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+        if (dup) return set_err(h, CTR_EINVAL, "table write: a row appears twice");
+    }
+    const int64_t nrows = (int64_t)top + 1;
+    if (!h->tab[which]) RET(table_alloc(h, which, nrows, width));
+    else if (nrows > h->tab_rows[which]) {
+        // every buffer is mapped first; the row count changes only once all of them hold the new rows
+        const int64_t old = h->tab_rows[which];
+        const long ld = h->tab_ld[which];
+        const bool mom = which == CTR_TABLE_ITEM_EMB && h->emb_m;
+        int rc = CTR_OK;
+        RET(launch(h, "table_grow", [&] {
+            for (GrowBuf<float>* b : {&h->tab_mem[which], mom ? &h->emb_m : nullptr, mom ? &h->emb_v : nullptr})
+                if (b && rc == CTR_OK && (rc = grow_buf(h, *b, (size_t)nrows * ld)) == CTR_OK)
+                    cudaMemsetAsync(b->get() + (size_t)old * ld, 0, (size_t)(nrows - old) * ld * sizeof(float), st);
+        }));
+        RET(rc);
+        h->tab[which] = h->tab_mem[which].get();
+        h->tab_rows[which] = h->tab_local_rows[which] = nrows;
+    }
+    // host rows in chunks: through two pinned buffers (the caller's may be pageable) into two device slots
+    const size_t row_b = (size_t)width * sizeof(float), total = (size_t)n * row_b;
+    const size_t kChunk = (size_t)32 << 20;
+    const int64_t per = (int64_t)std::max<size_t>(1, kChunk / row_b);
+    const bool pinned = total >= ((size_t)8 << 20);
+    const size_t slot = std::min<size_t>((size_t)per, (size_t)n) * row_b;
+    PinnedBuf<unsigned char> pin[2]; DevBuf<unsigned char> stage[2]; Event ev[2];
+    for (int b = 0; b < 2; b++) {
+        CU(h, stage[b].alloc(slot)); CU(h, ev[b].create(cudaEventDisableTiming));
+        if (pinned) CU(h, pin[b].alloc(slot));
+    }
+    std::unique_ptr<CopyPool> pool;
+    if (pinned) pool.reset(new CopyPool(7));
+    float* mo = which == CTR_TABLE_ITEM_EMB && h->emb_m ? h->emb_m.get() : nullptr;
+    float* vo = mo ? h->emb_v.get() : nullptr;
+    for (int64_t r0 = 0, k = 0; r0 < n; r0 += per, k++) {
+        const int b = (int)(k & 1);
+        const int64_t nr = std::min<int64_t>(per, n - r0);
+        const char* src = (const char*)data + (size_t)r0 * row_b;
+        if (k >= 2) CU(h, cudaEventSynchronize(ev[b]));
+        if (pinned) { pool->copy(pin[b], src, (size_t)nr * row_b); src = (const char*)pin[b].get(); }
+        CU(h, cudaMemcpyAsync(stage[b], src, (size_t)nr * row_b, cudaMemcpyHostToDevice, st));
+        RET(launch(h, "table_write_rows", [&] {
+            k_table_write_rows<<<(int)std::min<int64_t>((nr + 7) / 8, G), 256, 0, st>>>(h->tab[which], h->tab_ld[which], d_rows.get() + r0,
+                                                                                                   (const float*)stage[b].get(), (long)nr, width, mo, vo);
+        }));
+        CU(h, cudaEventRecord(ev[b], st));
+    }
+    CU(h, cudaStreamSynchronize(st));
     return CTR_OK;
 }
 

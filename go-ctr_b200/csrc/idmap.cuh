@@ -24,20 +24,42 @@ k_idmap_clear(unsigned long long* __restrict__ keys, int* __restrict__ vals, uns
     }
 }
 
-// row of ids[i] is i.  flags[0] |= 1 on a duplicate id, |= 2 on the reserved id.
+// row of ids[i] is base + i.  flags[0] |= 1 on a duplicate id, |= 2 on the reserved id.
 __global__ void __launch_bounds__(256)
 k_idmap_insert(unsigned long long* __restrict__ keys, int* __restrict__ vals, unsigned long long mask,
-               const long long* __restrict__ ids, long n, int* __restrict__ flags) {
+               const long long* __restrict__ ids, long n, int* __restrict__ flags, int base) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
         const unsigned long long id = (unsigned long long)ids[i];
         if (id == kIdEmpty) { atomicOr(flags, 2); continue; }
         unsigned long long slot = idmap_hash(id) & mask;
         for (;;) {
             const unsigned long long prev = atomicCAS(&keys[slot], kIdEmpty, id);
-            if (prev == kIdEmpty) { vals[slot] = (int)i; break; }
-            if (prev == id) { atomicOr(flags, 1); atomicMin(&vals[slot], (int)i); break; }
+            if (prev == kIdEmpty) { vals[slot] = base + (int)i; break; }
+            if (prev == id) { atomicOr(flags, 1); atomicMin(&vals[slot], base + (int)i); break; }
             slot = (slot + 1) & mask;
         }
+    }
+}
+
+// ctr_idmap_insert outgrowing its table: every entry of the old table (old_cap slots) into the cleared new one
+__global__ void __launch_bounds__(256)
+k_idmap_rehash(const unsigned long long* __restrict__ old_keys, const int* __restrict__ old_vals, unsigned long long old_cap,
+               unsigned long long* __restrict__ keys, int* __restrict__ vals, unsigned long long mask) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < old_cap; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long id = old_keys[i];
+        if (id == kIdEmpty) continue;
+        unsigned long long slot = idmap_hash(id) & mask;
+        while (atomicCAS(&keys[slot], kIdEmpty, id) != kIdEmpty) slot = (slot + 1) & mask;   // ids are distinct
+        vals[slot] = old_vals[i];
+    }
+}
+
+// ctr_idmap_download: ids[row] = the id of every row (rows are dense, so every ids[r] is written)
+__global__ void __launch_bounds__(256)
+k_idmap_dump(const unsigned long long* __restrict__ keys, const int* __restrict__ vals, unsigned long long cap, long long* __restrict__ ids) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < cap; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long id = keys[i];
+        if (id != kIdEmpty) ids[vals[i]] = (long long)id;
     }
 }
 
@@ -76,6 +98,7 @@ __device__ __forceinline__ int idmap_find(const unsigned long long* __restrict__
 // when the map has no entry; first_pos[row] = the smallest position of the row's id (first_pos starts at 0xFFFFFFFF);
 // *n_side counts the tokens without an entry.  Positions ascend with the lane, so among the lanes of a warp holding
 // one row the lowest lane carries the minimum, and a plain read skips the atomic once an earlier position is stored.
+// ctr_idmap_insert's probe passes first_pos == nullptr: rows and the count only.
 __global__ void __launch_bounds__(256)
 k_idmap_first_pos(const unsigned long long* __restrict__ keys, const int* __restrict__ vals, unsigned long long mask,
                   const long long* __restrict__ ids, long n, int* __restrict__ rows, unsigned* __restrict__ first_pos,
@@ -87,6 +110,7 @@ k_idmap_first_pos(const unsigned long long* __restrict__ keys, const int* __rest
         if (in) rows[i0] = row;
         const unsigned side = __ballot_sync(0xffffffffu, in && row < 0);
         if (lane == 0 && side) atomicAdd(n_side, (unsigned long long)__popc(side));
+        if (!first_pos) continue;
         const unsigned peers = __match_any_sync(0xffffffffu, row);
         if (row >= 0 && lane == __ffs(peers) - 1 && (unsigned)i0 < *(volatile unsigned*)(first_pos + row)) atomicMin(first_pos + row, (unsigned)i0);
     }

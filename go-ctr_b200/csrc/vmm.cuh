@@ -6,6 +6,7 @@
 // in-process; the bigger the table the worse — TLB misses).  The VMM API keeps 2 MB pages on both sides: the owner
 // creates the allocation with cuMemCreate (exportable as a POSIX file descriptor), the peers import the descriptor
 // (passed over a Unix-domain socket, SCM_RIGHTS) and cuMemMap it into their own address space.
+// GrowBuf (below) uses the same API in one process: tables that grow in place without a copy.
 //
 // Driver entry points are resolved through cudaGetDriverEntryPoint: the library links cudart only and still loads
 // on a machine without libcuda (CPU-side ABI tests).
@@ -20,6 +21,8 @@
 #include <errno.h>
 #include <algorithm>
 #include <string>
+#include <utility>
+#include <vector>
 
 namespace ctr {
 
@@ -121,6 +124,106 @@ inline bool vmm_import(int fd, size_t bytes, int dev, VmmBuf* out, std::string* 
     *out = b;
     return true;
 }
+
+// ---- growable device memory: the single-GPU tables and ITEM_EMB's row-Adam moments (ctr_table_write_rows) ------
+// A virtual range reserved with headroom; physical chunks (non-shareable handles) are created and mapped at the end of
+// what is mapped as the buffer grows, each about 1/8 of the mapped size and at least one granule, so a run of one-row
+// growths maps O(log n) chunks.  When the reservation is full, a range twice the new size is reserved and the same
+// chunks are mapped into it: no byte is copied, and the old and the new buffer never need memory side by side.  The old
+// range is unmapped after `st` (the stream of every kernel that holds the old base) has passed them.
+// One owner, like Buf (owner.cuh): destroyed or reset, it releases every chunk and range (after a device synchronise,
+// which is what cudaFree does).
+template <typename T>
+class GrowBuf {
+public:
+    GrowBuf() = default;
+    GrowBuf(GrowBuf&& o) noexcept { take(o); }
+    GrowBuf& operator=(GrowBuf&& o) noexcept { if (this != &o) { reset(); take(o); } return *this; }
+    ~GrowBuf() { reset(); }
+    // at least n elements mapped; the contents of the part mapped here are undefined.  get() may change.
+    bool grow(size_t n, int dev, cudaStream_t st, std::string* err) {
+        const size_t need = n * sizeof(T);
+        if (need <= mapped_) return true;
+        if (!drv_load(err)) return false;
+        DrvApi& d = drv();
+        CUmemAllocationProp prop = vmm_prop(dev);
+        prop.requestedHandleTypes = CU_MEM_HANDLE_TYPE_NONE;
+        if (!gran_ && (d.MemGetAllocationGranularity(&gran_, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED) != CUDA_SUCCESS || gran_ == 0)) {
+            gran_ = 0; *err = "cuMemGetAllocationGranularity failed"; return false;
+        }
+        const size_t chunk = round(std::max(need - mapped_, mapped_ / 8));
+        CUmemGenericAllocationHandle hnd = 0;
+        if (d.MemCreate(&hnd, chunk, &prop, 0) != CUDA_SUCCESS) { *err = "cuMemCreate failed (out of device memory?)"; return false; }
+        if (mapped_ + chunk > reserved_ && !move(2 * (mapped_ + chunk), dev, st, err)) { d.MemRelease(hnd); return false; }
+        if (!map(va_ + mapped_, chunk, hnd, dev)) { d.MemRelease(hnd); *err = "cuMemMap / cuMemSetAccess failed"; return false; }
+        chunks_.push_back({hnd, chunk});
+        mapped_ += chunk;
+        return true;
+    }
+    void reset() {
+        if (!va_) return;
+        cudaDeviceSynchronize();
+        DrvApi& d = drv();
+        unmap_all(va_);
+        d.MemAddressFree(va_, reserved_);
+        for (const Chunk& c : chunks_) d.MemRelease(c.h);
+        chunks_.clear(); va_ = 0; reserved_ = mapped_ = 0;
+    }
+    T* get() const { return reinterpret_cast<T*>(va_); }
+    operator T*() const { return get(); }
+    size_t capacity() const { return mapped_ / sizeof(T); }     // elements mapped
+    size_t chunks() const { return chunks_.size(); }
+    int moves() const { return moves_; }                         // reservations replaced by a larger one
+private:
+    struct Chunk { CUmemGenericAllocationHandle h; size_t bytes; };
+    size_t round(size_t b) const { return (std::max<size_t>(b, 1) + gran_ - 1) / gran_ * gran_; }
+    static bool map(CUdeviceptr va, size_t bytes, CUmemGenericAllocationHandle hnd, int dev) {
+        DrvApi& d = drv();
+        if (d.MemMap(va, bytes, 0, hnd, 0) != CUDA_SUCCESS) return false;
+        CUmemAccessDesc acc; memset(&acc, 0, sizeof acc);
+        acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE; acc.location.id = dev; acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+        if (d.MemSetAccess(va, bytes, &acc, 1) != CUDA_SUCCESS) { d.MemUnmap(va, bytes); return false; }
+        return true;
+    }
+    void unmap_all(CUdeviceptr va) {
+        size_t off = 0;
+        for (const Chunk& c : chunks_) { drv().MemUnmap(va + off, c.bytes); off += c.bytes; }
+    }
+    // a new reservation of `bytes` holding the mapped chunks at the same offsets
+    bool move(size_t bytes, int dev, cudaStream_t st, std::string* err) {
+        DrvApi& d = drv();
+        // big ranges: 512 MB alignment lets the driver pick its largest page size (as vmm_map does)
+        const size_t align = bytes >= ((size_t)512 << 20) ? ((size_t)512 << 20) : 0;
+        if (align) bytes = (bytes + align - 1) / align * align;
+        CUdeviceptr va = 0;
+        if (d.MemAddressReserve(&va, bytes, align, 0, 0) != CUDA_SUCCESS) { *err = "cuMemAddressReserve failed"; return false; }
+        size_t off = 0;
+        for (size_t i = 0; i < chunks_.size(); i++) {
+            if (!map(va + off, chunks_[i].bytes, chunks_[i].h, dev)) {
+                for (size_t j = 0, o = 0; j < i; o += chunks_[j].bytes, j++) d.MemUnmap(va + o, chunks_[j].bytes);
+                d.MemAddressFree(va, bytes);
+                *err = "cuMemMap / cuMemSetAccess failed"; return false;
+            }
+            off += chunks_[i].bytes;
+        }
+        if (va_) {
+            cudaStreamSynchronize(st);
+            unmap_all(va_);
+            d.MemAddressFree(va_, reserved_);
+            moves_++;
+        }
+        va_ = va; reserved_ = bytes;
+        return true;
+    }
+    void take(GrowBuf& o) {
+        va_ = std::exchange(o.va_, 0); reserved_ = std::exchange(o.reserved_, 0); mapped_ = std::exchange(o.mapped_, 0);
+        gran_ = o.gran_; moves_ = o.moves_; chunks_ = std::move(o.chunks_); o.chunks_.clear();
+    }
+    CUdeviceptr va_ = 0;
+    size_t reserved_ = 0, mapped_ = 0, gran_ = 0;
+    int moves_ = 0;
+    std::vector<Chunk> chunks_;
+};
 
 // ---- file descriptors between the rank processes: abstract Unix-domain sockets + SCM_RIGHTS -----------------
 inline void uds_addr(const char* name, sockaddr_un* a, socklen_t* len) {

@@ -27,6 +27,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_train_step_idx_dev", "ctr_predict_idx_dev", "ctr_last_cost", "ctr_sync", "ctr_get_stream",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
+           "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys"]
@@ -353,6 +354,39 @@ class Engine:
         out = np.empty(a.size, np.int32)
         self._ck(self.L.ctr_idmap_lookup(self.h, C.c_int(which), a.ctypes.data_as(_lp), C.c_int64(a.size), out.ctypes.data_as(_ip)))
         return out
+
+    def idmap_insert(self, which, ids):
+        """Adds ids to a live map (ctr_idmap_insert): ids it lacks get the next rows in order of first occurrence, ids it
+        holds keep theirs.  Returns the row of every id.  With the item map, extends `item_ids` (the row -> id list
+        serving.Recommend maps rows back through) when the engine carries one."""
+        a = np.ascontiguousarray(ids, np.int64)
+        out = np.empty(a.size, np.int32)
+        self._ck(self.L.ctr_idmap_insert(self.h, C.c_int(which), a.ctypes.data_as(_lp), C.c_int64(a.size), out.ctypes.data_as(_ip)))
+        known = getattr(self, "item_ids", None)
+        if which == IDMAP_ITEM and known is not None:
+            known = np.asarray(known, np.int64)
+            fresh = out >= known.size
+            if fresh.any():
+                new_rows, first = np.unique(out[fresh], return_index=True)
+                self.item_ids = np.concatenate([known, a[fresh][first]])
+                assert self.item_ids.size == new_rows[-1] + 1
+        return out
+
+    def idmap_download(self, which):
+        """The ids of a map in row order (ctr_idmap_download): ids[r] is the id of row r."""
+        n = C.c_int64(0)
+        self._ck(self.L.ctr_idmap_download(self.h, C.c_int(which), None, C.c_int64(0), C.byref(n)))
+        out = np.empty(n.value, np.int64)
+        self._ck(self.L.ctr_idmap_download(self.h, C.c_int(which), out.ctypes.data_as(_lp), C.c_int64(n.value), C.byref(n)))
+        return out
+
+    def table_write_rows(self, which, rows, data):
+        """Writes rows of a live table in HBM (ctr_table_write_rows): row rows[i] = data[i]; a row past the end grows
+        the table (the gap reads as zero).  ITEM_EMB's written rows restart their row-Adam moments at zero."""
+        r, rp = _i(np.atleast_1d(rows))
+        d, dp = _f(data)
+        d = d.reshape(r.size, -1) if d.size else d.reshape(r.size, 0)
+        self._ck(self.L.ctr_table_write_rows(self.h, C.c_int(which), rp, dp, C.c_int64(r.size), C.c_int32(d.shape[1])))
 
     def item_emb_train(self, item_ids, cfg=None, **kw):
         """recommend.Train's embedding stage into ITEM_EMB (ctr_item_emb_train): item2vec over the int64 item stream,

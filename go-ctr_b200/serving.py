@@ -131,6 +131,32 @@ class UserBehaviorCache:
         return int((~keep).sum())
 
 
+class FeatureCache:
+    """The Set of UserFeatureCache / ItemFeatureCache (rcmd.go:25-26, 34-35) over the engine's live id maps and tables: a
+    user or item that was not there when the engine was set up gets a row and its features in HBM, so the next Rank /
+    BatchPredict / Recommend / train_keys sees it.  Setting a known id overwrites its row."""
+
+    def __init__(self, engine):
+        self.e = engine
+
+    def SetUser(self, userId, feature):
+        """The user's USER_FEAT row (uP floats); returns its row."""
+        row = self.e.idmap_insert(_e.IDMAP_USER, [int(userId)])
+        self.e.table_write_rows(_e.TABLE_USER_FEAT, row, np.asarray(feature, np.float32).reshape(1, -1))
+        return int(row[0])
+
+    def SetItem(self, itemId, feature, embedding=None):
+        """The item's ITEM_FEAT row (cF floats) and, when given, its ITEM_EMB row (D floats).  Without one a new item's
+        embedding reads as zeros until the next item2vec run, the reference's "embedding not found" (rcmd.go:501-505).
+        Returns its row."""
+        row = self.e.idmap_insert(_e.IDMAP_ITEM, [int(itemId)])
+        if self.e.cfg.cF > 0:
+            self.e.table_write_rows(_e.TABLE_ITEM_FEAT, row, np.asarray(feature, np.float32).reshape(1, -1))
+        if embedding is not None:
+            self.e.table_write_rows(_e.TABLE_ITEM_EMB, row, np.asarray(embedding, np.float32).reshape(1, -1))
+        return int(row[0])
+
+
 def load_id_maps(recSys, user_ids, item_ids):
     """user_ids[r] / item_ids[r] = external id of table row r (what the Go side's string-keyed caches hold,
     rcmd.go:472-505).  The item ids stay on the engine (item_ids) to map Recommend's rows back to ids."""

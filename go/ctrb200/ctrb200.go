@@ -196,6 +196,37 @@ func (e *Engine) DownloadUserBehavior() (offsets, ts []int64, itemRows []int32, 
 	return
 }
 
+// InsertIDs adds ids to a live id map (which: C.CTR_IDMAP_USER or C.CTR_IDMAP_ITEM; the map is created if none was
+// loaded).  Ids the map holds keep their rows; the others get the next rows in order of first occurrence.  Returns the
+// row of every id.
+func (e *Engine) InsertIDs(which int, ids []int64) ([]int32, error) {
+	if len(ids) == 0 {
+		return nil, nil
+	}
+	rows := make([]int32, len(ids))
+	return rows, e.err(C.ctr_idmap_insert(e.h, C.int(which), i64(ids), C.int64_t(len(ids)), i32(rows)))
+}
+
+// DownloadIDs returns a map's ids in row order (ids[r] is the id of row r): with LoadIDMaps, how a map grown by
+// InsertIDs is persisted and restored (checkpoints do not hold id maps).
+func (e *Engine) DownloadIDs(which int) ([]int64, error) {
+	var n C.int64_t
+	if err := e.err(C.ctr_idmap_download(e.h, C.int(which), nil, 0, &n)); err != nil {
+		return nil, err
+	}
+	ids := make([]int64, int(n))
+	return ids, e.err(C.ctr_idmap_download(e.h, C.int(which), i64n(ids), n, &n))
+}
+
+// WriteTableRows writes rows of a live table in HBM: row rows[i] becomes data[i*width : (i+1)*width].  A row past the
+// end grows the table in place (the gap reads as zero); ITEM_EMB's written rows restart their row-Adam moments at zero.
+func (e *Engine) WriteTableRows(which int, rows []int32, data []float32, width int) error {
+	if len(rows) == 0 || len(data) != len(rows)*width {
+		return fmt.Errorf("WriteTableRows: %d rows, %d floats, width %d", len(rows), len(data), width)
+	}
+	return e.err(C.ctr_table_write_rows(e.h, C.int(which), i32(rows), f32(data), C.int64_t(len(rows)), C.int32_t(width)))
+}
+
 // BatchPredict is recommend.BatchPredict (rcmd.go:277-337) over sample keys, entirely on the device.
 func (e *Engine) BatchPredict(sampleKeys []rcmd.Sample) ([]float32, error) {
 	n := len(sampleKeys)

@@ -237,6 +237,30 @@ int ctr_idmap_build(ctr_handle* h, int which, const int64_t* ids, int64_t n);
 int ctr_idmap_lookup(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows);
 int ctr_idmap_lookup_dev(ctr_handle* h, int which, const int64_t* d_ids, int64_t n, int32_t* d_rows);
 
+/* Live id maps and tables: a user or item that did not exist when the handle was set up gets a row and its features
+ * while the handle serves and trains, as the reference's feature caches fetch a new key's features on first use
+ * (rcmd.go:344-353, 472-492).  All three are single-GPU (world > 1: CTR_ESTATE), take the handle's mutex and run on the
+ * engine stream: work queued before sees the old state, work queued after the new one.  Arguments are validated before
+ * any device write, and a refused call changes nothing.
+ * insert: an id the map holds keeps its row; the ids it lacks get rows idmap_n, idmap_n + 1, ... in the order of their
+ *   first occurrence in ids (a repeated id gets one row).  rows (may be NULL) receives the row of every ids[i].  No map:
+ *   the call creates one, which on distinct ids equals ctr_idmap_build.  CTR_EINVAL: NULL ids, n outside [1, 2^31), a bad
+ *   which, INT64_MIN anywhere in ids, or more than INT32_MAX ids in all.  The load factor stays <= 0.5: a map that
+ *   outgrows its table is rehashed into one of the capacity ctr_idmap_build picks for the new count.
+ * download: *n = the id count; ids (may be NULL) [cap] receives the id of every row, ids[r] = the id of row r.  A
+ *   non-NULL ids with cap < *n is CTR_EINVAL, no map is CTR_ESTATE.  Checkpoints do not hold id maps: download +
+ *   ctr_idmap_build is how a map grown live is persisted and restored.
+ * write_rows: row rows[i] of table `which` becomes data[i] (data [n, width], width = the table's model dimension), bit
+ *   for bit.  CTR_EINVAL: a row outside [0, INT32_MAX) or the same row twice.  A row at or past the end grows the table
+ *   to max(rows) + 1 rows; the rows in between are zero (a missing row reads as zero anyway).  No table: the call creates
+ *   one.  Tables grow in place (reserved address space, memory mapped in chunks), without a second copy of the table.
+ *   ITEM_EMB: written and new rows get zero row-Adam moments, every other row keeps its moments; the step counter,
+ *   the dense weights and every other row are unchanged (ctr_table_upload, by contrast, resets the solver state).
+ *   Host data is staged in chunks; the caller's buffers may be pageable. */
+int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows);
+int ctr_idmap_download(ctr_handle* h, int which, int64_t* ids, int64_t cap, int64_t* n);
+int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const float* data, int64_t n, int32_t width);
+
 /* recommend.BatchPredict (rcmd.go:277-337) over sample keys {UserId, ItemId, Timestamp} (rcmd.go:189-194),
  * entirely on the device: id maps → rows, ubcache window at the sample's timestamp → history rows,
  * forward → scores [n].  Needs both id maps; without an uploaded ubcache the history is empty (the
