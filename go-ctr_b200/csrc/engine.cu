@@ -182,8 +182,9 @@ struct ctr_handle {
     DevBuf<long long> k_keys; PinnedBuf<unsigned char> k_host; DevBuf<int> k_flags;   // staging for ctr_batch_predict_keys (device, pinned host)
 
     // grow-only device scratch of the host-buffer entry points (gather / window / id lookup; slot 3: ctr_knn_search;
-    // slot 4: ctr_recommend_topk; slot 5: ubcache append / set): no cudaMalloc on the serving path
-    static constexpr int kScratch = 6;
+    // slot 4: ctr_recommend_topk; slot 5: ubcache append / set; slot 6: ctr_mlp_recommend_topk): no cudaMalloc on the
+    // serving path
+    static constexpr int kScratch = 7;
     DevBuf<unsigned char> scratch[kScratch];
 
     Comm comm;
@@ -2448,8 +2449,8 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     const int max_slices = (Bc + rps - 1) / rps;
     const int nex = exclude_history ? S : 0;
-    const size_t ssmem = rec::scan_smem_bytes(k, nex), msmem = knn::smem_bytes<knn::LogitKey>(1, 0, k);
-    CU(h, cudaFuncSetAttribute(rec::k_rec_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+    const size_t ssmem = rec::scan_smem_bytes<knn::LogitKey>(k, nex), msmem = knn::smem_bytes<knn::LogitKey>(1, 0, k);
+    CU(h, cudaFuncSetAttribute(rec::k_rec_scan<knn::LogitKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
     const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
 
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -2494,7 +2495,7 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
                 const int slices = (nb + rps - 1) / rps;
                 const bool first = c == 0, last = c == nchunks - 1;
                 RET(launch(h, "rec_topk", [&] {
-                    rec::k_rec_scan<<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, W, coll ? h->comm.rank : 0, rps, uh, nex, k,
+                    rec::k_rec_scan<knn::LogitKey><<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, W, coll ? h->comm.rank : 0, rps, uh, nex, k,
                                                                                 first ? nullptr : d_sl_s, first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
                 }));
                 // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
@@ -2517,7 +2518,7 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
                 knn::k_knn_merge<knn::LogitKey><<<ng, knn::kThreads, msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, d_lr, d_ls, nullptr);
             }));
         }
-        RET(launch(h, "rec_finish", [&] { rec::k_rec_finish<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
+        RET(launch(h, "rec_finish", [&] { rec::k_rec_finish<knn::LogitKey><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
         CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
         if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -3526,6 +3527,141 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
     }
     return CTR_OK;
 }
+
+// ctr_mlp_recommend_topk (see mlp64.cuh): per user, the prefix of layer 0 once; per chunk of items, layer 0 from it,
+// the later layers, and the selection of rec.cuh on the float64 logits.  Everything runs on h's stream.
+int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
+                  int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
+    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "recommend before fit");
+    MCU(m, cudaStreamSynchronize(m->stream));                            // h's stream reads the parameters
+    const int L = m->d.n_layers, H = m->d.units[1];
+    if (m->d.units[L - 1] != 1) return mlp_err(m, CTR_ESTATE, "recommendation ranks one output unit, the network has %d", m->d.units[L - 1]);
+    const int T_E = CTR_TABLE_ITEM_EMB, T_F = CTR_TABLE_ITEM_FEAT;
+    const int64_t N = h->tab_rows[T_E];
+    if (N > INT32_MAX) return mlp_err(m, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+    const ctr_config& c = h->cfg;
+    const int S = c.S, D = c.D, cF = c.cF, pcols = c.uP + S * D, T = D + cF;
+    int optin = 0;
+    MCU(m, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->dev));
+    // W0's item rows stay in shared memory when they fit beside the item tile; else they are read through L1
+    const bool smem_w = rec_layer0_smem(T, H, true) <= (size_t)optin;
+    const size_t l0smem = rec_layer0_smem(T, H, smem_w);
+    if (l0smem > (size_t)optin)
+        return mlp_err(m, CTR_ESTATE, "D + cF = %d item columns: a tile of %d items needs %zu bytes of shared memory (> %d)", T, kRecTile, l0smem, optin);
+
+    // ---- every user id, resolved before anything is written
+    const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy
+    const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
+    // items per chunk: pred_batch in whole tiles, at most the table.  The chunk's activations take
+    // Bc · (units[1] + … + units[L-1]) · 8 bytes of the classifier's buffers: a large catalogue wants a large pred_batch.
+    auto tiles = [](int64_t x) { return std::max<int64_t>((x + kRecTile - 1) / kRecTile, 1) * kRecTile; };
+    const int Bc = (int)std::min(tiles(c.pred_batch), tiles(N));
+    const int max_slices = (Bc + rps - 1) / rps;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t gk = (size_t)G * k, sl = (size_t)(1 + max_slices) * k;
+    const size_t b_id = al((size_t)nu * 8), b_ur = al((size_t)nu * 4), b_ts = al((size_t)G * 8), b_h = al((size_t)G * S * 4),
+                 b_pre = al((size_t)H * 8), b_sl = al(sl * 8), b_slr = al(sl * 4), b_l = al(gk * 8), b_lr = al(gk * 4), b_c = al((size_t)G * 4);
+    char* p = nullptr;
+    RET(scratch_get(h, 6, b_id + b_ur + b_ts + b_h + b_pre + b_sl + b_slr + 3 * b_l + 2 * b_lr + b_c, (void**)&p));
+    long long* d_ids = (long long*)p;      p += b_id;
+    int* d_urow = (int*)p;                 p += b_ur;
+    long long* d_ts = (long long*)p;       p += b_ts;
+    int* d_hist = (int*)p;                 p += b_h;
+    double* d_pre = (double*)p;            p += b_pre;
+    double* d_sl_s = (double*)p;           p += b_sl;      // [0, k): the user's running list, then the chunk's slice lists
+    int* d_sl_r = (int*)p;                 p += b_slr;
+    double* d_ls = (double*)p;             p += b_l;       // [G][k] the users' final lists
+    double* d_ol = (double*)p;             p += b_l;
+    float* d_os = (float*)p;               p += b_l;
+    int* d_lr = (int*)p;                   p += b_lr;
+    int* d_or = (int*)p;                   p += b_lr;
+    int* d_oc = (int*)p;
+    CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)nu * 8, cudaMemcpyHostToDevice, h->stream));
+    RET(launch(h, "mlp_rec_resolve", [&] {
+        k_idmap_lookup<<<mlp_grid(m, (long)nu), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, d_ids, (long)nu, d_urow);
+    }));
+    std::vector<int> urow((size_t)nu);
+    CU(h, cudaMemcpyAsync(urow.data(), d_urow, (size_t)nu * 4, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    for (int64_t u = 0; u < nu; u++)                                     // serving.Recommend's rule: the first unknown user
+        if (urow[(size_t)u] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[u]);
+
+    // ---- the classifier's activation buffers for one chunk; the last holds the logits
+    for (int l = 1; l < L; l++) {
+        const size_t need = (size_t)Bc * m->d.units[l];
+        if (m->act[l].size() < need) MCU(m, m->act[l].alloc(need));
+    }
+    const size_t ssmem = rec::scan_smem_bytes<knn::Logit64Key>(k, exclude_history ? S : 0), msmem = knn::smem_bytes<knn::Logit64Key>(1, 0, k);
+    CU(h, cudaFuncSetAttribute(rec::k_rec_scan<knn::Logit64Key>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+    CU(h, cudaFuncSetAttribute(knn::k_knn_merge<knn::Logit64Key>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem));
+    auto l0 = smem_w ? k_mlp64_rec_layer0<true> : k_mlp64_rec_layer0<false>;
+    CU(h, cudaFuncSetAttribute(l0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l0smem));
+    int l0_per_sm = 0;
+    CU(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l0_per_sm, l0, 256, l0smem));
+    const int l0_ctas = m->num_sms * std::max(1, l0_per_sm);
+    const int nex = exclude_history ? S : 0;
+    const float* ufeat = h->tab[CTR_TABLE_USER_FEAT];
+    const float* emb = h->tab[T_E];
+    const long lde = h->tab_ld[T_E], ldu = h->tab_ld[CTR_TABLE_USER_FEAT];
+    const int n_emb = (int)N;
+    const int nchunks = (int)((N + Bc - 1) / Bc);
+    for (int64_t g0 = 0; g0 < nu; g0 += G) {
+        const int ng = (int)std::min<int64_t>(G, nu - g0);
+        // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys)
+        if (h->ub_off) {
+            CU(h, cudaMemcpyAsync(d_ts, ts + g0, sizeof(long long) * (size_t)ng, cudaMemcpyHostToDevice, h->stream));
+            RET(launch(h, "ubcache_window", [&] {
+                k_ub_window<<<grid_for_warps(h, ng), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow + g0, d_ts, ng, S, (long)h->ub_users, d_hist);
+            }));
+        } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)ng * S, h->stream));
+        for (int j = 0; j < ng; j++) {
+            const int u = urow[(size_t)(g0 + j)];
+            const int* uh = d_hist + (size_t)j * S;
+            const float* up = (c.uP > 0 && u < h->tab_rows[CTR_TABLE_USER_FEAT]) ? ufeat + (long)u * ldu : nullptr;
+            RET(launch(h, "mlp_rec_prefix", [&] {
+                k_mlp64_prefix<<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, emb, lde, n_emb, uh, S, D, d_pre);
+            }));
+            for (int ch = 0; ch < nchunks; ch++) {
+                const int i0 = ch * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
+                const int ctas = std::min(l0_ctas, (nb + kRecTile - 1) / kRecTile);
+                RET(launch(h, "mlp_rec_layer0", [&] {
+                    l0<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, emb, lde, h->tab[T_F], h->tab_ld[T_F], (long)h->tab_rows[T_F],
+                                                        D, cF, (long)i0, nb, m->act[1]);
+                }));
+                for (int l = 1; l + 1 < L; l++)                       // the output layer leaves the logits in act[L-1]
+                    RET(launch(h, "mlp_rec_layers", [&] {
+                        k_mlp64_layer<true><<<mlp_grid(m, (long)nb * m->d.units[l + 1]), 256, 0, h->stream>>>(m->params, m->d, l, nullptr, 0, nullptr,
+                                                                                                          m->act[l], m->act[l + 1], nb);
+                    }));
+                const int slices = (nb + rps - 1) / rps;
+                const bool first = ch == 0, last = ch == nchunks - 1;
+                RET(launch(h, "mlp_rec_topk", [&] {
+                    rec::k_rec_scan<knn::Logit64Key><<<slices, knn::kThreads, ssmem, h->stream>>>(m->act[L - 1], nb, i0, 1, 0, rps, uh, nex, k,
+                                                                                                first ? nullptr : d_sl_s, first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
+                }));
+                // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
+                const int ns = first ? slices : slices + 1;
+                RET(launch(h, "mlp_rec_merge", [&] {
+                    knn::k_knn_merge<knn::Logit64Key><<<1, knn::kThreads, msmem, h->stream>>>(
+                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, ns, k, (long)ns * k, k,
+                        last ? d_lr + (size_t)j * k : d_sl_r, last ? d_ls + (size_t)j * k : d_sl_s, nullptr);
+                }));
+            }
+            if (nchunks == 0)            // an empty table: an empty list
+                RET(launch(h, "mlp_rec_merge", [&] {
+                    knn::k_knn_merge<knn::Logit64Key><<<1, knn::kThreads, msmem, h->stream>>>(d_sl_s, d_sl_r, 0, k, 0, 0, d_lr + (size_t)j * k, d_ls + (size_t)j * k, nullptr);
+                }));
+        }
+        const long n = (long)ng * k;
+        RET(launch(h, "mlp_rec_finish", [&] { rec::k_rec_finish<knn::Logit64Key><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
+        CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_count + g0, d_oc, (size_t)ng * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));          // d_hist and the result buffers are reused by the next group
+    }
+    return CTR_OK;
+}
 }  // namespace
 
 int ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label,
@@ -3549,6 +3685,19 @@ int ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, con
     m->err.clear(); h->err.clear();
     int rc = mlp_keys_check(m, h);
     if (rc == CTR_OK) rc = mlp_predict_keys(m, h, user_ids, item_ids, ts, n, scores);
+    return mlp_keys_done(m, h, rc);
+}
+
+int ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
+                           int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
+    if (!m) return CTR_EINVAL;
+    if (!h || !user_ids || !ts || !out_rows || !out_scores || !out_count || nu < 1 || k < 1 || k > knn::kMaxK)
+        return mlp_err(m, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user ids and ts, non-null outputs)", knn::kMaxK);
+    std::lock_guard<std::mutex> lh(h->mu);
+    std::lock_guard<std::mutex> lm(m->mu);
+    m->err.clear(); h->err.clear();
+    int rc = mlp_keys_check(m, h);
+    if (rc == CTR_OK) rc = mlp_recommend(m, h, user_ids, ts, nu, k, exclude_history, out_rows, out_scores, out_logits, out_count);
     return mlp_keys_done(m, h, rc);
 }
 

@@ -54,6 +54,12 @@ struct LogitKey {
     __device__ static float empty() { return -__int_as_float(0x7f800000); }
     __device__ static bool qualifies(float s) { return s == s; }
 };
+// the float64 MLP's recommendation (ctr_mlp_recommend_topk): float64 output-layer logits, LogitKey's rule
+struct Logit64Key {
+    using T = double;
+    __device__ static double empty() { return -__longlong_as_double(0x7ff0000000000000ll); }
+    __device__ static bool qualifies(double s) { return s == s; }
+};
 
 // shared-memory layout of QT queries' top-k state
 template <class K>

@@ -15,8 +15,7 @@
 // order (k ascending), so the only differences against the CPU restatement are FMA contraction and libm ulps.
 // Parameter layout = the reference's packed vector (:459-463): per layer [intercepts(fo) | coefs(fi x fo row-major)].
 #pragma once
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "common.cuh"
 
 namespace ctr {
 
@@ -30,8 +29,19 @@ struct Mlp64Dims {
     int hidden_act;
 };
 
+__device__ __forceinline__ double mlp64_logistic(double z) { return 1.0 / (1.0 + exp(-z)); }   // :82-88
+// the activation of layer l+1 on its pre-activation z; the output layer (last) is logistic (out_activation :423-425)
+__device__ __forceinline__ double mlp64_act(double z, int hidden_act, bool last) {
+    if (last || hidden_act == MLP_ACT_LOGISTIC) z = mlp64_logistic(z);
+    else if (hidden_act == MLP_ACT_RELU) z = z < 0.0 ? 0.0 : z;             // :96-104
+    else if (hidden_act == MLP_ACT_TANH) z = tanh(-z);                       // :88-94 — the argument is negated
+    return z;
+}
+
 // hidden / output layer l -> l+1 for the m rows of the minibatch: out[r, j] = act(b[j] + sum_k in[r, k] * W[k, j]).
 // in == nullptr: layer 0 reads the dataset rows X[idx[r]] (the shuffled visiting order, basemlp64.go:788-808).
+// kLogit: the output layer writes its pre-activation z, the logit (ctr_mlp_recommend_topk ranks by it).
+template <bool kLogit = false>
 __global__ void __launch_bounds__(256)
 k_mlp64_layer(const double* __restrict__ params, Mlp64Dims d, int l, const double* __restrict__ X, long ldx, const long* __restrict__ idx,
               const double* __restrict__ in, double* __restrict__ out, int m) {
@@ -45,10 +55,126 @@ k_mlp64_layer(const double* __restrict__ params, Mlp64Dims d, int l, const doubl
         double z = 0.0;
         for (int k = 0; k < fi; k++) z += a[k] * W[(long)k * fo + j];
         z += b[j];                                                              // addIntercepts64 :205
-        if (last || d.hidden_act == MLP_ACT_LOGISTIC) z = 1.0 / (1.0 + exp(-z));   // :82-88, out_activation :423-425
-        else if (d.hidden_act == MLP_ACT_RELU) z = z < 0.0 ? 0.0 : z;             // :96-104
-        else if (d.hidden_act == MLP_ACT_TANH) z = tanh(-z);                       // :88-94 — the argument is negated
+        if (!(kLogit && last)) z = mlp64_act(z, d.hidden_act, last);
         out[t] = z;
+    }
+}
+
+// ---- ctr_mlp_recommend_topk: one user against every item row ------------------------------------------------------
+// Layer 0's input is [user_feat (uP) | S window rows (S·D) | item emb (D) | item feat (cF)]; only the last D + cF columns
+// depend on the item.  k_mlp64_layer's chain for output j is z = 0; z += a[k]·W0[k, j] for k ascending (one DFMA each);
+// z += b[j].  So the user's partial sum over the first pcols = uP + S·D columns is computed once (k_mlp64_prefix) and each
+// item continues the same chain from it over its own columns (k_mlp64_rec_layer0): the same DFMAs in the same order, so
+// the same bits as the predict route.  No DMMA: its accumulation order differs.
+
+// pre[j] = sum_{k < pcols} x[k]·W0[k, j], x = [USER_FEAT row urow | ITEM_EMB rows hist[0, S)], widened from float32 as
+// k_gather_rows<double> widens them.  A missing row (urow == nullptr, a history row outside [0, n_emb)) is zeros, and
+// its columns are walked like any other: 0·inf stays NaN, as on the predict route.
+__global__ void __launch_bounds__(128)
+k_mlp64_prefix(const double* __restrict__ params, Mlp64Dims d, const float* __restrict__ urow, int uP,
+               const float* __restrict__ emb, long lde, int n_emb, const int* __restrict__ hist, int S, int D, double* __restrict__ pre) {
+    const int fo = d.units[1];
+    const double* W = params + d.off[0] + fo;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < fo; j += gridDim.x * blockDim.x) {
+        double z = 0.0;
+        long k = 0;
+        for (int c = 0; c < uP; c++, k++) z += (urow ? (double)__ldg(urow + c) : 0.0) * W[k * fo + j];
+        for (int s = 0; s < S; s++) {
+            const int row = __ldg(hist + s);
+            const float* e = row_ok(row, n_emb) ? emb + (long)row * lde : nullptr;
+            for (int c = 0; c < D; c++, k++) z += (e ? (double)__ldg(e + c) : 0.0) * W[k * fo + j];
+        }
+        pre[j] = z;
+    }
+}
+
+constexpr int kRecTile = 128;    // items per tile: lane l of a warp owns items l, l + 32, l + 64, l + 96 of it
+constexpr int kRecJ = 4;         // hidden units a warp carries at a time
+// pitch (floats) of the tile's item columns in shared memory: odd, so the lanes' strided reads hit 32 distinct banks
+__host__ __device__ inline int rec_tile_pitch(int T) { return T | 1; }
+__host__ __device__ inline int rec_units_pad(int H) { return (H + kRecJ - 1) / kRecJ * kRecJ; }
+// dynamic shared memory: [T][Hp] float64 slice of W0 (SMEM_W only), then [kRecTile][pitch] float32 item columns
+__host__ inline size_t rec_layer0_smem(int T, int H, bool smem_w) {
+    return (smem_w ? (size_t)T * rec_units_pad(H) * 8 : 0) + (size_t)kRecTile * rec_tile_pitch(T) * 4;
+}
+
+// out[b, j] = act(pre[j] + sum_{c < T} x_b[c]·W0[pcols + c, j] + b[j]) for items b = row0 .. row0 + n - 1, T = D + cF,
+// x_b = [ITEM_EMB row | ITEM_FEAT row (zeros past n_ifeat)].  The output layer (a network without hidden layers) writes
+// the logit.  A CTA stages the W0 rows of the item columns once (SMEM_W; else they are read through L1), then walks
+// tiles of kRecTile items: the tile's columns are read from HBM once, coalesced, and each warp takes kRecJ units at a
+// time for all the tile's items, so a W0 value in shared memory is a broadcast and an item value a conflict-free read.
+template <bool SMEM_W>
+__global__ void __launch_bounds__(256)
+k_mlp64_rec_layer0(const double* __restrict__ params, Mlp64Dims d, const double* __restrict__ pre, int pcols,
+                   const float* __restrict__ emb, long lde, const float* __restrict__ ifeat, long ldi, long n_ifeat,
+                   int D, int cF, long row0, int n, double* __restrict__ out) {
+    extern __shared__ __align__(16) char smem_raw[];
+    const int H = d.units[1], Hp = rec_units_pad(H), T = D + cF, Tp = rec_tile_pitch(T);
+    const bool last = d.n_layers == 2;
+    const double* b = params + d.off[0];
+    const double* W = b + H + (long)pcols * H;                 // W0 rows pcols .. pcols + T - 1
+    double* ws = reinterpret_cast<double*>(smem_raw);
+    float* xs = reinterpret_cast<float*>(smem_raw + (SMEM_W ? (size_t)T * Hp * 8 : 0));
+    if (SMEM_W)
+        for (int i = threadIdx.x; i < T * Hp; i += blockDim.x) {
+            const int k = i / Hp, j = i - k * Hp;
+            ws[i] = j < H ? W[(long)k * H + j] : 0.0;
+        }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int ntiles = (n + kRecTile - 1) / kRecTile;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int b0 = t * kRecTile, nb = min(kRecTile, n - b0);
+        __syncthreads();                                        // the previous tile has been read
+        for (int i = threadIdx.x; i < kRecTile * T; i += blockDim.x) {
+            const int r = i / T, c = i - r * T;
+            float v = 0.0f;
+            if (r < nb) {
+                const long row = row0 + b0 + r;
+                if (c < D) v = __ldg(emb + row * lde + c);
+                else if (row < n_ifeat) v = __ldg(ifeat + row * ldi + (c - D));
+            }
+            xs[r * Tp + c] = v;
+        }
+        __syncthreads();
+        for (int j0 = warp * kRecJ; j0 < H; j0 += nw * kRecJ) {
+            double acc[4][kRecJ];
+#pragma unroll
+            for (int jj = 0; jj < kRecJ; jj++) {
+                const double p = j0 + jj < H ? pre[j0 + jj] : 0.0;
+#pragma unroll
+                for (int r = 0; r < 4; r++) acc[r][jj] = p;
+            }
+#pragma unroll 2
+            for (int k = 0; k < T; k++) {
+                double w[kRecJ];
+                if (SMEM_W) {
+                    const double2 w01 = *reinterpret_cast<const double2*>(ws + (size_t)k * Hp + j0);
+                    const double2 w23 = *reinterpret_cast<const double2*>(ws + (size_t)k * Hp + j0 + 2);
+                    w[0] = w01.x; w[1] = w01.y; w[2] = w23.x; w[3] = w23.y;
+                } else {
+#pragma unroll
+                    for (int jj = 0; jj < kRecJ; jj++) w[jj] = j0 + jj < H ? __ldg(W + (long)k * H + j0 + jj) : 0.0;
+                }
+#pragma unroll
+                for (int r = 0; r < 4; r++) {
+                    const double x = (double)xs[(lane + 32 * r) * Tp + k];
+#pragma unroll
+                    for (int jj = 0; jj < kRecJ; jj++) acc[r][jj] = fma(x, w[jj], acc[r][jj]);
+                }
+            }
+#pragma unroll
+            for (int r = 0; r < 4; r++) {
+                const int i = lane + 32 * r;
+                if (i >= nb) continue;
+#pragma unroll
+                for (int jj = 0; jj < kRecJ; jj++) {
+                    const int j = j0 + jj;
+                    if (j >= H) continue;
+                    const double z = acc[r][jj] + b[j];
+                    out[(long)(b0 + i) * H + j] = last ? z : mlp64_act(z, d.hidden_act, false);
+                }
+            }
+        }
     }
 }
 

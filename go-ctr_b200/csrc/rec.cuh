@@ -8,19 +8,23 @@
 //   k_rec_scan:   grid = slices of the chunk; each CTA writes the top-k of its slice as it stands (empty entries included)
 //   k_knn_merge<LogitKey>: merges the user's running list with the slices' lists
 //   k_rec_finish: the users' lists → rows (-1 past the count), logits and scores (0 past the count), counts
+// ctr_mlp_recommend_topk runs the same three kernels on the float64 MLP's logits, with Logit64Key.
 #pragma once
 #include "knn.cuh"
+#include "mlp64.cuh"
 
 namespace ctr {
 namespace rec {
 
 using knn::LogitKey;
+using knn::Logit64Key;
 using knn::kEmptyRow;
 using knn::kStep;
 using knn::kThreads;
 
 // dynamic shared memory of k_rec_scan: the list/buffer state plus the exclusion rows that fall into the slice
-__host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<LogitKey>(1, 0, k) + (size_t)nex * 4 + 16; }
+template <class K>
+__host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<K>(1, 0, k) + (size_t)nex * 4 + 16; }
 
 // z[b] is the logit of local row row0 + b, b < n; local row l is global row l·world + rank (a row-sharded ITEM_EMB; 1
 // and 0 otherwise).  excl[0, nex): global rows that must not be returned (duplicates and rows outside the table are
@@ -28,16 +32,18 @@ __host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<
 // beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row lies in an
 // earlier chunk, so the fillers are told apart by row and written back as empty entries.
 // Out: per slice the top-k list of global rows, [slices][k].
-__global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
+template <class K>
+__global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
                                                         const int* __restrict__ excl, int nex, int k,
-                                                        const float* run_s, const int* run_r,
-                                                        float* __restrict__ out_s, int* __restrict__ out_row) {
+                                                        const typename K::T* run_s, const int* run_r,
+                                                        typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
+    using T = typename K::T;
     extern __shared__ __align__(16) char smem_raw[];
-    const knn::Smem<LogitKey> sm = knn::carve<LogitKey>(smem_raw, 1, 0, k);
-    int* ex = reinterpret_cast<int*>(smem_raw + knn::smem_bytes<LogitKey>(1, 0, k));
+    const knn::Smem<K> sm = knn::carve<K>(smem_raw, 1, 0, k);
+    int* ex = reinterpret_cast<int*>(smem_raw + knn::smem_bytes<K>(1, 0, k));
     __shared__ int nx;
     const int r0 = blockIdx.x * rows_per_slice, r1 = min(n, r0 + rows_per_slice);
-    const float t_s = run_r ? run_s[k - 1] : LogitKey::empty();
+    const T t_s = run_r ? run_s[k - 1] : K::empty();
     const int t_r = run_r ? run_r[k - 1] : kEmptyRow;
     for (int i = threadIdx.x; i < k; i += kThreads) { sm.ls[i] = t_s; sm.lr[i] = t_r; }
     if (threadIdx.x == 0) { sm.bn[0] = 0; nx = 0; }
@@ -65,15 +71,20 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const float* __restrict__
     }
     for (int i = threadIdx.x; i < k; i += kThreads) {
         const bool filler = sm.lr[i] == t_r;
-        out_s[(size_t)blockIdx.x * k + i] = filler ? LogitKey::empty() : sm.ls[i];
+        out_s[(size_t)blockIdx.x * k + i] = filler ? K::empty() : sm.ls[i];
         out_row[(size_t)blockIdx.x * k + i] = filler ? kEmptyRow : sm.lr[i];
     }
 }
 
-// n = users * k list entries.  The score is sigmoid32 of the logit, the function k_head applies: bit-identical to the
-// score ctr_predict_idx returns for the same sample.
-__global__ void k_rec_finish(const float* __restrict__ ls, const int* __restrict__ lr, int k, long n,
-                             int32_t* __restrict__ out_row, float* __restrict__ out_logit, float* __restrict__ out_score,
+// the score of a logit, bit-identical to what the predict route returns for the same sample: sigmoid32, the function
+// k_head applies (ctr_predict_idx); the float64 MLP's logistic output narrowed to float32 (ctr_mlp_predict_keys)
+__device__ __forceinline__ float rec_score(float z) { return sigmoid32(z); }
+__device__ __forceinline__ float rec_score(double z) { return (float)mlp64_logistic(z); }
+
+// n = users * k list entries
+template <class K>
+__global__ void k_rec_finish(const typename K::T* __restrict__ ls, const int* __restrict__ lr, int k, long n,
+                             int32_t* __restrict__ out_row, typename K::T* __restrict__ out_logit, float* __restrict__ out_score,
                              int32_t* __restrict__ out_count) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -81,8 +92,8 @@ __global__ void k_rec_finish(const float* __restrict__ ls, const int* __restrict
     const int p = (int)(i - j * k);
     const bool v = lr[i] != kEmptyRow;
     out_row[i] = v ? lr[i] : -1;
-    out_logit[i] = v ? ls[i] : 0.0f;
-    out_score[i] = v ? sigmoid32(ls[i]) : 0.0f;
+    out_logit[i] = v ? ls[i] : typename K::T(0);
+    out_score[i] = v ? rec_score(ls[i]) : 0.0f;
     // valid entries are a prefix of the sorted list
     if (v && (p == k - 1 || lr[i + 1] == kEmptyRow)) out_count[j] = p + 1;
     if (!v && p == 0) out_count[j] = 0;

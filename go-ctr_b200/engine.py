@@ -30,7 +30,8 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
-           "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys"]
+           "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
+           "ctr_mlp_recommend_topk"]
 
 
 class CtrError(RuntimeError):
@@ -595,6 +596,23 @@ class MLPClassifier:
         self._ck(self.L.ctr_mlp_predict_keys(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
                                              C.c_int64(u.size), out.ctypes.data_as(_fp)))
         return out
+
+    def recommend_topk(self, engine, user_ids, ts, k, exclude_history=True):
+        """Top-k recommendation over every ITEM_EMB row of the feature store `engine` (ctr_mlp_recommend_topk): users
+        are external ids, each windowed at its ts (empty history without a ubcache).  Returns (rows [nu, k] int32, scores
+        [nu, k] float32, logits [nu, k] float64, counts [nu] int32), best first (logit descending, then row ascending);
+        positions past a user's count hold row -1, score 0 and logit 0.  Each score is bit for bit what predict_keys
+        returns for (user, the row's item id, ts).  An unknown user raises CtrError with code ENOTFOUND."""
+        u = np.atleast_1d(np.ascontiguousarray(user_ids, np.int64)); t = np.atleast_1d(np.ascontiguousarray(ts, np.int64))
+        if u.size != t.size:
+            raise ValueError("user_ids and ts differ in length: %d, %d" % (u.size, t.size))
+        out_r = np.empty((u.size, k), np.int32); out_s = np.empty((u.size, k), np.float32)
+        out_l = np.empty((u.size, k), np.float64); cnt = np.empty(u.size, np.int32)
+        self._ck(self.L.ctr_mlp_recommend_topk(self.h, engine.h, u.ctypes.data_as(_lp), t.ctypes.data_as(_lp), C.c_int64(u.size),
+                                               C.c_int32(k), C.c_int32(int(bool(exclude_history))), out_r.ctypes.data_as(_ip),
+                                               out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(C.POINTER(C.c_double)),
+                                               cnt.ctypes.data_as(_ip)))
+        return out_r, out_s, out_l, cnt
 
     def get_params(self):
         n = C.c_int64(0)

@@ -15,6 +15,7 @@ engine; the seam is Fitter / PredictAbstract + Train / Predict + the Marshal JSO
 (SURVEY.md §8b).  The Go binding of the same C ABI is go/ctrb200/ctrb200.go.
 """
 import json
+import time
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -229,12 +230,24 @@ class SimpleMlpPredWrap:
         return self.pred.predict(X).reshape(-1, 1)
 
     def batch_predict_keys(self, user_ids, item_ids, ts):
-        """Scores sample keys through the bound feature store (ctr_mlp_predict_keys), so serving.BatchPredict and
-        serving.Rank serve the MLP as they serve an engine.  serving.Recommend over the whole item table is not
-        available for the MLP: it needs the engine's own model."""
+        """Scores sample keys through the bound feature store (ctr_mlp_predict_keys), so serving.BatchPredict,
+        serving.Rank and serving.Recommend serve the MLP as they serve an engine."""
+        self._bound()
+        return self.pred.predict_keys(self.engine, user_ids, item_ids, ts)
+
+    def recommend(self, userId, k, now=None, exclude_history=True):
+        """The k best items of the bound feature store's whole ITEM_EMB table for one user at `now` (default: the
+        current time), scored by this MLP on the device (ctr_mlp_recommend_topk).  Returns (rows [n] int32, scores [n]
+        float32, logits [n] float64), best first, n <= k; serving.Recommend maps the rows to item ids."""
+        self._bound()
+        ts = int(time.time()) if now is None else int(now)
+        rows, scores, logits, cnt = self.pred.recommend_topk(self.engine, [int(userId)], [ts], k, exclude_history=exclude_history)
+        n = int(cnt[0])
+        return rows[0, :n], scores[0, :n], logits[0, :n]
+
+    def _bound(self):
         if self.engine is None:
             raise RuntimeError("this predictor was fitted from dense X: no feature store is bound (use FitKeys)")
-        return self.pred.predict_keys(self.engine, user_ids, item_ids, ts)
 
 
 class SimpleMlpFitWrap:
@@ -256,7 +269,7 @@ class SimpleMlpFitWrap:
         """rcmd.Train (rcmd.go:197-246) with this fitter, GetSample on the device: `engine` holds the id maps, the tables
         and optionally the ubcache; the sample width is its uP + S·D + D + cF.  Keys with an unknown user or item are
         dropped (Model.rows_used counts the rest).  Returns a SimpleMlpPredWrap bound to `engine`, which
-        serving.BatchPredict / serving.Rank accept in place of an engine; serving.Recommend does not serve the MLP."""
+        serving.BatchPredict / serving.Rank / serving.Recommend accept in place of an engine."""
         c = engine.cfg
         self.Model = _e.MLPClassifier(c.uP + c.S * c.D + c.D + c.cF, **self.mlp_kw)
         self.Model.fit_keys(engine, user_ids, item_ids, ts, label)

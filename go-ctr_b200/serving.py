@@ -9,6 +9,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import engine as _e
+from . import model as _m
 
 
 @dataclass
@@ -52,8 +53,14 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     On an engine whose ITEM_EMB is row-sharded over several GPUs the call is collective: every rank's process makes
     the same call (same user, k, now and history) and receives the same complete result (Engine.recommend_topk).
     A sharded deployment must pass `now` explicitly, the value broadcast with the request: the default reads each
-    process's own clock, so ranks can window different histories and then all fail with CTR_EINVAL."""
+    process's own clock, so ranks can window different histories and then all fail with CTR_EINVAL.
+    recSys may also be the SimpleMlpPredWrap that SimpleMlpFitWrap.FitKeys returns, main.go's model: its MLP scores
+    every ITEM_EMB row of the feature store it is bound to (ctr_mlp_recommend_topk), under the same rules."""
     ts = int(time.time()) if now is None else int(now)
+    if isinstance(recSys, _m.SimpleMlpPredWrap):
+        rows, scores, _ = recSys.recommend(userId, k, now=ts, exclude_history=exclude_history)
+        item_ids = recSys.engine.item_ids
+        return [ItemScore(int(item_ids[r]), float(s)) for r, s in zip(rows, scores)]
     row = int(recSys.idmap_lookup(_e.IDMAP_USER, [int(userId)])[0])
     if row < 0:
         raise _e.CtrError(_e.ENOTFOUND, "user %d is not found" % int(userId))

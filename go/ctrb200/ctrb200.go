@@ -705,3 +705,31 @@ func (p *MlpPredWrap) Rank(e *Engine, userId int, itemIds []int) ([]rcmd.ItemSco
 	}
 	return out, nil
 }
+
+// Recommend is the default recall of recommend/api.go's empty itemIdList (api.go:115-118) for the MLP: every ITEM_EMB
+// row of the feature store e scored for each user, windowed at ts[j], and the best k kept on the device (logit
+// descending, then row ascending).  outRows, scores and logits are [len(userIds)·k]; counts[j] results of user j are
+// valid.  Each score is what BatchPredict returns for (user, the row's item id, ts[j]).  An unknown user is an error.
+func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, excludeHistory bool) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
+	nu := len(userIds)
+	if nu == 0 || k < 1 || len(ts) != nu {
+		return nil, nil, nil, nil, fmt.Errorf("MlpPredWrap.Recommend needs at least one user, one ts per user and k >= 1")
+	}
+	u := make([]int64, nu)
+	for i, id := range userIds {
+		u[i] = int64(id)
+	}
+	ex := C.int32_t(0)
+	if excludeHistory {
+		ex = 1
+	}
+	outRows = make([]int32, nu*k)
+	scores = make([]float32, nu*k)
+	logits = make([]float64, nu*k)
+	counts = make([]int32, nu)
+	if rc := C.ctr_mlp_recommend_topk(p.m, e.h, i64(u), i64(ts), C.int64_t(nu), C.int32_t(k), ex, i32(outRows), f32(scores),
+		(*C.double)(unsafe.Pointer(&logits[0])), i32(counts)); rc != C.CTR_OK {
+		return nil, nil, nil, nil, fmt.Errorf("ctr_mlp_recommend_topk: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+	}
+	return outRows, scores, logits, counts, nil
+}

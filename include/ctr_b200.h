@@ -494,6 +494,24 @@ int  ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const 
                       const float* label, int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used);
 int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
                           int64_t n, float* scores);
+/* Top-k recommendation over the whole item table with the classifier: the default recall recommend/api.go leaves as a
+ * todo (api.go:115-118), for main.go's model.  h is the feature store, as for ctr_mlp_predict_keys.
+ *   Users are external ids (h's user map); user j's history is GetUserBehavior(uid, S, -1, ts[j]) from the device
+ *     ubcache, empty without one.  Every ITEM_EMB row is scored, as ctr_recommend_topk scores them; a missing ITEM_FEAT
+ *     row reads as zeros.  Each item's score is bit for bit what ctr_mlp_predict_keys returns for (user, the item's id,
+ *     ts[j]): the user's part of layer 0 is computed once and each item continues the same float64 chain.
+ *   Order: output-layer logit (before the logistic) descending, then row ascending; a NaN logit never qualifies.
+ *     exclude_history skips the rows of the user's window.  out_rows / out_scores (float32 probabilities) / out_logits
+ *     (float64, may be NULL) are [nu, k]; out_count[j] may be less than k, and positions at or past it hold row -1,
+ *     score 0 and logit 0.
+ *   Refusals write nothing: CTR_EINVAL for k outside [1, 1024], nu < 1, null inputs or outputs and ctr_mlp_predict_keys'
+ *     argument refusals; CTR_ESTATE for a classifier not fitted or with more than one output, a missing id map or table,
+ *     or world > 1; CTR_ENOTFOUND for any unknown user id, naming the first.
+ *   Items are scored in chunks of h's pred_batch (whole tiles of 128) in the classifier's activation buffers,
+ *     pred_batch · (units[1] + … + units[L-1]) · 8 bytes: a large catalogue wants a large pred_batch.  Only nu·k
+ *     results cross PCIe.  Locking: h's mutex, then m's. */
+int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k,
+                            int32_t exclude_history, int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count);
 /* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the length */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
