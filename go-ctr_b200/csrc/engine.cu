@@ -3118,6 +3118,11 @@ struct ctr_mlp {
     // key-fed fit / predict: [rows, nin] float64 inputs a feature store gathers (two, so minibatch k+1 is gathered on the
     // store's stream while k trains); stage_free[s]: the minibatch that last read stage[s] is done; stage_full[s]: gathered
     DevBuf<double> stage[2]; Event stage_free[2], stage_full[2];
+    // LabelBinarizer64.Classes (basemlp64.go:1294-1313): empty for labels all 0 or 1 (no binarizer, one logistic output).
+    // Otherwise the output width is max(1, classes.size()) and predictions are class labels.  class_dev mirrors it.
+    std::vector<double> classes;
+    DevBuf<double> class_dev;                                         // [kMlpMaxClasses]
+    DevBuf<int> cls;                                                  // [n] the class index of each sample of the last fit
     double adam_calls = 0;                                           // AdamOptimizer64.t
     double t = 0;                                                     // BaseMultilayerPerceptron64.t: samples since initialize (:412,814)
     bool fitted = false;
@@ -3156,12 +3161,79 @@ int mlp_upload_x(ctr_mlp* m, const float* X, int64_t n, int nin) {
     }
     return rc;
 }
-// forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads the [*, nin] matrix X through idx (may be null = identity)
+// forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads the [*, nin] matrix X through idx (may be null = identity).
+// More than one output column: the output layer keeps its pre-activations and a softmax follows (:504-511).
 void mlp_forward(ctr_mlp* m, const double* X, const long* idx, int rows) {
-    const int L = m->d.n_layers, nin = m->d.units[0];
+    const int L = m->d.n_layers, nin = m->d.units[0], no = m->d.units[L - 1];
+    auto layer = no > 1 ? k_mlp64_layer<true> : k_mlp64_layer<false>;
     for (int l = 0; l + 1 < L; l++)
-        k_mlp64_layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, X, nin, idx,
-                                                                                      l == 0 ? nullptr : m->act[l].get(), m->act[l + 1], rows);
+        layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, X, nin, idx,
+                                                                              l == 0 ? nullptr : m->act[l].get(), m->act[l + 1], rows);
+    if (no > 1) k_mlp64_softmax<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, no);
+}
+// the float32 [rows] answer of predict from the output layer: the probability, or with classes the class label (:917-931)
+void mlp_output(ctr_mlp* m, int rows, float* out) {
+    const int L = m->d.n_layers;
+    if (m->classes.empty()) k_f64_to_f32<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], out, rows);
+    else k_mlp64_predict_label<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, m->d.units[L - 1], m->class_dev, out);
+}
+// installs the classes (empty: binary) and the output width they imply; parameters, gradients and moments are
+// reallocated, zero, when the width changes, and the model then counts as not fitted.  Nothing changes on a failure.
+int mlp_set_head(ctr_mlp* m, const std::vector<double>& classes) {
+    const int L = m->d.n_layers, no = std::max<int>(1, (int)classes.size());
+    const long np = m->d.off[L - 2] + (long)(1 + m->d.units[L - 2]) * no;
+    DevBuf<double> b[4];
+    if (no != m->d.units[L - 1])
+        for (DevBuf<double>& x : b) { MCU(m, x.alloc((size_t)np)); MCU(m, cudaMemsetAsync(x, 0, sizeof(double) * (size_t)np, m->stream)); }
+    if (!classes.empty() && !m->class_dev) MCU(m, m->class_dev.alloc(kMlpMaxClasses));
+    if (!classes.empty()) MCU(m, cudaMemcpyAsync(m->class_dev, classes.data(), sizeof(double) * classes.size(), cudaMemcpyHostToDevice, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    if (no != m->d.units[L - 1]) {
+        m->params = std::move(b[0]); m->grads = std::move(b[1]); m->ms = std::move(b[2]); m->vs = std::move(b[3]);
+        m->d.units[L - 1] = no;
+        m->np = np;
+        m->fitted = false;
+    }
+    m->classes = classes;
+    return CTR_OK;
+}
+// BaseMultilayerPerceptron64.Fit's label handling (basemlp64.go:578-598) over the n labels Y of a fit, on the device:
+// isBinarized64 (:1378-1388) and LabelBinarizer64.Fit (:1294-1313).  At a cold initialise the head follows the labels;
+// a warm start keeps it and refuses labels whose class set differs.  With classes, *cls = each sample's class index
+// (m->cls), else null.  The host reads the class count back once.  A refusal changes nothing.
+int mlp_labels(ctr_mlp* m, const float* Y, long n, const int** cls) {
+    *cls = nullptr;
+    size_t t_sort = 0, t_uniq = 0;
+    MCU(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (const float*)nullptr, (float*)nullptr, (const long*)nullptr, (long*)nullptr, n, 0, 32, m->stream));
+    MCU(m, cub::DeviceSelect::UniqueByKey(nullptr, t_uniq, (const float*)nullptr, (const long*)nullptr, (float*)nullptr, (long*)nullptr, (long*)nullptr, n, m->stream));
+    DevBuf<float> k0, k1; DevBuf<long> p0, p1; DevBuf<char> tmp; DevBuf<Mlp64Classes> res;
+    MCU(m, k0.alloc((size_t)n)); MCU(m, k1.alloc((size_t)n)); MCU(m, p0.alloc((size_t)n)); MCU(m, p1.alloc((size_t)n));
+    MCU(m, tmp.alloc(std::max(t_sort, t_uniq))); MCU(m, res.alloc(1));
+    MCU(m, cudaMemsetAsync(res, 0, sizeof(Mlp64Classes), m->stream));
+    k_mlp64_label_keys<<<mlp_grid(m, n), 256, 0, m->stream>>>(Y, n, k0, p0, res);
+    MCU(m, cub::DeviceRadixSort::SortPairs(tmp.get(), t_sort, k0.get(), k1.get(), p0.get(), p1.get(), n, 0, 32, m->stream));
+    // the stable sort leaves each class's first position at the head of its run; the unique keys go to k0, their positions to p0
+    MCU(m, cub::DeviceSelect::UniqueByKey(tmp.get(), t_uniq, k1.get(), p1.get(), k0.get(), p0.get(), &res.get()->count, n, m->stream));
+    k_mlp64_class_values<<<kMlpMaxClasses / 256, 256, 0, m->stream>>>(Y, p0, res);
+    std::unique_ptr<Mlp64Classes> r(new Mlp64Classes);
+    MCU(m, cudaMemcpyAsync(r.get(), res, sizeof(Mlp64Classes), cudaMemcpyDeviceToHost, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    MCU(m, cudaGetLastError());
+    if (r->nan) return mlp_err(m, CTR_EINVAL, "a label is NaN: the classes would be ill-defined (DESIGN.md §2)");
+    if (r->count > kMlpMaxClasses) return mlp_err(m, CTR_EINVAL, "%ld distinct labels: at most %d classes", r->count, kMlpMaxClasses);
+    std::vector<double> classes(r->value, r->value + r->count);
+    if (std::all_of(classes.begin(), classes.end(), [](double v) { return v == 0.0 || v == 1.0; })) classes.clear();   // isBinarized64
+    if (m->cfg.warm_start && m->fitted) {                                // the head is kept; the binarizer is refitted (:592-597)
+        const bool same = classes.size() == m->classes.size() && std::equal(classes.begin(), classes.end(), m->classes.begin());
+        if (!same) return mlp_err(m, CTR_EINVAL, "warm start: the labels have %zu classes%s, the fitted model %zu (0 = labels in {0, 1}); the classes must match",
+                                  classes.size(), classes.size() == m->classes.size() ? " of other values" : "", m->classes.size());
+    }
+    if (!classes.empty() && m->cls.size() < (size_t)n) MCU(m, m->cls.alloc((size_t)n));
+    RET(mlp_set_head(m, classes));
+    if (classes.empty()) return CTR_OK;
+    k_mlp64_class_index<<<mlp_grid(m, n), 256, 0, m->stream>>>(Y, n, m->class_dev, (int)classes.size(), m->cls);
+    *cls = m->cls;
+    return CTR_OK;
 }
 // the two [rows, nin] staging buffers and their events of the key-fed entry points (grow-only; events made once)
 int mlp_stage(ctr_mlp* m, long rows) {
@@ -3196,10 +3268,11 @@ int mlp_init_params(ctr_mlp* m) {
 // Layer 0's input of minibatch k (0-based within the epoch), whose samples are bi[0, rows): *X = a [rows, nin] matrix
 // read row by row, or left null to read X64 through bi (ctr_mlp_fit).
 using MlpInput = std::function<int(long k, const long* bi, int rows, const double** X)>;
-// fitStochastic (basemlp64.go:729-857) over n samples with the device labels Y [n], in minibatches of bs: a fresh optimizer,
+// fitStochastic (basemlp64.go:729-857) over n samples with the device labels Y [n] (binary) or class indices cls [n]
+// (mlp_labels; cls non-null), in minibatches of bs: a fresh optimizer,
 // the per-epoch shuffle, the solvers, weight decay, the stopping rules and the t carry.  Only layer 0's input differs
 // between the callers (input may be empty).  m->idx holds n entries and the activations bs rows.
-int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const MlpInput& input, int32_t* n_iter, double* loss_curve) {
+int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const int* cls, const MlpInput& input, int32_t* n_iter, double* loss_curve) {
     const ctr_mlp_config& c = m->cfg;
     const int nin = m->d.units[0];
     const ctr_mlp_options& o = m->opts;
@@ -3229,7 +3302,8 @@ int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const MlpInput& inpu
             if (o.weight_decay > 0.0)                                    // backprop :342-346
                 k_mlp64_decay<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->np, 1.0 - o.weight_decay);
             mlp_forward(m, X0, xi, rows);
-            k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
+            if (cls) k_mlp64_loss_cls<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], cls, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
+            else k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
             for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
                 k_mlp64_grads<<<mlp_grid(m, (long)(m->d.units[l] + 1) * m->d.units[l + 1]), 256, 0, m->stream>>>(
                     m->params, m->grads, m->d, l, X0, nin, xi, l == 0 ? nullptr : m->act[l].get(), m->del[l + 1], rows, c.alpha);
@@ -3365,6 +3439,32 @@ int ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np) {
     return CTR_OK;
 }
 
+int ctr_mlp_get_classes(ctr_mlp* m, double* classes, int32_t cap, int32_t* n) {
+    if (!m) return CTR_EINVAL;
+    std::lock_guard<std::mutex> lk(m->mu);
+    const int32_t c = (int32_t)m->classes.size();
+    if (n) *n = c;
+    if (!classes) return CTR_OK;
+    if (cap < c) return mlp_err(m, CTR_EINVAL, "class buffer too small: need %d", c);
+    std::copy(m->classes.begin(), m->classes.end(), classes);
+    return CTR_OK;
+}
+// the arguments are checked before the handle, so a refusal's message is readable through ctr_mlp_last_error(m) (or
+// ctr_mlp_last_error(NULL) when m is null)
+int ctr_mlp_set_classes(ctr_mlp* m, const double* classes, int32_t n) {
+    if (n < 0 || n > kMlpMaxClasses || (n > 0 && !classes)) return mlp_err(m, CTR_EINVAL, "n = %d classes: in [0, %d], non-null when n > 0", n, kMlpMaxClasses);
+    for (int32_t i = 0; i < n; i++) {
+        if (std::isnan(classes[i])) return mlp_err(m, CTR_EINVAL, "class %d is NaN", i);
+        if (i > 0 && !(classes[i - 1] < classes[i])) return mlp_err(m, CTR_EINVAL, "the classes must be strictly ascending (class %d)", i);
+    }
+    if (!m) return mlp_err(nullptr, CTR_EINVAL, "null classifier");
+    std::lock_guard<std::mutex> lk(m->mu);
+    MCU(m, cudaSetDevice(m->dev));
+    RET(mlp_set_head(m, std::vector<double>(classes, classes + n)));
+    m->fitted = false;
+    return CTR_OK;
+}
+
 int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, int32_t* n_iter, double* loss_curve) {
     if (!m || !X || !Y || n < 1) return mlp_err(m, CTR_EINVAL, "bad fit arguments");
     std::lock_guard<std::mutex> lk(m->mu);
@@ -3376,16 +3476,18 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
     if (m->Y32.size() < (size_t)n) MCU(m, m->Y32.alloc((size_t)n));
     if (m->idx.size() < (size_t)n) MCU(m, m->idx.alloc((size_t)n));
     MCU(m, cudaMemcpyAsync(m->Y32, Y, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
+    const int* cls = nullptr;
+    RET(mlp_labels(m, m->Y32, n, &cls));
     RET(mlp_rows(m, bs));
     RET(mlp_init_params(m));
-    return mlp_epochs(m, n, bs, m->Y32, MlpInput(), n_iter, loss_curve);
+    return mlp_epochs(m, n, bs, m->Y32, cls, MlpInput(), n_iter, loss_curve);
 }
 
 int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float* out) {
     if (!m || !X || !out || n < 1) return mlp_err(m, CTR_EINVAL, "bad predict arguments");
     std::lock_guard<std::mutex> lk(m->mu);
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
-    const int nin = m->d.units[0], L = m->d.n_layers;
+    const int nin = m->d.units[0];
     if (xcols != nin) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, nin);
     MCU(m, cudaSetDevice(m->dev));
     RET(mlp_upload_x(m, X, n, nin));
@@ -3394,10 +3496,10 @@ int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float*
     DevBuf<float> d_out;
     MCU(m, d_out.alloc((size_t)std::min<long>(chunk, n)));
     int rc = CTR_OK;
-    for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predictProbas :897-931: raw probabilities for the f64 class
+    for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predict :917-931: raw probabilities for the f64 class, or class labels
         const int rows = (int)std::min<long>(chunk, n - r0);
         mlp_forward(m, m->X64 + r0 * nin, nullptr, rows);
-        k_f64_to_f32<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], d_out, rows);
+        mlp_output(m, rows, d_out);
         if (cudaMemcpyAsync(out + r0, d_out, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, m->stream) != cudaSuccess ||
             cudaStreamSynchronize(m->stream) != cudaSuccess) rc = mlp_err(m, CTR_ECUDA, "predict: %s", cudaGetErrorString(cudaGetLastError()));
     }
@@ -3464,9 +3566,11 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
     // ---- the classifier: minibatch k's rows are gathered on h's stream into stage[k & 1] while minibatch k-1 trains
     const long bs = mlp_batch(m, ns);
     if (m->idx.size() < (size_t)ns) MCU(m, m->idx.alloc((size_t)ns));
-    RET(mlp_rows(m, bs));
     RET(mlp_stage(m, bs));
     RET(mlp_after_store(m, h, 0));                                     // labels and windows before the first loss
+    const int* cls = nullptr;
+    RET(mlp_labels(m, h->kt_label, ns, &cls));                          // the survivors' labels
+    RET(mlp_rows(m, bs));
     RET(mlp_init_params(m));
     const RowSrc r = idx_src(h, h->kt_user, h->kt_item, h->kt_hist_all, (int)ns);
     const int nin = m->d.units[0];
@@ -3484,12 +3588,12 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
         *X = m->stage[s];
         return CTR_OK;
     };
-    return mlp_epochs(m, ns, bs, h->kt_label, input, n_iter, loss_curve);
+    return mlp_epochs(m, ns, bs, h->kt_label, cls, input, n_iter, loss_curve);
 }
 
 int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
-    const int B = h->cfg.pred_batch, S = h->cfg.S, nin = m->d.units[0], L = m->d.n_layers;
+    const int B = h->cfg.pred_batch, S = h->cfg.S, nin = m->d.units[0];
     RET(keys_stage_init(h));
     RET(mlp_rows(m, B));
     RET(mlp_stage(m, B));
@@ -3516,7 +3620,7 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
         }));
         RET(mlp_after_store(m, h, 0));
         mlp_forward(m, m->stage[0], nullptr, nb);
-        k_f64_to_f32<<<mlp_grid(m, nb), 256, 0, m->stream>>>(m->act[L - 1], d_out, nb);
+        mlp_output(m, nb, d_out);
         MCU(m, cudaMemcpyAsync(hs, d_out, sizeof(float) * (size_t)nb, cudaMemcpyDeviceToHost, m->stream));
         MCU(m, cudaStreamSynchronize(m->stream));                      // the next chunk's gather overwrites stage[0]
         CU(h, cudaStreamSynchronize(h->stream));
@@ -3533,6 +3637,8 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
 int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
                   int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "recommend before fit");
+    if (!m->classes.empty())
+        return mlp_err(m, CTR_ESTATE, "the classifier predicts %zu class labels: there is no click probability to rank items by", m->classes.size());
     MCU(m, cudaStreamSynchronize(m->stream));                            // h's stream reads the parameters
     const int L = m->d.n_layers, H = m->d.units[1];
     if (m->d.units[L - 1] != 1) return mlp_err(m, CTR_ESTATE, "recommendation ranks one output unit, the network has %d", m->d.units[L - 1]);

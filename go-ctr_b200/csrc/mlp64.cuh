@@ -4,7 +4,8 @@
 // forwardPass :259, AdamOptimizer64.updateParams :1075).
 //
 // One hidden layer or more, biases, relu / logistic / identity / tanh hidden activation, logistic output + binary_log_loss with the
-// probabilities clipped to (nextafter(0,1), nextafter(1,0)) (:180-195), L2 term alpha/(2n)·Σw² in the loss (:361) and
+// probabilities clipped to (nextafter(0,1), nextafter(1,0)) (:180-195) — or, for labels that are not all 0 or 1, a
+// softmax output + log_loss over the label classes (see "labels that are not all 0 or 1" below) — L2 term alpha/(2n)·Σw² in the loss (:361) and
 // alpha/n·w in the coefficient gradients (:327), Adam whose beta powers advance once per parameter ELEMENT
 // (:1082-1090 — the bias correction is gone within the first call) or SGD with momentum / Nesterov (:1024-1039),
 // weight decay of the whole packed vector before every minibatch (:342-346), minibatches of 200 visited through a per-epoch
@@ -211,6 +212,108 @@ k_mlp64_loss(const double* __restrict__ params, Mlp64Dims d, const double* __res
         const double loss = ll + (0.5 * alpha) * red[0] / (double)m;
         *loss_out = loss;
         if (epoch_acc) *epoch_acc += loss * (double)m;
+    }
+}
+
+// ---- labels that are not all 0 or 1 (BaseMultilayerPerceptron64.Fit :578-598) -----------------------------------
+// LabelBinarizer64(0, 1) (:1294-1351): the classes are the distinct label values in ascending order, the target of a
+// sample is the one-hot row of its class, and C >= 2 classes make a softmax output trained on log_loss (:504-511).
+// The targets are never materialised: each sample carries its class index (int32), found by a binary search.
+constexpr int kMlpMaxClasses = 1024;
+// what class discovery hands the host in one copy
+struct Mlp64Classes {
+    double value[kMlpMaxClasses];    // the first min(count, kMlpMaxClasses) classes, ascending
+    long count;                      // the number of distinct labels (written by cub::DeviceSelect::UniqueByKey)
+    int nan;                         // a NaN label was seen
+};
+
+// discovery pass 1: sort keys and positions.  −0 becomes +0, so ±0 fall into one run (the reference's map compares with
+// ==); a NaN label is flagged and the host refuses the fit.
+__global__ void __launch_bounds__(256)
+k_mlp64_label_keys(const float* __restrict__ Y, long n, float* __restrict__ key, long* __restrict__ pos, Mlp64Classes* __restrict__ res) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const float y = Y[i];
+        if (y != y) res->nan = 1;
+        key[i] = y == 0.0f ? 0.0f : y;
+        pos[i] = i;
+    }
+}
+// discovery pass 3, after a stable sort by key and UniqueByKey: first[c] is the first position of class c in sample
+// order, so the class keeps the sign of its first occurrence (the map of :1303-1309 keeps the first value it meets)
+__global__ void __launch_bounds__(256)
+k_mlp64_class_values(const float* __restrict__ Y, const long* __restrict__ first, Mlp64Classes* __restrict__ res) {
+    const long c_n = res->count < kMlpMaxClasses ? res->count : kMlpMaxClasses;
+    for (long c = blockIdx.x * (long)blockDim.x + threadIdx.x; c < c_n; c += (long)gridDim.x * blockDim.x) res->value[c] = (double)Y[first[c]];
+}
+// cls[i] = the index of label i in classes[0, C) (ascending, every label present; ±0 compare equal)
+__global__ void __launch_bounds__(256)
+k_mlp64_class_index(const float* __restrict__ Y, long n, const double* __restrict__ classes, int C, int* __restrict__ cls) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const double y = (double)Y[i];
+        int lo = 0, hi = C;
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (classes[mid] < y) lo = mid + 1; else hi = mid; }
+        cls[i] = lo;
+    }
+}
+
+// softmax of each row of the output layer's pre-activations, in place (:104-117): exp of every column, their sum in
+// column order, then one division per column.  No max subtraction: an overflow gives inf / inf = NaN, as in the reference.
+__global__ void __launch_bounds__(256)
+k_mlp64_softmax(double* __restrict__ h, int rows, int C) {
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+        double* z = h + (long)r * C;
+        double sum = 0.0;
+        for (int j = 0; j < C; j++) { const double e = exp(z[j]); z[j] = e; sum += e; }
+        for (int j = 0; j < C; j++) z[j] /= sum;
+    }
+}
+
+// k_mlp64_loss for targets given as class indices cls[idx[r]]: log_loss (:162-178) — −y·log(clip(h)) summed only where
+// y != 0, the clip of binary_log_loss, divided by the rows — or, with one output column (a single class v ∉ {0, 1}: an
+// all-ones target), binary_log_loss, which on y = 1 is the same term.  Delta h − y, L2 and the accumulator as k_mlp64_loss.
+__global__ void __launch_bounds__(256)
+k_mlp64_loss_cls(const double* __restrict__ params, Mlp64Dims d, const double* __restrict__ h, const int* __restrict__ cls, const long* __restrict__ idx,
+                 int m, double alpha, double* __restrict__ delta, double* __restrict__ loss_out, double* __restrict__ epoch_acc) {
+    __shared__ double red[256];
+    const int no = d.units[d.n_layers - 1];
+    const double hmin = 4.9406564584124654e-324, hmax = 0.99999999999999989;     // nextafter(0,1), nextafter(1,0)
+    double s = 0.0;
+    for (int i = threadIdx.x; i < m * no; i += 256) {
+        const int r = i / no, j = i % no;
+        const double y = cls[idx ? idx[r] : (long)r] == j ? 1.0 : 0.0;
+        double hv = h[i];
+        delta[i] = hv - y;
+        hv = hv < hmin ? hmin : (hv > hmax ? hmax : hv);
+        if (y != 0.0) s += -y * log(hv);
+    }
+    red[threadIdx.x] = s; __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
+    const double ll = red[0] / (double)m;
+    __syncthreads();
+    double sq = 0.0;
+    for (int l = 0; l + 1 < d.n_layers; l++) {
+        const double* W = params + d.off[l] + d.units[l + 1];
+        const long cnt = (long)d.units[l] * d.units[l + 1];
+        for (long i = threadIdx.x; i < cnt; i += 256) sq += W[i] * W[i];
+    }
+    red[threadIdx.x] = sq; __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
+    if (threadIdx.x == 0) {
+        const double loss = ll + (0.5 * alpha) * red[0] / (double)m;
+        *loss_out = loss;
+        if (epoch_acc) *epoch_acc += loss * (double)m;
+    }
+}
+
+// Predict with classes (:917-931): out[r] = float32(classes[MaxIdx64(h[r, 0:C))]) — the first strict maximum
+// (mathCompat.go:93-101), so a NaN in column 0 wins and a NaN elsewhere never does.  One column: classes[0].
+__global__ void __launch_bounds__(256)
+k_mlp64_predict_label(const double* __restrict__ h, int rows, int C, const double* __restrict__ classes, float* __restrict__ out) {
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+        const double* z = h + (long)r * C;
+        int mi = 0;
+        for (int j = 1; j < C; j++) if (z[j] > z[mi]) mi = j;
+        out[r] = (float)classes[mi];
     }
 }
 

@@ -31,7 +31,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
-           "ctr_mlp_recommend_topk"]
+           "ctr_mlp_recommend_topk", "ctr_mlp_get_classes", "ctr_mlp_set_classes"]
 
 
 class CtrError(RuntimeError):
@@ -494,7 +494,12 @@ class MLPClassifier:
     NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:81-90, basemlp64.go:227-256).
 
     `adaptive=True` is `learning_rate="adaptive"`; naming another schedule beside it raises.  solver "lbfgs",
-    early_stopping and batch_normalize are not built and raise instead of being ignored."""
+    early_stopping and batch_normalize are not built and raise instead of being ignored.
+
+    Labels all 0 or 1 train one logistic output and predict returns probabilities.  Other labels are classes (the
+    reference's LabelBinarizer64): after a cold fit, classes_ holds their distinct values ascending, the network has a
+    softmax output per class (one logistic output for a single class), and predict / predict_keys return the predicted
+    class label of each row.  A warm start keeps the classes and refuses labels with a different class set."""
 
     def __init__(self, n_features, hidden=(100,), activation="relu", alpha=1e-4, batch=200, max_iter=200, lr_init=1e-3,
                  adaptive=False, shuffle=True, seed=0, tol=1e-4, n_iter_no_change=10, warm_start=False, device=0,
@@ -614,13 +619,29 @@ class MLPClassifier:
                                                cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
 
+    @property
+    def classes_(self):
+        """The installed classes, float64 ascending; empty for labels all 0 or 1 (ctr_mlp_get_classes)."""
+        n = C.c_int32(0)
+        self._ck(self.L.ctr_mlp_get_classes(self.h, None, C.c_int32(0), C.byref(n)))
+        c = np.empty(n.value, np.float64)
+        self._ck(self.L.ctr_mlp_get_classes(self.h, c.ctypes.data_as(C.POINTER(C.c_double)), C.c_int32(n.value), C.byref(n)))
+        return c
+
     def get_params(self):
+        """The packed parameter vector; its length follows classes_.  Restore a model with set_params(p, classes_)."""
         n = C.c_int64(0)
         self._ck(self.L.ctr_mlp_get_params(self.h, None, C.c_int64(0), C.byref(n)))
         p = np.empty(n.value, np.float64)
         self._ck(self.L.ctr_mlp_get_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(n.value), C.byref(n)))
         return p
 
-    def set_params(self, p):
+    def set_params(self, p, classes=None):
+        """Installs the packed parameters and marks the model fitted.  classes (ascending, at most 1024; empty for a
+        binary model) first installs those classes and sizes the output layer for them (ctr_mlp_set_classes); None
+        keeps the current ones."""
         p = np.ascontiguousarray(p, np.float64)
+        if classes is not None:
+            c = np.ascontiguousarray(classes, np.float64).reshape(-1)
+            self._ck(self.L.ctr_mlp_set_classes(self.h, c.ctypes.data_as(C.POINTER(C.c_double)), C.c_int32(c.size)))
         self._ck(self.L.ctr_mlp_set_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(p.size)))

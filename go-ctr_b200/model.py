@@ -219,7 +219,8 @@ class YoutubeDnnImpl(_Impl):
 
 
 class SimpleMlpPredWrap:
-    """model/mlp/mlp.go:11-39: PredictAbstract over the fitted classifier — float32 X in, float32 [n, 1] out."""
+    """model/mlp/mlp.go:11-39: PredictAbstract over the fitted classifier — float32 X in, float32 [n, 1] out: click
+    probabilities, or the predicted labels when the classifier was fitted on labels other than 0 / 1 (pred.classes_)."""
 
     def __init__(self, pred, engine=None):
         self.pred = pred
@@ -238,7 +239,8 @@ class SimpleMlpPredWrap:
     def recommend(self, userId, k, now=None, exclude_history=True):
         """The k best items of the bound feature store's whole ITEM_EMB table for one user at `now` (default: the
         current time), scored by this MLP on the device (ctr_mlp_recommend_topk).  Returns (rows [n] int32, scores [n]
-        float32, logits [n] float64), best first, n <= k; serving.Recommend maps the rows to item ids."""
+        float32, logits [n] float64), best first, n <= k; serving.Recommend maps the rows to item ids.  A classifier
+        with classes has no click probability to rank by: CtrError with code ESTATE."""
         self._bound()
         ts = int(time.time()) if now is None else int(now)
         rows, scores, logits, cnt = self.pred.recommend_topk(self.engine, [int(userId)], [ts], k, exclude_history=exclude_history)
@@ -252,7 +254,8 @@ class SimpleMlpPredWrap:
 
 class SimpleMlpFitWrap:
     """model/mlp/mlp.go:41-65: Fitter over nn.MLPClassifier (main.go:42-52 builds it with NewMLPClassifier([]int{100},
-    "relu", "adam", 1e-4) — pass the same through **mlp_kw).  Model is created at Fit time from the sample width."""
+    "relu", "adam", 1e-4) — pass the same through **mlp_kw).  Model is created at Fit time from the sample width.
+    Labels other than 0 / 1 (ratings, say) make it a multi-class classifier whose predictor returns labels."""
 
     def __init__(self, **mlp_kw):
         self.mlp_kw = mlp_kw

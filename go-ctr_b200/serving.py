@@ -28,7 +28,8 @@ class ItemScore:                   # rcmd.go:184-187
 
 def BatchPredict(recSys, sampleKeys):
     """rcmd.go:277-337.  Returns float32 [n, 1] like the tensor the reference hands back.  An unknown
-    user/item in key 0 raises (CtrError code ENOTFOUND), in later keys it scores as a zero X row."""
+    user/item in key 0 raises (CtrError code ENOTFOUND), in later keys it scores as a zero X row.  Over an MLP fitted
+    on labels other than 0 / 1 the scores are predicted labels."""
     if len(sampleKeys) == 0:
         raise ValueError("no sample keys")
     u = np.fromiter((s.UserId for s in sampleKeys), np.int64, len(sampleKeys))
@@ -55,7 +56,8 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     A sharded deployment must pass `now` explicitly, the value broadcast with the request: the default reads each
     process's own clock, so ranks can window different histories and then all fail with CTR_EINVAL.
     recSys may also be the SimpleMlpPredWrap that SimpleMlpFitWrap.FitKeys returns, main.go's model: its MLP scores
-    every ITEM_EMB row of the feature store it is bound to (ctr_mlp_recommend_topk), under the same rules."""
+    every ITEM_EMB row of the feature store it is bound to (ctr_mlp_recommend_topk), under the same rules.  An MLP
+    fitted on labels other than 0 / 1 predicts labels, not click probabilities, and raises CtrError with code ESTATE."""
     ts = int(time.time()) if now is None else int(now)
     if isinstance(recSys, _m.SimpleMlpPredWrap):
         rows, scores, _ = recSys.recommend(userId, k, now=ts, exclude_history=exclude_history)

@@ -498,6 +498,10 @@ func NewEngineWith(kind Kind, uP, S, D, cF, batchSize, predBatchSize, tableOpt i
 // carry the names of BaseMultilayerPerceptron64's (basemlp64.go:25-50); a zero value means the reference default,
 // and pointer fields exist where zero is itself a meaningful setting.  Fit returns an error for what the engine
 // does not build (solver "lbfgs", EarlyStopping, BatchNormalize) instead of training something else.
+// Labels: when every Y is 0 or 1 the classifier has one logistic output and predicts click probabilities.  Any other
+// labels (ratings, say) are classes, as the reference's LabelBinarizer64 makes them: one softmax output per distinct
+// value (one logistic output for a single value), and the predictor returns the predicted label of each row.  A NaN
+// label or more than 1024 distinct labels is an error.
 type MlpFitWrap struct {
 	Hidden      []int   // HiddenLayerSizes, default {100}
 	Activation  int     // C.CTR_MLP_RELU (default) | CTR_MLP_LOGISTIC | CTR_MLP_IDENTITY | CTR_MLP_TANH
@@ -629,7 +633,8 @@ func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, e
 	return p, nil
 }
 
-// Predict follows SimpleMlpPredWrap.Predict (mlp.go:15-39), including nil on failure.
+// Predict follows SimpleMlpPredWrap.Predict (mlp.go:15-39), including nil on failure: probabilities, or the predicted
+// labels of a classifier fitted on labels other than 0 / 1.
 func (p *MlpPredWrap) Predict(X tensor.Tensor) tensor.Tensor {
 	n := X.Shape()[0]
 	y := make([]float32, n)
@@ -709,7 +714,9 @@ func (p *MlpPredWrap) Rank(e *Engine, userId int, itemIds []int) ([]rcmd.ItemSco
 // Recommend is the default recall of recommend/api.go's empty itemIdList (api.go:115-118) for the MLP: every ITEM_EMB
 // row of the feature store e scored for each user, windowed at ts[j], and the best k kept on the device (logit
 // descending, then row ascending).  outRows, scores and logits are [len(userIds)·k]; counts[j] results of user j are
-// valid.  Each score is what BatchPredict returns for (user, the row's item id, ts[j]).  An unknown user is an error.
+// valid.  Each score is what BatchPredict returns for (user, the row's item id, ts[j]).  An unknown user is an error,
+// and so is a classifier fitted on labels other than 0 / 1: it predicts labels, so it has no click probability to
+// rank items by (CTR_ESTATE, with nothing written).
 func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, excludeHistory bool) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
 	nu := len(userIds)
 	if nu == 0 || k < 1 || len(ts) != nu {

@@ -424,15 +424,29 @@ int  ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t*
 /* ---- model/mlp: the float64 MLP classifier of the reference's default path (BASELINE configs[0]; SURVEY.md §8a row
  * a11) — main.go:42-52 → model/mlp/mlp.go:45-65 (SimpleMlpFitWrap.Fit / SimpleMlpPredWrap.Predict: float32 samples →
  * float64 → nn.MLPClassifier) → nn/neural_network/basemlp64.go.  Float64 arithmetic on the device; packed parameter
- * vector in the reference's layout (basemlp64.go:459-463: per layer [intercepts | coefs row-major]). -------------- */
+ * vector in the reference's layout (basemlp64.go:459-463: per layer [intercepts | coefs row-major]).
+ * Labels, classes and outputs (BaseMultilayerPerceptron64.Fit, basemlp64.go:578-598), decided at every cold initialise
+ * from the labels the classifier sees (for ctr_mlp_fit_keys, the survivors'):
+ *   - every label == 0 or == 1 (−0 counts as 0): no classes; one logistic output on binary_log_loss, and predict
+ *     returns probabilities;
+ *   - otherwise the classes are the distinct labels, ascending, widened to float64 (LabelBinarizer64, :1294-1313); ±0
+ *     are one class, whose value keeps the sign of its first occurrence in sample order.  C >= 2 classes: C softmax
+ *     outputs (exp, sum in column order, divide; no max subtraction, so an overflow gives NaN) on log_loss (:162-178),
+ *     each sample's target the one-hot row of its class; C = 1 (every label one v not in {0, 1}): one logistic output
+ *     on an all-ones target.  Predict returns float32(classes[MaxIdx64(outputs)]): the first strict maximum, so a
+ *     NaN in output 0 wins and a NaN elsewhere never does (:917-931, mathCompat.go:93-101).  With C = 1, v.
+ *   - a warm start of a fitted model keeps the output layer and needs the same classes (0 of them for binary labels).
+ * The packed vector's last layer has max(1, C) outputs: np = Σ (1 + fi)·fo.  cfg.units[n_layers-1] is 1, the binary
+ * width, as NOutputs comes from the labels in the reference.  Refused with CTR_EINVAL, changing nothing (DESIGN.md §2):
+ * a NaN label, more than 1024 classes, and a warm start whose classes differ from the fitted ones. -------------- */
 enum { CTR_MLP_RELU = 0, CTR_MLP_LOGISTIC = 1, CTR_MLP_IDENTITY = 2, CTR_MLP_TANH = 3 };
 enum { CTR_MLP_SOLVER_ADAM = 0, CTR_MLP_SOLVER_SGD = 1 };                              /* Solver "adam" | "sgd" */
 enum { CTR_MLP_LR_CONSTANT = 0, CTR_MLP_LR_INVSCALING = 1, CTR_MLP_LR_ADAPTIVE = 2 };  /* LearningRate */
 typedef struct ctr_mlp ctr_mlp;
 typedef struct {
     int32_t n_layers;                 /* len(layerUnits): hidden layers + 2 (basemlp64.go:495-497) */
-    int32_t units[8];                 /* [nFeatures, HiddenLayerSizes..., 1] */
-    int32_t hidden_act;               /* Activation "relu" (:229) | "logistic" | "identity" | "tanh"; the output is logistic (:423-425) */
+    int32_t units[8];                 /* [nFeatures, HiddenLayerSizes..., 1]; the output width follows the labels (above) */
+    int32_t hidden_act;               /* Activation "relu" (:229) | "logistic" | "identity" | "tanh"; one output is logistic (:423-425), more are softmax */
     int32_t batch, max_iter, n_iter_no_change;   /* BatchSize 200, MaxIter 200, NIterNoChange 10 (:233,238,254) */
     int32_t shuffle, adaptive;        /* Shuffle true (:241); LearningRate == "adaptive" */
     int32_t warm_start;               /* WarmStart (:245): keep the current parameters instead of re-initialising */
@@ -462,13 +476,13 @@ void ctr_mlp_options_default(ctr_mlp_options* opts);                       /* ad
 int  ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out);
 void ctr_mlp_destroy(ctr_mlp* m);
 const char* ctr_mlp_last_error(const ctr_mlp* m);
-/* SimpleMlpFitWrap.Fit (mlp.go:45-65): X [n, xcols] float32, Y [n] float32 in {0,1} → fit (basemlp64.go:484-567 →
+/* SimpleMlpFitWrap.Fit (mlp.go:45-65): X [n, xcols] float32, Y [n] float32 labels (classes as above) → fit (basemlp64.go:484-567 →
  * fitStochastic :729-857, solver adam or sgd).  The sample count t of "invscaling" carries over warm-start fits
  * (and ctr_mlp_set_params) and restarts at 0 whenever the parameters are initialised.  *n_iter = epochs run (NIter); loss_curve (may be NULL) receives max_iter
  * per-epoch losses at most. */
 int  ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, int32_t* n_iter, double* loss_curve);
-/* SimpleMlpPredWrap.Predict (mlp.go:15-39): probabilities as float32 [n] (the 64-bit class returns them raw,
- * basemlp64.go:897-931). */
+/* SimpleMlpPredWrap.Predict (mlp.go:15-39): float32 [n] probabilities (the 64-bit class returns them raw,
+ * basemlp64.go:897-931), or with classes installed the predicted class labels. */
 int  ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float* out);
 /* The classifier fed by sample keys {UserId, ItemId, Timestamp, Label} from a feature store: no X on the host.  The
  * handle h is used only as the feature store — its id maps, USER_FEAT / ITEM_EMB / ITEM_FEAT tables, optional device
@@ -481,7 +495,8 @@ int  ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float
  *   stopping rules and the t carry.  Each minibatch's float64 rows are gathered on the device into a [batch, nin]
  *   buffer the classifier owns; resident cost is about (S + 7)·4 bytes per survivor instead of nin·8.  *rows_used
  *   (may be NULL) = survivors; none is CTR_ENOTFOUND with the parameters untouched.  n in [1, 2^31).
- * predict: recommend.BatchPredict / Rank (rcmd.go:248-337) with model/mlp: keys → probabilities scores [n], in
+ * predict: recommend.BatchPredict / Rank (rcmd.go:248-337) with model/mlp: keys → scores [n] (probabilities, or class
+ *   labels as ctr_mlp_predict returns them), in
  *   chunks of h's pred_batch, history windowed at each key's ts.  An unknown key scores as an all-zero X row, unless
  *   it is key 0, which fails the call with CTR_ENOTFOUND (rcmd.go:300-303).
  * Refusals change nothing: CTR_EINVAL for null or short arguments, a width mismatch, or m and h on different devices;
@@ -505,16 +520,23 @@ int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, co
  *     (float64, may be NULL) are [nu, k]; out_count[j] may be less than k, and positions at or past it hold row -1,
  *     score 0 and logit 0.
  *   Refusals write nothing: CTR_EINVAL for k outside [1, 1024], nu < 1, null inputs or outputs and ctr_mlp_predict_keys'
- *     argument refusals; CTR_ESTATE for a classifier not fitted or with more than one output, a missing id map or table,
+ *     argument refusals; CTR_ESTATE for a classifier not fitted or with classes (it predicts labels, not a click
+ *     probability), a missing id map or table,
  *     or world > 1; CTR_ENOTFOUND for any unknown user id, naming the first.
  *   Items are scored in chunks of h's pred_batch (whole tiles of 128) in the classifier's activation buffers,
  *     pred_batch · (units[1] + … + units[L-1]) · 8 bytes: a large catalogue wants a large pred_batch.  Only nu·k
  *     results cross PCIe.  Locking: h's mutex, then m's. */
 int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k,
                             int32_t exclude_history, int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count);
-/* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the length */
+/* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the current length (it follows the classes) */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
+/* the installed classes, ascending; *n = 0 for binary labels.  get with classes == NULL returns only *n.  To restore a
+ * model: ctr_mlp_set_classes, then ctr_mlp_set_params.  set_classes refuses (CTR_EINVAL, changing nothing) more than
+ * 1024 classes, NaN and classes that are not strictly ascending; it sizes the output layer for them (n = 0: binary),
+ * zeroing the parameters when the width changes, and the model counts as not fitted until ctr_mlp_set_params. */
+int  ctr_mlp_get_classes(ctr_mlp* m, double* classes, int32_t cap, int32_t* n);
+int  ctr_mlp_set_classes(ctr_mlp* m, const double* classes, int32_t n);
 
 /* Multi-GPU (world > 1): one handle per rank/process.  The id is ncclUniqueId bytes produced on
  * rank 0 by ctr_comm_unique_id and distributed by the host (torch.distributed / Go). */
