@@ -3101,7 +3101,7 @@ int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const fl
     return CTR_OK;
 }
 
-// ---- model/mlp: the float64 MLP classifier (row a11) ---------------------------------------------------------
+// ---- model/mlp: the float64 MLP classifier and regressor (row a11) -------------------------------------------
 struct ctr_mlp {
     ctr_mlp_config cfg{};
     ctr_mlp_options opts{};
@@ -3123,6 +3123,8 @@ struct ctr_mlp {
     std::vector<double> classes;
     DevBuf<double> class_dev;                                         // [kMlpMaxClasses]
     DevBuf<int> cls;                                                  // [n] the class index of each sample of the last fit
+    bool regressor = false;                                           // MLPRegressor: no labels, targets [n, units[L-1]]
+    int out_kind = CTR_MLP_OUT_LOGISTIC;                              // OutActivation; d.out_act mirrors it
     double adam_calls = 0;                                           // AdamOptimizer64.t
     double t = 0;                                                     // BaseMultilayerPerceptron64.t: samples since initialize (:412,814)
     bool fitted = false;
@@ -3162,20 +3164,26 @@ int mlp_upload_x(ctr_mlp* m, const float* X, int64_t n, int nin) {
     return rc;
 }
 // forwardPass (basemlp64.go:259-275) over m rows; layer 0 reads the [*, nin] matrix X through idx (may be null = identity).
-// More than one output column: the output layer keeps its pre-activations and a softmax follows (:504-511).
+// A softmax output keeps the output layer's pre-activations and normalises them after (:504-511).
 void mlp_forward(ctr_mlp* m, const double* X, const long* idx, int rows) {
     const int L = m->d.n_layers, nin = m->d.units[0], no = m->d.units[L - 1];
-    auto layer = no > 1 ? k_mlp64_layer<true> : k_mlp64_layer<false>;
+    const bool softmax = m->out_kind == CTR_MLP_OUT_SOFTMAX;
+    auto layer = softmax ? k_mlp64_layer<true> : k_mlp64_layer<false>;
     for (int l = 0; l + 1 < L; l++)
         layer<<<mlp_grid(m, (long)rows * m->d.units[l + 1]), 256, 0, m->stream>>>(m->params, m->d, l, X, nin, idx,
                                                                               l == 0 ? nullptr : m->act[l].get(), m->act[l + 1], rows);
-    if (no > 1) k_mlp64_softmax<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, no);
+    if (softmax) k_mlp64_softmax<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, no);
 }
-// the float32 [rows] answer of predict from the output layer: the probability, or with classes the class label (:917-931)
+// the float32 answer of predict from the output layer: without classes the output layer itself, [rows, units[L-1]] (the
+// probability of a binary classifier, a regressor's values), with classes the class label [rows] (:917-931)
 void mlp_output(ctr_mlp* m, int rows, float* out) {
     const int L = m->d.n_layers;
-    if (m->classes.empty()) k_f64_to_f32<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], out, rows);
+    if (m->classes.empty()) k_f64_to_f32<<<mlp_grid(m, (long)rows * m->d.units[L - 1]), 256, 0, m->stream>>>(m->act[L - 1], out, (long)rows * m->d.units[L - 1]);
     else k_mlp64_predict_label<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, m->d.units[L - 1], m->class_dev, out);
+}
+void mlp_set_out(ctr_mlp* m, int kind) {
+    m->out_kind = kind;
+    m->d.out_act = kind == CTR_MLP_OUT_LOGISTIC ? MLP_ACT_LOGISTIC : MLP_ACT_IDENTITY;
 }
 // installs the classes (empty: binary) and the output width they imply; parameters, gradients and moments are
 // reallocated, zero, when the width changes, and the model then counts as not fitted.  Nothing changes on a failure.
@@ -3195,6 +3203,7 @@ int mlp_set_head(ctr_mlp* m, const std::vector<double>& classes) {
         m->fitted = false;
     }
     m->classes = classes;
+    mlp_set_out(m, classes.size() > 1 ? CTR_MLP_OUT_SOFTMAX : CTR_MLP_OUT_LOGISTIC);
     return CTR_OK;
 }
 // BaseMultilayerPerceptron64.Fit's label handling (basemlp64.go:578-598) over the n labels Y of a fit, on the device:
@@ -3235,6 +3244,24 @@ int mlp_labels(ctr_mlp* m, const float* Y, long n, const int** cls) {
     *cls = m->cls;
     return CTR_OK;
 }
+// MLPRegressor.Fit's targets (basemlp64.go:495-511): Y [n·no] on the device, one pass that flags a target not 0 or 1
+// and a non-finite one; the host reads back the two flags.  A cold initialise decides the output from them; a warm start
+// of a fitted model keeps its output.  A NaN or ±inf target is refused and changes nothing (DESIGN.md §2).
+int mlp_targets(ctr_mlp* m, const float* Y, long n) {
+    DevBuf<int> fl;
+    MCU(m, fl.alloc(2));
+    MCU(m, cudaMemsetAsync(fl, 0, 2 * sizeof(int), m->stream));
+    k_mlp64_target_flags<<<mlp_grid(m, n), 256, 0, m->stream>>>(Y, n, fl);
+    int f[2] = {0, 0};
+    MCU(m, cudaMemcpyAsync(f, fl, sizeof f, cudaMemcpyDeviceToHost, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    MCU(m, cudaGetLastError());
+    if (f[1]) return mlp_err(m, CTR_EINVAL, "a target is NaN or infinite (DESIGN.md §2)");
+    if (m->cfg.warm_start && m->fitted) return CTR_OK;
+    const int no = m->d.units[m->d.n_layers - 1];
+    mlp_set_out(m, f[0] ? CTR_MLP_OUT_IDENTITY : no == 1 ? CTR_MLP_OUT_LOGISTIC : CTR_MLP_OUT_SOFTMAX);
+    return CTR_OK;
+}
 // the two [rows, nin] staging buffers and their events of the key-fed entry points (grow-only; events made once)
 int mlp_stage(ctr_mlp* m, long rows) {
     const size_t n = (size_t)rows * m->d.units[0];
@@ -3268,8 +3295,8 @@ int mlp_init_params(ctr_mlp* m) {
 // Layer 0's input of minibatch k (0-based within the epoch), whose samples are bi[0, rows): *X = a [rows, nin] matrix
 // read row by row, or left null to read X64 through bi (ctr_mlp_fit).
 using MlpInput = std::function<int(long k, const long* bi, int rows, const double** X)>;
-// fitStochastic (basemlp64.go:729-857) over n samples with the device labels Y [n] (binary) or class indices cls [n]
-// (mlp_labels; cls non-null), in minibatches of bs: a fresh optimizer,
+// fitStochastic (basemlp64.go:729-857) over n samples with the device targets Y [n, units[L-1]] (binary labels or a
+// regressor's targets) or class indices cls [n] (mlp_labels; cls non-null), in minibatches of bs: a fresh optimizer,
 // the per-epoch shuffle, the solvers, weight decay, the stopping rules and the t carry.  Only layer 0's input differs
 // between the callers (input may be empty).  m->idx holds n entries and the activations bs rows.
 int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const int* cls, const MlpInput& input, int32_t* n_iter, double* loss_curve) {
@@ -3303,7 +3330,9 @@ int mlp_epochs(ctr_mlp* m, long n, long bs, const float* Y, const int* cls, cons
                 k_mlp64_decay<<<mlp_grid(m, m->np), 256, 0, m->stream>>>(m->params, m->np, 1.0 - o.weight_decay);
             mlp_forward(m, X0, xi, rows);
             if (cls) k_mlp64_loss_cls<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], cls, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
-            else k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
+            else if (m->out_kind == CTR_MLP_OUT_LOGISTIC) k_mlp64_loss<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->del[L - 1], m->scal, m->scal + 1);
+            else k_mlp64_loss_dense<<<1, 256, 0, m->stream>>>(m->params, m->d, m->act[L - 1], Y, bi, rows, c.alpha, m->out_kind == CTR_MLP_OUT_IDENTITY,
+                                                              m->del[L - 1], m->scal, m->scal + 1);
             for (int l = L - 2; l >= 0; l--) {                           // backprop :382-402
                 k_mlp64_grads<<<mlp_grid(m, (long)(m->d.units[l] + 1) * m->d.units[l + 1]), 256, 0, m->stream>>>(
                     m->params, m->grads, m->d, l, X0, nin, xi, l == 0 ? nullptr : m->act[l].get(), m->del[l + 1], rows, c.alpha);
@@ -3367,13 +3396,17 @@ const char* ctr_mlp_last_error(const ctr_mlp* m) { return m ? m->err.c_str() : g
 
 int ctr_mlp_create(const ctr_mlp_config* cfg, ctr_mlp** out) { return ctr_mlp_create_ex(cfg, nullptr, out); }
 
-int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out) {
+namespace {
+// NewMLPClassifier / NewMLPRegressor: every argument is checked before the device is looked for
+int mlp_create(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, bool regressor, ctr_mlp** out) {
     if (!cfg || !out) return mlp_err(nullptr, CTR_EINVAL, "null argument");
     *out = nullptr;
     const ctr_mlp_config& c = *cfg;
     if (c.n_layers < 2 || c.n_layers > kMlpMaxLayers) return mlp_err(nullptr, CTR_EINVAL, "n_layers must be in [2, %d]", kMlpMaxLayers);
     for (int i = 0; i < c.n_layers; i++) if (c.units[i] < 1) return mlp_err(nullptr, CTR_EINVAL, "layer %d has %d units", i, c.units[i]);
-    if (c.units[c.n_layers - 1] != 1) return mlp_err(nullptr, CTR_EINVAL, "binary classifier: one output unit (basemlp64.go:423-425)");
+    const int no = c.units[c.n_layers - 1];
+    if (regressor && no > kMlpMaxClasses) return mlp_err(nullptr, CTR_EINVAL, "regressor: %d targets, at most %d", no, kMlpMaxClasses);
+    if (!regressor && no != 1) return mlp_err(nullptr, CTR_EINVAL, "binary classifier: one output unit (basemlp64.go:423-425)");
     if (c.hidden_act < CTR_MLP_RELU || c.hidden_act > CTR_MLP_TANH || c.max_iter < 1) return mlp_err(nullptr, CTR_EINVAL, "bad activation / max_iter");
     ctr_mlp_options o;
     ctr_mlp_options_default(&o);
@@ -3399,6 +3432,8 @@ int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ct
     ctr_mlp* m = new ctr_mlp();
     m->cfg = c; m->opts = o; m->dev = c.device; m->num_sms = prop.multiProcessorCount;
     m->d.n_layers = c.n_layers; m->d.hidden_act = c.hidden_act;
+    m->regressor = regressor;
+    mlp_set_out(m, regressor ? CTR_MLP_OUT_IDENTITY : CTR_MLP_OUT_LOGISTIC);
     long off = 0;
     for (int l = 0; l < c.n_layers; l++) { m->d.units[l] = c.units[l]; if (l + 1 < c.n_layers) { m->d.off[l] = off; off += (long)(1 + c.units[l]) * c.units[l + 1]; } }
     m->np = off;
@@ -3409,6 +3444,10 @@ int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ct
     *out = m;
     return CTR_OK;
 }
+}  // namespace
+
+int ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out) { return mlp_create(cfg, opts, false, out); }
+int ctr_mlp_regressor_create(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out) { return mlp_create(cfg, opts, true, out); }
 
 void ctr_mlp_destroy(ctr_mlp* m) {
     if (!m) return;
@@ -3459,6 +3498,7 @@ int ctr_mlp_set_classes(ctr_mlp* m, const double* classes, int32_t n) {
     }
     if (!m) return mlp_err(nullptr, CTR_EINVAL, "null classifier");
     std::lock_guard<std::mutex> lk(m->mu);
+    if (m->regressor) return mlp_err(m, CTR_ESTATE, "a regressor has no classes");
     MCU(m, cudaSetDevice(m->dev));
     RET(mlp_set_head(m, std::vector<double>(classes, classes + n)));
     m->fitted = false;
@@ -3472,12 +3512,14 @@ int ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t x
     if (xcols != nin) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, nin);
     MCU(m, cudaSetDevice(m->dev));
     const long bs = mlp_batch(m, n);
+    const size_t ny = (size_t)n * (m->regressor ? m->d.units[m->d.n_layers - 1] : 1);      // Y [n, no] for a regressor
     RET(mlp_upload_x(m, X, n, nin));
-    if (m->Y32.size() < (size_t)n) MCU(m, m->Y32.alloc((size_t)n));
+    if (m->Y32.size() < ny) MCU(m, m->Y32.alloc(ny));
     if (m->idx.size() < (size_t)n) MCU(m, m->idx.alloc((size_t)n));
-    MCU(m, cudaMemcpyAsync(m->Y32, Y, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
+    MCU(m, cudaMemcpyAsync(m->Y32, Y, sizeof(float) * ny, cudaMemcpyHostToDevice, m->stream));
     const int* cls = nullptr;
-    RET(mlp_labels(m, m->Y32, n, &cls));
+    if (m->regressor) RET(mlp_targets(m, m->Y32, (long)ny));
+    else RET(mlp_labels(m, m->Y32, n, &cls));
     RET(mlp_rows(m, bs));
     RET(mlp_init_params(m));
     return mlp_epochs(m, n, bs, m->Y32, cls, MlpInput(), n_iter, loss_curve);
@@ -3492,18 +3534,92 @@ int ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float*
     MCU(m, cudaSetDevice(m->dev));
     RET(mlp_upload_x(m, X, n, nin));
     const long chunk = 8192;
+    const int ow = m->classes.empty() ? m->d.units[m->d.n_layers - 1] : 1;   // floats per row of out
     RET(mlp_rows(m, std::min<long>(chunk, n)));
     DevBuf<float> d_out;
-    MCU(m, d_out.alloc((size_t)std::min<long>(chunk, n)));
+    MCU(m, d_out.alloc((size_t)std::min<long>(chunk, n) * ow));
     int rc = CTR_OK;
-    for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predict :917-931: raw probabilities for the f64 class, or class labels
+    for (long r0 = 0; r0 < n && rc == CTR_OK; r0 += chunk) {            // predict :917-931: raw outputs for the f64 class, or class labels
         const int rows = (int)std::min<long>(chunk, n - r0);
         mlp_forward(m, m->X64 + r0 * nin, nullptr, rows);
         mlp_output(m, rows, d_out);
-        if (cudaMemcpyAsync(out + r0, d_out, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, m->stream) != cudaSuccess ||
+        if (cudaMemcpyAsync(out + r0 * ow, d_out, sizeof(float) * (size_t)rows * ow, cudaMemcpyDeviceToHost, m->stream) != cudaSuccess ||
             cudaStreamSynchronize(m->stream) != cudaSuccess) rc = mlp_err(m, CTR_ECUDA, "predict: %s", cudaGetErrorString(cudaGetLastError()));
     }
     return rc;
+}
+
+namespace {
+// the float64 output layer [n, units[L-1]] of X, written to out (host or device memory), in chunks of 8192 rows
+int mlp_output64(ctr_mlp* m, const float* X, int64_t n, double* out) {
+    const int L = m->d.n_layers, nin = m->d.units[0], no = m->d.units[L - 1];
+    RET(mlp_upload_x(m, X, n, nin));
+    const long chunk = 8192;
+    RET(mlp_rows(m, std::min<long>(chunk, n)));
+    for (long r0 = 0; r0 < n; r0 += chunk) {
+        const int rows = (int)std::min<long>(chunk, n - r0);
+        mlp_forward(m, m->X64 + r0 * nin, nullptr, rows);
+        MCU(m, cudaMemcpyAsync(out + r0 * no, m->act[L - 1], sizeof(double) * (size_t)rows * no, cudaMemcpyDefault, m->stream));
+    }
+    MCU(m, cudaStreamSynchronize(m->stream));
+    return CTR_OK;
+}
+}  // namespace
+
+int ctr_mlp_predict_f64(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, double* out) {
+    if (!m || !X || !out || n < 1) return mlp_err(m, CTR_EINVAL, "bad predict arguments");
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
+    if (xcols != m->d.units[0]) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, m->d.units[0]);
+    MCU(m, cudaSetDevice(m->dev));
+    return mlp_output64(m, X, n, out);
+}
+
+int ctr_mlp_score(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* r2) {
+    if (!m || !X || !Y || !r2 || n < 1) return mlp_err(m, CTR_EINVAL, "bad score arguments");
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (!m->regressor) return mlp_err(m, CTR_ESTATE, "score is the regressor's R²; a classifier's accuracy score is not built");
+    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "score before fit");
+    if (xcols != m->d.units[0]) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, m->d.units[0]);
+    MCU(m, cudaSetDevice(m->dev));
+    const int no = m->d.units[m->d.n_layers - 1];
+    const size_t ny = (size_t)n * no;
+    DevBuf<double> pred, mean, r, res; DevBuf<float> y; DevBuf<double2> part;
+    MCU(m, pred.alloc(ny)); MCU(m, y.alloc(ny)); MCU(m, part.alloc((size_t)no * kR2Parts));
+    MCU(m, mean.alloc((size_t)no)); MCU(m, r.alloc(2 * (size_t)no)); MCU(m, res.alloc(2));
+    MCU(m, cudaMemcpyAsync(y, Y, sizeof(float) * ny, cudaMemcpyHostToDevice, m->stream));
+    RET(mlp_output64(m, X, n, pred));                                     // MLPRegressor.Score → Predict (:64-70)
+    k_mlp64_r2_part<<<dim3(kR2Parts, no), 256, 0, m->stream>>>(nullptr, y, (long)n, no, nullptr, part);
+    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, (long)n, no, mean, nullptr, nullptr);
+    k_mlp64_r2_part<<<dim3(kR2Parts, no), 256, 0, m->stream>>>(pred, y, (long)n, no, mean, part);
+    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, (long)n, no, mean, r, res);
+    double h[2] = {0, 0};
+    MCU(m, cudaMemcpyAsync(h, res, sizeof h, cudaMemcpyDeviceToHost, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    MCU(m, cudaGetLastError());
+    if (h[1] >= 0.0) return mlp_err(m, CTR_EINVAL, "target column %d is constant: R² divides by 0 (the reference panics)", (int)h[1]);
+    *r2 = h[0];
+    return CTR_OK;
+}
+
+int ctr_mlp_get_output(ctr_mlp* m, int32_t* kind) {
+    if (!m || !kind) return CTR_EINVAL;
+    std::lock_guard<std::mutex> lk(m->mu);
+    *kind = m->out_kind;
+    return CTR_OK;
+}
+int ctr_mlp_set_output(ctr_mlp* m, int32_t kind) {
+    if (!m) return mlp_err(nullptr, CTR_EINVAL, "null model");
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (!m->regressor) return mlp_err(m, CTR_ESTATE, "a classifier's output follows its classes (ctr_mlp_set_classes)");
+    const int no = m->d.units[m->d.n_layers - 1];
+    if (kind != CTR_MLP_OUT_IDENTITY && kind != CTR_MLP_OUT_LOGISTIC && kind != CTR_MLP_OUT_SOFTMAX)
+        return mlp_err(m, CTR_EINVAL, "output kind %d: identity (0), logistic (1) or softmax (2)", kind);
+    if ((kind == CTR_MLP_OUT_LOGISTIC) != (no == 1) && kind != CTR_MLP_OUT_IDENTITY)
+        return mlp_err(m, CTR_EINVAL, "%d targets: 0/1 targets make a logistic output for one target and a softmax for more (basemlp64.go:502-511)", no);
+    mlp_set_out(m, kind);
+    m->fitted = false;
+    return CTR_OK;
 }
 
 // ---- the MLP fed by sample keys from a feature store (ctr_mlp_fit_keys / ctr_mlp_predict_keys) -------------
@@ -3539,8 +3655,16 @@ int mlp_after_store(ctr_mlp* m, ctr_handle* h, int slot) {
     return CTR_OK;
 }
 
+// a sample key carries one label: a regressor fed by keys has one target
+int mlp_keys_width(ctr_mlp* m) {
+    const int no = m->d.units[m->d.n_layers - 1];
+    if (m->regressor && no != 1) return mlp_err(m, CTR_EINVAL, "a key-fed regressor has one target, this one %d", no);
+    return CTR_OK;
+}
+
 int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label, int64_t n,
                  int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    RET(mlp_keys_width(m));
     const int S = h->cfg.S;
     // ---- GetSample's resolution, as in ctr_train_keys: survivors resident in kt_*, input order kept
     RET(feed_init(h));
@@ -3569,7 +3693,8 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
     RET(mlp_stage(m, bs));
     RET(mlp_after_store(m, h, 0));                                     // labels and windows before the first loss
     const int* cls = nullptr;
-    RET(mlp_labels(m, h->kt_label, ns, &cls));                          // the survivors' labels
+    if (m->regressor) RET(mlp_targets(m, h->kt_label, ns));             // the survivors' labels are their targets
+    else RET(mlp_labels(m, h->kt_label, ns, &cls));                     // the survivors' labels
     RET(mlp_rows(m, bs));
     RET(mlp_init_params(m));
     const RowSrc r = idx_src(h, h->kt_user, h->kt_item, h->kt_hist_all, (int)ns);
@@ -3593,6 +3718,7 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
 
 int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
+    RET(mlp_keys_width(m));
     const int B = h->cfg.pred_batch, S = h->cfg.S, nin = m->d.units[0];
     RET(keys_stage_init(h));
     RET(mlp_rows(m, B));
@@ -3759,7 +3885,11 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
                 }));
         }
         const long n = (long)ng * k;
-        RET(launch(h, "mlp_rec_finish", [&] { rec::k_rec_finish<knn::Logit64Key><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
+        RET(launch(h, "mlp_rec_finish", [&] {
+            rec::k_rec_finish<knn::Logit64Key><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc);
+            // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
+            if (m->out_kind == CTR_MLP_OUT_IDENTITY) k_f64_to_f32<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ol, d_os, n);
+        }));
         CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
         if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));

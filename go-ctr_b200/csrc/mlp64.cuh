@@ -1,7 +1,8 @@
 // mlp64.cuh — model/mlp on the device (SURVEY.md §8a row a11, BASELINE configs[0]): the float64 scikit-learn-style
 // MLP classifier the reference's default path trains (main.go:42-52 → model/mlp/mlp.go:45-65 →
 // nn/neural_network/basemlp64.go `BaseMultilayerPerceptron64`: fit :484, fitStochastic :729, backprop :340,
-// forwardPass :259, AdamOptimizer64.updateParams :1075).
+// forwardPass :259, AdamOptimizer64.updateParams :1075), and the regressor over the same network (MLPRegressor,
+// multilayer_perceptron.go:9-71: identity output on square_loss, dense multi-column targets, R²; see "the regressor").
 //
 // One hidden layer or more, biases, relu / logistic / identity / tanh hidden activation, logistic output + binary_log_loss with the
 // probabilities clipped to (nextafter(0,1), nextafter(1,0)) (:180-195) — or, for labels that are not all 0 or 1, a
@@ -28,14 +29,18 @@ struct Mlp64Dims {
     int units[kMlpMaxLayers];        // [nFeatures, hidden..., nOutputs]
     long off[kMlpMaxLayers];         // offset of layer l's [intercepts | coefs] in the packed vector
     int hidden_act;
+    // OutActivation (:418-430): MLP_ACT_LOGISTIC, or MLP_ACT_IDENTITY for the regressor's identity output and for a
+    // softmax output, whose pre-activations k_mlp64_softmax then normalises
+    int out_act;
 };
 
 __device__ __forceinline__ double mlp64_logistic(double z) { return 1.0 / (1.0 + exp(-z)); }   // :82-88
-// the activation of layer l+1 on its pre-activation z; the output layer (last) is logistic (out_activation :423-425)
-__device__ __forceinline__ double mlp64_act(double z, int hidden_act, bool last) {
-    if (last || hidden_act == MLP_ACT_LOGISTIC) z = mlp64_logistic(z);
-    else if (hidden_act == MLP_ACT_RELU) z = z < 0.0 ? 0.0 : z;             // :96-104
-    else if (hidden_act == MLP_ACT_TANH) z = tanh(-z);                       // :88-94 — the argument is negated
+// the activation of layer l+1 on its pre-activation z: the hidden activation, or the output layer's (last)
+__device__ __forceinline__ double mlp64_act(double z, const Mlp64Dims& d, bool last) {
+    const int act = last ? d.out_act : d.hidden_act;
+    if (act == MLP_ACT_LOGISTIC) z = mlp64_logistic(z);
+    else if (act == MLP_ACT_RELU) z = z < 0.0 ? 0.0 : z;                     // :96-104
+    else if (act == MLP_ACT_TANH) z = tanh(-z);                              // :88-94 — the argument is negated
     return z;
 }
 
@@ -56,7 +61,7 @@ k_mlp64_layer(const double* __restrict__ params, Mlp64Dims d, int l, const doubl
         double z = 0.0;
         for (int k = 0; k < fi; k++) z += a[k] * W[(long)k * fo + j];
         z += b[j];                                                              // addIntercepts64 :205
-        if (!(kLogit && last)) z = mlp64_act(z, d.hidden_act, last);
+        if (!(kLogit && last)) z = mlp64_act(z, d, last);
         out[t] = z;
     }
 }
@@ -172,10 +177,30 @@ k_mlp64_rec_layer0(const double* __restrict__ params, Mlp64Dims d, const double*
                     const int j = j0 + jj;
                     if (j >= H) continue;
                     const double z = acc[r][jj] + b[j];
-                    out[(long)(b0 + i) * H + j] = last ? z : mlp64_act(z, d.hidden_act, false);
+                    out[(long)(b0 + i) * H + j] = last ? z : mlp64_act(z, d, false);
                 }
             }
         }
+    }
+}
+
+// the tail every loss kernel shares: ll is the data term; adds the L2 term (:361) over sumCoefSquares (:311-319) and
+// writes the minibatch loss and the epoch accumulator acc += loss * m (:805).  red is the block's [256] scratch.
+__device__ __forceinline__ void mlp64_loss_finish(const double* __restrict__ params, const Mlp64Dims& d, double* red, double ll, int m,
+                                                  double alpha, double* __restrict__ loss_out, double* __restrict__ epoch_acc) {
+    __syncthreads();
+    double sq = 0.0;
+    for (int l = 0; l + 1 < d.n_layers; l++) {
+        const double* W = params + d.off[l] + d.units[l + 1];
+        const long cnt = (long)d.units[l] * d.units[l + 1];
+        for (long i = threadIdx.x; i < cnt; i += 256) sq += W[i] * W[i];
+    }
+    red[threadIdx.x] = sq; __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
+    if (threadIdx.x == 0) {
+        const double loss = ll + (0.5 * alpha) * red[0] / (double)m;
+        *loss_out = loss;
+        if (epoch_acc) *epoch_acc += loss * (double)m;
     }
 }
 
@@ -198,21 +223,7 @@ k_mlp64_loss(const double* __restrict__ params, Mlp64Dims d, const double* __res
     }
     red[threadIdx.x] = s; __syncthreads();
     for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
-    const double ll = red[0] / (double)m;
-    __syncthreads();
-    double sq = 0.0;                                                              // sumCoefSquares :311-319
-    for (int l = 0; l + 1 < d.n_layers; l++) {
-        const double* W = params + d.off[l] + d.units[l + 1];
-        const long cnt = (long)d.units[l] * d.units[l + 1];
-        for (long i = threadIdx.x; i < cnt; i += 256) sq += W[i] * W[i];
-    }
-    red[threadIdx.x] = sq; __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
-    if (threadIdx.x == 0) {
-        const double loss = ll + (0.5 * alpha) * red[0] / (double)m;
-        *loss_out = loss;
-        if (epoch_acc) *epoch_acc += loss * (double)m;
-    }
+    mlp64_loss_finish(params, d, red, red[0] / (double)m, m, alpha, loss_out, epoch_acc);
 }
 
 // ---- labels that are not all 0 or 1 (BaseMultilayerPerceptron64.Fit :578-598) -----------------------------------
@@ -288,21 +299,7 @@ k_mlp64_loss_cls(const double* __restrict__ params, Mlp64Dims d, const double* _
     }
     red[threadIdx.x] = s; __syncthreads();
     for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
-    const double ll = red[0] / (double)m;
-    __syncthreads();
-    double sq = 0.0;
-    for (int l = 0; l + 1 < d.n_layers; l++) {
-        const double* W = params + d.off[l] + d.units[l + 1];
-        const long cnt = (long)d.units[l] * d.units[l + 1];
-        for (long i = threadIdx.x; i < cnt; i += 256) sq += W[i] * W[i];
-    }
-    red[threadIdx.x] = sq; __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
-    if (threadIdx.x == 0) {
-        const double loss = ll + (0.5 * alpha) * red[0] / (double)m;
-        *loss_out = loss;
-        if (epoch_acc) *epoch_acc += loss * (double)m;
-    }
+    mlp64_loss_finish(params, d, red, red[0] / (double)m, m, alpha, loss_out, epoch_acc);
 }
 
 // Predict with classes (:917-931): out[r] = float32(classes[MaxIdx64(h[r, 0:C))]) — the first strict maximum
@@ -314,6 +311,100 @@ k_mlp64_predict_label(const double* __restrict__ h, int rows, int C, const doubl
         int mi = 0;
         for (int j = 1; j < C; j++) if (z[j] > z[mi]) mi = j;
         out[r] = (float)classes[mi];
+    }
+}
+
+// ---- the regressor (MLPRegressor, multilayer_perceptron.go:9-71): dense [n, no] targets -----------------------------
+// The cold initialise decides the output from every target (:502-511): some target not 0 or 1 → identity output and
+// square_loss; else one column → logistic and binary_log_loss (k_mlp64_loss, the binary classifier); else softmax and
+// log_loss over the dense 0/1 rows, which need not be one-hot.
+
+// flags[0] = some target is neither 0 nor 1; flags[1] = some target is NaN or ±inf (refused, DESIGN.md §2)
+__global__ void __launch_bounds__(256)
+k_mlp64_target_flags(const float* __restrict__ Y, long n, int* __restrict__ flags) {
+    int not01 = 0, bad = 0;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const float y = Y[i];
+        not01 |= y != 0.0f && y != 1.0f;
+        bad |= !isfinite(y);
+    }
+    if (__syncthreads_or(not01) && threadIdx.x == 0) flags[0] = 1;
+    if (__syncthreads_or(bad) && threadIdx.x == 0) flags[1] = 1;
+}
+
+// k_mlp64_loss for dense targets Y[idx[r], 0:no): square_loss (:152-161) — Σ (h − y)², then / 2 / rows — or, with
+// square == false, log_loss (:162-178) — −y·log(clip(h)) summed where y != 0, / rows.  Delta h − y, L2 and the
+// accumulator as k_mlp64_loss.
+__global__ void __launch_bounds__(256)
+k_mlp64_loss_dense(const double* __restrict__ params, Mlp64Dims d, const double* __restrict__ h, const float* __restrict__ Y, const long* __restrict__ idx,
+                   int m, double alpha, bool square, double* __restrict__ delta, double* __restrict__ loss_out, double* __restrict__ epoch_acc) {
+    __shared__ double red[256];
+    const int no = d.units[d.n_layers - 1];
+    const double hmin = 4.9406564584124654e-324, hmax = 0.99999999999999989;     // nextafter(0,1), nextafter(1,0)
+    double s = 0.0;
+    for (int i = threadIdx.x; i < m * no; i += 256) {
+        const int r = i / no, j = i % no;
+        const double y = (double)Y[(idx ? idx[r] : (long)r) * no + j];
+        double hv = h[i];
+        const double e = hv - y;
+        delta[i] = e;
+        if (square) s += e * e;
+        else {
+            hv = hv < hmin ? hmin : (hv > hmax ? hmax : hv);
+            if (y != 0.0) s += -y * log(hv);
+        }
+    }
+    red[threadIdx.x] = s; __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
+    mlp64_loss_finish(params, d, red, square ? red[0] / 2.0 / (double)m : red[0] / (double)m, m, alpha, loss_out, epoch_acc);
+}
+
+// r2Score64 (basemlp64.go:1116-1141) over pred [n, no] and Y [n, no] in two passes, each a fixed partition of the rows
+// into kR2Parts contiguous ranges per column (block (p, c)), a fixed tree inside the block, and the parts folded in
+// order by one thread per column: the same bits on every run.
+constexpr int kR2Parts = 256;
+// mean == nullptr: part[c][p] = Σ y over part p of column c.  Else part[c][p] = {Σ (pred − y)², Σ (y − mean[c])²}.
+__global__ void __launch_bounds__(256)
+k_mlp64_r2_part(const double* __restrict__ pred, const float* __restrict__ Y, long n, int no, const double* __restrict__ mean, double2* __restrict__ part) {
+    __shared__ double2 red[256];
+    const int p = blockIdx.x, c = blockIdx.y;
+    const long per = (n + kR2Parts - 1) / kR2Parts, r0 = p * per, r1 = min(n, r0 + per);
+    double a = 0.0, b = 0.0;
+    for (long r = r0 + threadIdx.x; r < r1; r += 256) {
+        const double y = (double)Y[r * no + c];
+        if (!mean) { a += y; continue; }
+        const double t = pred[r * no + c] - y, u = y - mean[c];
+        a += t * t;
+        b += u * u;
+    }
+    red[threadIdx.x] = make_double2(a, b); __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) { red[threadIdx.x].x += red[threadIdx.x + o].x; red[threadIdx.x].y += red[threadIdx.x + o].y; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) part[(long)c * kR2Parts + p] = red[0];
+}
+// pass 1 (r2 == nullptr): mean[c] = Σ y / rows.  Pass 2: r2[c] = 1 − num/den and r2[no + c] = den; out[0] = the mean
+// of the columns' r2 in column order, out[1] = the first column whose den is 0 (the reference panics there), or −1.
+// One block.
+__global__ void __launch_bounds__(256)
+k_mlp64_r2_fold(const double2* __restrict__ part, long n, int no, double* __restrict__ mean, double* __restrict__ r2, double* __restrict__ out) {
+    for (int c = threadIdx.x; c < no; c += blockDim.x) {
+        double a = 0.0, b = 0.0;
+        for (int p = 0; p < kR2Parts; p++) { a += part[(long)c * kR2Parts + p].x; b += part[(long)c * kR2Parts + p].y; }
+        if (!r2) mean[c] = a / (double)n;
+        else { r2[c] = 1.0 - a / b; r2[no + c] = b; }
+    }
+    if (!r2) return;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double acc = 0.0, bad = -1.0;
+        for (int c = 0; c < no; c++) {
+            if (bad < 0.0 && r2[no + c] == 0.0) bad = (double)c;
+            acc += r2[c];
+        }
+        out[0] = acc / (double)no;
+        out[1] = bad;
     }
 }
 

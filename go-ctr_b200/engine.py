@@ -9,7 +9,7 @@ import numpy as np
 
 from . import build as _build
 
-__all__ = ["Engine", "Config", "MLPClassifier", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
+__all__ = ["Engine", "Config", "MLPClassifier", "MLPRegressor", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
            "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE"]
 
@@ -31,7 +31,8 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
-           "ctr_mlp_recommend_topk", "ctr_mlp_get_classes", "ctr_mlp_set_classes"]
+           "ctr_mlp_recommend_topk", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
+           "ctr_mlp_score", "ctr_mlp_get_output", "ctr_mlp_set_output"]
 
 
 class CtrError(RuntimeError):
@@ -489,17 +490,11 @@ MLP_SOLVER = {"adam": 0, "sgd": 1}
 MLP_LR = {"constant": 0, "invscaling": 1, "adaptive": 2}
 
 
-class MLPClassifier:
-    """nn.MLPClassifier on the device (float64): NewMLPClassifier(hidden, activation, solver, alpha) with
-    NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:81-90, basemlp64.go:227-256).
-
-    `adaptive=True` is `learning_rate="adaptive"`; naming another schedule beside it raises.  solver "lbfgs",
-    early_stopping and batch_normalize are not built and raise instead of being ignored.
-
-    Labels all 0 or 1 train one logistic output and predict returns probabilities.  Other labels are classes (the
-    reference's LabelBinarizer64): after a cold fit, classes_ holds their distinct values ascending, the network has a
-    softmax output per class (one logistic output for a single class), and predict / predict_keys return the predicted
-    class label of each row.  A warm start keeps the classes and refuses labels with a different class set."""
+class _Mlp64:
+    """What MLPClassifier and MLPRegressor share: BaseMultilayerPerceptron64 on the device (float64), its
+    constructor, fits and the key-fed calls."""
+    n_outputs = 1
+    _CREATE = "ctr_mlp_create_ex"
 
     def __init__(self, n_features, hidden=(100,), activation="relu", alpha=1e-4, batch=200, max_iter=200, lr_init=1e-3,
                  adaptive=False, shuffle=True, seed=0, tol=1e-4, n_iter_no_change=10, warm_start=False, device=0,
@@ -531,7 +526,7 @@ class MLPClassifier:
         self.opts = opts
         cfg = MlpConfig()
         self.L.ctr_mlp_config_default(C.byref(cfg), C.c_int32(n_features))
-        units = [n_features, *hidden, 1]
+        units = [n_features, *hidden, self.n_outputs]
         cfg.n_layers = len(units)
         for i, u in enumerate(units):
             cfg.units[i] = u
@@ -540,7 +535,7 @@ class MLPClassifier:
         cfg.warm_start = int(warm_start); cfg.device = device
         self.cfg = cfg
         self.h = C.c_void_p()
-        rc = self.L.ctr_mlp_create_ex(C.byref(cfg), C.byref(opts), C.byref(self.h))
+        rc = getattr(self.L, self._CREATE)(C.byref(cfg), C.byref(opts), C.byref(self.h))
         if rc != 0:
             raise CtrError(rc, self.L.ctr_mlp_last_error(None).decode())
         self.n_iter = 0; self.loss_curve = np.zeros(0); self.rows_used = 0
@@ -565,12 +560,6 @@ class MLPClassifier:
         self._ck(self.L.ctr_mlp_fit(self.h, Xp, Yp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), C.byref(it), curve.ctypes.data_as(C.POINTER(C.c_double))))
         self.n_iter = it.value; self.loss_curve = curve[:it.value]
         return self
-
-    def predict(self, X):
-        Xa, Xp = _f(X)
-        out = np.empty(Xa.shape[0], np.float32)
-        self._ck(self.L.ctr_mlp_predict(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), out.ctypes.data_as(_fp)))
-        return out
 
     @staticmethod
     def _keys(user_ids, item_ids, ts):
@@ -619,6 +608,33 @@ class MLPClassifier:
                                                cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
 
+    def get_params(self):
+        """The packed parameter vector (its length follows classes_ on a classifier)."""
+        n = C.c_int64(0)
+        self._ck(self.L.ctr_mlp_get_params(self.h, None, C.c_int64(0), C.byref(n)))
+        p = np.empty(n.value, np.float64)
+        self._ck(self.L.ctr_mlp_get_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(n.value), C.byref(n)))
+        return p
+
+
+class MLPClassifier(_Mlp64):
+    """nn.MLPClassifier on the device (float64): NewMLPClassifier(hidden, activation, solver, alpha) with
+    NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:81-90, basemlp64.go:227-256).
+
+    `adaptive=True` is `learning_rate="adaptive"`; naming another schedule beside it raises.  solver "lbfgs",
+    early_stopping and batch_normalize are not built and raise instead of being ignored.
+
+    Labels all 0 or 1 train one logistic output and predict returns probabilities.  Other labels are classes (the
+    reference's LabelBinarizer64): after a cold fit, classes_ holds their distinct values ascending, the network has a
+    softmax output per class (one logistic output for a single class), and predict / predict_keys return the predicted
+    class label of each row.  A warm start keeps the classes and refuses labels with a different class set."""
+
+    def predict(self, X):
+        Xa, Xp = _f(X)
+        out = np.empty(Xa.shape[0], np.float32)
+        self._ck(self.L.ctr_mlp_predict(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), out.ctypes.data_as(_fp)))
+        return out
+
     @property
     def classes_(self):
         """The installed classes, float64 ascending; empty for labels all 0 or 1 (ctr_mlp_get_classes)."""
@@ -628,14 +644,6 @@ class MLPClassifier:
         self._ck(self.L.ctr_mlp_get_classes(self.h, c.ctypes.data_as(C.POINTER(C.c_double)), C.c_int32(n.value), C.byref(n)))
         return c
 
-    def get_params(self):
-        """The packed parameter vector; its length follows classes_.  Restore a model with set_params(p, classes_)."""
-        n = C.c_int64(0)
-        self._ck(self.L.ctr_mlp_get_params(self.h, None, C.c_int64(0), C.byref(n)))
-        p = np.empty(n.value, np.float64)
-        self._ck(self.L.ctr_mlp_get_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(n.value), C.byref(n)))
-        return p
-
     def set_params(self, p, classes=None):
         """Installs the packed parameters and marks the model fitted.  classes (ascending, at most 1024; empty for a
         binary model) first installs those classes and sizes the output layer for them (ctr_mlp_set_classes); None
@@ -644,4 +652,75 @@ class MLPClassifier:
         if classes is not None:
             c = np.ascontiguousarray(classes, np.float64).reshape(-1)
             self._ck(self.L.ctr_mlp_set_classes(self.h, c.ctypes.data_as(C.POINTER(C.c_double)), C.c_int32(c.size)))
+        self._ck(self.L.ctr_mlp_set_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(p.size)))
+
+
+MLP_OUT = {"identity": 0, "logistic": 1, "softmax": 2}
+
+
+class MLPRegressor(_Mlp64):
+    """nn.MLPRegressor on the device (float64): NewMLPRegressor(hidden, activation, solver, alpha) with
+    NewBaseMultilayerPerceptron64's defaults (multilayer_perceptron.go:19-28), and the same constructor as
+    MLPClassifier plus n_outputs, the number of target columns (1 to 1024).
+
+    Targets are float32 [n, n_outputs] ([n] for one).  A cold fit decides the output from all of them: some target not
+    0 or 1 gives an identity output on square_loss; 0/1 targets give a logistic output (one column, the binary
+    classifier) or a softmax (more).  out_activation_ names it.  A NaN or infinite target raises CtrError (EINVAL) and
+    changes nothing.  predict returns [n, n_outputs]; score is R², the mean of the columns' (MLPRegressor.Score)."""
+    _CREATE = "ctr_mlp_regressor_create"
+
+    def __init__(self, n_features, *args, n_outputs=1, **kw):
+        if kw.get("early_stopping"):
+            raise ValueError("early_stopping is not built: the reference's validation split, best score and best-parameter copy "
+                             "(basemlp64.go:826-853) are a change of their own, on top of score")
+        self.n_outputs = int(n_outputs)
+        super().__init__(n_features, *args, **kw)
+
+    def _targets(self, X, Y):
+        Xa, Xp = _f(X); Ya, Yp = _f(Y)
+        if Ya.size != Xa.shape[0] * self.n_outputs:
+            raise ValueError("Y has %d values for %d rows of %d targets" % (Ya.size, Xa.shape[0], self.n_outputs))
+        return Xa, Xp, Ya, Yp
+
+    def fit(self, X, Y):
+        self._targets(X, Y)
+        return super().fit(X, Y)
+
+    def predict(self, X):
+        """MLPRegressor.Predict → float32 [n, n_outputs], float32 of predict_f64 bit for bit"""
+        Xa, Xp = _f(X)
+        out = np.empty((Xa.shape[0], self.n_outputs), np.float32)
+        self._ck(self.L.ctr_mlp_predict(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), out.ctypes.data_as(_fp)))
+        return out
+
+    def predict_f64(self, X):
+        """the float64 output layer [n, n_outputs] (ctr_mlp_predict_f64)"""
+        Xa, Xp = _f(X)
+        out = np.empty((Xa.shape[0], self.n_outputs), np.float64)
+        self._ck(self.L.ctr_mlp_predict_f64(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]),
+                                            out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
+
+    def score(self, X, Y):
+        """MLPRegressor.Score: R² per target column, averaged.  A constant column raises CtrError (EINVAL)."""
+        Xa, Xp, Ya, Yp = self._targets(X, Y)
+        r2 = C.c_double(0)
+        self._ck(self.L.ctr_mlp_score(self.h, Xp, Yp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), C.byref(r2)))
+        return r2.value
+
+    @property
+    def out_activation_(self):
+        """"identity", "logistic" or "softmax" (ctr_mlp_get_output)"""
+        k = C.c_int32(0)
+        self._ck(self.L.ctr_mlp_get_output(self.h, C.byref(k)))
+        return {v: n for n, v in MLP_OUT.items()}[k.value]
+
+    def set_params(self, p, out_activation=None):
+        """Installs the packed parameters and marks the model fitted.  out_activation ("identity", "logistic" or
+        "softmax") first sets the output kind (ctr_mlp_set_output); None keeps the current one."""
+        p = np.ascontiguousarray(p, np.float64)
+        if out_activation is not None:
+            if out_activation not in MLP_OUT:
+                raise ValueError("out_activation must be one of %s, got %r" % (sorted(MLP_OUT), out_activation))
+            self._ck(self.L.ctr_mlp_set_output(self.h, C.c_int32(MLP_OUT[out_activation])))
         self._ck(self.L.ctr_mlp_set_params(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), C.c_int64(p.size)))

@@ -531,8 +531,9 @@ type MlpPredWrap struct {
 	xcols int
 }
 
-// create maps the options onto a classifier of xcols inputs, or refuses what the engine does not build.
-func (f *MlpFitWrap) create(xcols int) (*C.ctr_mlp, error) {
+// create maps the options onto a classifier (or a one-target regressor) of xcols inputs, or refuses what the engine
+// does not build.
+func (f *MlpFitWrap) create(xcols int, regressor bool) (*C.ctr_mlp, error) {
 	var cfg C.ctr_mlp_config
 	C.ctr_mlp_config_default(&cfg, C.int32_t(xcols))
 	if len(f.Hidden) > 0 {
@@ -611,14 +612,22 @@ func (f *MlpFitWrap) create(xcols int) (*C.ctr_mlp, error) {
 	}
 	opts.weight_decay = C.double(f.WeightDecay)
 	var m *C.ctr_mlp
-	if rc := C.ctr_mlp_create_ex(&cfg, &opts, &m); rc != C.CTR_OK {
+	if regressor {
+		if rc := C.ctr_mlp_regressor_create(&cfg, &opts, &m); rc != C.CTR_OK {
+			return nil, fmt.Errorf("ctr_mlp_regressor_create: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(nil)))
+		}
+	} else if rc := C.ctr_mlp_create_ex(&cfg, &opts, &m); rc != C.CTR_OK {
 		return nil, fmt.Errorf("ctr_mlp_create_ex: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(nil)))
 	}
 	return m, nil
 }
 
 func (f *MlpFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, error) {
-	m, err := f.create(trainSample.XCols)
+	return f.fit(trainSample, false)
+}
+
+func (f *MlpFitWrap) fit(trainSample *rcmd.TrainSample, regressor bool) (rcmd.PredictAbstract, error) {
+	m, err := f.create(trainSample.XCols, regressor)
 	if err != nil {
 		return nil, err
 	}
@@ -644,17 +653,50 @@ func (p *MlpPredWrap) Predict(X tensor.Tensor) tensor.Tensor {
 	return tensor.NewDense(tensor.Float32, tensor.Shape{n, 1}, tensor.WithBacking(y))
 }
 
+// Score is MLPRegressor.Score (multilayer_perceptron.go:64-70) of a predictor MlpRegressorFitWrap made: R² of its
+// predictions on X against Y, one target per row.  A constant Y, or a classifier's predictor, is an error.
+func (p *MlpPredWrap) Score(X tensor.Tensor, Y []float32) (float64, error) {
+	n := X.Shape()[0]
+	if len(Y) != n {
+		return 0, fmt.Errorf("MlpPredWrap.Score: %d targets for %d rows", len(Y), n)
+	}
+	var r2 C.double
+	if rc := C.ctr_mlp_score(p.m, f32(X.Data().([]float32)), f32(Y), C.int64_t(n), C.int32_t(p.xcols), &r2); rc != C.CTR_OK {
+		return 0, fmt.Errorf("ctr_mlp_score: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+	}
+	return float64(r2), nil
+}
+
+// MlpRegressorFitWrap satisfies recommend.Fitter with nn.NewMLPRegressor (multilayer_perceptron.go:19-28) in place of
+// the classifier, with MlpFitWrap's options and refusals.  Each TrainSample.Y is the target: a rating, say.  Some
+// target not 0 or 1 gives an identity output trained on square_loss, and the predictor returns predicted values, which
+// Recommend then ranks; targets all 0 or 1 give the binary classifier exactly.  A NaN or infinite target is an error.
+type MlpRegressorFitWrap struct{ MlpFitWrap }
+
+func (f *MlpRegressorFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAbstract, error) {
+	return f.fit(trainSample, true)
+}
+
 // FitKeys is rcmd.Train (rcmd.go:197-246) with this fitter, with GetSample (rcmd.go:339-460) on the device: e is the
 // feature store (id maps, tables, optional ubcache), samples are its keys.  Samples whose user or item is unknown are
 // dropped; rowsUsed counts the rest.  The classifier has e's uP + S·D + D + cF inputs and trains bit for bit as Fit
 // would on the rows GetSample builds.  The options and refusals are Fit's.  The predictor serves keys through e.
 func (f *MlpFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
+	return f.fitKeys(e, samples, false)
+}
+
+// FitKeys is MlpFitWrap.FitKeys with the regressor: each sample's Label is its target.
+func (f *MlpRegressorFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
+	return f.fitKeys(e, samples, true)
+}
+
+func (f *MlpFitWrap) fitKeys(e *Engine, samples []rcmd.Sample, regressor bool) (*MlpPredWrap, int64, error) {
 	n := len(samples)
 	if n == 0 {
 		return nil, 0, fmt.Errorf("MlpFitWrap.FitKeys: no samples")
 	}
 	xcols := int(e.cfg.uP + e.cfg.S*e.cfg.D + e.cfg.D + e.cfg.cF)
-	m, err := f.create(xcols)
+	m, err := f.create(xcols, regressor)
 	if err != nil {
 		return nil, 0, err
 	}

@@ -438,10 +438,18 @@ int  ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t*
  *   - a warm start of a fitted model keeps the output layer and needs the same classes (0 of them for binary labels).
  * The packed vector's last layer has max(1, C) outputs: np = Σ (1 + fi)·fo.  cfg.units[n_layers-1] is 1, the binary
  * width, as NOutputs comes from the labels in the reference.  Refused with CTR_EINVAL, changing nothing (DESIGN.md §2):
- * a NaN label, more than 1024 classes, and a warm start whose classes differ from the fitted ones. -------------- */
+ * a NaN label, more than 1024 classes, and a warm start whose classes differ from the fitted ones.
+ * The regressor (nn.MLPRegressor, multilayer_perceptron.go:9-71; ctr_mlp_regressor_create) shares the network, the
+ * solvers and every fit rule, but has no labels: its targets are [n, units[n_layers-1]] float32, and the output kind is
+ * decided at every cold initialise from all of them (basemlp64.go:502-511): some target not 0 or 1 → identity output
+ * on square_loss (Σ (h − y)² / 2 / rows, :152-161); all 0 or 1 with one column → logistic on binary_log_loss, the
+ * binary classifier bit for bit; all 0 or 1 with more columns → softmax on log_loss over the dense 0/1 rows (not
+ * necessarily one-hot).  A warm start of a fitted regressor keeps its output kind.  A NaN or ±inf target is refused
+ * with CTR_EINVAL, changing nothing (DESIGN.md §2). -------------- */
 enum { CTR_MLP_RELU = 0, CTR_MLP_LOGISTIC = 1, CTR_MLP_IDENTITY = 2, CTR_MLP_TANH = 3 };
 enum { CTR_MLP_SOLVER_ADAM = 0, CTR_MLP_SOLVER_SGD = 1 };                              /* Solver "adam" | "sgd" */
 enum { CTR_MLP_LR_CONSTANT = 0, CTR_MLP_LR_INVSCALING = 1, CTR_MLP_LR_ADAPTIVE = 2 };  /* LearningRate */
+enum { CTR_MLP_OUT_IDENTITY = 0, CTR_MLP_OUT_LOGISTIC = 1, CTR_MLP_OUT_SOFTMAX = 2 };   /* OutActivation */
 typedef struct ctr_mlp ctr_mlp;
 typedef struct {
     int32_t n_layers;                 /* len(layerUnits): hidden layers + 2 (basemlp64.go:495-497) */
@@ -474,6 +482,9 @@ void ctr_mlp_options_default(ctr_mlp_options* opts);                       /* ad
 /* ctr_mlp_create(cfg, out) == ctr_mlp_create_ex(cfg, NULL, out): default options, lr_schedule adaptive iff cfg->adaptive.
  * cfg->adaptive together with a non-adaptive opts->lr_schedule is CTR_EINVAL. */
 int  ctr_mlp_create_ex(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out);
+/* nn.NewMLPRegressor: cfg->units[n_layers-1] is the target count, in [1, 1024]; opts (may be NULL) and every other
+ * argument are checked as by ctr_mlp_create_ex, before any device is looked for. */
+int  ctr_mlp_regressor_create(const ctr_mlp_config* cfg, const ctr_mlp_options* opts, ctr_mlp** out);
 void ctr_mlp_destroy(ctr_mlp* m);
 const char* ctr_mlp_last_error(const ctr_mlp* m);
 /* SimpleMlpFitWrap.Fit (mlp.go:45-65): X [n, xcols] float32, Y [n] float32 labels (classes as above) → fit (basemlp64.go:484-567 →
@@ -482,8 +493,23 @@ const char* ctr_mlp_last_error(const ctr_mlp* m);
  * per-epoch losses at most. */
 int  ctr_mlp_fit(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, int32_t* n_iter, double* loss_curve);
 /* SimpleMlpPredWrap.Predict (mlp.go:15-39): float32 [n] probabilities (the 64-bit class returns them raw,
- * basemlp64.go:897-931), or with classes installed the predicted class labels. */
+ * basemlp64.go:897-931), or with classes installed the predicted class labels.  For a regressor, Y and out are
+ * [n, units[n_layers-1]] row-major, and out is float32 of ctr_mlp_predict_f64's values, bit for bit. */
 int  ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float* out);
+/* The float64 output layer [n, units[n_layers-1]] of any fitted model: MLPRegressor.Predict (:53-62) for a regressor,
+ * predictProbas (basemlp64.go:897-915) for a classifier. */
+int  ctr_mlp_predict_f64(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, double* out);
+/* MLPRegressor.Score (:64-70 → r2Score64, basemlp64.go:1116-1141) on the device: per target column, mean = Σ y / n,
+ * r2 = 1 − Σ (pred − y)² / Σ (y − mean)²; *r2 = the mean over the columns.  The sums are fixed-order reductions: the
+ * same bits on every run.  CTR_EINVAL for a column whose Σ (y − mean)² is 0 (the reference panics), CTR_ESTATE for a
+ * classifier (its accuracy score is not built) or an unfitted regressor. */
+int  ctr_mlp_score(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* r2);
+/* The output kind (CTR_MLP_OUT_*).  A classifier's follows its classes.  To restore a regressor (the reference's JSON
+ * carries OutActivation): ctr_mlp_set_output, then ctr_mlp_set_params; set_output leaves the model unfitted until
+ * set_params.  set_output is CTR_ESTATE on a classifier, and CTR_EINVAL for a logistic output with more than one
+ * target or a softmax with one (0/1 targets never make them). */
+int  ctr_mlp_get_output(ctr_mlp* m, int32_t* kind);
+int  ctr_mlp_set_output(ctr_mlp* m, int32_t kind);
 /* The classifier fed by sample keys {UserId, ItemId, Timestamp, Label} from a feature store: no X on the host.  The
  * handle h is used only as the feature store — its id maps, USER_FEAT / ITEM_EMB / ITEM_FEAT tables, optional device
  * ubcache and uP, S, D, cF; its model kind and dense weights are not used.  m->units[0] must equal uP + S·D + D + cF.
@@ -496,9 +522,10 @@ int  ctr_mlp_predict(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, float
  *   buffer the classifier owns; resident cost is about (S + 7)·4 bytes per survivor instead of nin·8.  *rows_used
  *   (may be NULL) = survivors; none is CTR_ENOTFOUND with the parameters untouched.  n in [1, 2^31).
  * predict: recommend.BatchPredict / Rank (rcmd.go:248-337) with model/mlp: keys → scores [n] (probabilities, or class
- *   labels as ctr_mlp_predict returns them), in
+ *   labels as ctr_mlp_predict returns them, or a regressor's predicted values), in
  *   chunks of h's pred_batch, history windowed at each key's ts.  An unknown key scores as an all-zero X row, unless
  *   it is key 0, which fails the call with CTR_ENOTFOUND (rcmd.go:300-303).
+ * A regressor takes each key's label as its target (one target: units[n_layers-1] must be 1, else CTR_EINVAL).
  * Refusals change nothing: CTR_EINVAL for null or short arguments, a width mismatch, or m and h on different devices;
  * CTR_ESTATE for a missing id map, missing tables, h with world > 1 (sharded feature stores are not served), and
  * predict before any fit or ctr_mlp_set_params.  The message is readable through both ctr_mlp_last_error(m) and
@@ -518,10 +545,11 @@ int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, co
  *   Order: output-layer logit (before the logistic) descending, then row ascending; a NaN logit never qualifies.
  *     exclude_history skips the rows of the user's window.  out_rows / out_scores (float32 probabilities) / out_logits
  *     (float64, may be NULL) are [nu, k]; out_count[j] may be less than k, and positions at or past it hold row -1,
- *     score 0 and logit 0.
+ *     score 0 and logit 0.  A regressor with an identity output ranks by its predicted value, which is both the
+ *     logit and, as float32, the score; one with a logistic output (0/1 targets) is the binary classifier.
  *   Refusals write nothing: CTR_EINVAL for k outside [1, 1024], nu < 1, null inputs or outputs and ctr_mlp_predict_keys'
  *     argument refusals; CTR_ESTATE for a classifier not fitted or with classes (it predicts labels, not a click
- *     probability), a missing id map or table,
+ *     probability), a model with more than one output, a missing id map or table,
  *     or world > 1; CTR_ENOTFOUND for any unknown user id, naming the first.
  *   Items are scored in chunks of h's pred_batch (whole tiles of 128) in the classifier's activation buffers,
  *     pred_batch · (units[1] + … + units[L-1]) · 8 bytes: a large catalogue wants a large pred_batch.  Only nu·k
@@ -531,7 +559,7 @@ int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, 
 /* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the current length (it follows the classes) */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
-/* the installed classes, ascending; *n = 0 for binary labels.  get with classes == NULL returns only *n.  To restore a
+/* the installed classes, ascending; *n = 0 for binary labels and for a regressor, on which set_classes is CTR_ESTATE.  get with classes == NULL returns only *n.  To restore a
  * model: ctr_mlp_set_classes, then ctr_mlp_set_params.  set_classes refuses (CTR_EINVAL, changing nothing) more than
  * 1024 classes, NaN and classes that are not strictly ascending; it sizes the output layer for them (n = 0: binary),
  * zeroing the parameters when the width changes, and the model counts as not fitted until ctr_mlp_set_params. */
