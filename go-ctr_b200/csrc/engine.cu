@@ -145,8 +145,9 @@ struct ctr_handle {
     DevBuf<unsigned long long> kt_count;
     static constexpr int kCnt = 8;                       // pinned ring of survivor counts read back chunk by chunk
     PinnedBuf<unsigned long long> kt_count_host; Event kt_counted[kCnt];
-    // history windows of batch b+1 are cut on their own stream while batch b trains (two buffers)
-    Stream win_stream; DevBuf<int> kt_hist[2]; Event kt_win[2], kt_used[2];
+    // history windows of batch b+1 are cut on their own stream while batch b trains (two buffers); kt_queued marks the
+    // engine stream's work queued before a ctr_train_keys call, which the call's first windows wait for
+    Stream win_stream; DevBuf<int> kt_hist[2]; Event kt_win[2], kt_used[2], kt_queued;
     // ctr_mlp_fit_keys: the history window of every survivor [survivors, S], cut once per fit
     DevBuf<int> kt_hist_all;
     // dense-X residency
@@ -1211,7 +1212,9 @@ int ub_batch_set(ctr_handle* h, const int32_t* user_rows, const int64_t* offsets
     return CTR_OK;
 }
 
-// the rewrite: offsets, stored events and new events into the spare CSR, then the swap
+// the rewrite: offsets, stored events and new events into the spare CSR, then the swap.  It returns with the kernels
+// still queued; the readers order themselves after them: engine-stream kernels by stream order, ctr_train_keys' windows
+// by the window stream's wait on the engine stream at the start of that call.
 int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users) {
     long long U, n; ub_stored(h, &U, &n);
     const int64_t n_new = n + ub.grow;
@@ -1686,15 +1689,22 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
         h->kt_count_host = std::move(ring);
     }
     if (!h->win_stream) {               // the window stream, its two buffers and their events, moved in together
-        Stream ws; DevBuf<int> hist[2]; Event win[2], used[2];
+        Stream ws; DevBuf<int> hist[2]; Event win[2], used[2], queued;
         CU(h, ws.create());
         for (int i = 0; i < 2; i++) {
             RET(dalloc(h, hist[i], (size_t)h->Bmax * S, false));
             CU(h, win[i].create(cudaEventDisableTiming)); CU(h, used[i].create(cudaEventDisableTiming));
         }
+        CU(h, queued.create(cudaEventDisableTiming));
         for (int i = 0; i < 2; i++) { h->kt_hist[i] = std::move(hist[i]); h->kt_win[i] = std::move(win[i]); h->kt_used[i] = std::move(used[i]); }
+        h->kt_queued = std::move(queued);
         h->win_stream = std::move(ws);
     }
+    // The windows read the ubcache CSR, which an ubcache append / set rewrites on the engine stream without waiting for
+    // it: every window of this call comes after the work already queued there.  (keys_prepare also drains the engine
+    // stream from the host today; the windows' order does not rest on that.)
+    CU(h, cudaEventRecord(h->kt_queued, h->stream));
+    CU(h, cudaStreamWaitEvent(h->win_stream, h->kt_queued, 0));
     // one step of model.Train's loop over the resident samples [b*B, b*B + B) of which `have` exist so far.  The batch's
     // history windows (GetUserBehavior at the sample's timestamp) are cut on the window stream into one of two buffers,
     // so the window kernel of batch b+1 runs under the train step of batch b.

@@ -325,6 +325,11 @@ class Engine:
         self._ck(self.L.ctr_ubcache_window(self.h, up, t.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int32(u.size), out.ctypes.data_as(_ip)))
         return out
 
+    def ubcache_window_dev(self, d_user, d_max_ts, B, d_hist):
+        """ubcache_window on device pointers (ints, e.g. torch.Tensor.data_ptr()): d_user [B] int32, d_max_ts [B] int64
+        → d_hist [B, S] int32; asynchronous on the engine stream."""
+        self._ck(self.L.ctr_ubcache_window_dev(self.h, C.c_void_p(d_user), C.c_void_p(d_max_ts), C.c_int32(B), C.c_void_p(d_hist)))
+
     def ubcache_append(self, user_rows, ts, item_rows):
         """Appends events to the device ubcache (ctr_ubcache_append): equal timestamps keep the most recent arrival first."""
         u, up = _i(user_rows); t = np.ascontiguousarray(ts, np.int64); it, ip = _i(item_rows)
@@ -356,6 +361,11 @@ class Engine:
         out = np.empty(a.size, np.int32)
         self._ck(self.L.ctr_idmap_lookup(self.h, C.c_int(which), a.ctypes.data_as(_lp), C.c_int64(a.size), out.ctypes.data_as(_ip)))
         return out
+
+    def idmap_lookup_dev(self, which, d_ids, n, d_rows):
+        """idmap_lookup on device pointers (ints): d_ids [n] int64 → d_rows [n] int32, -1 for an unknown id;
+        asynchronous on the engine stream."""
+        self._ck(self.L.ctr_idmap_lookup_dev(self.h, C.c_int(which), C.c_void_p(d_ids), C.c_int64(n), C.c_void_p(d_rows)))
 
     def idmap_insert(self, which, ids):
         """Adds ids to a live map (ctr_idmap_insert): ids it lacks get the next rows in order of first occurrence, ids it
