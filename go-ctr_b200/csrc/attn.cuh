@@ -508,12 +508,34 @@ struct BwdOut {
     int    hot_rows, hot_reps;
     float* scatter_base;    // where row gradients are added (row idx * lde): the table itself, or the per-lookup
                             // gradient buffer of the sharded path
+    // CTR_TABLE_ADAM on a row-sharded table (PEER): row gradients go to the owner's gradient buffer (peer_adam[j],
+    // layout adam) instead of its rows, and every occurrence marks the row touched; hot_touch[row] = 1 marks a hot row
+    unsigned char* peer_adam[kMaxPeers];
+    ShardGrad adam;
+    float* hot_touch;
 };
 
 // destination of one row's (already -lr scaled) gradient: a hot-row replica accumulator or the table row
 __device__ __forceinline__ float* scatter_dst(const RowSrc& r, const Dims& d, const BwdOut& o, int idx, int rep) {
     if (idx < o.hot_rows) return o.hot_acc + ((long)rep * o.hot_rows + idx) * d.D;
     return o.scatter_base + (long)idx * r.lde;
+}
+// the same on a row-sharded table: the hot-row replica accumulators, else the owner's row over NVLink (SGD) or the
+// owner's gradient row (row Adam).  lead: the one lane of the row's group that marks the row touched — the first
+// marker of a row appends its local row to the owner's list
+__device__ __forceinline__ float* peer_scatter_dst(const RowSrc& r, const Dims& d, const BwdOut& o, int idx, int rep, bool lead) {
+    if (idx < o.hot_rows) {
+        if (o.hot_touch && lead) o.hot_touch[idx] = 1.0f;
+        return scatter_dst(r, d, o, idx, rep);
+    }
+    if (!o.peer_adam[0]) return shard_row(r, r.peer_emb, idx, r.lde);
+    unsigned char* base = o.peer_adam[idx & r.wmask];
+    const long lr = idx >> r.wshift;
+    if (lead && atomicExch_system(reinterpret_cast<unsigned*>(base + o.adam.flag_off) + lr, 1u) == 0u) {
+        const unsigned slot = atomicAdd_system(reinterpret_cast<unsigned*>(base), 1u);
+        reinterpret_cast<int*>(base + o.adam.list_off)[slot] = (int)lr;
+    }
+    return reinterpret_cast<float*>(base + o.adam.grad_off) + lr * r.lde;
 }
 
 // Backward coefficients of history row s (u) for the lanes of its group: du = c1*g + c2*v + c3*u and
@@ -654,7 +676,8 @@ k_attn_bwd_vec(RowSrc r, Dims d, const float* __restrict__ att,
 // Requires S <= 64.
 // PEER (row-sharded tables over NVLink, see k_attn_fwd_idx): rows are re-read from rows_cache (what the forward
 // fetched — the gradient is taken at the step-start table values, and nothing crosses NVLink twice), and each row
-// gradient leaves as red.global.add.v4.f32 straight into the OWNER's table over NVLink, pre-scaled by -lr/world.
+// gradient leaves as red.global.add.v4.f32 straight into the OWNER's table over NVLink, pre-scaled by -lr/world (row
+// Adam: into the owner's gradient shard, scaled by 1/world, marking the row touched — peer_scatter_dst).
 template <int LPR, int VPL, int MODEL, bool FUSED, bool PEER>
 __global__ void __launch_bounds__(kAttnThreads, kAttnMinBlocks)
 k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
@@ -725,7 +748,7 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
             if (s < d.S) {
                 const float e1 = c.c1 * sc, e2 = c.c2 * sc, e3 = c.c3 * sc;
                 float* dst = nullptr;
-                if (FUSED) { if (row >= 0) dst = ((PEER && row >= o.hot_rows) ? emb_ptr<true>(r, row) : scatter_dst(r, d, o, row, rep)) + lir * 4; }
+                if (FUSED) { if (row >= 0) dst = (PEER ? peer_scatter_dst(r, d, o, row, rep, lir == 0) : scatter_dst(r, d, o, row, rep)) + lir * 4; }
                 else if (o.dUb) dst = o.dUb + ((long)b * d.S + s) * d.D + lir * 4;
 #pragma unroll
                 for (int q = 0; q < VPL; q++) {
@@ -747,7 +770,7 @@ k_attn_bwd_idx(RowSrc r, Dims d, const float* __restrict__ att,
         sum_subgroups<LPR, VPL>(dvu);
         if (sub == 0) {
             float* dst = nullptr;
-            if (FUSED) { if (id.z >= 0) dst = ((PEER && id.z >= o.hot_rows) ? emb_ptr<true>(r, id.z) : scatter_dst(r, d, o, id.z, rep)) + lir * 4; }
+            if (FUSED) { if (id.z >= 0) dst = (PEER ? peer_scatter_dst(r, d, o, id.z, rep, lir == 0) : scatter_dst(r, d, o, id.z, rep)) + lir * 4; }
             else if (o.dIt) dst = o.dIt + (long)b * d.D + lir * 4;
 #pragma unroll
             for (int q = 0; q < VPL; q++) {
@@ -808,6 +831,17 @@ k_hot_writeback(float* __restrict__ shard, long lde, const float* __restrict__ h
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)hot_k * q4; i += (long)gridDim.x * blockDim.x) {
         const int row = (int)(i / q4), c = (int)(i % q4) * 4;
         if (row % world == rank) *reinterpret_cast<float4*>(shard + (long)(row / world) * lde + c) = *reinterpret_cast<const float4*>(hot_tab + (long)row * lde + c);
+    }
+}
+// the reverse for data that only the owner holds (the row-Adam moments): hot[row] = this rank's shard row for the rows
+// it owns, zero for the others — summed over the ranks (all-reduce), every rank then holds every hot row's values
+__global__ void __launch_bounds__(256)
+k_hot_own(float* __restrict__ hot, const float* __restrict__ shard, long lde, int hot_k, int D, int world, int rank) {
+    const int q4 = D / 4;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)hot_k * q4; i += (long)gridDim.x * blockDim.x) {
+        const int row = (int)(i / q4), c = (int)(i % q4) * 4;
+        *reinterpret_cast<float4*>(hot + (long)row * D + c) =
+            (shard && row % world == rank) ? *reinterpret_cast<const float4*>(shard + (long)(row / world) * lde + c) : zero4();
     }
 }
 // sharded search by row: out[i] = ITEM_EMB row rows[i] (valid), widened to float64, for the vector instantiation of
@@ -1061,6 +1095,57 @@ k_apply_table_adam(float* __restrict__ tab, float* __restrict__ grad, float* __r
             row_adam_elem(ww, mm, vv, grad[o], a);
             tab[o] = ww; mo[o] = mm; vo[o] = vv; grad[o] = 0.0f;
         }
+    }
+}
+// row-sharded table, owner side (after the barrier that follows every rank's backward): one row Adam update per row of
+// this rank's touched list with the gradient the ranks added into gbuf, then the gradient row, the flag and (last block
+// out) the count go back to zero.  One warp per row.
+__global__ void __launch_bounds__(256)
+k_shard_adam(unsigned char* __restrict__ gbuf, ShardGrad L, float* __restrict__ tab, float* __restrict__ mo, float* __restrict__ vo,
+             long lde, int D, RowAdam a) {
+    unsigned* cnt = reinterpret_cast<unsigned*>(gbuf);
+    const long n = *reinterpret_cast<volatile unsigned*>(cnt);
+    const int* list = reinterpret_cast<const int*>(gbuf + L.list_off);
+    unsigned* flag = reinterpret_cast<unsigned*>(gbuf + L.flag_off);
+    float* grad = reinterpret_cast<float*>(gbuf + L.grad_off);
+    const int lane = threadIdx.x & 31;
+    const long nw = ((long)gridDim.x * blockDim.x) >> 5;
+    for (long i = (blockIdx.x * (long)blockDim.x + threadIdx.x) >> 5; i < n; i += nw) {
+        const long lr = list[i];
+        for (int c = lane * 4; c < D; c += 128) {
+            const long o = lr * lde + c;
+            float4 w = *reinterpret_cast<float4*>(tab + o), m = *reinterpret_cast<float4*>(mo + o), v = *reinterpret_cast<float4*>(vo + o);
+            const float4 g = *reinterpret_cast<const float4*>(grad + o);
+            row_adam_elem(w.x, m.x, v.x, g.x, a); row_adam_elem(w.y, m.y, v.y, g.y, a);
+            row_adam_elem(w.z, m.z, v.z, g.z, a); row_adam_elem(w.w, m.w, v.w, g.w, a);
+            *reinterpret_cast<float4*>(tab + o) = w; *reinterpret_cast<float4*>(mo + o) = m; *reinterpret_cast<float4*>(vo + o) = v;
+            *reinterpret_cast<float4*>(grad + o) = zero4();
+        }
+        if (lane == 0) flag[lr] = 0u;
+    }
+    __syncthreads();                 // every block has read the count before the last one resets it
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(cnt + 1, 1u) == gridDim.x - 1) { cnt[0] = 0u; cnt[1] = 0u; }
+    }
+}
+// the replicated hot rows under row Adam: every rank applies the same update to its replica from the all-reduced
+// gradient sums (sum) and touch marks (touch, > 0 = some rank's batch holds the row), then zeroes both.  One warp per row.
+__global__ void __launch_bounds__(256)
+k_hot_adam(float* __restrict__ hot_tab, float* __restrict__ sum, float* __restrict__ touch, float* __restrict__ mo, float* __restrict__ vo,
+           int hot_k, int D, RowAdam a) {
+    const int lane = threadIdx.x & 31;
+    const long nw = ((long)gridDim.x * blockDim.x) >> 5;
+    for (long row = (blockIdx.x * (long)blockDim.x + threadIdx.x) >> 5; row < hot_k; row += nw) {
+        if (touch[row] == 0.0f) continue;
+        for (int c = lane; c < D; c += 32) {
+            const long o = row * D + c;
+            float ww = hot_tab[o], mm = mo[o], vv = vo[o];
+            row_adam_elem(ww, mm, vv, sum[o], a);
+            hot_tab[o] = ww; mo[o] = mm; vo[o] = vv; sum[o] = 0.0f;
+        }
+        __syncwarp();
+        if (lane == 0) touch[row] = 0.0f;
     }
 }
 

@@ -43,7 +43,7 @@ struct Comm {
     int wshift = 0;                                   // log2(world)
     float* peer_emb[kMaxPeers] = {};                  // rank j's ITEM_EMB shard ([j == rank] = the local table)
     float* peer_ifeat[kMaxPeers] = {};                // rank j's ITEM_FEAT shard when sharded
-    VmmBuf peer_map[kMaxPeers][3];                    // this process's mappings of rank j's {ITEM_EMB, ITEM_FEAT, arena} (vmm.cuh)
+    VmmBuf peer_map[kMaxPeers][4];                    // this process's mappings of rank j's {ITEM_EMB, ITEM_FEAT, arena, row-Adam gradients} (vmm.cuh)
     uint64_t published_gen = 0;                       // ctr_handle::tab_gen the mappings belong to (0 = none)
     VmmBuf arena_vmm; unsigned char* arena = nullptr; // shared arena of this rank
     int lsock = -1; unsigned long long job_hash = 0;  // descriptor socket of this rank (abstract UDS named after the NCCL id)
@@ -55,7 +55,13 @@ struct Comm {
     // replicated hot rows of a sharded ITEM_EMB: rows [0, hot_k) live on every rank (hot_tab), their -lr/world scaled
     // gradient sums (hot_sum) are all-reduced with the dense gradients — a Zipf-popular row is neither pulled over
     // NVLink by every sample nor hammered by every rank's red.add
+    // (hot_sum holds hot_k more floats after the row sums: the touch marks of CTR_TABLE_ADAM, all-reduced with them)
     int hot_k = 0; DevBuf<float> hot_tab, hot_sum, hot_acc; int hot_reps = 0;
+    // CTR_TABLE_ADAM on the sharded ITEM_EMB: this rank's shareable owner-side gradient buffer (layout ShardGrad,
+    // attn.cuh), every rank's mapping of it, and the hot rows' two moments (replicated like hot_tab)
+    VmmBuf adam_vmm; ShardGrad adam_lay{};
+    unsigned char* peer_adam[kMaxPeers] = {};
+    DevBuf<float> hot_m, hot_v;
 };
 
 // the fixed header a collective serving call all-gathers first (comm_agree): the call's shape, a hash of every input

@@ -68,11 +68,12 @@ __global__ void k_peer_barrier(BarArgs a) {
     __threadfence_system();
 }
 
-// what one rank publishes about its three shareable buffers (ITEM_EMB shard, ITEM_FEAT shard, arena): sizes via the
-// NCCL all-gather (which doubles as the rendezvous barrier), the allocations themselves as file descriptors over
-// Unix-domain sockets (vmm.cuh)
-struct PubRec { unsigned long long bytes[3]; int has[3]; int pad; };
-struct FdHdr { int rank, nfds; int which[3]; };
+// what one rank publishes about its shareable buffers (ITEM_EMB shard, ITEM_FEAT shard, arena, and under CTR_TABLE_ADAM
+// the owner-side gradient buffer): sizes via the NCCL all-gather (which doubles as the rendezvous barrier), the
+// allocations themselves as file descriptors over Unix-domain sockets (vmm.cuh)
+constexpr int kPub = 4;
+struct PubRec { unsigned long long bytes[kPub]; int has[kPub]; };
+struct FdHdr { int rank, nfds; int which[kPub]; };
 
 void comm_sock_name(const Comm& cm, int rank, char* out, size_t n) { snprintf(out, n, "ctrb200.%016llx.%d", (unsigned long long)cm.job_hash, rank); }
 
@@ -81,8 +82,8 @@ int comm_hot_setup(ctr_handle* h);
 int comm_close_peers(ctr_handle* h) {
     Comm& cm = h->comm;
     for (int j = 0; j < kMaxPeers; j++)
-        for (int k = 0; k < 3; k++) vmm_free(&cm.peer_map[j][k]);
-    for (int j = 0; j < kMaxPeers; j++) { cm.peer_emb[j] = nullptr; cm.peer_ifeat[j] = nullptr; cm.peer_arena[j] = nullptr; }
+        for (int k = 0; k < kPub; k++) vmm_free(&cm.peer_map[j][k]);
+    for (int j = 0; j < kMaxPeers; j++) { cm.peer_emb[j] = nullptr; cm.peer_ifeat[j] = nullptr; cm.peer_arena[j] = nullptr; cm.peer_adam[j] = nullptr; }
     cm.published_gen = 0;
     return CTR_OK;
 }
@@ -95,9 +96,24 @@ int comm_publish(ctr_handle* h) {
     std::string err;
     CU(h, cudaStreamSynchronize(h->stream));
     comm_close_peers(h);
-    const VmmBuf* mine[3] = {&h->tab_vmm[CTR_TABLE_ITEM_EMB], h->tab_sharded[CTR_TABLE_ITEM_FEAT] ? &h->tab_vmm[CTR_TABLE_ITEM_FEAT] : nullptr, &cm.arena_vmm};
+    // row Adam: the owner-side gradient buffer of this table generation, sized by the largest shard (one layout on every
+    // rank), zero; another table_opt leaves it unallocated
+    const bool adam = h->cfg.table_opt == CTR_TABLE_ADAM;
+    if (adam) {
+        const int64_t rows = (h->tab_rows[CTR_TABLE_ITEM_EMB] + W - 1) / W;
+        const ShardGrad lay = shard_grad_layout((long)std::max<int64_t>(rows, 1), h->tab_ld[CTR_TABLE_ITEM_EMB]);
+        if (!cm.adam_vmm.live || cm.adam_lay.bytes != lay.bytes) {
+            vmm_free(&cm.adam_vmm);
+            if (!vmm_alloc((size_t)lay.bytes, h->dev, &cm.adam_vmm, &err)) return set_err(h, CTR_ENOMEM, "row-Adam gradient shard (%ld bytes): %s", lay.bytes, err.c_str());
+        }
+        cm.adam_lay = lay;
+        CU(h, cudaMemsetAsync(cm.adam_vmm.ptr, 0, (size_t)lay.bytes, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+    } else vmm_free(&cm.adam_vmm);
+    const VmmBuf* mine[kPub] = {&h->tab_vmm[CTR_TABLE_ITEM_EMB], h->tab_sharded[CTR_TABLE_ITEM_FEAT] ? &h->tab_vmm[CTR_TABLE_ITEM_FEAT] : nullptr, &cm.arena_vmm,
+                                adam ? &cm.adam_vmm : nullptr};
     PubRec rec{};
-    for (int k = 0; k < 3; k++) if (mine[k] && mine[k]->live) { rec.bytes[k] = mine[k]->bytes; rec.has[k] = 1; }
+    for (int k = 0; k < kPub; k++) if (mine[k] && mine[k]->live) { rec.bytes[k] = mine[k]->bytes; rec.has[k] = 1; }
     if (!rec.has[0] || !rec.has[2]) return set_err(h, CTR_ESTATE, "row-sharded ITEM_EMB is not in shareable memory (upload the table after ctr_create with world > 1)");
     if (!cm.d_xchg) RET(dalloc(h, cm.d_xchg, 256 * (size_t)(kMaxPeers + 1), false));
     PubRec* d_send = (PubRec*)cm.d_xchg.get(); PubRec* d_recv = d_send + 1;
@@ -108,15 +124,16 @@ int comm_publish(ctr_handle* h) {
     CU(h, cudaStreamSynchronize(h->stream));
     for (int j = 0; j < W; j++)
         if (all[(size_t)j].has[1] != rec.has[1]) return set_err(h, CTR_ESTATE, "rank %d disagrees on the ITEM_FEAT placement", j);
+        else if (all[(size_t)j].has[3] != rec.has[3] || all[(size_t)j].bytes[3] != rec.bytes[3]) return set_err(h, CTR_ESTATE, "rank %d disagrees on the table optimiser or the ITEM_EMB rows", j);
     // my descriptors to every peer (connect + one small message each: lands in the peer's backlog / socket buffer) ...
     for (int j = 0; j < W; j++) {
         if (j == cm.rank) continue;
         char name[64]; comm_sock_name(cm, j, name, sizeof name);
         const int s = uds_connect(name, 30000);
         if (s < 0) return set_err(h, CTR_ECOMM, "cannot reach rank %d's descriptor socket", j);
-        FdHdr hd{}; hd.rank = cm.rank; int fds[3]; 
+        FdHdr hd{}; hd.rank = cm.rank; int fds[kPub];
         bool ok = true;
-        for (int k = 0; k < 3 && ok; k++) if (rec.has[k]) { ok = vmm_export_fd(*mine[k], &fds[hd.nfds], &err); hd.which[hd.nfds] = k; if (ok) hd.nfds++; }
+        for (int k = 0; k < kPub && ok; k++) if (rec.has[k]) { ok = vmm_export_fd(*mine[k], &fds[hd.nfds], &err); hd.which[hd.nfds] = k; if (ok) hd.nfds++; }
         ok = ok && uds_send_fds(s, &hd, sizeof hd, fds, hd.nfds);
         for (int i = 0; i < hd.nfds; i++) close(fds[i]);
         close(s);
@@ -126,22 +143,24 @@ int comm_publish(ctr_handle* h) {
     for (int n = 0; n < W - 1; n++) {
         const int s = accept(cm.lsock, nullptr, nullptr);
         if (s < 0) return set_err(h, CTR_ECOMM, "accept on the descriptor socket failed");
-        FdHdr hd{}; int fds[4]; int nf = 0;
-        const bool ok = uds_recv_fds(s, &hd, sizeof hd, fds, 4, &nf);
+        FdHdr hd{}; int fds[kPub]; int nf = 0;
+        const bool ok = uds_recv_fds(s, &hd, sizeof hd, fds, kPub, &nf);
         close(s);
         if (!ok || hd.rank < 0 || hd.rank >= W || hd.rank == cm.rank || nf != hd.nfds) { for (int i = 0; i < nf; i++) close(fds[i]); return set_err(h, CTR_ECOMM, "bad descriptor message"); }
         for (int i = 0; i < nf; i++) {
             const int k = hd.which[i];
-            if (k < 0 || k > 2 || !vmm_import(fds[i], (size_t)all[(size_t)hd.rank].bytes[k], h->dev, &cm.peer_map[hd.rank][k], &err)) {
+            if (k < 0 || k >= kPub || !vmm_import(fds[i], (size_t)all[(size_t)hd.rank].bytes[k], h->dev, &cm.peer_map[hd.rank][k], &err)) {
                 for (int i2 = i + 1; i2 < nf; i2++) close(fds[i2]);
                 return set_err(h, CTR_ECOMM, "mapping rank %d's buffer %d: %s — row-sharded tables need peer access between the GPUs of the box", hd.rank, k, err.c_str());
             }
         }
     }
     for (int j = 0; j < W; j++) {
-        if (j == cm.rank) { cm.peer_emb[j] = (float*)mine[0]->ptr; cm.peer_ifeat[j] = rec.has[1] ? (float*)mine[1]->ptr : nullptr; cm.peer_arena[j] = (unsigned char*)mine[2]->ptr; }
-        else { cm.peer_emb[j] = (float*)cm.peer_map[j][0].ptr; cm.peer_ifeat[j] = (float*)cm.peer_map[j][1].ptr; cm.peer_arena[j] = (unsigned char*)cm.peer_map[j][2].ptr; }
-        if (!cm.peer_emb[j] || !cm.peer_arena[j] || (rec.has[1] && !cm.peer_ifeat[j])) return set_err(h, CTR_ESTATE, "rank %d published no shard", j);
+        if (j == cm.rank) { cm.peer_emb[j] = (float*)mine[0]->ptr; cm.peer_ifeat[j] = rec.has[1] ? (float*)mine[1]->ptr : nullptr; cm.peer_arena[j] = (unsigned char*)mine[2]->ptr;
+                            cm.peer_adam[j] = rec.has[3] ? (unsigned char*)mine[3]->ptr : nullptr; }
+        else { cm.peer_emb[j] = (float*)cm.peer_map[j][0].ptr; cm.peer_ifeat[j] = (float*)cm.peer_map[j][1].ptr; cm.peer_arena[j] = (unsigned char*)cm.peer_map[j][2].ptr;
+               cm.peer_adam[j] = (unsigned char*)cm.peer_map[j][3].ptr; }
+        if (!cm.peer_emb[j] || !cm.peer_arena[j] || (rec.has[1] && !cm.peer_ifeat[j]) || (rec.has[3] && !cm.peer_adam[j])) return set_err(h, CTR_ESTATE, "rank %d published no shard", j);
     }
     cm.published_gen = h->tab_gen;
     return comm_hot_setup(h);
@@ -155,16 +174,30 @@ int comm_hot_setup(ctr_handle* h) {
     if (want == 0) want = 32768;
     if (want < 0) want = 0;
     want = (int)std::min<int64_t>(want, h->tab_rows[CTR_TABLE_ITEM_EMB]);
-    cm.hot_tab.reset(); cm.hot_sum.reset(); cm.hot_acc.reset();
+    cm.hot_tab.reset(); cm.hot_sum.reset(); cm.hot_acc.reset(); cm.hot_m.reset(); cm.hot_v.reset();
     cm.hot_k = want; cm.hot_reps = 0;
     if (want == 0) return CTR_OK;
     if (h->tab_ld[CTR_TABLE_ITEM_EMB] != D) return set_err(h, CTR_EINVAL, "replicated hot rows need D %% 4 == 0");
-    RET(dalloc(h, cm.hot_tab, (size_t)want * D, false)); RET(dalloc(h, cm.hot_sum, (size_t)want * D));
+    RET(dalloc(h, cm.hot_tab, (size_t)want * D, false)); RET(dalloc(h, cm.hot_sum, (size_t)want * (D + 1)));     // + the row-Adam touch marks
     cm.hot_reps = (int)std::min<size_t>(16, std::max<size_t>(1, ((size_t)64 << 20) / ((size_t)want * D * sizeof(float))));
     RET(dalloc(h, cm.hot_acc, (size_t)cm.hot_reps * want * D));
     RowSrc r{}; r.lde = D; r.wmask = cm.world - 1; r.wshift = cm.wshift; r.world = cm.world;
     for (int j = 0; j < cm.world; j++) r.peer_emb[j] = cm.peer_emb[j];
     RET(launch(h, "hot_rows_pull", [&] { k_hot_pull<<<h->num_sms * 4, 256, 0, h->stream>>>(r, cm.hot_tab, want, D); }));
+    if (h->cfg.table_opt == CTR_TABLE_ADAM) {
+        // the hot rows' moments from their owners' moment shards (zero where an owner has none yet): each rank fills
+        // the rows it owns, the all-reduce hands every rank all of them
+        RET(dalloc(h, cm.hot_m, (size_t)want * D, false)); RET(dalloc(h, cm.hot_v, (size_t)want * D, false));
+        const long lde = h->tab_ld[CTR_TABLE_ITEM_EMB];
+        RET(launch(h, "hot_moments_pull", [&] {
+            k_hot_own<<<h->num_sms * 4, 256, 0, h->stream>>>(cm.hot_m, h->emb_m.get(), lde, want, D, cm.world, cm.rank);
+            k_hot_own<<<h->num_sms * 4, 256, 0, h->stream>>>(cm.hot_v, h->emb_v.get(), lde, want, D, cm.world, cm.rank);
+        }));
+        NC(h, g_nccl.GroupStart());
+        NC(h, g_nccl.AllReduce(cm.hot_m, cm.hot_m, (size_t)want * D, kNcclFloat32, kNcclSum, cm.nccl, h->stream));
+        NC(h, g_nccl.AllReduce(cm.hot_v, cm.hot_v, (size_t)want * D, kNcclFloat32, kNcclSum, cm.nccl, h->stream));
+        NC(h, g_nccl.GroupEnd());
+    }
     CU(h, cudaStreamSynchronize(h->stream));
     return CTR_OK;
 }
@@ -172,8 +205,14 @@ int comm_hot_setup(ctr_handle* h) {
 int comm_hot_writeback(ctr_handle* h) {
     Comm& cm = h->comm;
     if (cm.hot_k <= 0 || !cm.hot_tab || cm.published_gen != h->tab_gen) return CTR_OK;
+    if (cm.hot_m) RET(ensure_moments(h));      // row Adam: the owner's moment shards receive the hot rows' moments too
+    const long lde = h->tab_ld[CTR_TABLE_ITEM_EMB];
     return launch(h, "hot_rows_writeback", [&] {
-        k_hot_writeback<<<h->num_sms * 4, 256, 0, h->stream>>>(h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], cm.hot_tab, cm.hot_k, h->cfg.D, cm.world, cm.rank);
+        k_hot_writeback<<<h->num_sms * 4, 256, 0, h->stream>>>(h->tab[CTR_TABLE_ITEM_EMB], lde, cm.hot_tab, cm.hot_k, h->cfg.D, cm.world, cm.rank);
+        if (cm.hot_m) {
+            k_hot_writeback<<<h->num_sms * 4, 256, 0, h->stream>>>(h->emb_m, lde, cm.hot_m, cm.hot_k, h->cfg.D, cm.world, cm.rank);
+            k_hot_writeback<<<h->num_sms * 4, 256, 0, h->stream>>>(h->emb_v, lde, cm.hot_v, cm.hot_k, h->cfg.D, cm.world, cm.rank);
+        }
     });
 }
 
@@ -379,6 +418,7 @@ static int comm_init(ctr_handle* h, const void* id, int32_t id_bytes) {
 static void comm_destroy(ctr_handle* h) {
     Comm& cm = h->comm;
     comm_close_peers(h);
+    vmm_free(&cm.adam_vmm);
     vmm_free(&cm.arena_vmm);
     cm.arena = nullptr;
     if (cm.lsock >= 0) { close(cm.lsock); cm.lsock = -1; }

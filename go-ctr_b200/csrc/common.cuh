@@ -121,6 +121,19 @@ struct RowSrc {
     int hot_k; const float* hot_tab;
 };
 
+// CTR_TABLE_ADAM on a row-sharded ITEM_EMB: every owner's shareable gradient buffer, the same layout on every rank
+// (rows = the largest shard's local rows): bytes [0, 4) the touched-row count, [4, 8) the update kernel's block ticket,
+// then a touched flag per local row (u32), the list of touched local rows (i32) and the fp32 gradient shard [rows, lde];
+// all of it zero between steps
+struct ShardGrad { long flag_off, list_off, grad_off, bytes; };
+inline ShardGrad shard_grad_layout(long rows, long lde) {
+    auto up = [](long b) { return (b + 255) & ~255L; };
+    ShardGrad s;
+    s.flag_off = 256; s.list_off = s.flag_off + up(rows * 4); s.grad_off = s.list_off + up(rows * 4);
+    s.bytes = s.grad_off + rows * lde * (long)sizeof(float);
+    return s;
+}
+
 struct Dims { int uP, S, D, cF, in; };
 
 __device__ __forceinline__ bool row_ok(int idx, int n) { return (unsigned)idx < (unsigned)n; }

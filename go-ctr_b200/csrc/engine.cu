@@ -651,6 +651,13 @@ int ensure_moments(ctr_handle* h) {
     h->emb_m = std::move(m); h->emb_v = std::move(v);
     return CTR_OK;
 }
+// the row-Adam constants of this step (the dense solver's step counter t = step + 1, gradient divided by adam_batch)
+RowAdam row_adam_of(const ctr_handle* h, int adam_batch) {
+    const ctr_config& c = h->cfg;
+    const int t = (int)h->step + 1;
+    return RowAdam{c.table_lr, c.beta1, c.beta2, c.eps, (float)(1.0 - std::pow((double)c.beta1, (double)t)), (float)(1.0 - std::pow((double)c.beta2, (double)t)),
+                   adam_batch > 1 ? 1.0f / (float)adam_batch : 1.0f};
+}
 
 int deterministic_table_update(ctr_handle* h, const RowSrc& r, int B, int adam_batch) {
     const int S = h->cfg.S, D = h->cfg.D;
@@ -769,7 +776,7 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
         const bool fused_only = o.comm || o.table_grad;        // multi-GPU steps always scatter with red.add
         const bool sorted_rows = c.table_opt == CTR_TABLE_SGD_DETERMINISTIC || c.table_opt == CTR_TABLE_ADAM;   // per-unique-row update from sorted keys
         const bool adam_rows = learn_rows && c.table_opt == CTR_TABLE_ADAM;
-        if (adam_rows && o.peer) return set_err(h, CTR_ESTATE, "CTR_TABLE_ADAM is not available with row-sharded tables (use CTR_TABLE_SGD, or a replicated table)");
+        const bool shard_adam = adam_rows && o.peer;           // owner-side gradient shards + touched lists (comm_impl.cuh)
         const bool buffers = o.want_rows || (learn_rows && sorted_rows && !fused_only);
         if (buffers) RET(ensure_rowgrad_buffers(h, B));
         BwdOut bo{}; bo.datt = h->G[3]; bo.dUb = buffers ? h->dUb.get() : nullptr; bo.dIt = buffers ? h->dIt.get() : nullptr;
@@ -782,13 +789,29 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
         if (hot) { RET(ensure_hot(h)); bo.hot_acc = h->hot_acc; bo.hot_rows = h->hot_rows; bo.hot_reps = h->hot_reps; }
         const bool peer_hot = o.peer && bo.sgd && h->comm.hot_k > 0;
         if (peer_hot) { bo.hot_acc = h->comm.hot_acc; bo.hot_rows = h->comm.hot_k; bo.hot_reps = h->comm.hot_reps; }
-        // sharded tables: nobody's red.add may land in a row before every rank's forward has read it
-        if (o.peer && bo.sgd) RET(comm_barrier(h));
+        if (shard_adam) {
+            for (int j = 0; j < h->comm.world; j++) bo.peer_adam[j] = h->comm.peer_adam[j];
+            bo.adam = h->comm.adam_lay;
+            if (peer_hot) bo.hot_touch = h->comm.hot_sum.get() + (size_t)h->comm.hot_k * c.D;
+        }
+        // sharded tables: nobody's red.add may land in a row before every rank's forward has read it (row Adam adds
+        // into the gradient shards, which nobody reads before the owner's update)
+        if (o.peer && bo.sgd && !shard_adam) RET(comm_barrier(h));
         RET(attn_backward(h, r, bo, B));
         if (peer_hot)      // replica accumulators of the replicated hot rows → this rank's gradient sum (all-reduced below)
             RET(launch(h, "hot_rows_fold", [&] {
                 k_hot_apply<<<h->num_sms * 4, 256, 0, h->stream>>>(h->comm.hot_sum, c.D, h->comm.hot_acc, h->comm.hot_k, h->comm.hot_reps, c.D, 1.0f);
             }));
+        if (shard_adam) {  // every rank's red.adds into this rank's gradient shard have landed (and every forward has read
+                           // the rows): the owner updates the rows its list holds
+            RET(comm_barrier(h));
+            RET(ensure_moments(h));
+            const RowAdam ra = row_adam_of(h, o.adam_batch > 0 ? o.adam_batch : B);
+            RET(launch(h, "shard_row_adam", [&] {
+                k_shard_adam<<<h->num_sms * 8, 256, 0, h->stream>>>(h->comm.peer_adam[h->comm.rank], h->comm.adam_lay, h->tab[CTR_TABLE_ITEM_EMB],
+                                                                   h->emb_m, h->emb_v, h->tab_ld[CTR_TABLE_ITEM_EMB], c.D, ra);
+            }));
+        }
         if (hot && h->hot_rows > 0)
             RET(launch(h, "hot_rows_apply", [&] {
                 k_hot_apply<<<h->num_sms * 4, 256, 0, h->stream>>>(bo.scatter_base, h->tab_ld[CTR_TABLE_ITEM_EMB], h->hot_acc,
@@ -799,8 +822,16 @@ int step_core(ctr_handle* h, const RowSrc& r, int B, const StepOpts& o) {
     if (o.update) {
         const bool tg = o.table_grad && c.table_opt != CTR_TABLE_FROZEN;
         const bool ph = o.peer && c.table_opt != CTR_TABLE_FROZEN && h->comm.hot_k > 0;
-        if (o.comm || o.table_grad) RET(comm_allreduce_grads(h, tg ? o.table_grad : ph ? h->comm.hot_sum.get() : nullptr, tg ? o.table_grad_n : ph ? (size_t)h->comm.hot_k * c.D : 0));
-        if (ph)
+        const bool ph_adam = ph && c.table_opt == CTR_TABLE_ADAM;      // the hot rows' touch marks travel with their sums
+        const size_t ph_n = (size_t)h->comm.hot_k * (c.D + (ph_adam ? 1 : 0));
+        if (o.comm || o.table_grad) RET(comm_allreduce_grads(h, tg ? o.table_grad : ph ? h->comm.hot_sum.get() : nullptr, tg ? o.table_grad_n : ph ? ph_n : 0));
+        if (ph_adam) {
+            const RowAdam ra = row_adam_of(h, o.adam_batch > 0 ? o.adam_batch : B);
+            RET(launch(h, "hot_rows_adam", [&] {
+                k_hot_adam<<<h->num_sms * 8, 256, 0, h->stream>>>(h->comm.hot_tab, h->comm.hot_sum, h->comm.hot_sum.get() + (size_t)h->comm.hot_k * c.D,
+                                                                 h->comm.hot_m, h->comm.hot_v, h->comm.hot_k, c.D, ra);
+            }));
+        } else if (ph)
             RET(launch(h, "hot_rows_apply", [&] {
                 k_apply_table_grad<<<h->num_sms * 8, 256, 0, h->stream>>>(h->comm.hot_tab, h->comm.hot_sum, (long)h->comm.hot_k * c.D / 4);
             }));

@@ -38,7 +38,17 @@ enum { CTR_TABLE_USER_FEAT = 0, CTR_TABLE_ITEM_FEAT = 1, CTR_TABLE_ITEM_EMB = 2 
  * segment in a fixed order — the parity-test mode.  ADAM applies the dense solver's update (model.go:88: Adam, step
  * table_lr, cfg betas / eps, gradient divided by the batch size first, no L2) once per DISTINCT row of the batch with
  * that row's summed gradient (sorted keys → segment reduction, deterministic); rows the batch did not touch keep their
- * moments ("lazy" Adam).  Single GPU or replicated table; the moments are part of the checkpoint. */
+ * moments ("lazy" Adam).  The moments are part of the checkpoint.  Every placement: one GPU, a replicated table, or a
+ * row-sharded ITEM_EMB under world > 1.  On a row-sharded table a step of `world` ranks x batch B applies the update one
+ * GPU with batch world*B applies to the whole table, with the replicated placement's scaling (row gradients scaled by
+ * 1/world, Adam batch world*B, the dense step counter t): every distinct row that occurs in a valid slot (a history or
+ * target id inside the table, in a sample below nvalid) of any rank's batch gets exactly one update with its gradient
+ * summed over all ranks, also when that sum is exactly 0 (the row counts as touched by occurrence: its moments decay
+ * and its weights move); untouched rows keep their weights and both moments bit for bit.  Each owner keeps, beside its
+ * shard, an fp32 gradient shard plus a touched flag and a list slot per local row that the peers add into over NVLink:
+ * 4*D + 8 bytes per local row, in addition to the 8*D bytes of the two moment shards.  The hot rows replicated on every
+ * rank (reserved[0]) carry their two moments on every rank too.  The sums use red.add in arbitrary order: results are
+ * not bitwise reproducible run to run (the sharded SGD step is not either). */
 enum { CTR_TABLE_FROZEN = 0, CTR_TABLE_SGD = 1, CTR_TABLE_SGD_DETERMINISTIC = 2, CTR_TABLE_ADAM = 3 };
 
 /* dense-layer GEMM engine: exact fp32 FFMA, or wgmma 3xTF32 (error-compensated, fp32 accumulate
