@@ -19,6 +19,8 @@
 // _vec and _idx share their per-row math (attn_gate, bwd_coef, sum_subgroups); _gen keeps exact sqrtf / division.
 #pragma once
 #include "common.cuh"
+#include <algorithm>
+#include <type_traits>
 
 namespace ctr {
 
@@ -89,6 +91,45 @@ __device__ __forceinline__ float gate_cos(float dot, float nx2, float ny, float 
 // shows occupancy, not software pipelining, is what hides the gate's MUFU/shuffle latency — 32 warps/SM
 // at <= 64 registers reach ~5.9 TB/s.
 constexpr int kAttnThreads = 128, kAttnMinBlocks = 8;
+
+// grid of the _vec / _idx / _user kernels for B samples (one warp each): two waves of 8 resident blocks at most
+inline int attn_grid(int num_sms, int B) { return std::max(1, std::min((B + 3) / 4, num_sms * 16)); }
+
+// Lane map of the _vec / _idx kernels for a row of D = 4·LPR·VPL floats: LPR lanes x VPL float4 each, one load group in
+// flight per warp, 128-thread blocks at 8 blocks/SM: the gather is latency bound, so occupancy rather than deeper
+// per-warp unrolling keeps enough loads in flight (tests/cuda/gather_probe.cu, bwd_probe.cu).  The engine and the
+// kernel-level probe (tests/cuda/shard_probe.cu) both instantiate from this table.
+struct Lanes { int lpr, vpl; };
+constexpr Lanes kLanes[2][2][4] = {        // [backward][PEER][D = 16, 32, 64, 128]
+    // forward.  PEER, D = 64: over NVLink the request size matters more than the shuffle count, so 8 lanes x 2 float4
+    // (128-byte contiguous segments per load instruction) rather than 4 x 4 (64-byte segments)
+    {{{4, 1}, {4, 2}, {4, 4}, {8, 4}}, {{4, 1}, {4, 2}, {8, 2}, {8, 4}}},
+    // backward.  D = 64: 8 x 2 (128-byte contiguous red.add / load segments per row) rather than 4 x 4, although the
+    // latter executes a third fewer instructions (tests/cuda/bwd_probe.cu compares them)
+    {{{4, 1}, {4, 2}, {8, 2}, {16, 2}}, {{4, 1}, {4, 2}, {8, 2}, {16, 2}}},
+};
+template <int LPR_, int VPL_> struct LaneMap { static constexpr int LPR = LPR_, VPL = VPL_; };
+template <bool BWD, bool PEER, int I> using lanes_at = LaneMap<kLanes[BWD][PEER][I].lpr, kLanes[BWD][PEER][I].vpl>;
+
+// f(LaneMap) for D in {16, 32, 64, 128}
+template <bool BWD, bool PEER, typename F>
+void with_lanes(int D, F&& f) {
+    switch (D) {
+        case 16: f(lanes_at<BWD, PEER, 0>{}); break;
+        case 32: f(lanes_at<BWD, PEER, 1>{}); break;
+        case 64: f(lanes_at<BWD, PEER, 2>{}); break;
+        default: f(lanes_at<BWD, PEER, 3>{}); break;
+    }
+}
+// f(std::integral_constant<int, MODEL>)
+template <typename F>
+void with_model(int model, F&& f) {
+    switch (model) {
+        case MODEL_YOUTUBE: f(std::integral_constant<int, MODEL_YOUTUBE>{}); break;
+        case MODEL_DIN_COS: f(std::integral_constant<int, MODEL_DIN_COS>{}); break;
+        default:            f(std::integral_constant<int, MODEL_DIN_EUC>{}); break;
+    }
+}
 
 // attention gate a of history row s, u, against the item row v (ny = |v|); att[s] reads as 0 beyond S.  MODEL is a
 // template parameter (no per-row branches); mean pooling has a = 1.

@@ -123,8 +123,9 @@ struct RowSrc {
 
 // CTR_TABLE_ADAM on a row-sharded ITEM_EMB: every owner's shareable gradient buffer, the same layout on every rank
 // (rows = the largest shard's local rows): bytes [0, 4) the touched-row count, [4, 8) the update kernel's block ticket,
-// then a touched flag per local row (u32), the list of touched local rows (i32) and the fp32 gradient shard [rows, lde];
-// all of it zero between steps
+// then a touched flag per local row (u32), the list of touched local rows (i32) and the fp32 gradient shard [rows, lde].
+// Between steps the count, the ticket, every flag and every gradient row are zero; the list keeps the last step's rows,
+// which nobody reads: only its first `count` entries are meaningful
 struct ShardGrad { long flag_off, list_off, grad_off, bytes; };
 inline ShardGrad shard_grad_layout(long rows, long lde) {
     auto up = [](long b) { return (b + 255) & ~255L; };

@@ -282,45 +282,10 @@ AttnPath attn_path(const ctr_handle* h, const RowSrc& r) {
     return {idx_fwd ? ATTN_IDX : ATTN_VEC, ATTN_IDX};
 }
 
-// Lane map of the _vec / _idx kernels for a row of D = 4·LPR·VPL floats: LPR lanes x VPL float4 each, one load group in
-// flight per warp, 128-thread blocks at 8 blocks/SM: the gather is latency bound, so occupancy rather than deeper
-// per-warp unrolling keeps enough loads in flight (tests/cuda/gather_probe.cu, bwd_probe.cu).
-struct Lanes { int lpr, vpl; };
-constexpr Lanes kLanes[2][2][4] = {        // [backward][PEER][D = 16, 32, 64, 128]
-    // forward.  PEER, D = 64: over NVLink the request size matters more than the shuffle count, so 8 lanes x 2 float4
-    // (128-byte contiguous segments per load instruction) rather than 4 x 4 (64-byte segments)
-    {{{4, 1}, {4, 2}, {4, 4}, {8, 4}}, {{4, 1}, {4, 2}, {8, 2}, {8, 4}}},
-    // backward.  D = 64: 8 x 2 (128-byte contiguous red.add / load segments per row) rather than 4 x 4, although the
-    // latter executes a third fewer instructions (tests/cuda/bwd_probe.cu compares them)
-    {{{4, 1}, {4, 2}, {8, 2}, {16, 2}}, {{4, 1}, {4, 2}, {8, 2}, {16, 2}}},
-};
-template <int LPR_, int VPL_> struct LaneMap { static constexpr int LPR = LPR_, VPL = VPL_; };
-template <bool BWD, bool PEER, int I> using lanes_at = LaneMap<kLanes[BWD][PEER][I].lpr, kLanes[BWD][PEER][I].vpl>;
-
-// f(LaneMap) for D in {16, 32, 64, 128}
-template <bool BWD, bool PEER, typename F>
-void with_lanes(int D, F&& f) {
-    switch (D) {
-        case 16: f(lanes_at<BWD, PEER, 0>{}); break;
-        case 32: f(lanes_at<BWD, PEER, 1>{}); break;
-        case 64: f(lanes_at<BWD, PEER, 2>{}); break;
-        default: f(lanes_at<BWD, PEER, 3>{}); break;
-    }
-}
-// f(std::integral_constant<int, MODEL>)
-template <typename F>
-void with_model(int model, F&& f) {
-    switch (model) {
-        case CTR_MODEL_YOUTUBE: f(std::integral_constant<int, MODEL_YOUTUBE>{}); break;
-        case CTR_MODEL_DIN_COS: f(std::integral_constant<int, MODEL_DIN_COS>{}); break;
-        default:                f(std::integral_constant<int, MODEL_DIN_EUC>{}); break;
-    }
-}
-
-int grid_attn(const ctr_handle* h, int B) {
-    int blocks = (B + 3) / 4;
-    return std::max(1, std::min(blocks, h->num_sms * 16));     // two waves of 8 resident blocks
-}
+// the lane maps (kLanes, with_lanes), with_model and the grid rule live in attn.cuh
+static_assert(CTR_MODEL_YOUTUBE == MODEL_YOUTUBE && CTR_MODEL_DIN_COS == MODEL_DIN_COS && CTR_MODEL_DIN_EUC == MODEL_DIN_EUC,
+              "with_model takes the API's model ids");
+int grid_attn(const ctr_handle* h, int B) { return attn_grid(h->num_sms, B); }
 
 int attn_forward(ctr_handle* h, const RowSrc& r, int B) {
     const AttnFamily f = attn_path(h, r).fwd;
