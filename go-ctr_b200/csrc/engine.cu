@@ -1088,7 +1088,7 @@ int64_t ub_row_bound(const ctr_handle* h) {
     return std::max({h->ub_off ? h->ub_users : (int64_t)0, h->tab_rows[CTR_TABLE_USER_FEAT], h->idm_keys[CTR_IDMAP_USER] ? h->idm_n[CTR_IDMAP_USER] : (int64_t)0});
 }
 
-// device workspace of one update, carved from scratch slot 5 (pass base = nullptr to size it)
+// device workspace of one call, carved from a scratch slot in 256-byte pieces (pass base = nullptr to size it)
 struct Carve {
     char* base; size_t used = 0;
     template <typename T> T* take(size_t n) { T* p = (T*)(base + used); used += (std::max<size_t>(n, 1) * sizeof(T) + 255) & ~(size_t)255; return p; }
@@ -1238,6 +1238,84 @@ int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users
     h->ub_users = new_users; h->ub_n = n_new;
     return CTR_OK;
 }
+}  // namespace
+
+// ---- whole-table top-k recommendation (ctr_recommend_topk / ctr_mlp_recommend_topk; kernels in rec.cuh)
+namespace {
+// The selection over logits of key type K, on h's stream.  Per user, chunk by chunk, k_rec_scan writes the slices'
+// lists behind the running list in sl[0, k); chunk 0 merges its slices only, later chunks merge the running list with
+// theirs, in place, and the last chunk writes the user's row of ls / lr.
+template <class K>
+struct RecTopk {
+    using T = typename K::T;
+    ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge and <pre>_finish
+    int k, nex, world, rank;                // nex exclusion rows per user; local row l is global row l·world + rank
+    int64_t N; int Bc;                      // the items scored, per chunk
+    // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
+    const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
+    const size_t ssmem = rec::scan_smem_bytes<K>(k, nex), msmem = knn::smem_bytes<K>(1, 0, k);
+    const std::string n_topk = std::string(pre) + "_topk", n_merge = std::string(pre) + "_merge", n_finish = std::string(pre) + "_finish";
+    T *sl_s, *ls, *ol; int *sl_r, *lr, *orow, *oc; float* os;
+
+    // scratch slot `slot`: the caller's buffers (own(c)), then the running and slice lists, then [G][k] lists and outputs
+    template <class F>
+    int setup(int slot, int64_t G, F&& own) {
+        CU(h, cudaFuncSetAttribute(rec::k_rec_scan<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+        CU(h, cudaFuncSetAttribute(knn::k_knn_merge<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem));
+        const size_t sl = (size_t)(1 + (Bc + rps - 1) / rps) * k, gk = (size_t)G * k;
+        auto carve = [&](char* base) {
+            Carve c{base};
+            own(c);
+            sl_s = c.take<T>(sl); sl_r = c.take<int>(sl);
+            ls = c.take<T>(gk); lr = c.take<int>(gk); orow = c.take<int>(gk); ol = c.take<T>(gk); os = c.take<float>(gk); oc = c.take<int>(G);
+            return c.used;
+        };
+        char* ws = nullptr;
+        RET(scratch_get(h, slot, carve(nullptr), (void**)&ws));
+        carve(ws);
+        return CTR_OK;
+    }
+    // user j of the group, excluding excl[0, nex): score(i0, nb) queues the logits of items [i0, i0 + nb) into z
+    template <class F>
+    int user(int j, const int* excl, const T* z, F&& score) {
+        const int nchunks = (int)((N + Bc - 1) / Bc);
+        T* us = ls + (size_t)j * k; int* ur = lr + (size_t)j * k;
+        for (int c = 0; c < nchunks; c++) {
+            const int i0 = c * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
+            RET(score(i0, nb));
+            const int slices = (nb + rps - 1) / rps;
+            const bool first = c == 0, last = c == nchunks - 1;
+            RET(launch(h, n_topk.c_str(), [&] {
+                rec::k_rec_scan<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, world, rank, rps, excl, nex, k,
+                                                                               first ? nullptr : sl_s, first ? nullptr : sl_r, sl_s + k, sl_r + k);
+            }));
+            const int ns = first ? slices : slices + 1;
+            RET(launch(h, n_merge.c_str(), [&] {
+                knn::k_knn_merge<K><<<1, knn::kThreads, msmem, h->stream>>>(first ? sl_s + k : sl_s, first ? sl_r + k : sl_r, ns, k, (long)ns * k, k,
+                                                                          last ? ur : sl_r, last ? us : sl_s, nullptr);
+            }));
+        }
+        if (nchunks == 0)            // an empty table or shard: an empty list
+            RET(launch(h, n_merge.c_str(), [&] { knn::k_knn_merge<K><<<1, knn::kThreads, msmem, h->stream>>>(sl_s, sl_r, 0, k, 0, 0, ur, us, nullptr); }));
+        return CTR_OK;
+    }
+    // the lists of users [g0, g0 + ng) → the caller's outputs; after(n) runs under the same launch as k_rec_finish
+    template <class F>
+    int finish(int64_t g0, int ng, int32_t* out_rows, float* out_scores, T* out_logits, int32_t* out_count, F&& after) {
+        const long n = (long)ng * k;
+        RET(launch(h, n_finish.c_str(), [&] {
+            rec::k_rec_finish<K><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(ls, lr, k, n, orow, ol, os, oc);
+            after(n);
+        }));
+        CU(h, cudaMemcpyAsync(out_rows + g0 * k, orow, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_scores + g0 * k, os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, ol, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_count + g0, oc, (size_t)ng * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));          // the caller's per-group buffers and the lists are reused by the next group
+        return CTR_OK;
+    }
+};
+
 }  // namespace
 
 // =====================================================================================================
@@ -2451,41 +2529,20 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     }
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
     const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
-    // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
-    const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
-    const int max_slices = (Bc + rps - 1) / rps;
-    const int nex = exclude_history ? S : 0;
-    const size_t ssmem = rec::scan_smem_bytes<knn::LogitKey>(k, nex), msmem = knn::smem_bytes<knn::LogitKey>(1, 0, k);
-    CU(h, cudaFuncSetAttribute(rec::k_rec_scan<knn::LogitKey>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+    RecTopk<knn::LogitKey> sel{h, "rec", k, exclude_history ? S : 0, W, coll ? h->comm.rank : 0, N, Bc};
     const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
-
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t gk = (size_t)G * k, sl = (size_t)(1 + max_slices) * k;
-    const size_t b_h = al((size_t)G * S * 4), b_sl = al(sl * 4), b_l = al(gk * 4), b_c = al((size_t)G * 4),
-                 b_g = coll ? al((size_t)W * gk * 4) : 0;
-    char* p = nullptr;
-    RET(scratch_get(h, 4, b_h + 2 * b_sl + 5 * b_l + b_c + 2 * b_g, (void**)&p));
-    int* d_hist = (int*)p;                 p += b_h;
-    float* d_sl_s = (float*)p;             p += b_sl;      // [0, k): the user's running list, then the chunk's slice lists
-    int* d_sl_r = (int*)p;                 p += b_sl;
-    float* d_ls = (float*)p;               p += b_l;       // [G][k] the users' final lists
-    int* d_lr = (int*)p;                   p += b_l;
-    int* d_or = (int*)p;                   p += b_l;
-    float* d_ol = (float*)p;               p += b_l;
-    float* d_os = (float*)p;               p += b_l;
-    int* d_oc = (int*)p;                   p += b_c;
-    float* d_gs = (float*)p;               p += b_g;       // [W][G][k] the ranks' lists of the group
-    int* d_gr = (int*)p;
-
-    const int nchunks = (int)((N + Bc - 1) / Bc);
+    int* d_hist; float* d_gs = nullptr; int* d_gr = nullptr;      // [W][G][k] the ranks' lists of the group
+    RET(sel.setup(4, G, [&](Carve& c) {
+        d_hist = c.take<int>((size_t)G * S);
+        if (coll) { d_gs = c.take<float>((size_t)W * G * k); d_gr = c.take<int>((size_t)W * G * k); }
+    }));
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
         const int ng = (int)std::min<int64_t>(G, nu - g0);
         if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + g0 * S, (size_t)ng * S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
         for (int j = 0; j < ng; j++) {
             const int user = user_rows[g0 + j];
             const int* uh = d_hist + (size_t)j * S;
-            for (int c = 0; c < nchunks; c++) {
-                const int i0 = c * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
+            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) {
                 StepOpts o;
                 RowSrc r;
                 if (user_kernel) {
@@ -2497,39 +2554,17 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
                     RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
                     r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
                 }
-                RET(step_core(h, r, nb, o));
-                const int slices = (nb + rps - 1) / rps;
-                const bool first = c == 0, last = c == nchunks - 1;
-                RET(launch(h, "rec_topk", [&] {
-                    rec::k_rec_scan<knn::LogitKey><<<slices, knn::kThreads, ssmem, h->stream>>>(h->Z, nb, i0, W, coll ? h->comm.rank : 0, rps, uh, nex, k,
-                                                                                first ? nullptr : d_sl_s, first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
-                }));
-                // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
-                const int ns = first ? slices : slices + 1;
-                RET(launch(h, "rec_merge", [&] {
-                    knn::k_knn_merge<knn::LogitKey><<<1, knn::kThreads, msmem, h->stream>>>(
-                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, ns, k, (long)ns * k, k,
-                        last ? d_lr + (size_t)j * k : d_sl_r, last ? d_ls + (size_t)j * k : d_sl_s, nullptr);
-                }));
-            }
-            if (nchunks == 0)            // an empty shard contributes an empty list
-                RET(launch(h, "rec_merge", [&] {
-                    knn::k_knn_merge<knn::LogitKey><<<1, knn::kThreads, msmem, h->stream>>>(d_sl_s, d_sl_r, 0, k, 0, 0, d_lr + (size_t)j * k, d_ls + (size_t)j * k, nullptr);
-                }));
-        }
-        const long n = (long)ng * k;
-        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
-            RET(comm_gather_lists(h, d_ls, d_gs, sizeof(float), d_lr, d_gr, (size_t)n));
-            RET(launch(h, "rec_merge_ranks", [&] {
-                knn::k_knn_merge<knn::LogitKey><<<ng, knn::kThreads, msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, d_lr, d_ls, nullptr);
+                return step_core(h, r, nb, o);
             }));
         }
-        RET(launch(h, "rec_finish", [&] { rec::k_rec_finish<knn::LogitKey><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc); }));
-        CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-        if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaMemcpyAsync(out_count + g0, d_oc, (size_t)ng * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaStreamSynchronize(h->stream));          // d_hist and the result buffers are reused by the next group
+        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
+            const long n = (long)ng * k;
+            RET(comm_gather_lists(h, sel.ls, d_gs, sizeof(float), sel.lr, d_gr, (size_t)n));
+            RET(launch(h, "rec_merge_ranks", [&] {
+                knn::k_knn_merge<knn::LogitKey><<<ng, knn::kThreads, sel.msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, sel.lr, sel.ls, nullptr);
+            }));
+        }
+        RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [](long) {}));
     }
     return CTR_OK;
 }
@@ -3789,31 +3824,16 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
 
     // ---- every user id, resolved before anything is written
     const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy
-    const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     // items per chunk: pred_batch in whole tiles, at most the table.  The chunk's activations take
     // Bc · (units[1] + … + units[L-1]) · 8 bytes of the classifier's buffers: a large catalogue wants a large pred_batch.
     auto tiles = [](int64_t x) { return std::max<int64_t>((x + kRecTile - 1) / kRecTile, 1) * kRecTile; };
     const int Bc = (int)std::min(tiles(c.pred_batch), tiles(N));
-    const int max_slices = (Bc + rps - 1) / rps;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t gk = (size_t)G * k, sl = (size_t)(1 + max_slices) * k;
-    const size_t b_id = al((size_t)nu * 8), b_ur = al((size_t)nu * 4), b_ts = al((size_t)G * 8), b_h = al((size_t)G * S * 4),
-                 b_pre = al((size_t)H * 8), b_sl = al(sl * 8), b_slr = al(sl * 4), b_l = al(gk * 8), b_lr = al(gk * 4), b_c = al((size_t)G * 4);
-    char* p = nullptr;
-    RET(scratch_get(h, 6, b_id + b_ur + b_ts + b_h + b_pre + b_sl + b_slr + 3 * b_l + 2 * b_lr + b_c, (void**)&p));
-    long long* d_ids = (long long*)p;      p += b_id;
-    int* d_urow = (int*)p;                 p += b_ur;
-    long long* d_ts = (long long*)p;       p += b_ts;
-    int* d_hist = (int*)p;                 p += b_h;
-    double* d_pre = (double*)p;            p += b_pre;
-    double* d_sl_s = (double*)p;           p += b_sl;      // [0, k): the user's running list, then the chunk's slice lists
-    int* d_sl_r = (int*)p;                 p += b_slr;
-    double* d_ls = (double*)p;             p += b_l;       // [G][k] the users' final lists
-    double* d_ol = (double*)p;             p += b_l;
-    float* d_os = (float*)p;               p += b_l;
-    int* d_lr = (int*)p;                   p += b_lr;
-    int* d_or = (int*)p;                   p += b_lr;
-    int* d_oc = (int*)p;
+    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude_history ? S : 0, 1, 0, N, Bc};
+    long long *d_ids, *d_ts; int *d_urow, *d_hist; double* d_pre;
+    RET(sel.setup(6, G, [&](Carve& cv) {
+        d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
+        d_pre = cv.take<double>(H);
+    }));
     CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)nu * 8, cudaMemcpyHostToDevice, h->stream));
     RET(launch(h, "mlp_rec_resolve", [&] {
         k_idmap_lookup<<<mlp_grid(m, (long)nu), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, d_ids, (long)nu, d_urow);
@@ -3829,20 +3849,15 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
         const size_t need = (size_t)Bc * m->d.units[l];
         if (m->act[l].size() < need) MCU(m, m->act[l].alloc(need));
     }
-    const size_t ssmem = rec::scan_smem_bytes<knn::Logit64Key>(k, exclude_history ? S : 0), msmem = knn::smem_bytes<knn::Logit64Key>(1, 0, k);
-    CU(h, cudaFuncSetAttribute(rec::k_rec_scan<knn::Logit64Key>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
-    CU(h, cudaFuncSetAttribute(knn::k_knn_merge<knn::Logit64Key>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem));
     auto l0 = smem_w ? k_mlp64_rec_layer0<true> : k_mlp64_rec_layer0<false>;
     CU(h, cudaFuncSetAttribute(l0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l0smem));
     int l0_per_sm = 0;
     CU(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l0_per_sm, l0, 256, l0smem));
     const int l0_ctas = m->num_sms * std::max(1, l0_per_sm);
-    const int nex = exclude_history ? S : 0;
     const float* ufeat = h->tab[CTR_TABLE_USER_FEAT];
     const float* emb = h->tab[T_E];
     const long lde = h->tab_ld[T_E], ldu = h->tab_ld[CTR_TABLE_USER_FEAT];
     const int n_emb = (int)N;
-    const int nchunks = (int)((N + Bc - 1) / Bc);
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
         const int ng = (int)std::min<int64_t>(G, nu - g0);
         // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys)
@@ -3859,48 +3874,24 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
             RET(launch(h, "mlp_rec_prefix", [&] {
                 k_mlp64_prefix<<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, emb, lde, n_emb, uh, S, D, d_pre);
             }));
-            for (int ch = 0; ch < nchunks; ch++) {
-                const int i0 = ch * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
+            RET(sel.user(j, uh, m->act[L - 1], [&](int i0, int nb) -> int {       // the output layer leaves the logits in act[L-1]
                 const int ctas = std::min(l0_ctas, (nb + kRecTile - 1) / kRecTile);
                 RET(launch(h, "mlp_rec_layer0", [&] {
                     l0<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, emb, lde, h->tab[T_F], h->tab_ld[T_F], (long)h->tab_rows[T_F],
                                                         D, cF, (long)i0, nb, m->act[1]);
                 }));
-                for (int l = 1; l + 1 < L; l++)                       // the output layer leaves the logits in act[L-1]
+                for (int l = 1; l + 1 < L; l++)
                     RET(launch(h, "mlp_rec_layers", [&] {
                         k_mlp64_layer<true><<<mlp_grid(m, (long)nb * m->d.units[l + 1]), 256, 0, h->stream>>>(m->params, m->d, l, nullptr, 0, nullptr,
                                                                                                           m->act[l], m->act[l + 1], nb);
                     }));
-                const int slices = (nb + rps - 1) / rps;
-                const bool first = ch == 0, last = ch == nchunks - 1;
-                RET(launch(h, "mlp_rec_topk", [&] {
-                    rec::k_rec_scan<knn::Logit64Key><<<slices, knn::kThreads, ssmem, h->stream>>>(m->act[L - 1], nb, i0, 1, 0, rps, uh, nex, k,
-                                                                                                first ? nullptr : d_sl_s, first ? nullptr : d_sl_r, d_sl_s + k, d_sl_r + k);
-                }));
-                // chunk 0 merges its slices only; later chunks merge the running list in d_sl[0, k) with theirs, in place
-                const int ns = first ? slices : slices + 1;
-                RET(launch(h, "mlp_rec_merge", [&] {
-                    knn::k_knn_merge<knn::Logit64Key><<<1, knn::kThreads, msmem, h->stream>>>(
-                        first ? d_sl_s + k : d_sl_s, first ? d_sl_r + k : d_sl_r, ns, k, (long)ns * k, k,
-                        last ? d_lr + (size_t)j * k : d_sl_r, last ? d_ls + (size_t)j * k : d_sl_s, nullptr);
-                }));
-            }
-            if (nchunks == 0)            // an empty table: an empty list
-                RET(launch(h, "mlp_rec_merge", [&] {
-                    knn::k_knn_merge<knn::Logit64Key><<<1, knn::kThreads, msmem, h->stream>>>(d_sl_s, d_sl_r, 0, k, 0, 0, d_lr + (size_t)j * k, d_ls + (size_t)j * k, nullptr);
-                }));
+                return CTR_OK;
+            }));
         }
-        const long n = (long)ng * k;
-        RET(launch(h, "mlp_rec_finish", [&] {
-            rec::k_rec_finish<knn::Logit64Key><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ls, d_lr, k, n, d_or, d_ol, d_os, d_oc);
+        RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [&](long n) {
             // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
-            if (m->out_kind == CTR_MLP_OUT_IDENTITY) k_f64_to_f32<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ol, d_os, n);
+            if (m->out_kind == CTR_MLP_OUT_IDENTITY) k_f64_to_f32<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(sel.ol, sel.os, n);
         }));
-        CU(h, cudaMemcpyAsync(out_rows + g0 * k, d_or, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaMemcpyAsync(out_scores + g0 * k, d_os, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-        if (out_logits) CU(h, cudaMemcpyAsync(out_logits + g0 * k, d_ol, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaMemcpyAsync(out_count + g0, d_oc, (size_t)ng * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaStreamSynchronize(h->stream));          // d_hist and the result buffers are reused by the next group
     }
     return CTR_OK;
 }
