@@ -1316,6 +1316,120 @@ struct RecTopk {
     }
 };
 
+// The counting pass of the held-out ranks over logits of key type K, on h's stream (kernels in rec.cuh).  A pass is
+// m <= kMaxK targets of one (user, window): the chunks that hold a target are scored first and their targets' logits
+// copied out, then every chunk is scored and counted against the sorted targets.
+template <class K>
+struct RecRank {
+    using T = typename K::T;
+    ctr_handle* h; const char* pre;         // profile keys <pre>_target and <pre>_count
+    int nex;                                // exclusion rows per pass
+    int64_t N; int Bc;                      // the items scored, per chunk
+    const std::string n_target = std::string(pre) + "_target", n_count = std::string(pre) + "_count";
+    int *rows, *place, *nvalid, *sr; T *tl, *ss, *ol; unsigned long long* bins; long long* orank;
+
+    // scratch slot `slot`: the caller's buffers (own(c)), then one pass's target state
+    template <class F>
+    int setup(int slot, F&& own) {
+        CU(h, cudaFuncSetAttribute(rec::k_rec_rank<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(nex, 1) * 4));
+        const size_t M = knn::kMaxK;
+        auto carve = [&](char* base) {
+            Carve c{base};
+            own(c);
+            rows = c.take<int>(M); place = c.take<int>(M); nvalid = c.take<int>(1); sr = c.take<int>(M);
+            tl = c.take<T>(M); ss = c.take<T>(M); ol = c.take<T>(M); bins = c.take<unsigned long long>(M + 1); orank = c.take<long long>(M);
+            return c.used;
+        };
+        char* ws = nullptr;
+        RET(scratch_get(h, slot, carve(nullptr), (void**)&ws));
+        carve(ws);
+        return CTR_OK;
+    }
+    // targets trow[0, m) of one (user, window), excluding excl[0, nex): score(i0, nb) queues the logits of items
+    // [i0, i0 + nb) into z.  Ranks and logits go to out_rank / out_logit[0, m) (host) in stream order.
+    template <class F>
+    int pass(const int* trow, int m, const int* excl, const T* z, F&& score, int64_t* out_rank, T* out_logit) {
+        std::vector<int64_t> chunks;                         // the chunks that hold a target, each once
+        for (int j = 0; j < m; j++)
+            if (trow[j] >= 0 && trow[j] < N) chunks.push_back(trow[j] / Bc);
+        std::sort(chunks.begin(), chunks.end());
+        chunks.erase(std::unique(chunks.begin(), chunks.end()), chunks.end());
+        CU(h, cudaMemcpyAsync(rows, trow, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+        for (const int64_t c : chunks) {
+            const int i0 = (int)(c * Bc), nb = (int)std::min<int64_t>(Bc, N - i0);
+            RET(score(i0, nb));
+            RET(launch(h, n_target.c_str(), [&] { rec::k_rec_target_logits<T><<<(m + 255) / 256, 256, 0, h->stream>>>(z, nb, i0, rows, m, tl); }));
+        }
+        RET(launch(h, n_target.c_str(), [&] {
+            rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tl, m, (long)N, excl, nex, place, nvalid, ss, sr, bins);
+        }));
+        for (int64_t i0 = 0; i0 < N; i0 += Bc) {
+            const int nb = (int)std::min<int64_t>(Bc, N - i0);
+            RET(score((int)i0, nb));
+            RET(launch(h, n_count.c_str(), [&] {
+                rec::k_rec_rank<K><<<(nb + rec::kRankRows - 1) / rec::kRankRows, rec::kRankThreads, (size_t)nex * 4, h->stream>>>(
+                    z, nb, (int)i0, excl, nex, ss, sr, nvalid, bins);
+            }));
+        }
+        RET(launch(h, n_count.c_str(), [&] {
+            rec::k_rec_rank_finish<T><<<1, knn::kMaxK, 0, h->stream>>>(rows, tl, place, m, (long)N, bins, orank, ol);
+        }));
+        static_assert(sizeof(long long) == sizeof(int64_t), "int64 ranks");
+        CU(h, cudaMemcpyAsync(out_rank, orank, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(out_logit, ol, (size_t)m * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));             // the next pass reuses the target state
+        return CTR_OK;
+    }
+};
+
+// Keys grouped into passes: keys with equal key(i) share a pass, groups in order of first appearance, at most kMaxK
+// keys per pass.  Returns the passes as lists of key indices.
+template <class F>
+std::vector<std::vector<int64_t>> rank_passes(int64_t n, F&& key) {
+    std::map<decltype(key(0)), size_t> seen;
+    std::vector<std::vector<int64_t>> groups;
+    for (int64_t i = 0; i < n; i++) {
+        auto it = seen.emplace(key(i), groups.size()).first;
+        if (it->second == groups.size()) groups.emplace_back();
+        groups[it->second].push_back(i);
+    }
+    std::vector<std::vector<int64_t>> passes;
+    for (auto& g : groups)
+        for (size_t a = 0; a < g.size(); a += knn::kMaxK)
+            passes.emplace_back(g.begin() + a, g.begin() + std::min(g.size(), a + (size_t)knn::kMaxK));
+    return passes;
+}
+
+// a compensated (Neumaier) float64 sum in input order: the same terms give the same bits (ctr_rank_metrics)
+struct NeumaierSum {
+    double s = 0.0, c = 0.0;
+    void add(double x) {
+        const double t = s + x;
+        c += std::fabs(s) >= std::fabs(x) ? (s - t) + x : (x - t) + s;
+        s = t;
+    }
+    double value() const { return s + c; }
+};
+
+// ctr_recommend_topk's and ctr_rank_items' scoring pass on a single-GPU or row-sharded ITEM_EMB: the logits of items
+// [i0, i0 + nb) for (user, history uh on the device) into h->Z.  user_kernel: k_attn_fwd_user (ugrid CTAs); else index
+// buffers of the repeated user and history for the ordinary attention kernels.
+int rec_score_chunk(ctr_handle* h, bool user_kernel, bool coll, int ugrid, int user, const int* uh, int i0, int nb) {
+    const int S = h->cfg.S;
+    StepOpts o;
+    RowSrc r;
+    if (user_kernel) {
+        r = coll ? comm_src(h, nullptr, nullptr, nullptr, nb, false) : idx_src(h, nullptr, nullptr, nullptr, nb);
+        RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
+        o.x0_ready = true;
+    } else {
+        const int fg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)nb * std::max(S, 1) + 255) / 256, (int64_t)h->num_sms * 8));
+        RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
+        r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+    }
+    return step_core(h, r, nb, o);
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -2542,20 +2656,7 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
         for (int j = 0; j < ng; j++) {
             const int user = user_rows[g0 + j];
             const int* uh = d_hist + (size_t)j * S;
-            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) {
-                StepOpts o;
-                RowSrc r;
-                if (user_kernel) {
-                    r = coll ? comm_src(h, nullptr, nullptr, nullptr, nb, false) : idx_src(h, nullptr, nullptr, nullptr, nb);
-                    RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
-                    o.x0_ready = true;
-                } else {
-                    const int fg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)nb * std::max(S, 1) + 255) / 256, (int64_t)h->num_sms * 8));
-                    RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
-                    r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
-                }
-                return step_core(h, r, nb, o);
-            }));
+            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, uh, i0, nb); }));
         }
         if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
             const long n = (long)ng * k;
@@ -2565,6 +2666,92 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
             }));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [](long) {}));
+    }
+    return CTR_OK;
+}
+
+int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int32_t* item_rows, int64_t n,
+                   int32_t exclude_history, int64_t* out_rank, float* out_logit) {
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    const int T = CTR_TABLE_ITEM_EMB;
+    const int S = h->cfg.S, Bc = h->Bmax;
+    if (n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank)
+        return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank)");
+    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ranking needs a single-GPU ITEM_EMB (world=%d)", h->comm.world);
+    RET(check_tables(h));
+    const int64_t N = h->tab_rows[T];
+    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+    CU(h, cudaSetDevice(h->dev));
+    int optin = 0;
+    CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
+    const bool user_kernel = attn_user_ok(h, (size_t)optin);
+    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, false) : 0;
+
+    // keys with the same user row and window share a pass
+    const auto passes = rank_passes(n, [&](int64_t i) {
+        std::vector<int> k(hist_rows + i * S, hist_rows + (i + 1) * S);
+        k.push_back(user_rows[i]);
+        return k;
+    });
+    RecRank<knn::LogitKey> rk{h, "rank", exclude_history ? S : 0, N, Bc};
+    int* d_hist;
+    RET(rk.setup(4, [&](Carve& c) { d_hist = c.take<int>((size_t)S); }));
+    std::vector<int64_t> rank((size_t)n); std::vector<float> logit((size_t)n), pl(knn::kMaxK);
+    std::vector<int> trow(knn::kMaxK); std::vector<int64_t> pr(knn::kMaxK);
+    for (const auto& p : passes) {
+        const int64_t i = p[0];
+        const int user = user_rows[i], m = (int)p.size();
+        for (int j = 0; j < m; j++) trow[j] = item_rows[p[j]];
+        if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + i * S, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+        RET(rk.pass(trow.data(), m, d_hist, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, false, ugrid, user, d_hist, i0, nb); },
+                    pr.data(), pl.data()));
+        for (int j = 0; j < m; j++) { rank[(size_t)p[j]] = pr[j]; logit[(size_t)p[j]] = pl[j]; }
+    }
+    memcpy(out_rank, rank.data(), sizeof(int64_t) * (size_t)n);
+    if (out_logit) memcpy(out_logit, logit.data(), sizeof(float) * (size_t)n);
+    return CTR_OK;
+}
+
+int ctr_rank_metrics(const int64_t* rank, const int64_t* group, int64_t n, const int32_t* ks, int32_t nks,
+                     double* hit, double* recall, double* ndcg, double* mrr) {
+    if (!rank || !group || !ks || n < 1 || nks < 1) return set_err(nullptr, CTR_EINVAL, "bad rank metric arguments (n >= 1, nks >= 1, non-null rank, group and ks)");
+    for (int a = 0; a < nks; a++)
+        if (ks[a] < 1) return set_err(nullptr, CTR_EINVAL, "k = %d: every k must be >= 1", ks[a]);
+    for (int64_t i = 0; i < n; i++)
+        if (rank[i] == 0 || rank[i] < -1) return set_err(nullptr, CTR_EINVAL, "rank[%lld] = %lld: a rank is >= 1, or -1 for a miss", (long long)i, (long long)rank[i]);
+    // groups in order of first appearance, their keys in input order
+    std::map<int64_t, size_t> gid;
+    std::vector<std::vector<int64_t>> gk;
+    for (int64_t i = 0; i < n; i++) {
+        auto it = gid.emplace(group[i], gk.size()).first;
+        if (it->second == gk.size()) gk.emplace_back();
+        gk[it->second].push_back(rank[i]);
+    }
+    const double G = (double)gk.size();
+    for (int a = 0; a < nks; a++) {
+        const int64_t k = ks[a];
+        NeumaierSum h_sum, r_sum, n_sum;
+        for (const auto& g : gk) {
+            NeumaierSum dcg, idcg;
+            int64_t hits = 0;
+            for (const int64_t r : g)
+                if (r > 0 && r <= k) { hits++; dcg.add(1.0 / std::log2((double)r + 1.0)); }
+            for (int64_t j = 1; j <= std::min<int64_t>((int64_t)g.size(), k); j++) idcg.add(1.0 / std::log2((double)j + 1.0));
+            h_sum.add((double)hits);
+            r_sum.add((double)hits / (double)g.size());
+            n_sum.add(dcg.value() / idcg.value());
+        }
+        if (hit) hit[a] = h_sum.value() / (double)n;
+        if (recall) recall[a] = r_sum.value() / G;
+        if (ndcg) ndcg[a] = n_sum.value() / G;
+    }
+    if (mrr) {
+        NeumaierSum s;
+        for (int64_t i = 0; i < n; i++)
+            if (rank[i] > 0) s.add(1.0 / (double)rank[i]);
+        *mrr = s.value() / (double)n;
     }
     return CTR_OK;
 }
@@ -3799,36 +3986,91 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
     return CTR_OK;
 }
 
+// The float64 MLP's scoring pass over the item table (ctr_mlp_recommend_topk, ctr_mlp_rank_items; see mlp64.cuh), on
+// h's stream: per user, the prefix of layer 0 once (prefix); per chunk of items, layer 0 from it and the later layers
+// (chunk), which leave the chunk's logits in z().
+struct MlpRecScore {
+    ctr_mlp* m; ctr_handle* h;
+    int L = 0, H = 0, pcols = 0, Bc = 0, l0_ctas = 0;
+    int64_t N = 0;
+    bool smem_w = false; size_t l0smem = 0;
+
+    // the refusals, before anything is written
+    int check() {
+        if (!m->fitted) return mlp_err(m, CTR_ESTATE, "recommend before fit");
+        if (!m->classes.empty())
+            return mlp_err(m, CTR_ESTATE, "the classifier predicts %zu class labels: there is no click probability to rank items by", m->classes.size());
+        MCU(m, cudaStreamSynchronize(m->stream));                        // h's stream reads the parameters
+        L = m->d.n_layers; H = m->d.units[1];
+        if (m->d.units[L - 1] != 1) return mlp_err(m, CTR_ESTATE, "recommendation ranks one output unit, the network has %d", m->d.units[L - 1]);
+        N = h->tab_rows[CTR_TABLE_ITEM_EMB];
+        if (N > INT32_MAX) return mlp_err(m, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+        const ctr_config& c = h->cfg;
+        const int T = c.D + c.cF;
+        pcols = c.uP + c.S * c.D;
+        int optin = 0;
+        MCU(m, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->dev));
+        // W0's item rows stay in shared memory when they fit beside the item tile; else they are read through L1
+        smem_w = rec_layer0_smem(T, H, true) <= (size_t)optin;
+        l0smem = rec_layer0_smem(T, H, smem_w);
+        if (l0smem > (size_t)optin)
+            return mlp_err(m, CTR_ESTATE, "D + cF = %d item columns: a tile of %d items needs %zu bytes of shared memory (> %d)", T, kRecTile, l0smem, optin);
+        // items per chunk: pred_batch in whole tiles, at most the table.  The chunk's activations take
+        // Bc · (units[1] + … + units[L-1]) · 8 bytes of the classifier's buffers: a large catalogue wants a large pred_batch.
+        auto tiles = [](int64_t x) { return std::max<int64_t>((x + kRecTile - 1) / kRecTile, 1) * kRecTile; };
+        Bc = (int)std::min(tiles(c.pred_batch), tiles(N));
+        return CTR_OK;
+    }
+    // the classifier's activation buffers for one chunk (the last holds the logits) and layer 0's launch shape
+    int prepare() {
+        for (int l = 1; l < L; l++) {
+            const size_t need = (size_t)Bc * m->d.units[l];
+            if (m->act[l].size() < need) MCU(m, m->act[l].alloc(need));
+        }
+        CU(h, cudaFuncSetAttribute(l0(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l0smem));
+        int l0_per_sm = 0;
+        CU(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l0_per_sm, l0(), 256, l0smem));
+        l0_ctas = m->num_sms * std::max(1, l0_per_sm);
+        return CTR_OK;
+    }
+    decltype(&k_mlp64_rec_layer0<true>) l0() const { return smem_w ? k_mlp64_rec_layer0<true> : k_mlp64_rec_layer0<false>; }
+    const double* z() const { return m->act[L - 1]; }
+    // user row u with window uh (device): layer 0's user columns into d_pre [H]
+    int prefix(int u, const int* uh, double* d_pre) {
+        const ctr_config& c = h->cfg;
+        const float* up = (c.uP > 0 && u < h->tab_rows[CTR_TABLE_USER_FEAT]) ? h->tab[CTR_TABLE_USER_FEAT] + (long)u * h->tab_ld[CTR_TABLE_USER_FEAT] : nullptr;
+        return launch(h, "mlp_rec_prefix", [&] {
+            k_mlp64_prefix<<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], (int)N, uh, c.S, c.D, d_pre);
+        });
+    }
+    // the logits of items [i0, i0 + nb) from d_pre into z()
+    int chunk(const double* d_pre, int i0, int nb) {
+        const ctr_config& c = h->cfg;
+        const int ctas = std::min(l0_ctas, (nb + kRecTile - 1) / kRecTile);
+        RET(launch(h, "mlp_rec_layer0", [&] {
+            l0()<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], h->tab[CTR_TABLE_ITEM_FEAT],
+                                                  h->tab_ld[CTR_TABLE_ITEM_FEAT], (long)h->tab_rows[CTR_TABLE_ITEM_FEAT], c.D, c.cF, (long)i0, nb, m->act[1]);
+        }));
+        for (int l = 1; l + 1 < L; l++)
+            RET(launch(h, "mlp_rec_layers", [&] {
+                k_mlp64_layer<true><<<mlp_grid(m, (long)nb * m->d.units[l + 1]), 256, 0, h->stream>>>(m->params, m->d, l, nullptr, 0, nullptr,
+                                                                                                  m->act[l], m->act[l + 1], nb);
+            }));
+        return CTR_OK;
+    }
+};
+
 // ctr_mlp_recommend_topk (see mlp64.cuh): per user, the prefix of layer 0 once; per chunk of items, layer 0 from it,
 // the later layers, and the selection of rec.cuh on the float64 logits.  Everything runs on h's stream.
 int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
                   int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
-    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "recommend before fit");
-    if (!m->classes.empty())
-        return mlp_err(m, CTR_ESTATE, "the classifier predicts %zu class labels: there is no click probability to rank items by", m->classes.size());
-    MCU(m, cudaStreamSynchronize(m->stream));                            // h's stream reads the parameters
-    const int L = m->d.n_layers, H = m->d.units[1];
-    if (m->d.units[L - 1] != 1) return mlp_err(m, CTR_ESTATE, "recommendation ranks one output unit, the network has %d", m->d.units[L - 1]);
-    const int T_E = CTR_TABLE_ITEM_EMB, T_F = CTR_TABLE_ITEM_FEAT;
-    const int64_t N = h->tab_rows[T_E];
-    if (N > INT32_MAX) return mlp_err(m, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
-    const ctr_config& c = h->cfg;
-    const int S = c.S, D = c.D, cF = c.cF, pcols = c.uP + S * D, T = D + cF;
-    int optin = 0;
-    MCU(m, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->dev));
-    // W0's item rows stay in shared memory when they fit beside the item tile; else they are read through L1
-    const bool smem_w = rec_layer0_smem(T, H, true) <= (size_t)optin;
-    const size_t l0smem = rec_layer0_smem(T, H, smem_w);
-    if (l0smem > (size_t)optin)
-        return mlp_err(m, CTR_ESTATE, "D + cF = %d item columns: a tile of %d items needs %zu bytes of shared memory (> %d)", T, kRecTile, l0smem, optin);
+    MlpRecScore sc{m, h};
+    RET(sc.check());
+    const int S = h->cfg.S, H = sc.H;
 
     // ---- every user id, resolved before anything is written
     const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy
-    // items per chunk: pred_batch in whole tiles, at most the table.  The chunk's activations take
-    // Bc · (units[1] + … + units[L-1]) · 8 bytes of the classifier's buffers: a large catalogue wants a large pred_batch.
-    auto tiles = [](int64_t x) { return std::max<int64_t>((x + kRecTile - 1) / kRecTile, 1) * kRecTile; };
-    const int Bc = (int)std::min(tiles(c.pred_batch), tiles(N));
-    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude_history ? S : 0, 1, 0, N, Bc};
+    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude_history ? S : 0, 1, 0, sc.N, sc.Bc};
     long long *d_ids, *d_ts; int *d_urow, *d_hist; double* d_pre;
     RET(sel.setup(6, G, [&](Carve& cv) {
         d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
@@ -3844,20 +4086,7 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
     for (int64_t u = 0; u < nu; u++)                                     // serving.Recommend's rule: the first unknown user
         if (urow[(size_t)u] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[u]);
 
-    // ---- the classifier's activation buffers for one chunk; the last holds the logits
-    for (int l = 1; l < L; l++) {
-        const size_t need = (size_t)Bc * m->d.units[l];
-        if (m->act[l].size() < need) MCU(m, m->act[l].alloc(need));
-    }
-    auto l0 = smem_w ? k_mlp64_rec_layer0<true> : k_mlp64_rec_layer0<false>;
-    CU(h, cudaFuncSetAttribute(l0, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l0smem));
-    int l0_per_sm = 0;
-    CU(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l0_per_sm, l0, 256, l0smem));
-    const int l0_ctas = m->num_sms * std::max(1, l0_per_sm);
-    const float* ufeat = h->tab[CTR_TABLE_USER_FEAT];
-    const float* emb = h->tab[T_E];
-    const long lde = h->tab_ld[T_E], ldu = h->tab_ld[CTR_TABLE_USER_FEAT];
-    const int n_emb = (int)N;
+    RET(sc.prepare());
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
         const int ng = (int)std::min<int64_t>(G, nu - g0);
         // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys)
@@ -3868,31 +4097,77 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
             }));
         } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)ng * S, h->stream));
         for (int j = 0; j < ng; j++) {
-            const int u = urow[(size_t)(g0 + j)];
             const int* uh = d_hist + (size_t)j * S;
-            const float* up = (c.uP > 0 && u < h->tab_rows[CTR_TABLE_USER_FEAT]) ? ufeat + (long)u * ldu : nullptr;
-            RET(launch(h, "mlp_rec_prefix", [&] {
-                k_mlp64_prefix<<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, emb, lde, n_emb, uh, S, D, d_pre);
-            }));
-            RET(sel.user(j, uh, m->act[L - 1], [&](int i0, int nb) -> int {       // the output layer leaves the logits in act[L-1]
-                const int ctas = std::min(l0_ctas, (nb + kRecTile - 1) / kRecTile);
-                RET(launch(h, "mlp_rec_layer0", [&] {
-                    l0<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, emb, lde, h->tab[T_F], h->tab_ld[T_F], (long)h->tab_rows[T_F],
-                                                        D, cF, (long)i0, nb, m->act[1]);
-                }));
-                for (int l = 1; l + 1 < L; l++)
-                    RET(launch(h, "mlp_rec_layers", [&] {
-                        k_mlp64_layer<true><<<mlp_grid(m, (long)nb * m->d.units[l + 1]), 256, 0, h->stream>>>(m->params, m->d, l, nullptr, 0, nullptr,
-                                                                                                          m->act[l], m->act[l + 1], nb);
-                    }));
-                return CTR_OK;
-            }));
+            RET(sc.prefix(urow[(size_t)(g0 + j)], uh, d_pre));
+            RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [&](long n) {
             // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
             if (m->out_kind == CTR_MLP_OUT_IDENTITY) k_f64_to_f32<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(sel.ol, sel.os, n);
         }));
     }
+    return CTR_OK;
+}
+
+// ctr_mlp_rank_items: mlp_recommend's scoring pass, counted by rec.cuh's rank kernels.  Keys with the same user row and
+// ts share a pass, and so a window.
+int mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+                   int32_t exclude_history, int64_t* out_rank, double* out_logit) {
+    MlpRecScore sc{m, h};
+    RET(sc.check());
+    const int S = h->cfg.S;
+    RecRank<knn::Logit64Key> rk{h, "mlp_rank", exclude_history ? S : 0, sc.N, sc.Bc};
+    long long *d_ids, *d_ts; int *d_rows, *d_urow, *d_hist; double* d_pre;
+    RET(rk.setup(6, [&](Carve& cv) {
+        d_ids = cv.take<long long>((size_t)2 * n); d_rows = cv.take<int>((size_t)2 * n); d_ts = cv.take<long long>(n); d_urow = cv.take<int>(n);
+        d_hist = cv.take<int>((size_t)n * S); d_pre = cv.take<double>(sc.H);
+    }));
+    // ---- user and item ids → rows; every user resolved before anything is written
+    CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(d_ids + n, item_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    RET(launch(h, "mlp_rank_resolve", [&] {
+        for (int w = 0; w < 2; w++)
+            k_idmap_lookup<<<mlp_grid(m, (long)n), 256, 0, h->stream>>>(h->idm_keys[w], h->idm_vals[w], h->idm_keys[w].size() - 1, d_ids + w * n, (long)n, d_rows + w * n);
+    }));
+    std::vector<int> rows((size_t)2 * n);
+    CU(h, cudaMemcpyAsync(rows.data(), d_rows, (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    for (int64_t i = 0; i < n; i++)
+        if (rows[(size_t)i] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[i]);
+    const int* urow = rows.data(); const int* irow = rows.data() + n;
+
+    // ---- one window per (user row, ts): GetUserBehavior(uid, S, -1, ts) from the device ubcache, empty without one
+    const auto passes = rank_passes(n, [&](int64_t i) { return std::make_pair(urow[i], ts[i]); });
+    std::vector<int> pu; std::vector<long long> pts;           // the distinct (user, ts) in pass order, each once
+    std::vector<size_t> win(passes.size());
+    for (size_t p = 0; p < passes.size(); p++) {
+        const int64_t i = passes[p][0];
+        if (p > 0 && urow[passes[p - 1][0]] == urow[i] && ts[passes[p - 1][0]] == ts[i]) { win[p] = win[p - 1]; continue; }
+        win[p] = pu.size(); pu.push_back(urow[i]); pts.push_back(ts[i]);
+    }
+    const int nw = (int)pu.size();
+    if (h->ub_off) {
+        CU(h, cudaMemcpyAsync(d_urow, pu.data(), sizeof(int) * (size_t)nw, cudaMemcpyHostToDevice, h->stream));
+        CU(h, cudaMemcpyAsync(d_ts, pts.data(), sizeof(long long) * (size_t)nw, cudaMemcpyHostToDevice, h->stream));
+        RET(launch(h, "ubcache_window", [&] {
+            k_ub_window<<<grid_for_warps(h, nw), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow, d_ts, nw, S, (long)h->ub_users, d_hist);
+        }));
+    } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)nw * S, h->stream));
+
+    RET(sc.prepare());
+    std::vector<int64_t> rank((size_t)n); std::vector<double> logit((size_t)n), pl(knn::kMaxK);
+    std::vector<int> trow(knn::kMaxK); std::vector<int64_t> pr(knn::kMaxK);
+    for (size_t p = 0; p < passes.size(); p++) {
+        const auto& keys = passes[p];
+        const int m_ = (int)keys.size();
+        const int* uh = d_hist + win[p] * S;
+        for (int j = 0; j < m_; j++) trow[j] = irow[keys[j]];
+        RET(sc.prefix(urow[keys[0]], uh, d_pre));
+        RET(rk.pass(trow.data(), m_, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, pr.data(), pl.data()));
+        for (int j = 0; j < m_; j++) { rank[(size_t)keys[j]] = pr[j]; logit[(size_t)keys[j]] = pl[j]; }
+    }
+    memcpy(out_rank, rank.data(), sizeof(int64_t) * (size_t)n);
+    if (out_logit) memcpy(out_logit, logit.data(), sizeof(double) * (size_t)n);
     return CTR_OK;
 }
 }  // namespace
@@ -3931,6 +4206,19 @@ int ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, c
     m->err.clear(); h->err.clear();
     int rc = mlp_keys_check(m, h);
     if (rc == CTR_OK) rc = mlp_recommend(m, h, user_ids, ts, nu, k, exclude_history, out_rows, out_scores, out_logits, out_count);
+    return mlp_keys_done(m, h, rc);
+}
+
+int ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+                       int32_t exclude_history, int64_t* out_rank, double* out_logit) {
+    if (!m) return CTR_EINVAL;
+    if (!h || !user_ids || !item_ids || !ts || !out_rank || n < 1 || n > INT32_MAX)
+        return mlp_err(m, CTR_EINVAL, "bad rank arguments (n in [1, 2^31), user ids, item ids and ts, non-null out_rank)");
+    std::lock_guard<std::mutex> lh(h->mu);
+    std::lock_guard<std::mutex> lm(m->mu);
+    m->err.clear(); h->err.clear();
+    int rc = mlp_keys_check(m, h);
+    if (rc == CTR_OK) rc = mlp_rank_items(m, h, user_ids, item_ids, ts, n, exclude_history, out_rank, out_logit);
     return mlp_keys_done(m, h, rc);
 }
 

@@ -19,6 +19,7 @@ namespace rec {
 using knn::LogitKey;
 using knn::Logit64Key;
 using knn::kEmptyRow;
+using knn::kMaxK;
 using knn::kStep;
 using knn::kThreads;
 
@@ -97,6 +98,136 @@ __global__ void k_rec_finish(const typename K::T* __restrict__ ls, const int* __
     // valid entries are a prefix of the sorted list
     if (v && (p == k - 1 || lr[i + 1] == kEmptyRow)) out_count[j] = p + 1;
     if (!v && p == 0) out_count[j] = 0;
+}
+
+// ---- the rank of held-out items (ctr_rank_items / ctr_mlp_rank_items): the same scoring pass, counted instead of
+// selected.  One pass holds m <= kMaxK targets of one (user, window).  rank = 1 + the items that come before the
+// target in the list order (knn::better), NaN logits and the window's rows (nex > 0) never counting; -1 for a target
+// outside [0, n_items), in the window, or with a NaN logit.  The target's logit is copied out of the pass's own scoring
+// (k_rec_target_logits), so it is the list's logit bit for bit, and the counts are integer sums: deterministic.
+//   k_rec_target_logits: per chunk holding a target, the logits of the chunk's targets
+//   k_rec_rank_sort:     one CTA; the valid targets sorted in list order, each target's place, the bins zeroed
+//   k_rec_rank<K>:       per chunk; each item's bin = the first sorted target it comes before (binary search), counted
+//                        per CTA in shared memory, then one integer atomicAdd per bin
+//   k_rec_rank_finish:   one CTA; rank of the target in place p = 1 + bins[0] + ... + bins[p]
+constexpr int kRankThreads = 256;
+constexpr int kRankRows = 2048;               // items per CTA of k_rec_rank
+
+// z[b] is the logit of row row0 + b, b < n; tl[j] = the logit of target j when rows[j] lies in this chunk
+template <class T>
+__global__ void k_rec_target_logits(const T* __restrict__ z, int n, int row0, const int* __restrict__ rows, int m, T* __restrict__ tl) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const long b = (long)rows[j] - row0;
+    if (b >= 0 && b < n) tl[j] = z[b];
+}
+
+// <<<1, kMaxK>>>.  place[j]: target j's place among the v valid targets (ties by index), -1 when invalid; ss / sr [v]:
+// the valid targets' (logit, row) in list order; bins[0, m] zeroed.
+template <class K>
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int m, long n_items,
+                                                         const int* __restrict__ excl, int nex, int* __restrict__ place, int* __restrict__ nvalid,
+                                                         typename K::T* __restrict__ ss, int* __restrict__ sr, unsigned long long* __restrict__ bins) {
+    using T = typename K::T;
+    __shared__ T s[kMaxK];
+    __shared__ int r[kMaxK];
+    __shared__ int cnt;
+    const int j = threadIdx.x;
+    if (j == 0) cnt = 0;
+    bool ok = false;
+    if (j < m) {
+        r[j] = rows[j];
+        ok = r[j] >= 0 && r[j] < n_items;
+        s[j] = ok ? tl[j] : T(0);
+        ok = ok && K::qualifies(s[j]);
+        for (int e = 0; e < nex && ok; e++) ok = __ldg(excl + e) != r[j];
+        if (!ok) r[j] = -1;                                   // marks the target invalid for the others
+    }
+    for (int i = j; i <= m; i += blockDim.x) bins[i] = 0;
+    __syncthreads();
+    if (ok) atomicAdd(&cnt, 1);
+    int p = -1;
+    if (ok) {
+        p = 0;
+        for (int i = 0; i < m; i++)
+            if (r[i] >= 0 && (knn::better(s[i], r[i], s[j], r[j]) || (i < j && s[i] == s[j] && r[i] == r[j]))) p++;
+        ss[p] = s[j]; sr[p] = r[j];
+    }
+    if (j < m) place[j] = p;
+    __syncthreads();
+    if (j == 0) *nvalid = cnt;
+}
+
+// grid = slices of kRankRows items of the chunk z[0, n) (rows row0 + b); the chunk's items counted into bins[0, v)
+template <class K>
+__global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* __restrict__ z, int n, int row0, const int* __restrict__ excl, int nex,
+                                                           const typename K::T* __restrict__ ss, const int* __restrict__ sr, const int* __restrict__ nvalid,
+                                                           unsigned long long* __restrict__ bins) {
+    using T = typename K::T;
+    __shared__ T ks[kMaxK];
+    __shared__ int kr[kMaxK];
+    __shared__ int cb[kMaxK + 1];
+    extern __shared__ int ex[];                              // the exclusion rows that fall into this slice
+    __shared__ int nx;
+    const int v = *nvalid;
+    if (v == 0) return;
+    const int r0 = blockIdx.x * kRankRows, r1 = min(n, r0 + kRankRows);
+    for (int i = threadIdx.x; i < v; i += kRankThreads) { ks[i] = ss[i]; kr[i] = sr[i]; }
+    for (int i = threadIdx.x; i <= v; i += kRankThreads) cb[i] = 0;
+    if (threadIdx.x == 0) nx = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < nex; i += kRankThreads) {
+        const int e = __ldg(excl + i);
+        const long b = (long)e - row0;
+        if (b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+    }
+    __syncthreads();
+    const int mx = nx, lane = threadIdx.x & 31;
+    for (int base = r0; base < r1; base += kRankThreads) {    // uniform per warp: every lane reaches the match
+        const int b = base + threadIdx.x;
+        int q = v;                                            // bin v: comes before no target
+        if (b < r1) {
+            const T s = __ldg(z + b);
+            const int row = row0 + b;
+            bool skip = !K::qualifies(s);
+            for (int e = 0; e < mx; e++) skip |= ex[e] == row;
+            if (!skip) {
+                int lo = 0, hi = v;                           // the first target this item comes before
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (knn::better(s, row, ks[mid], kr[mid])) hi = mid; else lo = mid + 1;
+                }
+                q = lo;
+            }
+        }
+        const unsigned peers = __match_any_sync(0xffffffffu, q);
+        if (q < v && lane == __ffs(peers) - 1) atomicAdd(&cb[q], __popc(peers));
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < v; i += kRankThreads)
+        if (cb[i]) atomicAdd(bins + i, (unsigned long long)cb[i]);
+}
+
+// <<<1, kMaxK>>>: out_rank[j] and out_logit[j] (NaN for a row outside [0, n_items))
+template <class T>
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_finish(const int* __restrict__ rows, const T* __restrict__ tl, const int* __restrict__ place, int m,
+                                                           long n_items, const unsigned long long* __restrict__ bins, long long* __restrict__ out_rank,
+                                                           T* __restrict__ out_logit) {
+    __shared__ unsigned long long cum[kMaxK];
+    const int j = threadIdx.x;
+    if (j < m) cum[j] = bins[j];
+    __syncthreads();
+    for (int o = 1; o < m; o <<= 1) {                        // inclusive scan
+        unsigned long long a = 0;
+        if (j < m && j >= o) a = cum[j - o];
+        __syncthreads();
+        if (j < m) cum[j] += a;
+        __syncthreads();
+    }
+    if (j >= m) return;
+    const int p = place[j];
+    out_rank[j] = p < 0 ? -1 : (long long)cum[p] + 1;
+    out_logit[j] = rows[j] >= 0 && rows[j] < n_items ? tl[j] : T(__longlong_as_double(0x7ff8000000000000ll));
 }
 
 // the fallback route: index buffers of B samples (user, item row0 + b, hist) for the ordinary attention kernels

@@ -11,7 +11,7 @@ from . import build as _build
 
 __all__ = ["Engine", "Config", "MLPClassifier", "MLPRegressor", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
-           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE"]
+           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE", "rank_metrics"]
 
 MODEL_YOUTUBE, MODEL_DIN_COS, MODEL_DIN_EUC = 0, 1, 2
 TABLE_USER_FEAT, TABLE_ITEM_FEAT, TABLE_ITEM_EMB = 0, 1, 2
@@ -28,10 +28,10 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
-           "ctr_mlp_recommend_topk", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
+           "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
            "ctr_mlp_score", "ctr_mlp_get_output", "ctr_mlp_set_output"]
 
 
@@ -494,6 +494,39 @@ class Engine:
                                            cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
 
+    def rank_items(self, user_rows, hist, item_rows, exclude_history=True):
+        """Full-catalogue rank of held-out items (ctr_rank_items): key i is (user_rows[i], hist[i] [S], item_rows[i]).
+        Returns (ranks [n] int64, logits [n] float32): rank r means recommend_topk(user, hist, k) lists the item at
+        position r - 1 for every k >= r; -1 when it can never be listed (outside the table, in an excluded history, or a
+        NaN logit).  Each logit is bit for bit the one the list reports for that row (NaN outside the table)."""
+        u, up = _i(np.atleast_1d(user_rows))
+        it, ip = _i(np.atleast_1d(item_rows))
+        hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
+        if it.size != u.size:
+            raise ValueError("user_rows and item_rows differ in length: %d, %d" % (u.size, it.size))
+        ranks = np.empty(u.size, np.int64); logits = np.empty(u.size, np.float32)
+        self._ck(self.L.ctr_rank_items(self.h, up, hp, ip, C.c_int64(u.size), C.c_int32(int(bool(exclude_history))),
+                                       ranks.ctypes.data_as(_lp), logits.ctypes.data_as(_fp)))
+        return ranks, logits
+
+
+def rank_metrics(ranks, groups, ks):
+    """HR@k, Recall@k and NDCG@k for every k in ks, and MRR, of ranks from rank_items (ctr_rank_metrics); groups[i] is
+    key i's group (normally its user).  Returns (hit [len(ks)], recall [len(ks)], ndcg [len(ks)], mrr)."""
+    r = np.ascontiguousarray(ranks, np.int64).ravel(); g = np.ascontiguousarray(groups, np.int64).ravel()
+    k = np.ascontiguousarray(np.atleast_1d(ks), np.int32)
+    if r.size != g.size:
+        raise ValueError("ranks and groups differ in length: %d, %d" % (r.size, g.size))
+    hit = np.empty(k.size, np.float64); rec = np.empty(k.size, np.float64); ndcg = np.empty(k.size, np.float64)
+    mrr = C.c_double(0)
+    dp = C.POINTER(C.c_double)
+    L = load_library()
+    rc = L.ctr_rank_metrics(r.ctypes.data_as(_lp), g.ctypes.data_as(_lp), C.c_int64(r.size), k.ctypes.data_as(_ip), C.c_int32(k.size),
+                            hit.ctypes.data_as(dp), rec.ctypes.data_as(dp), ndcg.ctypes.data_as(dp), C.byref(mrr))
+    if rc != 0:
+        raise CtrError(rc, L.ctr_last_error(None).decode())
+    return hit, rec, ndcg, mrr.value
+
 
 MLP_ACT = {"relu": 0, "logistic": 1, "identity": 2, "tanh": 3}
 MLP_SOLVER = {"adam": 0, "sgd": 1}
@@ -617,6 +650,18 @@ class _Mlp64:
                                                out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(C.POINTER(C.c_double)),
                                                cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
+
+    def rank_items(self, engine, user_ids, item_ids, ts, exclude_history=True):
+        """Full-catalogue rank of held-out items over the feature store `engine` (ctr_mlp_rank_items): key i is (user,
+        item, ts) in external ids, windowed at ts as recommend_topk windows it.  Returns (ranks [n] int64, logits [n]
+        float64) under Engine.rank_items' rules; an unknown item id ranks -1 (logit NaN), an unknown user raises CtrError
+        with code ENOTFOUND."""
+        u, i, t = self._keys(np.atleast_1d(user_ids), np.atleast_1d(item_ids), np.atleast_1d(ts))
+        ranks = np.empty(u.size, np.int64); logits = np.empty(u.size, np.float64)
+        self._ck(self.L.ctr_mlp_rank_items(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
+                                           C.c_int64(u.size), C.c_int32(int(bool(exclude_history))), ranks.ctypes.data_as(_lp),
+                                           logits.ctypes.data_as(C.POINTER(C.c_double))))
+        return ranks, logits
 
     def get_params(self):
         """The packed parameter vector (its length follows classes_ on a classifier)."""

@@ -77,6 +77,43 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     return [ItemScore(int(item_ids[rows[0, i]]), float(scores[0, i])) for i in range(int(cnt[0]))]
 
 
+def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
+    """Offline full-catalogue evaluation of Recommend: each held-out Sample's ItemId is ranked against every ITEM_EMB row
+    for its UserId, with the history windowed at its Timestamp (the window cut), exactly as Recommend(userId, k,
+    now=Timestamp, exclude_history) would list it (Engine.rank_items / _Mlp64.rank_items).  Samples are grouped by
+    (UserId, Timestamp).  Returns {"HR@k", "Recall@k", "NDCG@k" for every k in ks, "MRR"} (engine.rank_metrics); an
+    item the model can never list — unknown to the item map, in an excluded window, a NaN logit — is a miss.
+    recSys is an Engine or a SimpleMlpPredWrap, as for Recommend.  An unknown user raises CtrError with code ENOTFOUND."""
+    if len(heldOut) == 0:
+        raise ValueError("no held-out samples")
+    u = np.fromiter((s.UserId for s in heldOut), np.int64, len(heldOut))
+    i = np.fromiter((s.ItemId for s in heldOut), np.int64, len(heldOut))
+    t = np.fromiter((s.Timestamp for s in heldOut), np.int64, len(heldOut))
+    if isinstance(recSys, _m.SimpleMlpPredWrap):
+        recSys._bound()
+        ranks, _ = recSys.pred.rank_items(recSys.engine, u, i, t, exclude_history=exclude_history)
+    else:
+        rows = recSys.idmap_lookup(_e.IDMAP_USER, u)
+        if (rows < 0).any():
+            raise _e.CtrError(_e.ENOTFOUND, "user %d is not found" % int(u[int(np.flatnonzero(rows < 0)[0])]))
+        try:
+            hist = recSys.ubcache_window(rows, t)
+        except _e.CtrError as err:          # ESTATE: no ubcache uploaded
+            if err.code != _e.ESTATE:
+                raise
+            hist = np.full((u.size, recSys.cfg.S), -1, np.int32)
+        items = recSys.idmap_lookup(_e.IDMAP_ITEM, i)
+        ranks, _ = recSys.rank_items(rows, hist, items, exclude_history=exclude_history)
+    _, groups = np.unique(np.stack([u, t], axis=1), axis=0, return_inverse=True)
+    ks = [int(k) for k in ks]
+    hit, recall, ndcg, mrr = _e.rank_metrics(ranks, groups.ravel(), ks)
+    out = {}
+    for a, k in enumerate(ks):
+        out["HR@%d" % k] = float(hit[a]); out["Recall@%d" % k] = float(recall[a]); out["NDCG@%d" % k] = float(ndcg[a])
+    out["MRR"] = float(mrr)
+    return out
+
+
 class UserBehaviorCache:
     """feature/ubcache's UserBehaviorCache (cache.go:16-55) over the engine's device ubcache, keyed by external ids
     through the engine's id maps (load_id_maps).  Every change is applied in HBM, so the next Rank / BatchPredict /

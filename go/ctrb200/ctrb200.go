@@ -328,6 +328,44 @@ func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory boo
 	return outRows, scores, logits, counts, nil
 }
 
+// RankItems is the full-catalogue rank of held-out items: for key i, every ITEM_EMB row is scored as Recommend scores it
+// for (userRows[i], histRows[i*S:(i+1)*S]) and ranks[i] is the place itemRows[i] would take in that list (1 = first),
+// or -1 when it can never be listed (outside the table, in an excluded history, or a NaN logit). For every k up to
+// 1024, Recommend(k) lists the item exactly when 0 < rank <= k, at position rank-1, with logits[i] as its logit.
+func (e *Engine) RankItems(userRows, histRows, itemRows []int32, excludeHistory bool) (ranks []int64, logits []float32, err error) {
+	n := len(userRows)
+	if n == 0 || len(itemRows) != n || len(histRows) != n*int(e.cfg.S) {
+		return nil, nil, fmt.Errorf("ctrb200: RankItems needs at least one key, one item and S history rows per key")
+	}
+	ex := C.int32_t(0)
+	if excludeHistory {
+		ex = 1
+	}
+	ranks = make([]int64, n)
+	logits = make([]float32, n)
+	if err = e.err(C.ctr_rank_items(e.h, i32(userRows), i32(histRows), i32(itemRows), C.int64_t(n), ex, i64(ranks), f32(logits))); err != nil {
+		return nil, nil, err
+	}
+	return ranks, logits, nil
+}
+
+// RankMetrics turns ranks from RankItems into HR@k, Recall@k and NDCG@k for every k in ks, and MRR; groups[i] names key
+// i's group (normally its user). A rank of -1 is a miss. Host only: no engine is needed.
+func RankMetrics(ranks, groups []int64, ks []int32) (hit, recall, ndcg []float64, mrr float64, err error) {
+	n := len(ranks)
+	if n == 0 || len(groups) != n || len(ks) == 0 {
+		return nil, nil, nil, 0, fmt.Errorf("ctrb200: RankMetrics needs equally long, non-empty ranks and groups and at least one k")
+	}
+	hit, recall, ndcg = make([]float64, len(ks)), make([]float64, len(ks)), make([]float64, len(ks))
+	var m C.double
+	rc := C.ctr_rank_metrics(i64(ranks), i64(groups), C.int64_t(n), i32(ks), C.int32_t(len(ks)), (*C.double)(unsafe.Pointer(&hit[0])),
+		(*C.double)(unsafe.Pointer(&recall[0])), (*C.double)(unsafe.Pointer(&ndcg[0])), &m)
+	if rc != C.CTR_OK {
+		return nil, nil, nil, 0, fmt.Errorf("ctr_rank_metrics: %d: %s", int(rc), C.GoString(C.ctr_last_error(nil)))
+	}
+	return hit, recall, ndcg, float64(m), nil
+}
+
 // SaveCheckpoint / LoadCheckpoint: binary snapshot of weights, Adam moments, step counter and tables.
 func (e *Engine) SaveCheckpoint(path string) error {
 	cs := C.CString(path)
@@ -781,4 +819,30 @@ func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, exc
 		return nil, nil, nil, nil, fmt.Errorf("ctr_mlp_recommend_topk: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
 	}
 	return outRows, scores, logits, counts, nil
+}
+
+// RankItems is the full-catalogue rank of held-out items for the MLP: key i is (userIds[i], itemIds[i], ts[i]), the
+// user's window cut at ts[i] as Recommend cuts it, and ranks[i] the place the item would take in Recommend's list for
+// (userIds[i], ts[i]), or -1 when it can never be listed (an unknown item id, an excluded window row, a NaN logit).
+// logits[i] is the list's float64 logit for the item. An unknown user is an error.
+func (p *MlpPredWrap) RankItems(e *Engine, userIds, itemIds []int, ts []int64, excludeHistory bool) (ranks []int64, logits []float64, err error) {
+	n := len(userIds)
+	if n == 0 || len(itemIds) != n || len(ts) != n {
+		return nil, nil, fmt.Errorf("MlpPredWrap.RankItems needs at least one key and one item and ts per key")
+	}
+	u, it := make([]int64, n), make([]int64, n)
+	for i := range userIds {
+		u[i], it[i] = int64(userIds[i]), int64(itemIds[i])
+	}
+	ex := C.int32_t(0)
+	if excludeHistory {
+		ex = 1
+	}
+	ranks = make([]int64, n)
+	logits = make([]float64, n)
+	if rc := C.ctr_mlp_rank_items(p.m, e.h, i64(u), i64(it), i64(ts), C.int64_t(n), ex, i64(ranks),
+		(*C.double)(unsafe.Pointer(&logits[0]))); rc != C.CTR_OK {
+		return nil, nil, fmt.Errorf("ctr_mlp_rank_items: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+	}
+	return ranks, logits, nil
 }

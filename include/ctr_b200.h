@@ -358,6 +358,40 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
 int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k,
                        int32_t exclude_history, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count);
 
+/* Full-catalogue rank of held-out items (the offline protocol of item recommendation): for each of n keys (user_rows[i],
+ * hist_rows[i] [n, S], item_rows[i]) every ITEM_EMB row is scored exactly as ctr_recommend_topk scores it for
+ * (user_rows[i], hist_rows[i]) — the same kernels, chunks and logits — and the target item is ranked in that list's order
+ * (logit descending, then row ascending):
+ *   out_rank[i] = 1 + the number of items that come before the target, never counting an item whose logit is NaN nor,
+ *     with exclude_history != 0, a row of the key's valid history.  For every k in [1, 1024], 0 < rank <= k exactly when
+ *     ctr_recommend_topk(user, hist, k, exclude_history) lists the target, at position rank - 1.
+ *   out_rank[i] = -1 ("cannot be recommended") for a target outside [0, I), one with a NaN logit, or, with
+ *     exclude_history, one in its own history.
+ *   out_logit (may be NULL): the target's logit from the same scoring pass, bit for bit the logit the list reports for
+ *     that row; NaN for a target outside [0, I).
+ *   Keys with the same user row and history share one scoring pass (1024 targets at most; more take several), so the
+ *     cost is about one ctr_recommend_topk per distinct (user, history) without its selection, plus one chunk re-scored
+ *     per distinct chunk that holds a target.  Ranks do not depend on how keys are grouped into calls.
+ *   Refusals write nothing: CTR_EINVAL for n < 1 and null inputs or out_rank; CTR_ESTATE for missing tables or ITEM_EMB,
+ *     more than INT32_MAX rows, or world > 1.
+ *   Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
+int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int32_t* item_rows, int64_t n,
+                   int32_t exclude_history, int64_t* out_rank, float* out_logit);
+
+/* Ranking metrics of ranks from ctr_rank_items / ctr_mlp_rank_items (host only, no device).  group[i] names key i's
+ * group (normally the user, or the user and the window cut); m_g keys in group g; hit(k) = 0 < rank <= k.
+ *   hit[a]    HR@ks[a]: the mean over keys of hit(ks[a])
+ *   recall[a] Recall@ks[a]: the mean over groups of (hits in the group) / m_g
+ *   ndcg[a]   NDCG@ks[a]: the mean over groups of DCG / IDCG, DCG = sum over hits of 1/log2(rank + 1),
+ *             IDCG = sum_{j=1..min(m_g, k)} 1/log2(j + 1)
+ *   mrr       the mean over keys of 1/rank (0 for -1)
+ * A key of rank -1 is a miss and stays in every denominator.  Groups are taken in order of first appearance and every
+ * sum is compensated in a fixed order, so a repeated call gives the same bits.  Each output may be NULL; hit, recall and
+ * ndcg have nks entries.  CTR_EINVAL (nothing written) for n < 1, nks < 1, null rank / group / ks, a k < 1, or a rank
+ * of 0 or below -1; the message is readable through ctr_last_error(NULL). */
+int ctr_rank_metrics(const int64_t* rank, const int64_t* group, int64_t n, const int32_t* ks, int32_t nks,
+                     double* hit, double* recall, double* ndcg, double* mrr);
+
 /* ---- item2vec (BASELINE config 5; SURVEY.md §8f row f1) ------------------------------------------------
  * embedding.TrainEmbedding(ch, window, dim, iter) (feature/embedding/wordemb.go:9-32): SkipGram +
  * HierarchicalSoftmax word2vec over the users' item sequences; its output is the ITEM_EMB table the hot
@@ -566,6 +600,20 @@ int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, co
  *     results cross PCIe.  Locking: h's mutex, then m's. */
 int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k,
                             int32_t exclude_history, int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count);
+/* Full-catalogue rank of held-out items with the classifier, ctr_rank_items' definition over ctr_mlp_recommend_topk's
+ * scoring: key i is (user_ids[i], item_ids[i], ts[i]); the user's window is GetUserBehavior(uid, S, -1, ts[i]), empty
+ * without a ubcache.  out_rank[i] = 1 + the items before the target in the (float64 logit descending, row ascending)
+ * order, NaN logits and (exclude_history) the window's rows never counting; -1 for a target that is excluded, has a
+ * NaN logit, or whose item id h's item map does not hold.  For every k in [1, 1024], 0 < rank <= k exactly when
+ * ctr_mlp_recommend_topk(user, ts, k, exclude_history) lists the target, at position rank - 1.  out_logit (may be NULL)
+ * is the target's float64 logit, bit for bit the list's (NaN for an unknown item).  Keys with the same user and ts
+ * share one scoring pass (1024 targets at most).
+ *   Refusals write nothing: CTR_EINVAL for n outside [1, 2^31), null inputs or out_rank and ctr_mlp_predict_keys'
+ *     argument refusals; CTR_ESTATE as ctr_mlp_recommend_topk (not fitted, classes, more than one output, a missing id
+ *     map or table, world > 1); CTR_ENOTFOUND for any unknown user id, naming the first.
+ *   Locking: h's mutex, then m's; everything runs on h's stream. */
+int  ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+                        int32_t exclude_history, int64_t* out_rank, double* out_logit);
 /* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the current length (it follows the classes) */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
