@@ -300,7 +300,8 @@ static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
     CU(h, cudaStreamSynchronize(h->stream));
     for (int j = 1; j < W; j++) {
         const CommHdr& a = all[0]; const CommHdr& b = all[(size_t)j];
-        if (a.n != b.n || a.k != b.k || a.mode != b.mode || a.flag != b.flag || a.hash[0] != b.hash[0] || a.hash[1] != b.hash[1])
+        if (a.n != b.n || a.k != b.k || a.mode != b.mode || a.flag != b.flag || a.hash[0] != b.hash[0] || a.hash[1] != b.hash[1] ||
+            a.hash[2] != b.hash[2])
             return set_err(h, CTR_EINVAL, "ranks disagree on the arguments of this collective call: rank %d (n %lld, k %d) differs from rank 0 (n %lld, k %d) — every rank must pass the same arguments",
                            j, (long long)b.n, b.k, (long long)a.n, a.k);
     }
@@ -314,14 +315,24 @@ static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
 }
 
 // The ranks' top-k lists, all-gathered on the engine stream (device buffers of the caller's scratch): send_s / send_r
-// hold n entries, recv_s / recv_r receive [world][n].  Every rank's reads of the table are queued before its send, so
-// the gather completes on a rank only after every rank has finished reading.
+// hold n entries, recv_s / recv_r receive [world][n]; send_r == nullptr gathers the scores alone (as bytes: a -0 stays
+// -0).  Every rank's reads of the table are queued before its send, so the gather completes on a rank only after every
+// rank has finished reading.
 static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, size_t score_bytes, const int* send_r, int* recv_r, size_t n) {
     Comm& cm = h->comm;
     NC(h, g_nccl.GroupStart());
     NC(h, g_nccl.AllGather(send_s, recv_s, n * score_bytes, kNcclChar, cm.nccl, h->stream));
-    NC(h, g_nccl.AllGather(send_r, recv_r, n, kNcclInt32, cm.nccl, h->stream));
+    if (send_r) NC(h, g_nccl.AllGather(send_r, recv_r, n, kNcclInt32, cm.nccl, h->stream));
     NC(h, g_nccl.GroupEnd());
+    h->launches += 1;
+    return CTR_OK;
+}
+
+// buf[0, n) summed over the ranks, in place on the engine stream (the per-target bins of ctr_rank_items).  As for
+// comm_gather_lists, the sum completes on a rank only after every rank has queued its reads before it.
+static int comm_sum_u64(ctr_handle* h, unsigned long long* buf, size_t n) {
+    Comm& cm = h->comm;
+    NC(h, g_nccl.AllReduce(buf, buf, n, kNcclUint64, kNcclSum, cm.nccl, h->stream));
     h->launches += 1;
     return CTR_OK;
 }

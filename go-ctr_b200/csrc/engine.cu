@@ -1318,15 +1318,19 @@ struct RecTopk {
 
 // The counting pass of the held-out ranks over logits of key type K, on h's stream (kernels in rec.cuh).  A pass is
 // m <= kMaxK targets of one (user, window): the chunks that hold a target are scored first and their targets' logits
-// copied out, then every chunk is scored and counted against the sorted targets.
+// copied out, then every chunk is scored and counted against the sorted targets.  On a row-sharded ITEM_EMB
+// (world > 1; collective) each rank scores its own shard: the targets' logits are all-gathered from their owners
+// before the sort, and the ranks' bins are summed before the ranks are read off.
 template <class K>
 struct RecRank {
     using T = typename K::T;
     ctr_handle* h; const char* pre;         // profile keys <pre>_target and <pre>_count
     int nex;                                // exclusion rows per pass
-    int64_t N; int Bc;                      // the items scored, per chunk
+    int64_t N; int Bc;                      // the items this rank scores (its local rows), per chunk
+    int world = 1, rank = 0;                // local row l is global row l·world + rank
+    int64_t I = N;                          // the global row count
     const std::string n_target = std::string(pre) + "_target", n_count = std::string(pre) + "_count";
-    int *rows, *place, *nvalid, *sr; T *tl, *ss, *ol; unsigned long long* bins; long long* orank;
+    int *rows, *place, *nvalid, *sr; T *tl, *tlg, *ss, *ol; unsigned long long* bins; long long* orank;
 
     // scratch slot `slot`: the caller's buffers (own(c)), then one pass's target state
     template <class F>
@@ -1338,6 +1342,7 @@ struct RecRank {
             own(c);
             rows = c.take<int>(M); place = c.take<int>(M); nvalid = c.take<int>(1); sr = c.take<int>(M);
             tl = c.take<T>(M); ss = c.take<T>(M); ol = c.take<T>(M); bins = c.take<unsigned long long>(M + 1); orank = c.take<long long>(M);
+            tlg = world > 1 ? c.take<T>((size_t)world * M) : tl;      // [world][m] the ranks' target logits
             return c.used;
         };
         char* ws = nullptr;
@@ -1349,30 +1354,38 @@ struct RecRank {
     // [i0, i0 + nb) into z.  Ranks and logits go to out_rank / out_logit[0, m) (host) in stream order.
     template <class F>
     int pass(const int* trow, int m, const int* excl, const T* z, F&& score, int64_t* out_rank, T* out_logit) {
-        std::vector<int64_t> chunks;                         // the chunks that hold a target, each once
+        std::vector<int64_t> chunks;                         // the local chunks that hold a target this rank owns, each once
         for (int j = 0; j < m; j++)
-            if (trow[j] >= 0 && trow[j] < N) chunks.push_back(trow[j] / Bc);
+            if (trow[j] >= 0 && trow[j] < I && trow[j] % world == rank) chunks.push_back(trow[j] / world / Bc);
         std::sort(chunks.begin(), chunks.end());
         chunks.erase(std::unique(chunks.begin(), chunks.end()), chunks.end());
         CU(h, cudaMemcpyAsync(rows, trow, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
         for (const int64_t c : chunks) {
             const int i0 = (int)(c * Bc), nb = (int)std::min<int64_t>(Bc, N - i0);
             RET(score(i0, nb));
-            RET(launch(h, n_target.c_str(), [&] { rec::k_rec_target_logits<T><<<(m + 255) / 256, 256, 0, h->stream>>>(z, nb, i0, rows, m, tl); }));
+            RET(launch(h, n_target.c_str(), [&] {
+                rec::k_rec_target_logits<T><<<(m + 255) / 256, 256, 0, h->stream>>>(z, nb, i0, world, rank, rows, m, tl);
+            }));
         }
+        // every rank's slot, bits as they are (a float sum would turn a -0 logit into +0); a rank owning no target
+        // sends a slot nobody reads
+        if (world > 1) RET(comm_gather_lists(h, tl, tlg, sizeof(T), nullptr, nullptr, (size_t)m));
         RET(launch(h, n_target.c_str(), [&] {
-            rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tl, m, (long)N, excl, nex, place, nvalid, ss, sr, bins);
+            rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, m, (long)I, excl, nex, place, nvalid, ss, sr, bins);
         }));
         for (int64_t i0 = 0; i0 < N; i0 += Bc) {
             const int nb = (int)std::min<int64_t>(Bc, N - i0);
             RET(score((int)i0, nb));
             RET(launch(h, n_count.c_str(), [&] {
                 rec::k_rec_rank<K><<<(nb + rec::kRankRows - 1) / rec::kRankRows, rec::kRankThreads, (size_t)nex * 4, h->stream>>>(
-                    z, nb, (int)i0, excl, nex, ss, sr, nvalid, bins);
+                    z, nb, (int)i0, world, rank, excl, nex, ss, sr, nvalid, bins);
             }));
         }
+        // the ranks' counts: queued after this rank's last read of the shard, so it completes only once every rank
+        // has finished reading, and a step queued after the call cannot change a row still being read
+        if (world > 1) RET(comm_sum_u64(h, bins, (size_t)m + 1));
         RET(launch(h, n_count.c_str(), [&] {
-            rec::k_rec_rank_finish<T><<<1, knn::kMaxK, 0, h->stream>>>(rows, tl, place, m, (long)N, bins, orank, ol);
+            rec::k_rec_rank_finish<T><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, place, m, (long)I, bins, orank, ol);
         }));
         static_assert(sizeof(long long) == sizeof(int64_t), "int64 ranks");
         CU(h, cudaMemcpyAsync(out_rank, orank, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
@@ -2675,27 +2688,54 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
     std::lock_guard<std::mutex> lk(h->mu);
     const int T = CTR_TABLE_ITEM_EMB;
+    // a row-sharded ITEM_EMB makes the call collective: every rank counts its shard, the ranks' counts are summed
+    const bool coll = emb_sharded(h);
+    const int W = coll ? h->comm.world : 1;
     const int S = h->cfg.S, Bc = h->Bmax;
-    if (n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank)
-        return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank)");
-    if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
-    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ranking needs a single-GPU ITEM_EMB (world=%d)", h->comm.world);
-    RET(check_tables(h));
-    const int64_t N = h->tab_rows[T];
-    if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
-    CU(h, cudaSetDevice(h->dev));
     int optin = 0;
-    CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
-    const bool user_kernel = attn_user_ok(h, (size_t)optin);
-    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, false) : 0;
-
+    bool user_kernel = false;
+    CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
+    const bool args_ok = !(n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank);
+    const int verdict = [&]() -> int {
+        if (!args_ok) return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank)");
+        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+        RET(coll ? comm_check(h) : check_tables(h));
+        const int64_t N = h->tab_rows[T];
+        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+        CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
+        user_kernel = attn_user_ok(h, (size_t)optin);
+        if (coll && !user_kernel)
+            return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)", S, attn_user_smem(h), optin);
+        return CTR_OK;
+    }();
     // keys with the same user row and window share a pass
-    const auto passes = rank_passes(n, [&](int64_t i) {
-        std::vector<int> k(hist_rows + i * S, hist_rows + (i + 1) * S);
-        k.push_back(user_rows[i]);
-        return k;
-    });
-    RecRank<knn::LogitKey> rk{h, "rank", exclude_history ? S : 0, N, Bc};
+    std::vector<std::vector<int64_t>> passes;
+    if (args_ok)
+        passes = rank_passes(n, [&](int64_t i) {
+            std::vector<int> k(hist_rows + i * S, hist_rows + (i + 1) * S);
+            k.push_back(user_rows[i]);
+            return k;
+        });
+    if (!coll) RET(verdict);
+    else {
+        // the arguments are hashed whenever they are well-formed, whatever this rank's state (see ctr_knn_search)
+        CommHdr hd{};
+        hd.n = n; hd.flag = exclude_history ? 1 : 0;
+        if (args_ok) {
+            hd.hash[0] = comm_hash(user_rows, (size_t)n * sizeof(int32_t));
+            hd.hash[1] = comm_hash(hist_rows, (size_t)n * S * sizeof(int32_t));
+            hd.hash[2] = comm_hash(item_rows, (size_t)n * sizeof(int32_t));
+            hd.plan = (int64_t)passes.size();            // two collectives per pass
+        }
+        const int rc = comm_agree(h, hd, verdict);
+        if (rc != CTR_OK || verdict != CTR_OK) return rc != CTR_OK ? rc : verdict;
+        RET(comm_ensure(h, false));
+        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
+        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+    }
+    const int64_t N = h->tab_local_rows[T];   // the items this rank scores
+    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
+    RecRank<knn::LogitKey> rk{h, "rank", exclude_history ? S : 0, N, Bc, W, coll ? h->comm.rank : 0, h->tab_rows[T]};
     int* d_hist;
     RET(rk.setup(4, [&](Carve& c) { d_hist = c.take<int>((size_t)S); }));
     std::vector<int64_t> rank((size_t)n); std::vector<float> logit((size_t)n), pl(knn::kMaxK);
@@ -2705,7 +2745,7 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
         const int user = user_rows[i], m = (int)p.size();
         for (int j = 0; j < m; j++) trow[j] = item_rows[p[j]];
         if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + i * S, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-        RET(rk.pass(trow.data(), m, d_hist, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, false, ugrid, user, d_hist, i0, nb); },
+        RET(rk.pass(trow.data(), m, d_hist, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, d_hist, i0, nb); },
                     pr.data(), pl.data()));
         for (int j = 0; j < m; j++) { rank[(size_t)p[j]] = pr[j]; logit[(size_t)p[j]] = pl[j]; }
     }

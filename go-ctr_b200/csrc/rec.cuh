@@ -110,24 +110,34 @@ __global__ void k_rec_finish(const typename K::T* __restrict__ ls, const int* __
 //   k_rec_rank<K>:       per chunk; each item's bin = the first sorted target it comes before (binary search), counted
 //                        per CTA in shared memory, then one integer atomicAdd per bin
 //   k_rec_rank_finish:   one CTA; rank of the target in place p = 1 + bins[0] + ... + bins[p]
+// On a row-sharded ITEM_EMB (world > 1) each rank scores its own shard (local row l = global row l·world + rank): a
+// target's logit comes from the rank that owns its row, the ranks' target logits are all-gathered into tl [world][tls]
+// (target j read from slot rows[j] % world), every rank sorts the same targets, and the bins the ranks count over their
+// shards are summed before k_rec_rank_finish.  With world = 1 and tls = m these are the single-table kernels.
 constexpr int kRankThreads = 256;
 constexpr int kRankRows = 2048;               // items per CTA of k_rec_rank
 
-// z[b] is the logit of row row0 + b, b < n; tl[j] = the logit of target j when rows[j] lies in this chunk
+// z[b] is the logit of local row row0 + b, b < n (global row (row0 + b)·world + rank); tl[j] = the logit of target j
+// when this rank owns rows[j] and it lies in this chunk
 template <class T>
-__global__ void k_rec_target_logits(const T* __restrict__ z, int n, int row0, const int* __restrict__ rows, int m, T* __restrict__ tl) {
+__global__ void k_rec_target_logits(const T* __restrict__ z, int n, int row0, int world, int rank, const int* __restrict__ rows, int m,
+                                    T* __restrict__ tl) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= m) return;
-    const long b = (long)rows[j] - row0;
+    const int t = rows[j];
+    if (t < 0 || t % world != rank) return;
+    const long b = (long)(t / world) - row0;
     if (b >= 0 && b < n) tl[j] = z[b];
 }
 
-// <<<1, kMaxK>>>.  place[j]: target j's place among the v valid targets (ties by index), -1 when invalid; ss / sr [v]:
-// the valid targets' (logit, row) in list order; bins[0, m] zeroed.
+// <<<1, kMaxK>>>.  tl [world][tls]: target j's logit at tl[(rows[j] % world)·tls + j].  place[j]: target j's place
+// among the v valid targets (ties by index), -1 when invalid; ss / sr [v]: the valid targets' (logit, row) in list
+// order; bins[0, m] zeroed.  n_items: the global row count.
 template <class K>
-__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int m, long n_items,
-                                                         const int* __restrict__ excl, int nex, int* __restrict__ place, int* __restrict__ nvalid,
-                                                         typename K::T* __restrict__ ss, int* __restrict__ sr, unsigned long long* __restrict__ bins) {
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
+                                                         long n_items, const int* __restrict__ excl, int nex, int* __restrict__ place,
+                                                         int* __restrict__ nvalid, typename K::T* __restrict__ ss, int* __restrict__ sr,
+                                                         unsigned long long* __restrict__ bins) {
     using T = typename K::T;
     __shared__ T s[kMaxK];
     __shared__ int r[kMaxK];
@@ -138,7 +148,7 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__
     if (j < m) {
         r[j] = rows[j];
         ok = r[j] >= 0 && r[j] < n_items;
-        s[j] = ok ? tl[j] : T(0);
+        s[j] = ok ? tl[(size_t)(r[j] % world) * tls + j] : T(0);
         ok = ok && K::qualifies(s[j]);
         for (int e = 0; e < nex && ok; e++) ok = __ldg(excl + e) != r[j];
         if (!ok) r[j] = -1;                                   // marks the target invalid for the others
@@ -158,10 +168,12 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__
     if (j == 0) *nvalid = cnt;
 }
 
-// grid = slices of kRankRows items of the chunk z[0, n) (rows row0 + b); the chunk's items counted into bins[0, v)
+// grid = slices of kRankRows items of the chunk z[0, n) (local rows row0 + b, global (row0 + b)·world + rank); the
+// chunk's items counted into bins[0, v).  excl: global rows (duplicates, -1 and rows past the table are harmless).
 template <class K>
-__global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* __restrict__ z, int n, int row0, const int* __restrict__ excl, int nex,
-                                                           const typename K::T* __restrict__ ss, const int* __restrict__ sr, const int* __restrict__ nvalid,
+__global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* __restrict__ z, int n, int row0, int world, int rank,
+                                                           const int* __restrict__ excl, int nex, const typename K::T* __restrict__ ss,
+                                                           const int* __restrict__ sr, const int* __restrict__ nvalid,
                                                            unsigned long long* __restrict__ bins) {
     using T = typename K::T;
     __shared__ T ks[kMaxK];
@@ -178,8 +190,8 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* 
     __syncthreads();
     for (int i = threadIdx.x; i < nex; i += kRankThreads) {
         const int e = __ldg(excl + i);
-        const long b = (long)e - row0;
-        if (b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+        const long b = (long)(e / world) - row0;
+        if (e >= 0 && e % world == rank && b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
     }
     __syncthreads();
     const int mx = nx, lane = threadIdx.x & 31;
@@ -188,7 +200,7 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* 
         int q = v;                                            // bin v: comes before no target
         if (b < r1) {
             const T s = __ldg(z + b);
-            const int row = row0 + b;
+            const int row = (row0 + b) * world + rank;
             bool skip = !K::qualifies(s);
             for (int e = 0; e < mx; e++) skip |= ex[e] == row;
             if (!skip) {
@@ -208,11 +220,11 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* 
         if (cb[i]) atomicAdd(bins + i, (unsigned long long)cb[i]);
 }
 
-// <<<1, kMaxK>>>: out_rank[j] and out_logit[j] (NaN for a row outside [0, n_items))
+// <<<1, kMaxK>>>: out_rank[j] and out_logit[j] (NaN for a row outside [0, n_items)); tl [world][tls] as for k_rec_rank_sort
 template <class T>
-__global__ void __launch_bounds__(kMaxK) k_rec_rank_finish(const int* __restrict__ rows, const T* __restrict__ tl, const int* __restrict__ place, int m,
-                                                           long n_items, const unsigned long long* __restrict__ bins, long long* __restrict__ out_rank,
-                                                           T* __restrict__ out_logit) {
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_finish(const int* __restrict__ rows, const T* __restrict__ tl, int tls, int world,
+                                                           const int* __restrict__ place, int m, long n_items, const unsigned long long* __restrict__ bins,
+                                                           long long* __restrict__ out_rank, T* __restrict__ out_logit) {
     __shared__ unsigned long long cum[kMaxK];
     const int j = threadIdx.x;
     if (j < m) cum[j] = bins[j];
@@ -227,7 +239,8 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_finish(const int* __restrict
     if (j >= m) return;
     const int p = place[j];
     out_rank[j] = p < 0 ? -1 : (long long)cum[p] + 1;
-    out_logit[j] = rows[j] >= 0 && rows[j] < n_items ? tl[j] : T(__longlong_as_double(0x7ff8000000000000ll));
+    const int t = rows[j];
+    out_logit[j] = t >= 0 && t < n_items ? tl[(size_t)(t % world) * tls + j] : T(__longlong_as_double(0x7ff8000000000000ll));
 }
 
 // the fallback route: index buffers of B samples (user, item row0 + b, hist) for the ordinary attention kernels

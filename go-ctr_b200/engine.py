@@ -498,7 +498,11 @@ class Engine:
         """Full-catalogue rank of held-out items (ctr_rank_items): key i is (user_rows[i], hist[i] [S], item_rows[i]).
         Returns (ranks [n] int64, logits [n] float32): rank r means recommend_topk(user, hist, k) lists the item at
         position r - 1 for every k >= r; -1 when it can never be listed (outside the table, in an excluded history, or a
-        NaN logit).  Each logit is bit for bit the one the list reports for that row (NaN outside the table)."""
+        NaN logit).  Each logit is bit for bit the one the list reports for that row (NaN outside the table).
+        On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search: every rank calls it with
+        the same user, history and item rows and receives the same ranks and logits, bit-identical to one GPU holding the
+        whole table; rows that differ between the ranks raise CTR_EINVAL on every rank.  No sync is needed after
+        training."""
         u, up = _i(np.atleast_1d(user_rows))
         it, ip = _i(np.atleast_1d(item_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))

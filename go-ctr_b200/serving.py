@@ -83,7 +83,10 @@ def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
     now=Timestamp, exclude_history) would list it (Engine.rank_items / _Mlp64.rank_items).  Samples are grouped by
     (UserId, Timestamp).  Returns {"HR@k", "Recall@k", "NDCG@k" for every k in ks, "MRR"} (engine.rank_metrics); an
     item the model can never list — unknown to the item map, in an excluded window, a NaN logit — is a miss.
-    recSys is an Engine or a SimpleMlpPredWrap, as for Recommend.  An unknown user raises CtrError with code ENOTFOUND."""
+    recSys is an Engine or a SimpleMlpPredWrap, as for Recommend.  An unknown user raises CtrError with code ENOTFOUND.
+    On an Engine with a row-sharded ITEM_EMB, Evaluate is collective (Engine.rank_items): every rank passes the same
+    held-out samples and returns the same metrics.  The ranks' windows and item rows must agree too, so every rank needs
+    the same id maps and behaviour cache; a rank whose rows differ makes the call raise CtrError EINVAL on every rank."""
     if len(heldOut) == 0:
         raise ValueError("no held-out samples")
     u = np.fromiter((s.UserId for s in heldOut), np.int64, len(heldOut))

@@ -332,6 +332,7 @@ func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory boo
 // for (userRows[i], histRows[i*S:(i+1)*S]) and ranks[i] is the place itemRows[i] would take in that list (1 = first),
 // or -1 when it can never be listed (outside the table, in an excluded history, or a NaN logit). For every k up to
 // 1024, Recommend(k) lists the item exactly when 0 < rank <= k, at position rank-1, with logits[i] as its logit.
+// With a row-sharded ITEM_EMB (world > 1, large table) RankItems is collective, under the same rule as Search.
 func (e *Engine) RankItems(userRows, histRows, itemRows []int32, excludeHistory bool) (ranks []int64, logits []float32, err error) {
 	n := len(userRows)
 	if n == 0 || len(itemRows) != n || len(histRows) != n*int(e.cfg.S) {

@@ -373,7 +373,15 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
  *     cost is about one ctr_recommend_topk per distinct (user, history) without its selection, plus one chunk re-scored
  *     per distinct chunk that holds a target.  Ranks do not depend on how keys are grouped into calls.
  *   Refusals write nothing: CTR_EINVAL for n < 1 and null inputs or out_rank; CTR_ESTATE for missing tables or ITEM_EMB,
- *     more than INT32_MAX rows, or world > 1.
+ *     or more than INT32_MAX rows.
+ *   Row-sharded ITEM_EMB (world > 1, large table): collective, under the same rule as ctr_knn_search — every rank calls
+ *     with the same arguments and receives the same out_rank and out_logit, bit-identical to one GPU holding the whole
+ *     table with the same weights and pred_batch; row ids stay global.  Each rank scores and counts its own shard's
+ *     items, a target's logit comes from the rank that owns its row, and the ranks' counts are summed.  Disagreeing
+ *     arguments (user, history or item rows) are CTR_EINVAL everywhere ("ranks disagree ..."), otherwise every rank
+ *     returns the verdict of the lowest failing rank; no ctr_sync or host barrier is needed between training and this
+ *     call, nor between this call and the next step.  It needs the user's history rows in shared memory (else
+ *     CTR_ESTATE, as ctr_recommend_topk).  A replicated ITEM_EMB is ranked locally, by each rank alone.
  *   Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
 int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int32_t* item_rows, int64_t n,
                    int32_t exclude_history, int64_t* out_rank, float* out_logit);

@@ -1,0 +1,77 @@
+"""Builds and loads tests/cuda/shard_rank_probe.cu: ctypes entry points that launch the rank kernels of
+go-ctr_b200/csrc/rec.cuh (the header itself, not a copy) on device buffers the test owns.  Arguments are torch tensors on
+the GPU (or None for a null pointer); the kernels run on the default stream and every call synchronises the device."""
+import ctypes as C
+import os
+import subprocess
+
+from tests import shard_probe
+
+ROOT = shard_probe.ROOT
+SRC = os.path.join(ROOT, "tests", "cuda", "shard_rank_probe.cu")
+SO = os.path.join(ROOT, "tests", "cuda", "_build", "libshard_rank_probe.so")
+DEPS = [SRC] + [os.path.join(shard_probe.CSRC, h) for h in ("rec.cuh", "knn.cuh", "mlp64.cuh", "attn.cuh", "common.cuh")]
+
+
+def build_probe(force=False):
+    """Compiles the probe with the library's own flags when it is missing or older than its sources.  Returns
+    (path, ptxas -v log or None when nothing was compiled).  Without nvcc an existing library is used as it is."""
+    nvcc = shard_probe._nvcc()
+    fresh = os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in DEPS)
+    if nvcc is None:
+        if not os.path.exists(SO):
+            raise RuntimeError("no nvcc and no %s: build the probe where nvcc is (pytest tests/test_shard_rank_probe_cpu.py)" % SO)
+        return SO, None
+    if fresh and not force:
+        return SO, None
+    os.makedirs(os.path.dirname(SO), exist_ok=True)
+    tmp = SO + ".tmp.%d" % os.getpid()                      # built aside and renamed, like go-ctr_b200/build.py
+    cmd = [nvcc] + shard_probe._library_flags() + ["-Xptxas", "-v", "-I", shard_probe.CSRC, "-o", tmp, SRC]
+    try:
+        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if r.returncode != 0:
+            raise RuntimeError("probe build failed:\n" + r.stdout)
+        os.replace(tmp, SO)
+    finally:
+        if os.path.exists(tmp):
+            os.unlink(tmp)
+    return SO, r.stdout
+
+
+_lib = None
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        L = C.CDLL(build_probe()[0])
+        L.shard_rank_probe_error.restype = C.c_char_p
+        _lib = L
+    return _lib
+
+
+def _vp(t):
+    return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+def _check(rc):
+    if rc != 0:
+        raise RuntimeError(lib().shard_rank_probe_error().decode())
+
+
+def target_logits(z, n, row0, world, rank, rows, m, tl):
+    _check(lib().shard_rank_probe_target_logits(_vp(z), n, row0, world, rank, _vp(rows), m, _vp(tl)))
+
+
+def sort(rows, tl, tls, world, m, n_items, excl, nex, place, nvalid, ss, sr, bins):
+    _check(lib().shard_rank_probe_sort(_vp(rows), _vp(tl), tls, world, m, C.c_longlong(n_items), _vp(excl), nex, _vp(place), _vp(nvalid),
+                                       _vp(ss), _vp(sr), _vp(bins)))
+
+
+def count(z, n, row0, world, rank, excl, nex, ss, sr, nvalid, bins):
+    _check(lib().shard_rank_probe_count(_vp(z), n, row0, world, rank, _vp(excl), nex, _vp(ss), _vp(sr), _vp(nvalid), _vp(bins)))
+
+
+def finish(rows, tl, tls, world, place, m, n_items, bins, out_rank, out_logit):
+    _check(lib().shard_rank_probe_finish(_vp(rows), _vp(tl), tls, world, _vp(place), m, C.c_longlong(n_items), _vp(bins), _vp(out_rank),
+                                         _vp(out_logit)))
