@@ -1242,32 +1242,53 @@ int ub_rewrite(ctr_handle* h, const UbBatch& ub, bool replace, int64_t new_users
 
 // ---- whole-table top-k recommendation (ctr_recommend_topk / ctr_mlp_recommend_topk; kernels in rec.cuh)
 namespace {
+// the exclusion mode is one of CTR_EXCLUDE_*, and CTR_EXCLUDE_SEEN comes with its cuts
+bool exclude_ok(int32_t exclude, const int64_t* max_ts) {
+    return exclude >= CTR_EXCLUDE_NONE && exclude <= CTR_EXCLUDE_SEEN && (exclude != CTR_EXCLUDE_SEEN || max_ts);
+}
+
+// CTR_EXCLUDE_SEEN: the seen bitmap of one pass (k_ub_seen) over the global rows [0, I), for user row u, cut max_ts
+// and the window uh [S] on the device; profile key `key`
+int rec_build_seen(ctr_handle* h, const char* key, unsigned* seen, int64_t I, int u, long long max_ts, const int* uh) {
+    const int S = h->cfg.S;
+    const int64_t ne = h->ub_off ? h->ub_n : 0;                         // an upper bound on the user's events
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((ne + S + 255) / 256, (int64_t)h->num_sms * 4));
+    CU(h, cudaMemsetAsync(seen, 0, (size_t)(I + 31) / 32 * sizeof(unsigned), h->stream));
+    return launch(h, key, [&] {
+        k_ub_seen<<<grid, 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->ub_off ? (long)h->ub_users : 0L, u, max_ts, uh, S, (long)I, seen);
+    });
+}
+
 // The selection over logits of key type K, on h's stream.  Per user, chunk by chunk, k_rec_scan writes the slices'
 // lists behind the running list in sl[0, k); chunk 0 merges its slices only, later chunks merge the running list with
 // theirs, in place, and the last chunk writes the user's row of ls / lr.
 template <class K>
 struct RecTopk {
     using T = typename K::T;
-    ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge and <pre>_finish
+    ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge, <pre>_finish and <pre>_seen
     int k, nex, world, rank;                // nex exclusion rows per user; local row l is global row l·world + rank
     int64_t N; int Bc;                      // the items scored, per chunk
+    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (world = 1, nex = 0): each user's seen bitmap excludes
     // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
     const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     const size_t ssmem = rec::scan_smem_bytes<K>(k, nex), msmem = knn::smem_bytes<K>(1, 0, k);
-    const std::string n_topk = std::string(pre) + "_topk", n_merge = std::string(pre) + "_merge", n_finish = std::string(pre) + "_finish";
-    T *sl_s, *ls, *ol; int *sl_r, *lr, *orow, *oc; float* os;
+    const std::string n_topk = std::string(pre) + "_topk", n_merge = std::string(pre) + "_merge", n_finish = std::string(pre) + "_finish",
+                      n_seen = std::string(pre) + "_seen";
+    T *sl_s, *ls, *ol; int *sl_r, *lr, *orow, *oc; float* os; unsigned* seen = nullptr;
 
     // scratch slot `slot`: the caller's buffers (own(c)), then the running and slice lists, then [G][k] lists and outputs
     template <class F>
     int setup(int slot, int64_t G, F&& own) {
         CU(h, cudaFuncSetAttribute(rec::k_rec_scan<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
         CU(h, cudaFuncSetAttribute(knn::k_knn_merge<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem));
+        if (by_seen) CU(h, cudaFuncSetAttribute(rec::k_rec_scan_seen<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
         const size_t sl = (size_t)(1 + (Bc + rps - 1) / rps) * k, gk = (size_t)G * k;
         auto carve = [&](char* base) {
             Carve c{base};
             own(c);
             sl_s = c.take<T>(sl); sl_r = c.take<int>(sl);
             ls = c.take<T>(gk); lr = c.take<int>(gk); orow = c.take<int>(gk); ol = c.take<T>(gk); os = c.take<float>(gk); oc = c.take<int>(G);
+            if (by_seen) seen = c.take<unsigned>((size_t)(N + 31) / 32);
             return c.used;
         };
         char* ws = nullptr;
@@ -1275,19 +1296,25 @@ struct RecTopk {
         carve(ws);
         return CTR_OK;
     }
-    // user j of the group, excluding excl[0, nex): score(i0, nb) queues the logits of items [i0, i0 + nb) into z
+    // user j of the group, excluding excl[0, nex), or under by_seen the seen set of (user row u, cut max_ts, window
+    // excl [S]): score(i0, nb) queues the logits of items [i0, i0 + nb) into z
     template <class F>
-    int user(int j, const int* excl, const T* z, F&& score) {
+    int user(int j, const int* excl, const T* z, F&& score, int u = -1, long long max_ts = 0) {
         const int nchunks = (int)((N + Bc - 1) / Bc);
         T* us = ls + (size_t)j * k; int* ur = lr + (size_t)j * k;
+        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, N, u, max_ts, excl));
         for (int c = 0; c < nchunks; c++) {
             const int i0 = c * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
             RET(score(i0, nb));
             const int slices = (nb + rps - 1) / rps;
             const bool first = c == 0, last = c == nchunks - 1;
             RET(launch(h, n_topk.c_str(), [&] {
-                rec::k_rec_scan<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, world, rank, rps, excl, nex, k,
-                                                                               first ? nullptr : sl_s, first ? nullptr : sl_r, sl_s + k, sl_r + k);
+                if (by_seen)
+                    rec::k_rec_scan_seen<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, rps, seen, k, first ? nullptr : sl_s,
+                                                                                        first ? nullptr : sl_r, sl_s + k, sl_r + k);
+                else
+                    rec::k_rec_scan<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, world, rank, rps, excl, nex, k,
+                                                                                   first ? nullptr : sl_s, first ? nullptr : sl_r, sl_s + k, sl_r + k);
             }));
             const int ns = first ? slices : slices + 1;
             RET(launch(h, n_merge.c_str(), [&] {
@@ -1324,13 +1351,14 @@ struct RecTopk {
 template <class K>
 struct RecRank {
     using T = typename K::T;
-    ctr_handle* h; const char* pre;         // profile keys <pre>_target and <pre>_count
+    ctr_handle* h; const char* pre;         // profile keys <pre>_target, <pre>_count and <pre>_seen
     int nex;                                // exclusion rows per pass
     int64_t N; int Bc;                      // the items this rank scores (its local rows), per chunk
     int world = 1, rank = 0;                // local row l is global row l·world + rank
     int64_t I = N;                          // the global row count
-    const std::string n_target = std::string(pre) + "_target", n_count = std::string(pre) + "_count";
-    int *rows, *place, *nvalid, *sr; T *tl, *tlg, *ss, *ol; unsigned long long* bins; long long* orank;
+    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (world = 1, nex = 0): each pass's seen bitmap excludes
+    const std::string n_target = std::string(pre) + "_target", n_count = std::string(pre) + "_count", n_seen = std::string(pre) + "_seen";
+    int *rows, *place, *nvalid, *sr; T *tl, *tlg, *ss, *ol; unsigned long long* bins; long long* orank; unsigned* seen = nullptr;
 
     // scratch slot `slot`: the caller's buffers (own(c)), then one pass's target state
     template <class F>
@@ -1343,6 +1371,7 @@ struct RecRank {
             rows = c.take<int>(M); place = c.take<int>(M); nvalid = c.take<int>(1); sr = c.take<int>(M);
             tl = c.take<T>(M); ss = c.take<T>(M); ol = c.take<T>(M); bins = c.take<unsigned long long>(M + 1); orank = c.take<long long>(M);
             tlg = world > 1 ? c.take<T>((size_t)world * M) : tl;      // [world][m] the ranks' target logits
+            if (by_seen) seen = c.take<unsigned>((size_t)(I + 31) / 32);
             return c.used;
         };
         char* ws = nullptr;
@@ -1350,10 +1379,11 @@ struct RecRank {
         carve(ws);
         return CTR_OK;
     }
-    // targets trow[0, m) of one (user, window), excluding excl[0, nex): score(i0, nb) queues the logits of items
-    // [i0, i0 + nb) into z.  Ranks and logits go to out_rank / out_logit[0, m) (host) in stream order.
+    // targets trow[0, m) of one (user, window), excluding excl[0, nex), or under by_seen the seen set of (user row u,
+    // cut max_ts, window excl [S]): score(i0, nb) queues the logits of items [i0, i0 + nb) into z.  Ranks and logits
+    // go to out_rank / out_logit[0, m) (host) in stream order.
     template <class F>
-    int pass(const int* trow, int m, const int* excl, const T* z, F&& score, int64_t* out_rank, T* out_logit) {
+    int pass(const int* trow, int m, const int* excl, const T* z, F&& score, int64_t* out_rank, T* out_logit, int u = -1, long long max_ts = 0) {
         std::vector<int64_t> chunks;                         // the local chunks that hold a target this rank owns, each once
         for (int j = 0; j < m; j++)
             if (trow[j] >= 0 && trow[j] < I && trow[j] % world == rank) chunks.push_back(trow[j] / world / Bc);
@@ -1370,15 +1400,18 @@ struct RecRank {
         // every rank's slot, bits as they are (a float sum would turn a -0 logit into +0); a rank owning no target
         // sends a slot nobody reads
         if (world > 1) RET(comm_gather_lists(h, tl, tlg, sizeof(T), nullptr, nullptr, (size_t)m));
+        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, I, u, max_ts, excl));
         RET(launch(h, n_target.c_str(), [&] {
-            rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, m, (long)I, excl, nex, place, nvalid, ss, sr, bins);
+            if (by_seen) rec::k_rec_rank_sort_seen<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, (long)I, seen, place, nvalid, ss, sr, bins);
+            else rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, m, (long)I, excl, nex, place, nvalid, ss, sr, bins);
         }));
         for (int64_t i0 = 0; i0 < N; i0 += Bc) {
             const int nb = (int)std::min<int64_t>(Bc, N - i0);
+            const int grid = (nb + rec::kRankRows - 1) / rec::kRankRows;
             RET(score((int)i0, nb));
             RET(launch(h, n_count.c_str(), [&] {
-                rec::k_rec_rank<K><<<(nb + rec::kRankRows - 1) / rec::kRankRows, rec::kRankThreads, (size_t)nex * 4, h->stream>>>(
-                    z, nb, (int)i0, world, rank, excl, nex, ss, sr, nvalid, bins);
+                if (by_seen) rec::k_rec_rank_seen<K><<<grid, rec::kRankThreads, 0, h->stream>>>(z, nb, (int)i0, seen, ss, sr, nvalid, bins);
+                else rec::k_rec_rank<K><<<grid, rec::kRankThreads, (size_t)nex * 4, h->stream>>>(z, nb, (int)i0, world, rank, excl, nex, ss, sr, nvalid, bins);
             }));
         }
         // the ranks' counts: queued after this rank's last read of the shard, so it completes only once every rank
@@ -2614,6 +2647,12 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
 
 int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k, int32_t exclude_history,
                        int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count) {
+    return ctr_recommend_topk_ex(h, user_rows, hist_rows, nullptr, nu, k, exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, out_rows, out_scores,
+                                 out_logits, out_count);
+}
+
+int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, int64_t nu, int32_t k,
+                          int32_t exclude, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
     std::lock_guard<std::mutex> lk(h->mu);
     const int T = CTR_TABLE_ITEM_EMB;
@@ -2624,10 +2663,13 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     int optin = 0;
     bool user_kernel = false;
     CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
-    const bool args_ok = !(k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count);
+    const bool args_ok = !(k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count) &&
+                         exclude_ok(exclude, max_ts);
     const int verdict = [&]() -> int {
         if (!args_ok)
-            return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs)", knn::kMaxK);
+            return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs, "
+                                          "exclude in [0, 2], max_ts under CTR_EXCLUDE_SEEN)", knn::kMaxK);
+        if (coll && exclude == CTR_EXCLUDE_SEEN) return set_err(h, CTR_ESTATE, "CTR_EXCLUDE_SEEN on a row-sharded ITEM_EMB");
         if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
         RET(coll ? comm_check(h) : check_tables(h));
         const int64_t N = h->tab_rows[T];
@@ -2642,7 +2684,7 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     else {
         // the arguments are hashed whenever they are well-formed, whatever this rank's state (see ctr_knn_search)
         CommHdr hd{};
-        hd.n = nu; hd.k = k; hd.flag = exclude_history ? 1 : 0;
+        hd.n = nu; hd.k = k; hd.flag = exclude;
         if (args_ok) {
             hd.hash[0] = comm_hash(user_rows, (size_t)nu * sizeof(int32_t));
             hd.hash[1] = comm_hash(hist_rows, (size_t)nu * S * sizeof(int32_t));
@@ -2656,7 +2698,8 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
     }
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
     const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
-    RecTopk<knn::LogitKey> sel{h, "rec", k, exclude_history ? S : 0, W, coll ? h->comm.rank : 0, N, Bc};
+    const bool seen = exclude == CTR_EXCLUDE_SEEN;
+    RecTopk<knn::LogitKey> sel{h, "rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, N, Bc, seen};
     const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
     int* d_hist; float* d_gs = nullptr; int* d_gr = nullptr;      // [W][G][k] the ranks' lists of the group
     RET(sel.setup(4, G, [&](Carve& c) {
@@ -2669,7 +2712,8 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
         for (int j = 0; j < ng; j++) {
             const int user = user_rows[g0 + j];
             const int* uh = d_hist + (size_t)j * S;
-            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, uh, i0, nb); }));
+            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, uh, i0, nb); },
+                         user, seen ? max_ts[g0 + j] : 0));
         }
         if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
             const long n = (long)ng * k;
@@ -2685,6 +2729,11 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
 
 int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int32_t* item_rows, int64_t n,
                    int32_t exclude_history, int64_t* out_rank, float* out_logit) {
+    return ctr_rank_items_ex(h, user_rows, hist_rows, nullptr, item_rows, n, exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, out_rank, out_logit);
+}
+
+int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, const int32_t* item_rows, int64_t n,
+                      int32_t exclude, int64_t* out_rank, float* out_logit) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
     std::lock_guard<std::mutex> lk(h->mu);
     const int T = CTR_TABLE_ITEM_EMB;
@@ -2695,9 +2744,13 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
     int optin = 0;
     bool user_kernel = false;
     CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
-    const bool args_ok = !(n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank);
+    const bool args_ok = !(n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank) && exclude_ok(exclude, max_ts);
+    const bool seen = exclude == CTR_EXCLUDE_SEEN;
     const int verdict = [&]() -> int {
-        if (!args_ok) return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank)");
+        if (!args_ok)
+            return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank, exclude in [0, 2], "
+                                          "max_ts under CTR_EXCLUDE_SEEN)");
+        if (coll && seen) return set_err(h, CTR_ESTATE, "CTR_EXCLUDE_SEEN on a row-sharded ITEM_EMB");
         if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
         RET(coll ? comm_check(h) : check_tables(h));
         const int64_t N = h->tab_rows[T];
@@ -2708,19 +2761,19 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
             return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)", S, attn_user_smem(h), optin);
         return CTR_OK;
     }();
-    // keys with the same user row and window share a pass
+    // keys with the same user row and window (and under CTR_EXCLUDE_SEEN the same cut) share a pass
     std::vector<std::vector<int64_t>> passes;
     if (args_ok)
         passes = rank_passes(n, [&](int64_t i) {
             std::vector<int> k(hist_rows + i * S, hist_rows + (i + 1) * S);
             k.push_back(user_rows[i]);
-            return k;
+            return std::make_pair(k, seen ? max_ts[i] : (int64_t)0);
         });
     if (!coll) RET(verdict);
     else {
         // the arguments are hashed whenever they are well-formed, whatever this rank's state (see ctr_knn_search)
         CommHdr hd{};
-        hd.n = n; hd.flag = exclude_history ? 1 : 0;
+        hd.n = n; hd.flag = exclude;
         if (args_ok) {
             hd.hash[0] = comm_hash(user_rows, (size_t)n * sizeof(int32_t));
             hd.hash[1] = comm_hash(hist_rows, (size_t)n * S * sizeof(int32_t));
@@ -2735,7 +2788,7 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
     }
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
     const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
-    RecRank<knn::LogitKey> rk{h, "rank", exclude_history ? S : 0, N, Bc, W, coll ? h->comm.rank : 0, h->tab_rows[T]};
+    RecRank<knn::LogitKey> rk{h, "rank", exclude == CTR_EXCLUDE_WINDOW ? S : 0, N, Bc, W, coll ? h->comm.rank : 0, h->tab_rows[T], seen};
     int* d_hist;
     RET(rk.setup(4, [&](Carve& c) { d_hist = c.take<int>((size_t)S); }));
     std::vector<int64_t> rank((size_t)n); std::vector<float> logit((size_t)n), pl(knn::kMaxK);
@@ -2746,7 +2799,7 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
         for (int j = 0; j < m; j++) trow[j] = item_rows[p[j]];
         if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + i * S, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
         RET(rk.pass(trow.data(), m, d_hist, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, d_hist, i0, nb); },
-                    pr.data(), pl.data()));
+                    pr.data(), pl.data(), user, seen ? max_ts[i] : 0));
         for (int j = 0; j < m; j++) { rank[(size_t)p[j]] = pr[j]; logit[(size_t)p[j]] = pl[j]; }
     }
     memcpy(out_rank, rank.data(), sizeof(int64_t) * (size_t)n);
@@ -4102,7 +4155,7 @@ struct MlpRecScore {
 
 // ctr_mlp_recommend_topk (see mlp64.cuh): per user, the prefix of layer 0 once; per chunk of items, layer 0 from it,
 // the later layers, and the selection of rec.cuh on the float64 logits.  Everything runs on h's stream.
-int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
+int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude,
                   int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
     MlpRecScore sc{m, h};
     RET(sc.check());
@@ -4110,7 +4163,8 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
 
     // ---- every user id, resolved before anything is written
     const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy
-    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude_history ? S : 0, 1, 0, sc.N, sc.Bc};
+    const bool seen = exclude == CTR_EXCLUDE_SEEN;
+    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, 1, 0, sc.N, sc.Bc, seen};
     long long *d_ids, *d_ts; int *d_urow, *d_hist; double* d_pre;
     RET(sel.setup(6, G, [&](Carve& cv) {
         d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
@@ -4139,7 +4193,7 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
         for (int j = 0; j < ng; j++) {
             const int* uh = d_hist + (size_t)j * S;
             RET(sc.prefix(urow[(size_t)(g0 + j)], uh, d_pre));
-            RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }));
+            RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, urow[(size_t)(g0 + j)], ts[g0 + j]));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [&](long n) {
             // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
@@ -4152,11 +4206,11 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
 // ctr_mlp_rank_items: mlp_recommend's scoring pass, counted by rec.cuh's rank kernels.  Keys with the same user row and
 // ts share a pass, and so a window.
 int mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
-                   int32_t exclude_history, int64_t* out_rank, double* out_logit) {
+                   int32_t exclude, int64_t* out_rank, double* out_logit) {
     MlpRecScore sc{m, h};
     RET(sc.check());
     const int S = h->cfg.S;
-    RecRank<knn::Logit64Key> rk{h, "mlp_rank", exclude_history ? S : 0, sc.N, sc.Bc};
+    RecRank<knn::Logit64Key> rk{h, "mlp_rank", exclude == CTR_EXCLUDE_WINDOW ? S : 0, sc.N, sc.Bc, 1, 0, sc.N, exclude == CTR_EXCLUDE_SEEN};
     long long *d_ids, *d_ts; int *d_rows, *d_urow, *d_hist; double* d_pre;
     RET(rk.setup(6, [&](Carve& cv) {
         d_ids = cv.take<long long>((size_t)2 * n); d_rows = cv.take<int>((size_t)2 * n); d_ts = cv.take<long long>(n); d_urow = cv.take<int>(n);
@@ -4203,7 +4257,8 @@ int mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int
         const int* uh = d_hist + win[p] * S;
         for (int j = 0; j < m_; j++) trow[j] = irow[keys[j]];
         RET(sc.prefix(urow[keys[0]], uh, d_pre));
-        RET(rk.pass(trow.data(), m_, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, pr.data(), pl.data()));
+        RET(rk.pass(trow.data(), m_, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, pr.data(), pl.data(),
+                    urow[keys[0]], ts[keys[0]]));
         for (int j = 0; j < m_; j++) { rank[(size_t)keys[j]] = pr[j]; logit[(size_t)keys[j]] = pl[j]; }
     }
     memcpy(out_rank, rank.data(), sizeof(int64_t) * (size_t)n);
@@ -4238,27 +4293,40 @@ int ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, con
 
 int ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude_history,
                            int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
+    return ctr_mlp_recommend_topk_ex(m, h, user_ids, ts, nu, k, exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, out_rows, out_scores,
+                                     out_logits, out_count);
+}
+
+int ctr_mlp_recommend_topk_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude,
+                              int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
     if (!m) return CTR_EINVAL;
     if (!h || !user_ids || !ts || !out_rows || !out_scores || !out_count || nu < 1 || k < 1 || k > knn::kMaxK)
         return mlp_err(m, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user ids and ts, non-null outputs)", knn::kMaxK);
+    if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
     std::lock_guard<std::mutex> lh(h->mu);
     std::lock_guard<std::mutex> lm(m->mu);
     m->err.clear(); h->err.clear();
     int rc = mlp_keys_check(m, h);
-    if (rc == CTR_OK) rc = mlp_recommend(m, h, user_ids, ts, nu, k, exclude_history, out_rows, out_scores, out_logits, out_count);
+    if (rc == CTR_OK) rc = mlp_recommend(m, h, user_ids, ts, nu, k, exclude, out_rows, out_scores, out_logits, out_count);
     return mlp_keys_done(m, h, rc);
 }
 
 int ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
                        int32_t exclude_history, int64_t* out_rank, double* out_logit) {
+    return ctr_mlp_rank_items_ex(m, h, user_ids, item_ids, ts, n, exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, out_rank, out_logit);
+}
+
+int ctr_mlp_rank_items_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+                          int32_t exclude, int64_t* out_rank, double* out_logit) {
     if (!m) return CTR_EINVAL;
     if (!h || !user_ids || !item_ids || !ts || !out_rank || n < 1 || n > INT32_MAX)
         return mlp_err(m, CTR_EINVAL, "bad rank arguments (n in [1, 2^31), user ids, item ids and ts, non-null out_rank)");
+    if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
     std::lock_guard<std::mutex> lh(h->mu);
     std::lock_guard<std::mutex> lm(m->mu);
     m->err.clear(); h->err.clear();
     int rc = mlp_keys_check(m, h);
-    if (rc == CTR_OK) rc = mlp_rank_items(m, h, user_ids, item_ids, ts, n, exclude_history, out_rank, out_logit);
+    if (rc == CTR_OK) rc = mlp_rank_items(m, h, user_ids, item_ids, ts, n, exclude, out_rank, out_logit);
     return mlp_keys_done(m, h, rc);
 }
 

@@ -8,7 +8,9 @@
 //   k_rec_scan:   grid = slices of the chunk; each CTA writes the top-k of its slice as it stands (empty entries included)
 //   k_knn_merge<LogitKey>: merges the user's running list with the slices' lists
 //   k_rec_finish: the users' lists → rows (-1 past the count), logits and scores (0 past the count), counts
-// ctr_mlp_recommend_topk runs the same three kernels on the float64 MLP's logits, with Logit64Key.
+// ctr_mlp_recommend_topk runs the same three kernels on the float64 MLP's logits, with Logit64Key.  Under
+// CTR_EXCLUDE_SEEN the _seen siblings of k_rec_scan, k_rec_rank_sort and k_rec_rank test each row against the user's
+// seen bitmap (k_ub_seen, ubcache.cuh) in place of the window's rows.
 #pragma once
 #include "knn.cuh"
 #include "mlp64.cuh"
@@ -27,17 +29,23 @@ using knn::kThreads;
 template <class K>
 __host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<K>(1, 0, k) + (size_t)nex * 4 + 16; }
 
+// The seen set of CTR_EXCLUDE_SEEN (k_ub_seen, ubcache.cuh): a bitmap over the global rows [0, I), bit r & 31 of word
+// r >> 5 set when row r is excluded.  Any history length costs one word load per item and ⌈I / 32⌉ words, a 32·D-th of
+// the ITEM_EMB table.  SEEN is single-table only (world = 1), so its kernels take no (world, rank).
+__device__ __forceinline__ bool rec_seen(const unsigned* __restrict__ seen, int row) { return (__ldg(seen + (row >> 5)) >> (row & 31)) & 1u; }
+
 // z[b] is the logit of local row row0 + b, b < n; local row l is global row l·world + rank (a row-sharded ITEM_EMB; 1
 // and 0 otherwise).  excl[0, nex): global rows that must not be returned (duplicates and rows outside the table are
 // harmless).  run_s / run_r: the user's running list over the earlier chunks (nullptr for the first): only rows that
 // beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row lies in an
 // earlier chunk, so the fillers are told apart by row and written back as empty entries.
-// Out: per slice the top-k list of global rows, [slices][k].
-template <class K>
-__global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
-                                                        const int* __restrict__ excl, int nex, int k,
-                                                        const typename K::T* run_s, const int* run_r,
-                                                        typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
+// Out: per slice the top-k list of global rows, [slices][k].  SEEN (k_rec_scan_seen): the rows of the bitmap seen are
+// excluded in place of excl.
+template <class K, bool SEEN>
+__device__ __forceinline__ void rec_scan(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
+                                         const int* __restrict__ excl, int nex, const unsigned* __restrict__ seen, int k,
+                                         const typename K::T* run_s, const int* run_r,
+                                         typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
     using T = typename K::T;
     extern __shared__ __align__(16) char smem_raw[];
     const knn::Smem<K> sm = knn::carve<K>(smem_raw, 1, 0, k);
@@ -49,12 +57,14 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __re
     for (int i = threadIdx.x; i < k; i += kThreads) { sm.ls[i] = t_s; sm.lr[i] = t_r; }
     if (threadIdx.x == 0) { sm.bn[0] = 0; nx = 0; }
     __syncthreads();
-    for (int i = threadIdx.x; i < nex; i += kThreads) {       // usually none of the user's rows fall into this slice
-        const int e = __ldg(excl + i);
-        const long b = (long)(e / world) - row0;
-        if (e >= 0 && e % world == rank && b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+    if constexpr (!SEEN) {
+        for (int i = threadIdx.x; i < nex; i += kThreads) {       // usually none of the user's rows fall into this slice
+            const int e = __ldg(excl + i);
+            const long b = (long)(e / world) - row0;
+            if (e >= 0 && e % world == rank && b >= r0 && b < r1) ex[atomicAdd(&nx, 1)] = e;
+        }
+        __syncthreads();
     }
-    __syncthreads();
     const int m = nx;
     for (int base = r0; base < r1; base += kStep) {
 #pragma unroll
@@ -63,7 +73,8 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __re
             if (b >= r1) continue;
             const int row = (row0 + b) * world + rank;
             bool skip = false;
-            for (int e = 0; e < m; e++) skip |= ex[e] == row;
+            if constexpr (SEEN) skip = rec_seen(seen, row);
+            else for (int e = 0; e < m; e++) skip |= ex[e] == row;
             if (!skip) knn::offer(sm, 0, k, __ldg(z + b), row);
         }
         __syncthreads();
@@ -75,6 +86,23 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __re
         out_s[(size_t)blockIdx.x * k + i] = filler ? K::empty() : sm.ls[i];
         out_row[(size_t)blockIdx.x * k + i] = filler ? kEmptyRow : sm.lr[i];
     }
+}
+
+template <class K>
+__global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
+                                                        const int* __restrict__ excl, int nex, int k,
+                                                        const typename K::T* run_s, const int* run_r,
+                                                        typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
+    rec_scan<K, false>(z, n, row0, world, rank, rows_per_slice, excl, nex, nullptr, k, run_s, run_r, out_s, out_row);
+}
+
+// k_rec_scan on a single table with the rows of the bitmap seen excluded; dynamic shared memory scan_smem_bytes<K>(k, 0)
+template <class K>
+__global__ void __launch_bounds__(kThreads) k_rec_scan_seen(const typename K::T* __restrict__ z, int n, int row0, int rows_per_slice,
+                                                             const unsigned* __restrict__ seen, int k,
+                                                             const typename K::T* run_s, const int* run_r,
+                                                             typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
+    rec_scan<K, true>(z, n, row0, 1, 0, rows_per_slice, nullptr, 0, seen, k, run_s, run_r, out_s, out_row);
 }
 
 // the score of a logit, bit-identical to what the predict route returns for the same sample: sigmoid32, the function
@@ -133,11 +161,11 @@ __global__ void k_rec_target_logits(const T* __restrict__ z, int n, int row0, in
 // <<<1, kMaxK>>>.  tl [world][tls]: target j's logit at tl[(rows[j] % world)·tls + j].  place[j]: target j's place
 // among the v valid targets (ties by index), -1 when invalid; ss / sr [v]: the valid targets' (logit, row) in list
 // order; bins[0, m] zeroed.  n_items: the global row count.
-template <class K>
-__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
-                                                         long n_items, const int* __restrict__ excl, int nex, int* __restrict__ place,
-                                                         int* __restrict__ nvalid, typename K::T* __restrict__ ss, int* __restrict__ sr,
-                                                         unsigned long long* __restrict__ bins) {
+template <class K, bool SEEN>
+__device__ __forceinline__ void rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
+                                              long n_items, const int* __restrict__ excl, int nex, const unsigned* __restrict__ seen,
+                                              int* __restrict__ place, int* __restrict__ nvalid, typename K::T* __restrict__ ss,
+                                              int* __restrict__ sr, unsigned long long* __restrict__ bins) {
     using T = typename K::T;
     __shared__ T s[kMaxK];
     __shared__ int r[kMaxK];
@@ -150,7 +178,8 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__
         ok = r[j] >= 0 && r[j] < n_items;
         s[j] = ok ? tl[(size_t)(r[j] % world) * tls + j] : T(0);
         ok = ok && K::qualifies(s[j]);
-        for (int e = 0; e < nex && ok; e++) ok = __ldg(excl + e) != r[j];
+        if constexpr (SEEN) ok = ok && !rec_seen(seen, r[j]);
+        else for (int e = 0; e < nex && ok; e++) ok = __ldg(excl + e) != r[j];
         if (!ok) r[j] = -1;                                   // marks the target invalid for the others
     }
     for (int i = j; i <= m; i += blockDim.x) bins[i] = 0;
@@ -166,6 +195,22 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__
     if (j < m) place[j] = p;
     __syncthreads();
     if (j == 0) *nvalid = cnt;
+}
+
+template <class K>
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
+                                                         long n_items, const int* __restrict__ excl, int nex, int* __restrict__ place,
+                                                         int* __restrict__ nvalid, typename K::T* __restrict__ ss, int* __restrict__ sr,
+                                                         unsigned long long* __restrict__ bins) {
+    rec_rank_sort<K, false>(rows, tl, tls, world, m, n_items, excl, nex, nullptr, place, nvalid, ss, sr, bins);
+}
+
+// k_rec_rank_sort on a single table (tl [m]) with the rows of the bitmap seen excluded
+template <class K>
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort_seen(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int m, long n_items,
+                                                              const unsigned* __restrict__ seen, int* __restrict__ place, int* __restrict__ nvalid,
+                                                              typename K::T* __restrict__ ss, int* __restrict__ sr, unsigned long long* __restrict__ bins) {
+    rec_rank_sort<K, true>(rows, tl, m, 1, m, n_items, nullptr, 0, seen, place, nvalid, ss, sr, bins);
 }
 
 // grid = slices of kRankRows items of the chunk z[0, n) (local rows row0 + b, global (row0 + b)·world + rank); the
@@ -204,6 +249,46 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* 
             bool skip = !K::qualifies(s);
             for (int e = 0; e < mx; e++) skip |= ex[e] == row;
             if (!skip) {
+                int lo = 0, hi = v;                           // the first target this item comes before
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (knn::better(s, row, ks[mid], kr[mid])) hi = mid; else lo = mid + 1;
+                }
+                q = lo;
+            }
+        }
+        const unsigned peers = __match_any_sync(0xffffffffu, q);
+        if (q < v && lane == __ffs(peers) - 1) atomicAdd(&cb[q], __popc(peers));
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < v; i += kRankThreads)
+        if (cb[i]) atomicAdd(bins + i, (unsigned long long)cb[i]);
+}
+
+// k_rec_rank on a single table with the rows of the bitmap seen excluded; no dynamic shared memory.  A copy of
+// k_rec_rank's counting loop rather than a body shared with it: sharing changes k_rec_rank's register allocation.
+template <class K>
+__global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K::T* __restrict__ z, int n, int row0, const unsigned* __restrict__ seen,
+                                                                const typename K::T* __restrict__ ss, const int* __restrict__ sr,
+                                                                const int* __restrict__ nvalid, unsigned long long* __restrict__ bins) {
+    using T = typename K::T;
+    __shared__ T ks[kMaxK];
+    __shared__ int kr[kMaxK];
+    __shared__ int cb[kMaxK + 1];
+    const int v = *nvalid;
+    if (v == 0) return;
+    const int r0 = blockIdx.x * kRankRows, r1 = min(n, r0 + kRankRows);
+    for (int i = threadIdx.x; i < v; i += kRankThreads) { ks[i] = ss[i]; kr[i] = sr[i]; }
+    for (int i = threadIdx.x; i <= v; i += kRankThreads) cb[i] = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    for (int base = r0; base < r1; base += kRankThreads) {    // uniform per warp: every lane reaches the match
+        const int b = base + threadIdx.x;
+        int q = v;                                            // bin v: comes before no target
+        if (b < r1) {
+            const T s = __ldg(z + b);
+            const int row = row0 + b;
+            if (K::qualifies(s) && !rec_seen(seen, row)) {
                 int lo = 0, hi = v;                           // the first target this item comes before
                 while (lo < hi) {
                     const int mid = (lo + hi) >> 1;

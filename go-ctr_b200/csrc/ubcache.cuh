@@ -43,6 +43,30 @@ k_ub_window(const long long* __restrict__ off, const long long* __restrict__ ts,
     }
 }
 
+// The seen set of CTR_EXCLUDE_SEEN as a bitmap over rows [0, n_items) (rec.cuh, rec_seen): the item rows of user u's
+// events with ts <= max_ts (max_ts == 0: every event; cache.go:71-94) and the window rows hist[0, S).  The events are one
+// run [first, end) of the time-descending sequence; every block finds `first` with its first warp, then the grid
+// strides over the run and the window.  Rows outside [0, n_items) are skipped; an unknown user, or no cache (off ==
+// nullptr), adds no event.  seen is zeroed by the caller.
+__global__ void __launch_bounds__(256)
+k_ub_seen(const long long* __restrict__ off, const long long* __restrict__ ts, const int* __restrict__ items, long n_users, int u,
+          long long max_ts, const int* __restrict__ hist, int S, long n_items, unsigned* __restrict__ seen) {
+    __shared__ long long first_s;
+    long long beg = 0, end = 0;
+    if (off && u >= 0 && u < n_users) { beg = off[u]; end = off[u + 1]; }
+    if (threadIdx.x < 32) {
+        long long first = beg;
+        if (end > beg && max_ts != 0) first = ub_first_leq(ts, beg, end, max_ts, threadIdx.x);   // uniform across the warp
+        if (threadIdx.x == 0) first_s = first;
+    }
+    __syncthreads();
+    const long long first = first_s, ne = end - first;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < ne + S; i += (long long)gridDim.x * blockDim.x) {
+        const int r = i < ne ? items[first + i] : hist[i - ne];
+        if (r >= 0 && r < n_items) atomicOr(seen + (r >> 5), 1u << (r & 31));
+    }
+}
+
 // ---- updates: ctr_ubcache_append / ctr_ubcache_set rewrite the CSR into a spare buffer --------------------------
 // A call touches T users (ascending rows tuser[k]).  Touched user k's stored segment is [ob[k], oe[k]) and its new
 // events are [bb[k], bb[k] + bcnt[k]) of the batch arrays (bts, bit; time-descending within the segment).  dcum[k] is

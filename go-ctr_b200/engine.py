@@ -11,7 +11,8 @@ from . import build as _build
 
 __all__ = ["Engine", "Config", "MLPClassifier", "MLPRegressor", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
-           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE", "rank_metrics"]
+           "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE", "rank_metrics",
+           "EXCLUDE_NONE", "EXCLUDE_WINDOW", "EXCLUDE_SEEN"]
 
 MODEL_YOUTUBE, MODEL_DIN_COS, MODEL_DIN_EUC = 0, 1, 2
 TABLE_USER_FEAT, TABLE_ITEM_FEAT, TABLE_ITEM_EMB = 0, 1, 2
@@ -19,6 +20,7 @@ TABLE_FROZEN, TABLE_SGD, TABLE_SGD_DETERMINISTIC, TABLE_ADAM = 0, 1, 2, 3
 GEMM_AUTO, GEMM_FP32, GEMM_TCGEN05_3XTF32 = 0, 1, 2
 IDMAP_USER, IDMAP_ITEM = 0, 1
 EINVAL, ESTATE, ENOTFOUND = 1, 5, 7
+EXCLUDE_NONE, EXCLUDE_WINDOW, EXCLUDE_SEEN = 0, 1, 2
 
 # every symbol include/ctr_b200.h declares (tests check the .so exports all of them)
 EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy", "ctr_last_error",
@@ -28,11 +30,24 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
-           "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
+           "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
            "ctr_mlp_score", "ctr_mlp_get_output", "ctr_mlp_set_output"]
+
+
+def _exclusion(n, max_ts, exclude_history, exclude_seen):
+    """(mode, cuts [n] int64 or None) of the _ex calls: exclude_seen implies exclude_history; max_ts (a scalar or [n];
+    None: 0, every event) is only read under exclude_seen."""
+    if not exclude_seen:
+        return (EXCLUDE_WINDOW if exclude_history else EXCLUDE_NONE), None
+    t = np.asarray(0 if max_ts is None else max_ts, np.int64)
+    if t.ndim == 0:
+        t = np.full(n, t, np.int64)
+    if t.shape != (n,):
+        raise ValueError("max_ts holds %d cuts for %d keys" % (t.size, n))
+    return EXCLUDE_SEEN, np.ascontiguousarray(t)
 
 
 class CtrError(RuntimeError):
@@ -480,21 +495,24 @@ class Engine:
                                        out_s.ctypes.data_as(C.POINTER(C.c_double)), cnt.ctypes.data_as(_ip)))
         return out_r, out_s, cnt
 
-    def recommend_topk(self, user_rows, hist, k, exclude_history=True):
-        """Top-k recommendation over every ITEM_EMB row (ctr_recommend_topk): user_rows [nu], hist [nu, S] (-1 padded).
+    def recommend_topk(self, user_rows, hist, k, exclude_history=True, max_ts=None, exclude_seen=False):
+        """Top-k recommendation over every ITEM_EMB row (ctr_recommend_topk_ex): user_rows [nu], hist [nu, S] (-1 padded).
         Returns (rows [nu, k] int32, scores [nu, k] float32, logits [nu, k] float32, counts [nu] int32), best first
         (logit descending, then row ascending); positions past a user's count hold row -1, score 0 and logit 0.
+        exclude_seen (implies exclude_history) also drops every item of the user's ubcache events with ts <= max_ts
+        (a scalar or [nu]; None or 0: every event); it is refused (ESTATE) on a row-sharded ITEM_EMB.
         On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search."""
         u, up = _i(np.atleast_1d(user_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
+        mode, t = _exclusion(u.size, max_ts, exclude_history, exclude_seen)
         out_r = np.empty((u.size, k), np.int32); out_s = np.empty((u.size, k), np.float32)
         out_l = np.empty((u.size, k), np.float32); cnt = np.empty(u.size, np.int32)
-        self._ck(self.L.ctr_recommend_topk(self.h, up, hp, C.c_int64(u.size), C.c_int32(k), C.c_int32(int(bool(exclude_history))),
-                                           out_r.ctypes.data_as(_ip), out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(_fp),
-                                           cnt.ctypes.data_as(_ip)))
+        self._ck(self.L.ctr_recommend_topk_ex(self.h, up, hp, None if t is None else t.ctypes.data_as(_lp), C.c_int64(u.size), C.c_int32(k),
+                                              C.c_int32(mode), out_r.ctypes.data_as(_ip), out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(_fp),
+                                              cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
 
-    def rank_items(self, user_rows, hist, item_rows, exclude_history=True):
+    def rank_items(self, user_rows, hist, item_rows, exclude_history=True, max_ts=None, exclude_seen=False):
         """Full-catalogue rank of held-out items (ctr_rank_items): key i is (user_rows[i], hist[i] [S], item_rows[i]).
         Returns (ranks [n] int64, logits [n] float32): rank r means recommend_topk(user, hist, k) lists the item at
         position r - 1 for every k >= r; -1 when it can never be listed (outside the table, in an excluded history, or a
@@ -502,15 +520,17 @@ class Engine:
         On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search: every rank calls it with
         the same user, history and item rows and receives the same ranks and logits, bit-identical to one GPU holding the
         whole table; rows that differ between the ranks raise CTR_EINVAL on every rank.  No sync is needed after
-        training."""
+        training.  exclude_seen and max_ts (a scalar or [n], key i's cut) as for recommend_topk: a target the user has
+        seen by the cut ranks -1."""
         u, up = _i(np.atleast_1d(user_rows))
         it, ip = _i(np.atleast_1d(item_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
         if it.size != u.size:
             raise ValueError("user_rows and item_rows differ in length: %d, %d" % (u.size, it.size))
+        mode, t = _exclusion(u.size, max_ts, exclude_history, exclude_seen)
         ranks = np.empty(u.size, np.int64); logits = np.empty(u.size, np.float32)
-        self._ck(self.L.ctr_rank_items(self.h, up, hp, ip, C.c_int64(u.size), C.c_int32(int(bool(exclude_history))),
-                                       ranks.ctypes.data_as(_lp), logits.ctypes.data_as(_fp)))
+        self._ck(self.L.ctr_rank_items_ex(self.h, up, hp, None if t is None else t.ctypes.data_as(_lp), ip, C.c_int64(u.size), C.c_int32(mode),
+                                          ranks.ctypes.data_as(_lp), logits.ctypes.data_as(_fp)))
         return ranks, logits
 
 
@@ -638,33 +658,37 @@ class _Mlp64:
                                              C.c_int64(u.size), out.ctypes.data_as(_fp)))
         return out
 
-    def recommend_topk(self, engine, user_ids, ts, k, exclude_history=True):
+    def recommend_topk(self, engine, user_ids, ts, k, exclude_history=True, exclude_seen=False):
         """Top-k recommendation over every ITEM_EMB row of the feature store `engine` (ctr_mlp_recommend_topk): users
         are external ids, each windowed at its ts (empty history without a ubcache).  Returns (rows [nu, k] int32, scores
         [nu, k] float32, logits [nu, k] float64, counts [nu] int32), best first (logit descending, then row ascending);
         positions past a user's count hold row -1, score 0 and logit 0.  Each score is bit for bit what predict_keys
-        returns for (user, the row's item id, ts).  An unknown user raises CtrError with code ENOTFOUND."""
+        returns for (user, the row's item id, ts).  An unknown user raises CtrError with code ENOTFOUND.  exclude_seen
+        (implies exclude_history) also drops every item of the user's ubcache events with ts <= the user's ts (0: every
+        event)."""
         u = np.atleast_1d(np.ascontiguousarray(user_ids, np.int64)); t = np.atleast_1d(np.ascontiguousarray(ts, np.int64))
         if u.size != t.size:
             raise ValueError("user_ids and ts differ in length: %d, %d" % (u.size, t.size))
         out_r = np.empty((u.size, k), np.int32); out_s = np.empty((u.size, k), np.float32)
         out_l = np.empty((u.size, k), np.float64); cnt = np.empty(u.size, np.int32)
-        self._ck(self.L.ctr_mlp_recommend_topk(self.h, engine.h, u.ctypes.data_as(_lp), t.ctypes.data_as(_lp), C.c_int64(u.size),
-                                               C.c_int32(k), C.c_int32(int(bool(exclude_history))), out_r.ctypes.data_as(_ip),
-                                               out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(C.POINTER(C.c_double)),
-                                               cnt.ctypes.data_as(_ip)))
+        mode = _exclusion(u.size, None, exclude_history, exclude_seen)[0]
+        self._ck(self.L.ctr_mlp_recommend_topk_ex(self.h, engine.h, u.ctypes.data_as(_lp), t.ctypes.data_as(_lp), C.c_int64(u.size),
+                                                  C.c_int32(k), C.c_int32(mode), out_r.ctypes.data_as(_ip),
+                                                  out_s.ctypes.data_as(_fp), out_l.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  cnt.ctypes.data_as(_ip)))
         return out_r, out_s, out_l, cnt
 
-    def rank_items(self, engine, user_ids, item_ids, ts, exclude_history=True):
+    def rank_items(self, engine, user_ids, item_ids, ts, exclude_history=True, exclude_seen=False):
         """Full-catalogue rank of held-out items over the feature store `engine` (ctr_mlp_rank_items): key i is (user,
         item, ts) in external ids, windowed at ts as recommend_topk windows it.  Returns (ranks [n] int64, logits [n]
         float64) under Engine.rank_items' rules; an unknown item id ranks -1 (logit NaN), an unknown user raises CtrError
-        with code ENOTFOUND."""
+        with code ENOTFOUND.  exclude_seen as for recommend_topk, each key cut at its ts."""
         u, i, t = self._keys(np.atleast_1d(user_ids), np.atleast_1d(item_ids), np.atleast_1d(ts))
+        mode = _exclusion(u.size, None, exclude_history, exclude_seen)[0]
         ranks = np.empty(u.size, np.int64); logits = np.empty(u.size, np.float64)
-        self._ck(self.L.ctr_mlp_rank_items(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
-                                           C.c_int64(u.size), C.c_int32(int(bool(exclude_history))), ranks.ctypes.data_as(_lp),
-                                           logits.ctypes.data_as(C.POINTER(C.c_double))))
+        self._ck(self.L.ctr_mlp_rank_items_ex(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
+                                              C.c_int64(u.size), C.c_int32(mode), ranks.ctypes.data_as(_lp),
+                                              logits.ctypes.data_as(C.POINTER(C.c_double))))
         return ranks, logits
 
     def get_params(self):

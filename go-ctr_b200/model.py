@@ -236,14 +236,16 @@ class SimpleMlpPredWrap:
         self._bound()
         return self.pred.predict_keys(self.engine, user_ids, item_ids, ts)
 
-    def recommend(self, userId, k, now=None, exclude_history=True):
+    def recommend(self, userId, k, now=None, exclude_history=True, exclude_seen=False):
         """The k best items of the bound feature store's whole ITEM_EMB table for one user at `now` (default: the
         current time), scored by this MLP on the device (ctr_mlp_recommend_topk).  Returns (rows [n] int32, scores [n]
         float32, logits [n] float64), best first, n <= k; serving.Recommend maps the rows to item ids.  A classifier
-        with classes has no click probability to rank by: CtrError with code ESTATE."""
+        with classes has no click probability to rank by: CtrError with code ESTATE.  exclude_seen drops every item the
+        user's ubcache events up to `now` hold, the window's included."""
         self._bound()
         ts = int(time.time()) if now is None else int(now)
-        rows, scores, logits, cnt = self.pred.recommend_topk(self.engine, [int(userId)], [ts], k, exclude_history=exclude_history)
+        rows, scores, logits, cnt = self.pred.recommend_topk(self.engine, [int(userId)], [ts], k, exclude_history=exclude_history,
+                                                             exclude_seen=exclude_seen)
         n = int(cnt[0])
         return rows[0, :n], scores[0, :n], logits[0, :n]
 

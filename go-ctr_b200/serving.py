@@ -45,11 +45,13 @@ def Rank(recSys, userId, itemIds, now=None):
     return [ItemScore(int(it), float(y[k, 0])) for k, it in enumerate(itemIds)]
 
 
-def Recommend(recSys, userId, k, now=None, exclude_history=True):
+def Recommend(recSys, userId, k, now=None, exclude_history=True, exclude_seen=False):
     """What recommend/api.go's empty-itemIdList branch would return (api.go:115-118, "todo: some default recall
     algorithm"): the k best items of the whole table for one user at the current time, best first, as [ItemScore].
     Every ITEM_EMB row is scored with the trained model (ctr_recommend_topk); the user's history is windowed from the
-    device ubcache at `now` (empty without one, as in BatchPredict); exclude_history drops the items of that window.
+    device ubcache at `now` (empty without one, as in BatchPredict); exclude_history drops the items of that window, and
+    exclude_seen (implies exclude_history) every item of the user's ubcache events up to `now`: nothing the user has
+    already consumed is recommended.  exclude_seen is refused (ESTATE) on a row-sharded ITEM_EMB.
     An unknown user raises CtrError with code ENOTFOUND, as BatchPredict does for an unresolvable first key.
     On an engine whose ITEM_EMB is row-sharded over several GPUs the call is collective: every rank's process makes
     the same call (same user, k, now and history) and receives the same complete result (Engine.recommend_topk).
@@ -60,7 +62,7 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
     fitted on labels other than 0 / 1 predicts labels, not click probabilities, and raises CtrError with code ESTATE."""
     ts = int(time.time()) if now is None else int(now)
     if isinstance(recSys, _m.SimpleMlpPredWrap):
-        rows, scores, _ = recSys.recommend(userId, k, now=ts, exclude_history=exclude_history)
+        rows, scores, _ = recSys.recommend(userId, k, now=ts, exclude_history=exclude_history, exclude_seen=exclude_seen)
         item_ids = recSys.engine.item_ids
         return [ItemScore(int(item_ids[r]), float(s)) for r, s in zip(rows, scores)]
     row = int(recSys.idmap_lookup(_e.IDMAP_USER, [int(userId)])[0])
@@ -72,12 +74,12 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True):
         if err.code != _e.ESTATE:
             raise
         hist = np.full((1, recSys.cfg.S), -1, np.int32)
-    rows, scores, _, cnt = recSys.recommend_topk([row], hist, k, exclude_history=exclude_history)
+    rows, scores, _, cnt = recSys.recommend_topk([row], hist, k, exclude_history=exclude_history, max_ts=ts, exclude_seen=exclude_seen)
     item_ids = recSys.item_ids
     return [ItemScore(int(item_ids[rows[0, i]]), float(scores[0, i])) for i in range(int(cnt[0]))]
 
 
-def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
+def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True, exclude_seen=False):
     """Offline full-catalogue evaluation of Recommend: each held-out Sample's ItemId is ranked against every ITEM_EMB row
     for its UserId, with the history windowed at its Timestamp (the window cut), exactly as Recommend(userId, k,
     now=Timestamp, exclude_history) would list it (Engine.rank_items / _Mlp64.rank_items).  Samples are grouped by
@@ -86,7 +88,10 @@ def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
     recSys is an Engine or a SimpleMlpPredWrap, as for Recommend.  An unknown user raises CtrError with code ENOTFOUND.
     On an Engine with a row-sharded ITEM_EMB, Evaluate is collective (Engine.rank_items): every rank passes the same
     held-out samples and returns the same metrics.  The ranks' windows and item rows must agree too, so every rank needs
-    the same id maps and behaviour cache; a rank whose rows differ makes the call raise CtrError EINVAL on every rank."""
+    the same id maps and behaviour cache; a rank whose rows differ makes the call raise CtrError EINVAL on every rank.
+    exclude_seen (implies exclude_history) is the filtered protocol: every item of the user's ubcache events with ts <=
+    the sample's Timestamp is removed from the catalogue it is ranked against (and ranks -1 itself), so no event after
+    the cut is excluded.  It is refused (ESTATE) on a row-sharded ITEM_EMB."""
     if len(heldOut) == 0:
         raise ValueError("no held-out samples")
     u = np.fromiter((s.UserId for s in heldOut), np.int64, len(heldOut))
@@ -94,7 +99,7 @@ def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
     t = np.fromiter((s.Timestamp for s in heldOut), np.int64, len(heldOut))
     if isinstance(recSys, _m.SimpleMlpPredWrap):
         recSys._bound()
-        ranks, _ = recSys.pred.rank_items(recSys.engine, u, i, t, exclude_history=exclude_history)
+        ranks, _ = recSys.pred.rank_items(recSys.engine, u, i, t, exclude_history=exclude_history, exclude_seen=exclude_seen)
     else:
         rows = recSys.idmap_lookup(_e.IDMAP_USER, u)
         if (rows < 0).any():
@@ -106,7 +111,7 @@ def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True):
                 raise
             hist = np.full((u.size, recSys.cfg.S), -1, np.int32)
         items = recSys.idmap_lookup(_e.IDMAP_ITEM, i)
-        ranks, _ = recSys.rank_items(rows, hist, items, exclude_history=exclude_history)
+        ranks, _ = recSys.rank_items(rows, hist, items, exclude_history=exclude_history, max_ts=t, exclude_seen=exclude_seen)
     _, groups = np.unique(np.stack([u, t], axis=1), axis=0, return_inverse=True)
     ks = [int(k) for k in ks]
     hit, recall, ndcg, mrr = _e.rank_metrics(ranks, groups.ravel(), ks)

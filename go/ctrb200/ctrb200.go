@@ -309,19 +309,38 @@ func (e *Engine) Search(queries []float64, rows []int32, k int) (outRows []int32
 // score 0 and logit 0.
 // With a row-sharded ITEM_EMB (world > 1, large table) Recommend is collective, under the same rule as Search.
 func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory bool) (outRows []int32, scores, logits []float32, counts []int32, err error) {
+	return e.recommend(userRows, histRows, nil, k, windowMode(excludeHistory))
+}
+
+// RecommendSeen is Recommend that never lists an item the user has already seen: besides the valid history rows, the
+// item of every event of the user's device behaviour cache with timestamp <= maxTs[j] (0: every event) is excluded.
+// maxTs has one cut per user. Refused (CTR_ESTATE) on a row-sharded ITEM_EMB.
+func (e *Engine) RecommendSeen(userRows, histRows []int32, maxTs []int64, k int) (outRows []int32, scores, logits []float32, counts []int32, err error) {
+	if len(maxTs) != len(userRows) {
+		return nil, nil, nil, nil, fmt.Errorf("ctrb200: RecommendSeen needs one maxTs per user")
+	}
+	return e.recommend(userRows, histRows, maxTs, k, C.CTR_EXCLUDE_SEEN)
+}
+
+// windowMode is the exclusion mode of an excludeHistory flag
+func windowMode(excludeHistory bool) C.int32_t {
+	if excludeHistory {
+		return C.CTR_EXCLUDE_WINDOW
+	}
+	return C.CTR_EXCLUDE_NONE
+}
+
+func (e *Engine) recommend(userRows, histRows []int32, maxTs []int64, k int, mode C.int32_t) (outRows []int32, scores, logits []float32, counts []int32, err error) {
 	nu := len(userRows)
 	if nu == 0 || k < 1 || len(histRows) != nu*int(e.cfg.S) {
 		return nil, nil, nil, nil, fmt.Errorf("ctrb200: Recommend needs at least one user, k >= 1 and S history rows per user")
-	}
-	ex := C.int32_t(0)
-	if excludeHistory {
-		ex = 1
 	}
 	outRows = make([]int32, nu*k)
 	scores = make([]float32, nu*k)
 	logits = make([]float32, nu*k)
 	counts = make([]int32, nu)
-	rc := C.ctr_recommend_topk(e.h, i32(userRows), i32(histRows), C.int64_t(nu), C.int32_t(k), ex, i32(outRows), f32(scores), f32(logits), i32(counts))
+	rc := C.ctr_recommend_topk_ex(e.h, i32(userRows), i32(histRows), i64n(maxTs), C.int64_t(nu), C.int32_t(k), mode, i32(outRows), f32(scores),
+		f32(logits), i32(counts))
 	if err = e.err(rc); err != nil {
 		return nil, nil, nil, nil, err
 	}
@@ -334,17 +353,27 @@ func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory boo
 // 1024, Recommend(k) lists the item exactly when 0 < rank <= k, at position rank-1, with logits[i] as its logit.
 // With a row-sharded ITEM_EMB (world > 1, large table) RankItems is collective, under the same rule as Search.
 func (e *Engine) RankItems(userRows, histRows, itemRows []int32, excludeHistory bool) (ranks []int64, logits []float32, err error) {
+	return e.rankItems(userRows, histRows, nil, itemRows, windowMode(excludeHistory))
+}
+
+// RankItemsSeen ranks as RecommendSeen lists: key i's seen set (its history rows and the items of the user's cached
+// events with timestamp <= maxTs[i]) is removed from the catalogue, and a target in it ranks -1. This is the filtered
+// full-ranking protocol; with maxTs[i] the held-out event's time, no later event is excluded.
+func (e *Engine) RankItemsSeen(userRows, histRows []int32, maxTs []int64, itemRows []int32) (ranks []int64, logits []float32, err error) {
+	if len(maxTs) != len(userRows) {
+		return nil, nil, fmt.Errorf("ctrb200: RankItemsSeen needs one maxTs per key")
+	}
+	return e.rankItems(userRows, histRows, maxTs, itemRows, C.CTR_EXCLUDE_SEEN)
+}
+
+func (e *Engine) rankItems(userRows, histRows []int32, maxTs []int64, itemRows []int32, mode C.int32_t) (ranks []int64, logits []float32, err error) {
 	n := len(userRows)
 	if n == 0 || len(itemRows) != n || len(histRows) != n*int(e.cfg.S) {
 		return nil, nil, fmt.Errorf("ctrb200: RankItems needs at least one key, one item and S history rows per key")
 	}
-	ex := C.int32_t(0)
-	if excludeHistory {
-		ex = 1
-	}
 	ranks = make([]int64, n)
 	logits = make([]float32, n)
-	if err = e.err(C.ctr_rank_items(e.h, i32(userRows), i32(histRows), i32(itemRows), C.int64_t(n), ex, i64(ranks), f32(logits))); err != nil {
+	if err = e.err(C.ctr_rank_items_ex(e.h, i32(userRows), i32(histRows), i64n(maxTs), i32(itemRows), C.int64_t(n), mode, i64(ranks), f32(logits))); err != nil {
 		return nil, nil, err
 	}
 	return ranks, logits, nil
@@ -799,6 +828,16 @@ func (p *MlpPredWrap) Rank(e *Engine, userId int, itemIds []int) ([]rcmd.ItemSco
 // and so is a classifier fitted on labels other than 0 / 1: it predicts labels, so it has no click probability to
 // rank items by (CTR_ESTATE, with nothing written).
 func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, excludeHistory bool) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
+	return p.recommend(e, userIds, ts, k, windowMode(excludeHistory))
+}
+
+// RecommendSeen is Recommend that never lists an item the user has already seen: every item of the user's cached events
+// with timestamp <= ts[j] (0: every event), the window's included.
+func (p *MlpPredWrap) RecommendSeen(e *Engine, userIds []int, ts []int64, k int) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
+	return p.recommend(e, userIds, ts, k, C.CTR_EXCLUDE_SEEN)
+}
+
+func (p *MlpPredWrap) recommend(e *Engine, userIds []int, ts []int64, k int, mode C.int32_t) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
 	nu := len(userIds)
 	if nu == 0 || k < 1 || len(ts) != nu {
 		return nil, nil, nil, nil, fmt.Errorf("MlpPredWrap.Recommend needs at least one user, one ts per user and k >= 1")
@@ -807,17 +846,13 @@ func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, exc
 	for i, id := range userIds {
 		u[i] = int64(id)
 	}
-	ex := C.int32_t(0)
-	if excludeHistory {
-		ex = 1
-	}
 	outRows = make([]int32, nu*k)
 	scores = make([]float32, nu*k)
 	logits = make([]float64, nu*k)
 	counts = make([]int32, nu)
-	if rc := C.ctr_mlp_recommend_topk(p.m, e.h, i64(u), i64(ts), C.int64_t(nu), C.int32_t(k), ex, i32(outRows), f32(scores),
+	if rc := C.ctr_mlp_recommend_topk_ex(p.m, e.h, i64(u), i64(ts), C.int64_t(nu), C.int32_t(k), mode, i32(outRows), f32(scores),
 		(*C.double)(unsafe.Pointer(&logits[0])), i32(counts)); rc != C.CTR_OK {
-		return nil, nil, nil, nil, fmt.Errorf("ctr_mlp_recommend_topk: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+		return nil, nil, nil, nil, fmt.Errorf("ctr_mlp_recommend_topk_ex: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
 	}
 	return outRows, scores, logits, counts, nil
 }
@@ -827,6 +862,16 @@ func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, exc
 // (userIds[i], ts[i]), or -1 when it can never be listed (an unknown item id, an excluded window row, a NaN logit).
 // logits[i] is the list's float64 logit for the item. An unknown user is an error.
 func (p *MlpPredWrap) RankItems(e *Engine, userIds, itemIds []int, ts []int64, excludeHistory bool) (ranks []int64, logits []float64, err error) {
+	return p.rankItems(e, userIds, itemIds, ts, windowMode(excludeHistory))
+}
+
+// RankItemsSeen ranks as RecommendSeen lists: every item of the user's cached events with timestamp <= ts[i] is removed
+// from the catalogue, and a target among them ranks -1.
+func (p *MlpPredWrap) RankItemsSeen(e *Engine, userIds, itemIds []int, ts []int64) (ranks []int64, logits []float64, err error) {
+	return p.rankItems(e, userIds, itemIds, ts, C.CTR_EXCLUDE_SEEN)
+}
+
+func (p *MlpPredWrap) rankItems(e *Engine, userIds, itemIds []int, ts []int64, mode C.int32_t) (ranks []int64, logits []float64, err error) {
 	n := len(userIds)
 	if n == 0 || len(itemIds) != n || len(ts) != n {
 		return nil, nil, fmt.Errorf("MlpPredWrap.RankItems needs at least one key and one item and ts per key")
@@ -835,15 +880,11 @@ func (p *MlpPredWrap) RankItems(e *Engine, userIds, itemIds []int, ts []int64, e
 	for i := range userIds {
 		u[i], it[i] = int64(userIds[i]), int64(itemIds[i])
 	}
-	ex := C.int32_t(0)
-	if excludeHistory {
-		ex = 1
-	}
 	ranks = make([]int64, n)
 	logits = make([]float64, n)
-	if rc := C.ctr_mlp_rank_items(p.m, e.h, i64(u), i64(it), i64(ts), C.int64_t(n), ex, i64(ranks),
+	if rc := C.ctr_mlp_rank_items_ex(p.m, e.h, i64(u), i64(it), i64(ts), C.int64_t(n), mode, i64(ranks),
 		(*C.double)(unsafe.Pointer(&logits[0]))); rc != C.CTR_OK {
-		return nil, nil, fmt.Errorf("ctr_mlp_rank_items: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+		return nil, nil, fmt.Errorf("ctr_mlp_rank_items_ex: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
 	}
 	return ranks, logits, nil
 }

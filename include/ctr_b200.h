@@ -358,6 +358,25 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
 int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, int64_t nu, int32_t k,
                        int32_t exclude_history, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count);
 
+/* Exclusion modes of the _ex recommendation and rank calls:
+ *   CTR_EXCLUDE_NONE    nothing but NaN logits (exclude_history = 0 of the plain calls)
+ *   CTR_EXCLUDE_WINDOW  the valid rows of the key's history window (exclude_history != 0)
+ *   CTR_EXCLUDE_SEEN    everything the user has seen up to the cut: the window's valid rows and the item row of every
+ *                       event of the user's device-ubcache sequence with ts <= max_ts (max_ts == 0: every event, as
+ *                       TimeSeq.Filter, cache.go:71-94).  No ubcache, or a user row outside the cache, adds no event;
+ *                       item rows of -1, rows past the table and repeated rows are harmless.  A superset of WINDOW, and
+ *                       an evaluation cut at a held-out event's time never excludes the events after it. */
+enum { CTR_EXCLUDE_NONE = 0, CTR_EXCLUDE_WINDOW = 1, CTR_EXCLUDE_SEEN = 2 };
+
+/* ctr_recommend_topk with an exclusion mode: ctr_recommend_topk(..., exclude_history, ...) ==
+ * ctr_recommend_topk_ex(..., NULL, ..., exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, ...).  max_ts [nu] is
+ * user j's cut under CTR_EXCLUDE_SEEN and may be NULL otherwise.  Refusals write nothing: CTR_EINVAL for an exclude
+ * outside the enum or SEEN with a NULL max_ts, besides ctr_recommend_topk's; CTR_ESTATE for SEEN on a row-sharded
+ * ITEM_EMB (world > 1, sharded placement; a replicated ITEM_EMB is served locally).  The seen set is built on the
+ * device per user (a bitmap over the ITEM_EMB rows, ⌈I / 32⌉ words of the handle's scratch): no length cap. */
+int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, int64_t nu, int32_t k,
+                          int32_t exclude, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count);
+
 /* Full-catalogue rank of held-out items (the offline protocol of item recommendation): for each of n keys (user_rows[i],
  * hist_rows[i] [n, S], item_rows[i]) every ITEM_EMB row is scored exactly as ctr_recommend_topk scores it for
  * (user_rows[i], hist_rows[i]) — the same kernels, chunks and logits — and the target item is ranked in that list's order
@@ -385,6 +404,14 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
  *   Runs on the engine stream under the handle's mutex, so it sees every update queued before it. */
 int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int32_t* item_rows, int64_t n,
                    int32_t exclude_history, int64_t* out_rank, float* out_logit);
+
+/* ctr_rank_items with an exclusion mode (CTR_EXCLUDE_*), as ctr_recommend_topk_ex extends ctr_recommend_topk: max_ts [n]
+ * is key i's cut under CTR_EXCLUDE_SEEN (may be NULL otherwise), a target in the key's seen set ranks -1, and for every
+ * k in [1, 1024], 0 < rank <= k exactly when ctr_recommend_topk_ex(user, hist, max_ts, k, exclude) lists the target at
+ * position rank - 1.  Under SEEN keys share a pass only with the same user row, history and max_ts.  Refusals as
+ * ctr_recommend_topk_ex's, besides ctr_rank_items'. */
+int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, const int32_t* item_rows, int64_t n,
+                      int32_t exclude, int64_t* out_rank, float* out_logit);
 
 /* Ranking metrics of ranks from ctr_rank_items / ctr_mlp_rank_items (host only, no device).  group[i] names key i's
  * group (normally the user, or the user and the window cut); m_g keys in group g; hit(k) = 0 < rank <= k.
@@ -622,6 +649,14 @@ int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, 
  *   Locking: h's mutex, then m's; everything runs on h's stream. */
 int  ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
                         int32_t exclude_history, int64_t* out_rank, double* out_logit);
+/* The classifier's recommendation and rank with an exclusion mode (CTR_EXCLUDE_*): the plain calls are these with
+ * exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE.  Under CTR_EXCLUDE_SEEN each key's ts is also its cut: every
+ * item of the user's ubcache events with ts <= the key's ts (0: every event) is excluded, the window included.
+ * CTR_EINVAL (nothing written) for an exclude outside the enum, besides the plain calls' refusals. */
+int  ctr_mlp_recommend_topk_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k,
+                               int32_t exclude, int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count);
+int  ctr_mlp_rank_items_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+                           int32_t exclude, int64_t* out_rank, double* out_logit);
 /* packed parameter vector; ctr_mlp_get_params(m, NULL, 0, &np) returns the current length (it follows the classes) */
 int  ctr_mlp_get_params(ctr_mlp* m, double* params, int64_t cap, int64_t* np);
 int  ctr_mlp_set_params(ctr_mlp* m, const double* params, int64_t np);
