@@ -267,10 +267,11 @@ static int comm_max_i64(ctr_handle* h, int64_t* v) {
     return CTR_OK;
 }
 
-// 64-bit hash of a caller array (FNV-1a over 8-byte words), for comparing the ranks' arguments of a collective call
-static uint64_t comm_hash(const void* p, size_t bytes) {
+// 64-bit hash of a caller array (FNV-1a over 8-byte words), for comparing the ranks' arguments of a collective call;
+// seed = the hash of an earlier array chains the two into one header slot
+static uint64_t comm_hash(const void* p, size_t bytes, uint64_t seed = 1469598103934665603ull) {
     const unsigned char* b = (const unsigned char*)p;
-    uint64_t hs = 1469598103934665603ull;
+    uint64_t hs = seed;
     for (size_t i = 0; i < bytes; i += 8) {
         uint64_t w = 0;
         memcpy(&w, b + i, std::min<size_t>(8, bytes - i));

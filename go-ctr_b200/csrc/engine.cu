@@ -1247,15 +1247,18 @@ bool exclude_ok(int32_t exclude, const int64_t* max_ts) {
     return exclude >= CTR_EXCLUDE_NONE && exclude <= CTR_EXCLUDE_SEEN && (exclude != CTR_EXCLUDE_SEEN || max_ts);
 }
 
-// CTR_EXCLUDE_SEEN: the seen bitmap of one pass (k_ub_seen) over the global rows [0, I), for user row u, cut max_ts
-// and the window uh [S] on the device; profile key `key`
-int rec_build_seen(ctr_handle* h, const char* key, unsigned* seen, int64_t I, int u, long long max_ts, const int* uh) {
+// CTR_EXCLUDE_SEEN: the seen bitmap of one pass (k_ub_seen) over this rank's N local rows of the I global rows (local
+// row l = global row l·world + rank), for user row u, cut max_ts and the window uh [S] on the device, from this rank's
+// behaviour cache; profile key `key`
+int rec_build_seen(ctr_handle* h, const char* key, unsigned* seen, int64_t I, int64_t N, int world, int rank, int u, long long max_ts,
+                   const int* uh) {
     const int S = h->cfg.S;
     const int64_t ne = h->ub_off ? h->ub_n : 0;                         // an upper bound on the user's events
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((ne + S + 255) / 256, (int64_t)h->num_sms * 4));
-    CU(h, cudaMemsetAsync(seen, 0, (size_t)(I + 31) / 32 * sizeof(unsigned), h->stream));
+    CU(h, cudaMemsetAsync(seen, 0, (size_t)(N + 31) / 32 * sizeof(unsigned), h->stream));
     return launch(h, key, [&] {
-        k_ub_seen<<<grid, 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->ub_off ? (long)h->ub_users : 0L, u, max_ts, uh, S, (long)I, seen);
+        k_ub_seen<<<grid, 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->ub_off ? (long)h->ub_users : 0L, u, max_ts, uh, S, (long)I,
+                                               world, rank, seen);
     });
 }
 
@@ -1268,7 +1271,8 @@ struct RecTopk {
     ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge, <pre>_finish and <pre>_seen
     int k, nex, world, rank;                // nex exclusion rows per user; local row l is global row l·world + rank
     int64_t N; int Bc;                      // the items scored, per chunk
-    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (world = 1, nex = 0): each user's seen bitmap excludes
+    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (nex = 0): each user's seen bitmap over the local rows excludes
+    int64_t I = N;                          // the global row count
     // selection slices of at least 4 steps and 8k rows: merging the slices' lists stays small against scanning them
     const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     const size_t ssmem = rec::scan_smem_bytes<K>(k, nex), msmem = knn::smem_bytes<K>(1, 0, k);
@@ -1281,7 +1285,10 @@ struct RecTopk {
     int setup(int slot, int64_t G, F&& own) {
         CU(h, cudaFuncSetAttribute(rec::k_rec_scan<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
         CU(h, cudaFuncSetAttribute(knn::k_knn_merge<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem));
-        if (by_seen) CU(h, cudaFuncSetAttribute(rec::k_rec_scan_seen<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+        if (by_seen) {      // the (world, rank) form of the overloaded name
+            void (*scan_seen)(const T*, int, int, int, int, int, const unsigned*, int, const T*, const int*, T*, int*) = rec::k_rec_scan_seen<K>;
+            CU(h, cudaFuncSetAttribute(scan_seen, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+        }
         const size_t sl = (size_t)(1 + (Bc + rps - 1) / rps) * k, gk = (size_t)G * k;
         auto carve = [&](char* base) {
             Carve c{base};
@@ -1302,7 +1309,7 @@ struct RecTopk {
     int user(int j, const int* excl, const T* z, F&& score, int u = -1, long long max_ts = 0) {
         const int nchunks = (int)((N + Bc - 1) / Bc);
         T* us = ls + (size_t)j * k; int* ur = lr + (size_t)j * k;
-        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, N, u, max_ts, excl));
+        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, I, N, world, rank, u, max_ts, excl));
         for (int c = 0; c < nchunks; c++) {
             const int i0 = c * Bc, nb = (int)std::min<int64_t>(Bc, N - i0);
             RET(score(i0, nb));
@@ -1310,7 +1317,7 @@ struct RecTopk {
             const bool first = c == 0, last = c == nchunks - 1;
             RET(launch(h, n_topk.c_str(), [&] {
                 if (by_seen)
-                    rec::k_rec_scan_seen<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, rps, seen, k, first ? nullptr : sl_s,
+                    rec::k_rec_scan_seen<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, world, rank, rps, seen, k, first ? nullptr : sl_s,
                                                                                         first ? nullptr : sl_r, sl_s + k, sl_r + k);
                 else
                     rec::k_rec_scan<K><<<slices, knn::kThreads, ssmem, h->stream>>>(z, nb, i0, world, rank, rps, excl, nex, k,
@@ -1347,7 +1354,8 @@ struct RecTopk {
 // m <= kMaxK targets of one (user, window): the chunks that hold a target are scored first and their targets' logits
 // copied out, then every chunk is scored and counted against the sorted targets.  On a row-sharded ITEM_EMB
 // (world > 1; collective) each rank scores its own shard: the targets' logits are all-gathered from their owners
-// before the sort, and the ranks' bins are summed before the ranks are read off.
+// before the sort, and the ranks' bins are summed before the ranks are read off.  Under CTR_EXCLUDE_SEEN each rank's
+// bitmap covers its own rows, and a target's seen flag comes from its owner in the same all-gather as its logit.
 template <class K>
 struct RecRank {
     using T = typename K::T;
@@ -1356,9 +1364,10 @@ struct RecRank {
     int64_t N; int Bc;                      // the items this rank scores (its local rows), per chunk
     int world = 1, rank = 0;                // local row l is global row l·world + rank
     int64_t I = N;                          // the global row count
-    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (world = 1, nex = 0): each pass's seen bitmap excludes
+    bool by_seen = false;                   // CTR_EXCLUDE_SEEN (nex = 0): each pass's seen bitmap over the local rows excludes
     const std::string n_target = std::string(pre) + "_target", n_count = std::string(pre) + "_count", n_seen = std::string(pre) + "_seen";
-    int *rows, *place, *nvalid, *sr; T *tl, *tlg, *ss, *ol; unsigned long long* bins; long long* orank; unsigned* seen = nullptr;
+    int *rows, *place, *nvalid, *sr; T *tl, *tlg, *ss, *ol; unsigned long long* bins; long long* orank;
+    unsigned* seen = nullptr; int *flag = nullptr, *flagg = nullptr;      // by_seen: the bitmap, the targets' flags [m], [world][m]
 
     // scratch slot `slot`: the caller's buffers (own(c)), then one pass's target state
     template <class F>
@@ -1371,7 +1380,11 @@ struct RecRank {
             rows = c.take<int>(M); place = c.take<int>(M); nvalid = c.take<int>(1); sr = c.take<int>(M);
             tl = c.take<T>(M); ss = c.take<T>(M); ol = c.take<T>(M); bins = c.take<unsigned long long>(M + 1); orank = c.take<long long>(M);
             tlg = world > 1 ? c.take<T>((size_t)world * M) : tl;      // [world][m] the ranks' target logits
-            if (by_seen) seen = c.take<unsigned>((size_t)(I + 31) / 32);
+            if (by_seen) {
+                seen = c.take<unsigned>((size_t)(N + 31) / 32);
+                flag = c.take<int>(M);
+                flagg = world > 1 ? c.take<int>((size_t)world * M) : flag;
+            }
             return c.used;
         };
         char* ws = nullptr;
@@ -1380,8 +1393,8 @@ struct RecRank {
         return CTR_OK;
     }
     // targets trow[0, m) of one (user, window), excluding excl[0, nex), or under by_seen the seen set of (user row u,
-    // cut max_ts, window excl [S]): score(i0, nb) queues the logits of items [i0, i0 + nb) into z.  Ranks and logits
-    // go to out_rank / out_logit[0, m) (host) in stream order.
+    // cut max_ts, window excl [S]) as each row's owner holds it: score(i0, nb) queues the logits of items [i0, i0 + nb)
+    // into z.  Ranks and logits go to out_rank / out_logit[0, m) (host) in stream order.
     template <class F>
     int pass(const int* trow, int m, const int* excl, const T* z, F&& score, int64_t* out_rank, T* out_logit, int u = -1, long long max_ts = 0) {
         std::vector<int64_t> chunks;                         // the local chunks that hold a target this rank owns, each once
@@ -1390,19 +1403,20 @@ struct RecRank {
         std::sort(chunks.begin(), chunks.end());
         chunks.erase(std::unique(chunks.begin(), chunks.end()), chunks.end());
         CU(h, cudaMemcpyAsync(rows, trow, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+        // the bitmap comes first: the owner's flags of its targets are written beside their logits
+        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, I, N, world, rank, u, max_ts, excl));
         for (const int64_t c : chunks) {
             const int i0 = (int)(c * Bc), nb = (int)std::min<int64_t>(Bc, N - i0);
             RET(score(i0, nb));
             RET(launch(h, n_target.c_str(), [&] {
-                rec::k_rec_target_logits<T><<<(m + 255) / 256, 256, 0, h->stream>>>(z, nb, i0, world, rank, rows, m, tl);
+                rec::k_rec_target_logits<T><<<(m + 255) / 256, 256, 0, h->stream>>>(z, nb, i0, world, rank, rows, m, tl, seen, flag);
             }));
         }
-        // every rank's slot, bits as they are (a float sum would turn a -0 logit into +0); a rank owning no target
-        // sends a slot nobody reads
-        if (world > 1) RET(comm_gather_lists(h, tl, tlg, sizeof(T), nullptr, nullptr, (size_t)m));
-        if (by_seen) RET(rec_build_seen(h, n_seen.c_str(), seen, I, u, max_ts, excl));
+        // every rank's slot, bits as they are (a float sum would turn a -0 logit into +0), and its seen flags in the
+        // same group; a rank owning no target sends a slot nobody reads
+        if (world > 1) RET(comm_gather_lists(h, tl, tlg, sizeof(T), flag, flagg, (size_t)m));
         RET(launch(h, n_target.c_str(), [&] {
-            if (by_seen) rec::k_rec_rank_sort_seen<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, (long)I, seen, place, nvalid, ss, sr, bins);
+            if (by_seen) rec::k_rec_rank_sort_seen<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, m, (long)I, flagg, place, nvalid, ss, sr, bins);
             else rec::k_rec_rank_sort<K><<<1, knn::kMaxK, 0, h->stream>>>(rows, tlg, m, world, m, (long)I, excl, nex, place, nvalid, ss, sr, bins);
         }));
         for (int64_t i0 = 0; i0 < N; i0 += Bc) {
@@ -1410,7 +1424,7 @@ struct RecRank {
             const int grid = (nb + rec::kRankRows - 1) / rec::kRankRows;
             RET(score((int)i0, nb));
             RET(launch(h, n_count.c_str(), [&] {
-                if (by_seen) rec::k_rec_rank_seen<K><<<grid, rec::kRankThreads, 0, h->stream>>>(z, nb, (int)i0, seen, ss, sr, nvalid, bins);
+                if (by_seen) rec::k_rec_rank_seen<K><<<grid, rec::kRankThreads, 0, h->stream>>>(z, nb, (int)i0, world, rank, seen, ss, sr, nvalid, bins);
                 else rec::k_rec_rank<K><<<grid, rec::kRankThreads, (size_t)nex * 4, h->stream>>>(z, nb, (int)i0, world, rank, excl, nex, ss, sr, nvalid, bins);
             }));
         }
@@ -2669,7 +2683,6 @@ int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t
         if (!args_ok)
             return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs, "
                                           "exclude in [0, 2], max_ts under CTR_EXCLUDE_SEEN)", knn::kMaxK);
-        if (coll && exclude == CTR_EXCLUDE_SEEN) return set_err(h, CTR_ESTATE, "CTR_EXCLUDE_SEEN on a row-sharded ITEM_EMB");
         if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
         RET(coll ? comm_check(h) : check_tables(h));
         const int64_t N = h->tab_rows[T];
@@ -2688,6 +2701,7 @@ int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t
         if (args_ok) {
             hd.hash[0] = comm_hash(user_rows, (size_t)nu * sizeof(int32_t));
             hd.hash[1] = comm_hash(hist_rows, (size_t)nu * S * sizeof(int32_t));
+            if (exclude == CTR_EXCLUDE_SEEN) hd.hash[2] = comm_hash(max_ts, (size_t)nu * sizeof(int64_t));
             hd.plan = std::min<int64_t>(nu, 256);      // users per list all-gather (G below)
         }
         const int rc = comm_agree(h, hd, verdict);
@@ -2699,7 +2713,7 @@ int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
     const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
     const bool seen = exclude == CTR_EXCLUDE_SEEN;
-    RecTopk<knn::LogitKey> sel{h, "rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, N, Bc, seen};
+    RecTopk<knn::LogitKey> sel{h, "rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, N, Bc, seen, h->tab_rows[T]};
     const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
     int* d_hist; float* d_gs = nullptr; int* d_gr = nullptr;      // [W][G][k] the ranks' lists of the group
     RET(sel.setup(4, G, [&](Carve& c) {
@@ -2750,7 +2764,6 @@ int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hi
         if (!args_ok)
             return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank, exclude in [0, 2], "
                                           "max_ts under CTR_EXCLUDE_SEEN)");
-        if (coll && seen) return set_err(h, CTR_ESTATE, "CTR_EXCLUDE_SEEN on a row-sharded ITEM_EMB");
         if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
         RET(coll ? comm_check(h) : check_tables(h));
         const int64_t N = h->tab_rows[T];
@@ -2778,6 +2791,7 @@ int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hi
             hd.hash[0] = comm_hash(user_rows, (size_t)n * sizeof(int32_t));
             hd.hash[1] = comm_hash(hist_rows, (size_t)n * S * sizeof(int32_t));
             hd.hash[2] = comm_hash(item_rows, (size_t)n * sizeof(int32_t));
+            if (seen) hd.hash[2] = comm_hash(max_ts, (size_t)n * sizeof(int64_t), hd.hash[2]);      // the cuts, chained
             hd.plan = (int64_t)passes.size();            // two collectives per pass
         }
         const int rc = comm_agree(h, hd, verdict);

@@ -10,7 +10,8 @@
 //   k_rec_finish: the users' lists → rows (-1 past the count), logits and scores (0 past the count), counts
 // ctr_mlp_recommend_topk runs the same three kernels on the float64 MLP's logits, with Logit64Key.  Under
 // CTR_EXCLUDE_SEEN the _seen siblings of k_rec_scan, k_rec_rank_sort and k_rec_rank test each row against the user's
-// seen bitmap (k_ub_seen, ubcache.cuh) in place of the window's rows.
+// seen bitmap (k_ub_seen, ubcache.cuh) in place of the window's rows; on a row-sharded ITEM_EMB each rank's bitmap
+// covers its own local rows, built from its own behaviour cache.
 #pragma once
 #include "knn.cuh"
 #include "mlp64.cuh"
@@ -29,9 +30,10 @@ using knn::kThreads;
 template <class K>
 __host__ inline size_t scan_smem_bytes(int k, int nex) { return knn::smem_bytes<K>(1, 0, k) + (size_t)nex * 4 + 16; }
 
-// The seen set of CTR_EXCLUDE_SEEN (k_ub_seen, ubcache.cuh): a bitmap over the global rows [0, I), bit r & 31 of word
-// r >> 5 set when row r is excluded.  Any history length costs one word load per item and ⌈I / 32⌉ words, a 32·D-th of
-// the ITEM_EMB table.  SEEN is single-table only (world = 1), so its kernels take no (world, rank).
+// The seen set of CTR_EXCLUDE_SEEN (k_ub_seen, ubcache.cuh): a bitmap over the rank's local rows [0, N_local), bit
+// l & 31 of word l >> 5 set when local row l (global row l·world + rank) is excluded; on a single table the global rows
+// [0, I).  Any history length costs one word load per item and ⌈N_local / 32⌉ words, a 32·D-th of the rank's shard.
+// The owner of a row decides: a target's verdict is read on its owner (k_rec_target_logits) and travels with its logit.
 __device__ __forceinline__ bool rec_seen(const unsigned* __restrict__ seen, int row) { return (__ldg(seen + (row >> 5)) >> (row & 31)) & 1u; }
 
 // z[b] is the logit of local row row0 + b, b < n; local row l is global row l·world + rank (a row-sharded ITEM_EMB; 1
@@ -39,8 +41,8 @@ __device__ __forceinline__ bool rec_seen(const unsigned* __restrict__ seen, int 
 // harmless).  run_s / run_r: the user's running list over the earlier chunks (nullptr for the first): only rows that
 // beat its k-th entry can enter the result, so the slice lists start out filled with that entry — its row lies in an
 // earlier chunk, so the fillers are told apart by row and written back as empty entries.
-// Out: per slice the top-k list of global rows, [slices][k].  SEEN (k_rec_scan_seen): the rows of the bitmap seen are
-// excluded in place of excl.
+// Out: per slice the top-k list of global rows, [slices][k].  SEEN (k_rec_scan_seen): the local rows of the bitmap seen
+// are excluded in place of excl.
 template <class K, bool SEEN>
 __device__ __forceinline__ void rec_scan(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
                                          const int* __restrict__ excl, int nex, const unsigned* __restrict__ seen, int k,
@@ -73,7 +75,7 @@ __device__ __forceinline__ void rec_scan(const typename K::T* __restrict__ z, in
             if (b >= r1) continue;
             const int row = (row0 + b) * world + rank;
             bool skip = false;
-            if constexpr (SEEN) skip = rec_seen(seen, row);
+            if constexpr (SEEN) skip = rec_seen(seen, row0 + b);
             else for (int e = 0; e < m; e++) skip |= ex[e] == row;
             if (!skip) knn::offer(sm, 0, k, __ldg(z + b), row);
         }
@@ -96,7 +98,16 @@ __global__ void __launch_bounds__(kThreads) k_rec_scan(const typename K::T* __re
     rec_scan<K, false>(z, n, row0, world, rank, rows_per_slice, excl, nex, nullptr, k, run_s, run_r, out_s, out_row);
 }
 
-// k_rec_scan on a single table with the rows of the bitmap seen excluded; dynamic shared memory scan_smem_bytes<K>(k, 0)
+// k_rec_scan with the local rows of the bitmap seen excluded; dynamic shared memory scan_smem_bytes<K>(k, 0)
+template <class K>
+__global__ void __launch_bounds__(kThreads) k_rec_scan_seen(const typename K::T* __restrict__ z, int n, int row0, int world, int rank, int rows_per_slice,
+                                                             const unsigned* __restrict__ seen, int k,
+                                                             const typename K::T* run_s, const int* run_r,
+                                                             typename K::T* __restrict__ out_s, int* __restrict__ out_row) {
+    rec_scan<K, true>(z, n, row0, world, rank, rows_per_slice, nullptr, 0, seen, k, run_s, run_r, out_s, out_row);
+}
+
+// the single-table form (world = 1, rank = 0)
 template <class K>
 __global__ void __launch_bounds__(kThreads) k_rec_scan_seen(const typename K::T* __restrict__ z, int n, int row0, int rows_per_slice,
                                                              const unsigned* __restrict__ seen, int k,
@@ -142,30 +153,38 @@ __global__ void k_rec_finish(const typename K::T* __restrict__ ls, const int* __
 // target's logit comes from the rank that owns its row, the ranks' target logits are all-gathered into tl [world][tls]
 // (target j read from slot rows[j] % world), every rank sorts the same targets, and the bins the ranks count over their
 // shards are summed before k_rec_rank_finish.  With world = 1 and tls = m these are the single-table kernels.
+// Under CTR_EXCLUDE_SEEN a target's verdict is its owner's: k_rec_target_logits also writes the owner's seen flag of
+// each target it copies, the flags travel in the same all-gather as the logits ([world][tls], the same slots), and
+// k_rec_rank_sort_seen reads them next to the logits.
 constexpr int kRankThreads = 256;
 constexpr int kRankRows = 2048;               // items per CTA of k_rec_rank
 
 // z[b] is the logit of local row row0 + b, b < n (global row (row0 + b)·world + rank); tl[j] = the logit of target j
-// when this rank owns rows[j] and it lies in this chunk
+// when this rank owns rows[j] and it lies in this chunk.  seen (CTR_EXCLUDE_SEEN; nullptr otherwise): this rank's
+// bitmap over its local rows, and flag[j] = whether that target is seen.
 template <class T>
 __global__ void k_rec_target_logits(const T* __restrict__ z, int n, int row0, int world, int rank, const int* __restrict__ rows, int m,
-                                    T* __restrict__ tl) {
+                                    T* __restrict__ tl, const unsigned* __restrict__ seen = nullptr, int* __restrict__ flag = nullptr) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= m) return;
     const int t = rows[j];
     if (t < 0 || t % world != rank) return;
     const long b = (long)(t / world) - row0;
-    if (b >= 0 && b < n) tl[j] = z[b];
+    if (b >= 0 && b < n) {
+        tl[j] = z[b];
+        if (seen) flag[j] = rec_seen(seen, row0 + (int)b);
+    }
 }
 
 // <<<1, kMaxK>>>.  tl [world][tls]: target j's logit at tl[(rows[j] % world)·tls + j].  place[j]: target j's place
 // among the v valid targets (ties by index), -1 when invalid; ss / sr [v]: the valid targets' (logit, row) in list
-// order; bins[0, m] zeroed.  n_items: the global row count.
+// order; bins[0, m] zeroed.  n_items: the global row count.  SEEN: a target is excluded when its owner's flag
+// (flag [world][tls], the slots of tl) is set, or on a single table (flag == nullptr) when the bitmap seen marks it.
 template <class K, bool SEEN>
 __device__ __forceinline__ void rec_rank_sort(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
                                               long n_items, const int* __restrict__ excl, int nex, const unsigned* __restrict__ seen,
-                                              int* __restrict__ place, int* __restrict__ nvalid, typename K::T* __restrict__ ss,
-                                              int* __restrict__ sr, unsigned long long* __restrict__ bins) {
+                                              const int* __restrict__ flag, int* __restrict__ place, int* __restrict__ nvalid,
+                                              typename K::T* __restrict__ ss, int* __restrict__ sr, unsigned long long* __restrict__ bins) {
     using T = typename K::T;
     __shared__ T s[kMaxK];
     __shared__ int r[kMaxK];
@@ -178,7 +197,7 @@ __device__ __forceinline__ void rec_rank_sort(const int* __restrict__ rows, cons
         ok = r[j] >= 0 && r[j] < n_items;
         s[j] = ok ? tl[(size_t)(r[j] % world) * tls + j] : T(0);
         ok = ok && K::qualifies(s[j]);
-        if constexpr (SEEN) ok = ok && !rec_seen(seen, r[j]);
+        if constexpr (SEEN) ok = ok && !(flag ? flag[(size_t)(r[j] % world) * tls + j] : rec_seen(seen, r[j]));
         else for (int e = 0; e < nex && ok; e++) ok = __ldg(excl + e) != r[j];
         if (!ok) r[j] = -1;                                   // marks the target invalid for the others
     }
@@ -202,15 +221,24 @@ __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort(const int* __restrict__
                                                          long n_items, const int* __restrict__ excl, int nex, int* __restrict__ place,
                                                          int* __restrict__ nvalid, typename K::T* __restrict__ ss, int* __restrict__ sr,
                                                          unsigned long long* __restrict__ bins) {
-    rec_rank_sort<K, false>(rows, tl, tls, world, m, n_items, excl, nex, nullptr, place, nvalid, ss, sr, bins);
+    rec_rank_sort<K, false>(rows, tl, tls, world, m, n_items, excl, nex, nullptr, nullptr, place, nvalid, ss, sr, bins);
 }
 
-// k_rec_rank_sort on a single table (tl [m]) with the rows of the bitmap seen excluded
+// k_rec_rank_sort with the targets their owners flag seen excluded: flag [world][tls] as tl (k_rec_target_logits)
+template <class K>
+__global__ void __launch_bounds__(kMaxK) k_rec_rank_sort_seen(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int tls, int world, int m,
+                                                              long n_items, const int* __restrict__ flag, int* __restrict__ place,
+                                                              int* __restrict__ nvalid, typename K::T* __restrict__ ss, int* __restrict__ sr,
+                                                              unsigned long long* __restrict__ bins) {
+    rec_rank_sort<K, true>(rows, tl, tls, world, m, n_items, nullptr, 0, nullptr, flag, place, nvalid, ss, sr, bins);
+}
+
+// the single-table form (tl [m]): the rows of the bitmap seen (global rows) excluded
 template <class K>
 __global__ void __launch_bounds__(kMaxK) k_rec_rank_sort_seen(const int* __restrict__ rows, const typename K::T* __restrict__ tl, int m, long n_items,
                                                               const unsigned* __restrict__ seen, int* __restrict__ place, int* __restrict__ nvalid,
                                                               typename K::T* __restrict__ ss, int* __restrict__ sr, unsigned long long* __restrict__ bins) {
-    rec_rank_sort<K, true>(rows, tl, m, 1, m, n_items, nullptr, 0, seen, place, nvalid, ss, sr, bins);
+    rec_rank_sort<K, true>(rows, tl, m, 1, m, n_items, nullptr, 0, seen, nullptr, place, nvalid, ss, sr, bins);
 }
 
 // grid = slices of kRankRows items of the chunk z[0, n) (local rows row0 + b, global (row0 + b)·world + rank); the
@@ -265,12 +293,12 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank(const typename K::T* 
         if (cb[i]) atomicAdd(bins + i, (unsigned long long)cb[i]);
 }
 
-// k_rec_rank on a single table with the rows of the bitmap seen excluded; no dynamic shared memory.  A copy of
-// k_rec_rank's counting loop rather than a body shared with it: sharing changes k_rec_rank's register allocation.
+// k_rec_rank with the local rows of the bitmap seen excluded; no dynamic shared memory.  A copy of k_rec_rank's
+// counting loop rather than a body shared with it: sharing changes k_rec_rank's register allocation.
 template <class K>
-__global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K::T* __restrict__ z, int n, int row0, const unsigned* __restrict__ seen,
-                                                                const typename K::T* __restrict__ ss, const int* __restrict__ sr,
-                                                                const int* __restrict__ nvalid, unsigned long long* __restrict__ bins) {
+__device__ __forceinline__ void rec_rank_seen(const typename K::T* __restrict__ z, int n, int row0, int world, int rank,
+                                              const unsigned* __restrict__ seen, const typename K::T* __restrict__ ss, const int* __restrict__ sr,
+                                              const int* __restrict__ nvalid, unsigned long long* __restrict__ bins) {
     using T = typename K::T;
     __shared__ T ks[kMaxK];
     __shared__ int kr[kMaxK];
@@ -287,8 +315,8 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K
         int q = v;                                            // bin v: comes before no target
         if (b < r1) {
             const T s = __ldg(z + b);
-            const int row = row0 + b;
-            if (K::qualifies(s) && !rec_seen(seen, row)) {
+            const int row = (row0 + b) * world + rank;
+            if (K::qualifies(s) && !rec_seen(seen, row0 + b)) {
                 int lo = 0, hi = v;                           // the first target this item comes before
                 while (lo < hi) {
                     const int mid = (lo + hi) >> 1;
@@ -303,6 +331,22 @@ __global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K
     __syncthreads();
     for (int i = threadIdx.x; i < v; i += kRankThreads)
         if (cb[i]) atomicAdd(bins + i, (unsigned long long)cb[i]);
+}
+
+template <class K>
+__global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K::T* __restrict__ z, int n, int row0, int world, int rank,
+                                                                const unsigned* __restrict__ seen, const typename K::T* __restrict__ ss,
+                                                                const int* __restrict__ sr, const int* __restrict__ nvalid,
+                                                                unsigned long long* __restrict__ bins) {
+    rec_rank_seen<K>(z, n, row0, world, rank, seen, ss, sr, nvalid, bins);
+}
+
+// the single-table form (world = 1, rank = 0)
+template <class K>
+__global__ void __launch_bounds__(kRankThreads) k_rec_rank_seen(const typename K::T* __restrict__ z, int n, int row0, const unsigned* __restrict__ seen,
+                                                                const typename K::T* __restrict__ ss, const int* __restrict__ sr,
+                                                                const int* __restrict__ nvalid, unsigned long long* __restrict__ bins) {
+    rec_rank_seen<K>(z, n, row0, 1, 0, seen, ss, sr, nvalid, bins);
 }
 
 // <<<1, kMaxK>>>: out_rank[j] and out_logit[j] (NaN for a row outside [0, n_items)); tl [world][tls] as for k_rec_rank_sort

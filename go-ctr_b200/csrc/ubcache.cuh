@@ -43,14 +43,16 @@ k_ub_window(const long long* __restrict__ off, const long long* __restrict__ ts,
     }
 }
 
-// The seen set of CTR_EXCLUDE_SEEN as a bitmap over rows [0, n_items) (rec.cuh, rec_seen): the item rows of user u's
-// events with ts <= max_ts (max_ts == 0: every event; cache.go:71-94) and the window rows hist[0, S).  The events are one
-// run [first, end) of the time-descending sequence; every block finds `first` with its first warp, then the grid
+// The seen set of CTR_EXCLUDE_SEEN as a bitmap over this rank's local rows (rec.cuh, rec_seen): the item rows of user
+// u's events with ts <= max_ts (max_ts == 0: every event; cache.go:71-94) and the window rows hist[0, S).  The events
+// are one run [first, end) of the time-descending sequence; every block finds `first` with its first warp, then the grid
 // strides over the run and the window.  Rows outside [0, n_items) are skipped; an unknown user, or no cache (off ==
-// nullptr), adds no event.  seen is zeroed by the caller.
+// nullptr), adds no event.  On a row-sharded ITEM_EMB only the rows this rank owns are marked (global row r is local
+// row r / world of rank r % world), so each row's verdict comes from its owner's cache; world = 1, rank = 0: the bitmap
+// over the global rows.  seen (⌈local rows / 32⌉ words) is zeroed by the caller.
 __global__ void __launch_bounds__(256)
 k_ub_seen(const long long* __restrict__ off, const long long* __restrict__ ts, const int* __restrict__ items, long n_users, int u,
-          long long max_ts, const int* __restrict__ hist, int S, long n_items, unsigned* __restrict__ seen) {
+          long long max_ts, const int* __restrict__ hist, int S, long n_items, int world, int rank, unsigned* __restrict__ seen) {
     __shared__ long long first_s;
     long long beg = 0, end = 0;
     if (off && u >= 0 && u < n_users) { beg = off[u]; end = off[u + 1]; }
@@ -63,7 +65,10 @@ k_ub_seen(const long long* __restrict__ off, const long long* __restrict__ ts, c
     const long long first = first_s, ne = end - first;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < ne + S; i += (long long)gridDim.x * blockDim.x) {
         const int r = i < ne ? items[first + i] : hist[i - ne];
-        if (r >= 0 && r < n_items) atomicOr(seen + (r >> 5), 1u << (r & 31));
+        if (r >= 0 && r < n_items && r % world == rank) {
+            const int l = r / world;
+            atomicOr(seen + (l >> 5), 1u << (l & 31));
+        }
     }
 }
 

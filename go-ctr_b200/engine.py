@@ -500,8 +500,11 @@ class Engine:
         Returns (rows [nu, k] int32, scores [nu, k] float32, logits [nu, k] float32, counts [nu] int32), best first
         (logit descending, then row ascending); positions past a user's count hold row -1, score 0 and logit 0.
         exclude_seen (implies exclude_history) also drops every item of the user's ubcache events with ts <= max_ts
-        (a scalar or [nu]; None or 0: every event); it is refused (ESTATE) on a row-sharded ITEM_EMB.
-        On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search."""
+        (a scalar or [nu]; None or 0: every event).
+        On a row-sharded ITEM_EMB the call is collective, under the same rule as knn_search; max_ts must agree too.
+        There exclude_seen follows the owner rule: row g is dropped when it is in the window, or when the ubcache of
+        rank g % world holds an event of the user with ts <= max_ts whose item is g.  With the same cache on every rank
+        (every ubcache upload, append and set applied on every rank) the lists equal one GPU's with that cache."""
         u, up = _i(np.atleast_1d(user_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))
         mode, t = _exclusion(u.size, max_ts, exclude_history, exclude_seen)
@@ -521,7 +524,8 @@ class Engine:
         the same user, history and item rows and receives the same ranks and logits, bit-identical to one GPU holding the
         whole table; rows that differ between the ranks raise CTR_EINVAL on every rank.  No sync is needed after
         training.  exclude_seen and max_ts (a scalar or [n], key i's cut) as for recommend_topk: a target the user has
-        seen by the cut ranks -1."""
+        seen by the cut ranks -1 and still reports its logit; on a row-sharded ITEM_EMB whether a row is seen is decided
+        by the rank that owns it, from its own ubcache (the owner rule of recommend_topk)."""
         u, up = _i(np.atleast_1d(user_rows))
         it, ip = _i(np.atleast_1d(item_rows))
         hs, hp = _i(np.asarray(hist).reshape(u.size, self.cfg.S))

@@ -51,7 +51,8 @@ def Recommend(recSys, userId, k, now=None, exclude_history=True, exclude_seen=Fa
     Every ITEM_EMB row is scored with the trained model (ctr_recommend_topk); the user's history is windowed from the
     device ubcache at `now` (empty without one, as in BatchPredict); exclude_history drops the items of that window, and
     exclude_seen (implies exclude_history) every item of the user's ubcache events up to `now`: nothing the user has
-    already consumed is recommended.  exclude_seen is refused (ESTATE) on a row-sharded ITEM_EMB.
+    already consumed is recommended.  On a row-sharded ITEM_EMB each row's seen verdict comes from the cache of the rank
+    that owns it, so keep the same behaviour cache on every rank (Engine.recommend_topk).
     An unknown user raises CtrError with code ENOTFOUND, as BatchPredict does for an unresolvable first key.
     On an engine whose ITEM_EMB is row-sharded over several GPUs the call is collective: every rank's process makes
     the same call (same user, k, now and history) and receives the same complete result (Engine.recommend_topk).
@@ -91,7 +92,8 @@ def Evaluate(recSys, heldOut, ks=(10,), exclude_history=True, exclude_seen=False
     the same id maps and behaviour cache; a rank whose rows differ makes the call raise CtrError EINVAL on every rank.
     exclude_seen (implies exclude_history) is the filtered protocol: every item of the user's ubcache events with ts <=
     the sample's Timestamp is removed from the catalogue it is ranked against (and ranks -1 itself), so no event after
-    the cut is excluded.  It is refused (ESTATE) on a row-sharded ITEM_EMB."""
+    the cut is excluded.  On a row-sharded ITEM_EMB it follows the owner rule (Engine.recommend_topk): with the same
+    behaviour cache on every rank, the metrics equal one GPU's."""
     if len(heldOut) == 0:
         raise ValueError("no held-out samples")
     u = np.fromiter((s.UserId for s in heldOut), np.int64, len(heldOut))

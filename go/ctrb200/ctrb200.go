@@ -314,7 +314,10 @@ func (e *Engine) Recommend(userRows, histRows []int32, k int, excludeHistory boo
 
 // RecommendSeen is Recommend that never lists an item the user has already seen: besides the valid history rows, the
 // item of every event of the user's device behaviour cache with timestamp <= maxTs[j] (0: every event) is excluded.
-// maxTs has one cut per user. Refused (CTR_ESTATE) on a row-sharded ITEM_EMB.
+// maxTs has one cut per user. With a row-sharded ITEM_EMB RecommendSeen is collective like Recommend, and every rank
+// must pass the same maxTs. The rank that owns a row decides whether it is seen: row g is excluded when it is a valid
+// history row, or when the behaviour cache of rank g % world holds such an event for item g. Apply every cache upload,
+// append and set on every rank; then the result equals one GPU holding the whole table and that cache.
 func (e *Engine) RecommendSeen(userRows, histRows []int32, maxTs []int64, k int) (outRows []int32, scores, logits []float32, counts []int32, err error) {
 	if len(maxTs) != len(userRows) {
 		return nil, nil, nil, nil, fmt.Errorf("ctrb200: RecommendSeen needs one maxTs per user")
@@ -358,7 +361,8 @@ func (e *Engine) RankItems(userRows, histRows, itemRows []int32, excludeHistory 
 
 // RankItemsSeen ranks as RecommendSeen lists: key i's seen set (its history rows and the items of the user's cached
 // events with timestamp <= maxTs[i]) is removed from the catalogue, and a target in it ranks -1. This is the filtered
-// full-ranking protocol; with maxTs[i] the held-out event's time, no later event is excluded.
+// full-ranking protocol; with maxTs[i] the held-out event's time, no later event is excluded. With a row-sharded
+// ITEM_EMB it is collective, under RecommendSeen's owner rule: a target's verdict comes from the rank that owns it.
 func (e *Engine) RankItemsSeen(userRows, histRows []int32, maxTs []int64, itemRows []int32) (ranks []int64, logits []float32, err error) {
 	if len(maxTs) != len(userRows) {
 		return nil, nil, fmt.Errorf("ctrb200: RankItemsSeen needs one maxTs per key")

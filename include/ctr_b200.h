@@ -227,7 +227,9 @@ int ctr_ubcache_window_dev(ctr_handle* h, const int32_t* d_user_row, const int64
  * [0, max(cache users, USER_FEAT rows, user id map size)); the cache's user count grows to the largest row + 1.
  * Everything is validated on the host before any device work (CTR_EINVAL), and a failed call leaves the cache as it
  * was.  One call rewrites the CSR into a spare buffer and swaps the two (O(stored events + users) of HBM traffic), on
- * the engine stream.  With world > 1 each rank's cache is its own; these calls are not collective.
+ * the engine stream.  With world > 1 each rank's cache is its own; these calls are not collective.  CTR_EXCLUDE_SEEN
+ * on a row-sharded ITEM_EMB reads each row's events from the cache of the rank that owns the row, so apply every
+ * upload, append and set on every rank.
  * download: the live cache back to the host.  *n_users and *n are always written; offsets [n_users+1] is written when
  *   non-NULL and cap_users >= n_users, ts / item_rows [n] when non-NULL and cap_events >= n; a non-NULL array that is
  *   too small is CTR_EINVAL, no cache is CTR_ESTATE. */
@@ -365,15 +367,24 @@ int ctr_recommend_topk(ctr_handle* h, const int32_t* user_rows, const int32_t* h
  *                       event of the user's device-ubcache sequence with ts <= max_ts (max_ts == 0: every event, as
  *                       TimeSeq.Filter, cache.go:71-94).  No ubcache, or a user row outside the cache, adds no event;
  *                       item rows of -1, rows past the table and repeated rows are harmless.  A superset of WINDOW, and
- *                       an evaluation cut at a held-out event's time never excludes the events after it. */
+ *                       an evaluation cut at a held-out event's time never excludes the events after it.
+ *                       Row-sharded ITEM_EMB (world > 1): the owner of a row decides.  Row g is excluded when it is a
+ *                       valid row of the window, or when the ubcache of rank g % world holds an event of the user with
+ *                       ts <= max_ts whose item is g.  With the same cache on every rank (apply ctr_ubcache_upload,
+ *                       _append and _set on every rank) the result is bit-identical to one GPU holding the whole table
+ *                       and that cache.  Caches that differ still give every rank the same complete result, each row
+ *                       following its owner's cache; no union of the ranks' caches is formed. */
 enum { CTR_EXCLUDE_NONE = 0, CTR_EXCLUDE_WINDOW = 1, CTR_EXCLUDE_SEEN = 2 };
 
 /* ctr_recommend_topk with an exclusion mode: ctr_recommend_topk(..., exclude_history, ...) ==
  * ctr_recommend_topk_ex(..., NULL, ..., exclude_history ? CTR_EXCLUDE_WINDOW : CTR_EXCLUDE_NONE, ...).  max_ts [nu] is
  * user j's cut under CTR_EXCLUDE_SEEN and may be NULL otherwise.  Refusals write nothing: CTR_EINVAL for an exclude
- * outside the enum or SEEN with a NULL max_ts, besides ctr_recommend_topk's; CTR_ESTATE for SEEN on a row-sharded
- * ITEM_EMB (world > 1, sharded placement; a replicated ITEM_EMB is served locally).  The seen set is built on the
- * device per user (a bitmap over the ITEM_EMB rows, ⌈I / 32⌉ words of the handle's scratch): no length cap. */
+ * outside the enum or SEEN with a NULL max_ts, besides ctr_recommend_topk's.  The seen set is built on the device per
+ * user (a bitmap over the rank's ITEM_EMB rows, ⌈I / 32⌉ words of the handle's scratch, ⌈I_local / 32⌉ on a shard): no
+ * length cap.  On a row-sharded ITEM_EMB SEEN is collective like the other modes, under the owner rule of
+ * CTR_EXCLUDE_SEEN: each rank marks the rows it owns from its own ubcache, with no exchange beyond the lists' merge.
+ * The ranks must also agree on max_ts (else CTR_EINVAL everywhere, "ranks disagree ...").  A replicated ITEM_EMB is
+ * served locally, from each rank's own cache. */
 int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, int64_t nu, int32_t k,
                           int32_t exclude, int32_t* out_rows, float* out_scores, float* out_logits, int32_t* out_count);
 
@@ -409,7 +420,9 @@ int ctr_rank_items(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_
  * is key i's cut under CTR_EXCLUDE_SEEN (may be NULL otherwise), a target in the key's seen set ranks -1, and for every
  * k in [1, 1024], 0 < rank <= k exactly when ctr_recommend_topk_ex(user, hist, max_ts, k, exclude) lists the target at
  * position rank - 1.  Under SEEN keys share a pass only with the same user row, history and max_ts.  Refusals as
- * ctr_recommend_topk_ex's, besides ctr_rank_items'. */
+ * ctr_recommend_topk_ex's, besides ctr_rank_items'.  On a row-sharded ITEM_EMB SEEN follows the owner rule of
+ * CTR_EXCLUDE_SEEN: a target's verdict comes from the rank that owns its row, in the same exchange as its logit, and a
+ * seen target still reports its logit.  The ranks must agree on max_ts as on the rows (CTR_EINVAL otherwise). */
 int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hist_rows, const int64_t* max_ts, const int32_t* item_rows, int64_t n,
                       int32_t exclude, int64_t* out_rank, float* out_logit);
 
