@@ -9,6 +9,8 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 namespace ctr {
 
@@ -215,6 +217,213 @@ __global__ void k_gauc_final(const GaucPart* __restrict__ part, int nparts, cons
     p = gauc_block_sum(p);
     if (threadIdx.x == 0)
         *res = {p.used > 0 ? (p.hi + p.lo) / (double)p.w : __longlong_as_double(0x7ff8000000000000ll), (long long)*runs, p.used};
+}
+
+// ---- curves and average precision (ctr_roc_curve, ctr_pr_curve, ctr_average_precision): binaryClfCurve --------------
+// (ranking.go:13-57) on ctr_roc_auc's key sort and positive-count scan.  The ends of the threshold groups are compacted
+// into points (tp_j, fp_j, key_j), one per group from the highest score down; small kernels turn the points into the
+// ROC arrays (ranking.go:71-103), the PR arrays (:183-209) or the AP terms (:212-222).  Every NaN these kernels make
+// is the quiet NaN 0x7ff8000000000000.
+
+__device__ __forceinline__ double clf_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+// float32 bits widened to float64 exactly, without float arithmetic (no flush of subnormals); NaNs keep sign and payload
+__device__ __forceinline__ double clf_widen(unsigned u) {
+    const unsigned long long s = (unsigned long long)(u >> 31) << 63, m = u & 0x7fffffu;
+    const unsigned e = (u >> 23) & 0xffu;
+    if (e == 0xffu) return __longlong_as_double((long long)(s | 0x7ff0000000000000ull | m << 29));
+    if (e == 0u) { const double d = __dmul_rn((double)m, 0x1p-149); return s ? -d : d; }
+    return __longlong_as_double((long long)(s | (unsigned long long)(e + 896u) << 52 | m << 29));
+}
+// the threshold of a threshold group: the inverse of auc_score_key, widened (the ±0 group has key(+0), so +0.0)
+__device__ __forceinline__ double clf_threshold(unsigned key) {
+    const unsigned v = ~key;
+    return clf_widen((v & 0x80000000u) ? (v & 0x7fffffffu) : ~v);
+}
+
+struct ClfPoint { int tp, fp; unsigned key; };
+// m points; tp / fp of the first and last point; last_ind = the first j with tp_j >= tp_last (sort.SearchFloat64s);
+// other = 1 when some label is neither the lowest nor the highest label (typeOfTarget is not "binary"), or NaN
+struct ClfSummary { int m, tp0, fp0, tp_last, fp_last, last_ind; unsigned lo, hi; int other; };
+
+// an order-preserving key of a non-NaN label (-0 read as +0), for the label range; clf_label_of inverts it
+__device__ __forceinline__ unsigned clf_label_key(float v) {
+    if (v == 0.0f) v = 0.0f;
+    const unsigned u = __float_as_uint(v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float clf_label_of(unsigned k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+// lowest and highest non-NaN label (typeOfTarget's lo / hi); sum->lo / sum->hi start at 0xffffffff / 0
+__global__ void k_clf_label_range(const float* __restrict__ y, long n, ClfSummary* __restrict__ sum) {
+    unsigned lo = 0xffffffffu, hi = 0u;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const float v = y[i];
+        if (v != v) continue;
+        const unsigned k = clf_label_key(v);
+        lo = k < lo ? k : lo; hi = k > hi ? k : hi;
+    }
+    lo = __reduce_min_sync(0xffffffffu, lo); hi = __reduce_max_sync(0xffffffffu, hi);
+    if ((threadIdx.x & 31) == 0) { atomicMin(&sum->lo, lo); atomicMax(&sum->hi, hi); }
+}
+// typeOfTarget's second loop: a label equal to neither lo nor hi (a NaN among them) makes the target not binary.
+// With rewrite, y[i] becomes 1 where y[i] == 1 and 0 elsewhere, so that auc_positive reads pos_label = 1.
+__global__ void k_clf_label_check(float* __restrict__ y, long n, ClfSummary* __restrict__ sum, int rewrite) {
+    const float lo = clf_label_of(sum->lo), hi = clf_label_of(sum->hi);
+    unsigned other = 0;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        const float v = y[i];
+        other |= (v != lo && v != hi) ? 1u : 0u;
+        if (rewrite) y[i] = v == 1.0f ? 1.0f : 0.0f;
+    }
+    other = __reduce_or_sync(0xffffffffu, other);
+    if ((threadIdx.x & 31) == 0 && other) atomicOr(&sum->other, 1);
+}
+
+__global__ void k_clf_keys(const float* __restrict__ pred, const float* __restrict__ y, long n, double pos_label,
+                           unsigned* __restrict__ keys, int* __restrict__ pos_flag) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        keys[i] = auc_score_key(pred[i]);
+        pos_flag[i] = (double)y[i] == pos_label ? 1 : 0;                  // ranking.go:41
+    }
+}
+// selects the last element of each threshold group in the sorted keys
+struct ClfIsEnd {
+    const unsigned* keys; long n;
+    __device__ __forceinline__ bool operator()(const int& i) const { return i + 1 == n || keys[i + 1] != keys[i]; }
+};
+__global__ void k_clf_points(const unsigned* __restrict__ keys, const int* __restrict__ tp, const int* __restrict__ ends,
+                             const int* __restrict__ d_m, long n, ClfPoint* __restrict__ pts, ClfSummary* __restrict__ sum) {
+    const int m = *d_m, tp_last = tp[n - 1];
+    for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j < m; j += (long)gridDim.x * blockDim.x) {
+        const int i = ends[j], t = tp[i];
+        const ClfPoint p{t, i + 1 - t, keys[i]};
+        pts[j] = p;
+        if (j == 0) { sum->m = m; sum->tp0 = p.tp; sum->fp0 = p.fp; }
+        if (j == m - 1) { sum->tp_last = p.tp; sum->fp_last = p.fp; }
+        if (t >= tp_last && (j == 0 || tp[ends[j - 1]] < tp_last)) sum->last_ind = (int)j;
+    }
+}
+
+// ROCCurve: the point (0, 0) prepended when fp_0 != 0 with threshold thresholds[0] + 1 (a NaN threshold kept as it is),
+// fpr = fps * (1 / fpmax) and tpr = tps * (1 / tpmax) as floats.Scale does, all NaN when fpmax / tpmax is 0
+__global__ void k_clf_roc(const ClfPoint* __restrict__ pts, const ClfSummary* __restrict__ sum, double* __restrict__ fpr,
+                          double* __restrict__ tpr, double* __restrict__ thr) {
+    const ClfSummary s = *sum;
+    const int pre = s.fp0 != 0 ? 1 : 0;
+    const double rf = 1.0 / (double)s.fp_last, rt = 1.0 / (double)s.tp_last;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < (long)s.m + pre; o += (long)gridDim.x * blockDim.x) {
+        double fp = 0.0, tp = 0.0, t;
+        if (o < pre) {
+            const double t0 = clf_threshold(pts[0].key);
+            t = t0 != t0 ? t0 : __dadd_rn(t0, 1.0);
+        } else {
+            const ClfPoint p = pts[o - pre];
+            fp = (double)p.fp; tp = (double)p.tp; t = clf_threshold(p.key);
+        }
+        fpr[o] = s.fp_last > 0 ? __dmul_rn(fp, rf) : clf_nan();
+        tpr[o] = s.tp_last > 0 ? __dmul_rn(tp, rt) : clf_nan();
+        thr[o] = t;
+    }
+}
+// PrecisionRecallCurve: the points 0 … last_ind reversed, precision tp / (tp + fp), recall tp / tp_last (NaN when
+// tp_last is 0), then (precision 1, recall 0) without a threshold
+__global__ void k_clf_pr(const ClfPoint* __restrict__ pts, const ClfSummary* __restrict__ sum, double* __restrict__ prec,
+                         double* __restrict__ rec, double* __restrict__ thr) {
+    const ClfSummary s = *sum;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o <= (long)s.last_ind + 1; o += (long)gridDim.x * blockDim.x) {
+        if (o > s.last_ind) { prec[o] = 1.0; rec[o] = 0.0; continue; }
+        const ClfPoint p = pts[s.last_ind - o];
+        prec[o] = __ddiv_rn((double)p.tp, (double)(p.tp + p.fp));
+        rec[o] = s.tp_last > 0 ? __ddiv_rn((double)p.tp, (double)s.tp_last) : clf_nan();
+        thr[o] = clf_threshold(p.key);
+    }
+}
+
+// one AP term of ranking.go:218: (recall_j - recall_{j-1}) * precision_j with recall_{-1} = 0, from the counts of point
+// j, the positives of point j - 1 (tpp) and the positives P of the whole curve
+__device__ __forceinline__ double ap_term(int tp, int fp, int tpp, bool first, int P) {
+    const double r = __ddiv_rn((double)tp, (double)P), rp = first ? 0.0 : __ddiv_rn((double)tpp, (double)P);
+    return __dmul_rn(__dsub_rn(r, rp), __ddiv_rn((double)tp, (double)(tp + fp)));
+}
+// the AP terms of points 0 … last_ind as per-block double-double sums, each thread's terms in index order; with
+// gauc_block_sum and a fixed grid the sum is the same bits on every call.  w counts the terms.
+__global__ void k_ap_terms(const ClfPoint* __restrict__ pts, const ClfSummary* __restrict__ sum, GaucPart* __restrict__ part) {
+    const ClfSummary s = *sum;
+    GaucPart p{0.0, 0.0, 0, 0};
+    if (s.tp_last > 0)
+        for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j <= s.last_ind; j += (long)gridDim.x * blockDim.x) {
+            const ClfPoint c = pts[j];
+            dd_add(p.hi, p.lo, ap_term(c.tp, c.fp, j > 0 ? pts[j - 1].tp : 0, j == 0, s.tp_last), 0.0);
+            p.w++;
+        }
+    p = gauc_block_sum(p);
+    if (threadIdx.x == 0) part[blockIdx.x] = p;
+}
+// AP = the parts summed in block order; NaN with no positives (every recall is 0 / 0 in the reference)
+__global__ void k_ap_final(const GaucPart* __restrict__ part, int nparts, const ClfSummary* __restrict__ sum, double* __restrict__ ap) {
+    GaucPart p{0.0, 0.0, 0, 0};
+    for (int b = threadIdx.x; b < nparts; b += blockDim.x) p = gauc_part_add(p, part[b]);
+    p = gauc_block_sum(p);
+    if (threadIdx.x == 0) *ap = sum->tp_last > 0 ? p.hi + p.lo : clf_nan();
+}
+
+// ---- grouped AP (ctr_group_average_precision): GAUC's (group, score) order and scan, AP terms per group -------------
+struct GapAgg { double hi, lo; int n, pos; };
+struct GapAggOp {
+    __device__ __forceinline__ GapAgg operator()(GapAgg a, const GapAgg& b) const {
+        dd_add(a.hi, a.lo, b.hi, b.lo);
+        a.n += b.n; a.pos += b.pos;
+        return a;
+    }
+};
+// each group's positives P_g, stored at the group's first element (the terms need them before the reduction)
+__global__ void k_gap_pos(const unsigned long long* __restrict__ gkey, const GaucScan* __restrict__ s, long n, int* __restrict__ gpos) {
+    for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j < n; j += (long)gridDim.x * blockDim.x) {
+        if (j + 1 < n && gkey[j + 1] == gkey[j]) continue;
+        const GaucScan e = s[j];
+        gpos[e.gs] = e.tp - (e.gs > 0 ? s[e.gs - 1].tp : 0);
+    }
+}
+// each threshold-group end adds its AP term, counted from its group's start (nothing in a group without positives).
+// The terms after the group's last_ind are (1 - 1) * precision = 0 exactly, so they need no cut.
+__global__ void k_gap_terms(const unsigned long long* __restrict__ gkey, const unsigned long long* __restrict__ packed,
+                            const GaucScan* __restrict__ s, const int* __restrict__ gpos, long n, GapAgg* __restrict__ val) {
+    for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j < n; j += (long)gridDim.x * blockDim.x) {
+        const unsigned long long v = packed[j];
+        double term = 0.0;
+        if (j + 1 == n || gkey[j + 1] != gkey[j] || (packed[j + 1] >> 32) != (v >> 32)) {
+            const GaucScan e = s[j];
+            const int P = gpos[e.gs];
+            if (P > 0) {
+                const int base = e.gs > 0 ? s[e.gs - 1].tp : 0;
+                const int tp = e.tp - base, fp = (int)(j - e.gs + 1) - tp;
+                const bool first = e.ts == e.gs;
+                term = ap_term(tp, fp, first ? 0 : s[e.ts - 1].tp - base, first, P);
+            }
+        }
+        val[j] = {term, 0.0, 1, (int)(v & 1)};
+    }
+}
+// per group: AP_g (NaN when P_g = 0) and the per-group outputs the caller asked for; per block: its part of the sum of
+// AP_g over the used groups, with w = used so that k_gauc_final's (hi + lo) / w is the unweighted mean
+__global__ void k_gap_groups(const unsigned long long* __restrict__ uniq, const GapAgg* __restrict__ agg, const int* __restrict__ runs,
+                             long long* __restrict__ out_group, int* __restrict__ out_n, int* __restrict__ out_pos,
+                             double* __restrict__ out_ap, GaucPart* __restrict__ part) {
+    const long R = *runs;
+    GaucPart p{0.0, 0.0, 0, 0};
+    for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < R; g += (long)gridDim.x * blockDim.x) {
+        const GapAgg a = agg[g];
+        const double ap = a.pos > 0 ? a.hi + a.lo : clf_nan();
+        if (out_group) out_group[g] = (long long)(uniq[g] ^ 0x8000000000000000ull);
+        if (out_n) out_n[g] = a.n;
+        if (out_pos) out_pos[g] = a.pos;
+        if (out_ap) out_ap[g] = ap;
+        if (a.pos > 0) { dd_add(p.hi, p.lo, ap, 0.0); p.w++; p.used++; }
+    }
+    p = gauc_block_sum(p);
+    if (threadIdx.x == 0) part[blockIdx.x] = p;
 }
 
 }  // namespace ctr

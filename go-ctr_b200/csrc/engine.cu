@@ -2533,6 +2533,200 @@ int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_
     return gauc_run(h, pred, y, group, (long)n, gauc, n_groups, n_used, out_group, out_n, out_pos, out_auc);
 }
 
+namespace {
+
+// binaryClfCurve on the engine stream (auc.cuh): with check_labels the labels' range and binariness first, then
+// ctr_roc_auc's key sort and positive-count scan, the threshold-group ends selected and turned into points.  Leaves
+// the points and the summary on the device and the summary in *s.
+struct ClfCurve { DevBuf<ClfPoint> pts; DevBuf<ClfSummary> sum; };
+int clf_build(ctr_handle* h, const float* pred_h, const float* y_h, long n, double pos_label, bool check_labels,
+              ClfCurve& c, ClfSummary* s) {
+    cudaStream_t st = h->stream;
+    const size_t N = (size_t)n;
+    const int grid = (int)std::min<long>((n + 255) / 256, (long)h->num_sms * 8);
+    DevBuf<float> d_pred, d_y; DevBuf<unsigned> k0, k1; DevBuf<int> f0, f1, tp, d_m;
+    DevBuf<unsigned char> tmp;
+    CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N));
+    CU(h, k0.alloc(N)); CU(h, k1.alloc(N)); CU(h, f0.alloc(N)); CU(h, f1.alloc(N)); CU(h, tp.alloc(N));
+    CU(h, d_m.alloc(1)); CU(h, c.pts.alloc(N)); CU(h, c.sum.alloc(1));
+    int* ends = f0.get();                     // free once the sort has read it
+    size_t b[3] = {0, 0, 0};
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[0], k0.get(), k1.get(), f0.get(), f1.get(), (int)n, 0, 32, st));
+    CU(h, cub::DeviceScan::InclusiveSum(nullptr, b[1], f1.get(), tp.get(), (int)n, st));
+    CU(h, cub::DeviceSelect::If(nullptr, b[2], thrust::counting_iterator<int>(0), ends, d_m.get(), (int)n, ClfIsEnd{k1.get(), n}, st));
+    size_t bytes = std::max(std::max(b[0], b[1]), b[2]);
+    CU(h, tmp.alloc(std::max<size_t>(bytes, 1)));
+    const ClfSummary init{0, 0, 0, 0, 0, 0, 0xffffffffu, 0u, 0};
+    CU(h, cudaMemcpyAsync(c.sum, &init, sizeof init, cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_pred, pred_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_y, y_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (check_labels) {
+        RET(launch(h, "ap_label_range", [&] { k_clf_label_range<<<grid, 256, 0, st>>>(d_y, n, c.sum); }));
+        RET(launch(h, "ap_label_check", [&] { k_clf_label_check<<<grid, 256, 0, st>>>(d_y, n, c.sum, 0); }));
+    }
+    RET(launch(h, "clf_keys", [&] { k_clf_keys<<<grid, 256, 0, st>>>(d_pred, d_y, n, pos_label, k0, f0); }));
+    RET(launch(h, "clf_sort", [&] {
+        cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, k0.get(), k1.get(), f0.get(), f1.get(), (int)n, 0, 32, st); }));
+    RET(launch(h, "clf_scan", [&] { cub::DeviceScan::InclusiveSum(tmp.get(), bytes, f1.get(), tp.get(), (int)n, st); }));
+    RET(launch(h, "clf_ends", [&] {
+        cub::DeviceSelect::If(tmp.get(), bytes, thrust::counting_iterator<int>(0), ends, d_m.get(), (int)n, ClfIsEnd{k1.get(), n}, st); }));
+    RET(launch(h, "clf_points", [&] { k_clf_points<<<grid, 256, 0, st>>>(k1, tp, ends, d_m, n, c.pts, c.sum); }));
+    CU(h, cudaMemcpyAsync(s, c.sum, sizeof *s, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+
+// ctr_roc_curve (roc) or ctr_pr_curve: the points turned into the three arrays on the device; the arrays the caller
+// passed come back, and nothing is written when the curve needs more than cap points (*npoints says how many)
+int clf_curve_run(ctr_handle* h, bool roc, const float* pred, const float* y, long n, double pos_label,
+                  double* a_h, double* b_h, double* thr_h, int64_t cap, int64_t* npoints) {
+    ClfCurve c; ClfSummary s{};
+    RET(clf_build(h, pred, y, n, pos_label, false, c, &s));
+    const long np_ = roc ? (long)s.m + (s.fp0 != 0 ? 1 : 0) : (long)s.last_ind + 2;
+    *npoints = np_;
+    if (np_ > cap)
+        return set_err(h, CTR_EINVAL, "%s curve needs %ld points, cap is %lld", roc ? "roc" : "pr", np_, (long long)cap);
+    cudaStream_t st = h->stream;
+    const int grid = (int)std::min<long>((np_ + 255) / 256, (long)h->num_sms * 8);
+    DevBuf<double> a, b, t;
+    CU(h, a.alloc((size_t)np_)); CU(h, b.alloc((size_t)np_)); CU(h, t.alloc((size_t)np_));
+    if (roc) RET(launch(h, "clf_roc", [&] { k_clf_roc<<<grid, 256, 0, st>>>(c.pts, c.sum, a, b, t); }));
+    else RET(launch(h, "clf_pr", [&] { k_clf_pr<<<grid, 256, 0, st>>>(c.pts, c.sum, a, b, t); }));
+    const size_t nt = (size_t)(roc ? np_ : np_ - 1);
+    if (a_h) CU(h, cudaMemcpyAsync(a_h, a, (size_t)np_ * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (b_h) CU(h, cudaMemcpyAsync(b_h, b, (size_t)np_ * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (thr_h) CU(h, cudaMemcpyAsync(thr_h, t, nt * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+
+}  // namespace
+
+int ctr_roc_curve(ctr_handle* h, const float* pred, const float* y, int64_t n, double pos_label, double* fpr, double* tpr,
+                  double* thresholds, int64_t cap, int64_t* npoints) {
+    if (!h || !pred || !y || !npoints || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad roc curve arguments (n must be in [1, 2^31); pred, y and npoints non-null)");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return clf_curve_run(h, true, pred, y, (long)n, pos_label, fpr, tpr, thresholds, cap, npoints);
+}
+
+int ctr_pr_curve(ctr_handle* h, const float* pred, const float* y, int64_t n, double pos_label, double* precision,
+                 double* recall, double* thresholds, int64_t cap, int64_t* npoints) {
+    if (!h || !pred || !y || !npoints || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad pr curve arguments (n must be in [1, 2^31); pred, y and npoints non-null)");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return clf_curve_run(h, false, pred, y, (long)n, pos_label, precision, recall, thresholds, cap, npoints);
+}
+
+int ctr_average_precision(ctr_handle* h, const float* pred, const float* y, int64_t n, double* ap) {
+    if (!h || !pred || !y || !ap || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad average precision arguments (n must be in [1, 2^31); pred, y and ap non-null)");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    ClfCurve c; ClfSummary s{};
+    RET(clf_build(h, pred, y, (long)n, 1.0, true, c, &s));
+    if (s.other) return set_err(h, CTR_EINVAL, "average precision needs binary labels (every label the lowest or the highest, no NaN)");
+    cudaStream_t st = h->stream;
+    const int gparts = h->num_sms * 2;
+    DevBuf<GaucPart> part; DevBuf<double> d_ap;
+    CU(h, part.alloc(gparts)); CU(h, d_ap.alloc(1));
+    RET(launch(h, "ap_terms", [&] { k_ap_terms<<<gparts, 256, 0, st>>>(c.pts, c.sum, part); }));
+    RET(launch(h, "ap_final", [&] { k_ap_final<<<1, 256, 0, st>>>(part, gparts, c.sum, d_ap); }));
+    double r = 0;
+    CU(h, cudaMemcpyAsync(&r, d_ap, sizeof r, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *ap = r;
+    return CTR_OK;
+}
+
+namespace {
+
+// ctr_group_average_precision: the label check (labels rewritten to pos_label = 1), GAUC's (group, score) order, heads
+// and scan, each group's positives, the AP terms, one reduce-by-key of (double-double sum, n, positives) over the
+// sorted group keys, then the per-group AP and their mean; only the result and the arrays asked for come back
+int gap_run(ctr_handle* h, const float* pred_h, const float* y_h, const int64_t* group_h, long n, double* map,
+            int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_ap) {
+    cudaStream_t st = h->stream;
+    const size_t N = (size_t)n;
+    const int grid = (int)std::min<long>((n + 255) / 256, (long)h->num_sms * 8), gparts = h->num_sms * 2;
+    DevBuf<float> d_pred, d_y; DevBuf<long long> d_group;
+    DevBuf<unsigned> k0, k1; DevBuf<int> i0, i1, d_runs;
+    DevBuf<unsigned long long> g0, g1, v0, v1;
+    DevBuf<GaucScan> scan; DevBuf<GapAgg> val, agg; DevBuf<GaucPart> part; DevBuf<GaucResult> res; DevBuf<ClfSummary> lab;
+    DevBuf<long long> o_group; DevBuf<int> o_n, o_pos; DevBuf<double> o_ap;
+    DevBuf<unsigned char> tmp;
+    CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N)); CU(h, d_group.alloc(N));
+    CU(h, k0.alloc(N)); CU(h, k1.alloc(N)); CU(h, i0.alloc(N)); CU(h, i1.alloc(N));
+    CU(h, g0.alloc(N)); CU(h, g1.alloc(N)); CU(h, v0.alloc(N)); CU(h, v1.alloc(N));
+    CU(h, scan.alloc(N)); CU(h, val.alloc(N)); CU(h, agg.alloc(N));
+    CU(h, d_runs.alloc(1)); CU(h, part.alloc(gparts)); CU(h, res.alloc(1)); CU(h, lab.alloc(1));
+    if (out_group) CU(h, o_group.alloc(N));
+    if (out_n) CU(h, o_n.alloc(N));
+    if (out_pos) CU(h, o_pos.alloc(N));
+    if (out_ap) CU(h, o_ap.alloc(N));
+    unsigned long long* uniq = g0.get();     // free once the group pass has read it
+    int* gpos = i0.get();                    // free once the score pass has read it
+    size_t b[4] = {0, 0, 0, 0};
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[0], k0.get(), k1.get(), i0.get(), i1.get(), (int)n, 0, 32, st));
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[1], g0.get(), g1.get(), v0.get(), v1.get(), (int)n, 0, 64, st));
+    CU(h, cub::DeviceScan::InclusiveScan(nullptr, b[2], scan.get(), scan.get(), GaucScanOp(), (int)n, st));
+    CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b[3], g1.get(), uniq, val.get(), agg.get(), d_runs.get(), GapAggOp(), (int)n, st));
+    size_t bytes = std::max(std::max(b[0], b[1]), std::max(b[2], b[3]));
+    CU(h, tmp.alloc(std::max<size_t>(bytes, 1)));
+    const ClfSummary init{0, 0, 0, 0, 0, 0, 0xffffffffu, 0u, 0};
+    CU(h, cudaMemcpyAsync(lab, &init, sizeof init, cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_pred, pred_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_y, y_h, N * sizeof(float), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(d_group, group_h, N * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    RET(launch(h, "gap_label_range", [&] { k_clf_label_range<<<grid, 256, 0, st>>>(d_y, n, lab); }));
+    RET(launch(h, "gap_label_check", [&] { k_clf_label_check<<<grid, 256, 0, st>>>(d_y, n, lab, 1); }));
+    RET(launch(h, "gap_keys", [&] { k_gauc_keys<<<grid, 256, 0, st>>>(d_pred, n, k0, i0); }));
+    RET(launch(h, "gap_sort_score", [&] {
+        cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, k0.get(), k1.get(), i0.get(), i1.get(), (int)n, 0, 32, st); }));
+    RET(launch(h, "gap_gather", [&] { k_gauc_gather<<<grid, 256, 0, st>>>(k1, i1, d_group, d_y, n, g0, v0); }));
+    RET(launch(h, "gap_sort_group", [&] {
+        cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, g0.get(), g1.get(), v0.get(), v1.get(), (int)n, 0, 64, st); }));
+    RET(launch(h, "gap_heads", [&] { k_gauc_heads<<<grid, 256, 0, st>>>(g1, v1, n, scan); }));
+    RET(launch(h, "gap_scan", [&] {
+        cub::DeviceScan::InclusiveScan(tmp.get(), bytes, scan.get(), scan.get(), GaucScanOp(), (int)n, st); }));
+    RET(launch(h, "gap_pos", [&] { k_gap_pos<<<grid, 256, 0, st>>>(g1, scan, n, gpos); }));
+    RET(launch(h, "gap_terms", [&] { k_gap_terms<<<grid, 256, 0, st>>>(g1, v1, scan, gpos, n, val); }));
+    RET(launch(h, "gap_reduce", [&] {
+        cub::DeviceReduce::ReduceByKey(tmp.get(), bytes, g1.get(), uniq, val.get(), agg.get(), d_runs.get(), GapAggOp(), (int)n, st); }));
+    RET(launch(h, "gap_groups", [&] { k_gap_groups<<<gparts, 256, 0, st>>>(uniq, agg, d_runs, o_group, o_n, o_pos, o_ap, part); }));
+    RET(launch(h, "gap_final", [&] { k_gauc_final<<<1, 256, 0, st>>>(part, gparts, d_runs, res); }));
+    GaucResult r{}; ClfSummary ls{};
+    CU(h, cudaMemcpyAsync(&r, res, sizeof r, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(&ls, lab, sizeof ls, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (ls.other)
+        return set_err(h, CTR_EINVAL, "group average precision needs binary labels (every label the lowest or the highest, no NaN)");
+    const size_t R = (size_t)r.groups;
+    if (out_group) CU(h, cudaMemcpyAsync(out_group, o_group, R * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_n) CU(h, cudaMemcpyAsync(out_n, o_n, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_pos) CU(h, cudaMemcpyAsync(out_pos, o_pos, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_ap) CU(h, cudaMemcpyAsync(out_ap, o_ap, R * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *map = r.gauc;
+    if (n_groups) *n_groups = r.groups;
+    if (n_used) *n_used = r.used;
+    return CTR_OK;
+}
+
+}  // namespace
+
+int ctr_group_average_precision(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n, double* map,
+                                int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos,
+                                double* out_ap) {
+    if (!h || !pred || !y || !group || !map || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad group average precision arguments (n must be in [1, 2^31); pred, y, group and map non-null)");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return gap_run(h, pred, y, group, (long)n, map, n_groups, n_used, out_group, out_n, out_pos, out_ap);
+}
+
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");

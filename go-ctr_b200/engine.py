@@ -30,7 +30,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
            "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
@@ -471,6 +471,61 @@ class Engine:
         if outs is None:
             return gauc.value, ng.value, nu.value
         return gauc.value, ng.value, nu.value, {k: v[:ng.value].copy() for k, v in outs.items()}
+
+    def _curve(self, fn, pred, y, pos_label):
+        p, pp = _f(pred); t, tp = _f(y)
+        if p.size != t.size:
+            raise ValueError("pred and y differ in length: %d, %d" % (p.size, t.size))
+        cap = p.size + 1
+        a, b, th = np.empty(cap), np.empty(cap), np.empty(cap)
+        npts = C.c_int64(0)
+        dp = lambda x: x.ctypes.data_as(C.POINTER(C.c_double))
+        self._ck(fn(self.h, pp, tp, C.c_int64(p.size), C.c_double(pos_label), dp(a), dp(b), dp(th), C.c_int64(cap),
+                    C.byref(npts)))
+        return a, b, th, npts.value
+
+    def roc_curve(self, pred, y, pos_label=1.0):
+        """ROCCurve (ctr_roc_curve): (fpr, tpr, thresholds) as float64 arrays, one point per distinct score from the
+        highest down, (0, 0) first when the top score holds a negative.  A sample is positive when y == pos_label."""
+        fpr, tpr, th, m = self._curve(self.L.ctr_roc_curve, pred, y, pos_label)
+        return fpr[:m].copy(), tpr[:m].copy(), th[:m].copy()
+
+    def precision_recall_curve(self, pred, y, pos_label=1.0):
+        """PrecisionRecallCurve (ctr_pr_curve): (precision, recall, thresholds), recall decreasing to the final
+        (precision 1, recall 0), which has no threshold.  A sample is positive when y == pos_label."""
+        prec, rec, th, m = self._curve(self.L.ctr_pr_curve, pred, y, pos_label)
+        return prec[:m].copy(), rec[:m].copy(), th[:m - 1].copy()
+
+    def average_precision(self, pred, y):
+        """AveragePrecisionScore of a binary target (ctr_average_precision): the area under the precision-recall
+        curve as the reference sums it, positives y == 1; NaN with no positives, CtrError (EINVAL) for non-binary labels."""
+        p, pp = _f(pred); t, tp = _f(y)
+        if p.size != t.size:
+            raise ValueError("pred and y differ in length: %d, %d" % (p.size, t.size))
+        ap = C.c_double(0)
+        self._ck(self.L.ctr_average_precision(self.h, pp, tp, C.c_int64(p.size), C.byref(ap)))
+        return ap.value
+
+    def group_average_precision(self, pred, y, group, per_group=False):
+        """Mean average precision over groups (ctr_group_average_precision): AP within each group (normally the user
+        id), averaged without weights over the groups that hold a positive.  Returns (map, n_groups, n_used); with
+        per_group=True also a dict of the ascending group ids and their n, positives and AP (NaN with no positive)."""
+        p, pp = _f(pred); t, tp = _f(y)
+        gr = np.ascontiguousarray(group, np.int64)
+        if not p.size == t.size == gr.size:
+            raise ValueError("pred, y and group differ in length: %d, %d, %d" % (p.size, t.size, gr.size))
+        m = C.c_double(0); ng = C.c_int64(0); nu = C.c_int64(0)
+        outs = None
+        if per_group:
+            outs = dict(group=np.empty(p.size, np.int64), n=np.empty(p.size, np.int32), pos=np.empty(p.size, np.int32),
+                        ap=np.empty(p.size, np.float64))
+        ptr = (lambda k, ty: outs[k].ctypes.data_as(C.POINTER(ty))) if outs else (lambda k, ty: None)
+        self._ck(self.L.ctr_group_average_precision(self.h, pp, tp, gr.ctypes.data_as(_lp), C.c_int64(p.size), C.byref(m),
+                                                    C.byref(ng), C.byref(nu), ptr("group", C.c_int64), ptr("n", C.c_int32),
+                                                    ptr("pos", C.c_int32), ptr("ap", C.c_double)))
+        if outs is None:
+            return m.value, ng.value, nu.value
+        return m.value, ng.value, nu.value, {k: v[:ng.value].copy() for k, v in outs.items()}
 
     def knn_search(self, k, queries=None, rows=None):
         """search.Searcher on ITEM_EMB (ctr_knn_search): queries [nq, D] float64 vectors (rows: optional row to exclude

@@ -24,7 +24,8 @@ from . import engine as _e
 
 __all__ = ["SampleInfo", "TrainSample", "DinNet", "YoutubeDnn", "NewDinNet", "NewDinNetFromJson",
            "NewYoutubeDnn", "NewYoutubeDnnFromJson", "Train", "InitForwardOnlyVm", "Predict",
-           "DinImpl", "YoutubeDnnImpl", "RocAuc32", "GroupAuc32", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
+           "DinImpl", "YoutubeDnnImpl", "RocAuc32", "GroupAuc32", "ROCCurve", "PrecisionRecallCurve",
+           "AveragePrecisionScore", "GroupAveragePrecision32", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
 
 mlp0_1, mlp1_2 = 200, 80          # din.go:17-18
 
@@ -292,3 +293,39 @@ def GroupAuc32(pred, y, group, engine=None):
     counts over the groups that hold both classes — the metric go-ctr's README quotes (README.md:17, 25, 33)."""
     eng = engine or _e.Engine(_e.default_config(_e.MODEL_YOUTUBE, batch=1, pred_batch=1))
     return eng.group_auc(pred, y, group)[0]
+
+
+def _eval_engine(engine):
+    return engine or _e.Engine(_e.default_config(_e.MODEL_YOUTUBE, batch=1, pred_batch=1))
+
+
+def _column(a):
+    """A vector, or a matrix of one column (the reference's *mat.Dense of one output), as a flat array."""
+    a = np.asarray(a)
+    if a.ndim == 2 and a.shape[1] == 1:
+        return a.ravel()
+    if a.ndim != 1:
+        raise ValueError("expected a vector or one column, got shape %s" % (a.shape,))
+    return a
+
+
+def ROCCurve(Ytrue, Yscore, posLabel, engine=None):
+    """metrics.ROCCurve (nn/metrics/ranking.go:71-103) on the device (ctr_roc_curve): (fpr, tpr, thresholds)."""
+    return _eval_engine(engine).roc_curve(_column(Yscore), _column(Ytrue), posLabel)
+
+
+def PrecisionRecallCurve(Ytrue, ProbasPred, posLabel, engine=None):
+    """metrics.PrecisionRecallCurve (ranking.go:183-209) on the device (ctr_pr_curve): (precision, recall, thresholds)."""
+    return _eval_engine(engine).precision_recall_curve(_column(ProbasPred), _column(Ytrue), posLabel)
+
+
+def AveragePrecisionScore(Ytrue, Yscore, engine=None):
+    """metrics.AveragePrecisionScore (ranking.go:212-222) of a binary target on the device (ctr_average_precision).
+    Labels that are not binary raise CtrError (EINVAL) where the reference prints "unsupported" and returns 0."""
+    return _eval_engine(engine).average_precision(_column(Yscore), _column(Ytrue))
+
+
+def GroupAveragePrecision32(pred, y, group, engine=None):
+    """Mean average precision on the device (ctr_group_average_precision): AveragePrecisionScore per group (normally
+    the UserId), averaged without weights over the groups that hold a positive — MAP, next to GroupAuc32's GAUC."""
+    return _eval_engine(engine).group_average_precision(pred, y, group)[0]

@@ -267,6 +267,87 @@ func (e *Engine) GroupAUC(pred, y []float32, group []int64, perGroup bool) (gauc
 	return float64(g), int64(nu), groups, n, pos, auc, nil
 }
 
+func f64(p []float64) *C.double { return (*C.double)(unsafe.Pointer(&p[0])) }
+
+// curve runs ctr_roc_curve (roc) or ctr_pr_curve with room for n + 1 points and trims the three arrays; the PR curve's
+// last point has no threshold.
+func (e *Engine) curve(roc bool, pred, y []float32, posLabel float64) (a, b, thresholds []float64, err error) {
+	m := len(pred)
+	if m == 0 || len(y) != m {
+		return nil, nil, nil, fmt.Errorf("ctrb200: a curve needs equally long, non-empty pred and y")
+	}
+	a, b, thresholds = make([]float64, m+1), make([]float64, m+1), make([]float64, m+1)
+	var k C.int64_t
+	var rc C.int
+	if roc {
+		rc = C.ctr_roc_curve(e.h, f32(pred), f32(y), C.int64_t(m), C.double(posLabel), f64(a), f64(b), f64(thresholds), C.int64_t(m+1), &k)
+	} else {
+		rc = C.ctr_pr_curve(e.h, f32(pred), f32(y), C.int64_t(m), C.double(posLabel), f64(a), f64(b), f64(thresholds), C.int64_t(m+1), &k)
+	}
+	if err = e.err(rc); err != nil {
+		return nil, nil, nil, err
+	}
+	nt := int(k)
+	if !roc {
+		nt--
+	}
+	return a[:k], b[:k], thresholds[:nt], nil
+}
+
+// ROCCurve is metrics.ROCCurve (nn/metrics/ranking.go:71-103) on the device: one point per distinct score from the
+// highest down, (0, 0) first when the top score holds a negative; a sample is positive when y == posLabel.
+func (e *Engine) ROCCurve(pred, y []float32, posLabel float64) (fpr, tpr, thresholds []float64, err error) {
+	return e.curve(true, pred, y, posLabel)
+}
+
+// PrecisionRecallCurve is metrics.PrecisionRecallCurve (ranking.go:183-209) on the device: recall decreasing to the
+// final (precision 1, recall 0), which has no threshold.
+func (e *Engine) PrecisionRecallCurve(pred, y []float32, posLabel float64) (precision, recall, thresholds []float64, err error) {
+	return e.curve(false, pred, y, posLabel)
+}
+
+// AveragePrecision is metrics.AveragePrecisionScore (ranking.go:212-222) of a binary target on the device, positives
+// y == 1; NaN with no positives.  Labels that are not binary are an error where the reference returns 0.
+func (e *Engine) AveragePrecision(pred, y []float32) (float64, error) {
+	m := len(pred)
+	if m == 0 || len(y) != m {
+		return 0, fmt.Errorf("ctrb200: AveragePrecision needs equally long, non-empty pred and y")
+	}
+	var ap C.double
+	if err := e.err(C.ctr_average_precision(e.h, f32(pred), f32(y), C.int64_t(m), &ap)); err != nil {
+		return 0, err
+	}
+	return float64(ap), nil
+}
+
+// GroupAveragePrecision is the mean average precision (MAP) over groups (normally the sample's UserId): AveragePrecision
+// within each group, averaged without weights over the groups that hold a positive; NaN when none does.  With
+// perGroup, groups holds the distinct ids ascending and n / pos / ap their samples, positives and AP (NaN without a
+// positive), so another weighting is one dot product away.
+func (e *Engine) GroupAveragePrecision(pred, y []float32, group []int64, perGroup bool) (mapScore float64, usedGroups int64, groups []int64, n, pos []int32, ap []float64, err error) {
+	m := len(pred)
+	if m == 0 || len(y) != m || len(group) != m {
+		return 0, 0, nil, nil, nil, nil, fmt.Errorf("ctrb200: GroupAveragePrecision needs equally long, non-empty pred, y and group")
+	}
+	var r C.double
+	var ng, nu C.int64_t
+	var gp *C.int64_t
+	var np, pp *C.int32_t
+	var app *C.double
+	if perGroup {
+		groups, n, pos, ap = make([]int64, m), make([]int32, m), make([]int32, m), make([]float64, m)
+		gp, np, pp, app = i64(groups), i32(n), i32(pos), f64(ap)
+	}
+	if err = e.err(C.ctr_group_average_precision(e.h, f32(pred), f32(y), i64(group), C.int64_t(m), &r, &ng, &nu, gp, np, pp, app)); err != nil {
+		return 0, 0, nil, nil, nil, nil, err
+	}
+	if perGroup {
+		k := int(ng)
+		groups, n, pos, ap = groups[:k], n[:k], pos[:k], ap[:k]
+	}
+	return float64(r), int64(nu), groups, n, pos, ap, nil
+}
+
 // Search is search.Searcher (feature/embedding/search/search.go:66-134) over the ITEM_EMB table on the device: the k
 // rows most cosine-similar to each query. queries holds nq float64 vectors of the table's width (SearchVector; rows,
 // if not nil, names a row to exclude per query, -1 for none), or is nil and rows holds the query rows (SearchInternal,

@@ -313,6 +313,49 @@ int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_
                   double* gauc, int64_t* n_groups, int64_t* n_used,
                   int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc);
 
+/* The curves and average precision of nn/metrics/ranking.go, on the device.  All four follow binaryClfCurve
+ * (ranking.go:13-57): scores ordered as ctr_roc_auc orders them (descending; -0 and +0 one threshold group; every NaN
+ * bit pattern its own group, positive NaNs above +inf, negative NaNs below -inf), one point per threshold group from the
+ * highest score down with the cumulative integer counts tp_j / fp_j, its threshold the group's score widened to double
+ * (+0.0 for the ±0 group, a NaN with its bits).  A sample is positive when (double)y[i] == pos_label.  Every NaN the
+ * calls compute (as opposed to a NaN threshold) is 0x7ff8000000000000.
+ * n in [1, 2^31); h, pred, y and the scalar outputs non-NULL, else CTR_EINVAL.  Host buffers; needs no tables (a
+ * handle created with batch = pred_batch = 1 is enough).  Runs on the engine stream under the handle's mutex.  Not
+ * collective under world > 1: each rank evaluates the samples it passes.  A refusal writes no output except as stated.
+ *
+ * ROCCurve (ranking.go:71-103): when fp_0 != 0 the point (0, 0) comes first with threshold thresholds[0] + 1 (a NaN
+ * threshold stays itself); fpr = fp * (1.0 / fp_max) and tpr = tp * (1.0 / tp_max), each a product, all NaN when
+ * fp_max (resp. tp_max) is 0.  *npoints = the number of points; fpr, tpr and thresholds each receive that many values
+ * and may each be NULL.  A curve of more than cap points is CTR_EINVAL with only *npoints written; cap = n + 1 always
+ * suffices. */
+int ctr_roc_curve(ctr_handle* h, const float* pred, const float* y, int64_t n, double pos_label,
+                  double* fpr, double* tpr, double* thresholds, int64_t cap, int64_t* npoints);
+
+/* PrecisionRecallCurve (ranking.go:183-209): precision_j = tp_j / (tp_j + fp_j), recall_j = tp_j / tp_last (a
+ * division; NaN when tp_last = 0), cut at last_ind = the first j with tp_j >= tp_last, reversed, then precision 1 and
+ * recall 0 appended.  *npoints = last_ind + 2 precision and recall values; thresholds receives last_ind + 1.  With no
+ * positives: precision {0, 1}, recall {NaN, 0}, one threshold.  NULL arrays and cap as in ctr_roc_curve. */
+int ctr_pr_curve(ctr_handle* h, const float* pred, const float* y, int64_t n, double pos_label,
+                 double* precision, double* recall, double* thresholds, int64_t cap, int64_t* npoints);
+
+/* AveragePrecisionScore (ranking.go:212-222) of a binary target, pos_label = 1: the terms
+ * (recall_j - recall_{j-1}) * precision_j for j = 0 … last_ind (recall_{-1} = 0), each computed as in ctr_pr_curve,
+ * summed as a double-double in a fixed order (within 1 ulp of the exactly rounded sum; identical inputs give identical
+ * bits; the reference sums them one by one from the high-recall end).  NaN with no positives.  Labels that are not
+ * binary (some label equal to neither the lowest nor the highest label, or any NaN label; base.go:89-119) are
+ * CTR_EINVAL with *ap untouched, where the reference prints "unsupported" and returns 0. */
+int ctr_average_precision(ctr_handle* h, const float* pred, const float* y, int64_t n, double* ap);
+
+/* Mean average precision over groups (normally the sample's UserId), shaped like ctr_group_auc: groups ordered by
+ * ascending signed int64; AP_g = ctr_average_precision over the group's samples (recall divided by the group's own
+ * positives P_g); a group is used when P_g > 0; *map = the unweighted mean of AP_g over the used groups, a compensated
+ * sum in a fixed order, NaN when no group is used.  The binary-label rule applies to the whole call.  n_groups, n_used
+ * and the out_* arrays may each be NULL; a non-NULL out_* array has room for n entries, and its first *n_groups
+ * entries receive, in ascending group order, the group id, n_g, P_g and AP_g (NaN when P_g = 0). */
+int ctr_group_average_precision(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n,
+                                double* map, int64_t* n_groups, int64_t* n_used,
+                                int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_ap);
+
 /* search.Searcher (feature/embedding/search/search.go:66-134): the k items of ITEM_EMB most cosine-similar to each
  * query, on the device.  queries == NULL: search by row — query i is ITEM_EMB row query_rows[i] widened to float64 and
  * excluded from its own result (SearchInternal, with the word→row map on the caller's side); a row outside [0, rows)
