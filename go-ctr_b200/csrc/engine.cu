@@ -12,6 +12,7 @@
 #include "mlp64.cuh"
 #include "knn.cuh"
 #include "rec.cuh"
+#include "metrics.cuh"
 #include "comm.cuh"
 
 #include <nvtx3/nvToolsExt.h>
@@ -2727,6 +2728,240 @@ int ctr_group_average_precision(ctr_handle* h, const float* pred, const float* y
     return gap_run(h, pred, y, group, (long)n, map, n_groups, n_used, out_group, out_n, out_pos, out_ap);
 }
 
+// ---- nn/metrics classification.go and regression.go (metrics.cuh) -----------------------------------------------
+namespace {
+
+int met_grid(const ctr_handle* h, long work) { return (int)std::max<long>(1, std::min<long>((work + 255) / 256, (long)h->num_sms * 8)); }
+int met_bits(unsigned long long max_key) { return max_key ? 64 - __builtin_clzll(max_key) : 1; }
+constexpr unsigned long long kMetNone = ~0ull;
+
+// The per-class outputs of ctr_precision_recall_fscore (null for ctr_confusion_matrix)
+struct MetPrf { double beta; int average, pos_label; double *p, *r, *f, *support, *per_class; };
+
+// ConfusionMatrix and PrecisionRecallFScoreSupport on the engine stream, one pipeline: the classes of y_true
+// (class_sort_unique), both label vectors encoded and counted (k_met_encode), with weights the sorted segment sums
+// (k_met_seg_*), then the matrix or the scores.  Every refusal comes before any output except *n_classes.
+int met_class_run(ctr_handle* h, const char* what, const double* yt_h, const double* yp_h, const double* w_h, long n,
+                  double* classes_h, double* cm_h, int64_t cap, int32_t* n_classes, const MetPrf* prf) {
+    cudaStream_t st = h->stream;
+    const size_t N = (size_t)n;
+    const int grid = met_grid(h, n);
+    DevBuf<double> yt, yp, w, key0, key1, classes; DevBuf<long> p0, p1, d_count; DevBuf<MetFlags> fl;
+    DevBuf<unsigned char> tmp;
+    CU(h, yt.alloc(N)); CU(h, yp.alloc(N)); if (w_h) CU(h, w.alloc(N));
+    CU(h, key0.alloc(N)); CU(h, key1.alloc(N)); CU(h, p0.alloc(N)); CU(h, p1.alloc(N));
+    CU(h, classes.alloc(N)); CU(h, d_count.alloc(1)); CU(h, fl.alloc(1));
+    size_t bytes = 0;
+    CU(h, class_sort_unique<double>(nullptr, &bytes, nullptr, nullptr, nullptr, nullptr, nullptr, n, st));
+    CU(h, tmp.alloc(bytes));
+    CU(h, cudaMemcpyAsync(yt, yt_h, N * sizeof(double), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(yp, yp_h, N * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (w_h) CU(h, cudaMemcpyAsync(w, w_h, N * sizeof(double), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemsetAsync(fl, 0xff, sizeof(MetFlags), st));
+    RET(launch(h, "met_keys", [&] { k_met_keys<<<grid, 256, 0, st>>>(yt, yp, w, n, key0, p0, fl); }));
+    RET(launch(h, "met_classes", [&] { class_sort_unique<double>(tmp.get(), &bytes, key0.get(), key1.get(), p0.get(), p1.get(), d_count.get(), n, st); }));
+    RET(launch(h, "met_class_values", [&] { k_class_values<double><<<grid, 256, 0, st>>>(yt, p0, d_count, LONG_MAX, classes); }));
+    MetFlags f{}; long C = 0;
+    CU(h, cudaMemcpyAsync(&f, fl, sizeof f, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(&C, d_count, sizeof C, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (f.nan_true != kMetNone) return set_err(h, CTR_EINVAL, "%s: y_true[%llu] is NaN: the classes would be ill-defined", what, f.nan_true);
+    *n_classes = (int32_t)C;
+    if (f.nan_pred != kMetNone) return set_err(h, CTR_EINVAL, "%s: y_pred[%llu] is NaN", what, f.nan_pred);
+    if (f.bad_weight != kMetNone) return set_err(h, CTR_EINVAL, "%s: weight[%llu] = %g is not finite", what, f.bad_weight, w_h[f.bad_weight]);
+    if (prf && prf->pos_label >= C) return set_err(h, CTR_EINVAL, "%s: pos_label %d, but y_true has %ld classes", what, prf->pos_label, C);
+    if (!prf && C * C > cap) return set_err(h, CTR_EINVAL, "%s: %ld classes need %ld cells, cap is %lld", what, C, C * C, (long long)cap);
+    if (prf && prf->per_class && C > cap) return set_err(h, CTR_EINVAL, "%s: %ld classes, cap is %lld", what, C, (long long)cap);
+    // LabelEncoder.Transform of both vectors and the unweighted counts
+    const long cmc = !prf && cm_h ? C * C : 0;
+    DevBuf<unsigned long long> cell, pcls, cm_u, cls_u;
+    CU(h, cell.alloc(N)); CU(h, pcls.alloc(N)); CU(h, cls_u.alloc(3 * (size_t)C));
+    if (cmc) CU(h, cm_u.alloc((size_t)cmc));
+    CU(h, cudaMemsetAsync(cls_u, 0, 3 * (size_t)C * sizeof(unsigned long long), st));
+    if (cmc) CU(h, cudaMemsetAsync(cm_u, 0, (size_t)cmc * sizeof(unsigned long long), st));
+    const bool sh_cls = C <= kMetSmemClasses, sh_cnt = cmc + 3 * C <= kMetSmemCounts;
+    const size_t smem = (sh_cls ? (size_t)C * sizeof(double) : 0) + (sh_cnt ? (size_t)(cmc + 3 * C) * sizeof(unsigned long long) : 0);
+    const int Ci = (int)C;
+    RET(launch(h, "met_encode", [&] {
+        auto k = sh_cls ? (sh_cnt ? k_met_encode<true, true> : k_met_encode<true, false>) : (sh_cnt ? k_met_encode<false, true> : k_met_encode<false, false>);
+        k<<<grid, 256, smem, st>>>(yt, yp, n, classes, Ci, cell, pcls, cm_u, cls_u, fl); }));
+    CU(h, cudaMemcpyAsync(&f, fl, sizeof f, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (f.above != kMetNone)
+        return set_err(h, CTR_EINVAL, "%s: y_pred[%llu] = %g is above the largest class (the reference writes outside the row)", what, f.above, yp_h[f.above]);
+    // weighted sums: (key, weight) sorted, then each segment summed in array order (k_met_seg_*)
+    DevBuf<double> cm_w, tp_w, true_w, pred_w;
+    if (w_h) {
+        DevBuf<unsigned long long> ks; DevBuf<double> ws; DevBuf<double2> piece; DevBuf<long> heads; DevBuf<int> nheads;
+        DevBuf<unsigned char> tmp2;
+        CU(h, ks.alloc(N)); CU(h, ws.alloc(N)); CU(h, piece.alloc(N)); CU(h, heads.alloc(N)); CU(h, nheads.alloc(1));
+        size_t b[2] = {0, 0};
+        CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[0], cell.get(), ks.get(), w.get(), ws.get(), (int)n, 0, 64, st));
+        CU(h, cub::DeviceSelect::If(nullptr, b[1], thrust::counting_iterator<long>(0), heads.get(), nheads.get(), (int)n, MetSegHead{ks.get(), 1}, st));
+        size_t b2 = std::max<size_t>(std::max(b[0], b[1]), 1);
+        CU(h, tmp2.alloc(b2));
+        auto seg = [&](unsigned long long div, double* out, double* diag) -> int {
+            RET(launch(h, "met_seg_piece", [&] { k_met_seg_piece<<<grid, 256, 0, st>>>(ks, div, ws, n, piece); }));
+            RET(launch(h, "met_seg_heads", [&] {
+                cub::DeviceSelect::If(tmp2.get(), b2, thrust::counting_iterator<long>(0), heads.get(), nheads.get(), (int)n, MetSegHead{ks.get(), div}, st); }));
+            return launch(h, "met_seg_total", [&] { k_met_seg_total<<<grid, 256, 0, st>>>(ks, div, heads, nheads, n, piece, Ci, out, diag); });
+        };
+        RET(launch(h, "met_sort_cells", [&] {
+            cub::DeviceRadixSort::SortPairs(tmp2.get(), b2, cell.get(), ks.get(), w.get(), ws.get(), (int)n, 0, met_bits((unsigned long long)C * C - 1), st); }));
+        if (cmc) {
+            CU(h, cm_w.alloc((size_t)cmc)); CU(h, cudaMemsetAsync(cm_w, 0, (size_t)cmc * sizeof(double), st));
+            RET(seg(1, cm_w, nullptr));
+        }
+        if (prf) {
+            CU(h, tp_w.alloc((size_t)C)); CU(h, true_w.alloc((size_t)C)); CU(h, pred_w.alloc((size_t)C));
+            for (double* a : {tp_w.get(), true_w.get(), pred_w.get()}) CU(h, cudaMemsetAsync(a, 0, (size_t)C * sizeof(double), st));
+            RET(seg(1, nullptr, tp_w));
+            RET(seg((unsigned long long)C, true_w, nullptr));
+            RET(launch(h, "met_sort_cols", [&] {
+                cub::DeviceRadixSort::SortPairs(tmp2.get(), b2, pcls.get(), ks.get(), w.get(), ws.get(), (int)n, 0, met_bits((unsigned long long)C - 1), st); }));
+            RET(seg(1, pred_w, nullptr));
+        }
+    }
+    double r4[4] = {0, 0, 0, 0};
+    DevBuf<double> out4, pc;
+    if (!prf) {
+        if (cmc && !w_h) {
+            CU(h, cm_w.alloc((size_t)cmc));
+            RET(launch(h, "met_cm", [&] { k_met_cm_f64<<<met_grid(h, cmc), 256, 0, st>>>(cm_u, cmc, cm_w); }));
+        }
+        if (cmc) CU(h, cudaMemcpyAsync(cm_h, cm_w, (size_t)cmc * sizeof(double), cudaMemcpyDeviceToHost, st));
+    } else {
+        CU(h, out4.alloc(4));
+        if (prf->per_class) CU(h, pc.alloc(4 * (size_t)C));
+        RET(launch(h, "met_prf", [&] {
+            k_met_prf<<<1, 256, 0, st>>>(cls_u, tp_w, true_w, pred_w, Ci, prf->beta, prf->pos_label, prf->average, pc, out4); }));
+        CU(h, cudaMemcpyAsync(r4, out4, sizeof r4, cudaMemcpyDeviceToHost, st));
+        if (prf->per_class) CU(h, cudaMemcpyAsync(prf->per_class, pc, 4 * (size_t)C * sizeof(double), cudaMemcpyDeviceToHost, st));
+    }
+    if (classes_h) CU(h, cudaMemcpyAsync(classes_h, classes, (size_t)C * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (prf) {
+        if (prf->p) *prf->p = r4[0];
+        if (prf->r) *prf->r = r4[1];
+        if (prf->f) *prf->f = r4[2];
+        if (prf->support) *prf->support = r4[3];
+    }
+    return CTR_OK;
+}
+
+// R2Score (kind < 0) or MeanSquaredError / MeanAbsoluteError on the engine stream: k_mlp64_r2_part / k_mlp64_r2_fold
+// over the [n, no] host matrices; out receives no values (RAW) or one
+int met_regression_run(ctr_handle* h, const double* yt_h, const double* yp_h, const double* w_h, long n, int no, int kind,
+                       int multioutput, double* out_h) {
+    cudaStream_t st = h->stream;
+    const size_t NN = (size_t)n * (size_t)no;
+    DevBuf<double> yt, yp, w, mean, r, res; DevBuf<double2> part;
+    CU(h, yt.alloc(NN)); CU(h, yp.alloc(NN)); if (w_h) CU(h, w.alloc((size_t)n));
+    CU(h, mean.alloc((size_t)no)); CU(h, r.alloc(2 * (size_t)no)); CU(h, res.alloc(3)); CU(h, part.alloc((size_t)no * kR2Parts));
+    CU(h, cudaMemcpyAsync(yt, yt_h, NN * sizeof(double), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(yp, yp_h, NN * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (w_h) CU(h, cudaMemcpyAsync(w, w_h, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+    const dim3 g(kR2Parts, no);
+    const double* raw = mean;
+    if (kind < 0) {
+        RET(launch(h, "r2_mean", [&] { k_mlp64_r2_part<double><<<g, 256, 0, st>>>(nullptr, yt, w, n, no, kR2Mean, nullptr, part); }));
+        RET(launch(h, "r2_mean_fold", [&] { k_mlp64_r2_fold<<<1, 256, 0, st>>>(part, no, 0.0, mean, nullptr, nullptr); }));
+        RET(launch(h, "r2_sums", [&] { k_mlp64_r2_part<double><<<g, 256, 0, st>>>(yp, yt, w, n, no, kR2Sums, mean, part); }));
+        RET(launch(h, "r2_fold", [&] { k_mlp64_r2_fold<<<1, 256, 0, st>>>(part, no, 1e-20, mean, r, res); }));
+        raw = r;
+    } else {
+        const int k = kind == CTR_ERROR_SQUARED ? kErrSquared : kErrAbsolute;
+        RET(launch(h, "err_sums", [&] { k_mlp64_r2_part<double><<<g, 256, 0, st>>>(yp, yt, nullptr, n, no, k, nullptr, part); }));
+        RET(launch(h, "err_fold", [&] { k_mlp64_r2_fold<<<1, 256, 0, st>>>(part, no, 0.0, mean, nullptr, res); }));
+    }
+    if (multioutput == CTR_MULTIOUTPUT_RAW) CU(h, cudaMemcpyAsync(out_h, raw, (size_t)no * sizeof(double), cudaMemcpyDeviceToHost, st));
+    else CU(h, cudaMemcpyAsync(out_h, res.get() + (multioutput == CTR_MULTIOUTPUT_UNIFORM ? 0 : 2), sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+
+}  // namespace
+
+// The arguments are checked before the handle, so each refusal's message is readable through ctr_last_error(h), or
+// ctr_last_error(NULL) when h is null.
+int ctr_accuracy_score(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, const double* weight,
+                       int32_t normalize, double* score) {
+    if (!y_true || !y_pred || !score || n < 1 || n > 0x7fffffff || n_out < 1 || n_out > 1024)
+        return set_err(h, CTR_EINVAL, "bad accuracy arguments (n in [1, 2^31), n_out in [1, 1024]; y_true, y_pred and score non-null)");
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const size_t NN = (size_t)n * (size_t)n_out;
+    DevBuf<double> yt, yp, w, out; DevBuf<MetAccPart> part;
+    CU(h, yt.alloc(NN)); CU(h, yp.alloc(NN)); if (weight) CU(h, w.alloc((size_t)n));
+    CU(h, out.alloc(2)); CU(h, part.alloc(kMetParts));
+    CU(h, cudaMemcpyAsync(yt, y_true, NN * sizeof(double), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(yp, y_pred, NN * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (weight) CU(h, cudaMemcpyAsync(w, weight, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+    RET(launch(h, "acc_part", [&] { k_met_acc_part<<<kMetParts, 256, 0, st>>>(yt, yp, w, (long)n, n_out, part); }));
+    RET(launch(h, "acc_final", [&] { k_met_acc_final<<<1, 256, 0, st>>>(part, (long)n, weight != nullptr, normalize, out); }));
+    double r[2] = {0, 0};
+    CU(h, cudaMemcpyAsync(r, out, sizeof r, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (r[1] != 0.0) return set_err(h, CTR_EINVAL, "accuracy: a weight is NaN or infinite");
+    *score = r[0];
+    return CTR_OK;
+}
+
+int ctr_confusion_matrix(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, const double* weight, double* classes,
+                         double* cm, int64_t cap, int32_t* n_classes) {
+    if (!y_true || !y_pred || !n_classes || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad confusion matrix arguments (n in [1, 2^31); y_true, y_pred and n_classes non-null)");
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return met_class_run(h, "confusion matrix", y_true, y_pred, weight, (long)n, classes, cm, cap, n_classes, nullptr);
+}
+
+int ctr_precision_recall_fscore(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, const double* weight, double beta,
+                                int32_t average, int32_t pos_label, double* p, double* r, double* f, double* support,
+                                double* per_class, int64_t cap, int32_t* n_classes) {
+    if (!y_true || !y_pred || !n_classes || n < 1 || n > 0x7fffffff)
+        return set_err(h, CTR_EINVAL, "bad precision/recall arguments (n in [1, 2^31); y_true, y_pred and n_classes non-null)");
+    if (average != CTR_AVERAGE_MACRO && average != CTR_AVERAGE_MICRO && average != CTR_AVERAGE_WEIGHTED)
+        return set_err(h, CTR_EINVAL, "average %d: macro (%d), micro (%d) or weighted (%d)", average, CTR_AVERAGE_MACRO, CTR_AVERAGE_MICRO, CTR_AVERAGE_WEIGHTED);
+    if (!std::isfinite(beta)) return set_err(h, CTR_EINVAL, "beta %g must be finite", beta);
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    const MetPrf prf{beta, average, pos_label < 0 ? -1 : pos_label, p, r, f, support, per_class};
+    return met_class_run(h, "precision/recall", y_true, y_pred, weight, (long)n, nullptr, nullptr, cap, n_classes, &prf);
+}
+
+int ctr_r2_score(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, const double* weight,
+                 int32_t multioutput, double* out) {
+    if (!y_true || !y_pred || !out || n < 1 || n > 0x7fffffff || n_out < 1 || n_out > 1024)
+        return set_err(h, CTR_EINVAL, "bad r2 arguments (n in [1, 2^31), n_out in [1, 1024]; y_true, y_pred and out non-null)");
+    if (multioutput != CTR_MULTIOUTPUT_RAW && multioutput != CTR_MULTIOUTPUT_UNIFORM && multioutput != CTR_MULTIOUTPUT_VARIANCE_WEIGHTED)
+        return set_err(h, CTR_EINVAL, "multioutput %d: raw (%d), uniform (%d) or variance weighted (%d)", multioutput,
+                       CTR_MULTIOUTPUT_RAW, CTR_MULTIOUTPUT_UNIFORM, CTR_MULTIOUTPUT_VARIANCE_WEIGHTED);
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return met_regression_run(h, y_true, y_pred, weight, (long)n, n_out, -1, multioutput, out);
+}
+
+int ctr_mean_error(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, int32_t kind,
+                   int32_t multioutput, double* out) {
+    if (!y_true || !y_pred || !out || n < 1 || n > 0x7fffffff || n_out < 1 || n_out > 1024)
+        return set_err(h, CTR_EINVAL, "bad mean error arguments (n in [1, 2^31), n_out in [1, 1024]; y_true, y_pred and out non-null)");
+    if (kind != CTR_ERROR_SQUARED && kind != CTR_ERROR_ABSOLUTE)
+        return set_err(h, CTR_EINVAL, "kind %d: squared (%d) or absolute (%d)", kind, CTR_ERROR_SQUARED, CTR_ERROR_ABSOLUTE);
+    if (multioutput != CTR_MULTIOUTPUT_RAW && multioutput != CTR_MULTIOUTPUT_UNIFORM)
+        return set_err(h, CTR_EINVAL, "multioutput %d: raw (%d) or uniform (%d); the mean errors have no variance weighting", multioutput,
+                       CTR_MULTIOUTPUT_RAW, CTR_MULTIOUTPUT_UNIFORM);
+    if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    return met_regression_run(h, y_true, y_pred, nullptr, (long)n, n_out, kind, multioutput, out);
+}
+
 int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_rows, int64_t nq, int32_t k,
                    int32_t* out_rows, double* out_sim, int32_t* out_count) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
@@ -3741,18 +3976,16 @@ int mlp_set_head(ctr_mlp* m, const std::vector<double>& classes) {
 // (m->cls), else null.  The host reads the class count back once.  A refusal changes nothing.
 int mlp_labels(ctr_mlp* m, const float* Y, long n, const int** cls) {
     *cls = nullptr;
-    size_t t_sort = 0, t_uniq = 0;
-    MCU(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (const float*)nullptr, (float*)nullptr, (const long*)nullptr, (long*)nullptr, n, 0, 32, m->stream));
-    MCU(m, cub::DeviceSelect::UniqueByKey(nullptr, t_uniq, (const float*)nullptr, (const long*)nullptr, (float*)nullptr, (long*)nullptr, (long*)nullptr, n, m->stream));
+    size_t t_tmp = 0;
+    MCU(m, class_sort_unique<float>(nullptr, &t_tmp, nullptr, nullptr, nullptr, nullptr, nullptr, n, m->stream));
     DevBuf<float> k0, k1; DevBuf<long> p0, p1; DevBuf<char> tmp; DevBuf<Mlp64Classes> res;
     MCU(m, k0.alloc((size_t)n)); MCU(m, k1.alloc((size_t)n)); MCU(m, p0.alloc((size_t)n)); MCU(m, p1.alloc((size_t)n));
-    MCU(m, tmp.alloc(std::max(t_sort, t_uniq))); MCU(m, res.alloc(1));
+    MCU(m, tmp.alloc(t_tmp)); MCU(m, res.alloc(1));
     MCU(m, cudaMemsetAsync(res, 0, sizeof(Mlp64Classes), m->stream));
     k_mlp64_label_keys<<<mlp_grid(m, n), 256, 0, m->stream>>>(Y, n, k0, p0, res);
-    MCU(m, cub::DeviceRadixSort::SortPairs(tmp.get(), t_sort, k0.get(), k1.get(), p0.get(), p1.get(), n, 0, 32, m->stream));
     // the stable sort leaves each class's first position at the head of its run; the unique keys go to k0, their positions to p0
-    MCU(m, cub::DeviceSelect::UniqueByKey(tmp.get(), t_uniq, k1.get(), p1.get(), k0.get(), p0.get(), &res.get()->count, n, m->stream));
-    k_mlp64_class_values<<<kMlpMaxClasses / 256, 256, 0, m->stream>>>(Y, p0, res);
+    MCU(m, class_sort_unique<float>(tmp.get(), &t_tmp, k0.get(), k1.get(), p0.get(), p1.get(), &res.get()->count, n, m->stream));
+    k_class_values<float><<<kMlpMaxClasses / 256, 256, 0, m->stream>>>(Y, p0, &res.get()->count, kMlpMaxClasses, res.get()->value);
     std::unique_ptr<Mlp64Classes> r(new Mlp64Classes);
     MCU(m, cudaMemcpyAsync(r.get(), res, sizeof(Mlp64Classes), cudaMemcpyDeviceToHost, m->stream));
     MCU(m, cudaStreamSynchronize(m->stream));
@@ -4107,7 +4340,7 @@ int ctr_mlp_predict_f64(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, do
 int ctr_mlp_score(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* r2) {
     if (!m || !X || !Y || !r2 || n < 1) return mlp_err(m, CTR_EINVAL, "bad score arguments");
     std::lock_guard<std::mutex> lk(m->mu);
-    if (!m->regressor) return mlp_err(m, CTR_ESTATE, "score is the regressor's R²; a classifier's accuracy score is not built");
+    if (!m->regressor) return mlp_err(m, CTR_ESTATE, "score is the regressor's R²; a classifier's accuracy score is ctr_mlp_accuracy");
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "score before fit");
     if (xcols != m->d.units[0]) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, m->d.units[0]);
     MCU(m, cudaSetDevice(m->dev));
@@ -4115,19 +4348,48 @@ int ctr_mlp_score(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t
     const size_t ny = (size_t)n * no;
     DevBuf<double> pred, mean, r, res; DevBuf<float> y; DevBuf<double2> part;
     MCU(m, pred.alloc(ny)); MCU(m, y.alloc(ny)); MCU(m, part.alloc((size_t)no * kR2Parts));
-    MCU(m, mean.alloc((size_t)no)); MCU(m, r.alloc(2 * (size_t)no)); MCU(m, res.alloc(2));
+    MCU(m, mean.alloc((size_t)no)); MCU(m, r.alloc(2 * (size_t)no)); MCU(m, res.alloc(3));
     MCU(m, cudaMemcpyAsync(y, Y, sizeof(float) * ny, cudaMemcpyHostToDevice, m->stream));
     RET(mlp_output64(m, X, n, pred));                                     // MLPRegressor.Score → Predict (:64-70)
-    k_mlp64_r2_part<<<dim3(kR2Parts, no), 256, 0, m->stream>>>(nullptr, y, (long)n, no, nullptr, part);
-    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, (long)n, no, mean, nullptr, nullptr);
-    k_mlp64_r2_part<<<dim3(kR2Parts, no), 256, 0, m->stream>>>(pred, y, (long)n, no, mean, part);
-    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, (long)n, no, mean, r, res);
+    k_mlp64_r2_part<float><<<dim3(kR2Parts, no), 256, 0, m->stream>>>(nullptr, y, nullptr, (long)n, no, kR2Mean, nullptr, part);
+    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, no, 0.0, mean, nullptr, nullptr);
+    k_mlp64_r2_part<float><<<dim3(kR2Parts, no), 256, 0, m->stream>>>(pred, y, nullptr, (long)n, no, kR2Sums, mean, part);
+    k_mlp64_r2_fold<<<1, 256, 0, m->stream>>>(part, no, 0.0, mean, r, res);
     double h[2] = {0, 0};
     MCU(m, cudaMemcpyAsync(h, res, sizeof h, cudaMemcpyDeviceToHost, m->stream));
     MCU(m, cudaStreamSynchronize(m->stream));
     MCU(m, cudaGetLastError());
     if (h[1] >= 0.0) return mlp_err(m, CTR_EINVAL, "target column %d is constant: R² divides by 0 (the reference panics)", (int)h[1]);
     *r2 = h[0];
+    return CTR_OK;
+}
+
+int ctr_mlp_accuracy(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* acc) {
+    if (!m || !X || !Y || !acc || n < 1) return mlp_err(m, CTR_EINVAL, "bad accuracy arguments");
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->regressor) return mlp_err(m, CTR_ESTATE, "a regressor's score is R² (ctr_mlp_score)");
+    if (!m->fitted) return mlp_err(m, CTR_ESTATE, "accuracy before fit");
+    const int L = m->d.n_layers, nin = m->d.units[0], no = m->d.units[L - 1];
+    if (xcols != nin) return mlp_err(m, CTR_EINVAL, "X has %d columns, the network %d inputs", xcols, nin);
+    MCU(m, cudaSetDevice(m->dev));
+    RET(mlp_upload_x(m, X, n, nin));
+    DevBuf<float> y; DevBuf<unsigned long long> hits;
+    MCU(m, y.alloc((size_t)n)); MCU(m, hits.alloc(1));
+    MCU(m, cudaMemcpyAsync(y, Y, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
+    MCU(m, cudaMemsetAsync(hits, 0, sizeof(unsigned long long), m->stream));
+    const long chunk = 8192;
+    RET(mlp_rows(m, std::min<long>(chunk, n)));
+    const double* cls = m->classes.empty() ? nullptr : m->class_dev.get();
+    for (long r0 = 0; r0 < n; r0 += chunk) {                             // Score → Predict (:127-133), in chunks as ctr_mlp_predict
+        const int rows = (int)std::min<long>(chunk, n - r0);
+        mlp_forward(m, m->X64 + r0 * nin, nullptr, rows);
+        k_mlp64_acc_count<<<mlp_grid(m, rows), 256, 0, m->stream>>>(m->act[L - 1], rows, no, cls, y + r0, hits);
+    }
+    unsigned long long c = 0;
+    MCU(m, cudaMemcpyAsync(&c, hits, sizeof c, cudaMemcpyDeviceToHost, m->stream));
+    MCU(m, cudaStreamSynchronize(m->stream));
+    MCU(m, cudaGetLastError());
+    *acc = (double)c / (double)n;                                         // AccuracyScore64 :1143-1155
     return CTR_OK;
 }
 

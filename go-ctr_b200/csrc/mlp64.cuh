@@ -249,22 +249,17 @@ k_mlp64_label_keys(const float* __restrict__ Y, long n, float* __restrict__ key,
         pos[i] = i;
     }
 }
-// discovery pass 3, after a stable sort by key and UniqueByKey: first[c] is the first position of class c in sample
-// order, so the class keeps the sign of its first occurrence (the map of :1303-1309 keeps the first value it meets)
-__global__ void __launch_bounds__(256)
-k_mlp64_class_values(const float* __restrict__ Y, const long* __restrict__ first, Mlp64Classes* __restrict__ res) {
-    const long c_n = res->count < kMlpMaxClasses ? res->count : kMlpMaxClasses;
-    for (long c = blockIdx.x * (long)blockDim.x + threadIdx.x; c < c_n; c += (long)gridDim.x * blockDim.x) res->value[c] = (double)Y[first[c]];
+// discovery pass 2 is class_sort_unique and pass 3 k_class_values (metrics.cuh), shared with ctr_confusion_matrix.
+// sort.SearchFloat64s (label.go:330): the first class >= y, C when y is above every class (or NaN)
+__device__ __forceinline__ int class_lower_bound(const double* __restrict__ classes, int C, double y) {
+    int lo = 0, hi = C;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (classes[mid] < y) lo = mid + 1; else hi = mid; }
+    return lo;
 }
 // cls[i] = the index of label i in classes[0, C) (ascending, every label present; ±0 compare equal)
 __global__ void __launch_bounds__(256)
 k_mlp64_class_index(const float* __restrict__ Y, long n, const double* __restrict__ classes, int C, int* __restrict__ cls) {
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-        const double y = (double)Y[i];
-        int lo = 0, hi = C;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (classes[mid] < y) lo = mid + 1; else hi = mid; }
-        cls[i] = lo;
-    }
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) cls[i] = class_lower_bound(classes, C, (double)Y[i]);
 }
 
 // softmax of each row of the output layer's pre-activations, in place (:104-117): exp of every column, their sum in
@@ -361,21 +356,36 @@ k_mlp64_loss_dense(const double* __restrict__ params, Mlp64Dims d, const double*
 
 // r2Score64 (basemlp64.go:1116-1141) over pred [n, no] and Y [n, no] in two passes, each a fixed partition of the rows
 // into kR2Parts contiguous ranges per column (block (p, c)), a fixed tree inside the block, and the parts folded in
-// order by one thread per column: the same bits on every run.
+// order by one thread per column: the same bits on every run.  The same column sums serve R2Score, MeanSquaredError
+// and MeanAbsoluteError (nn/metrics/regression.go, ctr_r2_score / ctr_mean_error): optional sample weights w [n]
+// (null: every weight 1, and the sums are those of the unweighted form bit for bit), float or double targets.
 constexpr int kR2Parts = 256;
-// mean == nullptr: part[c][p] = Σ y over part p of column c.  Else part[c][p] = {Σ (pred − y)², Σ (y − mean[c])²}.
+enum : int {
+    kR2Mean = 0,      // part[c][p] = {Σ w·y, Σ w}
+    kR2Sums = 1,      // part[c][p] = {Σ w·(pred − y)², Σ w·(y − mean[c])²}
+    kErrSquared = 2,  // part[c][p] = {Σ (pred − y)², rows}
+    kErrAbsolute = 3  // part[c][p] = {Σ |pred − y|, rows}
+};
+template <class TY>
 __global__ void __launch_bounds__(256)
-k_mlp64_r2_part(const double* __restrict__ pred, const float* __restrict__ Y, long n, int no, const double* __restrict__ mean, double2* __restrict__ part) {
+k_mlp64_r2_part(const double* __restrict__ pred, const TY* __restrict__ Y, const double* __restrict__ w, long n, int no, int kind,
+                const double* __restrict__ mean, double2* __restrict__ part) {
     __shared__ double2 red[256];
     const int p = blockIdx.x, c = blockIdx.y;
     const long per = (n + kR2Parts - 1) / kR2Parts, r0 = p * per, r1 = min(n, r0 + per);
     double a = 0.0, b = 0.0;
     for (long r = r0 + threadIdx.x; r < r1; r += 256) {
         const double y = (double)Y[r * no + c];
-        if (!mean) { a += y; continue; }
-        const double t = pred[r * no + c] - y, u = y - mean[c];
-        a += t * t;
-        b += u * u;
+        if (kind == kR2Mean) {
+            if (!w) { a += y; b += 1.0; } else { a += w[r] * y; b += w[r]; }
+            continue;
+        }
+        const double t = pred[r * no + c] - y;
+        if (kind == kErrSquared) { a += t * t; b += 1.0; continue; }
+        if (kind == kErrAbsolute) { a += fabs(t); b += 1.0; continue; }
+        const double u = y - mean[c];
+        if (!w) { a += t * t; b += u * u; }
+        else { a += w[r] * (t * t); b += w[r] * (u * u); }
     }
     red[threadIdx.x] = make_double2(a, b); __syncthreads();
     for (int o = 128; o > 0; o >>= 1) {
@@ -384,27 +394,38 @@ k_mlp64_r2_part(const double* __restrict__ pred, const float* __restrict__ Y, lo
     }
     if (threadIdx.x == 0) part[(long)c * kR2Parts + p] = red[0];
 }
-// pass 1 (r2 == nullptr): mean[c] = Σ y / rows.  Pass 2: r2[c] = 1 − num/den and r2[no + c] = den; out[0] = the mean
-// of the columns' r2 in column order, out[1] = the first column whose den is 0 (the reference panics there), or −1.
-// One block.
+// Pass 1 (r2 == nullptr; kR2Mean or an error kind): mean[c] = a / b, the weighted column mean or the mean error, and
+// when out is non-null out[0] = the mean of the columns' values in column order.  Pass 2 (kR2Sums): r2[c] = 1 − num /
+// max(den, floor) (floor 0 for r2Score64, 1e-20 for R2Score, regression.go:112; a NaN den stays NaN, as Go's math.Max)
+// and r2[no + c] = den; out[0] = the mean of the columns' r2 in column order, out[1] = the first column whose den is 0
+// (r2Score64 panics there), or −1, out[2] = Σ den·r2 · (1 / Σ den) (R2Score's variance_weighted, :118-123).  One block.
 __global__ void __launch_bounds__(256)
-k_mlp64_r2_fold(const double2* __restrict__ part, long n, int no, double* __restrict__ mean, double* __restrict__ r2, double* __restrict__ out) {
+k_mlp64_r2_fold(const double2* __restrict__ part, int no, double floor, double* __restrict__ mean, double* __restrict__ r2, double* __restrict__ out) {
     for (int c = threadIdx.x; c < no; c += blockDim.x) {
         double a = 0.0, b = 0.0;
         for (int p = 0; p < kR2Parts; p++) { a += part[(long)c * kR2Parts + p].x; b += part[(long)c * kR2Parts + p].y; }
-        if (!r2) mean[c] = a / (double)n;
-        else { r2[c] = 1.0 - a / b; r2[no + c] = b; }
+        if (!r2) mean[c] = a / b;
+        else { r2[c] = 1.0 - a / (b < floor ? floor : b); r2[no + c] = b; }
     }
-    if (!r2) return;
+    if (!out) return;
     __syncthreads();
     if (threadIdx.x == 0) {
-        double acc = 0.0, bad = -1.0;
+        if (!r2) {
+            double acc = 0.0;
+            for (int c = 0; c < no; c++) acc += mean[c];
+            out[0] = acc / (double)no;
+            return;
+        }
+        double acc = 0.0, bad = -1.0, dot = 0.0, sden = 0.0;
         for (int c = 0; c < no; c++) {
             if (bad < 0.0 && r2[no + c] == 0.0) bad = (double)c;
             acc += r2[c];
+            dot += r2[no + c] * r2[c];
+            sden += r2[no + c];
         }
         out[0] = acc / (double)no;
         out[1] = bad;
+        out[2] = dot * (1.0 / sden);
     }
 }
 

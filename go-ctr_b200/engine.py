@@ -12,7 +12,7 @@ from . import build as _build
 __all__ = ["Engine", "Config", "MLPClassifier", "MLPRegressor", "MlpConfig", "MlpOptions", "StepStats", "CtrError", "load_library", "MODEL_YOUTUBE", "MODEL_DIN_COS",
            "MODEL_DIN_EUC", "TABLE_USER_FEAT", "TABLE_ITEM_FEAT", "TABLE_ITEM_EMB", "TABLE_FROZEN", "TABLE_SGD",
            "TABLE_SGD_DETERMINISTIC", "TABLE_ADAM", "GEMM_AUTO", "GEMM_FP32", "GEMM_TCGEN05_3XTF32", "EXPORTS", "IDMAP_USER", "IDMAP_ITEM", "ENOTFOUND", "EINVAL", "ESTATE", "rank_metrics",
-           "EXCLUDE_NONE", "EXCLUDE_WINDOW", "EXCLUDE_SEEN"]
+           "EXCLUDE_NONE", "EXCLUDE_WINDOW", "EXCLUDE_SEEN", "AVERAGE", "MULTIOUTPUT", "ERROR_KIND"]
 
 MODEL_YOUTUBE, MODEL_DIN_COS, MODEL_DIN_EUC = 0, 1, 2
 TABLE_USER_FEAT, TABLE_ITEM_FEAT, TABLE_ITEM_EMB = 0, 1, 2
@@ -21,6 +21,9 @@ GEMM_AUTO, GEMM_FP32, GEMM_TCGEN05_3XTF32 = 0, 1, 2
 IDMAP_USER, IDMAP_ITEM = 0, 1
 EINVAL, ESTATE, ENOTFOUND = 1, 5, 7
 EXCLUDE_NONE, EXCLUDE_WINDOW, EXCLUDE_SEEN = 0, 1, 2
+AVERAGE = {"macro": 0, "micro": 1, "weighted": 2}                                 # CTR_AVERAGE_*
+MULTIOUTPUT = {"raw_values": 0, "uniform_average": 1, "variance_weighted": 2}      # CTR_MULTIOUTPUT_*
+ERROR_KIND = {"squared": 0, "absolute": 1}                                        # CTR_ERROR_*
 
 # every symbol include/ctr_b200.h declares (tests check the .so exports all of them)
 EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy", "ctr_last_error",
@@ -30,11 +33,11 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
            "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
-           "ctr_mlp_score", "ctr_mlp_get_output", "ctr_mlp_set_output"]
+           "ctr_mlp_score", "ctr_mlp_accuracy", "ctr_mlp_get_output", "ctr_mlp_set_output"]
 
 
 def _exclusion(n, max_ts, exclude_history, exclude_seen):
@@ -118,6 +121,44 @@ def load_library():
 def _f(a):
     a = np.ascontiguousarray(a, dtype=np.float32)
     return a, a.ctypes.data_as(_fp)
+
+
+_dp = C.POINTER(C.c_double)
+
+
+def _d(a):
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    return a, a.ctypes.data_as(_dp)
+
+
+def _targets(y_true, y_pred):
+    """(y_true, y_pred) as float64 [n, n_out] arrays of the same shape; a vector is one column"""
+    t = np.asarray(y_true, np.float64); p = np.asarray(y_pred, np.float64)
+    if t.shape != p.shape:
+        raise ValueError("y_true and y_pred differ in shape: %s, %s" % (t.shape, p.shape))
+    if t.ndim == 1:
+        t, p = t[:, None], p[:, None]
+    if t.ndim != 2:
+        raise ValueError("expected [n] or [n, n_out] targets, got shape %s" % (t.shape,))
+    return np.ascontiguousarray(t), np.ascontiguousarray(p)
+
+
+def _weights(weight, n):
+    if weight is None:
+        return None, None
+    w = np.ascontiguousarray(weight, np.float64).reshape(-1)
+    if w.size != n:
+        raise ValueError("weight has %d entries for %d samples" % (w.size, n))
+    return w, w.ctypes.data_as(_dp)
+
+
+def _mode(table, v, what):
+    """a mode given by name (the reference's strings) or as the C enum's integer, which is passed through"""
+    if isinstance(v, str):
+        if v not in table:
+            raise ValueError("%s must be one of %s, got %r" % (what, sorted(table), v))
+        return table[v]
+    return int(v)
 
 
 def _i(a):
@@ -527,6 +568,75 @@ class Engine:
             return m.value, ng.value, nu.value
         return m.value, ng.value, nu.value, {k: v[:ng.value].copy() for k, v in outs.items()}
 
+    def accuracy_score(self, y_true, y_pred, normalize=True, weight=None):
+        """AccuracyScore (ctr_accuracy_score): the weight of the rows whose every column is equal (==) over all the
+        weight, or that weight itself with normalize=False.  y_true / y_pred: [n] or [n, n_out]; weight: [n] or None."""
+        t, p = _targets(y_true, y_pred)
+        w, wp = _weights(weight, t.shape[0])
+        out = C.c_double(0)
+        self._ck(self.L.ctr_accuracy_score(self.h, t.ctypes.data_as(_dp), p.ctypes.data_as(_dp), C.c_int64(t.shape[0]),
+                                           C.c_int32(t.shape[1]), wp, C.c_int32(int(bool(normalize))), C.byref(out)))
+        return out.value
+
+    def _class_labels(self, y_true, y_pred):
+        t = np.ascontiguousarray(y_true, np.float64).reshape(-1); p = np.ascontiguousarray(y_pred, np.float64).reshape(-1)
+        if t.size != p.size:
+            raise ValueError("y_true and y_pred differ in length: %d, %d" % (t.size, p.size))
+        return t, p
+
+    def confusion_matrix(self, y_true, y_pred, weight=None):
+        """ConfusionMatrix (ctr_confusion_matrix) of 1-D labels: (classes [C] float64 ascending, cm [C, C] float64),
+        cm[r, c] the weight (or count) of true class r predicted as c; a prediction between two classes counts as the
+        higher one.  Runs the pipeline twice: once for C, once for the matrix."""
+        t, p = self._class_labels(y_true, y_pred)
+        w, wp = _weights(weight, t.size)
+        nc = C.c_int32(0)
+        classes = np.empty(t.size, np.float64)
+        args = (self.h, t.ctypes.data_as(_dp), p.ctypes.data_as(_dp), C.c_int64(t.size), wp)
+        self._ck(self.L.ctr_confusion_matrix(*args, classes.ctypes.data_as(_dp), None, C.c_int64(t.size * t.size), C.byref(nc)))
+        cm = np.empty((nc.value, nc.value), np.float64)
+        self._ck(self.L.ctr_confusion_matrix(*args, None, cm.ctypes.data_as(_dp), C.c_int64(cm.size), C.byref(nc)))
+        return classes[:nc.value].copy(), cm
+
+    def precision_recall_fscore(self, y_true, y_pred, beta=1.0, average="macro", pos_label=-1, weight=None, per_class=False):
+        """PrecisionRecallFScoreSupport (ctr_precision_recall_fscore): (precision, recall, fscore, support) of the class
+        index pos_label, or with pos_label < 0 their average ("macro", "micro" or "weighted", which equals "macro" as in
+        the reference; support 0).  per_class=True also returns the [C, 4] rows (p, r, f, support) of every class."""
+        t, p = self._class_labels(y_true, y_pred)
+        w, wp = _weights(weight, t.size)
+        avg = _mode(AVERAGE, average, "average")
+        nc = C.c_int32(0)
+        o = [C.c_double(0) for _ in range(4)]
+        pc = np.empty((t.size, 4), np.float64) if per_class else None
+        self._ck(self.L.ctr_precision_recall_fscore(self.h, t.ctypes.data_as(_dp), p.ctypes.data_as(_dp), C.c_int64(t.size), wp,
+                                                    C.c_double(beta), C.c_int32(avg), C.c_int32(pos_label),
+                                                    *[C.byref(x) for x in o], pc.ctypes.data_as(_dp) if per_class else None,
+                                                    C.c_int64(t.size), C.byref(nc)))
+        res = tuple(x.value for x in o)
+        return res + (pc[:nc.value].copy(),) if per_class else res
+
+    def r2_score(self, y_true, y_pred, weight=None, multioutput="uniform_average"):
+        """R2Score (ctr_r2_score): "raw_values" gives the [n_out] scores, "uniform_average" (or "") their mean,
+        "variance_weighted" their mean weighted by each column's weighted variance.  weight: [n] or None."""
+        t, p = _targets(y_true, y_pred)
+        w, wp = _weights(weight, t.shape[0])
+        mode = _mode(MULTIOUTPUT, "uniform_average" if multioutput == "" else multioutput, "multioutput")
+        out = np.empty(t.shape[1], np.float64)
+        self._ck(self.L.ctr_r2_score(self.h, t.ctypes.data_as(_dp), p.ctypes.data_as(_dp), C.c_int64(t.shape[0]), C.c_int32(t.shape[1]),
+                                     wp, C.c_int32(mode), out.ctypes.data_as(_dp)))
+        return out if mode == MULTIOUTPUT["raw_values"] else float(out[0])
+
+    def mean_error(self, y_true, y_pred, kind="squared", multioutput="uniform_average"):
+        """MeanSquaredError (kind "squared") or MeanAbsoluteError ("absolute") (ctr_mean_error): "raw_values" gives the
+        [n_out] column means, "uniform_average" (or "") their mean.  "variance_weighted" raises CtrError (EINVAL)."""
+        t, p = _targets(y_true, y_pred)
+        k = _mode(ERROR_KIND, kind, "kind")
+        mode = _mode(MULTIOUTPUT, "uniform_average" if multioutput == "" else multioutput, "multioutput")
+        out = np.empty(t.shape[1], np.float64)
+        self._ck(self.L.ctr_mean_error(self.h, t.ctypes.data_as(_dp), p.ctypes.data_as(_dp), C.c_int64(t.shape[0]), C.c_int32(t.shape[1]),
+                                       C.c_int32(k), C.c_int32(mode), out.ctypes.data_as(_dp)))
+        return out if mode == MULTIOUTPUT["raw_values"] else float(out[0])
+
     def knn_search(self, k, queries=None, rows=None):
         """search.Searcher on ITEM_EMB (ctr_knn_search): queries [nq, D] float64 vectors (rows: optional row to exclude
         per query, -1 = none), or queries=None and rows = the query rows.  Returns (rows [nq, k] int32, sims [nq, k]
@@ -776,6 +886,17 @@ class MLPClassifier(_Mlp64):
         out = np.empty(Xa.shape[0], np.float32)
         self._ck(self.L.ctr_mlp_predict(self.h, Xp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), out.ctypes.data_as(_fp)))
         return out
+
+    def score(self, X, Y):
+        """MLPClassifier.Score (ctr_mlp_accuracy): the share of rows whose prediction equals the label.  With classes the
+        prediction is the class label; a binary model compares the float64 probability itself, as the reference does,
+        so only probabilities of exactly 0.0 or 1.0 can count."""
+        Xa, Xp = _f(X); Ya, Yp = _f(Y)
+        if Ya.size != Xa.shape[0]:
+            raise ValueError("Y has %d labels for %d rows" % (Ya.size, Xa.shape[0]))
+        acc = C.c_double(0)
+        self._ck(self.L.ctr_mlp_accuracy(self.h, Xp, Yp, C.c_int64(Xa.shape[0]), C.c_int32(Xa.shape[1]), C.byref(acc)))
+        return acc.value
 
     @property
     def classes_(self):

@@ -25,7 +25,9 @@ from . import engine as _e
 __all__ = ["SampleInfo", "TrainSample", "DinNet", "YoutubeDnn", "NewDinNet", "NewDinNetFromJson",
            "NewYoutubeDnn", "NewYoutubeDnnFromJson", "Train", "InitForwardOnlyVm", "Predict",
            "DinImpl", "YoutubeDnnImpl", "RocAuc32", "GroupAuc32", "ROCCurve", "PrecisionRecallCurve",
-           "AveragePrecisionScore", "GroupAveragePrecision32", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
+           "AveragePrecisionScore", "GroupAveragePrecision32", "AccuracyScore", "ConfusionMatrix", "PrecisionScore",
+           "RecallScore", "F1Score", "FBetaScore", "PrecisionRecallFScoreSupport", "R2Score", "MeanSquaredError",
+           "MeanAbsoluteError", "SimpleMlpFitWrap", "SimpleMlpPredWrap"]
 
 mlp0_1, mlp1_2 = 200, 80          # din.go:17-18
 
@@ -329,3 +331,91 @@ def GroupAveragePrecision32(pred, y, group, engine=None):
     """Mean average precision on the device (ctr_group_average_precision): AveragePrecisionScore per group (normally
     the UserId), averaged without weights over the groups that hold a positive — MAP, next to GroupAuc32's GAUC."""
     return _eval_engine(engine).group_average_precision(pred, y, group)[0]
+
+
+# ---- nn/metrics classification.go and regression.go (the averages and modes by the reference's strings) ----------
+_AVERAGES = ("macro", "micro", "weighted")
+
+
+def _average(average):
+    if average not in _AVERAGES:
+        raise ValueError("average must be one of %s, got %r" % (list(_AVERAGES), average))
+    return average
+
+
+def AccuracyScore(Ytrue, Ypred, normalize, sampleWeight, engine=None):
+    """metrics.AccuracyScore (classification.go:12-34) on the device (ctr_accuracy_score): [n] or [n, n_out] labels,
+    sampleWeight [n] (or [n, 1]) or None."""
+    return _eval_engine(engine).accuracy_score(Ytrue, Ypred, normalize, sampleWeight)
+
+
+def ConfusionMatrix(YTrue, YPred, sampleWeight, engine=None):
+    """metrics.ConfusionMatrix (classification.go:150-153) of 1-D labels on the device (ctr_confusion_matrix): the
+    [C, C] matrix over the classes of YTrue."""
+    return _eval_engine(engine).confusion_matrix(_column(YTrue), _column(YPred), sampleWeight)[1]
+
+
+def PrecisionRecallFScoreSupport(YTrue, YPred, beta, labels, posLabel, average, warnFor, sampleWeight, engine=None):
+    """metrics.PrecisionRecallFScoreSupport (classification.go:74-148) on the device (ctr_precision_recall_fscore):
+    (precision, recall, fscore, support).  "weighted" averages like "macro", as the reference does (sklearn would weight
+    by support).  The reference ignores labels and warnFor; here a non-empty one raises ValueError instead of being
+    dropped."""
+    if labels is not None and len(labels):
+        raise ValueError("labels is not used by the reference's PrecisionRecallFScoreSupport: pass None or []")
+    if warnFor is not None and len(warnFor):
+        raise ValueError("warnFor is not used by the reference's PrecisionRecallFScoreSupport: pass None or []")
+    avg = _average(average)
+    return _eval_engine(engine).precision_recall_fscore(_column(YTrue), _column(YPred), beta, avg, posLabel, sampleWeight)
+
+
+def PrecisionScore(Ytrue, Ypred, average, sampleWeight, engine=None):
+    """metrics.PrecisionScore (classification.go:37-42) on the device"""
+    return PrecisionRecallFScoreSupport(Ytrue, Ypred, 1.0, None, -1, average, [], sampleWeight, engine)[0]
+
+
+def RecallScore(Ytrue, Ypred, average, sampleWeight, engine=None):
+    """metrics.RecallScore (classification.go:44-49) on the device"""
+    return PrecisionRecallFScoreSupport(Ytrue, Ypred, 1.0, None, -1, average, [], sampleWeight, engine)[1]
+
+
+def FBetaScore(Ytrue, Ypred, beta, average, sampleWeight, engine=None):
+    """metrics.FBetaScore (classification.go:58-68) on the device"""
+    return PrecisionRecallFScoreSupport(Ytrue, Ypred, beta, None, -1, average, [], sampleWeight, engine)[2]
+
+
+def F1Score(Ytrue, Ypred, average, sampleWeight, engine=None):
+    """metrics.F1Score (classification.go:51-56) on the device"""
+    return FBetaScore(Ytrue, Ypred, 1.0, average, sampleWeight, engine)
+
+
+def _multioutput(multioutput, modes):
+    m = "uniform_average" if multioutput == "" else multioutput
+    if m not in modes:
+        raise ValueError("multioutput must be one of %s or \"\", got %r" % (list(modes), multioutput))
+    return m
+
+
+def R2Score(yTrue, yPred, sampleWeight, multioutput, engine=None):
+    """metrics.R2Score (regression.go:83-128) on the device (ctr_r2_score): "raw_values" returns the [n_out] scores,
+    "variance_weighted" and "uniform_average" (or "") one float.  A constant column is not refused."""
+    m = _multioutput(multioutput, ("raw_values", "uniform_average", "variance_weighted"))
+    return _eval_engine(engine).r2_score(yTrue, yPred, sampleWeight, m)
+
+
+def _mean_error(kind, yTrue, yPred, sampleWeight, multioutput, engine):
+    if sampleWeight is not None:
+        raise ValueError("sampleWeight is not supported: the reference reads sampleWeight.At(0, j) for every sample of "
+                         "column j (regression.go:163, :230), which cancels out or gives 0/0")
+    m = multioutput if multioutput == "variance_weighted" else _multioutput(multioutput, ("raw_values", "uniform_average"))
+    return _eval_engine(engine).mean_error(yTrue, yPred, kind, m)
+
+
+def MeanSquaredError(yTrue, yPred, sampleWeight, multioutput, engine=None):
+    """metrics.MeanSquaredError (regression.go:153-176) on the device (ctr_mean_error); "variance_weighted" reaches
+    the C call and raises CtrError (EINVAL)."""
+    return _mean_error("squared", yTrue, yPred, sampleWeight, multioutput, engine)
+
+
+def MeanAbsoluteError(yTrue, yPred, sampleWeight, multioutput, engine=None):
+    """metrics.MeanAbsoluteError (regression.go:220-244) on the device (ctr_mean_error)"""
+    return _mean_error("absolute", yTrue, yPred, sampleWeight, multioutput, engine)

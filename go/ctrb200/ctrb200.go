@@ -320,6 +320,118 @@ func (e *Engine) AveragePrecision(pred, y []float32) (float64, error) {
 	return float64(ap), nil
 }
 
+// f64n is f64, or nil for an empty slice (the C calls' optional weights)
+func f64n(p []float64) *C.double {
+	if len(p) == 0 {
+		return nil
+	}
+	return f64(p)
+}
+
+// Averages of PrecisionRecallFScore and modes of R2Score / MeanError (the reference's strings, as the C enums)
+const (
+	AverageMacro    = int(C.CTR_AVERAGE_MACRO)
+	AverageMicro    = int(C.CTR_AVERAGE_MICRO)
+	AverageWeighted = int(C.CTR_AVERAGE_WEIGHTED) // equals AverageMacro, as in the reference (classification.go:116-131)
+
+	MultioutputRaw              = int(C.CTR_MULTIOUTPUT_RAW)
+	MultioutputUniform          = int(C.CTR_MULTIOUTPUT_UNIFORM)
+	MultioutputVarianceWeighted = int(C.CTR_MULTIOUTPUT_VARIANCE_WEIGHTED)
+
+	ErrorSquared  = int(C.CTR_ERROR_SQUARED)
+	ErrorAbsolute = int(C.CTR_ERROR_ABSOLUTE)
+)
+
+// AccuracyScore is metrics.AccuracyScore (classification.go:12-34) on the device: yTrue and yPred are [n, nOut]
+// row-major; a row is correct when every column is equal (==).  weight is per sample (nil: all 1) and must be finite.
+func (e *Engine) AccuracyScore(yTrue, yPred []float64, nOut int, weight []float64, normalize bool) (float64, error) {
+	if nOut < 1 || len(yTrue) == 0 || len(yTrue)%nOut != 0 || len(yPred) != len(yTrue) || (weight != nil && len(weight) != len(yTrue)/nOut) {
+		return 0, fmt.Errorf("ctrb200: AccuracyScore needs [n, nOut] yTrue and yPred and nil or n weights")
+	}
+	norm := 0
+	if normalize {
+		norm = 1
+	}
+	var r C.double
+	if err := e.err(C.ctr_accuracy_score(e.h, f64(yTrue), f64(yPred), C.int64_t(len(yTrue)/nOut), C.int32_t(nOut), f64n(weight), C.int32_t(norm), &r)); err != nil {
+		return 0, err
+	}
+	return float64(r), nil
+}
+
+// ConfusionMatrix is metrics.ConfusionMatrix (classification.go:150-178) of 1-D labels on the device: the classes of
+// yTrue ascending and the [C, C] matrix, row-major.  A prediction between two classes counts as the higher one; one
+// above the largest class, or a NaN, is an error.
+func (e *Engine) ConfusionMatrix(yTrue, yPred, weight []float64) (classes, cm []float64, err error) {
+	m := len(yTrue)
+	if m == 0 || len(yPred) != m || (weight != nil && len(weight) != m) {
+		return nil, nil, fmt.Errorf("ctrb200: ConfusionMatrix needs equally long, non-empty yTrue, yPred (and weight)")
+	}
+	var nc C.int32_t
+	classes = make([]float64, m)
+	if err = e.err(C.ctr_confusion_matrix(e.h, f64(yTrue), f64(yPred), C.int64_t(m), f64n(weight), f64(classes), nil,
+		C.int64_t(int64(m)*int64(m)), &nc)); err != nil {
+		return nil, nil, err
+	}
+	cm = make([]float64, int(nc)*int(nc))
+	if err = e.err(C.ctr_confusion_matrix(e.h, f64(yTrue), f64(yPred), C.int64_t(m), f64n(weight), nil, f64(cm),
+		C.int64_t(len(cm)), &nc)); err != nil {
+		return nil, nil, err
+	}
+	return classes[:nc], cm, nil
+}
+
+// PrecisionRecallFScore is metrics.PrecisionRecallFScoreSupport (classification.go:74-148) on the device: the class
+// posLabel's precision, recall, F-beta and support, or with posLabel < 0 the average (AverageMacro, AverageMicro or
+// AverageWeighted; support 0).  PrecisionScore, RecallScore and F1Score are beta = 1, FBetaScore the beta given.
+// perClass holds [C, 4] rows (p, r, f, support).
+func (e *Engine) PrecisionRecallFScore(yTrue, yPred, weight []float64, beta float64, average, posLabel int) (p, r, f, support float64, perClass []float64, err error) {
+	m := len(yTrue)
+	if m == 0 || len(yPred) != m || (weight != nil && len(weight) != m) {
+		return 0, 0, 0, 0, nil, fmt.Errorf("ctrb200: PrecisionRecallFScore needs equally long, non-empty yTrue, yPred (and weight)")
+	}
+	var cp, cr, cf, cs C.double
+	var nc C.int32_t
+	perClass = make([]float64, 4*m)
+	if err = e.err(C.ctr_precision_recall_fscore(e.h, f64(yTrue), f64(yPred), C.int64_t(m), f64n(weight), C.double(beta),
+		C.int32_t(average), C.int32_t(posLabel), &cp, &cr, &cf, &cs, f64(perClass), C.int64_t(m), &nc)); err != nil {
+		return 0, 0, 0, 0, nil, err
+	}
+	return float64(cp), float64(cr), float64(cf), float64(cs), perClass[:4*int(nc)], nil
+}
+
+// R2Score is metrics.R2Score (regression.go:83-128) on the device over [n, nOut] row-major targets: nOut scores for
+// MultioutputRaw, else one.  weight is per sample (nil: all 1).  A constant column is not an error.
+func (e *Engine) R2Score(yTrue, yPred []float64, nOut int, weight []float64, multioutput int) ([]float64, error) {
+	if nOut < 1 || len(yTrue) == 0 || len(yTrue)%nOut != 0 || len(yPred) != len(yTrue) || (weight != nil && len(weight) != len(yTrue)/nOut) {
+		return nil, fmt.Errorf("ctrb200: R2Score needs [n, nOut] yTrue and yPred and nil or n weights")
+	}
+	out := make([]float64, nOut)
+	if err := e.err(C.ctr_r2_score(e.h, f64(yTrue), f64(yPred), C.int64_t(len(yTrue)/nOut), C.int32_t(nOut), f64n(weight), C.int32_t(multioutput), f64(out))); err != nil {
+		return nil, err
+	}
+	if multioutput != MultioutputRaw {
+		out = out[:1]
+	}
+	return out, nil
+}
+
+// MeanError is metrics.MeanSquaredError (kind ErrorSquared) or MeanAbsoluteError (ErrorAbsolute) (regression.go:153-244)
+// on the device, without sample weights: nOut column means for MultioutputRaw, their mean for MultioutputUniform.
+func (e *Engine) MeanError(yTrue, yPred []float64, nOut, kind, multioutput int) ([]float64, error) {
+	if nOut < 1 || len(yTrue) == 0 || len(yTrue)%nOut != 0 || len(yPred) != len(yTrue) {
+		return nil, fmt.Errorf("ctrb200: MeanError needs [n, nOut] yTrue and yPred")
+	}
+	out := make([]float64, nOut)
+	if err := e.err(C.ctr_mean_error(e.h, f64(yTrue), f64(yPred), C.int64_t(len(yTrue)/nOut), C.int32_t(nOut), C.int32_t(kind), C.int32_t(multioutput), f64(out))); err != nil {
+		return nil, err
+	}
+	if multioutput != MultioutputRaw {
+		out = out[:1]
+	}
+	return out, nil
+}
+
 // GroupAveragePrecision is the mean average precision (MAP) over groups (normally the sample's UserId): AveragePrecision
 // within each group, averaged without weights over the groups that hold a positive; NaN when none does.  With
 // perGroup, groups holds the distinct ids ascending and n / pos / ap their samples, positives and AP (NaN without a
@@ -818,6 +930,22 @@ func (p *MlpPredWrap) Score(X tensor.Tensor, Y []float32) (float64, error) {
 		return 0, fmt.Errorf("ctr_mlp_score: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
 	}
 	return float64(r2), nil
+}
+
+// Accuracy is MLPClassifier.Score (multilayer_perceptron.go:127-133) of a classifier's predictor: the share of rows
+// whose prediction equals Y.  With classes the prediction is the class label; a binary model compares its float64
+// probability itself, as the reference does, so only probabilities of exactly 0 or 1 count.  A regressor's predictor
+// is an error (its score is Score).
+func (p *MlpPredWrap) Accuracy(X tensor.Tensor, Y []float32) (float64, error) {
+	n := X.Shape()[0]
+	if len(Y) != n {
+		return 0, fmt.Errorf("MlpPredWrap.Accuracy: %d labels for %d rows", len(Y), n)
+	}
+	var acc C.double
+	if rc := C.ctr_mlp_accuracy(p.m, f32(X.Data().([]float32)), f32(Y), C.int64_t(n), C.int32_t(p.xcols), &acc); rc != C.CTR_OK {
+		return 0, fmt.Errorf("ctr_mlp_accuracy: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(p.m)))
+	}
+	return float64(acc), nil
 }
 
 // MlpRegressorFitWrap satisfies recommend.Fitter with nn.NewMLPRegressor (multilayer_perceptron.go:19-28) in place of

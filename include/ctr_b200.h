@@ -356,6 +356,71 @@ int ctr_group_average_precision(ctr_handle* h, const float* pred, const float* y
                                 double* map, int64_t* n_groups, int64_t* n_used,
                                 int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_ap);
 
+/* The classification and regression metrics of nn/metrics (classification.go, regression.go) on the device.  Shared
+ * rules: host buffers of double (the reference's mat.Dense; float32 labels and predictions widen exactly); n in
+ * [1, 2^31); a handle created with batch = pred_batch = 1 is enough.  The calls run on the engine stream under the
+ * handle's mutex and are not collective under world > 1: each rank evaluates the samples it passes.  Every refusal comes
+ * before any output is written (except as stated) and its message is in ctr_last_error; the arguments are checked
+ * before the handle, so with h NULL the message is in ctr_last_error(NULL).  Identical inputs give identical bits.
+ * Unweighted counts are exact integers; every weighted or floating-point sum is taken over fixed partitions in a fixed
+ * order (a double-double wherever the reference has sample weights). */
+enum { CTR_AVERAGE_MACRO = 0, CTR_AVERAGE_MICRO = 1, CTR_AVERAGE_WEIGHTED = 2 };
+enum { CTR_MULTIOUTPUT_RAW = 0, CTR_MULTIOUTPUT_UNIFORM = 1, CTR_MULTIOUTPUT_VARIANCE_WEIGHTED = 2 };
+enum { CTR_ERROR_SQUARED = 0, CTR_ERROR_ABSOLUTE = 1 };
+
+/* AccuracyScore (classification.go:12-34): y_true and y_pred are [n, n_out] row-major, n_out in [1, 1024].  A row is
+ * correct when each of its n_out columns compares equal with == (-0 == +0; a NaN never equals).  weight [n] (NULL: every
+ * weight 1) must be finite, else CTR_EINVAL; zero and negative weights are used as given.  N = the weights of the correct
+ * rows, D = all weights; *score = N / D with normalize != 0 (NaN when every weight is 0, as the reference's 0/0; a
+ * nonzero N over D = 0 is ±inf), else N. */
+int ctr_accuracy_score(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, const double* weight,
+                       int32_t normalize, double* score);
+
+/* ConfusionMatrix (classification.go:150-178) of 1-D labels.  The classes are LabelEncoder.Fit's on y_true
+ * (label.go:288-321): the C distinct values ascending, -0 and +0 one class whose value keeps the sign of its first
+ * occurrence in sample order.  Each label maps as sort.SearchFloat64s maps it (label.go:324-339), to the first class
+ * >= it: a prediction between two classes counts as the higher one.  cm[r*C + c] = the summed weights (weight NULL:
+ * counts) of the samples of true class r predicted as c.  CTR_EINVAL, naming the first offending sample, for a NaN in
+ * y_true or y_pred, a weight that is not finite, or a prediction above the largest class (there the reference writes
+ * into the cell before (r, 0), or panics when r = 0).  *n_classes = C is written whenever y_true holds no NaN, even by
+ * a refusal.  classes (C values; C <= n) and cm (cap cells) may each be NULL; C*C > cap is CTR_EINVAL. */
+int ctr_confusion_matrix(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, const double* weight, double* classes,
+                         double* cm, int64_t cap, int32_t* n_classes);
+
+/* PrecisionRecallFScoreSupport (classification.go:74-148) over the classes and cells of ctr_confusion_matrix (same
+ * pipeline, same refusals).  Per class: tp = the diagonal cell, truesum = the row's weights, predsum = the column's (each
+ * a compensated sum over the samples; the reference sums the matrix's cells); p = tp / predsum (0 when predsum <= 0),
+ * r = tp / truesum (0 when truesum <= 0), f = (1+beta^2)*p*r / (beta^2*p + r) (0 when that denominator is not > 0), each
+ * operation rounded on its own; support = the unweighted count of y_true in the class (le.Support).  pos_label >= 0:
+ * *p, *r, *f, *support are that class's (pos_label >= C is CTR_EINVAL; the reference panics).  pos_label < 0: the average
+ * -- CTR_AVERAGE_MACRO the plain mean over the classes; CTR_AVERAGE_WEIGHTED the same mean, bit for bit, because the
+ * reference builds the support weights and then calls stat.Mean(p, nil) (:116-131; sklearn would weight by support);
+ * CTR_AVERAGE_MICRO the per-class formulas on tp, truesum and predsum summed over the classes -- and *support = 0.
+ * Another average is CTR_EINVAL (the reference returns zeros), as is a beta that is not finite.  p, r, f and support
+ * may each be NULL.  per_class (NULL or cap rows) receives [C, 4] rows (p, r, f, support); with per_class non-NULL,
+ * C > cap is CTR_EINVAL (C <= n, so cap = n always suffices).  *n_classes as in ctr_confusion_matrix.
+ * PrecisionScore, RecallScore and F1Score are this call with beta = 1, FBetaScore with the beta given. */
+int ctr_precision_recall_fscore(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, const double* weight, double beta,
+                                int32_t average, int32_t pos_label, double* p, double* r, double* f, double* support,
+                                double* per_class, int64_t cap, int32_t* n_classes);
+
+/* R2Score (regression.go:83-128) of [n, n_out] targets, n_out in [1, 1024].  With weight [n] (NULL: every weight 1),
+ * per column j: num_j = sum w*(pred - true)^2, avg_j = sum w*true / sum w, den_j = sum w*(true - avg_j)^2,
+ * r2_j = 1 - num_j / max(den_j, 1e-20).  CTR_MULTIOUTPUT_RAW writes out[n_out] = r2_j; CTR_MULTIOUTPUT_VARIANCE_WEIGHTED
+ * writes out[0] = sum den_j*r2_j * (1 / sum den_j), NaN when every den_j is 0; CTR_MULTIOUTPUT_UNIFORM writes out[0] =
+ * the mean of the r2_j.  A constant column is not refused (unlike ctr_mlp_score); NaN and +-inf inputs propagate as IEEE
+ * arithmetic makes them.  The sums are the fixed-partition column reductions of ctr_mlp_score. */
+int ctr_r2_score(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, const double* weight,
+                 int32_t multioutput, double* out);
+
+/* MeanSquaredError (kind CTR_ERROR_SQUARED, regression.go:153-176) and MeanAbsoluteError (CTR_ERROR_ABSOLUTE, :220-244):
+ * per column the mean of (pred - true)^2 or |pred - true| over the n rows; CTR_MULTIOUTPUT_RAW writes out[n_out],
+ * CTR_MULTIOUTPUT_UNIFORM out[0] = their mean.  CTR_MULTIOUTPUT_VARIANCE_WEIGHTED is CTR_EINVAL: these functions have no
+ * such mode.  No sample weights: the reference reads sampleWeight.At(0, j) (:163, :230), one weight for every sample of
+ * column j, which either cancels out of N / D or gives 0 / 0. */
+int ctr_mean_error(ctr_handle* h, const double* y_true, const double* y_pred, int64_t n, int32_t n_out, int32_t kind,
+                   int32_t multioutput, double* out);
+
 /* search.Searcher (feature/embedding/search/search.go:66-134): the k items of ITEM_EMB most cosine-similar to each
  * query, on the device.  queries == NULL: search by row — query i is ITEM_EMB row query_rows[i] widened to float64 and
  * excluded from its own result (SearchInternal, with the word→row map on the caller's side); a row outside [0, rows)
@@ -637,8 +702,17 @@ int  ctr_mlp_predict_f64(ctr_mlp* m, const float* X, int64_t n, int32_t xcols, d
 /* MLPRegressor.Score (:64-70 → r2Score64, basemlp64.go:1116-1141) on the device: per target column, mean = Σ y / n,
  * r2 = 1 − Σ (pred − y)² / Σ (y − mean)²; *r2 = the mean over the columns.  The sums are fixed-order reductions: the
  * same bits on every run.  CTR_EINVAL for a column whose Σ (y − mean)² is 0 (the reference panics), CTR_ESTATE for a
- * classifier (its accuracy score is not built) or an unfitted regressor. */
+ * classifier (its accuracy score is ctr_mlp_accuracy) or an unfitted regressor. */
 int  ctr_mlp_score(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* r2);
+/* MLPClassifier.Score (multilayer_perceptron.go:127-133 → AccuracyScore64, basemlp64.go:1143-1155) on the device: the
+ * forward pass in chunks as ctr_mlp_predict runs it, the comparison and the count on the device, *acc = correct / n.
+ * Y [n] holds the labels.  With classes a row is correct when classes[argmax] (ctr_mlp_predict's label) == (double)Y[i];
+ * with one class that is "Y[i] == the class".  A binary model (labels all 0 or 1) compares, as the reference does, the
+ * float64 PROBABILITY of ctr_mlp_predict_f64 with the label: a row counts only where that probability is exactly 0.0 or
+ * 1.0 and equals its label (not the float32 probability of ctr_mlp_predict, nor a 0.5 threshold).  Equal, bit for bit,
+ * to ctr_accuracy_score of Y against those predictions.  CTR_ESTATE on a regressor (its score is ctr_mlp_score) or
+ * before a fit; CTR_EINVAL for null arguments, n < 1 or xcols != the network's inputs. */
+int  ctr_mlp_accuracy(ctr_mlp* m, const float* X, const float* Y, int64_t n, int32_t xcols, double* acc);
 /* The output kind (CTR_MLP_OUT_*).  A classifier's follows its classes.  To restore a regressor (the reference's JSON
  * carries OutActivation): ctr_mlp_set_output, then ctr_mlp_set_params; set_output leaves the model unfitted until
  * set_params.  set_output is CTR_ESTATE on a classifier, and CTR_EINVAL for a logistic output with more than one
