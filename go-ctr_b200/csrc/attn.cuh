@@ -258,17 +258,6 @@ __device__ __forceinline__ float4 ld4_peer(const float* p) {
                  : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
     return r;
 }
-template <bool PEER>
-__device__ __forceinline__ float* emb_ptr(const RowSrc& r, int idx) {
-    return PEER ? shard_row(r, r.peer_emb, idx, r.lde) : const_cast<float*>(r.emb) + (long)idx * r.lde;
-}
-// read side of a sharded table: the replicated hot rows are local
-template <bool PEER>
-__device__ __forceinline__ const float* emb_src(const RowSrc& r, int idx) {
-    if (PEER && idx < r.hot_k) return r.hot_tab + (long)idx * r.lde;
-    return emb_ptr<PEER>(r, idx);
-}
-
 // PEER: ITEM_EMB (and ITEM_FEAT when large) are row-sharded over the GPUs of the box and every shard is mapped into
 // this process (CUDA IPC): the gather reads the owner's HBM directly over NVLink — the transfer is the load itself, so
 // it overlaps the gate math of the other warps tile by tile — and keeps each fetched row in rows_cache for the
@@ -1013,7 +1002,21 @@ struct RowsByIdx {
     __device__ __forceinline__ int operator()(int b) const { return (int)__ldg(idx + b); }
 };
 
-template <typename T, typename Rows>
+// PEER (a row-sharded ITEM_EMB, index mode): the ITEM_EMB rows come through emb_src<true> — the hot rows from this
+// rank's replica, which is current after a sharded step while the owners' shard copies are not, the rest from their
+// owners — and ITEM_FEAT rows through ifeat_row, sharded or replicated
+__device__ __forceinline__ const float* peer_ub(const RowSrc& r, const Dims& d, int b, int s) {
+    if (b >= r.nvalid) return nullptr;
+    const int idx = __ldg(r.hist + (long)b * d.S + s);
+    return row_ok(idx, r.n_emb) ? emb_src<true>(r, idx) : nullptr;
+}
+__device__ __forceinline__ const float* peer_it(const RowSrc& r, int b) {
+    if (b >= r.nvalid) return nullptr;
+    const int idx = r.item_row[b];
+    return row_ok(idx, r.n_emb) ? emb_src<true>(r, idx) : nullptr;
+}
+
+template <typename T, typename Rows, bool PEER = false>
 __global__ void __launch_bounds__(256)
 k_gather_rows(RowSrc r, Dims d, T* __restrict__ X, long ldx, int B, Rows rows) {
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -1024,10 +1027,10 @@ k_gather_rows(RowSrc r, Dims d, T* __restrict__ X, long ldx, int B, Rows rows) {
         const float* pu = src_up(r, sb);
         for (int j = lane; j < d.uP; j += 32) x[j] = pu ? (T)__ldg(pu + j) : (T)0;
         for (int s = 0; s < d.S; s++) {
-            const float* up = src_ub(r, d, sb, s);
+            const float* up = PEER ? peer_ub(r, d, sb, s) : src_ub(r, d, sb, s);
             for (int j = lane; j < d.D; j += 32) x[d.uP + (long)s * d.D + j] = up ? (T)__ldg(up + j) : (T)0;
         }
-        const float* ip = src_it(r, d, sb);
+        const float* ip = PEER ? peer_it(r, sb) : src_it(r, d, sb);
         T* xi = x + d.uP + (long)d.S * d.D;
         for (int j = lane; j < d.D; j += 32) xi[j] = ip ? (T)__ldg(ip + j) : (T)0;
         const float* pc = src_cx(r, sb);

@@ -72,7 +72,8 @@ struct CommHdr {
     int32_t code;               // CTR_OK or this rank's error code ...
     uint64_t hash[3];
     int64_t plan;               // what fixes the number of collectives (queries per chunk / users per group / rank passes)
-    char msg[200];              // ... and its message
+    uint64_t rows;              // a hash of the rows this rank's id maps resolved the call's ids to (0: no ids)
+    char msg[192];              // ... and its message
 };
 static_assert(sizeof(CommHdr) == 256, "one all-gather slot of Comm::d_xchg");
 
@@ -86,6 +87,7 @@ static int comm_predict(ctr_handle* h, const int32_t* d_user, const int32_t* d_i
 static int comm_barrier(ctr_handle* h);
 static int comm_max_i64(ctr_handle* h, int64_t* v);
 static int comm_sum_u64(ctr_handle* h, unsigned long long* buf, size_t n);
+static int comm_bcast0(ctr_handle* h, void* buf, size_t bytes);
 static int comm_unique_id(void* id_out, int32_t* id_bytes);
 static int comm_init(ctr_handle* h, const void* id, int32_t id_bytes);
 static void comm_destroy(ctr_handle* h);

@@ -16,6 +16,7 @@ struct NcclApi {
     int (*GroupEnd)() = nullptr;
     int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
+    int (*Broadcast)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     const char* (*GetErrorString)(int) = nullptr;
 };
 enum { kNcclChar = 0, kNcclInt32 = 2, kNcclInt64 = 4, kNcclUint64 = 5, kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2 };
@@ -31,7 +32,7 @@ bool nccl_load(std::string* err) {
 #define SYM(field, name) *(void**)(&g_nccl.field) = dlsym(lib, name); if (!g_nccl.field) { *err = std::string("missing NCCL symbol ") + name; return false; }
     SYM(GetUniqueId, "ncclGetUniqueId") SYM(CommInitRank, "ncclCommInitRank") SYM(CommDestroy, "ncclCommDestroy")
     SYM(GroupStart, "ncclGroupStart") SYM(GroupEnd, "ncclGroupEnd")
-    SYM(AllReduce, "ncclAllReduce") SYM(AllGather, "ncclAllGather") SYM(GetErrorString, "ncclGetErrorString")
+    SYM(AllReduce, "ncclAllReduce") SYM(AllGather, "ncclAllGather") SYM(Broadcast, "ncclBroadcast") SYM(GetErrorString, "ncclGetErrorString")
 #undef SYM
     g_nccl.lib = lib;
     return true;
@@ -308,6 +309,9 @@ static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
     }
     for (int j = 0; j < W; j++)
         if (all[(size_t)j].code != CTR_OK) return set_err(h, all[(size_t)j].code, "%s", all[(size_t)j].msg);
+    for (int j = 1; j < W; j++)          // every rank valid: its id maps resolved the ids to the same rows
+        if (all[(size_t)j].rows != all[0].rows)
+            return set_err(h, CTR_EINVAL, "ranks resolve the ids of this collective call to different rows: rank %d's id maps differ from rank 0's", j);
     for (int j = 1; j < W; j++)          // every rank valid: their plans must give the same sequence of all-gathers
         if (all[(size_t)j].plan != all[0].plan)
             return set_err(h, CTR_EINVAL, "ranks disagree on the plan of this collective call: rank %d would exchange %lld entries per round, rank 0 %lld",
@@ -334,6 +338,15 @@ static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, si
 static int comm_sum_u64(ctr_handle* h, unsigned long long* buf, size_t n) {
     Comm& cm = h->comm;
     NC(h, g_nccl.AllReduce(buf, buf, n, kNcclUint64, kNcclSum, cm.nccl, h->stream));
+    h->launches += 1;
+    return CTR_OK;
+}
+
+// buf[0, bytes) of rank 0 onto every rank, in place on the engine stream (the behaviour windows of the key-fed MLP's
+// collective calls: every rank scores its shard for the window rank 0's cache cuts)
+static int comm_bcast0(ctr_handle* h, void* buf, size_t bytes) {
+    Comm& cm = h->comm;
+    NC(h, g_nccl.Broadcast(buf, buf, bytes, kNcclChar, 0, cm.nccl, h->stream));
     h->launches += 1;
     return CTR_OK;
 }

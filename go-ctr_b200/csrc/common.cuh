@@ -150,6 +150,16 @@ __device__ __forceinline__ const float* emb_row(const RowSrc& r, int idx) {
 __device__ __forceinline__ const float* ifeat_row(const RowSrc& r, int idx) {
     return r.ifeat_sharded ? shard_row(r, r.peer_ifeat, idx, r.ldi) : r.ifeat + (long)idx * r.ldi;
 }
+template <bool PEER>
+__device__ __forceinline__ float* emb_ptr(const RowSrc& r, int idx) {
+    return PEER ? shard_row(r, r.peer_emb, idx, r.lde) : const_cast<float*>(r.emb) + (long)idx * r.lde;
+}
+// read side of a sharded table: the replicated hot rows are local
+template <bool PEER>
+__device__ __forceinline__ const float* emb_src(const RowSrc& r, int idx) {
+    if (PEER && idx < r.hot_k) return r.hot_tab + (long)idx * r.lde;
+    return emb_ptr<PEER>(r, idx);
+}
 
 __device__ __forceinline__ const float* src_ub(const RowSrc& r, const Dims& d, int b, int s) {
     if (b >= r.nvalid) return nullptr;

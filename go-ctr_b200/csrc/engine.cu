@@ -914,7 +914,8 @@ RowSrc idx_src(const ctr_handle* h, const int* d_user, const int* d_item, const 
     return r;
 }
 
-int check_tables(const ctr_handle* h) {
+// every table the configuration needs is uploaded with its width (this rank's shard of a row-sharded one)
+int check_widths(const ctr_handle* h) {
     const ctr_config& c = h->cfg;
     if (!h->tab[CTR_TABLE_ITEM_EMB] || h->tab_width[CTR_TABLE_ITEM_EMB] != c.D)
         return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded with width D=%d", c.D);
@@ -922,6 +923,11 @@ int check_tables(const ctr_handle* h) {
         return set_err(h, CTR_ESTATE, "USER_FEAT table not uploaded with width uP=%d", c.uP);
     if (c.cF > 0 && (!h->tab[CTR_TABLE_ITEM_FEAT] || h->tab_width[CTR_TABLE_ITEM_FEAT] != c.cF))
         return set_err(h, CTR_ESTATE, "ITEM_FEAT table not uploaded with width cF=%d", c.cF);
+    return CTR_OK;
+}
+
+int check_tables(const ctr_handle* h) {
+    RET(check_widths(h));
     if (h->comm.world > 1 && (h->tab_sharded[CTR_TABLE_ITEM_EMB] || h->tab_sharded[CTR_TABLE_ITEM_FEAT]))
         return set_err(h, CTR_ESTATE, "this entry point gathers locally: ITEM_EMB / ITEM_FEAT must both be replicated (or both sharded for the train / predict entry points)");
     return CTR_OK;
@@ -4415,18 +4421,33 @@ int ctr_mlp_set_output(ctr_mlp* m, int32_t kind) {
 
 // ---- the MLP fed by sample keys from a feature store (ctr_mlp_fit_keys / ctr_mlp_predict_keys) -------------
 namespace {
-// the refusals shared by both calls; h->mu and m->mu are held, m's device is made current
+// the refusals shared by every key-fed call; h->mu and m->mu are held, m's device is made current.  First this rank's
+// own objects, then the feature store's tables: with ITEM_EMB and ITEM_FEAT both replicated (or one GPU) this GPU's
+// tables serve alone; a row-sharded ITEM_EMB needs this rank's shard and the communicator (ITEM_FEAT sharded or
+// replicated); a replicated ITEM_EMB beside a sharded ITEM_FEAT is refused (check_tables)
 int mlp_keys_check(ctr_mlp* m, ctr_handle* h) {
     const ctr_config& c = h->cfg;
     const long width = (long)c.uP + (long)c.S * c.D + c.D + c.cF;
     if (m->dev != h->dev) return mlp_err(m, CTR_EINVAL, "the classifier is on device %d, the feature store on device %d", m->dev, h->dev);
     if (m->d.units[0] != width)
         return mlp_err(m, CTR_EINVAL, "the network has %d inputs, the feature store's samples uP + S*D + D + cF = %ld columns", m->d.units[0], width);
-    if (h->comm.world > 1) return mlp_err(m, CTR_ESTATE, "the key-fed MLP needs a single-GPU feature store (world=%d)", h->comm.world);
     if (!h->idm_keys[0] || !h->idm_keys[1]) return mlp_err(m, CTR_ESTATE, "the key-fed MLP needs both id maps of the feature store (ctr_idmap_build)");
-    RET(check_tables(h));
     MCU(m, cudaSetDevice(m->dev));
-    return CTR_OK;
+    if (!emb_sharded(h)) return check_tables(h);
+    RET(comm_check_emb(h));
+    return check_widths(h);
+}
+// the agreement of a collective key-fed call (comm_agree, on a row-sharded ITEM_EMB): a rank whose checks failed takes
+// part with its message, and every rank returns the same verdict.  Then, as for ctr_recommend_topk_ex, the mappings
+// are published, every rank's row updates queued before the call have landed and the shard's hot rows are current.
+int mlp_agree(ctr_mlp* m, ctr_handle* h, CommHdr hd, int verdict) {
+    if (verdict != CTR_OK && h->err.empty()) h->err = m->err;
+    CU(h, cudaSetDevice(h->dev));        // the checks may have stopped before making it current
+    const int rc = comm_agree(h, hd, verdict);
+    if (rc != CTR_OK) { m->err = h->err; return rc; }
+    RET(comm_ensure(h, false));
+    RET(comm_barrier(h));
+    return comm_hot_writeback(h);
 }
 // every exit of a key-fed call: no work of m may still read h's buffers, and the message is readable from both objects
 int mlp_keys_done(ctr_mlp* m, ctr_handle* h, int rc) {
@@ -4511,6 +4532,10 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
     if (!m->fitted) return mlp_err(m, CTR_ESTATE, "predict before fit");
     RET(mlp_keys_width(m));
     const int B = h->cfg.pred_batch, S = h->cfg.S, nin = m->d.units[0];
+    // a row-sharded ITEM_EMB: each rank scores its own keys and reads the rows from their owners, as comm_predict does
+    // (the publish after a table change is collective; training and prediction are kept apart by the caller)
+    const bool sh = emb_sharded(h);
+    if (sh) RET(comm_ensure(h, false));
     RET(keys_stage_init(h));
     RET(mlp_rows(m, B));
     RET(mlp_stage(m, B));
@@ -4531,9 +4556,10 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
                                                                     h->ub_off, h->ub_ts, h->ub_items, (long)h->ub_users, h->k_keys, nb, S, h->s_user, h->s_item, h->s_hist);
         }));
         if (s == 0) CU(h, cudaMemcpyAsync(hfirst, h->s_user, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        const RowSrc r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+        const RowSrc r = sh ? comm_src(h, h->s_user, h->s_item, h->s_hist, nb, false) : idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
         RET(launch(h, "mlp_gather", [&] {
-            k_gather_rows<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), m->stage[0].get(), (long)nin, nb, RowsAsIs{});
+            if (sh) k_gather_rows<double, RowsAsIs, true><<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), m->stage[0].get(), (long)nin, nb, RowsAsIs{});
+            else k_gather_rows<<<grid_for_warps(h, nb), 256, 0, h->stream>>>(r, dims_of(h), m->stage[0].get(), (long)nin, nb, RowsAsIs{});
         }));
         RET(mlp_after_store(m, h, 0));
         mlp_forward(m, m->stage[0], nullptr, nb);
@@ -4551,12 +4577,16 @@ int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
 
 // The float64 MLP's scoring pass over the item table (ctr_mlp_recommend_topk, ctr_mlp_rank_items; see mlp64.cuh), on
 // h's stream: per user, the prefix of layer 0 once (prefix); per chunk of items, layer 0 from it and the later layers
-// (chunk), which leave the chunk's logits in z().
+// (chunk), which leave the chunk's logits in z().  On a row-sharded ITEM_EMB the chunks are this rank's local rows and
+// the prefix reads the window's rows from their owners (k_mlp64_prefix<true>); each item's chain is the same as on one
+// GPU, so its logit is too, whatever the chunk size.
 struct MlpRecScore {
     ctr_mlp* m; ctr_handle* h;
     int L = 0, H = 0, pcols = 0, Bc = 0, l0_ctas = 0;
-    int64_t N = 0;
+    int64_t N = 0, NL = 0;                  // ITEM_EMB's rows, the rows this GPU scores
+    bool coll = false;                      // a row-sharded ITEM_EMB
     bool smem_w = false; size_t l0smem = 0;
+    RowSrc src{};
 
     // the refusals, before anything is written
     int check() {
@@ -4566,7 +4596,9 @@ struct MlpRecScore {
         MCU(m, cudaStreamSynchronize(m->stream));                        // h's stream reads the parameters
         L = m->d.n_layers; H = m->d.units[1];
         if (m->d.units[L - 1] != 1) return mlp_err(m, CTR_ESTATE, "recommendation ranks one output unit, the network has %d", m->d.units[L - 1]);
+        coll = emb_sharded(h);
         N = h->tab_rows[CTR_TABLE_ITEM_EMB];
+        NL = coll ? h->tab_local_rows[CTR_TABLE_ITEM_EMB] : N;
         if (N > INT32_MAX) return mlp_err(m, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
         const ctr_config& c = h->cfg;
         const int T = c.D + c.cF;
@@ -4581,10 +4613,11 @@ struct MlpRecScore {
         // items per chunk: pred_batch in whole tiles, at most the table.  The chunk's activations take
         // Bc · (units[1] + … + units[L-1]) · 8 bytes of the classifier's buffers: a large catalogue wants a large pred_batch.
         auto tiles = [](int64_t x) { return std::max<int64_t>((x + kRecTile - 1) / kRecTile, 1) * kRecTile; };
-        Bc = (int)std::min(tiles(c.pred_batch), tiles(N));
+        Bc = (int)std::min(tiles(c.pred_batch), tiles(NL));
         return CTR_OK;
     }
-    // the classifier's activation buffers for one chunk (the last holds the logits) and layer 0's launch shape
+    // the classifier's activation buffers for one chunk (the last holds the logits) and layer 0's launch shape; on a
+    // row-sharded ITEM_EMB before the agreement, so that a rank which cannot allocate them says so in its verdict
     int prepare() {
         for (int l = 1; l < L; l++) {
             const size_t need = (size_t)Bc * m->d.units[l];
@@ -4596,6 +4629,8 @@ struct MlpRecScore {
         l0_ctas = m->num_sms * std::max(1, l0_per_sm);
         return CTR_OK;
     }
+    // the rows the prefix reads; on a row-sharded ITEM_EMB after the agreement has published the peer mappings
+    void bind_rows() { src = coll ? comm_src(h, nullptr, nullptr, nullptr, 0, false) : idx_src(h, nullptr, nullptr, nullptr, 0); }
     decltype(&k_mlp64_rec_layer0<true>) l0() const { return smem_w ? k_mlp64_rec_layer0<true> : k_mlp64_rec_layer0<false>; }
     const double* z() const { return m->act[L - 1]; }
     // user row u with window uh (device): layer 0's user columns into d_pre [H]
@@ -4603,16 +4638,22 @@ struct MlpRecScore {
         const ctr_config& c = h->cfg;
         const float* up = (c.uP > 0 && u < h->tab_rows[CTR_TABLE_USER_FEAT]) ? h->tab[CTR_TABLE_USER_FEAT] + (long)u * h->tab_ld[CTR_TABLE_USER_FEAT] : nullptr;
         return launch(h, "mlp_rec_prefix", [&] {
-            k_mlp64_prefix<<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], (int)N, uh, c.S, c.D, d_pre);
+            if (coll) k_mlp64_prefix<true><<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, src, uh, c.S, c.D, d_pre);
+            else k_mlp64_prefix<false><<<(H + 127) / 128, 128, 0, h->stream>>>(m->params, m->d, up, c.uP, src, uh, c.S, c.D, d_pre);
         });
     }
-    // the logits of items [i0, i0 + nb) from d_pre into z()
+    // the logits of (local) items [i0, i0 + nb) from d_pre into z()
     int chunk(const double* d_pre, int i0, int nb) {
         const ctr_config& c = h->cfg;
+        const int F = CTR_TABLE_ITEM_FEAT;
         const int ctas = std::min(l0_ctas, (nb + kRecTile - 1) / kRecTile);
+        // ITEM_FEAT beside a row-sharded ITEM_EMB: sharded alike (local rows), or replicated (global rows)
+        const bool fsh = coll && h->tab_sharded[F];
+        const int fworld = coll && !fsh ? h->comm.world : 1, frank = coll && !fsh ? h->comm.rank : 0;
         RET(launch(h, "mlp_rec_layer0", [&] {
-            l0()<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], h->tab[CTR_TABLE_ITEM_FEAT],
-                                                  h->tab_ld[CTR_TABLE_ITEM_FEAT], (long)h->tab_rows[CTR_TABLE_ITEM_FEAT], c.D, c.cF, (long)i0, nb, m->act[1]);
+            l0()<<<ctas, 256, l0smem, h->stream>>>(m->params, m->d, d_pre, pcols, h->tab[CTR_TABLE_ITEM_EMB], h->tab_ld[CTR_TABLE_ITEM_EMB], h->tab[F],
+                                                  h->tab_ld[F], (long)(fsh ? h->tab_local_rows[F] : h->tab_rows[F]), fworld, frank, c.D, c.cF, (long)i0, nb,
+                                                  m->act[1]);
         }));
         for (int l = 1; l + 1 < L; l++)
             RET(launch(h, "mlp_rec_layers", [&] {
@@ -4624,46 +4665,78 @@ struct MlpRecScore {
 };
 
 // ctr_mlp_recommend_topk (see mlp64.cuh): per user, the prefix of layer 0 once; per chunk of items, layer 0 from it,
-// the later layers, and the selection of rec.cuh on the float64 logits.  Everything runs on h's stream.
-int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude,
+// the later layers, and the selection of rec.cuh on the float64 logits.  Everything runs on h's stream.  On a row-sharded
+// ITEM_EMB the call is collective (ctr_recommend_topk_ex's rule): every rank checks the call and resolves the user ids
+// with its own id map, the ranks agree, then each scores its shard for the windows rank 0's cache cuts, and the ranks'
+// lists of each group are all-gathered and merged: the same total order over the same logits, so one GPU's result.
+// args: CTR_OK, or the refusal of the caller's arguments (a collective call still takes part in the agreement).
+int mlp_recommend(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude,
                   int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
     MlpRecScore sc{m, h};
-    RET(sc.check());
-    const int S = h->cfg.S, H = sc.H;
+    const bool coll = emb_sharded(h);
+    const int W = coll ? h->comm.world : 1, S = h->cfg.S;
+    const int vcheck = args != CTR_OK ? args : [&]() -> int { RET(mlp_keys_check(m, h)); return sc.check(); }();
 
     // ---- every user id, resolved before anything is written
-    const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy
+    const int64_t G = std::min<int64_t>(nu, 256);                        // users per result copy (and list all-gather)
     const bool seen = exclude == CTR_EXCLUDE_SEEN;
-    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, 1, 0, sc.N, sc.Bc, seen};
+    RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, sc.NL, sc.Bc, seen, sc.N};
     long long *d_ids, *d_ts; int *d_urow, *d_hist; double* d_pre;
-    RET(sel.setup(6, G, [&](Carve& cv) {
-        d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
-        d_pre = cv.take<double>(H);
-    }));
-    CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)nu * 8, cudaMemcpyHostToDevice, h->stream));
-    RET(launch(h, "mlp_rec_resolve", [&] {
-        k_idmap_lookup<<<mlp_grid(m, (long)nu), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, d_ids, (long)nu, d_urow);
-    }));
-    std::vector<int> urow((size_t)nu);
-    CU(h, cudaMemcpyAsync(urow.data(), d_urow, (size_t)nu * 4, cudaMemcpyDeviceToHost, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
-    for (int64_t u = 0; u < nu; u++)                                     // serving.Recommend's rule: the first unknown user
-        if (urow[(size_t)u] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[u]);
+    double* d_gs = nullptr; int* d_gr = nullptr;                         // [W][G][k] the ranks' lists of the group
+    std::vector<int> urow;
+    const int verdict = vcheck != CTR_OK ? vcheck : [&]() -> int {
+        RET(sel.setup(6, G, [&](Carve& cv) {
+            d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
+            d_pre = cv.take<double>(sc.H);
+            if (coll) { d_gs = cv.take<double>((size_t)W * G * k); d_gr = cv.take<int>((size_t)W * G * k); }
+        }));
+        CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)nu * 8, cudaMemcpyHostToDevice, h->stream));
+        RET(launch(h, "mlp_rec_resolve", [&] {
+            k_idmap_lookup<<<mlp_grid(m, (long)nu), 256, 0, h->stream>>>(h->idm_keys[0], h->idm_vals[0], h->idm_keys[0].size() - 1, d_ids, (long)nu, d_urow);
+        }));
+        urow.resize((size_t)nu);
+        CU(h, cudaMemcpyAsync(urow.data(), d_urow, (size_t)nu * 4, cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        for (int64_t u = 0; u < nu; u++)                                 // serving.Recommend's rule: the first unknown user
+            if (urow[(size_t)u] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[u]);
+        return sc.prepare();
+    }();
+    if (!coll) RET(verdict);
+    else {
+        CommHdr hd{};
+        hd.n = nu; hd.k = k; hd.flag = exclude;
+        if (args == CTR_OK) {
+            hd.hash[0] = comm_hash(user_ids, (size_t)nu * sizeof(int64_t));
+            hd.hash[1] = comm_hash(ts, (size_t)nu * sizeof(int64_t));
+            hd.plan = G;                                                 // users per list all-gather
+        }
+        if (verdict == CTR_OK) hd.rows = comm_hash(urow.data(), (size_t)nu * sizeof(int));
+        RET(mlp_agree(m, h, hd, verdict));
+    }
 
-    RET(sc.prepare());
+    sc.bind_rows();
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
         const int ng = (int)std::min<int64_t>(G, nu - g0);
-        // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys)
+        // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys).
+        // On a shard every rank takes rank 0's windows, so every rank scores for the same ones.
         if (h->ub_off) {
             CU(h, cudaMemcpyAsync(d_ts, ts + g0, sizeof(long long) * (size_t)ng, cudaMemcpyHostToDevice, h->stream));
             RET(launch(h, "ubcache_window", [&] {
                 k_ub_window<<<grid_for_warps(h, ng), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow + g0, d_ts, ng, S, (long)h->ub_users, d_hist);
             }));
         } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)ng * S, h->stream));
+        if (coll && S > 0) RET(comm_bcast0(h, d_hist, sizeof(int) * (size_t)ng * S));
         for (int j = 0; j < ng; j++) {
             const int* uh = d_hist + (size_t)j * S;
             RET(sc.prefix(urow[(size_t)(g0 + j)], uh, d_pre));
             RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, urow[(size_t)(g0 + j)], ts[g0 + j]));
+        }
+        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
+            const long n = (long)ng * k;
+            RET(comm_gather_lists(h, sel.ls, d_gs, sizeof(double), sel.lr, d_gr, (size_t)n));
+            RET(launch(h, "mlp_rec_merge_ranks", [&] {
+                knn::k_knn_merge<knn::Logit64Key><<<ng, knn::kThreads, sel.msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, sel.lr, sel.ls, nullptr);
+            }));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [&](long n) {
             // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
@@ -4674,34 +4747,58 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int6
 }
 
 // ctr_mlp_rank_items: mlp_recommend's scoring pass, counted by rec.cuh's rank kernels.  Keys with the same user row and
-// ts share a pass, and so a window.
-int mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
+// ts share a pass, and so a window.  On a row-sharded ITEM_EMB the call is collective (ctr_rank_items_ex's rule), with
+// mlp_recommend's agreement and rank 0's windows; each rank counts its shard and RecRank sums the counts.
+int mlp_rank_items(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
                    int32_t exclude, int64_t* out_rank, double* out_logit) {
     MlpRecScore sc{m, h};
-    RET(sc.check());
+    const bool coll = emb_sharded(h);
     const int S = h->cfg.S;
-    RecRank<knn::Logit64Key> rk{h, "mlp_rank", exclude == CTR_EXCLUDE_WINDOW ? S : 0, sc.N, sc.Bc, 1, 0, sc.N, exclude == CTR_EXCLUDE_SEEN};
+    const int vcheck = args != CTR_OK ? args : [&]() -> int { RET(mlp_keys_check(m, h)); return sc.check(); }();
+    RecRank<knn::Logit64Key> rk{h, "mlp_rank", exclude == CTR_EXCLUDE_WINDOW ? S : 0, sc.NL, sc.Bc, coll ? h->comm.world : 1, coll ? h->comm.rank : 0,
+                                sc.N, exclude == CTR_EXCLUDE_SEEN};
     long long *d_ids, *d_ts; int *d_rows, *d_urow, *d_hist; double* d_pre;
-    RET(rk.setup(6, [&](Carve& cv) {
-        d_ids = cv.take<long long>((size_t)2 * n); d_rows = cv.take<int>((size_t)2 * n); d_ts = cv.take<long long>(n); d_urow = cv.take<int>(n);
-        d_hist = cv.take<int>((size_t)n * S); d_pre = cv.take<double>(sc.H);
-    }));
+    std::vector<int> rows;
+    std::vector<std::vector<int64_t>> passes;
     // ---- user and item ids → rows; every user resolved before anything is written
-    CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaMemcpyAsync(d_ids + n, item_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
-    RET(launch(h, "mlp_rank_resolve", [&] {
-        for (int w = 0; w < 2; w++)
-            k_idmap_lookup<<<mlp_grid(m, (long)n), 256, 0, h->stream>>>(h->idm_keys[w], h->idm_vals[w], h->idm_keys[w].size() - 1, d_ids + w * n, (long)n, d_rows + w * n);
-    }));
-    std::vector<int> rows((size_t)2 * n);
-    CU(h, cudaMemcpyAsync(rows.data(), d_rows, (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
-    for (int64_t i = 0; i < n; i++)
-        if (rows[(size_t)i] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[i]);
+    const int verdict = vcheck != CTR_OK ? vcheck : [&]() -> int {
+        RET(rk.setup(6, [&](Carve& cv) {
+            d_ids = cv.take<long long>((size_t)2 * n); d_rows = cv.take<int>((size_t)2 * n); d_ts = cv.take<long long>(n); d_urow = cv.take<int>(n);
+            d_hist = cv.take<int>((size_t)n * S); d_pre = cv.take<double>(sc.H);
+        }));
+        CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+        CU(h, cudaMemcpyAsync(d_ids + n, item_ids, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+        RET(launch(h, "mlp_rank_resolve", [&] {
+            for (int w = 0; w < 2; w++)
+                k_idmap_lookup<<<mlp_grid(m, (long)n), 256, 0, h->stream>>>(h->idm_keys[w], h->idm_vals[w], h->idm_keys[w].size() - 1, d_ids + w * n, (long)n, d_rows + w * n);
+        }));
+        rows.resize((size_t)2 * n);
+        CU(h, cudaMemcpyAsync(rows.data(), d_rows, (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        for (int64_t i = 0; i < n; i++)
+            if (rows[(size_t)i] < 0) return mlp_err(m, CTR_ENOTFOUND, "user %lld is not found", (long long)user_ids[i]);
+        passes = rank_passes(n, [&](int64_t i) { return std::make_pair(rows[(size_t)i], ts[i]); });
+        return sc.prepare();
+    }();
+    if (!coll) RET(verdict);
+    else {
+        CommHdr hd{};
+        hd.n = n; hd.flag = exclude;
+        if (args == CTR_OK) {
+            hd.hash[0] = comm_hash(user_ids, (size_t)n * sizeof(int64_t));
+            hd.hash[1] = comm_hash(ts, (size_t)n * sizeof(int64_t));
+            hd.hash[2] = comm_hash(item_ids, (size_t)n * sizeof(int64_t));
+        }
+        if (verdict == CTR_OK) {
+            hd.rows = comm_hash(rows.data(), (size_t)2 * n * sizeof(int));   // the user rows, then the item rows
+            hd.plan = (int64_t)passes.size();                                // two collectives per pass
+        }
+        RET(mlp_agree(m, h, hd, verdict));
+    }
     const int* urow = rows.data(); const int* irow = rows.data() + n;
 
-    // ---- one window per (user row, ts): GetUserBehavior(uid, S, -1, ts) from the device ubcache, empty without one
-    const auto passes = rank_passes(n, [&](int64_t i) { return std::make_pair(urow[i], ts[i]); });
+    // ---- one window per (user row, ts): GetUserBehavior(uid, S, -1, ts) from the device ubcache, empty without one;
+    // on a shard rank 0's
     std::vector<int> pu; std::vector<long long> pts;           // the distinct (user, ts) in pass order, each once
     std::vector<size_t> win(passes.size());
     for (size_t p = 0; p < passes.size(); p++) {
@@ -4717,8 +4814,9 @@ int mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int
             k_ub_window<<<grid_for_warps(h, nw), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow, d_ts, nw, S, (long)h->ub_users, d_hist);
         }));
     } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)nw * S, h->stream));
+    if (coll && S > 0) RET(comm_bcast0(h, d_hist, sizeof(int) * (size_t)nw * S));
 
-    RET(sc.prepare());
+    sc.bind_rows();
     std::vector<int64_t> rank((size_t)n); std::vector<double> logit((size_t)n), pl(knn::kMaxK);
     std::vector<int> trow(knn::kMaxK); std::vector<int64_t> pr(knn::kMaxK);
     for (size_t p = 0; p < passes.size(); p++) {
@@ -4745,7 +4843,10 @@ int ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
     std::lock_guard<std::mutex> lh(h->mu);                           // the feature store first, then the classifier
     std::lock_guard<std::mutex> lm(m->mu);
     m->err.clear(); h->err.clear();
-    int rc = mlp_keys_check(m, h);
+    int rc = h->comm.world > 1 ? mlp_err(m, CTR_ESTATE, "ctr_mlp_fit_keys trains on one GPU (world=%d): data-parallel float64 training would "
+                                                        "not keep fit's bit-for-bit result; fit on one GPU and serve the parameters on every rank "
+                                                        "through ctr_mlp_set_params", h->comm.world)
+                               : mlp_keys_check(m, h);
     if (rc == CTR_OK) rc = mlp_fit_keys(m, h, user_ids, item_ids, ts, label, n, n_iter, loss_curve, rows_used);
     return mlp_keys_done(m, h, rc);
 }
@@ -4770,14 +4871,18 @@ int ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, c
 int ctr_mlp_recommend_topk_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k, int32_t exclude,
                               int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count) {
     if (!m) return CTR_EINVAL;
-    if (!h || !user_ids || !ts || !out_rows || !out_scores || !out_count || nu < 1 || k < 1 || k > knn::kMaxK)
-        return mlp_err(m, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user ids and ts, non-null outputs)", knn::kMaxK);
-    if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
+    auto args = [&]() -> int {
+        if (!h || !user_ids || !ts || !out_rows || !out_scores || !out_count || nu < 1 || k < 1 || k > knn::kMaxK)
+            return mlp_err(m, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user ids and ts, non-null outputs)", knn::kMaxK);
+        if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
+        return CTR_OK;
+    };
+    if (!h) return args();
     std::lock_guard<std::mutex> lh(h->mu);
     std::lock_guard<std::mutex> lm(m->mu);
+    if (!emb_sharded(h)) RET(args());    // a collective call: a rank with bad arguments still takes part in the agreement
     m->err.clear(); h->err.clear();
-    int rc = mlp_keys_check(m, h);
-    if (rc == CTR_OK) rc = mlp_recommend(m, h, user_ids, ts, nu, k, exclude, out_rows, out_scores, out_logits, out_count);
+    const int rc = mlp_recommend(m, h, args(), user_ids, ts, nu, k, exclude, out_rows, out_scores, out_logits, out_count);
     return mlp_keys_done(m, h, rc);
 }
 
@@ -4789,14 +4894,18 @@ int ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const
 int ctr_mlp_rank_items_ex(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
                           int32_t exclude, int64_t* out_rank, double* out_logit) {
     if (!m) return CTR_EINVAL;
-    if (!h || !user_ids || !item_ids || !ts || !out_rank || n < 1 || n > INT32_MAX)
-        return mlp_err(m, CTR_EINVAL, "bad rank arguments (n in [1, 2^31), user ids, item ids and ts, non-null out_rank)");
-    if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
+    auto args = [&]() -> int {
+        if (!h || !user_ids || !item_ids || !ts || !out_rank || n < 1 || n > INT32_MAX)
+            return mlp_err(m, CTR_EINVAL, "bad rank arguments (n in [1, 2^31), user ids, item ids and ts, non-null out_rank)");
+        if (!exclude_ok(exclude, ts)) return mlp_err(m, CTR_EINVAL, "bad exclusion mode %d (CTR_EXCLUDE_NONE, _WINDOW or _SEEN)", exclude);
+        return CTR_OK;
+    };
+    if (!h) return args();
     std::lock_guard<std::mutex> lh(h->mu);
     std::lock_guard<std::mutex> lm(m->mu);
+    if (!emb_sharded(h)) RET(args());    // a collective call: a rank with bad arguments still takes part in the agreement
     m->err.clear(); h->err.clear();
-    int rc = mlp_keys_check(m, h);
-    if (rc == CTR_OK) rc = mlp_rank_items(m, h, user_ids, item_ids, ts, n, exclude, out_rank, out_logit);
+    const int rc = mlp_rank_items(m, h, args(), user_ids, item_ids, ts, n, exclude, out_rank, out_logit);
     return mlp_keys_done(m, h, rc);
 }
 

@@ -74,11 +74,14 @@ k_mlp64_layer(const double* __restrict__ params, Mlp64Dims d, int l, const doubl
 // the same bits as the predict route.  No DMMA: its accumulation order differs.
 
 // pre[j] = sum_{k < pcols} x[k]·W0[k, j], x = [USER_FEAT row urow | ITEM_EMB rows hist[0, S)], widened from float32 as
-// k_gather_rows<double> widens them.  A missing row (urow == nullptr, a history row outside [0, n_emb)) is zeros, and
-// its columns are walked like any other: 0·inf stays NaN, as on the predict route.
+// k_gather_rows<double> widens them.  A missing row (urow == nullptr, a history row outside [0, r.n_emb)) is zeros, and
+// its columns are walked like any other: 0·inf stays NaN, as on the predict route.  The ITEM_EMB rows are r.emb's;
+// PEER (a row-sharded ITEM_EMB) reads them through emb_src<true> as k_attn_fwd_user<PEER> stages the DIN history: the
+// hot rows from this rank's replica, the rest from their owners.  The DFMA chain is the same in both forms.
+template <bool PEER>
 __global__ void __launch_bounds__(128)
 k_mlp64_prefix(const double* __restrict__ params, Mlp64Dims d, const float* __restrict__ urow, int uP,
-               const float* __restrict__ emb, long lde, int n_emb, const int* __restrict__ hist, int S, int D, double* __restrict__ pre) {
+               RowSrc r, const int* __restrict__ hist, int S, int D, double* __restrict__ pre) {
     const int fo = d.units[1];
     const double* W = params + d.off[0] + fo;
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < fo; j += gridDim.x * blockDim.x) {
@@ -87,7 +90,7 @@ k_mlp64_prefix(const double* __restrict__ params, Mlp64Dims d, const float* __re
         for (int c = 0; c < uP; c++, k++) z += (urow ? (double)__ldg(urow + c) : 0.0) * W[k * fo + j];
         for (int s = 0; s < S; s++) {
             const int row = __ldg(hist + s);
-            const float* e = row_ok(row, n_emb) ? emb + (long)row * lde : nullptr;
+            const float* e = row_ok(row, r.n_emb) ? (PEER ? emb_src<true>(r, row) : r.emb + (long)row * r.lde) : nullptr;
             for (int c = 0; c < D; c++, k++) z += (e ? (double)__ldg(e + c) : 0.0) * W[k * fo + j];
         }
         pre[j] = z;
@@ -109,10 +112,14 @@ __host__ inline size_t rec_layer0_smem(int T, int H, bool smem_w) {
 // the logit.  A CTA stages the W0 rows of the item columns once (SMEM_W; else they are read through L1), then walks
 // tiles of kRecTile items: the tile's columns are read from HBM once, coalesced, and each warp takes kRecJ units at a
 // time for all the tile's items, so a W0 value in shared memory is a broadcast and an item value a conflict-free read.
+// emb holds the rows this GPU scores: the whole table, or on a row-sharded ITEM_EMB this rank's shard (local row l is
+// global row l·world + rank).  Item row l's ITEM_FEAT row is l·fworld + frank: fworld = world, frank = rank for a
+// replicated ITEM_FEAT beside a sharded ITEM_EMB (n_ifeat its global rows); 1 and 0 for a sharded ITEM_FEAT (n_ifeat
+// its local rows) and on one GPU.
 template <bool SMEM_W>
 __global__ void __launch_bounds__(256)
 k_mlp64_rec_layer0(const double* __restrict__ params, Mlp64Dims d, const double* __restrict__ pre, int pcols,
-                   const float* __restrict__ emb, long lde, const float* __restrict__ ifeat, long ldi, long n_ifeat,
+                   const float* __restrict__ emb, long lde, const float* __restrict__ ifeat, long ldi, long n_ifeat, int fworld, int frank,
                    int D, int cF, long row0, int n, double* __restrict__ out) {
     extern __shared__ __align__(16) char smem_raw[];
     const int H = d.units[1], Hp = rec_units_pad(H), T = D + cF, Tp = rec_tile_pitch(T);
@@ -135,9 +142,9 @@ k_mlp64_rec_layer0(const double* __restrict__ params, Mlp64Dims d, const double*
             const int r = i / T, c = i - r * T;
             float v = 0.0f;
             if (r < nb) {
-                const long row = row0 + b0 + r;
+                const long row = row0 + b0 + r, frow = row * fworld + frank;
                 if (c < D) v = __ldg(emb + row * lde + c);
-                else if (row < n_ifeat) v = __ldg(ifeat + row * ldi + (c - D));
+                else if (frow < n_ifeat) v = __ldg(ifeat + frow * ldi + (c - D));
             }
             xs[r * Tp + c] = v;
         }

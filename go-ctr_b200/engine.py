@@ -820,7 +820,10 @@ class _Mlp64:
 
     def predict_keys(self, engine, user_ids, item_ids, ts):
         """recommend.BatchPredict for the MLP over sample keys (ctr_mlp_predict_keys) → float32 [n].  An unknown key
-        scores as an all-zero row, except key 0, which raises CtrError with code ENOTFOUND."""
+        scores as an all-zero row, except key 0, which raises CtrError with code ENOTFOUND.  On a row-sharded ITEM_EMB
+        (world > 1) each rank scores its own keys and reads the rows from their owners, as Engine.batch_predict_keys
+        does: the first call after a table change publishes the shard mappings and must run on every rank, and a
+        prediction after training needs sync() on every rank and a barrier between the processes first."""
         u, i, t = self._keys(user_ids, item_ids, ts)
         out = np.empty(u.size, np.float32)
         self._ck(self.L.ctr_mlp_predict_keys(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp),
@@ -834,7 +837,11 @@ class _Mlp64:
         positions past a user's count hold row -1, score 0 and logit 0.  Each score is bit for bit what predict_keys
         returns for (user, the row's item id, ts).  An unknown user raises CtrError with code ENOTFOUND.  exclude_seen
         (implies exclude_history) also drops every item of the user's ubcache events with ts <= the user's ts (0: every
-        event)."""
+        event).  On a row-sharded ITEM_EMB (world > 1) the call is collective: every rank calls it with the same
+        arguments and gets the same complete result, bit-identical to one GPU holding the whole table; arguments or id
+        maps that differ across ranks raise CtrError (EINVAL) everywhere, else every rank raises the lowest failing rank's
+        error.  Each user's window is the one rank 0's ubcache cuts; under exclude_seen the owner of a row decides from
+        its own ubcache.  No sync() is needed after training."""
         u = np.atleast_1d(np.ascontiguousarray(user_ids, np.int64)); t = np.atleast_1d(np.ascontiguousarray(ts, np.int64))
         if u.size != t.size:
             raise ValueError("user_ids and ts differ in length: %d, %d" % (u.size, t.size))
@@ -851,7 +858,8 @@ class _Mlp64:
         """Full-catalogue rank of held-out items over the feature store `engine` (ctr_mlp_rank_items): key i is (user,
         item, ts) in external ids, windowed at ts as recommend_topk windows it.  Returns (ranks [n] int64, logits [n]
         float64) under Engine.rank_items' rules; an unknown item id ranks -1 (logit NaN), an unknown user raises CtrError
-        with code ENOTFOUND.  exclude_seen as for recommend_topk, each key cut at its ts."""
+        with code ENOTFOUND.  exclude_seen as for recommend_topk, each key cut at its ts.  On a row-sharded ITEM_EMB the
+        call is collective under recommend_topk's rule."""
         u, i, t = self._keys(np.atleast_1d(user_ids), np.atleast_1d(item_ids), np.atleast_1d(ts))
         mode = _exclusion(u.size, None, exclude_history, exclude_seen)[0]
         ranks = np.empty(u.size, np.int64); logits = np.empty(u.size, np.float64)

@@ -962,6 +962,7 @@ func (f *MlpRegressorFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAb
 // feature store (id maps, tables, optional ubcache), samples are its keys.  Samples whose user or item is unknown are
 // dropped; rowsUsed counts the rest.  The classifier has e's uP + S·D + D + cF inputs and trains bit for bit as Fit
 // would on the rows GetSample builds.  The options and refusals are Fit's.  The predictor serves keys through e.
+// FitKeys needs a single-GPU feature store: on a multi-GPU one, fit on one GPU and install the parameters on every rank.
 func (f *MlpFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
 	return f.fitKeys(e, samples, false)
 }
@@ -998,7 +999,8 @@ func (f *MlpFitWrap) fitKeys(e *Engine, samples []rcmd.Sample, regressor bool) (
 }
 
 // BatchPredict is recommend.BatchPredict (rcmd.go:277-337) for the MLP over the feature store e: an unknown key scores
-// as an all-zero row, except key 0, which is an error.
+// as an all-zero row, except key 0, which is an error.  On a row-sharded ITEM_EMB (world > 1) each rank scores its own
+// keys under (*Engine).BatchPredict's rule: Sync on every rank and a barrier between training and prediction.
 func (p *MlpPredWrap) BatchPredict(e *Engine, sampleKeys []rcmd.Sample) ([]float32, error) {
 	n := len(sampleKeys)
 	if n == 0 {
@@ -1040,6 +1042,8 @@ func (p *MlpPredWrap) Rank(e *Engine, userId int, itemIds []int) ([]rcmd.ItemSco
 // valid.  Each score is what BatchPredict returns for (user, the row's item id, ts[j]).  An unknown user is an error,
 // and so is a classifier fitted on labels other than 0 / 1: it predicts labels, so it has no click probability to
 // rank items by (CTR_ESTATE, with nothing written).
+// With a row-sharded ITEM_EMB (world > 1) Recommend is collective, under the same rule as (*Engine).Recommend: every
+// rank calls it with the same users, ts and k and gets the same result; the users' windows are rank 0's.
 func (p *MlpPredWrap) Recommend(e *Engine, userIds []int, ts []int64, k int, excludeHistory bool) (outRows []int32, scores []float32, logits []float64, counts []int32, err error) {
 	return p.recommend(e, userIds, ts, k, windowMode(excludeHistory))
 }
@@ -1073,7 +1077,8 @@ func (p *MlpPredWrap) recommend(e *Engine, userIds []int, ts []int64, k int, mod
 // RankItems is the full-catalogue rank of held-out items for the MLP: key i is (userIds[i], itemIds[i], ts[i]), the
 // user's window cut at ts[i] as Recommend cuts it, and ranks[i] the place the item would take in Recommend's list for
 // (userIds[i], ts[i]), or -1 when it can never be listed (an unknown item id, an excluded window row, a NaN logit).
-// logits[i] is the list's float64 logit for the item. An unknown user is an error.
+// logits[i] is the list's float64 logit for the item. An unknown user is an error.  With a row-sharded ITEM_EMB it is
+// collective, as Recommend.
 func (p *MlpPredWrap) RankItems(e *Engine, userIds, itemIds []int, ts []int64, excludeHistory bool) (ranks []int64, logits []float64, err error) {
 	return p.rankItems(e, userIds, itemIds, ts, windowMode(excludeHistory))
 }

@@ -736,9 +736,15 @@ int  ctr_mlp_set_output(ctr_mlp* m, int32_t kind);
  *   it is key 0, which fails the call with CTR_ENOTFOUND (rcmd.go:300-303).
  * A regressor takes each key's label as its target (one target: units[n_layers-1] must be 1, else CTR_EINVAL).
  * Refusals change nothing: CTR_EINVAL for null or short arguments, a width mismatch, or m and h on different devices;
- * CTR_ESTATE for a missing id map, missing tables, h with world > 1 (sharded feature stores are not served), and
- * predict before any fit or ctr_mlp_set_params.  The message is readable through both ctr_mlp_last_error(m) and
- * ctr_last_error(h).
+ * CTR_ESTATE for a missing id map, missing tables, and predict before any fit or ctr_mlp_set_params.  The message is
+ * readable through both ctr_mlp_last_error(m) and ctr_last_error(h).
+ * Multi-GPU feature stores (world > 1): fit_keys is CTR_ESTATE — data-parallel float64 training would not keep fit's
+ *   bit-for-bit result; fit on one GPU and serve the parameters on every rank through ctr_mlp_set_params.  predict with
+ *   ITEM_EMB and ITEM_FEAT both replicated serves from this GPU's tables alone; with a row-sharded ITEM_EMB (ITEM_FEAT
+ *   sharded or replicated) each rank scores its own keys and reads the rows from their owners, the hot rows from its
+ *   replica, under ctr_batch_predict_keys' rule: the first call after a table change publishes the shard mappings and
+ *   must run on every rank, and after training every rank calls ctr_sync and the processes meet at a barrier before
+ *   predicting.  A replicated ITEM_EMB beside a sharded ITEM_FEAT is CTR_ESTATE.
  * Locking: both calls take h's mutex, then m's.  A caller that holds either object's lock across calls must take
  * them in the same order. */
 int  ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
@@ -758,11 +764,20 @@ int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, co
  *     logit and, as float32, the score; one with a logistic output (0/1 targets) is the binary classifier.
  *   Refusals write nothing: CTR_EINVAL for k outside [1, 1024], nu < 1, null inputs or outputs and ctr_mlp_predict_keys'
  *     argument refusals; CTR_ESTATE for a classifier not fitted or with classes (it predicts labels, not a click
- *     probability), a model with more than one output, a missing id map or table,
- *     or world > 1; CTR_ENOTFOUND for any unknown user id, naming the first.
+ *     probability), a model with more than one output, a missing id map or table; CTR_ENOTFOUND for any unknown user
+ *     id, naming the first.
  *   Items are scored in chunks of h's pred_batch (whole tiles of 128) in the classifier's activation buffers,
  *     pred_batch · (units[1] + … + units[L-1]) · 8 bytes: a large catalogue wants a large pred_batch.  Only nu·k
- *     results cross PCIe.  Locking: h's mutex, then m's. */
+ *     results cross PCIe.  Locking: h's mutex, then m's.
+ *   Multi-GPU feature stores: with ITEM_EMB and ITEM_FEAT both replicated each rank serves alone from its own tables.
+ *     On a row-sharded ITEM_EMB the call is collective, under ctr_recommend_topk's rule: every rank calls it with the
+ *     same arguments and gets the same complete result, bit-identical to one GPU holding the whole table.  Each rank
+ *     resolves the ids with its own id map; arguments or resolved rows that differ across ranks are CTR_EINVAL on
+ *     every rank, else every rank returns the lowest failing rank's verdict (CTR_ENOTFOUND for an unknown user
+ *     included).  Each user's window is the one rank 0's ubcache cuts (with equal caches, the single-GPU window);
+ *     CTR_EXCLUDE_SEEN follows ctr_recommend_topk_ex's owner rule.  Each rank scores its own rows: per group of 256
+ *     users one broadcast of rank 0's windows and one all-gather of the lists.  No ctr_sync is needed after training.
+ *     Scratch: [world][min(nu, 256)][k] gathered lists, 12 bytes an entry, beside the single-GPU scratch. */
 int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* ts, int64_t nu, int32_t k,
                             int32_t exclude_history, int32_t* out_rows, float* out_scores, double* out_logits, int32_t* out_count);
 /* Full-catalogue rank of held-out items with the classifier, ctr_rank_items' definition over ctr_mlp_recommend_topk's
@@ -775,8 +790,12 @@ int  ctr_mlp_recommend_topk(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, 
  * share one scoring pass (1024 targets at most).
  *   Refusals write nothing: CTR_EINVAL for n outside [1, 2^31), null inputs or out_rank and ctr_mlp_predict_keys'
  *     argument refusals; CTR_ESTATE as ctr_mlp_recommend_topk (not fitted, classes, more than one output, a missing id
- *     map or table, world > 1); CTR_ENOTFOUND for any unknown user id, naming the first.
- *   Locking: h's mutex, then m's; everything runs on h's stream. */
+ *     map or table); CTR_ENOTFOUND for any unknown user id, naming the first.
+ *   Locking: h's mutex, then m's; everything runs on h's stream.
+ *   Multi-GPU feature stores as ctr_mlp_recommend_topk: collective on a row-sharded ITEM_EMB, the item ids hashed with
+ *     the user ids and ts and the resolved rows compared; one broadcast of rank 0's windows per call, then per pass an
+ *     all-gather of the targets' logits (8 bytes each, [world][m], and the owners' seen flags) and a sum of the
+ *     counts. */
 int  ctr_mlp_rank_items(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n,
                         int32_t exclude_history, int64_t* out_rank, double* out_logit);
 /* The classifier's recommendation and rank with an exclusion mode (CTR_EXCLUDE_*): the plain calls are these with
