@@ -1224,6 +1224,29 @@ k_table_write_rows(float* __restrict__ t, long ld, const int* __restrict__ rows,
         if (mo) for (long c = lane; c < ld; c += 32) { mo[dst + c] = 0.0f; vo[dst + c] = 0.0f; }
     }
 }
+// ctr_table_write_rows on a row-sharded table (world > 1), on one rank: of the rows rows[i] (data [n, width] compact) it
+// writes the ones it owns (rows[i] % world == rank) into its shard at local row rows[i] / world, zeroing their row-Adam
+// moments mo / vo when non-null, and every row below hot_k into the hot-row replica hot ([hot_k, width]) when non-null,
+// zeroing its moments hm / hv when non-null.  Other rows are skipped.  One warp per row.
+__global__ void __launch_bounds__(256)
+k_shard_write_rows(float* __restrict__ t, long ld, const int* __restrict__ rows, const float* __restrict__ data, long n, int width,
+                   int world, int rank, float* __restrict__ mo, float* __restrict__ vo, float* __restrict__ hot, int hot_k,
+                   float* __restrict__ hm, float* __restrict__ hv) {
+    const int lane = threadIdx.x & 31;
+    for (long r = (blockIdx.x * (long)blockDim.x + threadIdx.x) >> 5; r < n; r += ((long)gridDim.x * blockDim.x) >> 5) {
+        const int row = rows[r];
+        if (row % world == rank) {
+            const long dst = (long)(row / world) * ld;
+            for (int c = lane; c < width; c += 32) t[dst + c] = data[r * width + c];
+            if (mo) for (long c = lane; c < ld; c += 32) { mo[dst + c] = 0.0f; vo[dst + c] = 0.0f; }
+        }
+        if (hot && row < hot_k) {
+            const long dst = (long)row * width;
+            for (int c = lane; c < width; c += 32) hot[dst + c] = data[r * width + c];
+            if (hm) for (int c = lane; c < width; c += 32) { hm[dst + c] = 0.0f; hv[dst + c] = 0.0f; }
+        }
+    }
+}
 // *dup = 1 when the ascending rows hold a value twice
 __global__ void __launch_bounds__(256)
 k_rows_dup(const int* __restrict__ sorted, long n, int* __restrict__ dup) {

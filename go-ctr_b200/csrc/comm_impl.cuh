@@ -17,6 +17,8 @@ struct NcclApi {
     int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
     int (*Broadcast)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
+    int (*Send)(const void*, size_t, int, int, void*, cudaStream_t) = nullptr;
+    int (*Recv)(void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     const char* (*GetErrorString)(int) = nullptr;
 };
 enum { kNcclChar = 0, kNcclInt32 = 2, kNcclInt64 = 4, kNcclUint64 = 5, kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2 };
@@ -32,7 +34,8 @@ bool nccl_load(std::string* err) {
 #define SYM(field, name) *(void**)(&g_nccl.field) = dlsym(lib, name); if (!g_nccl.field) { *err = std::string("missing NCCL symbol ") + name; return false; }
     SYM(GetUniqueId, "ncclGetUniqueId") SYM(CommInitRank, "ncclCommInitRank") SYM(CommDestroy, "ncclCommDestroy")
     SYM(GroupStart, "ncclGroupStart") SYM(GroupEnd, "ncclGroupEnd")
-    SYM(AllReduce, "ncclAllReduce") SYM(AllGather, "ncclAllGather") SYM(Broadcast, "ncclBroadcast") SYM(GetErrorString, "ncclGetErrorString")
+    SYM(AllReduce, "ncclAllReduce") SYM(AllGather, "ncclAllGather") SYM(Broadcast, "ncclBroadcast")
+    SYM(Send, "ncclSend") SYM(Recv, "ncclRecv") SYM(GetErrorString, "ncclGetErrorString")
 #undef SYM
     g_nccl.lib = lib;
     return true;
@@ -348,6 +351,48 @@ static int comm_bcast0(ctr_handle* h, void* buf, size_t bytes) {
     Comm& cm = h->comm;
     NC(h, g_nccl.Broadcast(buf, buf, bytes, kNcclChar, 0, cm.nccl, h->stream));
     h->launches += 1;
+    return CTR_OK;
+}
+
+// k int64 of every rank: all[j·k + i] = rank j's mine[i] (k <= 32); synchronises the engine stream
+static int comm_gather_i64(ctr_handle* h, const int64_t* mine, int k, int64_t* all) {
+    Comm& cm = h->comm;
+    if (!cm.d_xchg) RET(dalloc(h, cm.d_xchg, 256 * (size_t)(kMaxPeers + 1), false));
+    int64_t* d = (int64_t*)cm.d_xchg.get();
+    CU(h, cudaMemcpyAsync(d, mine, sizeof(int64_t) * (size_t)k, cudaMemcpyHostToDevice, h->stream));
+    NC(h, g_nccl.AllGather(d, d + k, (size_t)k, kNcclInt64, cm.nccl, h->stream));
+    CU(h, cudaMemcpyAsync(all, d + k, sizeof(int64_t) * (size_t)k * cm.world, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return CTR_OK;
+}
+
+// The ranks' segments concatenated in rank order on every rank: rank j's cnt[j] elements of `bytes` each sit at off[j]
+// of buf (off[j] = cnt[0] + ... + cnt[j-1]; this rank's own segment is in place already), one broadcast per non-empty
+// segment in one group, on the engine stream
+static int comm_concat(ctr_handle* h, void* buf, size_t bytes, const int64_t* cnt, const int64_t* off) {
+    Comm& cm = h->comm;
+    NC(h, g_nccl.GroupStart());
+    for (int j = 0; j < cm.world; j++)
+        if (cnt[j] > 0) NC(h, g_nccl.Broadcast((char*)buf + (size_t)off[j] * bytes, (char*)buf + (size_t)off[j] * bytes, (size_t)cnt[j] * bytes, kNcclChar, j, cm.nccl, h->stream));
+    NC(h, g_nccl.GroupEnd());
+    return CTR_OK;
+}
+
+// Point to point by destination: send[soff[k], soff[k] + scnt[k]) goes to rank k and lands at recv[roff[j], roff[j] +
+// rcnt[j]) of the rank it came from (elements of `bytes` each); this rank's own part is a device copy.  One group, on the
+// engine stream.
+static int comm_route(ctr_handle* h, const void* send, const int64_t* scnt, const int64_t* soff, void* recv, const int64_t* rcnt, const int64_t* roff, size_t bytes) {
+    Comm& cm = h->comm;
+    const int me = cm.rank;
+    if (scnt[me] > 0)
+        CU(h, cudaMemcpyAsync((char*)recv + (size_t)roff[me] * bytes, (const char*)send + (size_t)soff[me] * bytes, (size_t)scnt[me] * bytes, cudaMemcpyDeviceToDevice, h->stream));
+    NC(h, g_nccl.GroupStart());
+    for (int k = 0; k < cm.world; k++) {
+        if (k == me) continue;
+        if (scnt[k] > 0) NC(h, g_nccl.Send((const char*)send + (size_t)soff[k] * bytes, (size_t)scnt[k] * bytes, kNcclChar, k, cm.nccl, h->stream));
+        if (rcnt[k] > 0) NC(h, g_nccl.Recv((char*)recv + (size_t)roff[k] * bytes, (size_t)rcnt[k] * bytes, kNcclChar, k, cm.nccl, h->stream));
+    }
+    NC(h, g_nccl.GroupEnd());
     return CTR_OK;
 }
 

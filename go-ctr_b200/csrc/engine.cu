@@ -3599,10 +3599,6 @@ int ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, i
     return rc;
 }
 
-namespace {
-struct MinPos { __device__ int operator()(int a, int b) const { return a < b ? a : b; } };
-}  // namespace
-
 // recommend.Train's embedding stage (rcmd.go:207-213, 538-545) into the handle's ITEM_EMB: first-appearance numbering of
 // the item-id stream on the device (item2vec.cuh, idmap.cuh), the trainer on that document, one scatter into the rows.
 int ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n, int64_t* vocab_ids, int64_t cap,
@@ -3702,68 +3698,177 @@ unsigned long long idmap_cap_for(int64_t n) {
     while (cap < 2ull * (unsigned long long)n) cap <<= 1;                 // load factor <= 0.5, as ctr_idmap_build
     return cap;
 }
-}  // namespace
 
-// The ids the map lacks get rows idm_n, idm_n + 1, ... in order of first occurrence, numbered as ctr_item_emb_train
-// numbers its side words: the probe (k_idmap_first_pos) marks them, k_i2v_dict_side + a radix sort + ReduceByKey(MinPos)
-// give each distinct one its first position, and a sort by that position is the order.  Only the missing ids are sorted.
-int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows) {
-    if (!h || !ids || which < 0 || which > 1 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad idmap insert arguments");
-    std::lock_guard<std::mutex> lk(h->mu);
-    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_idmap_insert is single-GPU (world = %d)", h->comm.world);
-    for (int64_t i = 0; i < n; i++)
-        if ((unsigned long long)ids[i] == kIdEmpty) return set_err(h, CTR_EINVAL, "idmap insert: id INT64_MIN is reserved (position %lld)", (long long)i);
-    CU(h, cudaSetDevice(h->dev));
+// The ids of d_ids [n] the map lacks, numbered as ctr_item_emb_train numbers its side words: the probe
+// (k_idmap_first_pos) marks them, k_i2v_dict_side + a radix sort + ReduceByKey(MinPos) give each distinct one its first
+// position.  k0 / p0 [u]: the distinct missing ids (ascending as uint64) and their first positions; d_rows [n]: the row of
+// every id the map holds, -1 for the others; m: the ids without a row.  tmp also fits the sort by position of u entries.
+struct IdmapSide {
+    DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
+    unsigned long long m = 0; int u = 0;
+};
+int idmap_number(ctr_handle* h, int which, const long long* d_ids, int64_t n, int* d_rows, unsigned long long* d_cnt, IdmapSide* s) {
+    cudaStream_t st = h->stream;
+    const int G = h->num_sms * 8;
+    s->m = (unsigned long long)n;
+    if (h->idm_keys[which]) {
+        RET(launch(h, "idmap_probe", [&] {
+            k_idmap_first_pos<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows, nullptr, d_cnt);
+        }));
+        CU(h, cudaMemcpyAsync(&s->m, d_cnt, sizeof s->m, cudaMemcpyDeviceToHost, st));
+    } else CU(h, cudaMemsetAsync(d_rows, 0xff, sizeof(int) * (size_t)n, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (s->m == 0) return CTR_OK;
+    const unsigned long long m = s->m;
+    CU(h, s->k0.alloc(m)); CU(h, s->k1.alloc(m)); CU(h, s->p0.alloc(m)); CU(h, s->p1.alloc(m)); CU(h, s->d_u.alloc(1));
+    size_t b1 = 0, b2 = 0, b3 = 0;
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b1, s->k0.get(), s->k1.get(), s->p0.get(), s->p1.get(), (int)m, 0, 64, st));
+    CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b2, s->k1.get(), s->k0.get(), s->p1.get(), s->p0.get(), s->d_u.get(), MinPos{}, (int)m, st));
+    CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b3, s->p0.get(), s->p1.get(), s->k0.get(), s->k1.get(), (int)m, 0, 32, st));
+    CU(h, s->tmp.alloc(std::max(b1, std::max(b2, b3))));
+    RET(launch(h, "idmap_number", [&] { k_i2v_dict_side<<<G, 256, 0, st>>>(d_rows, d_ids, (long)n, s->k0, s->p0, d_cnt + 1); }));
+    RET(launch(h, "idmap_number", [&] { size_t tb = s->tmp.size(); cub::DeviceRadixSort::SortPairs(s->tmp.get(), tb, s->k0.get(), s->k1.get(), s->p0.get(), s->p1.get(), (int)m, 0, 64, st); }));
+    RET(launch(h, "idmap_number", [&] { size_t tb = s->tmp.size(); cub::DeviceReduce::ReduceByKey(s->tmp.get(), tb, s->k1.get(), s->k0.get(), s->p1.get(), s->p0.get(), s->d_u.get(), MinPos{}, (int)m, st); }));
+    CU(h, cudaMemcpyAsync(&s->u, s->d_u, sizeof s->u, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+
+// fresh [u] (ids the map lacks, distinct, in row order) get rows R, R + 1, ...: a table at the capacity ctr_idmap_build
+// picks for the new count (the old entries rehashed into it, then swapped), the inserts, and d_rows [n] looked up again
+// when `lookup`
+int idmap_add(ctr_handle* h, int which, const unsigned long long* fresh, int u, const long long* d_ids, int64_t n, int* d_rows, bool lookup) {
     cudaStream_t st = h->stream;
     const int G = h->num_sms * 8;
     const int64_t R = h->idm_n[which];
     const bool have = (bool)h->idm_keys[which];
+    const unsigned long long cap = idmap_cap_for(R + u), old_cap = have ? h->idm_keys[which].size() : 0;
+    if (cap > old_cap) {
+        DevBuf<unsigned long long> nk; DevBuf<int> nv;
+        RET(dalloc(h, nk, (size_t)cap, false)); RET(dalloc(h, nv, (size_t)cap, false));
+        RET(launch(h, "idmap_clear", [&] { k_idmap_clear<<<G, 256, 0, st>>>(nk, nv, cap); }));
+        if (have) RET(launch(h, "idmap_rehash", [&] { k_idmap_rehash<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], old_cap, nk, nv, cap - 1); }));
+        h->idm_keys[which] = std::move(nk); h->idm_vals[which] = std::move(nv);        // cudaFree of the old table waits for the rehash
+    }
+    RET(launch(h, "idmap_insert", [&] {
+        k_idmap_insert<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, (const long long*)fresh, (long)u, h->k_flags, (int)R);
+    }));
+    h->idm_n[which] = R + u;
+    if (lookup) RET(launch(h, "idmap_lookup", [&] {
+        k_idmap_lookup<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows);
+    }));
+    return CTR_OK;
+}
+
+// World > 1: every rank numbers its own missing ids, the ranks all-gather their lists (counts, then the lists padded to
+// the longest) and each runs the same merge (idmap_merge_ranks, idmap.cuh) and inserts its result, so every map ends as
+// the single-GPU insert of the ranks' ids concatenated in rank order.  Before any write the ranks agree on the arguments'
+// verdicts and on the map they start from: its id count and the order-independent digest of its (id, row) pairs.
+int idmap_insert_ranks(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows) {
+    Comm& cm = h->comm;
+    const int W = cm.world;
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const bool args_ok = !(which < 0 || which > 1 || n < 0 || n > 0x7fffffffLL || (n > 0 && !ids));
+    int verdict = args_ok ? CTR_OK : set_err(h, CTR_EINVAL, "bad idmap insert arguments");
+    for (int64_t i = 0; verdict == CTR_OK && i < n; i++)
+        if ((unsigned long long)ids[i] == kIdEmpty) verdict = set_err(h, CTR_EINVAL, "idmap insert: id INT64_MIN is reserved (position %lld of rank %d)", (long long)i, cm.rank);
+    unsigned long long* d_cnt = nullptr;                 // [0] ids without a row, [1] side counter, [2] map digest
+    RET(scratch_get(h, 2, 3 * sizeof(unsigned long long), (void**)&d_cnt));
+    CommHdr hd{};
+    if (args_ok) {
+        hd.k = which; hd.n = h->idm_n[which]; hd.mode = h->idm_keys[which] ? 1 : 0;
+        if (h->idm_keys[which]) {
+            CU(h, cudaMemsetAsync(d_cnt + 2, 0, sizeof(unsigned long long), st));
+            RET(launch(h, "idmap_digest", [&] {
+                k_idmap_digest<<<h->num_sms * 8, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size(), d_cnt + 2);
+            }));
+            CU(h, cudaMemcpyAsync(&hd.hash[0], d_cnt + 2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            CU(h, cudaStreamSynchronize(st));
+        }
+    }
+    {
+        const int rc = comm_agree(h, hd, verdict);
+        if (rc != CTR_OK) return rc;
+    }
+    const int64_t R = h->idm_n[which];
+    const int G = h->num_sms * 8;
+    long long* d_ids = nullptr; int* d_rows = nullptr;
+    RET(scratch_get(h, 0, sizeof(long long) * (size_t)std::max<int64_t>(n, 1), (void**)&d_ids));
+    RET(scratch_get(h, 1, sizeof(int) * (size_t)std::max<int64_t>(n, 1), (void**)&d_rows));
+    if (!h->k_flags) RET(dalloc(h, h->k_flags, 1));
+    if (n > 0) CU(h, big_copy(d_ids, ids, sizeof(int64_t) * (size_t)n, true, st));
+    CU(h, cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), st));
+    IdmapSide s;
+    RET(idmap_number(h, which, d_ids, n, d_rows, d_cnt, &s));
+    // the ranks' counts, then their lists padded to the longest
+    int64_t all[2 * kMaxPeers] = {};
+    const int64_t mine[2] = {s.u, n};
+    RET(comm_gather_i64(h, mine, 2, all));
+    RankLists L{};
+    int64_t stride = 0, total = 0;
+    for (int j = 0; j < W; j++) { L.cnt[j] = (int)all[2 * j]; L.off[j + 1] = L.off[j] + all[2 * j]; stride = std::max(stride, all[2 * j]); total += all[2 * j + 1]; }
+    // one GPU refuses a concatenation of more than INT32_MAX ids: so do the ranks, all of them, before any write
+    if (total > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "idmap insert: the ranks pass %lld ids in all (more than INT32_MAX)", (long long)total);
+    if (stride > 0) {
+        const int64_t m = L.off[W];
+        if (m > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "idmap insert: the ranks' new ids (%lld) exceed INT32_MAX", (long long)m);
+        DevBuf<unsigned long long> sid, gid, key0, key1, tag0, tag1; DevBuf<int> spos, gpos, d_u; DevBuf<unsigned char> tmp;
+        CU(h, sid.alloc((size_t)stride)); CU(h, spos.alloc((size_t)stride));
+        CU(h, gid.alloc((size_t)stride * W)); CU(h, gpos.alloc((size_t)stride * W));
+        CU(h, key0.alloc((size_t)m)); CU(h, key1.alloc((size_t)m)); CU(h, tag0.alloc((size_t)m)); CU(h, tag1.alloc((size_t)m)); CU(h, d_u.alloc(1));
+        const size_t tb = idmap_merge_tmp_bytes((int)m, st);
+        CU(h, tmp.alloc(std::max<size_t>(tb, 1)));
+        if (s.u > 0) {
+            CU(h, cudaMemcpyAsync(sid, s.k0, sizeof(unsigned long long) * (size_t)s.u, cudaMemcpyDeviceToDevice, st));
+            CU(h, cudaMemcpyAsync(spos, s.p0, sizeof(int) * (size_t)s.u, cudaMemcpyDeviceToDevice, st));
+        }
+        int rc = CTR_OK;
+        RET(launch(h, "idmap_gather_ranks", [&] { rc = comm_gather_lists(h, spos, gpos, sizeof(int), nullptr, nullptr, (size_t)stride); }));
+        RET(rc);
+        RET(launch(h, "idmap_gather_ranks", [&] { rc = comm_gather_lists(h, sid, gid, sizeof(unsigned long long), nullptr, nullptr, (size_t)stride); }));
+        RET(rc);
+        int u = 0;
+        cudaError_t e = cudaSuccess;
+        RET(launch(h, "idmap_merge_ranks", [&] { e = idmap_merge_ranks(gid, gpos, (long)stride, L, W, key0, key1, tag0, tag1, d_u, tmp, tb, G, st, &u); }));
+        CU(h, e);
+        if (R + u > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "idmap insert: %lld ids + %d new ones exceed INT32_MAX rows", (long long)R, u);
+        RET(idmap_add(h, which, key1, u, d_ids, n, d_rows, rows && s.m > 0));
+    }
+    if (rows && n > 0) CU(h, cudaMemcpyAsync(rows, d_rows, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+}  // namespace
+
+// The ids the map lacks get rows idm_n, idm_n + 1, ... in order of first occurrence (idmap_number), a sort by first
+// position being the order.  Only the missing ids are sorted.
+int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows) {
+    if (!h) return set_err(h, CTR_EINVAL, "bad idmap insert arguments");
+    if (h->comm.world > 1) {
+        std::lock_guard<std::mutex> lk(h->mu);
+        return idmap_insert_ranks(h, which, ids, n, rows);
+    }
+    if (!ids || which < 0 || which > 1 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad idmap insert arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    for (int64_t i = 0; i < n; i++)
+        if ((unsigned long long)ids[i] == kIdEmpty) return set_err(h, CTR_EINVAL, "idmap insert: id INT64_MIN is reserved (position %lld)", (long long)i);
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const int64_t R = h->idm_n[which];
     long long* d_ids = nullptr; int* d_rows = nullptr; unsigned long long* d_cnt = nullptr;
     RET(scratch_get(h, 0, sizeof(long long) * (size_t)n, (void**)&d_ids)); RET(scratch_get(h, 1, sizeof(int) * (size_t)n, (void**)&d_rows));
     RET(scratch_get(h, 2, 2 * sizeof(unsigned long long), (void**)&d_cnt));
     if (!h->k_flags) RET(dalloc(h, h->k_flags, 1));
     CU(h, big_copy(d_ids, ids, sizeof(int64_t) * (size_t)n, true, st));
     CU(h, cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), st));
-    unsigned long long m = (unsigned long long)n;
-    if (have) {
-        RET(launch(h, "idmap_probe", [&] {
-            k_idmap_first_pos<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows, nullptr, d_cnt);
-        }));
-        CU(h, cudaMemcpyAsync(&m, d_cnt, sizeof m, cudaMemcpyDeviceToHost, st));
-    } else CU(h, cudaMemsetAsync(d_rows, 0xff, sizeof(int) * (size_t)n, st));
-    CU(h, cudaStreamSynchronize(st));
-    if (m > 0) {
-        // distinct missing ids and their first positions, then ordered by first position: k1[j] gets row R + j
-        DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
-        CU(h, k0.alloc(m)); CU(h, k1.alloc(m)); CU(h, p0.alloc(m)); CU(h, p1.alloc(m)); CU(h, d_u.alloc(1));
-        size_t b1 = 0, b2 = 0, b3 = 0;
-        CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b1, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st));
-        CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b2, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st));
-        CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b3, p0.get(), p1.get(), k0.get(), k1.get(), (int)m, 0, 32, st));
-        CU(h, tmp.alloc(std::max(b1, std::max(b2, b3))));
-        RET(launch(h, "idmap_number", [&] { k_i2v_dict_side<<<G, 256, 0, st>>>(d_rows, d_ids, (long)n, k0, p0, d_cnt + 1); }));
-        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st); }));
-        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceReduce::ReduceByKey(tmp.get(), tb, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st); }));
-        int u = 0;
-        CU(h, cudaMemcpyAsync(&u, d_u, sizeof u, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+    IdmapSide s;
+    RET(idmap_number(h, which, d_ids, n, d_rows, d_cnt, &s));
+    if (s.m > 0) {
+        const int u = s.u;
         if (R + u > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "idmap insert: %lld ids + %d new ones exceed INT32_MAX rows", (long long)R, u);
-        RET(launch(h, "idmap_number", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, p0.get(), p1.get(), k0.get(), k1.get(), u, 0, 32, st); }));
-        // a table at the capacity ctr_idmap_build picks for the new count: the old entries rehashed into it, then swapped
-        const unsigned long long cap = idmap_cap_for(R + u), old_cap = have ? h->idm_keys[which].size() : 0;
-        if (cap > old_cap) {
-            DevBuf<unsigned long long> nk; DevBuf<int> nv;
-            RET(dalloc(h, nk, (size_t)cap, false)); RET(dalloc(h, nv, (size_t)cap, false));
-            RET(launch(h, "idmap_clear", [&] { k_idmap_clear<<<G, 256, 0, st>>>(nk, nv, cap); }));
-            if (have) RET(launch(h, "idmap_rehash", [&] { k_idmap_rehash<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], old_cap, nk, nv, cap - 1); }));
-            h->idm_keys[which] = std::move(nk); h->idm_vals[which] = std::move(nv);        // cudaFree of the old table waits for the rehash
-        }
-        RET(launch(h, "idmap_insert", [&] {
-            k_idmap_insert<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, (const long long*)k1.get(), (long)u, h->k_flags, (int)R);
-        }));
-        h->idm_n[which] = R + u;
-        if (rows) RET(launch(h, "idmap_lookup", [&] {
-            k_idmap_lookup<<<G, 256, 0, st>>>(h->idm_keys[which], h->idm_vals[which], h->idm_keys[which].size() - 1, d_ids, (long)n, d_rows);
-        }));
+        // ordered by first position: k1[j] gets row R + j
+        RET(launch(h, "idmap_number", [&] { size_t tb = s.tmp.size(); cub::DeviceRadixSort::SortPairs(s.tmp.get(), tb, s.p0.get(), s.p1.get(), s.k0.get(), s.k1.get(), u, 0, 32, st); }));
+        RET(idmap_add(h, which, s.k1, u, d_ids, n, d_rows, rows != nullptr));
     }
     if (rows) CU(h, cudaMemcpyAsync(rows, d_rows, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
     CU(h, cudaStreamSynchronize(st));
@@ -3773,7 +3878,6 @@ int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, in
 int ctr_idmap_download(ctr_handle* h, int which, int64_t* ids, int64_t cap, int64_t* n) {
     if (!h || !n || which < 0 || which > 1) return set_err(h, CTR_EINVAL, "bad idmap download arguments");
     std::lock_guard<std::mutex> lk(h->mu);
-    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_idmap_download is single-GPU (world = %d)", h->comm.world);
     if (!h->idm_keys[which]) return set_err(h, CTR_ESTATE, "idmap %d not built", which);
     *n = h->idm_n[which];
     if (!ids) return CTR_OK;
@@ -3788,15 +3892,190 @@ int ctr_idmap_download(ctr_handle* h, int which, int64_t* ids, int64_t cap, int6
     return CTR_OK;
 }
 
+namespace {
+// A table in growable memory (and ITEM_EMB's moments) grown to nrows rows in place, the new rows zero.  Every buffer is
+// mapped first; the row count changes only once all of them hold the new rows.
+int table_grow(ctr_handle* h, int which, int64_t nrows) {
+    cudaStream_t st = h->stream;
+    const int64_t old = h->tab_rows[which];
+    const long ld = h->tab_ld[which];
+    const bool mom = which == CTR_TABLE_ITEM_EMB && h->emb_m;
+    int rc = CTR_OK;
+    RET(launch(h, "table_grow", [&] {
+        for (GrowBuf<float>* b : {&h->tab_mem[which], mom ? &h->emb_m : nullptr, mom ? &h->emb_v : nullptr})
+            if (b && rc == CTR_OK && (rc = grow_buf(h, *b, (size_t)nrows * ld)) == CTR_OK)
+                cudaMemsetAsync(b->get() + (size_t)old * ld, 0, (size_t)(nrows - old) * ld * sizeof(float), st);
+    }));
+    RET(rc);
+    h->tab[which] = h->tab_mem[which].get();
+    h->tab_rows[which] = h->tab_local_rows[which] = nrows;
+    return CTR_OK;
+}
+
+// A row-sharded table grown to nrows logical rows: the shard by vmm_grow_rows (vmm.cuh: reallocated at twice its live
+// rows when the new ones do not fit, the new rows zero), ITEM_EMB's row-Adam moments in their growable memory.  tab_gen
+// is bumped either way (the row count fixes the hot rows and the row-Adam gradient layout), so the next collective call
+// republishes the mappings; ITEM_EMB's hot rows are written back into their owners' shards first, whichever table
+// grows, since that republish pulls them from there.
+int shard_grow(ctr_handle* h, int which, int64_t nrows) {
+    Comm& cm = h->comm;
+    cudaStream_t st = h->stream;
+    RET(comm_hot_writeback(h));        // any table's growth bumps tab_gen, and the republish re-pulls ITEM_EMB's hot rows
+    const long ld = h->tab_ld[which];
+    const size_t row_b = (size_t)ld * sizeof(float);
+    const int64_t old = h->tab_local_rows[which];
+    const int64_t local = (nrows - cm.rank + cm.world - 1) / cm.world;
+    int rc = CTR_OK;
+    RET(launch(h, "table_shard_grow", [&] {
+        std::string err;
+        if (!vmm_grow_rows(&h->tab_vmm[which], (size_t)old, (size_t)local, row_b, h->dev, st, &err)) { rc = set_err(h, CTR_ENOMEM, "table %d shard (%lld rows): %s", which, (long long)local, err.c_str()); return; }
+        h->tab[which] = (float*)h->tab_vmm[which].ptr;
+        if (which == CTR_TABLE_ITEM_EMB && h->emb_m && local > old)
+            for (GrowBuf<float>* b : {&h->emb_m, &h->emb_v})
+                if (rc == CTR_OK && (rc = grow_buf(h, *b, (size_t)local * ld)) == CTR_OK)
+                    cudaMemsetAsync(b->get() + (size_t)old * ld, 0, (size_t)(local - old) * row_b, st);
+    }));
+    RET(rc);
+    h->tab_rows[which] = nrows; h->tab_local_rows[which] = local;
+    h->tab_gen++;
+    return CTR_OK;
+}
+
+// World > 1: the result is the single-GPU write of the ranks' (rows, data) concatenated in rank order.  Row ids are
+// concatenated on every rank (one broadcast per rank, grouped) and checked for duplicates with the device sort.  A
+// replicated table concatenates the data the same way and every rank writes every row; a row-sharded table routes each
+// (row, data) to its owner by grouped send / recv, and a row below hot_k (the replicated hot rows of ITEM_EMB) to every
+// rank as well.
+int table_write_ranks(ctr_handle* h, int which, const int32_t* rows, const float* data, int64_t n, int32_t width) {
+    Comm& cm = h->comm;
+    const int W = cm.world, me = cm.rank;
+    CU(h, cudaSetDevice(h->dev));
+    cudaStream_t st = h->stream;
+    const int G = h->num_sms * 8;
+    const ctr_config& c = h->cfg;
+    const bool args_ok = !(which < 0 || which > 2 || n < 0 || n > 0x7fffffffLL || (n > 0 && (!rows || !data)));
+    int verdict = args_ok ? CTR_OK : set_err(h, CTR_EINVAL, "bad table write arguments");
+    int32_t top = -1;
+    if (verdict == CTR_OK) {
+        const int want = which == CTR_TABLE_USER_FEAT ? c.uP : which == CTR_TABLE_ITEM_FEAT ? c.cF : c.D;
+        if (width != want || width < 1) verdict = set_err(h, CTR_EINVAL, "table %d width %d != model dim %d (rank %d)", which, width, want, me);
+    }
+    for (int64_t i = 0; verdict == CTR_OK && i < n; i++) {
+        if (rows[i] < 0 || rows[i] == 0x7fffffff) verdict = set_err(h, CTR_EINVAL, "table write: row %d outside [0, INT32_MAX) at position %lld of rank %d", rows[i], (long long)i, me);
+        top = std::max(top, rows[i]);
+    }
+    // the table this call starts from must be the same everywhere: rows, width and placement
+    CommHdr hd{};
+    if (args_ok) { hd.k = which; hd.n = h->tab_rows[which]; hd.mode = h->tab_width[which]; hd.flag = (h->tab[which] ? 1 : 0) | (h->tab_sharded[which] ? 2 : 0); }
+    {
+        const int rc = comm_agree(h, hd, verdict);
+        if (rc != CTR_OK) return rc;
+    }
+    int64_t all[2 * kMaxPeers];
+    const int64_t mine[2] = {n, top};
+    RET(comm_gather_i64(h, mine, 2, all));
+    int64_t cnt[kMaxPeers], off[kMaxPeers + 1] = {0};
+    int64_t gtop = -1;
+    for (int j = 0; j < W; j++) { cnt[j] = all[2 * j]; off[j + 1] = off[j] + cnt[j]; gtop = std::max(gtop, all[2 * j + 1]); }
+    const int64_t N = off[W];
+    if (N == 0) return CTR_OK;
+    if (N > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "table write: the ranks write %lld rows in all (more than INT32_MAX)", (long long)N);
+    // every rank's row ids, concatenated; a row named twice anywhere is refused everywhere
+    DevBuf<int> g_rows;
+    CU(h, g_rows.alloc((size_t)N));
+    if (n > 0) CU(h, cudaMemcpyAsync(g_rows.get() + off[me], rows, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    int rc = CTR_OK;
+    RET(launch(h, "table_write_ranks", [&] { rc = comm_concat(h, g_rows, sizeof(int), cnt, off); }));
+    RET(rc);
+    if (N > 1) {
+        DevBuf<int> sorted, d_dup; DevBuf<unsigned char> tmp;
+        CU(h, sorted.alloc((size_t)N)); CU(h, d_dup.alloc(1));
+        int bits = 1; while (bits < 31 && (gtop >> bits) != 0) bits++;
+        size_t tb = 0;
+        CU(h, cub::DeviceRadixSort::SortKeys(nullptr, tb, g_rows.get(), sorted.get(), (int)N, 0, bits, st));
+        CU(h, tmp.alloc(tb));
+        CU(h, cudaMemsetAsync(d_dup, 0, sizeof(int), st));
+        RET(launch(h, "table_write_check", [&] { size_t b = tmp.size(); cub::DeviceRadixSort::SortKeys(tmp.get(), b, g_rows.get(), sorted.get(), (int)N, 0, bits, st); }));
+        RET(launch(h, "table_write_check", [&] { k_rows_dup<<<G, 256, 0, st>>>(sorted, (long)N, d_dup); }));
+        int dup = 0;
+        CU(h, cudaMemcpyAsync(&dup, d_dup, sizeof dup, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
+        if (dup) return set_err(h, CTR_EINVAL, "table write: a row appears twice across the ranks' rows");
+    }
+    // growth: no table yet takes ctr_table_upload's placement for the size; a table keeps its placement when it grows
+    const int64_t nrows = gtop + 1;
+    if (!h->tab[which]) RET(table_alloc(h, which, nrows, width));
+    else if (nrows > h->tab_rows[which]) RET(h->tab_sharded[which] ? shard_grow(h, which, nrows) : table_grow(h, which, nrows));
+    const size_t row_b = (size_t)width * sizeof(float);
+    float* mo = which == CTR_TABLE_ITEM_EMB && h->emb_m ? h->emb_m.get() : nullptr;
+    float* vo = mo ? h->emb_v.get() : nullptr;
+    if (!h->tab_sharded[which]) {
+        DevBuf<float> g_data;
+        CU(h, g_data.alloc((size_t)N * width));
+        if (n > 0) CU(h, big_copy(g_data.get() + (size_t)off[me] * width, data, (size_t)n * row_b, true, st));
+        RET(launch(h, "table_write_ranks", [&] { rc = comm_concat(h, g_data, row_b, cnt, off); }));
+        RET(rc);
+        RET(launch(h, "table_write_rows", [&] {
+            k_table_write_rows<<<(int)std::min<int64_t>((N + 7) / 8, G), 256, 0, st>>>(h->tab[which], h->tab_ld[which], g_rows, g_data, (long)N, width, mo, vo);
+        }));
+        CU(h, cudaStreamSynchronize(st));
+        return CTR_OK;
+    }
+    // row-sharded: this rank's rows by destination (the owner, and every rank for a hot row while the replica is live)
+    const bool hot = which == CTR_TABLE_ITEM_EMB && cm.hot_k > 0 && cm.hot_tab && cm.published_gen == h->tab_gen;
+    const int hot_k = hot ? cm.hot_k : 0;
+    int64_t scnt[kMaxPeers] = {}, soff[kMaxPeers + 1] = {0};
+    std::vector<int32_t> s_rows; std::vector<float> s_data;
+    for (int k = 0; k < W; k++) {
+        for (int64_t i = 0; i < n; i++)
+            if (rows[i] % W == k || rows[i] < hot_k) {
+                s_rows.push_back(rows[i]);
+                s_data.insert(s_data.end(), data + (size_t)i * width, data + (size_t)(i + 1) * width);
+                scnt[k]++;
+            }
+        soff[k + 1] = soff[k] + scnt[k];
+    }
+    int64_t allc[kMaxPeers * kMaxPeers];
+    RET(comm_gather_i64(h, scnt, W, allc));             // allc[j·W + k]: what rank j sends rank k
+    int64_t rcnt[kMaxPeers], roff[kMaxPeers + 1] = {0};
+    for (int j = 0; j < W; j++) { rcnt[j] = allc[j * W + me]; roff[j + 1] = roff[j] + rcnt[j]; }
+    const int64_t ns = soff[W], nr = roff[W];
+    DevBuf<int> d_srows, d_rrows; DevBuf<float> d_sdata, d_rdata;
+    CU(h, d_srows.alloc((size_t)std::max<int64_t>(ns, 1))); CU(h, d_sdata.alloc((size_t)std::max<int64_t>(ns, 1) * width));
+    CU(h, d_rrows.alloc((size_t)std::max<int64_t>(nr, 1))); CU(h, d_rdata.alloc((size_t)std::max<int64_t>(nr, 1) * width));
+    if (ns > 0) {
+        CU(h, cudaMemcpyAsync(d_srows, s_rows.data(), sizeof(int32_t) * (size_t)ns, cudaMemcpyHostToDevice, st));
+        CU(h, big_copy(d_sdata, s_data.data(), (size_t)ns * row_b, true, st));
+    }
+    RET(launch(h, "table_write_ranks", [&] {
+        rc = comm_route(h, d_srows, scnt, soff, d_rrows, rcnt, roff, sizeof(int));
+        if (rc == CTR_OK) rc = comm_route(h, d_sdata, scnt, soff, d_rdata, rcnt, roff, row_b);
+    }));
+    RET(rc);
+    if (nr > 0) {
+        float* hm = hot && cm.hot_m ? cm.hot_m.get() : nullptr;
+        RET(launch(h, "table_write_shard", [&] {
+            k_shard_write_rows<<<(int)std::min<int64_t>((nr + 7) / 8, G), 256, 0, st>>>(h->tab[which], h->tab_ld[which], d_rrows, d_rdata, (long)nr, width, W, me,
+                                                                                      mo, vo, hot ? cm.hot_tab.get() : nullptr, hot_k, hm, hm ? cm.hot_v.get() : nullptr);
+        }));
+    }
+    CU(h, cudaStreamSynchronize(st));
+    return CTR_OK;
+}
+}  // namespace
+
 // Rows are written in place; a row past the end grows the table (and ITEM_EMB's moments) in its growable memory, the
 // gap zeroed.  Validation (ranges on the host, duplicates by a device sort) comes before any write to the table.
 int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const float* data, int64_t n, int32_t width) {
-    if (!h || !rows || !data || which < 0 || which > 2 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad table write arguments");
+    if (!h) return set_err(h, CTR_EINVAL, "bad table write arguments");
+    if (h->comm.world > 1) {
+        std::lock_guard<std::mutex> lk(h->mu);
+        return table_write_ranks(h, which, rows, data, n, width);
+    }
+    if (!rows || !data || which < 0 || which > 2 || n < 1 || n > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "bad table write arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     const ctr_config& c = h->cfg;
     const int want = which == CTR_TABLE_USER_FEAT ? c.uP : which == CTR_TABLE_ITEM_FEAT ? c.cF : c.D;
     if (width != want || width < 1) return set_err(h, CTR_EINVAL, "table %d width %d != model dim %d", which, width, want);
-    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_table_write_rows is single-GPU (world = %d)", h->comm.world);
     int32_t top = -1;
     for (int64_t i = 0; i < n; i++) {
         if (rows[i] < 0 || rows[i] == 0x7fffffff) return set_err(h, CTR_EINVAL, "table write: row %d outside [0, INT32_MAX) at position %lld", rows[i], (long long)i);
@@ -3824,21 +4103,7 @@ int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const fl
     }
     const int64_t nrows = (int64_t)top + 1;
     if (!h->tab[which]) RET(table_alloc(h, which, nrows, width));
-    else if (nrows > h->tab_rows[which]) {
-        // every buffer is mapped first; the row count changes only once all of them hold the new rows
-        const int64_t old = h->tab_rows[which];
-        const long ld = h->tab_ld[which];
-        const bool mom = which == CTR_TABLE_ITEM_EMB && h->emb_m;
-        int rc = CTR_OK;
-        RET(launch(h, "table_grow", [&] {
-            for (GrowBuf<float>* b : {&h->tab_mem[which], mom ? &h->emb_m : nullptr, mom ? &h->emb_v : nullptr})
-                if (b && rc == CTR_OK && (rc = grow_buf(h, *b, (size_t)nrows * ld)) == CTR_OK)
-                    cudaMemsetAsync(b->get() + (size_t)old * ld, 0, (size_t)(nrows - old) * ld * sizeof(float), st);
-        }));
-        RET(rc);
-        h->tab[which] = h->tab_mem[which].get();
-        h->tab_rows[which] = h->tab_local_rows[which] = nrows;
-    }
+    else if (nrows > h->tab_rows[which]) RET(table_grow(h, which, nrows));
     // host rows in chunks: through two pinned buffers (the caller's may be pageable) into two device slots
     const size_t row_b = (size_t)width * sizeof(float), total = (size_t)n * row_b;
     const size_t kChunk = (size_t)32 << 20;

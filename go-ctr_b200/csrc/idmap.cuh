@@ -7,6 +7,9 @@
 #pragma once
 #include "common.cuh"
 #include "ubcache.cuh"
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
+#include <algorithm>
 
 namespace ctr {
 
@@ -80,6 +83,68 @@ k_idmap_lookup(const unsigned long long* __restrict__ keys, const int* __restric
         }
         rows[i] = row;
     }
+}
+
+// ---- ctr_idmap_insert with world > 1 (the ranks' ids concatenated in rank order) -----------------------------------
+// *digest += a mix of every (id, row) pair of the map: the sum is order-independent, so maps holding the same pairs agree
+// on it whatever their slot layout (the ranks compare it before any write).
+__global__ void __launch_bounds__(256)
+k_idmap_digest(const unsigned long long* __restrict__ keys, const int* __restrict__ vals, unsigned long long cap, unsigned long long* __restrict__ digest) {
+    unsigned long long s = 0;
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < cap; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long id = keys[i];
+        if (id != kIdEmpty) s += idmap_hash(id ^ idmap_hash(0x9e3779b97f4a7c15ull + (unsigned long long)(unsigned)vals[i]));
+    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0 && s) atomicAdd(digest, s);
+}
+
+// The ranks' lists, all-gathered: rank j's distinct missing ids (ascending) and their first positions in its own ids sit at
+// [j·stride, j·stride + cnt[j]).  Compacted to off[j] + e, each id is tagged (j << 32) | position: the tag orders
+// entries as their positions in the concatenation of the ranks' ids do.
+struct RankLists { long long off[kMaxPeers + 1]; int cnt[kMaxPeers]; };
+__global__ void __launch_bounds__(256)
+k_idmap_merge_ranks(const unsigned long long* __restrict__ ids, const int* __restrict__ pos, long stride, RankLists L, int world,
+                    unsigned long long* __restrict__ key, unsigned long long* __restrict__ tag) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < (long)world * stride; i += (long)gridDim.x * blockDim.x) {
+        const int j = (int)(i / stride);
+        const long e = i - (long)j * stride;
+        if (e >= L.cnt[j]) continue;
+        key[L.off[j] + e] = ids[i];
+        tag[L.off[j] + e] = ((unsigned long long)j << 32) | (unsigned)pos[i];
+    }
+}
+struct MinPos { __device__ int operator()(int a, int b) const { return a < b ? a : b; } };       // first positions (ReduceByKey)
+struct MinTag { __device__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a < b ? a : b; } };
+
+// Scratch of idmap_merge_ranks for m = L.off[world] gathered entries: key0, key1, tag0, tag1 [m] and tmp (this many bytes).
+inline size_t idmap_merge_tmp_bytes(int m, cudaStream_t st) {
+    size_t b1 = 0, b2 = 0, b3 = 0;
+    unsigned long long* k = nullptr; int* u = nullptr;
+    cub::DeviceRadixSort::SortPairs(nullptr, b1, k, k, k, k, m, 0, 64, st);
+    cub::DeviceReduce::ReduceByKey(nullptr, b2, k, k, k, k, u, MinTag{}, m, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, b3, k, k, k, k, m, 0, 64, st);
+    return std::max(b1, std::max(b2, b3));
+}
+// The merge every rank runs on the same gathered lists: the entries sorted by id, the smallest tag of each id kept
+// (ReduceByKey(MinTag)), then sorted by that tag.  key1[0, *u) receives the distinct ids in order of first occurrence in
+// the concatenation, the order a single-GPU insert of it gives new rows in.  Radix sorts and a keyed reduction over the
+// same input: the result is the same on every rank.  Synchronises st (reads *u back).
+inline cudaError_t idmap_merge_ranks(const unsigned long long* g_ids, const int* g_pos, long stride, const RankLists& L, int world,
+                                     unsigned long long* key0, unsigned long long* key1, unsigned long long* tag0, unsigned long long* tag1,
+                                     int* d_u, void* tmp, size_t tmp_bytes, int grid, cudaStream_t st, int* u) {
+    const int m = (int)L.off[world];
+    int wbits = 0; while ((1 << wbits) < world) wbits++;
+    *u = 0;
+    if (m == 0) return cudaSuccess;
+    k_idmap_merge_ranks<<<grid, 256, 0, st>>>(g_ids, g_pos, stride, L, world, key0, tag0);
+    size_t b = tmp_bytes;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, b, key0, key1, tag0, tag1, m, 0, 64, st);
+    if (e == cudaSuccess) { b = tmp_bytes; e = cub::DeviceReduce::ReduceByKey(tmp, b, key1, key0, tag1, tag0, d_u, MinTag{}, m, st); }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(u, d_u, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) { b = tmp_bytes; e = cub::DeviceRadixSort::SortPairs(tmp, b, tag0, tag1, key0, key1, *u, 0, 32 + wbits, st); }
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 __device__ __forceinline__ int idmap_find(const unsigned long long* __restrict__ keys, const int* __restrict__ vals,

@@ -125,6 +125,30 @@ inline bool vmm_import(int fd, size_t bytes, int dev, VmmBuf* out, std::string* 
     return true;
 }
 
+// A row-sharded table's shard holding `rows` live rows of row_b bytes, grown to `want` rows.  The shard is an exportable
+// allocation the peers map, which does not grow in place: when `want` rows exceed it, a new one of max(want, 2 x rows)
+// rows (geometric, so a run of small growths reallocates O(log n) times) receives the live rows, the rest zeroed, and the
+// old one is freed once the copy is done — old and new side by side at the peak.  Otherwise rows [rows, want) are
+// zeroed in place.  Synchronises st when it reallocates.
+inline bool vmm_grow_rows(VmmBuf* b, size_t rows, size_t want, size_t row_b, int dev, cudaStream_t st, std::string* err) {
+    if (want <= rows) return true;
+    if (want * row_b <= b->bytes) {
+        if (cudaMemsetAsync((char*)b->ptr + rows * row_b, 0, (want - rows) * row_b, st) != cudaSuccess) { *err = "cudaMemsetAsync failed"; return false; }
+        return true;
+    }
+    VmmBuf nb;
+    if (!vmm_alloc(std::max(want, 2 * rows) * row_b, dev, &nb, err)) return false;
+    if (cudaMemcpyAsync(nb.ptr, b->ptr, rows * row_b, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync((char*)nb.ptr + rows * row_b, 0, nb.bytes - rows * row_b, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+        *err = std::string("shard copy: ") + cudaGetErrorString(cudaGetLastError());
+        vmm_free(&nb);
+        return false;
+    }
+    vmm_free(b);
+    *b = nb;
+    return true;
+}
+
 // ---- growable device memory: the single-GPU tables and ITEM_EMB's row-Adam moments (ctr_table_write_rows) ------
 // A virtual range reserved with headroom; physical chunks (non-shareable handles) are created and mapped at the end of
 // what is mapped as the buffer grows, each about 1/8 of the mapped size and at least one granule, so a run of one-row

@@ -426,12 +426,16 @@ class Engine:
     def idmap_insert(self, which, ids):
         """Adds ids to a live map (ctr_idmap_insert): ids it lacks get the next rows in order of first occurrence, ids it
         holds keep theirs.  Returns the row of every id.  With the item map, extends `item_ids` (the row -> id list
-        serving.Recommend maps rows back through) when the engine carries one."""
+        serving.Recommend maps rows back through) when the engine carries one.  With world > 1 the call is collective:
+        every rank passes its own ids (possibly none) and every map ends as one GPU's insert of the ranks' ids concatenated
+        in rank order; maps that differ across ranks, or a refused id on any rank, raise CtrError on every rank."""
         a = np.ascontiguousarray(ids, np.int64)
         out = np.empty(a.size, np.int32)
         self._ck(self.L.ctr_idmap_insert(self.h, C.c_int(which), a.ctypes.data_as(_lp), C.c_int64(a.size), out.ctypes.data_as(_ip)))
         known = getattr(self, "item_ids", None)
-        if which == IDMAP_ITEM and known is not None:
+        if which == IDMAP_ITEM and known is not None and self.cfg.world > 1:
+            self.item_ids = self.idmap_download(IDMAP_ITEM)       # other ranks' ids may have taken rows too
+        elif which == IDMAP_ITEM and known is not None:
             known = np.asarray(known, np.int64)
             fresh = out >= known.size
             if fresh.any():
@@ -441,7 +445,8 @@ class Engine:
         return out
 
     def idmap_download(self, which):
-        """The ids of a map in row order (ctr_idmap_download): ids[r] is the id of row r."""
+        """The ids of a map in row order (ctr_idmap_download): ids[r] is the id of row r.  Local on every rank (the maps
+        of a multi-GPU handle are identical)."""
         n = C.c_int64(0)
         self._ck(self.L.ctr_idmap_download(self.h, C.c_int(which), None, C.c_int64(0), C.byref(n)))
         out = np.empty(n.value, np.int64)
@@ -450,11 +455,19 @@ class Engine:
 
     def table_write_rows(self, which, rows, data):
         """Writes rows of a live table in HBM (ctr_table_write_rows): row rows[i] = data[i]; a row past the end grows
-        the table (the gap reads as zero).  ITEM_EMB's written rows restart their row-Adam moments at zero."""
+        the table (the gap reads as zero).  ITEM_EMB's written rows restart their row-Adam moments at zero.  With world
+        > 1 the call is collective: every rank passes its own (rows, data), possibly none, and the table ends as one
+        GPU's write of the ranks' lists concatenated in rank order; a row named twice anywhere raises CtrError on every
+        rank.  A row-sharded table sends each row to its owner; a shard that outgrows its allocation is reallocated at
+        twice its rows."""
         r, rp = _i(np.atleast_1d(rows))
         d, dp = _f(data)
-        d = d.reshape(r.size, -1) if d.size else d.reshape(r.size, 0)
-        self._ck(self.L.ctr_table_write_rows(self.h, C.c_int(which), rp, dp, C.c_int64(r.size), C.c_int32(d.shape[1])))
+        if r.size:
+            d = d.reshape(r.size, -1) if d.size else d.reshape(r.size, 0)
+            width = d.shape[1]
+        else:           # a rank with nothing to write in a collective call: the table's width, not that of an empty array
+            width = d.shape[1] if d.ndim == 2 else {TABLE_USER_FEAT: self.cfg.uP, TABLE_ITEM_FEAT: self.cfg.cF, TABLE_ITEM_EMB: self.cfg.D}.get(which, 0)
+        self._ck(self.L.ctr_table_write_rows(self.h, C.c_int(which), rp, dp, C.c_int64(r.size), C.c_int32(width)))
 
     def item_emb_train(self, item_ids, cfg=None, **kw):
         """recommend.Train's embedding stage into ITEM_EMB (ctr_item_emb_train): item2vec over the int64 item stream,

@@ -198,17 +198,22 @@ func (e *Engine) DownloadUserBehavior() (offsets, ts []int64, itemRows []int32, 
 
 // InsertIDs adds ids to a live id map (which: C.CTR_IDMAP_USER or C.CTR_IDMAP_ITEM; the map is created if none was
 // loaded).  Ids the map holds keep their rows; the others get the next rows in order of first occurrence.  Returns the
-// row of every id.
+// row of every id.  With world > 1 InsertIDs is collective: every rank's process calls it with its own ids (possibly
+// none) and every map ends as one GPU's insert of the ranks' ids concatenated in rank order; maps that differ across
+// the ranks, or an id refused on any rank, fail on every rank.
 func (e *Engine) InsertIDs(which int, ids []int64) ([]int32, error) {
 	if len(ids) == 0 {
-		return nil, nil
+		if e.cfg.world <= 1 {
+			return nil, nil
+		}
+		return nil, e.err(C.ctr_idmap_insert(e.h, C.int(which), nil, 0, nil))
 	}
 	rows := make([]int32, len(ids))
 	return rows, e.err(C.ctr_idmap_insert(e.h, C.int(which), i64(ids), C.int64_t(len(ids)), i32(rows)))
 }
 
 // DownloadIDs returns a map's ids in row order (ids[r] is the id of row r): with LoadIDMaps, how a map grown by
-// InsertIDs is persisted and restored (checkpoints do not hold id maps).
+// InsertIDs is persisted and restored (checkpoints do not hold id maps).  Local: the maps of every rank are the same.
 func (e *Engine) DownloadIDs(which int) ([]int64, error) {
 	var n C.int64_t
 	if err := e.err(C.ctr_idmap_download(e.h, C.int(which), nil, 0, &n)); err != nil {
@@ -220,7 +225,14 @@ func (e *Engine) DownloadIDs(which int) ([]int64, error) {
 
 // WriteTableRows writes rows of a live table in HBM: row rows[i] becomes data[i*width : (i+1)*width].  A row past the
 // end grows the table in place (the gap reads as zero); ITEM_EMB's written rows restart their row-Adam moments at zero.
+// With world > 1 WriteTableRows is collective: every rank's process calls it with its own rows (possibly none) and the
+// table ends as one GPU's write of the ranks' rows concatenated in rank order; a row named twice, on one rank or across
+// ranks, fails on every rank.  A row-sharded table sends each row to its owner and reallocates a shard that outgrows
+// its allocation at twice its rows.
 func (e *Engine) WriteTableRows(which int, rows []int32, data []float32, width int) error {
+	if len(rows) == 0 && e.cfg.world > 1 && len(data) == 0 {
+		return e.err(C.ctr_table_write_rows(e.h, C.int(which), nil, nil, 0, C.int32_t(width)))
+	}
 	if len(rows) == 0 || len(data) != len(rows)*width {
 		return fmt.Errorf("WriteTableRows: %d rows, %d floats, width %d", len(rows), len(data), width)
 	}

@@ -251,9 +251,9 @@ int ctr_idmap_lookup_dev(ctr_handle* h, int which, const int64_t* d_ids, int64_t
 
 /* Live id maps and tables: a user or item that did not exist when the handle was set up gets a row and its features
  * while the handle serves and trains, as the reference's feature caches fetch a new key's features on first use
- * (rcmd.go:344-353, 472-492).  All three are single-GPU (world > 1: CTR_ESTATE), take the handle's mutex and run on the
- * engine stream: work queued before sees the old state, work queued after the new one.  Arguments are validated before
- * any device write, and a refused call changes nothing.
+ * (rcmd.go:344-353, 472-492).  All three take the handle's mutex and run on the engine stream: work queued before sees
+ * the old state, work queued after the new one.  Arguments are validated before any device write, and a refused call
+ * changes nothing.
  * insert: an id the map holds keeps its row; the ids it lacks get rows idmap_n, idmap_n + 1, ... in the order of their
  *   first occurrence in ids (a repeated id gets one row).  rows (may be NULL) receives the row of every ids[i].  No map:
  *   the call creates one, which on distinct ids equals ctr_idmap_build.  CTR_EINVAL: NULL ids, n outside [1, 2^31), a bad
@@ -268,7 +268,35 @@ int ctr_idmap_lookup_dev(ctr_handle* h, int which, const int64_t* d_ids, int64_t
  *   one.  Tables grow in place (reserved address space, memory mapped in chunks), without a second copy of the table.
  *   ITEM_EMB: written and new rows get zero row-Adam moments, every other row keeps its moments; the step counter,
  *   the dense weights and every other row are unchanged (ctr_table_upload, by contrast, resets the solver state).
- *   Host data is staged in chunks; the caller's buffers may be pageable. */
+ *   Host data is staged in chunks; the caller's buffers may be pageable.
+ * World > 1: insert and write_rows are collective (every rank calls them, each with its OWN arguments; n = 0 is allowed
+ *   there, with ids / rows / data then possibly NULL) and download is local.  The rule: afterwards every rank holds what
+ *   one GPU would hold after the same call on the ranks' arguments concatenated in rank order.  Every rank checks its
+ *   arguments, then the ranks exchange verdicts: if any rank fails, every rank returns the lowest failing rank's code and
+ *   nothing changes anywhere; a state that differs across ranks (the map's size or the order-independent digest of its
+ *   (id, row) pairs; a table's rows, width or placement) is CTR_EINVAL everywhere.  "Changes nothing" covers every
+ *   refusal decided from the arguments and the state.  It does not cover a CUDA or NCCL failure after the agreement,
+ *   such as running out of device memory while one rank grows its shard: as with the other collective calls, that rank
+ *   returns the error, the others may then wait in the exchange, and the ranks' tables may differ; such a handle is to
+ *   be rebuilt (ctr_table_upload, ctr_idmap_build) on every rank.
+ *   insert: each rank numbers its own missing ids, the ranks all-gather the counts and then the lists padded to the
+ *     longest (8 + 4 bytes an entry), and each runs the same deterministic merge (profile key idmap_merge_ranks): new ids
+ *     get rows by first (rank, position), so an id new on several ranks takes its first.  rows receives the rows of this
+ *     rank's own ids.  INT64_MIN on any rank, more than INT32_MAX rows in all, or more than INT32_MAX ids
+ *     passed in all (as one GPU refuses them) is refused on every rank.  When every rank passes n = 0 the call does
+ *     nothing.  Scratch: 4 x 8 bytes per gathered entry beside the single-GPU scratch.
+ *   write_rows: the row ids are concatenated on every rank (4 bytes a row, broadcast per rank) and a row named twice,
+ *     within or across ranks, is CTR_EINVAL everywhere.  A replicated table (USER_FEAT; ITEM_* at or under the placement
+ *     threshold) concatenates the data the same way and every rank writes every row: each rank receives the whole
+ *     union.  A row-sharded table sends each (row, data) to its owner row % world only (grouped send / recv, no
+ *     full-table traffic), which writes its local row row / world; a row below the replicated hot-row count goes to
+ *     every rank's hot-row replica too, and under CTR_TABLE_ADAM the written rows' moments are zeroed on the owner and in
+ *     the hot-moment replica.  A write past the end grows every table to max(rows) + 1 with zero rows in between and
+ *     keeps its placement (a replicated table never becomes sharded); no table yet is allocated by ctr_table_upload's
+ *     placement rule for that size.  A shard that outgrows its allocation (an exportable one the peers map, which
+ *     cannot grow in place) is reallocated at max(new local rows, 2 x old local rows) — the old and the new shard side
+ *     by side at the peak, plus ITEM_EMB's moments grown in place — and the next collective call republishes the peer
+ *     mappings.  Host staging: this rank's rows grouped by destination, one copy of its data. */
 int ctr_idmap_insert(ctr_handle* h, int which, const int64_t* ids, int64_t n, int32_t* rows);
 int ctr_idmap_download(ctr_handle* h, int which, int64_t* ids, int64_t cap, int64_t* n);
 int ctr_table_write_rows(ctr_handle* h, int which, const int32_t* rows, const float* data, int64_t n, int32_t width);
