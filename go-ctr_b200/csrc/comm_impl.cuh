@@ -322,6 +322,16 @@ static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
     return CTR_OK;
 }
 
+// The entry of a collective serving call (search, recommendation, held-out ranks; the key-fed MLP's too): the
+// agreement, then the peer mappings published, every rank's row updates queued before the call landed (a device
+// barrier) and the shard's copies of the hot rows made current, so that the call reads no stale row.
+static int comm_serve_enter(ctr_handle* h, CommHdr hd, int verdict) {
+    RET(comm_agree(h, hd, verdict));
+    RET(comm_ensure(h, false));
+    RET(comm_barrier(h));
+    return comm_hot_writeback(h);
+}
+
 // The ranks' top-k lists, all-gathered on the engine stream (device buffers of the caller's scratch): send_s / send_r
 // hold n entries, recv_s / recv_r receive [world][n]; send_r == nullptr gathers the scores alone (as bytes: a -0 stays
 // -0).  Every rank's reads of the table are queued before its send, so the gather completes on a rank only after every

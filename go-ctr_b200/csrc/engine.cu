@@ -1269,13 +1269,24 @@ int rec_build_seen(ctr_handle* h, const char* key, unsigned* seen, int64_t I, in
     });
 }
 
+// The ranks' lists [n][k] in ls / lr on a row-sharded table: all-gathered into gs / gr [world][n][k] and merged back
+// into ls / lr (and their lengths into count, when given) under profile key `name`.  The selection order is total, so
+// the result is that of one whole-table scan.
+template <class K>
+int merge_rank_lists(ctr_handle* h, const char* name, typename K::T* ls, int* lr, typename K::T* gs, int* gr, int n, int k, size_t msmem,
+                     int* count) {
+    const long nk = (long)n * k;
+    RET(comm_gather_lists(h, ls, gs, sizeof(typename K::T), lr, gr, (size_t)nk));
+    return launch(h, name, [&] { knn::k_knn_merge<K><<<n, knn::kThreads, msmem, h->stream>>>(gs, gr, h->comm.world, k, k, nk, lr, ls, count); });
+}
+
 // The selection over logits of key type K, on h's stream.  Per user, chunk by chunk, k_rec_scan writes the slices'
 // lists behind the running list in sl[0, k); chunk 0 merges its slices only, later chunks merge the running list with
 // theirs, in place, and the last chunk writes the user's row of ls / lr.
 template <class K>
 struct RecTopk {
     using T = typename K::T;
-    ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge, <pre>_finish and <pre>_seen
+    ctr_handle* h; const char* pre;         // profile keys <pre>_topk, <pre>_merge, <pre>_merge_ranks, <pre>_finish and <pre>_seen
     int k, nex, world, rank;                // nex exclusion rows per user; local row l is global row l·world + rank
     int64_t N; int Bc;                      // the items scored, per chunk
     bool by_seen = false;                   // CTR_EXCLUDE_SEEN (nex = 0): each user's seen bitmap over the local rows excludes
@@ -1284,10 +1295,11 @@ struct RecTopk {
     const int rps = round_up(std::max(4 * knn::kStep, 8 * k), knn::kStep);
     const size_t ssmem = rec::scan_smem_bytes<K>(k, nex), msmem = knn::smem_bytes<K>(1, 0, k);
     const std::string n_topk = std::string(pre) + "_topk", n_merge = std::string(pre) + "_merge", n_finish = std::string(pre) + "_finish",
-                      n_seen = std::string(pre) + "_seen";
-    T *sl_s, *ls, *ol; int *sl_r, *lr, *orow, *oc; float* os; unsigned* seen = nullptr;
+                      n_seen = std::string(pre) + "_seen", n_ranks = std::string(pre) + "_merge_ranks";
+    T *sl_s, *ls, *ol, *gs = nullptr; int *sl_r, *lr, *orow, *oc, *gr = nullptr; float* os; unsigned* seen = nullptr;
 
-    // scratch slot `slot`: the caller's buffers (own(c)), then the running and slice lists, then [G][k] lists and outputs
+    // scratch slot `slot`: the caller's buffers (own(c)), then the running and slice lists, then [G][k] lists and
+    // outputs, and on a row-sharded table the [world][G][k] gather of the ranks' lists
     template <class F>
     int setup(int slot, int64_t G, F&& own) {
         CU(h, cudaFuncSetAttribute(rec::k_rec_scan<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
@@ -1303,6 +1315,7 @@ struct RecTopk {
             sl_s = c.take<T>(sl); sl_r = c.take<int>(sl);
             ls = c.take<T>(gk); lr = c.take<int>(gk); orow = c.take<int>(gk); ol = c.take<T>(gk); os = c.take<float>(gk); oc = c.take<int>(G);
             if (by_seen) seen = c.take<unsigned>((size_t)(N + 31) / 32);
+            if (world > 1) { gs = c.take<T>((size_t)world * gk); gr = c.take<int>((size_t)world * gk); }
             return c.used;
         };
         char* ws = nullptr;
@@ -1340,10 +1353,12 @@ struct RecTopk {
             RET(launch(h, n_merge.c_str(), [&] { knn::k_knn_merge<K><<<1, knn::kThreads, msmem, h->stream>>>(sl_s, sl_r, 0, k, 0, 0, ur, us, nullptr); }));
         return CTR_OK;
     }
-    // the lists of users [g0, g0 + ng) → the caller's outputs; after(n) runs under the same launch as k_rec_finish
+    // the lists of users [g0, g0 + ng), on a row-sharded table every rank's merged, → the caller's outputs; after(n)
+    // runs under the same launch as k_rec_finish
     template <class F>
     int finish(int64_t g0, int ng, int32_t* out_rows, float* out_scores, T* out_logits, int32_t* out_count, F&& after) {
         const long n = (long)ng * k;
+        if (world > 1) RET(merge_rank_lists<K>(h, n_ranks.c_str(), ls, lr, gs, gr, ng, k, msmem, nullptr));
         RET(launch(h, n_finish.c_str(), [&] {
             rec::k_rec_finish<K><<<(int)((n + 255) / 256), 256, 0, h->stream>>>(ls, lr, k, n, orow, ol, os, oc);
             after(n);
@@ -1478,24 +1493,50 @@ struct NeumaierSum {
     double value() const { return s + c; }
 };
 
-// ctr_recommend_topk's and ctr_rank_items' scoring pass on a single-GPU or row-sharded ITEM_EMB: the logits of items
-// [i0, i0 + nb) for (user, history uh on the device) into h->Z.  user_kernel: k_attn_fwd_user (ugrid CTAs); else index
-// buffers of the repeated user and history for the ordinary attention kernels.
-int rec_score_chunk(ctr_handle* h, bool user_kernel, bool coll, int ugrid, int user, const int* uh, int i0, int nb) {
-    const int S = h->cfg.S;
-    StepOpts o;
-    RowSrc r;
-    if (user_kernel) {
-        r = coll ? comm_src(h, nullptr, nullptr, nullptr, nb, false) : idx_src(h, nullptr, nullptr, nullptr, nb);
-        RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
-        o.x0_ready = true;
-    } else {
-        const int fg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)nb * std::max(S, 1) + 255) / 256, (int64_t)h->num_sms * 8));
-        RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
-        r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+// ctr_recommend_topk's and ctr_rank_items' scoring pass over the item table on a single-GPU or row-sharded (coll)
+// ITEM_EMB, in MlpRecScore's shape: chunk() leaves the logits of a chunk of items in z().  With the user kernel
+// (k_attn_fwd_user, ugrid CTAs) the user's history rows are staged in shared memory; else index buffers of the repeated
+// user and history feed the ordinary attention kernels.
+struct AttnRecScore {
+    ctr_handle* h;
+    bool coll;
+    bool user_kernel = false;
+    int ugrid = 0;
+
+    // the refusals of the handle's state, before anything is written
+    int check() {
+        const int T = CTR_TABLE_ITEM_EMB;
+        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
+        RET(coll ? comm_check(h) : check_tables(h));
+        const int64_t N = h->tab_rows[T];
+        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
+        int optin = 0;
+        CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
+        user_kernel = attn_user_ok(h, (size_t)optin);
+        if (coll && !user_kernel)
+            return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)",
+                           h->cfg.S, attn_user_smem(h), optin);
+        return CTR_OK;
     }
-    return step_core(h, r, nb, o);
-}
+    void prepare() { ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0; }
+    const float* z() const { return h->Z; }
+    // the logits of (local) items [i0, i0 + nb) for (user, history uh on the device) into z()
+    int chunk(int user, const int* uh, int i0, int nb) {
+        const int S = h->cfg.S;
+        StepOpts o;
+        RowSrc r;
+        if (user_kernel) {
+            r = coll ? comm_src(h, nullptr, nullptr, nullptr, nb, false) : idx_src(h, nullptr, nullptr, nullptr, nb);
+            RET(attn_forward_user(h, r, user, uh, i0, nb, ugrid));
+            o.x0_ready = true;
+        } else {
+            const int fg = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)nb * std::max(S, 1) + 255) / 256, (int64_t)h->num_sms * 8));
+            RET(launch(h, "rec_fill_idx", [&] { rec::k_rec_fill_idx<<<fg, 256, 0, h->stream>>>(user, uh, S, i0, nb, h->s_user, h->s_item, h->s_hist); }));
+            r = idx_src(h, h->s_user, h->s_item, h->s_hist, nb);
+        }
+        return step_core(h, r, nb, o);
+    }
+};
 
 }  // namespace
 
@@ -1872,6 +1913,19 @@ int keys_resolve_chunk(ctr_handle* h, int64_t c, size_t chunk, const int64_t* us
     }));
     return launch(h, "keys_advance", [&] { k_keys_advance<<<1, 1, 0, rs>>>(h->kt_pos + m, h->kt_count); });
 }
+
+// GetUserBehavior(user row d_user[i], S, -1, d_ts[i]) into out[i·S, i·S + S) for i < n, on stream st, under profile key
+// ubcache_window; no ubcache (no UserBehavior provider) → every history empty (rcmd.go:498,509)
+int ub_windows(ctr_handle* h, cudaStream_t st, const int* d_user, const long long* d_ts, int n, int* out) {
+    const int S = h->cfg.S;
+    if (!h->ub_off) {
+        CU(h, cudaMemsetAsync(out, 0xff, sizeof(int) * (size_t)n * S, st));
+        return CTR_OK;
+    }
+    return launch(h, "ubcache_window", [&] {
+        k_ub_window<<<grid_for_warps(h, n), 256, 0, st>>>(h->ub_off, h->ub_ts, h->ub_items, d_user, d_ts, n, S, (long)h->ub_users, out);
+    });
+}
 }  // namespace
 
 int ctr_train_idx(ctr_handle* h, const int32_t* user_row, const int32_t* item_row, const int32_t* hist, const float* label,
@@ -1971,12 +2025,7 @@ int ctr_train_keys(ctr_handle* h, const int64_t* user_ids, const int64_t* item_i
         int* hist = h->kt_hist[k];
         if (nv > 0) {
             if (nrun >= 2) CU(h, cudaStreamWaitEvent(h->win_stream, h->kt_used[k], 0));         // the step two batches back has read this buffer
-            if (h->ub_off) {
-                RET(launch(h, "ubcache_window", [&] {
-                    k_ub_window<<<grid_for_warps(h, nv), 256, 0, h->win_stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->kt_user + start, h->kt_ts + start, nv, S,
-                                                                                 (long)h->ub_users, hist);
-                }));
-            } else CU(h, cudaMemsetAsync(hist, 0xff, sizeof(int) * (size_t)nv * S, h->win_stream));   // no UserBehavior provider → empty history (rcmd.go:498,509)
+            RET(ub_windows(h, h->win_stream, h->kt_user + start, h->kt_ts + start, nv, hist));
             CU(h, cudaEventRecord(h->kt_win[k], h->win_stream));
             CU(h, cudaStreamWaitEvent(h->stream, h->kt_win[k], 0));
         }
@@ -2154,10 +2203,7 @@ int ctr_ubcache_window_dev(ctr_handle* h, const int32_t* d_user_row, const int64
     if (!h || !d_user_row || !d_max_ts || !d_hist_rows || B < 1) return set_err(h, CTR_EINVAL, "bad ubcache window arguments");
     if (!h->ub_off) return set_err(h, CTR_ESTATE, "ubcache not uploaded");
     CU(h, cudaSetDevice(h->dev));
-    return launch(h, "ubcache_window", [&] {
-        k_ub_window<<<grid_for_warps(h, B), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_user_row, (const long long*)d_max_ts, B, h->cfg.S,
-                                                               (long)h->ub_users, d_hist_rows);
-    });
+    return ub_windows(h, h->stream, d_user_row, (const long long*)d_max_ts, B, d_hist_rows);
 }
 
 int ctr_ubcache_window(ctr_handle* h, const int32_t* user_row, const int64_t* max_ts, int32_t B, int32_t* hist_rows) {
@@ -3001,52 +3047,51 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
         if (queries) hd.hash[0] = comm_hash(queries, (size_t)nq * h->cfg.D * sizeof(double));
         if (query_rows) hd.hash[1] = comm_hash(query_rows, (size_t)nq * sizeof(int32_t));
     }
-    if (verdict != CTR_OK) {
-        if (!coll) return verdict;
-        const int rc = comm_agree(h, hd, verdict);
-        return rc != CTR_OK ? rc : verdict;
-    }
     const int64_t N = h->tab_local_rows[T];   // the rows this rank scans
     const int D = h->tab_width[T], Dp = (D + 3) & ~3;
-    // query tile: as wide as the batch needs, narrower when k's lists would not fit shared memory
-    int QT = 16;
-    while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
-    const size_t smem = knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k), msmem = knn::smem_bytes<knn::SimKey>(1, 0, k);
     // Row queries on a shard: the query rows are gathered (hot rows from the replica, the others from their owners)
     // and widened to float64, then scanned as vector queries that exclude their own row.  A product of two widened
     // floats is exact in float64, so the unfused sums of the vector instantiation equal the fused ones of ROWQ bit for bit.
     const bool rowq = by_row && !coll;
-    int occ = 1;      // also sets the instantiation's shared-memory limit
-    if (rowq) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
-    // row slices: enough CTAs to fill the GPU with the least idle tail (whole waves of resident CTAs); queries are
-    // chunked so that the slices' lists (and on a sharded table the ranks' gathered lists) stay within 256 MB of scratch
-    // On a shard the plan is made for the largest shard (rank 0's), so that every rank picks the same query chunk and
-    // the ranks' all-gathers match.
-    const int64_t Nplan = coll ? (h->tab_rows[T] + W - 1) / W : N;
-    const long steps = std::max<long>(1, (long)((Nplan + knn::kStep - 1) / knn::kStep));
     const int gw = coll ? W : 0;
-    const long wave = (long)h->num_sms * occ;
-    int64_t chunk = std::min<int64_t>(nq, 1024);
-    int slices = 1;
-    for (;;) {
-        const long tiles = (long)((chunk + QT - 1) / QT);
-        double best = -1;
-        for (long m = 1; m <= 8; m++) {
-            const long s = std::max<long>(1, std::min<long>({(m * wave + tiles - 1) / tiles, steps, 4096}));
-            const double w = (double)(s * tiles) / wave, eff = w / std::ceil(w);
-            if (eff > best + 0.02) { best = eff; slices = (int)s; }
+    const size_t msmem = knn::smem_bytes<knn::SimKey>(1, 0, k);
+    // the plan, made only when this rank's checks passed (the agreement reads it only when every rank's did)
+    int QT = 16, slices = 1;
+    int64_t chunk = 0;
+    long rps = 0;
+    size_t smem = 0;
+    if (verdict == CTR_OK) {
+        // query tile: as wide as the batch needs, narrower when k's lists would not fit shared memory
+        while (QT > 1 && (QT / 2 >= nq || knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k) > ((size_t)200 << 10))) QT /= 2;
+        smem = knn::kTileBytes + knn::smem_bytes<knn::SimKey>(QT, Dp, k);
+        int occ = 1;      // also sets the instantiation's shared-memory limit
+        if (rowq) knn_scan_dispatch<true>(h, QT, KnnArgs{}, true, smem, &occ); else knn_scan_dispatch<false>(h, QT, KnnArgs{}, true, smem, &occ);
+        // row slices: enough CTAs to fill the GPU with the least idle tail (whole waves of resident CTAs); queries are
+        // chunked so that the slices' lists (and on a sharded table the ranks' gathered lists) stay within 256 MB of scratch
+        // On a shard the plan is made for the largest shard (rank 0's), so that every rank picks the same query chunk and
+        // the ranks' all-gathers match.
+        const int64_t Nplan = coll ? (h->tab_rows[T] + W - 1) / W : N;
+        const long steps = std::max<long>(1, (long)((Nplan + knn::kStep - 1) / knn::kStep));
+        const long wave = (long)h->num_sms * occ;
+        chunk = std::min<int64_t>(nq, 1024);
+        for (;;) {
+            const long tiles = (long)((chunk + QT - 1) / QT);
+            double best = -1;
+            for (long m = 1; m <= 8; m++) {
+                const long s = std::max<long>(1, std::min<long>({(m * wave + tiles - 1) / tiles, steps, 4096}));
+                const double w = (double)(s * tiles) / wave, eff = w / std::ceil(w);
+                if (eff > best + 0.02) { best = eff; slices = (int)s; }
+            }
+            if (chunk == 1 || (size_t)chunk * (slices + gw) * k * 12 <= ((size_t)256 << 20)) break;
+            chunk = (chunk + 1) / 2;
         }
-        if (chunk == 1 || (size_t)chunk * (slices + gw) * k * 12 <= ((size_t)256 << 20)) break;
-        chunk = (chunk + 1) / 2;
+        rps = (steps + slices - 1) / slices * knn::kStep;
+        slices = (int)std::max<int64_t>(1, (N + rps - 1) / rps);     // an empty shard still writes (empty) lists
     }
-    const long rps = (steps + slices - 1) / slices * knn::kStep;
-    slices = (int)std::max<int64_t>(1, (N + rps - 1) / rps);     // an empty shard still writes (empty) lists
-    if (coll) {
+    if (!coll) RET(verdict);
+    else {
         hd.plan = chunk;                 // the number of list all-gathers follows from it: checked, not assumed equal
-        RET(comm_agree(h, hd, CTR_OK));
-        RET(comm_ensure(h, false));
-        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
-        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+        RET(comm_serve_enter(h, hd, verdict));
     }
 
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -3077,15 +3122,11 @@ int ctr_knn_search(ctr_handle* h, const double* queries, const int32_t* query_ro
             if (rowq) knn_scan_dispatch<true>(h, QT, a, false, smem, &unused); else knn_scan_dispatch<false>(h, QT, a, false, smem, &unused);
         }));
         const long sk = (long)slices * k;
-        if (!coll) {
-            RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, sk, k, d_or, d_os, d_oc); }));
-        } else {      // this rank's lists, then every rank's: the same total order, so the same result as one whole-table scan
-            RET(launch(h, "knn_merge", [&] { knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, sk, k, d_or, d_os, nullptr); }));
-            RET(comm_gather_lists(h, d_os, d_gs, sizeof(double), d_or, d_gr, (size_t)n * k));
-            RET(launch(h, "knn_merge_ranks", [&] {
-                knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_gs, d_gr, W, k, k, (long)n * k, d_or, d_os, d_oc);
-            }));
-        }
+        // this rank's lists, then on a shard every rank's
+        RET(launch(h, "knn_merge", [&] {
+            knn::k_knn_merge<knn::SimKey><<<n, knn::kThreads, msmem, h->stream>>>(d_ls, d_lr, slices, k, sk, k, d_or, d_os, coll ? nullptr : d_oc);
+        }));
+        if (coll) RET(merge_rank_lists<knn::SimKey>(h, "knn_merge_ranks", d_os, d_or, d_gs, d_gr, n, k, msmem, d_oc));
         CU(h, cudaMemcpyAsync(out_rows + s * k, d_or, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_sim + s * k, d_os, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaMemcpyAsync(out_count + s, d_oc, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -3109,25 +3150,13 @@ int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t
     const bool coll = emb_sharded(h);
     const int W = coll ? h->comm.world : 1;
     const int S = h->cfg.S, Bc = h->Bmax;
-    int optin = 0;
-    bool user_kernel = false;
+    AttnRecScore sc{h, coll};
     CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
     const bool args_ok = !(k < 1 || k > knn::kMaxK || nu < 1 || !user_rows || !hist_rows || !out_rows || !out_scores || !out_count) &&
                          exclude_ok(exclude, max_ts);
-    const int verdict = [&]() -> int {
-        if (!args_ok)
-            return set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs, "
-                                          "exclude in [0, 2], max_ts under CTR_EXCLUDE_SEEN)", knn::kMaxK);
-        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
-        RET(coll ? comm_check(h) : check_tables(h));
-        const int64_t N = h->tab_rows[T];
-        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
-        CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
-        user_kernel = attn_user_ok(h, (size_t)optin);
-        if (coll && !user_kernel)
-            return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)", S, attn_user_smem(h), optin);
-        return CTR_OK;
-    }();
+    const int verdict = args_ok ? sc.check()
+                                : set_err(h, CTR_EINVAL, "bad recommend arguments (k in [1, %d], nu >= 1, user and history rows, non-null outputs, "
+                                                         "exclude in [0, 2], max_ts under CTR_EXCLUDE_SEEN)", knn::kMaxK);
     if (!coll) RET(verdict);
     else {
         // the arguments are hashed whenever they are well-formed, whatever this rank's state (see ctr_knn_search)
@@ -3139,37 +3168,22 @@ int ctr_recommend_topk_ex(ctr_handle* h, const int32_t* user_rows, const int32_t
             if (exclude == CTR_EXCLUDE_SEEN) hd.hash[2] = comm_hash(max_ts, (size_t)nu * sizeof(int64_t));
             hd.plan = std::min<int64_t>(nu, 256);      // users per list all-gather (G below)
         }
-        const int rc = comm_agree(h, hd, verdict);
-        if (rc != CTR_OK || verdict != CTR_OK) return rc != CTR_OK ? rc : verdict;
-        RET(comm_ensure(h, false));
-        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
-        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+        RET(comm_serve_enter(h, hd, verdict));
     }
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
-    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
+    sc.prepare();
     const bool seen = exclude == CTR_EXCLUDE_SEEN;
     RecTopk<knn::LogitKey> sel{h, "rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, N, Bc, seen, h->tab_rows[T]};
     const int64_t G = std::min<int64_t>(nu, 256);          // users per result copy
-    int* d_hist; float* d_gs = nullptr; int* d_gr = nullptr;      // [W][G][k] the ranks' lists of the group
-    RET(sel.setup(4, G, [&](Carve& c) {
-        d_hist = c.take<int>((size_t)G * S);
-        if (coll) { d_gs = c.take<float>((size_t)W * G * k); d_gr = c.take<int>((size_t)W * G * k); }
-    }));
+    int* d_hist;
+    RET(sel.setup(4, G, [&](Carve& c) { d_hist = c.take<int>((size_t)G * S); }));
     for (int64_t g0 = 0; g0 < nu; g0 += G) {
         const int ng = (int)std::min<int64_t>(G, nu - g0);
         if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + g0 * S, (size_t)ng * S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
         for (int j = 0; j < ng; j++) {
             const int user = user_rows[g0 + j];
             const int* uh = d_hist + (size_t)j * S;
-            RET(sel.user(j, uh, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, uh, i0, nb); },
-                         user, seen ? max_ts[g0 + j] : 0));
-        }
-        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
-            const long n = (long)ng * k;
-            RET(comm_gather_lists(h, sel.ls, d_gs, sizeof(float), sel.lr, d_gr, (size_t)n));
-            RET(launch(h, "rec_merge_ranks", [&] {
-                knn::k_knn_merge<knn::LogitKey><<<ng, knn::kThreads, sel.msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, sel.lr, sel.ls, nullptr);
-            }));
+            RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(user, uh, i0, nb); }, user, seen ? max_ts[g0 + j] : 0));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [](long) {}));
     }
@@ -3190,25 +3204,13 @@ int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hi
     const bool coll = emb_sharded(h);
     const int W = coll ? h->comm.world : 1;
     const int S = h->cfg.S, Bc = h->Bmax;
-    int optin = 0;
-    bool user_kernel = false;
+    AttnRecScore sc{h, coll};
     CU(h, cudaSetDevice(h->dev));        // before any CUDA call, the agreement's lazy staging buffer included
     const bool args_ok = !(n < 1 || !user_rows || !hist_rows || !item_rows || !out_rank) && exclude_ok(exclude, max_ts);
     const bool seen = exclude == CTR_EXCLUDE_SEEN;
-    const int verdict = [&]() -> int {
-        if (!args_ok)
-            return set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank, exclude in [0, 2], "
-                                          "max_ts under CTR_EXCLUDE_SEEN)");
-        if (!h->tab[T]) return set_err(h, CTR_ESTATE, "ITEM_EMB table not uploaded");
-        RET(coll ? comm_check(h) : check_tables(h));
-        const int64_t N = h->tab_rows[T];
-        if (N > INT32_MAX) return set_err(h, CTR_ESTATE, "ITEM_EMB has %lld rows: row ids are int32", (long long)N);
-        CU(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
-        user_kernel = attn_user_ok(h, (size_t)optin);
-        if (coll && !user_kernel)
-            return set_err(h, CTR_ESTATE, "recommendation on a row-sharded ITEM_EMB needs the user's %d history rows in shared memory (%zu bytes > %d)", S, attn_user_smem(h), optin);
-        return CTR_OK;
-    }();
+    const int verdict = args_ok ? sc.check()
+                                : set_err(h, CTR_EINVAL, "bad rank arguments (n >= 1, user, history and item rows, non-null out_rank, exclude in [0, 2], "
+                                                         "max_ts under CTR_EXCLUDE_SEEN)");
     // keys with the same user row and window (and under CTR_EXCLUDE_SEEN the same cut) share a pass
     std::vector<std::vector<int64_t>> passes;
     if (args_ok)
@@ -3229,14 +3231,10 @@ int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hi
             if (seen) hd.hash[2] = comm_hash(max_ts, (size_t)n * sizeof(int64_t), hd.hash[2]);      // the cuts, chained
             hd.plan = (int64_t)passes.size();            // two collectives per pass
         }
-        const int rc = comm_agree(h, hd, verdict);
-        if (rc != CTR_OK || verdict != CTR_OK) return rc != CTR_OK ? rc : verdict;
-        RET(comm_ensure(h, false));
-        RET(comm_barrier(h));            // every rank's row updates queued before this call have landed
-        RET(comm_hot_writeback(h));      // the shard's copies of the hot rows are current
+        RET(comm_serve_enter(h, hd, verdict));
     }
     const int64_t N = h->tab_local_rows[T];   // the items this rank scores
-    const int ugrid = user_kernel ? h->num_sms * attn_user_prepare(h, coll) : 0;
+    sc.prepare();
     RecRank<knn::LogitKey> rk{h, "rank", exclude == CTR_EXCLUDE_WINDOW ? S : 0, N, Bc, W, coll ? h->comm.rank : 0, h->tab_rows[T], seen};
     int* d_hist;
     RET(rk.setup(4, [&](Carve& c) { d_hist = c.take<int>((size_t)S); }));
@@ -3247,8 +3245,8 @@ int ctr_rank_items_ex(ctr_handle* h, const int32_t* user_rows, const int32_t* hi
         const int user = user_rows[i], m = (int)p.size();
         for (int j = 0; j < m; j++) trow[j] = item_rows[p[j]];
         if (S > 0) CU(h, cudaMemcpyAsync(d_hist, hist_rows + i * S, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-        RET(rk.pass(trow.data(), m, d_hist, h->Z, [&](int i0, int nb) { return rec_score_chunk(h, user_kernel, coll, ugrid, user, d_hist, i0, nb); },
-                    pr.data(), pl.data(), user, seen ? max_ts[i] : 0));
+        RET(rk.pass(trow.data(), m, d_hist, sc.z(), [&](int i0, int nb) { return sc.chunk(user, d_hist, i0, nb); }, pr.data(), pl.data(), user,
+                    seen ? max_ts[i] : 0));
         for (int j = 0; j < m; j++) { rank[(size_t)p[j]] = pr[j]; logit[(size_t)p[j]] = pl[j]; }
     }
     memcpy(out_rank, rank.data(), sizeof(int64_t) * (size_t)n);
@@ -4702,17 +4700,14 @@ int mlp_keys_check(ctr_mlp* m, ctr_handle* h) {
     RET(comm_check_emb(h));
     return check_widths(h);
 }
-// the agreement of a collective key-fed call (comm_agree, on a row-sharded ITEM_EMB): a rank whose checks failed takes
-// part with its message, and every rank returns the same verdict.  Then, as for ctr_recommend_topk_ex, the mappings
-// are published, every rank's row updates queued before the call have landed and the shard's hot rows are current.
+// the entry of a collective key-fed call (comm_serve_enter, on a row-sharded ITEM_EMB): a rank whose checks failed takes
+// part with its message, and every rank returns the same verdict
 int mlp_agree(ctr_mlp* m, ctr_handle* h, CommHdr hd, int verdict) {
     if (verdict != CTR_OK && h->err.empty()) h->err = m->err;
     CU(h, cudaSetDevice(h->dev));        // the checks may have stopped before making it current
-    const int rc = comm_agree(h, hd, verdict);
-    if (rc != CTR_OK) { m->err = h->err; return rc; }
-    RET(comm_ensure(h, false));
-    RET(comm_barrier(h));
-    return comm_hot_writeback(h);
+    const int rc = comm_serve_enter(h, hd, verdict);
+    if (rc != CTR_OK) m->err = h->err;
+    return rc;
 }
 // every exit of a key-fed call: no work of m may still read h's buffers, and the message is readable from both objects
 int mlp_keys_done(ctr_mlp* m, ctr_handle* h, int rc) {
@@ -4758,12 +4753,7 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
     const long ns = (long)used;
     // ---- every survivor's history, GetUserBehavior(uid, S, -1, ts), cut once: h->mu is held, so the cache stays as it is
     RET(reserve(h, h->kt_hist_all, (size_t)ns * S, false));
-    if (h->ub_off) {
-        RET(launch(h, "ubcache_window", [&] {
-            k_ub_window<<<grid_for_warps(h, (int)ns), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, h->kt_user, h->kt_ts, (int)ns, S,
-                                                                           (long)h->ub_users, h->kt_hist_all);
-        }));
-    } else CU(h, cudaMemsetAsync(h->kt_hist_all, 0xff, sizeof(int) * (size_t)ns * S, h->stream));   // no UserBehavior provider → empty history
+    RET(ub_windows(h, h->stream, h->kt_user, h->kt_ts, (int)ns, h->kt_hist_all));
     // ---- the classifier: minibatch k's rows are gathered on h's stream into stage[k & 1] while minibatch k-1 trains
     const long bs = mlp_batch(m, ns);
     if (m->idx.size() < (size_t)ns) MCU(m, m->idx.alloc((size_t)ns));
@@ -4947,13 +4937,11 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids, 
     const bool seen = exclude == CTR_EXCLUDE_SEEN;
     RecTopk<knn::Logit64Key> sel{h, "mlp_rec", k, exclude == CTR_EXCLUDE_WINDOW ? S : 0, W, coll ? h->comm.rank : 0, sc.NL, sc.Bc, seen, sc.N};
     long long *d_ids, *d_ts; int *d_urow, *d_hist; double* d_pre;
-    double* d_gs = nullptr; int* d_gr = nullptr;                         // [W][G][k] the ranks' lists of the group
     std::vector<int> urow;
     const int verdict = vcheck != CTR_OK ? vcheck : [&]() -> int {
         RET(sel.setup(6, G, [&](Carve& cv) {
             d_ids = cv.take<long long>(nu); d_urow = cv.take<int>(nu); d_ts = cv.take<long long>(G); d_hist = cv.take<int>((size_t)G * S);
             d_pre = cv.take<double>(sc.H);
-            if (coll) { d_gs = cv.take<double>((size_t)W * G * k); d_gr = cv.take<int>((size_t)W * G * k); }
         }));
         CU(h, cudaMemcpyAsync(d_ids, user_ids, (size_t)nu * 8, cudaMemcpyHostToDevice, h->stream));
         RET(launch(h, "mlp_rec_resolve", [&] {
@@ -4984,24 +4972,13 @@ int mlp_recommend(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids, 
         const int ng = (int)std::min<int64_t>(G, nu - g0);
         // GetUserBehavior(uid, S, -1, ts) from the device ubcache; no ubcache → an empty history (ctr_mlp_predict_keys).
         // On a shard every rank takes rank 0's windows, so every rank scores for the same ones.
-        if (h->ub_off) {
-            CU(h, cudaMemcpyAsync(d_ts, ts + g0, sizeof(long long) * (size_t)ng, cudaMemcpyHostToDevice, h->stream));
-            RET(launch(h, "ubcache_window", [&] {
-                k_ub_window<<<grid_for_warps(h, ng), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow + g0, d_ts, ng, S, (long)h->ub_users, d_hist);
-            }));
-        } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)ng * S, h->stream));
+        if (h->ub_off) CU(h, cudaMemcpyAsync(d_ts, ts + g0, sizeof(long long) * (size_t)ng, cudaMemcpyHostToDevice, h->stream));
+        RET(ub_windows(h, h->stream, d_urow + g0, d_ts, ng, d_hist));
         if (coll && S > 0) RET(comm_bcast0(h, d_hist, sizeof(int) * (size_t)ng * S));
         for (int j = 0; j < ng; j++) {
             const int* uh = d_hist + (size_t)j * S;
             RET(sc.prefix(urow[(size_t)(g0 + j)], uh, d_pre));
             RET(sel.user(j, uh, sc.z(), [&](int i0, int nb) { return sc.chunk(d_pre, i0, nb); }, urow[(size_t)(g0 + j)], ts[g0 + j]));
-        }
-        if (coll) {      // every rank's lists of the group, merged: the same total order, so the same result as one whole-table scan
-            const long n = (long)ng * k;
-            RET(comm_gather_lists(h, sel.ls, d_gs, sizeof(double), sel.lr, d_gr, (size_t)n));
-            RET(launch(h, "mlp_rec_merge_ranks", [&] {
-                knn::k_knn_merge<knn::Logit64Key><<<ng, knn::kThreads, sel.msmem, h->stream>>>(d_gs, d_gr, W, k, k, n, sel.lr, sel.ls, nullptr);
-            }));
         }
         RET(sel.finish(g0, ng, out_rows, out_scores, out_logits, out_count, [&](long n) {
             // an identity output's score is the predicted value itself, as ctr_mlp_predict_keys returns it
@@ -5075,10 +5052,8 @@ int mlp_rank_items(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids,
     if (h->ub_off) {
         CU(h, cudaMemcpyAsync(d_urow, pu.data(), sizeof(int) * (size_t)nw, cudaMemcpyHostToDevice, h->stream));
         CU(h, cudaMemcpyAsync(d_ts, pts.data(), sizeof(long long) * (size_t)nw, cudaMemcpyHostToDevice, h->stream));
-        RET(launch(h, "ubcache_window", [&] {
-            k_ub_window<<<grid_for_warps(h, nw), 256, 0, h->stream>>>(h->ub_off, h->ub_ts, h->ub_items, d_urow, d_ts, nw, S, (long)h->ub_users, d_hist);
-        }));
-    } else CU(h, cudaMemsetAsync(d_hist, 0xff, sizeof(int) * (size_t)nw * S, h->stream));
+    }
+    RET(ub_windows(h, h->stream, d_urow, d_ts, nw, d_hist));
     if (coll && S > 0) RET(comm_bcast0(h, d_hist, sizeof(int) * (size_t)nw * S));
 
     sc.bind_rows();
