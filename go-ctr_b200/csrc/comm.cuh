@@ -73,13 +73,14 @@ struct CommHdr {
     uint64_t hash[3];
     int64_t plan;               // what fixes the number of collectives (queries per chunk / users per group / rank passes)
     uint64_t rows;              // a hash of the rows this rank's id maps resolved the call's ids to (0: no ids)
-    char msg[192];              // ... and its message
+    int64_t share;              // this rank's own share of the call (ctr_item_emb_train: its tokens); never compared
+    char msg[184];              // ... and its message
 };
 static_assert(sizeof(CommHdr) == 256, "one all-gather slot of Comm::d_xchg");
 
 }  // namespace ctr
 
-static int comm_agree(ctr_handle* h, ctr::CommHdr hd, int verdict);
+static int comm_agree(ctr_handle* h, ctr::CommHdr hd, int verdict, int64_t* shares = nullptr);
 static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, size_t score_bytes, const int* send_r, int* recv_r, size_t n);
 static int comm_allreduce_grads(ctr_handle* h, float* extra, size_t extra_n);
 static int comm_train_step(ctr_handle* h, const int32_t* d_user, const int32_t* d_item, const int32_t* d_hist, const float* d_label, int32_t B, int32_t nvalid);
@@ -87,6 +88,7 @@ static int comm_predict(ctr_handle* h, const int32_t* d_user, const int32_t* d_i
 static int comm_barrier(ctr_handle* h);
 static int comm_max_i64(ctr_handle* h, int64_t* v);
 static int comm_sum_u64(ctr_handle* h, unsigned long long* buf, size_t n);
+static int comm_min_u64(ctr_handle* h, unsigned long long* buf, size_t n);
 static int comm_bcast0(ctr_handle* h, void* buf, size_t bytes);
 static int comm_unique_id(void* id_out, int32_t* id_bytes);
 static int comm_init(ctr_handle* h, const void* id, int32_t id_bytes);

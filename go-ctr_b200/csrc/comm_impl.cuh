@@ -21,7 +21,7 @@ struct NcclApi {
     int (*Recv)(void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     const char* (*GetErrorString)(int) = nullptr;
 };
-enum { kNcclChar = 0, kNcclInt32 = 2, kNcclInt64 = 4, kNcclUint64 = 5, kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2 };
+enum { kNcclChar = 0, kNcclInt32 = 2, kNcclInt64 = 4, kNcclUint64 = 5, kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2, kNcclMin = 3 };
 
 NcclApi g_nccl;
 
@@ -290,7 +290,8 @@ static uint64_t comm_hash(const void* p, size_t bytes, uint64_t seed = 146959810
 // others blocked in NCCL: headers that differ give CTR_EINVAL everywhere, else the verdict of the lowest failing rank,
 // else CTR_EINVAL if the ranks' plans differ (hd.plan is read only when every rank is valid).  A failure after the
 // agreement (out of memory for scratch, a failed publish) still leaves the peers waiting, as in the sharded train step.
-static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
+// shares (optional, [world]): every rank's hd.share, filled once the agreement holds.
+static int comm_agree(ctr_handle* h, CommHdr hd, int verdict, int64_t* shares) {
     Comm& cm = h->comm;
     if (!cm.ready) return set_err(h, CTR_ESTATE, "world=%d but ctr_comm_init was not called", cm.world);
     hd.code = verdict;
@@ -319,6 +320,8 @@ static int comm_agree(ctr_handle* h, CommHdr hd, int verdict) {
         if (all[(size_t)j].plan != all[0].plan)
             return set_err(h, CTR_EINVAL, "ranks disagree on the plan of this collective call: rank %d would exchange %lld entries per round, rank 0 %lld",
                            j, (long long)all[(size_t)j].plan, (long long)all[0].plan);
+    if (shares)
+        for (int j = 0; j < W; j++) shares[j] = all[(size_t)j].share;
     return CTR_OK;
 }
 
@@ -351,6 +354,14 @@ static int comm_gather_lists(ctr_handle* h, const void* send_s, void* recv_s, si
 static int comm_sum_u64(ctr_handle* h, unsigned long long* buf, size_t n) {
     Comm& cm = h->comm;
     NC(h, g_nccl.AllReduce(buf, buf, n, kNcclUint64, kNcclSum, cm.nccl, h->stream));
+    h->launches += 1;
+    return CTR_OK;
+}
+
+// buf[0, n) at its minimum over the ranks, in place on the engine stream (ctr_item_emb_train's first-occurrence tags)
+static int comm_min_u64(ctr_handle* h, unsigned long long* buf, size_t n) {
+    Comm& cm = h->comm;
+    NC(h, g_nccl.AllReduce(buf, buf, n, kNcclUint64, kNcclMin, cm.nccl, h->stream));
     h->launches += 1;
     return CTR_OK;
 }

@@ -112,6 +112,7 @@ struct ctr_handle {
     VmmBuf tab_vmm[3];                    // a sharded table lives in shareable (VMM) memory; tab[] points into it
     GrowBuf<float> tab_mem[3];            // any other table lives in growable memory (ctr_table_write_rows); tab[] points into it
     uint64_t tab_gen = 1;                 // bumped whenever an ITEM_* table is (re)allocated: peers must re-map it
+    std::vector<int64_t> emb_vocab;       // ctr_item_emb_train's vocabulary when the caller's vocab_ids could not take it all
 
     // learnables, padded storage: W0 [Kp,H0p] W1 [H0p,H1p] W2 [H1p] att [Sp]; grads / Adam moments alike
     DevBuf<float> W[4], Mo[4], Vo[4];
@@ -3599,72 +3600,163 @@ int ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, i
 
 // recommend.Train's embedding stage (rcmd.go:207-213, 538-545) into the handle's ITEM_EMB: first-appearance numbering of
 // the item-id stream on the device (item2vec.cuh, idmap.cuh), the trainer on that document, one scatter into the rows.
+// With world > 1 every rank numbers its own shard of the stream against the words of the ranks' streams concatenated in
+// rank order (the first-occurrence tags of i2v_dict_ranks), trains its shard with model averaging and writes its rows.
+namespace {
+// world > 1: every rank's verdict, the configuration (device aside), ITEM_EMB's shape and placement, the item map (its
+// size and digest, compared once every rank is valid) and every rank's token count, in one agreement
+int item_emb_agree(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n, int64_t cap, int64_t* total) {
+    const int W = h->comm.world;
+    int verdict = CTR_OK;
+    if (!cfg || n < 0 || n > 0x7fffffffLL || (n > 0 && !item_ids) || cap < 0) verdict = set_err(h, CTR_EINVAL, "bad item embedding arguments");
+    else if (cfg->dim != h->cfg.D) verdict = set_err(h, CTR_EINVAL, "item2vec dim %d != model dim D=%d", cfg->dim, h->cfg.D);
+    else if ((verdict = i2v_check_cfg(*cfg, h)) != CTR_OK) {}
+    else if (cfg->reserved[0] == 1) verdict = set_err(h, CTR_EINVAL, "the sequential float64 mode is single-GPU");
+    else if (!h->idm_keys[CTR_IDMAP_ITEM]) verdict = set_err(h, CTR_ESTATE, "ctr_item_emb_train needs the item id map (ctr_idmap_build)");
+    else if (W > kMaxPeers) verdict = set_err(h, CTR_EINVAL, "ctr_item_emb_train supports at most %d ranks, got %d", kMaxPeers, W);
+    CommHdr hd{};
+    if (cfg) { ctr_i2v_config cc = *cfg; cc.device = 0; hd.hash[0] = comm_hash(&cc, sizeof cc); }
+    const int T = CTR_TABLE_ITEM_EMB;
+    const int64_t tab[4] = {h->tab[T] ? 1 : 0, h->tab_rows[T], h->tab_width[T], h->tab_sharded[T] ? 1 : 0};
+    hd.hash[1] = comm_hash(tab, sizeof tab);
+    hd.share = verdict == CTR_OK ? n : 0;
+    if (h->idm_keys[CTR_IDMAP_ITEM]) {
+        unsigned long long* d_dig = nullptr;
+        RET(scratch_get(h, 2, sizeof(unsigned long long), (void**)&d_dig));
+        CU(h, cudaMemsetAsync(d_dig, 0, sizeof(unsigned long long), h->stream));
+        RET(launch(h, "idmap_digest", [&] {
+            k_idmap_digest<<<h->num_sms * 8, 256, 0, h->stream>>>(h->idm_keys[CTR_IDMAP_ITEM], h->idm_vals[CTR_IDMAP_ITEM], h->idm_keys[CTR_IDMAP_ITEM].size(), d_dig);
+        }));
+        uint64_t map[2] = {(uint64_t)h->idm_n[CTR_IDMAP_ITEM], 0};
+        CU(h, cudaMemcpyAsync(&map[1], d_dig, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        hd.rows = comm_hash(map, sizeof map);
+    }
+    std::vector<int64_t> shares((size_t)W);
+    RET(comm_agree(h, hd, verdict, shares.data()));
+    *total = 0;
+    for (int64_t v : shares) *total += v;
+    if (*total == 0) return set_err(h, CTR_EINVAL, "ctr_item_emb_train: every rank's stream is empty");
+    return CTR_OK;
+}
+}  // namespace
+
 int ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n, int64_t* vocab_ids, int64_t cap,
                        int32_t* vocab, ctr_i2v_stats* stats) {
     if (!h) return set_err(nullptr, CTR_EINVAL, "null handle");
-    if (!cfg || !item_ids || n < 1 || n > 0x7fffffffLL || cap < 0) return set_err(h, CTR_EINVAL, "bad item embedding arguments");
+    Comm& cm = h->comm;
+    const int W = cm.world;
     std::lock_guard<std::mutex> lk(h->mu);
+    std::vector<int64_t>().swap(h->emb_vocab);
+    if (W == 1 && (!cfg || !item_ids || n < 1 || n > 0x7fffffffLL || cap < 0)) return set_err(h, CTR_EINVAL, "bad item embedding arguments");
+    if (W > 1) {
+        int64_t total = 0;
+        RET(item_emb_agree(h, cfg, item_ids, n, cap, &total));
+    } else {
+        if (cfg->dim != h->cfg.D) return set_err(h, CTR_EINVAL, "item2vec dim %d != model dim D=%d", cfg->dim, h->cfg.D);
+        RET(i2v_check_cfg(*cfg, h));
+        if (!h->idm_keys[CTR_IDMAP_ITEM]) return set_err(h, CTR_ESTATE, "ctr_item_emb_train needs the item id map (ctr_idmap_build)");
+    }
     const ctr_i2v_config& c = *cfg;
-    if (c.dim != h->cfg.D) return set_err(h, CTR_EINVAL, "item2vec dim %d != model dim D=%d", c.dim, h->cfg.D);
-    RET(i2v_check_cfg(c, h));
-    if (!h->idm_keys[CTR_IDMAP_ITEM]) return set_err(h, CTR_ESTATE, "ctr_item_emb_train needs the item id map (ctr_idmap_build)");
-    if (h->comm.world > 1) return set_err(h, CTR_ESTATE, "ctr_item_emb_train is single-GPU (world = %d)", h->comm.world);
     CU(h, cudaSetDevice(h->dev));
     cudaStream_t st = h->stream;
     const long R = (long)h->idm_n[CTR_IDMAP_ITEM];
     const int G = h->num_sms * 8;
+    const unsigned long long* mkeys = h->idm_keys[CTR_IDMAP_ITEM]; const int* mvals = h->idm_vals[CTR_IDMAP_ITEM];
+    const unsigned long long mcap = h->idm_keys[CTR_IDMAP_ITEM].size();
+    // the numbering across ranks runs under its own profile key; on one GPU its steps keep the keys of the steps they extend
+    const char* across_side = W > 1 ? "i2v_dict_ranks" : "i2v_dict_side";
+    const char* across_rows = W > 1 ? "i2v_dict_ranks" : "i2v_dict_rank";
     // kept to the end: the word-id document, row -> word, the vocabulary's item ids, the trained vectors
     DevBuf<int> d_doc, d_word_row; DevBuf<long long> d_vocab; DevBuf<float> d_syn0;
     int V = 0;
     {
-        DevBuf<long long> d_ids; DevBuf<unsigned> d_first; DevBuf<unsigned long long> d_cnt;
+        DevBuf<long long> d_ids; DevBuf<unsigned> d_first; DevBuf<unsigned long long> d_cnt, d_row_tag;
         CU(h, d_ids.alloc((size_t)n)); CU(h, d_doc.alloc((size_t)n));
-        CU(h, d_first.alloc((size_t)R)); CU(h, d_word_row.alloc((size_t)R)); CU(h, d_cnt.alloc(2));
-        CU(h, big_copy(d_ids, item_ids, sizeof(int64_t) * (size_t)n, true, st));
+        CU(h, d_first.alloc((size_t)R)); CU(h, d_row_tag.alloc((size_t)R)); CU(h, d_word_row.alloc((size_t)R)); CU(h, d_cnt.alloc(2));
+        if (n > 0) CU(h, big_copy(d_ids, item_ids, sizeof(int64_t) * (size_t)n, true, st));
         CU(h, cudaMemsetAsync(d_first, 0xff, sizeof(unsigned) * (size_t)R, st));
         CU(h, cudaMemsetAsync(d_word_row, 0xff, sizeof(int) * (size_t)R, st));
         CU(h, cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), st));
         // 1. every token through the item map; first position per row; tokens without an entry counted
-        RET(launch(h, "i2v_dict_resolve", [&] {
-            k_idmap_first_pos<<<G, 256, 0, st>>>(h->idm_keys[CTR_IDMAP_ITEM], h->idm_vals[CTR_IDMAP_ITEM], h->idm_keys[CTR_IDMAP_ITEM].size() - 1,
-                                                 d_ids, (long)n, d_doc, d_first, d_cnt);
-        }));
+        RET(launch(h, "i2v_dict_resolve", [&] { k_idmap_first_pos<<<G, 256, 0, st>>>(mkeys, mvals, mcap - 1, d_ids, (long)n, d_doc, d_first, d_cnt); }));
         unsigned long long m = 0;
         CU(h, cudaMemcpyAsync(&m, d_cnt, sizeof m, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
-        // 2. the side list: distinct unmapped ids (ascending as uint64) and the first position of each
-        DevBuf<unsigned long long> d_side_id; DevBuf<int> d_side_first, d_word_side;
-        int u = 0;
+        //    each row's first occurrence in the concatenation: this rank's tags, at their minimum over the ranks
+        int rc = CTR_OK;
+        RET(launch(h, across_rows, [&] {
+            i2v_first_tags(d_first, R, cm.rank, d_row_tag, G, st);
+            if (W > 1 && R > 0) rc = comm_min_u64(h, d_row_tag, (size_t)R);
+        }));
+        RET(rc);
+        // 2. this rank's side list: distinct unmapped ids (ascending as uint64) and the first position of each
+        DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
+        int ur = 0;
         if (m > 0) {
-            DevBuf<unsigned long long> k0, k1; DevBuf<int> p0, p1, d_u; DevBuf<unsigned char> tmp;
             CU(h, k0.alloc(m)); CU(h, k1.alloc(m)); CU(h, p0.alloc(m)); CU(h, p1.alloc(m)); CU(h, d_u.alloc(1));
-            size_t b1 = 0, b2 = 0;
-            CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b1, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st));
-            CU(h, cub::DeviceReduce::ReduceByKey(nullptr, b2, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st));
-            CU(h, tmp.alloc(std::max(b1, b2)));
-            RET(launch(h, "i2v_dict_side", [&] { k_i2v_dict_side<<<G, 256, 0, st>>>(d_doc, d_ids, (long)n, k0, p0, d_cnt + 1); }));
-            RET(launch(h, "i2v_dict_side", [&] { size_t tb = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), tb, k0.get(), k1.get(), p0.get(), p1.get(), (int)m, 0, 64, st); }));
-            RET(launch(h, "i2v_dict_side", [&] { size_t tb = tmp.size(); cub::DeviceReduce::ReduceByKey(tmp.get(), tb, k1.get(), k0.get(), p1.get(), p0.get(), d_u.get(), MinPos{}, (int)m, st); }));
-            CU(h, cudaMemcpyAsync(&u, d_u, sizeof u, cudaMemcpyDeviceToHost, st)); CU(h, cudaStreamSynchronize(st));
-            CU(h, d_side_id.alloc((size_t)u)); CU(h, d_side_first.alloc((size_t)u)); CU(h, d_word_side.alloc((size_t)u));
-            CU(h, cudaMemcpyAsync(d_side_id, k0, sizeof(unsigned long long) * (size_t)u, cudaMemcpyDeviceToDevice, st));
-            CU(h, cudaMemcpyAsync(d_side_first, p0, sizeof(int) * (size_t)u, cudaMemcpyDeviceToDevice, st));
+            CU(h, tmp.alloc(i2v_dict_side_tmp_bytes((int)m, st)));
+            cudaError_t e = cudaSuccess;
+            RET(launch(h, "i2v_dict_side", [&] { e = i2v_dict_side_list(d_doc, d_ids, (long)n, (int)m, k0, k1, p0, p1, d_cnt + 1, d_u, tmp, tmp.size(), G, st, &ur); }));
+            CU(h, e);
         }
-        // 3. rows and side words ordered by first position: the rank is the word id
+        //    the side words of the concatenation: the ranks' lists all-gathered (counts, then the lists padded to the longest),
+        //    reduced to the distinct ids ascending with the tag of each one's first occurrence
+        RankLists L{};
+        long stride = ur;
+        const unsigned long long* g_ids = k0; const int* g_pos = p0;
+        DevBuf<unsigned long long> sid, gid; DevBuf<int> spos, gpos;
+        L.cnt[0] = ur; L.off[1] = ur;
+        if (W > 1) {
+            int64_t all[kMaxPeers] = {};
+            const int64_t mine = ur;
+            RET(comm_gather_i64(h, &mine, 1, all));
+            stride = 0;
+            for (int j = 0; j < W; j++) { L.cnt[j] = (int)all[j]; L.off[j + 1] = L.off[j] + all[j]; stride = std::max<long>(stride, (long)all[j]); }
+            if (L.off[W] > 0x7fffffffLL) return set_err(h, CTR_EINVAL, "ctr_item_emb_train: the ranks' side ids (%lld) exceed INT32_MAX", (long long)L.off[W]);
+            if (stride > 0) {
+                CU(h, sid.alloc((size_t)stride)); CU(h, spos.alloc((size_t)stride));
+                CU(h, gid.alloc((size_t)stride * W)); CU(h, gpos.alloc((size_t)stride * W));
+                if (ur > 0) {
+                    CU(h, cudaMemcpyAsync(sid, k0, sizeof(unsigned long long) * (size_t)ur, cudaMemcpyDeviceToDevice, st));
+                    CU(h, cudaMemcpyAsync(spos, p0, sizeof(int) * (size_t)ur, cudaMemcpyDeviceToDevice, st));
+                }
+                RET(launch(h, "i2v_dict_ranks", [&] {
+                    rc = comm_gather_lists(h, spos, gpos, sizeof(int), nullptr, nullptr, (size_t)stride);
+                    if (rc == CTR_OK) rc = comm_gather_lists(h, sid, gid, sizeof(unsigned long long), nullptr, nullptr, (size_t)stride);
+                }));
+                RET(rc);
+            }
+            g_ids = gid; g_pos = gpos;
+        }
+        const int64_t mt = L.off[W];
+        DevBuf<unsigned long long> side_id, side_tag, key1, tag1; DevBuf<int> d_word_side, d_us; DevBuf<unsigned char> mtmp;
+        int u = 0;
+        if (mt > 0) {
+            CU(h, side_id.alloc((size_t)mt)); CU(h, side_tag.alloc((size_t)mt)); CU(h, key1.alloc((size_t)mt)); CU(h, tag1.alloc((size_t)mt)); CU(h, d_us.alloc(1));
+            const size_t tb = idmap_merge_tmp_bytes((int)mt, st);
+            CU(h, mtmp.alloc(std::max<size_t>(tb, 1)));
+            cudaError_t e = cudaSuccess;
+            RET(launch(h, across_side, [&] { e = idmap_merge_min(g_ids, g_pos, stride, L, W, side_id, key1, side_tag, tag1, d_us, mtmp, tb, G, st, &u); }));
+            CU(h, e);
+            CU(h, d_word_side.alloc((size_t)u));
+        }
+        // 3. rows and side words ordered by first occurrence: the rank is the word id
         {
             const long N = R + u;
-            DevBuf<unsigned> rk0, rk1; DevBuf<int> rv0, rv1, d_V; DevBuf<unsigned char> tmp;
+            DevBuf<unsigned long long> rk0, rk1; DevBuf<int> rv0, rv1, d_V; DevBuf<long long> d_row_id; DevBuf<unsigned char> otmp;
             CU(h, rk0.alloc((size_t)N)); CU(h, rk1.alloc((size_t)N)); CU(h, rv0.alloc((size_t)N)); CU(h, rv1.alloc((size_t)N));
-            CU(h, d_vocab.alloc((size_t)N)); CU(h, d_V.alloc(1));
-            size_t tb = 0;
-            CU(h, cub::DeviceRadixSort::SortPairs(nullptr, tb, rk0.get(), rk1.get(), rv0.get(), rv1.get(), (int)N, 0, 32, st));
-            CU(h, tmp.alloc(tb));
-            RET(launch(h, "i2v_dict_rank", [&] { k_i2v_dict_rank_keys<<<G, 256, 0, st>>>(d_first, R, d_side_first, u, rk0, rv0); }));
-            RET(launch(h, "i2v_dict_rank", [&] { size_t b = tmp.size(); cub::DeviceRadixSort::SortPairs(tmp.get(), b, rk0.get(), rk1.get(), rv0.get(), rv1.get(), (int)N, 0, 32, st); }));
-            RET(launch(h, "i2v_dict_rank", [&] { k_i2v_dict_rank<<<G, 256, 0, st>>>(rk1, rv1, N, d_ids, d_word_row, d_word_side, d_vocab, d_V); }));
-            CU(h, cudaMemcpyAsync(&V, d_V, sizeof V, cudaMemcpyDeviceToHost, st));
+            CU(h, d_row_id.alloc((size_t)R)); CU(h, d_vocab.alloc((size_t)N)); CU(h, d_V.alloc(1));
+            const size_t tb = i2v_dict_order_tmp_bytes(N, st);
+            CU(h, otmp.alloc(std::max<size_t>(tb, 1)));
+            cudaError_t e = cudaSuccess;
+            RET(launch(h, "i2v_dict_rank", [&] {
+                e = i2v_dict_order(mkeys, mvals, mcap, d_row_tag, R, side_id, side_tag, u, W, d_row_id, rk0, rk1, rv0, rv1, otmp, tb,
+                                   d_word_row, d_word_side, d_vocab, d_V, G, st, &V);
+            }));
+            CU(h, e);
         }
-        // 4. the int32 word-id document, in place over the resolved rows
-        RET(launch(h, "i2v_dict_doc", [&] { k_i2v_dict_doc<<<G, 256, 0, st>>>(d_doc, d_ids, (long)n, d_word_row, d_side_id, u, d_word_side); }));
+        // 4. this rank's int32 word-id document, in place over its resolved rows
+        RET(launch(h, "i2v_dict_doc", [&] { k_i2v_dict_doc<<<G, 256, 0, st>>>(d_doc, d_ids, (long)n, d_word_row, side_id, u, d_word_side); }));
         CU(h, cudaStreamSynchronize(st));
     }
     if (vocab) *vocab = V;
@@ -3672,20 +3764,43 @@ int ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* 
         CU(h, cudaMemcpyAsync(vocab_ids, d_vocab, sizeof(int64_t) * (size_t)std::min<int64_t>(cap, V), cudaMemcpyDeviceToHost, st));
         CU(h, cudaStreamSynchronize(st));
     }
+    if (vocab_ids && cap < V) {          // the rest stays readable (ctr_item_emb_vocab): a rank cannot size vocab_ids for
+        h->emb_vocab.resize((size_t)V);  // the unmapped ids of the other ranks' streams
+        CU(h, cudaMemcpyAsync(h->emb_vocab.data(), d_vocab, sizeof(int64_t) * (size_t)V, cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+    }
     if (V < 2) return set_err(h, CTR_EINVAL, "item2vec needs at least two distinct words in the stream (%d)", V);
     d_vocab.reset();
     ctr_i2v_stats s{};
-    RET(i2v_train_dev(c, d_doc, n, V, h->num_sms, st, d_syn0, &s, nullptr, h));
+    I2vDist dist;
+    if (W > 1) { dist.rank = cm.rank; dist.world = W; dist.nccl = cm.nccl; dist.sync_every = c.reserved[1] > 0 ? (long)c.reserved[1] : 4L << 20; }
+    RET(i2v_train_dev(c, d_doc, n, V, h->num_sms, st, d_syn0, &s, W > 1 ? &dist : nullptr, h));
     d_doc.reset();
     // ITEM_EMB [R, D]: as ctr_table_upload of the remapped table would leave it
     const int D = c.dim;
-    float* tab = h->tab[CTR_TABLE_ITEM_EMB];
-    if (tab && h->tab_rows[CTR_TABLE_ITEM_EMB] == R && h->tab_width[CTR_TABLE_ITEM_EMB] == D && !h->tab_sharded[CTR_TABLE_ITEM_EMB]) table_new_state(h, CTR_TABLE_ITEM_EMB);
-    else RET(table_alloc(h, CTR_TABLE_ITEM_EMB, R, D));
-    tab = h->tab[CTR_TABLE_ITEM_EMB];
-    RET(launch(h, "i2v_emb_scatter", [&] { k_i2v_emb_scatter<<<G, 256, 0, st>>>(d_syn0, d_word_row, R, D, tab); }));
+    const int T = CTR_TABLE_ITEM_EMB;
+    if (h->tab[T] && h->tab_rows[T] == R && h->tab_width[T] == D) table_new_state(h, T);
+    else RET(table_alloc(h, T, R, D));
+    // A row-sharded table: this rank writes the rows it owns from its own replica (the replicas are equal after the final
+    // averaging).  No peer still reads or writes this shard: the call's first collective (the agreement's all-gather on
+    // the engine stream) completed on this rank only once every rank had reached it in its own stream order, behind every
+    // earlier read or red.add of this shard it queued (a sharded step, a serving call); and tab_gen is bumped, so a peer's
+    // next collective call republishes the mappings and pulls the hot rows only after an exchange with this rank, which
+    // makes it after this write.
+    const bool sh = h->tab_sharded[T];
+    float* tab = h->tab[T];
+    RET(launch(h, "i2v_emb_scatter", [&] { k_i2v_emb_scatter<<<G, 256, 0, st>>>(d_syn0, d_word_row, R, D, sh ? W : 1, sh ? cm.rank : 0, tab); }));
     CU(h, cudaStreamSynchronize(st));
     if (stats) *stats = s;
+    return CTR_OK;
+}
+
+int ctr_item_emb_vocab(ctr_handle* h, int64_t* vocab_ids, int64_t cap, int32_t* vocab) {
+    if (!h || !vocab || cap < 0 || (cap > 0 && !vocab_ids)) return set_err(h, CTR_EINVAL, "bad item embedding vocabulary arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->emb_vocab.empty()) return set_err(h, CTR_ESTATE, "no item embedding vocabulary kept: the last ctr_item_emb_train returned all of it, or none");
+    *vocab = (int32_t)h->emb_vocab.size();
+    if (cap > 0) memcpy(vocab_ids, h->emb_vocab.data(), sizeof(int64_t) * (size_t)std::min<int64_t>(cap, (int64_t)h->emb_vocab.size()));
     return CTR_OK;
 }
 

@@ -126,15 +126,14 @@ inline size_t idmap_merge_tmp_bytes(int m, cudaStream_t st) {
     cub::DeviceRadixSort::SortPairs(nullptr, b3, k, k, k, k, m, 0, 64, st);
     return std::max(b1, std::max(b2, b3));
 }
-// The merge every rank runs on the same gathered lists: the entries sorted by id, the smallest tag of each id kept
-// (ReduceByKey(MinTag)), then sorted by that tag.  key1[0, *u) receives the distinct ids in order of first occurrence in
-// the concatenation, the order a single-GPU insert of it gives new rows in.  Radix sorts and a keyed reduction over the
-// same input: the result is the same on every rank.  Synchronises st (reads *u back).
-inline cudaError_t idmap_merge_ranks(const unsigned long long* g_ids, const int* g_pos, long stride, const RankLists& L, int world,
-                                     unsigned long long* key0, unsigned long long* key1, unsigned long long* tag0, unsigned long long* tag1,
-                                     int* d_u, void* tmp, size_t tmp_bytes, int grid, cudaStream_t st, int* u) {
+// The first half of the merge: the gathered entries compacted and tagged, sorted by id, the smallest tag of each id kept
+// (ReduceByKey(MinTag)).  key0 / tag0 [0, *u) receive the distinct ids ascending as uint64 and the tag of each one's
+// first occurrence in the concatenation (ctr_item_emb_train's side words stop here).  Radix sorts and a keyed reduction
+// over the same input: the result is the same on every rank.  Synchronises st (reads *u back).
+inline cudaError_t idmap_merge_min(const unsigned long long* g_ids, const int* g_pos, long stride, const RankLists& L, int world,
+                                   unsigned long long* key0, unsigned long long* key1, unsigned long long* tag0, unsigned long long* tag1,
+                                   int* d_u, void* tmp, size_t tmp_bytes, int grid, cudaStream_t st, int* u) {
     const int m = (int)L.off[world];
-    int wbits = 0; while ((1 << wbits) < world) wbits++;
     *u = 0;
     if (m == 0) return cudaSuccess;
     k_idmap_merge_ranks<<<grid, 256, 0, st>>>(g_ids, g_pos, stride, L, world, key0, tag0);
@@ -143,7 +142,19 @@ inline cudaError_t idmap_merge_ranks(const unsigned long long* g_ids, const int*
     if (e == cudaSuccess) { b = tmp_bytes; e = cub::DeviceReduce::ReduceByKey(tmp, b, key1, key0, tag1, tag0, d_u, MinTag{}, m, st); }
     if (e == cudaSuccess) e = cudaMemcpyAsync(u, d_u, sizeof(int), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) { b = tmp_bytes; e = cub::DeviceRadixSort::SortPairs(tmp, b, tag0, tag1, key0, key1, *u, 0, 32 + wbits, st); }
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+// The merge every rank runs on the same gathered lists: idmap_merge_min, then the distinct ids sorted by their tags.
+// key1[0, *u) receives the distinct ids in order of first occurrence in the concatenation, the order a single-GPU
+// insert of it gives new rows in.  Synchronises st.
+inline cudaError_t idmap_merge_ranks(const unsigned long long* g_ids, const int* g_pos, long stride, const RankLists& L, int world,
+                                     unsigned long long* key0, unsigned long long* key1, unsigned long long* tag0, unsigned long long* tag1,
+                                     int* d_u, void* tmp, size_t tmp_bytes, int grid, cudaStream_t st, int* u) {
+    int wbits = 0; while ((1 << wbits) < world) wbits++;
+    cudaError_t e = idmap_merge_min(g_ids, g_pos, stride, L, world, key0, key1, tag0, tag1, d_u, tmp, tmp_bytes, grid, st, u);
+    if (e != cudaSuccess || *u == 0) return e;
+    size_t b = tmp_bytes;
+    e = cub::DeviceRadixSort::SortPairs(tmp, b, tag0, tag1, key0, key1, *u, 0, 32 + wbits, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

@@ -25,6 +25,10 @@
 // pass (same thread, same address), except for hot nodes, whose updates wait in shared memory until the next flush.
 #pragma once
 #include "common.cuh"
+#include "idmap.cuh"
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
+#include <algorithm>
 
 namespace ctr {
 
@@ -318,28 +322,42 @@ k_i2v_dict_side(const int* __restrict__ rows, const long long* __restrict__ ids,
         if (side) { const unsigned long long o = base + __popc(b & ((1u << lane) - 1u)); key[o] = (unsigned long long)ids[i0]; pos[o] = (int)i0; }
     }
 }
-// sort input of the vocabulary: rows [0, R) keyed by their first position (0xFFFFFFFF: the row's id never occurs), then
-// the u side words keyed by theirs; val = row, or -(j+1) for side word j.  Positions are distinct, so the order is total.
+// A row's first occurrence across ranks: (rank << 32) | its first position in this rank's stream (first_pos from
+// k_idmap_first_pos), kI2vNever when this rank's stream never holds its id.  Positions stay below 2^31, so the minimum
+// over the ranks is the row's first occurrence in the ranks' streams concatenated in rank order; on one GPU the tag is
+// the position.
+constexpr unsigned long long kI2vNever = ~0ull;
 __global__ void __launch_bounds__(256)
-k_i2v_dict_rank_keys(const unsigned* __restrict__ first_pos, long R, const int* __restrict__ side_first, long u,
-                     unsigned* __restrict__ key, int* __restrict__ val) {
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R + u; i += (long)gridDim.x * blockDim.x) {
-        if (i < R) { key[i] = first_pos[i]; val[i] = (int)i; }
-        else { key[i] = (unsigned)side_first[i - R]; val[i] = -(int)(i - R) - 1; }
+k_i2v_first_tag(const unsigned* __restrict__ first_pos, long R, int rank, unsigned long long* __restrict__ tag) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R; i += (long)gridDim.x * blockDim.x) {
+        const unsigned p = first_pos[i];
+        tag[i] = p == 0xFFFFFFFFu ? kI2vNever : ((unsigned long long)rank << 32) | p;
     }
 }
-// after the sort: entry w < V is word w.  Its item id is the token at its first position; *V = the entries before the
-// first 0xFFFFFFFF key.  Rows whose id never occurs keep word_of_row = -1.
+// sort input of the vocabulary: rows [0, R) keyed by their first-occurrence tag (kI2vNever: the row's id never occurs),
+// then the u side words keyed by theirs; val = row, or -(j+1) for side word j.  Tags are distinct, so the order is total.
 __global__ void __launch_bounds__(256)
-k_i2v_dict_rank(const unsigned* __restrict__ key, const int* __restrict__ val, long N, const long long* __restrict__ ids,
-                int* __restrict__ word_of_row, int* __restrict__ word_of_side, long long* __restrict__ vocab_ids, int* __restrict__ V) {
+k_i2v_dict_rank_keys(const unsigned long long* __restrict__ row_tag, long R, const unsigned long long* __restrict__ side_tag, long u,
+                     unsigned long long* __restrict__ key, int* __restrict__ val) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R + u; i += (long)gridDim.x * blockDim.x) {
+        if (i < R) { key[i] = row_tag[i]; val[i] = (int)i; }
+        else { key[i] = side_tag[i - R]; val[i] = -(int)(i - R) - 1; }
+    }
+}
+// after the sort: entry w < V is word w.  Its item id is the map's id of its row (row_id: the map's row -> id list) or
+// the side list's id (side_id); *V = the entries before the first kI2vNever key.  Rows whose id never occurs keep
+// word_of_row = -1.
+__global__ void __launch_bounds__(256)
+k_i2v_dict_rank(const unsigned long long* __restrict__ key, const int* __restrict__ val, long N, const long long* __restrict__ row_id,
+                const unsigned long long* __restrict__ side_id, int* __restrict__ word_of_row, int* __restrict__ word_of_side,
+                long long* __restrict__ vocab_ids, int* __restrict__ V) {
     for (long w = blockIdx.x * (long)blockDim.x + threadIdx.x; w < N; w += (long)gridDim.x * blockDim.x) {
-        const unsigned k = key[w];
-        if (k == 0xFFFFFFFFu) continue;
+        const unsigned long long k = key[w];
+        if (k == kI2vNever) continue;
         const int v = val[w];
-        if (v >= 0) word_of_row[v] = (int)w; else word_of_side[-v - 1] = (int)w;
-        vocab_ids[w] = ids[k];
-        if (w + 1 == N || key[w + 1] == 0xFFFFFFFFu) *V = (int)(w + 1);
+        if (v >= 0) { word_of_row[v] = (int)w; vocab_ids[w] = row_id[v]; }
+        else { word_of_side[-v - 1] = (int)w; vocab_ids[w] = (long long)side_id[-v - 1]; }
+        if (w + 1 == N || key[w + 1] == kI2vNever) *V = (int)(w + 1);
     }
 }
 // the int32 word-id document, in place over rows[]: a mapped token takes its row's word, a side token the word of its id
@@ -356,14 +374,80 @@ k_i2v_dict_doc(int* __restrict__ doc, const long long* __restrict__ ids, long n,
         doc[i] = word_of_side[lo];
     }
 }
+// ---- the numbering over the ranks' streams (ctr_item_emb_train; one GPU runs the same code at world = 1) -----------
+// Each rank resolves its own stream (k_idmap_first_pos) and tags its rows' first positions (k_i2v_first_tag); the ranks'
+// tags meet in a min all-reduce.  Each rank builds its own side list (i2v_dict_side_list); the ranks all-gather the lists
+// and every rank reduces them to the distinct side ids with their smallest tags (idmap_merge_min, idmap.cuh).  Every rank
+// then orders the same rows and side words the same way (i2v_dict_order) and converts its own stream (k_i2v_dict_doc).
+
+// Scratch of i2v_dict_side_list for m side tokens: k0, k1 [m] (uint64), p0, p1 [m] (int) and tmp (this many bytes)
+inline size_t i2v_dict_side_tmp_bytes(int m, cudaStream_t st) {
+    size_t b1 = 0, b2 = 0;
+    unsigned long long* k = nullptr; int* p = nullptr;
+    cub::DeviceRadixSort::SortPairs(nullptr, b1, k, k, p, p, m, 0, 64, st);
+    cub::DeviceReduce::ReduceByKey(nullptr, b2, k, k, p, p, p, MinPos{}, m, st);
+    return std::max(b1, b2);
+}
+// One rank's side list: rows [n] from k_idmap_first_pos, m of them -1.  k0 / p0 [0, *u) receive the distinct unmapped ids
+// ascending as uint64 and the first position of each in this rank's stream; slot counts a zeroed slot claim.
+// Synchronises st (reads *u back).
+inline cudaError_t i2v_dict_side_list(const int* rows, const long long* ids, long n, int m, unsigned long long* k0, unsigned long long* k1, int* p0, int* p1,
+                                      unsigned long long* slot, int* d_u, void* tmp, size_t tmp_bytes, int grid, cudaStream_t st, int* u) {
+    *u = 0;
+    if (m == 0) return cudaSuccess;
+    k_i2v_dict_side<<<grid, 256, 0, st>>>(rows, ids, n, k0, p0, slot);
+    size_t b = tmp_bytes;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, b, k0, k1, p0, p1, m, 0, 64, st);
+    if (e == cudaSuccess) { b = tmp_bytes; e = cub::DeviceReduce::ReduceByKey(tmp, b, k1, k0, p1, p0, d_u, MinPos{}, m, st); }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(u, d_u, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+inline void i2v_first_tags(const unsigned* first_pos, long R, int rank, unsigned long long* tag, int grid, cudaStream_t st) {
+    k_i2v_first_tag<<<grid, 256, 0, st>>>(first_pos, R, rank, tag);
+}
+// Scratch of i2v_dict_order for N = R + u entries: key0, key1 [N] (uint64), val0, val1 [N] (int), row_id [R] and tmp
+inline size_t i2v_dict_order_tmp_bytes(long N, cudaStream_t st) {
+    size_t b = 0;
+    unsigned long long* k = nullptr; int* v = nullptr;
+    cub::DeviceRadixSort::SortPairs(nullptr, b, k, k, v, v, (int)N, 0, 64, st);
+    return b;
+}
+// The vocabulary, the same on every rank: the R map rows (row_tag, the ranks' minimum) and the u side words (side_id /
+// side_tag, the merge's output) sorted by tag; a word's rank in that order is its id.  The sort reads the low 32 +
+// ceil(log2 world) bits, which hold every tag (positions < 2^31) and order kI2vNever last; on one GPU that is a 32-bit
+// sort of positions.  The item id of a row's word comes from the map (row_id [R]: k_idmap_dump of keys / vals [cap]).
+// word_of_row [R] (-1 before the call), word_of_side [u], vocab_ids [R + u], *V.  Synchronises st (reads *V back).
+inline cudaError_t i2v_dict_order(const unsigned long long* keys, const int* vals, unsigned long long cap, const unsigned long long* row_tag, long R,
+                                  const unsigned long long* side_id, const unsigned long long* side_tag, long u, int world, long long* row_id,
+                                  unsigned long long* key0, unsigned long long* key1, int* val0, int* val1, void* tmp, size_t tmp_bytes,
+                                  int* word_of_row, int* word_of_side, long long* vocab_ids, int* d_V, int grid, cudaStream_t st, int* V) {
+    int wbits = 0; while ((1 << wbits) < world) wbits++;
+    const long N = R + u;
+    *V = 0;
+    cudaError_t e = cudaMemsetAsync(d_V, 0, sizeof(int), st);
+    if (e != cudaSuccess || N == 0) return e;
+    k_idmap_dump<<<grid, 256, 0, st>>>(keys, vals, cap, row_id);
+    k_i2v_dict_rank_keys<<<grid, 256, 0, st>>>(row_tag, R, side_tag, u, key0, val0);
+    size_t b = tmp_bytes;
+    e = cub::DeviceRadixSort::SortPairs(tmp, b, key0, key1, val0, val1, (int)N, 0, 32 + wbits, st);
+    if (e != cudaSuccess) return e;
+    k_i2v_dict_rank<<<grid, 256, 0, st>>>(key1, val1, N, row_id, side_id, word_of_row, word_of_side, vocab_ids, d_V);
+    e = cudaMemcpyAsync(V, d_V, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
 // ITEM_EMB [R, D] (row stride D: D is a power of two >= 4) from the trained syn0 [V, D]: row r takes its word's vector,
-// or zeros when its id never occurs.  One float4 per thread.
+// or zeros when its id never occurs.  One float4 per thread.  world > 1 with a row-sharded table: rank `rank` writes only
+// the rows it owns, global row l·world + rank into its local row l (world = 1: every row).
 __global__ void __launch_bounds__(256)
-k_i2v_emb_scatter(const float* __restrict__ syn0, const int* __restrict__ word_of_row, long R, int D, float* __restrict__ tab) {
+k_i2v_emb_scatter(const float* __restrict__ syn0, const int* __restrict__ word_of_row, long R, int D, int world, int rank, float* __restrict__ tab) {
     const int q = D / 4;
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < R * q; i += (long)gridDim.x * blockDim.x) {
-        const long r = i / q; const int c = (int)(i - r * q);
-        const int w = word_of_row[r];
+    const long local = (R - rank + world - 1) / world;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < local * q; i += (long)gridDim.x * blockDim.x) {
+        const long l = i / q; const int c = (int)(i - l * q);
+        const int w = word_of_row[l * world + rank];
         const float4 v = w >= 0 ? reinterpret_cast<const float4*>(syn0)[(long)w * q + c] : make_float4(0.f, 0.f, 0.f, 0.f);
         reinterpret_cast<float4*>(tab)[i] = v;
     }

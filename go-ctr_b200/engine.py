@@ -33,7 +33,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_item_emb_vocab", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
            "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
@@ -469,19 +469,36 @@ class Engine:
             width = d.shape[1] if d.ndim == 2 else {TABLE_USER_FEAT: self.cfg.uP, TABLE_ITEM_FEAT: self.cfg.cF, TABLE_ITEM_EMB: self.cfg.D}.get(which, 0)
         self._ck(self.L.ctr_table_write_rows(self.h, C.c_int(which), rp, dp, C.c_int64(r.size), C.c_int32(width)))
 
-    def item_emb_train(self, item_ids, cfg=None, **kw):
+    def item_emb_train(self, item_ids, cfg=None, sync_every=None, **kw):
         """recommend.Train's embedding stage into ITEM_EMB (ctr_item_emb_train): item2vec over the int64 item stream,
         words numbered by first appearance on the device, row r of ITEM_EMB = the vector of the item the item map sends
         to r (zeros when it never occurs).  cfg: an item2vec.I2vConfig (default: i2v_default_config(dim=D, **kw)).
-        Returns (vocab_ids [V] int64: the item id of every word in word-id order, I2vStats)."""
-        from .item2vec import I2vStats, i2v_default_config
-        cfg = cfg or i2v_default_config(**{"dim": self.cfg.D, **kw})
-        ids = np.ascontiguousarray(item_ids, np.int64)
+        Returns (vocab_ids [V] int64: the item id of every word in word-id order, I2vStats).
+
+        With world > 1 the call is collective: every rank passes its own shard of the stream (possibly empty) and ends as
+        one GPU would after the same call on the ranks' shards concatenated in rank order, except that the vectors come
+        from local SGD with the replicas averaged every sync_every centre positions (cfg.reserved[1]; None or 0: 4 Mi) and
+        the stats are this rank's.  vocab_ids is the whole vocabulary on every rank: when other ranks' unmapped ids make
+        it longer than this rank could size it, the rest is read back (ctr_item_emb_vocab)."""
+        from .item2vec import I2vConfig, I2vStats, i2v_default_config
+        cfg = I2vConfig.from_buffer_copy(cfg) if cfg is not None else i2v_default_config(**{"dim": self.cfg.D, **kw})
+        if sync_every is not None:
+            if isinstance(sync_every, (bool, np.bool_)) or not isinstance(sync_every, (int, np.integer)) or not 0 <= int(sync_every) < 2 ** 31:
+                raise ValueError("sync_every must be an int in [0, 2^31), got %r" % (sync_every,))
+            cfg.reserved[1] = int(sync_every)
+        ids = np.ascontiguousarray(item_ids, np.int64).reshape(-1)
+        cap = ids.size                          # one GPU: V <= n
+        if self.cfg.world > 1:                  # every item-map row may be a word; only other ranks' unmapped ids can exceed it
+            n = C.c_int64(0)
+            if self.L.ctr_idmap_download(self.h, C.c_int(IDMAP_ITEM), None, C.c_int64(0), C.byref(n)) == 0:
+                cap += n.value
         st = I2vStats(); V = C.c_int32(0)
-        cap = ids.size
         vocab = np.empty(max(cap, 1), np.int64)
-        self._ck(self.L.ctr_item_emb_train(self.h, C.byref(cfg), ids.ctypes.data_as(_lp), C.c_int64(ids.size), vocab.ctypes.data_as(_lp),
-                                           C.c_int64(cap), C.byref(V), C.byref(st)))
+        self._ck(self.L.ctr_item_emb_train(self.h, C.byref(cfg), ids.ctypes.data_as(_lp) if ids.size else None, C.c_int64(ids.size),
+                                           vocab.ctypes.data_as(_lp), C.c_int64(cap), C.byref(V), C.byref(st)))
+        if V.value > cap:
+            vocab = np.empty(V.value, np.int64)
+            self._ck(self.L.ctr_item_emb_vocab(self.h, vocab.ctypes.data_as(_lp), C.c_int64(vocab.size), C.byref(V)))
         return vocab[:V.value].copy(), st
 
     def batch_predict_keys(self, user_ids, item_ids, ts):

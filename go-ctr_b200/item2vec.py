@@ -137,7 +137,10 @@ def TrainItemEmbedding(engine, itemSeq, window=5, iter=1, **kw):
     """GetItemEmbeddingModelFromUb (rcmd.go:538-545) + GenEmbeddingMap32 into engine's ITEM_EMB (ctr_item_emb_train):
     embedding.TrainEmbedding(itemSeq, window, D, iter) with dim = the engine's D.  Row r of ITEM_EMB becomes the vector
     of the item the engine's item map sends to r, zeros for an item the stream never holds.  Returns (vocab_ids, I2vStats):
-    the item id of every word in word-id order (first appearance)."""
+    the item id of every word in word-id order (first appearance).  On a multi-GPU engine (world > 1) every rank's
+    process calls it with its own part of the item sequence, possibly empty: words are numbered over the ranks' parts
+    concatenated in rank order, so vocab_ids is the same on every rank, each rank trains its part with the replicas
+    averaged (sync_every=, Engine.item_emb_train), and each rank writes the ITEM_EMB rows it holds."""
     return engine.item_emb_train(item_ids_from_seq(itemSeq), window=window, iter=iter, **kw)
 
 

@@ -735,19 +735,37 @@ func (e *Engine) TrainKeys(samples []rcmd.Sample, epochs, earlyStop int) (lastCo
 // itemEmbeddingMap lookups, rcmd.go:207-213, 502, 519, 538-545) on the device: itemIds is what ItemSeqGenerator yields,
 // as int64, in corpus order.  Words are numbered by first appearance, embedding.TrainEmbedding(itemSeq, window, D, iter)
 // runs on them, and ITEM_EMB row r becomes the vector of the item LoadIDMaps put at row r (zeros when the item never
-// occurs).  No table crosses PCIe.  Returns the item id of every word in word-id order (SaveVectors, Searcher).
+// occurs).  No table crosses PCIe.  Returns the item id of every word in word-id order (SaveVectors, Searcher).  With
+// world > 1 TrainItemEmbedding is collective: every rank's process calls it with its own shard of the stream (possibly
+// empty), words are numbered by first appearance in the ranks' shards concatenated in rank order (the same ids on every
+// rank), each rank trains its shard with the replicas averaged, and each rank writes the ITEM_EMB rows it holds; item
+// maps or arguments that differ across the ranks, or a stream empty on every rank, fail on every rank.  The returned
+// vocabulary is whole and the same on every rank.
 func (e *Engine) TrainItemEmbedding(itemIds []int64, window, iter int) ([]int64, error) {
-	if len(itemIds) == 0 {
+	if len(itemIds) == 0 && e.cfg.world <= 1 {
 		return nil, fmt.Errorf("TrainItemEmbedding: empty item stream")
 	}
 	var cfg C.ctr_i2v_config
 	C.ctr_i2v_config_default(&cfg)
 	cfg.dim, cfg.window, cfg.iter = e.cfg.D, C.int32_t(window), C.int32_t(iter)
-	vocab := make([]int64, len(itemIds))
+	capacity := len(itemIds)
+	if e.cfg.world > 1 { // room for every item-map row as well; only other ranks' unmapped ids can exceed it
+		var rows C.int64_t
+		if err := e.err(C.ctr_idmap_download(e.h, C.CTR_IDMAP_ITEM, nil, 0, &rows)); err == nil {
+			capacity += int(rows)
+		}
+	}
+	vocab := make([]int64, capacity+1)
 	var v C.int32_t
-	rc := C.ctr_item_emb_train(e.h, &cfg, i64(itemIds), C.int64_t(len(itemIds)), i64(vocab), C.int64_t(len(vocab)), &v, nil)
+	rc := C.ctr_item_emb_train(e.h, &cfg, i64n(itemIds), C.int64_t(len(itemIds)), i64(vocab), C.int64_t(len(vocab)), &v, nil)
 	if err := e.err(rc); err != nil {
 		return nil, err
+	}
+	if int(v) > len(vocab) { // other ranks' unmapped ids: the handle kept the whole vocabulary
+		vocab = make([]int64, int(v))
+		if err := e.err(C.ctr_item_emb_vocab(e.h, i64(vocab), C.int64_t(len(vocab)), &v)); err != nil {
+			return nil, err
+		}
 	}
 	return vocab[:int(v)], nil
 }

@@ -636,18 +636,56 @@ int  ctr_i2v_train_dist(const ctr_i2v_config* cfg, const int32_t* tokens_shard, 
  * The rows are written only after training has succeeded: a refusal, or any error before that write, leaves ITEM_EMB
  * and its solver state as they were.
  * *vocab = V is written when vocab is non-NULL (also when V < 2 is refused); vocab_ids (may be NULL) receives the first
- * min(cap, V) words' item ids in word-id order (SaveVectors, the word ↔ row bookkeeping of a Searcher).  stats as
- * ctr_i2v_train fills it.
+ * min(cap, V) words' item ids in word-id order (SaveVectors, the word ↔ row bookkeeping of a Searcher).  When vocab_ids
+ * is non-NULL and cap < V, the handle keeps all V ids on the host until its next ctr_item_emb_train, and
+ * ctr_item_emb_vocab reads them.  stats as ctr_i2v_train fills it.
  * CTR_EINVAL: null or short arguments, cfg->dim != D, a configuration ctr_i2v_train refuses, n out of range, fewer than
- * two distinct words.  CTR_ESTATE: no item id map, or world > 1 (the ranks would need a global first-appearance order).
+ * two distinct words.  CTR_ESTATE: no item id map.
+ * world > 1: the call is collective.  Every rank passes its own shard of the item stream (n = 0 allowed, item_ids may
+ * then be NULL; each rank's n below 2^31, the concatenation may be longer) and afterwards holds what one GPU holds after
+ * the same call on the ranks' shards concatenated in rank order, except for two things: the trained vectors come from
+ * ctr_i2v_train_dist's local SGD with model averaging (the replicas averaged every cfg->reserved[1] centre positions;
+ * 0 selects 4 Mi), and stats is this rank's.  In detail:
+ *   - vocabulary: word ids by first appearance in the concatenation; *vocab and vocab_ids are identical on every rank and
+ *     equal, bit for bit, what one GPU returns for the concatenated stream (mapped items, unmapped ids, INT64_MIN, an id
+ *     first seen on a later rank, a run of one id across a shard boundary alike);
+ *   - training: MinCount, subsampling, the Huffman tree and the lr schedule use the global counts and token count; it
+ *     runs on the handle's communicator and engine stream.  Words below min_count are never trained, but their rows
+ *     pass through every replica average (an all-reduced sum, then a scale by 1/world): at world = 2 that gives the
+ *     one-GPU initial vector bit for bit, at world > 2 the sum of the equal copies can round, by about one ulp per
+ *     average;
+ *   - table: ITEM_EMB ends as [idmap_n(CTR_IDMAP_ITEM), D] under the one-GPU rules (in place when it has that shape,
+ *     otherwise allocated as ctr_table_upload allocates it, with the configuration's placement; moments and hot-row
+ *     accumulators reset, and the next collective call republishes the shards and rebuilds the hot-row replica from
+ *     the new rows).  A replicated table: every rank writes every row.  A row-sharded table: each rank writes only the
+ *     rows it owns from its own replica (global row l·world + rank into local row l); the replicas are equal after the
+ *     last average, so no rows travel;
+ *   - agreement: the call starts with every rank's verdict, a hash of the configuration (cfg->device aside), ITEM_EMB's
+ *     presence, shape and placement, the item map's size and digest and the ranks' token counts in one all-gather.
+ *     Every rank returns the same code, and no refusal changes a map or a table: CTR_ESTATE when a rank has no item map;
+ *     CTR_EINVAL when configurations, item maps or ITEM_EMB's shape or placement differ between ranks, for
+ *     reserved[0] == 1 (the sequential mode is single-GPU), fewer than two distinct words in the concatenation, or
+ *     every rank empty.  A CUDA or NCCL failure after the agreement (out of memory on one rank, say) can leave the
+ *     ranks apart, as with the other collective calls;
+ *   - vocab_ids: a rank cannot know how many unmapped ids the other ranks' streams bring, so cap may fall short of V;
+ *     the whole vocabulary is then read back with ctr_item_emb_vocab (local, the same on every rank).
+ *   Memory beside the one-GPU figures: the 8·R-byte first-occurrence tags (all-reduced); the ranks' side lists gathered
+ *   (12 bytes per entry, world × the longest list); the merge's four 8-byte buffers per gathered entry (mt = the ranks'
+ *   distinct unmapped ids summed, in place of u in the one-GPU figure's 32·u); and the trainer's two full replicas
+ *   (8·V·D bytes) on every rank.
+ * With world = 1 the call is single-GPU, n >= 1.
  * cfg->device is ignored: the handle's device is used.  Runs on the engine stream under the handle's mutex: ordered after
  * everything queued before it, and everything queued after it sees the new table.  The int64 stream is staged from
  * pageable memory through pinned bounce buffers.  Peak device memory beside the handle's own buffers, with R item-map
- * rows, m tokens without an item-map entry and u distinct such ids: at most 12·n + 24·m + 40·(R + u) bytes (+ sort
+ * rows, m tokens without an item-map entry and u distinct such ids: at most 12·n + 24·m + 72·(R + u) bytes (+ sort
  * scratch) while numbering — the whole stream is never sorted, only its m unmapped tokens — then 9·n + 4·R bytes plus
  * ctr_i2v_train's vocabulary tables while training, and 4·V·D + 4·R bytes next to ITEM_EMB for the final write. */
 int  ctr_item_emb_train(ctr_handle* h, const ctr_i2v_config* cfg, const int64_t* item_ids, int64_t n,
                         int64_t* vocab_ids, int64_t cap, int32_t* vocab, ctr_i2v_stats* stats);
+/* The vocabulary the last ctr_item_emb_train kept because its vocab_ids could not take all of it (cap < V): *vocab = V,
+ * and vocab_ids receives the first min(cap, V) item ids in word-id order.  Host memory only, not collective.
+ * CTR_ESTATE when nothing is kept (that call returned every id, or failed before numbering, or none was made). */
+int  ctr_item_emb_vocab(ctr_handle* h, int64_t* vocab_ids, int64_t cap, int32_t* vocab);
 
 /* ---- model/mlp: the float64 MLP classifier of the reference's default path (BASELINE configs[0]; SURVEY.md §8a row
  * a11) — main.go:42-52 → model/mlp/mlp.go:45-65 (SimpleMlpFitWrap.Fit / SimpleMlpPredWrap.Predict: float32 samples →
