@@ -4815,12 +4815,12 @@ int mlp_keys_check(ctr_mlp* m, ctr_handle* h) {
     RET(comm_check_emb(h));
     return check_widths(h);
 }
-// the entry of a collective key-fed call (comm_serve_enter, on a row-sharded ITEM_EMB): a rank whose checks failed takes
-// part with its message, and every rank returns the same verdict
+// the entry of a collective key-fed call (comm_serve_enter on a row-sharded ITEM_EMB, else the agreement alone): a rank
+// whose checks failed takes part with its message, and every rank returns the same verdict
 int mlp_agree(ctr_mlp* m, ctr_handle* h, CommHdr hd, int verdict) {
     if (verdict != CTR_OK && h->err.empty()) h->err = m->err;
     CU(h, cudaSetDevice(h->dev));        // the checks may have stopped before making it current
-    const int rc = comm_serve_enter(h, hd, verdict);
+    const int rc = emb_sharded(h) ? comm_serve_enter(h, hd, verdict) : comm_agree(h, hd, verdict);
     if (rc != CTR_OK) m->err = h->err;
     return rc;
 }
@@ -4849,37 +4849,39 @@ int mlp_keys_width(ctr_mlp* m) {
     return CTR_OK;
 }
 
-int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label, int64_t n,
-                 int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
-    RET(mlp_keys_width(m));
-    const int S = h->cfg.S;
-    // ---- GetSample's resolution, as in ctr_train_keys: survivors resident in kt_*, input order kept
+// GetSample's resolution of n >= 1 keys, as in ctr_train_keys: the survivors resident in kt_* (input order kept) and,
+// when there are any, each one's history GetUserBehavior(uid, S, -1, ts) in kt_hist_all, cut once (h->mu is held, so
+// the cache stays as it is).  *used = the survivor count.
+int mlp_keys_resolve(ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label, int64_t n,
+                     long* used) {
     RET(feed_init(h));
     const size_t chunk = std::min<size_t>((size_t)n, h->feed_bytes / 28);
     RET(keys_prepare(h, (size_t)n, chunk));
     cudaStream_t rs = h->copy_stream;
     const int64_t nchunks = (n + (int64_t)chunk - 1) / (int64_t)chunk;
     for (int64_t c = 0; c < nchunks; c++) RET(keys_resolve_chunk(h, c, chunk, user_ids, item_ids, ts, label, n, rs));
-    unsigned long long used = 0;
-    CU(h, cudaMemcpyAsync(&used, h->kt_count, sizeof used, cudaMemcpyDeviceToHost, rs));
+    unsigned long long cnt = 0;
+    CU(h, cudaMemcpyAsync(&cnt, h->kt_count, sizeof cnt, cudaMemcpyDeviceToHost, rs));
     CU(h, cudaStreamSynchronize(rs));
-    if (rows_used) *rows_used = (int64_t)used;
-    if (used == 0) return mlp_err(m, CTR_ENOTFOUND, "no sample resolved: every key has an unknown user or item");
-    const long ns = (long)used;
-    // ---- every survivor's history, GetUserBehavior(uid, S, -1, ts), cut once: h->mu is held, so the cache stays as it is
-    RET(reserve(h, h->kt_hist_all, (size_t)ns * S, false));
-    RET(ub_windows(h, h->stream, h->kt_user, h->kt_ts, (int)ns, h->kt_hist_all));
-    // ---- the classifier: minibatch k's rows are gathered on h's stream into stage[k & 1] while minibatch k-1 trains
+    *used = (long)cnt;
+    if (cnt == 0) return CTR_OK;
+    RET(reserve(h, h->kt_hist_all, (size_t)cnt * h->cfg.S, false));
+    return ub_windows(h, h->stream, h->kt_user, h->kt_ts, (int)cnt, h->kt_hist_all);
+}
+
+// The classifier over ns resolved samples (user / item rows [ns], history rows [ns, S], labels [ns], on h's device, queued
+// on h's stream): minibatch k's rows are gathered on h's stream into stage[k & 1] while minibatch k-1 trains.  peer: a
+// row-sharded ITEM_EMB, read through r = comm_src (the mappings published); else r reads this GPU's tables.
+int mlp_keys_train(ctr_mlp* m, ctr_handle* h, const RowSrc& r, bool peer, const float* label, long ns, int32_t* n_iter, double* loss_curve) {
     const long bs = mlp_batch(m, ns);
     if (m->idx.size() < (size_t)ns) MCU(m, m->idx.alloc((size_t)ns));
     RET(mlp_stage(m, bs));
     RET(mlp_after_store(m, h, 0));                                     // labels and windows before the first loss
     const int* cls = nullptr;
-    if (m->regressor) RET(mlp_targets(m, h->kt_label, ns));             // the survivors' labels are their targets
-    else RET(mlp_labels(m, h->kt_label, ns, &cls));                     // the survivors' labels
+    if (m->regressor) RET(mlp_targets(m, label, ns));                   // the survivors' labels are their targets
+    else RET(mlp_labels(m, label, ns, &cls));                           // the survivors' labels
     RET(mlp_rows(m, bs));
     RET(mlp_init_params(m));
-    const RowSrc r = idx_src(h, h->kt_user, h->kt_item, h->kt_hist_all, (int)ns);
     const int nin = m->d.units[0];
     auto input = [&](long k, const long* bi, int rows, const double** X) -> int {
         const int s = (int)(k & 1);
@@ -4888,14 +4890,108 @@ int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64
         if (k == 0) MCU(m, cudaEventRecord(m->stage_free[0], m->stream));
         MCU(m, cudaEventRecord(m->stage_free[(k + 1) & 1], m->stream));
         MCU(m, cudaStreamWaitEvent(h->stream, m->stage_free[s], 0));
-        RET(launch(h, "mlp_gather", [&] {
-            k_gather_rows<<<grid_for_warps(h, rows), 256, 0, h->stream>>>(r, dims_of(h), m->stage[s].get(), (long)nin, rows, RowsByIdx{bi});
+        // the PEER form reads the hot rows from this rank's replica and the rest from their owners: the same float32
+        // rows, so the same float64 ones, as the local gather over the whole table
+        RET(launch(h, peer ? "mlp_fit_gather_peer" : "mlp_gather", [&] {
+            if (peer) k_gather_rows<double, RowsByIdx, true><<<grid_for_warps(h, rows), 256, 0, h->stream>>>(r, dims_of(h), m->stage[s].get(), (long)nin, rows, RowsByIdx{bi});
+            else k_gather_rows<<<grid_for_warps(h, rows), 256, 0, h->stream>>>(r, dims_of(h), m->stage[s].get(), (long)nin, rows, RowsByIdx{bi});
         }));
         RET(mlp_after_store(m, h, s));
         *X = m->stage[s];
         return CTR_OK;
     };
-    return mlp_epochs(m, ns, bs, h->kt_label, cls, input, n_iter, loss_curve);
+    return mlp_epochs(m, ns, bs, label, cls, input, n_iter, loss_curve);
+}
+
+int mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label, int64_t n,
+                 int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    RET(mlp_keys_width(m));
+    long ns = 0;
+    RET(mlp_keys_resolve(h, user_ids, item_ids, ts, label, n, &ns));
+    if (rows_used) *rows_used = (int64_t)ns;
+    if (ns == 0) return mlp_err(m, CTR_ENOTFOUND, "no sample resolved: every key has an unknown user or item");
+    const RowSrc r = idx_src(h, h->kt_user, h->kt_item, h->kt_hist_all, (int)ns);
+    return mlp_keys_train(m, h, r, false, h->kt_label, ns, n_iter, loss_curve);
+}
+
+// A 64-bit digest of what must be equal on every rank before ctr_mlp_fit_keys_dist trains: the configuration (its device
+// aside; the unused units slots zeroed) and the options, the model kind and, on a warm start, whether the model is fitted
+// and, if so, its output kind, classes, t and packed parameters.  m's device is current.
+int mlp_fit_digest(ctr_mlp* m, uint64_t* out) {
+    ctr_mlp_config c = m->cfg;
+    c.device = 0;
+    for (int i = c.n_layers; i < 8; i++) c.units[i] = 0;
+    uint64_t d = comm_hash(&c, sizeof c);
+    d = comm_hash(&m->opts, sizeof m->opts, d);
+    const int64_t kind[3] = {m->regressor ? 1 : 0, c.warm_start ? 1 : 0, c.warm_start && m->fitted ? 1 : 0};
+    d = comm_hash(kind, sizeof kind, d);
+    if (c.warm_start && m->fitted) {
+        std::vector<double> p((size_t)m->np);
+        MCU(m, cudaMemcpyAsync(p.data(), m->params, sizeof(double) * (size_t)m->np, cudaMemcpyDeviceToHost, m->stream));
+        MCU(m, cudaStreamSynchronize(m->stream));
+        const int64_t out_kind = m->out_kind;
+        d = comm_hash(&out_kind, sizeof out_kind, d);
+        d = comm_hash(&m->t, sizeof m->t, d);
+        d = comm_hash(m->classes.data(), sizeof(double) * m->classes.size(), d);
+        d = comm_hash(p.data(), sizeof(double) * p.size(), d);
+    }
+    *out = d;
+    return CTR_OK;
+}
+
+// ctr_mlp_fit_keys_dist on world > 1 (see the header): every rank resolves and windows its own keys, the ranks agree on
+// their verdicts, the model and the placement, all-gather the survivor counts and then the survivor records in rank
+// order, and every rank runs the single-GPU fit over the same records.  args: CTR_OK or this rank's argument refusal.
+int mlp_fit_keys_ranks(ctr_mlp* m, ctr_handle* h, int args, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label,
+                       int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    const int W = h->comm.world, me = h->comm.rank, S = h->cfg.S;
+    // the counts' exchange holds kMaxPeers ranks; world is the same everywhere, so every rank refuses alike
+    if (W > kMaxPeers) return mlp_err(m, CTR_EINVAL, "fit_keys_dist: world %d, at most %d", W, kMaxPeers);
+    const bool sh = emb_sharded(h);
+    CommHdr hd{};
+    hd.flag = (h->tab_sharded[CTR_TABLE_ITEM_EMB] ? 1 : 0) | (h->tab_sharded[CTR_TABLE_ITEM_FEAT] ? 2 : 0);
+    // the digest whatever this rank's verdict, so that a refusal reaches the other ranks as itself
+    const cudaError_t de = cudaSetDevice(m->dev);
+    const int dg = de != cudaSuccess ? mlp_err(m, CTR_ECUDA, "cudaSetDevice(%d): %s", m->dev, cudaGetErrorString(de)) : mlp_fit_digest(m, &hd.hash[0]);
+    long ns = 0;
+    const int verdict = args != CTR_OK ? args : dg != CTR_OK ? dg : [&]() -> int {
+        RET(mlp_keys_check(m, h));
+        RET(mlp_keys_width(m));
+        CU(h, cudaSetDevice(h->dev));
+        return n > 0 ? mlp_keys_resolve(h, user_ids, item_ids, ts, label, n, &ns) : CTR_OK;
+    }();
+    RET(mlp_agree(m, h, hd, verdict));
+    // ---- the counts (keys and survivors of every rank), then the records, concatenated in rank order on every rank
+    int64_t all[2 * kMaxPeers] = {};
+    const int64_t mine[2] = {n, ns};
+    RET(comm_gather_i64(h, mine, 2, all));
+    int64_t keys = 0, cnt[kMaxPeers], off[kMaxPeers + 1] = {0};
+    for (int j = 0; j < W; j++) { keys += all[2 * j]; cnt[j] = all[2 * j + 1]; off[j + 1] = off[j] + cnt[j]; }
+    // one GPU refuses a concatenation of more than INT32_MAX keys: so do the ranks, all of them, before any write
+    if (keys > INT32_MAX) return mlp_err(m, CTR_EINVAL, "fit_keys_dist: the ranks pass %lld keys in all (more than INT32_MAX)", (long long)keys);
+    const int64_t T = off[W];
+    if (rows_used) *rows_used = T;
+    if (T == 0) return mlp_err(m, CTR_ENOTFOUND, "no sample resolved on any rank: every key has an unknown user or item");
+    DevBuf<int> g_user, g_item, g_hist; DevBuf<float> g_label;
+    CU(h, g_user.alloc((size_t)T)); CU(h, g_item.alloc((size_t)T)); CU(h, g_label.alloc((size_t)T));
+    CU(h, g_hist.alloc((size_t)std::max<int64_t>(T * S, 1)));
+    cudaStream_t st = h->stream;
+    if (ns > 0) {                                                    // this rank's segment in place (the windows are on st)
+        CU(h, cudaMemcpyAsync(g_user.get() + off[me], h->kt_user, sizeof(int) * (size_t)ns, cudaMemcpyDeviceToDevice, st));
+        CU(h, cudaMemcpyAsync(g_item.get() + off[me], h->kt_item, sizeof(int) * (size_t)ns, cudaMemcpyDeviceToDevice, st));
+        CU(h, cudaMemcpyAsync(g_label.get() + off[me], h->kt_label, sizeof(float) * (size_t)ns, cudaMemcpyDeviceToDevice, st));
+        if (S > 0) CU(h, cudaMemcpyAsync(g_hist.get() + off[me] * S, h->kt_hist_all, sizeof(int) * (size_t)ns * S, cudaMemcpyDeviceToDevice, st));
+    }
+    int rc = CTR_OK;
+    RET(launch(h, "mlp_fit_gather_ranks", [&] {
+        if (rc == CTR_OK) rc = comm_concat(h, g_user, sizeof(int), cnt, off);
+        if (rc == CTR_OK) rc = comm_concat(h, g_item, sizeof(int), cnt, off);
+        if (rc == CTR_OK) rc = comm_concat(h, g_label, sizeof(float), cnt, off);
+        if (rc == CTR_OK && S > 0) rc = comm_concat(h, g_hist, sizeof(int) * (size_t)S, cnt, off);
+    }));
+    RET(rc);
+    const RowSrc r = sh ? comm_src(h, g_user, g_item, g_hist, (int)T, false) : idx_src(h, g_user, g_item, g_hist, (int)T);
+    return mlp_keys_train(m, h, r, sh, g_label, (long)T, n_iter, loss_curve);
 }
 
 int mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {
@@ -5204,6 +5300,22 @@ int ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const i
                                : mlp_keys_check(m, h);
     if (rc == CTR_OK) rc = mlp_fit_keys(m, h, user_ids, item_ids, ts, label, n, n_iter, loss_curve, rows_used);
     return mlp_keys_done(m, h, rc);
+}
+
+// The arguments are checked before either object is touched; on world > 1 a rank whose arguments are bad still takes
+// part in the agreement with its refusal, so that no rank is left waiting.
+int ctr_mlp_fit_keys_dist(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, const float* label,
+                          int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used) {
+    const bool args_ok = n >= 0 && n <= INT32_MAX && (n == 0 || (user_ids && item_ids && ts && label));
+    if (!m || !h)
+        return mlp_err(m, CTR_EINVAL, args_ok ? "fit_keys_dist: null model or feature store"
+                                              : "bad fit_keys_dist arguments (n in [0, 2^31), the arrays non-null when n > 0)");
+    if (h->comm.world == 1) return ctr_mlp_fit_keys(m, h, user_ids, item_ids, ts, label, n, n_iter, loss_curve, rows_used);
+    std::lock_guard<std::mutex> lh(h->mu);                           // the feature store first, then the classifier
+    std::lock_guard<std::mutex> lm(m->mu);
+    m->err.clear(); h->err.clear();
+    const int args = args_ok ? CTR_OK : mlp_err(m, CTR_EINVAL, "bad fit_keys_dist arguments (n in [0, 2^31), the arrays non-null when n > 0)");
+    return mlp_keys_done(m, h, mlp_fit_keys_ranks(m, h, args, user_ids, item_ids, ts, label, n, n_iter, loss_curve, rows_used));
 }
 
 int ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts, int64_t n, float* scores) {

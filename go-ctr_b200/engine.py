@@ -35,7 +35,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
            "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_item_emb_vocab", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
-           "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_predict_keys",
+           "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_fit_keys_dist", "ctr_mlp_predict_keys",
            "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
            "ctr_mlp_score", "ctr_mlp_accuracy", "ctr_mlp_get_output", "ctr_mlp_set_output"]
 
@@ -845,6 +845,24 @@ class _Mlp64:
         it = C.c_int32(0); used = C.c_int64(0); curve = np.zeros(self.cfg.max_iter, np.float64)
         self._ck(self.L.ctr_mlp_fit_keys(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp), yp,
                                          C.c_int64(u.size), C.byref(it), curve.ctypes.data_as(C.POINTER(C.c_double)), C.byref(used)))
+        self.n_iter = it.value; self.loss_curve = curve[:it.value]; self.rows_used = used.value
+        return self
+
+    def fit_keys_dist(self, engine, user_ids, item_ids, ts, label):
+        """fit_keys on a multi-GPU feature store (ctr_mlp_fit_keys_dist), a row-sharded ITEM_EMB included.  Collective
+        when engine's world > 1: every rank calls it with its own keys (possibly none) and ends with the model, n_iter,
+        loss_curve and rows_used (the survivors of all ranks) that fit_keys on one GPU would give over all ranks' keys
+        concatenated in rank order, bit for bit.  Each key is windowed by the ubcache of the rank that passed it.  A
+        configuration, options or warm-start model that differs across ranks raises CtrError (EINVAL) everywhere; any
+        other refusal raises the lowest failing rank's error on every rank.  No sync() is needed after training.  On
+        world == 1 this is fit_keys."""
+        u, i, t = self._keys(user_ids, item_ids, ts)
+        y, yp = _f(label)
+        if y.size != u.size:
+            raise ValueError("label has %d entries for %d keys" % (y.size, u.size))
+        it = C.c_int32(0); used = C.c_int64(0); curve = np.zeros(self.cfg.max_iter, np.float64)
+        self._ck(self.L.ctr_mlp_fit_keys_dist(self.h, engine.h, u.ctypes.data_as(_lp), i.ctypes.data_as(_lp), t.ctypes.data_as(_lp), yp,
+                                              C.c_int64(u.size), C.byref(it), curve.ctypes.data_as(C.POINTER(C.c_double)), C.byref(used)))
         self.n_iter = it.value; self.loss_curve = curve[:it.value]; self.rows_used = used.value
         return self
 

@@ -992,19 +992,34 @@ func (f *MlpRegressorFitWrap) Fit(trainSample *rcmd.TrainSample) (rcmd.PredictAb
 // feature store (id maps, tables, optional ubcache), samples are its keys.  Samples whose user or item is unknown are
 // dropped; rowsUsed counts the rest.  The classifier has e's uP + S·D + D + cF inputs and trains bit for bit as Fit
 // would on the rows GetSample builds.  The options and refusals are Fit's.  The predictor serves keys through e.
-// FitKeys needs a single-GPU feature store: on a multi-GPU one, fit on one GPU and install the parameters on every rank.
+// FitKeys needs a single-GPU feature store: on a multi-GPU one use FitKeysDist.
 func (f *MlpFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
-	return f.fitKeys(e, samples, false)
+	return f.fitKeys(e, samples, false, false)
 }
 
 // FitKeys is MlpFitWrap.FitKeys with the regressor: each sample's Label is its target.
 func (f *MlpRegressorFitWrap) FitKeys(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
-	return f.fitKeys(e, samples, true)
+	return f.fitKeys(e, samples, true, false)
 }
 
-func (f *MlpFitWrap) fitKeys(e *Engine, samples []rcmd.Sample, regressor bool) (*MlpPredWrap, int64, error) {
+// FitKeysDist is FitKeys on a multi-GPU feature store, a row-sharded ITEM_EMB included (ctr_mlp_fit_keys_dist).  With
+// world > 1 it is collective: every rank calls it with its own samples (possibly none) and the same fitter options, and
+// every rank's predictor ends as FitKeys on one GPU over all ranks' samples concatenated in rank order, bit for bit;
+// rowsUsed counts the survivors of all ranks.  Each sample is windowed by the ubcache of the rank that passed it.  Options
+// that differ across ranks are CTR_EINVAL everywhere; any other refusal is the lowest failing rank's on every rank.  On a
+// single-GPU store it is FitKeys.
+func (f *MlpFitWrap) FitKeysDist(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
+	return f.fitKeys(e, samples, false, true)
+}
+
+// FitKeysDist is MlpFitWrap.FitKeysDist with the regressor: each sample's Label is its target.
+func (f *MlpRegressorFitWrap) FitKeysDist(e *Engine, samples []rcmd.Sample) (*MlpPredWrap, int64, error) {
+	return f.fitKeys(e, samples, true, true)
+}
+
+func (f *MlpFitWrap) fitKeys(e *Engine, samples []rcmd.Sample, regressor, dist bool) (*MlpPredWrap, int64, error) {
 	n := len(samples)
-	if n == 0 {
+	if n == 0 && !(dist && e.cfg.world > 1) {
 		return nil, 0, fmt.Errorf("MlpFitWrap.FitKeys: no samples")
 	}
 	xcols := int(e.cfg.uP + e.cfg.S*e.cfg.D + e.cfg.D + e.cfg.cF)
@@ -1018,8 +1033,20 @@ func (f *MlpFitWrap) fitKeys(e *Engine, samples []rcmd.Sample, regressor bool) (
 	}
 	var iters C.int32_t
 	var used C.int64_t
-	if rc := C.ctr_mlp_fit_keys(m, e.h, i64(u), i64(it), i64(ts), f32(y), C.int64_t(n), &iters, nil, &used); rc != C.CTR_OK {
-		err := fmt.Errorf("ctr_mlp_fit_keys: %d: %s", int(rc), C.GoString(C.ctr_mlp_last_error(m)))
+	var rc C.int
+	name := "ctr_mlp_fit_keys"
+	if dist {
+		name = "ctr_mlp_fit_keys_dist"
+		var yp *C.float // a rank without samples passes null arrays
+		if n > 0 {
+			yp = f32(y)
+		}
+		rc = C.ctr_mlp_fit_keys_dist(m, e.h, i64n(u), i64n(it), i64n(ts), yp, C.int64_t(n), &iters, nil, &used)
+	} else {
+		rc = C.ctr_mlp_fit_keys(m, e.h, i64(u), i64(it), i64(ts), f32(y), C.int64_t(n), &iters, nil, &used)
+	}
+	if rc != C.CTR_OK {
+		err := fmt.Errorf("%s: %d: %s", name, int(rc), C.GoString(C.ctr_mlp_last_error(m)))
 		C.ctr_mlp_destroy(m)
 		return nil, int64(used), err
 	}

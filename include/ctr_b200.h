@@ -805,7 +805,8 @@ int  ctr_mlp_set_output(ctr_mlp* m, int32_t kind);
  * CTR_ESTATE for a missing id map, missing tables, and predict before any fit or ctr_mlp_set_params.  The message is
  * readable through both ctr_mlp_last_error(m) and ctr_last_error(h).
  * Multi-GPU feature stores (world > 1): fit_keys is CTR_ESTATE — data-parallel float64 training would not keep fit's
- *   bit-for-bit result; fit on one GPU and serve the parameters on every rank through ctr_mlp_set_params.  predict with
+ *   bit-for-bit result; fit on one GPU and serve the parameters on every rank through ctr_mlp_set_params, or train on
+ *   every rank at once with ctr_mlp_fit_keys_dist (below), which replicates the fit instead.  predict with
  *   ITEM_EMB and ITEM_FEAT both replicated serves from this GPU's tables alone; with a row-sharded ITEM_EMB (ITEM_FEAT
  *   sharded or replicated) each rank scores its own keys and reads the rows from their owners, the hot rows from its
  *   replica, under ctr_batch_predict_keys' rule: the first call after a table change publishes the shard mappings and
@@ -817,6 +818,41 @@ int  ctr_mlp_fit_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const 
                       const float* label, int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used);
 int  ctr_mlp_predict_keys(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
                           int64_t n, float* scores);
+/* ctr_mlp_fit_keys on a multi-GPU feature store, including a row-sharded ITEM_EMB that no GPU holds whole.  On world == 1
+ * the call is ctr_mlp_fit_keys.  With world > 1 it is collective: every rank calls it with its OWN keys (n = 0 is allowed
+ * there, with the arrays then possibly NULL).  The rule: afterwards every rank's m holds what ctr_mlp_fit_keys on one GPU
+ * would hold after fitting on all ranks' keys concatenated in rank order, against a store holding the whole table:
+ * parameters, classes / output kind, t, *n_iter, loss_curve and *rows_used (the survivors of all ranks), bit for bit.
+ *   Training is replicated, not data-parallel: a step of this model is launch-bound, and what a row-sharded store
+ *   prevents is reading the rows, not computing the step.  Each rank resolves and windows its own keys on the device
+ *   with its own id maps and ubcache, exactly as fit_keys does: each key is windowed by the ubcache of the rank that
+ *   passed it, so parity with one GPU assumes the ranks' ubcaches agree, as they do when they are kept live through the
+ *   collective calls.  The survivor records (user row, item row, S history rows, label) are then all-gathered in rank
+ *   order, counts first, and every rank runs the single-GPU fit over the same records in the same shuffled order with
+ *   the same kernels.  Only layer 0's row gather differs: on a row-sharded ITEM_EMB it reads the hot rows from the rank's
+ *   replica and the rest from their owners (ITEM_FEAT sharded or replicated), the same float32 rows, so the same float64
+ *   ones (profile key mlp_fit_gather_peer; the record all-gather is mlp_fit_gather_ranks).  Nothing is all-reduced.  With
+ *   ITEM_EMB and ITEM_FEAT both replicated each rank gathers from its own tables; a replicated ITEM_EMB beside a sharded
+ *   ITEM_FEAT is CTR_ESTATE.
+ *   Every rank checks its arguments and state, then the ranks exchange verdicts: if any rank fails, every rank returns
+ *   the lowest failing rank's code and no model changes.  CTR_EINVAL everywhere: a ctr_mlp_config (the device aside) or
+ *   ctr_mlp_options that differs across ranks, a model kind that differs, a warm start whose fitted state (fitted or
+ *   not, output kind, classes, t, packed parameters) differs, a table placement that differs, or more than INT32_MAX
+ *   keys in all.  No survivor on any rank is CTR_ENOTFOUND everywhere.  A CUDA or NCCL failure after the agreement
+ *   follows the rule of the live-table calls above (ctr_idmap_insert): that rank returns the error and the models may
+ *   differ.  Null m or h, n < 0, n > INT32_MAX, or a NULL array with n > 0 is CTR_EINVAL (null m or h before any
+ *   collective work; a rank with other bad arguments still takes part in the agreement with its refusal).
+ *   Ordering: on a row-sharded ITEM_EMB the call enters as the whole-table serving calls do (the shard mappings
+ *   published, a device barrier behind every rank's queued row updates, the hot rows written back to their owners), so
+ *   no ctr_sync or barrier is needed after training or a live-table write; the next collective call orders itself
+ *   after this one likewise.
+ *   Memory: the one-GPU cost of about (S + 7)·4 bytes per survivor, now for ALL ranks' survivors on every rank: the
+ *   gathered records and the shuffle index take (S + 5)·4 bytes per survivor of the whole concatenation, beside this
+ *   rank's own resolution arrays (the all-gather staging: 20 bytes per own key and S·4 per own survivor).  The
+ *   all-gather moves (S + 3)·4 bytes per survivor to every rank.
+ *   Locking: h's mutex, then m's, as ctr_mlp_fit_keys. */
+int  ctr_mlp_fit_keys_dist(ctr_mlp* m, ctr_handle* h, const int64_t* user_ids, const int64_t* item_ids, const int64_t* ts,
+                           const float* label, int64_t n, int32_t* n_iter, double* loss_curve, int64_t* rows_used);
 /* Top-k recommendation over the whole item table with the classifier: the default recall recommend/api.go leaves as a
  * todo (api.go:115-118), for main.go's model.  h is the feature store, as for ctr_mlp_predict_keys.
  *   Users are external ids (h's user map); user j's history is GetUserBehavior(uid, S, -1, ts[j]) from the device
