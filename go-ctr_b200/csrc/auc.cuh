@@ -11,6 +11,10 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 #include <thrust/iterator/counting_iterator.h>
+#include <algorithm>
+#include <cmath>
+#include <utility>
+#include <vector>
 
 namespace ctr {
 
@@ -217,6 +221,213 @@ __global__ void k_gauc_final(const GaucPart* __restrict__ part, int nparts, cons
     p = gauc_block_sum(p);
     if (threadIdx.x == 0)
         *res = {p.used > 0 ? (p.hi + p.lo) / (double)p.w : __longlong_as_double(0x7ff8000000000000ll), (long long)*runs, p.used};
+}
+
+// The fold's shape is fixed (kGaucParts blocks of 256 threads, not a multiple of the device's SM count), so the weighted
+// mean depends on the sequence of groups alone: ctr_group_auc and ctr_group_auc_dist fold the same groups to the same bits.
+constexpr int kGaucParts = 264;
+
+// The grouped driver's launches, shared by ctr_group_auc and ctr_group_auc_dist (and the kernel probe).  launch(name, f)
+// runs f, a lambda that enqueues work on st, and returns 0 or an error code; the engine's launch() profiles it under name.
+// From samples sorted by (group key, score key) in gkey / packed: the groups' keys in uniq, their (area2, n, positives)
+// in agg and their number in *d_runs.  n >= 1.
+template <class Launch>
+int gauc_group_terms(Launch&& launch, const unsigned long long* gkey, const unsigned long long* packed, long n, GaucScan* scan,
+                     GaucAgg* val, unsigned long long* uniq, GaucAgg* agg, int* d_runs, void* tmp, size_t bytes, int grid, cudaStream_t st) {
+    int rc;
+    if ((rc = launch("gauc_heads", [&] { k_gauc_heads<<<grid, 256, 0, st>>>(gkey, packed, n, scan); }))) return rc;
+    if ((rc = launch("gauc_scan", [&] {
+             cub::DeviceScan::InclusiveScan(tmp, bytes, scan, scan, GaucScanOp(), (int)n, st); }))) return rc;
+    if ((rc = launch("gauc_terms", [&] { k_gauc_terms<<<grid, 256, 0, st>>>(gkey, packed, scan, n, val); }))) return rc;
+    return launch("gauc_reduce", [&] {
+        cub::DeviceReduce::ReduceByKey(tmp, bytes, gkey, uniq, val, agg, d_runs, GaucAggOp(), (int)n, st); });
+}
+// the per-group AUCs (the out_* arrays may be null) and the impression-weighted mean of the *d_runs groups in res
+template <class Launch>
+int gauc_fold_groups(Launch&& launch, const unsigned long long* uniq, const GaucAgg* agg, const int* d_runs, long long* out_group,
+                     int* out_n, int* out_pos, double* out_auc, GaucPart* part, GaucResult* res, cudaStream_t st) {
+    int rc;
+    if ((rc = launch("gauc_groups", [&] { k_gauc_groups<<<kGaucParts, 256, 0, st>>>(uniq, agg, d_runs, out_group, out_n, out_pos, out_auc, part); })))
+        return rc;
+    return launch("gauc_final", [&] { k_gauc_final<<<1, 256, 0, st>>>(part, kGaucParts, d_runs, res); });
+}
+
+// ---- ROC AUC and GAUC over every rank's samples (ctr_roc_auc_dist, ctr_group_auc_dist) ---------------------------------
+// Both calls range-partition their data by key so that everything one key decides meets on one rank: a tie group of
+// scores (ROC AUC) or a group of samples (GAUC).  Ranks own ascending key ranges in rank order.  The steps below are
+// per rank and take no handle, so the kernel probe runs them on shards of one device; the exchanges are in engine.cu.
+//
+// ROC AUC: a run is (score key, positives << 32 | negatives).  Each rank sorts its keys, sums the counts of equal keys
+// (auc_dist_rle), sends the runs of each key range to its owner, and sums equal keys again over what it received (the
+// same auc_dist_rle).  Counts packed this way add without carries while the total is below 2^32.  The area is the
+// integer sum over the owner's runs j of neg_j (2 tp_{j-1} + pos_j), where tp_{j-1} counts every positive of a lower key,
+// on this rank or on a lower rank.
+
+constexpr int kDistSamples = 31;   // regular samples of each rank's sorted keys; with the key count one gather slot of 32
+
+__global__ void k_auc_dist_keys(const float* __restrict__ pred, const float* __restrict__ y, long n, unsigned* __restrict__ keys,
+                                unsigned long long* __restrict__ cnt) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        keys[i] = auc_score_key(pred[i]);
+        cnt[i] = auc_positive(y[i]) ? 1ull << 32 : 1ull;
+    }
+}
+struct SumU64 { __device__ __forceinline__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a + b; } };
+
+// out[0] = the number of keys *d_u, out[1 + i] = key (i * u) / kDistSamples of the sorted keys (0 when u = 0)
+template <typename K>
+__global__ void k_dist_samples(const K* __restrict__ keys, const int* __restrict__ d_u, long long* __restrict__ out) {
+    const long u = *d_u;
+    const int t = threadIdx.x;
+    if (t == 0) out[0] = u;
+    if (t < kDistSamples) out[1 + t] = u > 0 ? (long long)keys[(long)t * u / kDistSamples] : 0;
+}
+// off[d] = the first sorted key that belongs to rank d or later: off[0] = 0, off[d] = #keys <= spl[d - 1], off[W] = u
+template <typename K>
+__global__ void k_dist_part(const K* __restrict__ keys, const int* __restrict__ d_u, const unsigned long long* __restrict__ spl, int W,
+                            long long* __restrict__ off) {
+    const long u = *d_u;
+    const int d = threadIdx.x;
+    if (d > W) return;
+    if (d == 0 || d == W) { off[d] = d == 0 ? 0 : u; return; }
+    const unsigned long long s = spl[d - 1];
+    long lo = 0, hi = u;
+    while (lo < hi) { const long mid = (lo + hi) >> 1; if ((unsigned long long)keys[mid] <= s) lo = mid + 1; else hi = mid; }
+    off[d] = lo;
+}
+// this rank's share of 2 x the area: neg_j (2 tp_{j-1} + pos_j) over its merged runs, inc the inclusive sum of cnt and
+// base the positives of every lower rank; the sum is exact (2 P N < 2^64), so the order of the atomics does not matter
+__global__ void k_auc_dist_area(const unsigned long long* __restrict__ cnt, const unsigned long long* __restrict__ inc, long m,
+                                unsigned long long base, unsigned long long* __restrict__ acc) {
+    unsigned long long local = 0;
+    for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j < m; j += (long)gridDim.x * blockDim.x) {
+        const unsigned long long c = cnt[j], pos = c >> 32, neg = c & 0xffffffffull;
+        const unsigned long long before = base + (inc[j] >> 32) - pos;
+        local += neg * (2 * before + pos);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
+    if ((threadIdx.x & 31) == 0 && local) atomicAdd(acc, local);
+}
+// GAUC's record of a sample: the group key to partition and sort by, and the score key with the label in bit 0
+__global__ void k_gauc_dist_rec(const float* __restrict__ pred, const float* __restrict__ y, const long long* __restrict__ group, long n,
+                                unsigned long long* __restrict__ gkey, unsigned long long* __restrict__ packed) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        gkey[i] = gauc_group_key(group[i]);
+        packed[i] = (unsigned long long)auc_score_key(pred[i]) << 32 | (unsigned)auc_positive(y[i]);
+    }
+}
+
+inline int dist_grid(long n) { long g = (n + 255) / 256; if (g > 132 * 8) g = 132 * 8; return (int)(g > 0 ? g : 1); }
+
+// CUB scratch of auc_dist_rle over n entries
+inline size_t auc_dist_rle_bytes(long n, cudaStream_t st) {
+    size_t a = 0, b = 0, c = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, a, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned long long*)nullptr,
+                                    (unsigned long long*)nullptr, (int)n, 0, 32, st);
+    cub::DeviceReduce::ReduceByKey(nullptr, b, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned long long*)nullptr,
+                                   (unsigned long long*)nullptr, (int*)nullptr, SumU64(), (int)n, st);
+    cub::DeviceScan::InclusiveSum(nullptr, c, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n, st);
+    return std::max(std::max(a, b), std::max(c, (size_t)1));
+}
+// runs of (key, count) pairs: sorted by key into ks / cs, equal keys summed into ukey / ucnt, their number in *d_u
+inline cudaError_t auc_dist_rle(const unsigned* k, const unsigned long long* c, long n, unsigned* ks, unsigned long long* cs,
+                                unsigned* ukey, unsigned long long* ucnt, int* d_u, void* tmp, size_t bytes, cudaStream_t st) {
+    if (n == 0) return cudaMemsetAsync(d_u, 0, sizeof(int), st);
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, bytes, k, ks, c, cs, (int)n, 0, 32, st);
+    if (e == cudaSuccess) e = cub::DeviceReduce::ReduceByKey(tmp, bytes, ks, ukey, cs, ucnt, d_u, SumU64(), (int)n, st);
+    return e;
+}
+// one rank's runs of its own samples (device pred / y; k0 / c0 / ks / cs scratch of n entries)
+inline cudaError_t auc_dist_local(const float* pred, const float* y, long n, unsigned* k0, unsigned long long* c0, unsigned* ks,
+                                  unsigned long long* cs, unsigned* ukey, unsigned long long* ucnt, int* d_u, void* tmp, size_t bytes,
+                                  cudaStream_t st) {
+    if (n > 0) k_auc_dist_keys<<<dist_grid(n), 256, 0, st>>>(pred, y, n, k0, c0);
+    const cudaError_t e = cudaGetLastError();
+    return e != cudaSuccess ? e : auc_dist_rle(k0, c0, n, ks, cs, ukey, ucnt, d_u, tmp, bytes, st);
+}
+// the regular samples of u sorted keys into smp[kDistSamples + 1] (device)
+template <typename K>
+inline cudaError_t dist_samples(const K* keys, const int* d_u, long long* smp, cudaStream_t st) {
+    k_dist_samples<K><<<1, 32, 0, st>>>(keys, d_u, smp);
+    return cudaGetLastError();
+}
+// The W - 1 splitters from every rank's samples (all[r (kDistSamples + 1)] = u_r, then its samples as in
+// k_dist_samples).  Every sample of rank r weighs u_r; splitter d is the smallest sample key at which the cumulative
+// weight in ascending key order reaches d / W of the total.  Rank d then owns the keys in (spl[d - 1], spl[d]].
+inline void dist_splitters(const int64_t* all, int W, unsigned long long* spl) {
+    std::vector<std::pair<unsigned long long, unsigned long long>> s;
+    unsigned long long total = 0;
+    for (int r = 0; r < W; r++) {
+        const int64_t* a = all + (size_t)r * (kDistSamples + 1);
+        if (a[0] <= 0) continue;
+        for (int i = 0; i < kDistSamples; i++) s.push_back({(unsigned long long)a[1 + i], (unsigned long long)a[0]});
+        total += (unsigned long long)a[0] * kDistSamples;
+    }
+    std::sort(s.begin(), s.end());
+    size_t i = 0;
+    unsigned long long cum = 0;
+    for (int d = 1; d < W; d++) {
+        while (i < s.size() && cum * (unsigned long long)W < (unsigned long long)d * total) cum += s[i++].second;
+        spl[d - 1] = i > 0 ? s[i - 1].first : 0ull;
+    }
+}
+// the send offsets off[0 .. W] of u sorted keys (device spl [W - 1], off [W + 1])
+template <typename K>
+inline cudaError_t dist_part(const K* keys, const int* d_u, const unsigned long long* spl, int W, long long* off, cudaStream_t st) {
+    k_dist_part<K><<<1, 32, 0, st>>>(keys, d_u, spl, W, off);
+    return cudaGetLastError();
+}
+// this rank's 2 x area into acc[0] (zeroed here) from its m merged runs; inc is scratch of m entries.  The positives and
+// negatives of the runs come back in *pos / *neg (host; synchronises st).
+inline cudaError_t auc_dist_totals(const unsigned long long* cnt, long m, unsigned long long* inc, void* tmp, size_t bytes,
+                                   unsigned long long* pos, unsigned long long* neg, cudaStream_t st) {
+    *pos = *neg = 0;
+    if (m == 0) return cudaSuccess;
+    cudaError_t e = cub::DeviceScan::InclusiveSum(tmp, bytes, cnt, inc, (int)m, st);
+    unsigned long long t = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&t, inc + (m - 1), sizeof t, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    *pos = t >> 32; *neg = t & 0xffffffffull;
+    return e;
+}
+inline cudaError_t auc_dist_area(const unsigned long long* cnt, const unsigned long long* inc, long m, unsigned long long base,
+                                 unsigned long long* acc, cudaStream_t st) {
+    cudaError_t e = cudaMemsetAsync(acc, 0, sizeof(unsigned long long), st);
+    if (e == cudaSuccess && m > 0) { k_auc_dist_area<<<dist_grid(m), 256, 0, st>>>(cnt, inc, m, base, acc); e = cudaGetLastError(); }
+    return e;
+}
+// ROC AUC from the integer totals, rounded once as auc_run rounds it
+inline double auc_dist_value(unsigned long long area2, unsigned long long P, unsigned long long N) {
+    return (P > 0 && N > 0) ? ((double)area2 * 0.5) / ((double)P * (double)N) : nan("");
+}
+
+// GAUC: records (group key, score key << 32 | label) sorted by group key on the sender, range-partitioned by group key,
+// then ordered by (group, score) on the owner with two stable radix passes and reduced by gauc_group_terms.
+inline size_t gauc_dist_bytes(long n, cudaStream_t st) {
+    size_t a = 0, b = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, a, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                    (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n, 0, 64, st);
+    cub::DeviceScan::InclusiveScan(nullptr, b, (GaucScan*)nullptr, (GaucScan*)nullptr, GaucScanOp(), (int)n, st);
+    size_t c = 0;
+    cub::DeviceReduce::ReduceByKey(nullptr, c, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (const GaucAgg*)nullptr,
+                                   (GaucAgg*)nullptr, (int*)nullptr, GaucAggOp(), (int)n, st);
+    return std::max(std::max(a, b), std::max(c, (size_t)1));
+}
+// one rank's records sorted by group key into g1 / v1 (g0 / v0 scratch); n >= 1
+inline cudaError_t gauc_dist_sort(const float* pred, const float* y, const long long* group, long n, unsigned long long* g0,
+                                  unsigned long long* v0, unsigned long long* g1, unsigned long long* v1, void* tmp, size_t bytes,
+                                  cudaStream_t st) {
+    k_gauc_dist_rec<<<dist_grid(n), 256, 0, st>>>(pred, y, group, n, g0, v0);
+    const cudaError_t e = cudaGetLastError();
+    return e != cudaSuccess ? e : cub::DeviceRadixSort::SortPairs(tmp, bytes, g0, g1, v0, v1, (int)n, 0, 64, st);
+}
+// the m received records (rg / rv) in (group, score) order in g1 / v1 (g0 / v0 scratch); m >= 1
+inline cudaError_t gauc_dist_order(const unsigned long long* rg, const unsigned long long* rv, long m, unsigned long long* g0,
+                                   unsigned long long* v0, unsigned long long* g1, unsigned long long* v1, void* tmp, size_t bytes,
+                                   cudaStream_t st) {
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, bytes, rv, v0, rg, g0, (int)m, 32, 64, st);
+    return e != cudaSuccess ? e : cub::DeviceRadixSort::SortPairs(tmp, bytes, g0, g1, v0, v1, (int)m, 0, 64, st);
 }
 
 // ---- curves and average precision (ctr_roc_curve, ctr_pr_curve, ctr_average_precision): binaryClfCurve --------------

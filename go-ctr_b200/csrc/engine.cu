@@ -2513,29 +2513,58 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
 
 namespace {
 
+// the engine's launch() in the shape the shared drivers of auc.cuh take
+auto profiled(ctr_handle* h) { return [h](const char* name, auto&& f) { return launch(h, name, f); }; }
+
+// The fold of ctr_group_auc and ctr_group_auc_dist over the groups in uniq / agg (*d_runs of them; room for the per-group
+// outputs of `room`), then the results: a non-null out_* array with cap < the group count is CTR_EINVAL with nothing
+// written.
+int gauc_fold(ctr_handle* h, const unsigned long long* uniq, const GaucAgg* agg, const int* d_runs, size_t room, int64_t cap, double* gauc,
+              int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+    cudaStream_t st = h->stream;
+    DevBuf<GaucPart> part; DevBuf<GaucResult> res;
+    DevBuf<long long> o_group; DevBuf<int> o_n, o_pos; DevBuf<double> o_auc;
+    CU(h, part.alloc(kGaucParts)); CU(h, res.alloc(1));
+    if (out_group) CU(h, o_group.alloc(room));
+    if (out_n) CU(h, o_n.alloc(room));
+    if (out_pos) CU(h, o_pos.alloc(room));
+    if (out_auc) CU(h, o_auc.alloc(room));
+    RET(gauc_fold_groups(profiled(h), uniq, agg, d_runs, o_group, o_n, o_pos, o_auc, part, res, st));
+    GaucResult r{};
+    CU(h, cudaMemcpyAsync(&r, res, sizeof r, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if ((out_group || out_n || out_pos || out_auc) && r.groups > cap)
+        return set_err(h, CTR_EINVAL, "group auc: %lld groups do not fit the per-group arrays (cap %lld)", (long long)r.groups, (long long)cap);
+    const size_t R = (size_t)r.groups;
+    if (out_group) CU(h, cudaMemcpyAsync(out_group, o_group, R * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_n) CU(h, cudaMemcpyAsync(out_n, o_n, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_pos) CU(h, cudaMemcpyAsync(out_pos, o_pos, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (out_auc) CU(h, cudaMemcpyAsync(out_auc, o_auc, R * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *gauc = r.gauc;
+    if (n_groups) *n_groups = r.groups;
+    if (n_used) *n_used = r.used;
+    return CTR_OK;
+}
+
 // ctr_group_auc on the engine stream: (group, score) order by two stable radix passes, one scan, one reduce-by-key,
 // then the per-group AUCs and their weighted mean on the device (auc.cuh); only the result, and the per-group arrays
 // when asked for, come back
 int gauc_run(ctr_handle* h, const float* pred_h, const float* y_h, const int64_t* group_h, long n, double* gauc,
-             int64_t* n_groups, int64_t* n_used, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+             int64_t* n_groups, int64_t* n_used, int64_t cap, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
     cudaStream_t st = h->stream;
     const size_t N = (size_t)n;
-    const int grid = (int)std::min<long>((n + 255) / 256, (long)h->num_sms * 8), gparts = h->num_sms * 2;
+    const int grid = (int)std::min<long>((n + 255) / 256, (long)h->num_sms * 8);
     DevBuf<float> d_pred, d_y; DevBuf<long long> d_group;
     DevBuf<unsigned> k0, k1; DevBuf<int> i0, i1, d_runs;
     DevBuf<unsigned long long> g0, g1, v0, v1;
-    DevBuf<GaucScan> scan; DevBuf<GaucAgg> val, agg; DevBuf<GaucPart> part; DevBuf<GaucResult> res;
-    DevBuf<long long> o_group; DevBuf<int> o_n, o_pos; DevBuf<double> o_auc;
+    DevBuf<GaucScan> scan; DevBuf<GaucAgg> val, agg;
     DevBuf<unsigned char> tmp;
     CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N)); CU(h, d_group.alloc(N));
     CU(h, k0.alloc(N)); CU(h, k1.alloc(N)); CU(h, i0.alloc(N)); CU(h, i1.alloc(N));
     CU(h, g0.alloc(N)); CU(h, g1.alloc(N)); CU(h, v0.alloc(N)); CU(h, v1.alloc(N));
     CU(h, scan.alloc(N)); CU(h, val.alloc(N)); CU(h, agg.alloc(N));
-    CU(h, d_runs.alloc(1)); CU(h, part.alloc(gparts)); CU(h, res.alloc(1));
-    if (out_group) CU(h, o_group.alloc(N));
-    if (out_n) CU(h, o_n.alloc(N));
-    if (out_pos) CU(h, o_pos.alloc(N));
-    if (out_auc) CU(h, o_auc.alloc(N));
+    CU(h, d_runs.alloc(1));
     unsigned long long* uniq = g0.get();     // free once the group pass has read it
     size_t b[4] = {0, 0, 0, 0};
     CU(h, cub::DeviceRadixSort::SortPairs(nullptr, b[0], k0.get(), k1.get(), i0.get(), i1.get(), (int)n, 0, 32, st));
@@ -2553,27 +2582,8 @@ int gauc_run(ctr_handle* h, const float* pred_h, const float* y_h, const int64_t
     RET(launch(h, "gauc_gather", [&] { k_gauc_gather<<<grid, 256, 0, st>>>(k1, i1, d_group, d_y, n, g0, v0); }));
     RET(launch(h, "gauc_sort_group", [&] {
         cub::DeviceRadixSort::SortPairs(tmp.get(), bytes, g0.get(), g1.get(), v0.get(), v1.get(), (int)n, 0, 64, st); }));
-    RET(launch(h, "gauc_heads", [&] { k_gauc_heads<<<grid, 256, 0, st>>>(g1, v1, n, scan); }));
-    RET(launch(h, "gauc_scan", [&] {
-        cub::DeviceScan::InclusiveScan(tmp.get(), bytes, scan.get(), scan.get(), GaucScanOp(), (int)n, st); }));
-    RET(launch(h, "gauc_terms", [&] { k_gauc_terms<<<grid, 256, 0, st>>>(g1, v1, scan, n, val); }));
-    RET(launch(h, "gauc_reduce", [&] {
-        cub::DeviceReduce::ReduceByKey(tmp.get(), bytes, g1.get(), uniq, val.get(), agg.get(), d_runs.get(), GaucAggOp(), (int)n, st); }));
-    RET(launch(h, "gauc_groups", [&] { k_gauc_groups<<<gparts, 256, 0, st>>>(uniq, agg, d_runs, o_group, o_n, o_pos, o_auc, part); }));
-    RET(launch(h, "gauc_final", [&] { k_gauc_final<<<1, 256, 0, st>>>(part, gparts, d_runs, res); }));
-    GaucResult r{};
-    CU(h, cudaMemcpyAsync(&r, res, sizeof r, cudaMemcpyDeviceToHost, st));
-    CU(h, cudaStreamSynchronize(st));
-    const size_t R = (size_t)r.groups;
-    if (out_group) CU(h, cudaMemcpyAsync(out_group, o_group, R * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    if (out_n) CU(h, cudaMemcpyAsync(out_n, o_n, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (out_pos) CU(h, cudaMemcpyAsync(out_pos, o_pos, R * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (out_auc) CU(h, cudaMemcpyAsync(out_auc, o_auc, R * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CU(h, cudaStreamSynchronize(st));
-    *gauc = r.gauc;
-    if (n_groups) *n_groups = r.groups;
-    if (n_used) *n_used = r.used;
-    return CTR_OK;
+    RET(gauc_group_terms(profiled(h), g1, v1, n, scan, val, uniq, agg, d_runs, tmp, bytes, grid, st));
+    return gauc_fold(h, uniq, agg, d_runs, N, cap, gauc, n_groups, n_used, out_group, out_n, out_pos, out_auc);
 }
 
 }  // namespace
@@ -2584,9 +2594,236 @@ int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_
         return set_err(h, CTR_EINVAL, "bad group auc arguments (n must be in [1, 2^31); pred, y, group and gauc non-null)");
     std::lock_guard<std::mutex> lk(h->mu);
     CU(h, cudaSetDevice(h->dev));
-    return gauc_run(h, pred, y, group, (long)n, gauc, n_groups, n_used, out_group, out_n, out_pos, out_auc);
+    return gauc_run(h, pred, y, group, (long)n, gauc, n_groups, n_used, n, out_group, out_n, out_pos, out_auc);
 }
 
+namespace {
+
+// The agreement of the two evaluation calls on world > 1: mode tells the calls apart, so that ranks in different calls
+// refuse together; every rank's sample count comes back in shares and their total is checked here.
+int eval_agree(ctr_handle* h, int mode, int verdict, int64_t n, int64_t* shares, int64_t* total) {
+    CommHdr hd{};
+    hd.mode = mode; hd.share = n;
+    RET(comm_agree(h, hd, verdict, shares));
+    *total = 0;
+    for (int j = 0; j < h->comm.world; j++) *total += shares[j];
+    if (*total < 1 || *total > (int64_t)0xffffffffll)
+        return set_err(h, CTR_EINVAL, "the ranks pass %lld samples in all; the total must be in [1, 2^32)", (long long)*total);
+    return CTR_OK;
+}
+
+// The exchange plan of a range partition: this rank's sorted keys are cut at the splitters of every rank's samples
+// (smp: this rank's samples on the device, off: the cut on the device), the send counts all-gathered, and the receive
+// counts and offsets derived.  Every rank computes the same matrix, so a receive over 2^31 - 1 is refused everywhere.
+// keys: unsigned (wide = false) or unsigned long long (wide = true)
+int dist_plan(ctr_handle* h, const char* key_part, const void* keys, bool wide, const int* d_u, long long* smp, unsigned long long* spl, long long* off,
+              std::vector<int64_t>& scnt, std::vector<int64_t>& soff, std::vector<int64_t>& rcnt, std::vector<int64_t>& roff, int64_t* recv) {
+    const int W = h->comm.world, me = h->comm.rank;
+    cudaStream_t st = h->stream;
+    int64_t mine[kDistSamples + 1], all[(kDistSamples + 1) * kMaxPeers];
+    RET(launch(h, key_part, [&] {
+        if (wide) dist_samples((const unsigned long long*)keys, d_u, smp, st); else dist_samples((const unsigned*)keys, d_u, smp, st); }));
+    CU(h, cudaMemcpyAsync(mine, smp, sizeof mine, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    RET(comm_gather_i64(h, mine, kDistSamples + 1, all));
+    unsigned long long hs[kMaxPeers];
+    dist_splitters(all, W, hs);
+    CU(h, cudaMemcpyAsync(spl, hs, sizeof(unsigned long long) * (size_t)(W - 1), cudaMemcpyHostToDevice, st));
+    RET(launch(h, key_part, [&] {
+        if (wide) dist_part((const unsigned long long*)keys, d_u, spl, W, off, st); else dist_part((const unsigned*)keys, d_u, spl, W, off, st); }));
+    int64_t o[kMaxPeers + 1];
+    CU(h, cudaMemcpyAsync(o, off, sizeof(int64_t) * (size_t)(W + 1), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    scnt.assign((size_t)W, 0); soff.assign((size_t)W, 0); rcnt.assign((size_t)W, 0); roff.assign((size_t)W, 0);
+    for (int k = 0; k < W; k++) { soff[(size_t)k] = o[k]; scnt[(size_t)k] = o[k + 1] - o[k]; }
+    int64_t mat[kMaxPeers * kMaxPeers];
+    RET(comm_gather_i64(h, scnt.data(), W, mat));            // mat[j·W + k]: what rank j sends rank k
+    *recv = 0;
+    for (int k = 0; k < W; k++) {
+        int64_t in = 0;
+        for (int j = 0; j < W; j++) in += mat[j * W + k];
+        if (in > 0x7fffffffll)
+            return set_err(h, CTR_EINVAL, "rank %d would receive %lld entries of one key range; a rank takes at most 2^31 - 1", k, (long long)in);
+    }
+    for (int j = 0; j < W; j++) { roff[(size_t)j] = *recv; rcnt[(size_t)j] = mat[j * W + me]; *recv += rcnt[(size_t)j]; }
+    return CTR_OK;
+}
+
+// ctr_roc_auc_dist on world > 1 after the agreement: local runs, range partition, runs to their owners, merge, the
+// positives below each rank, integer area summed over the ranks
+int auc_dist_ranks(ctr_handle* h, const float* pred_h, const float* y_h, long n, double* auc) {
+    cudaStream_t st = h->stream;
+    const int W = h->comm.world;
+    const size_t N = (size_t)std::max<long>(n, 1);
+    DevBuf<float> d_pred, d_y; DevBuf<unsigned> k0, ks, uk; DevBuf<unsigned long long> c0, cs, uc, spl, acc;
+    DevBuf<long long> smp, off; DevBuf<int> d_u; DevBuf<unsigned char> tmp;
+    CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N)); CU(h, k0.alloc(N)); CU(h, ks.alloc(N)); CU(h, uk.alloc(N));
+    CU(h, c0.alloc(N)); CU(h, cs.alloc(N)); CU(h, uc.alloc(N));
+    CU(h, spl.alloc(kMaxPeers)); CU(h, acc.alloc(1)); CU(h, smp.alloc(kDistSamples + 1)); CU(h, off.alloc(kMaxPeers + 1)); CU(h, d_u.alloc(1));
+    size_t bytes = auc_dist_rle_bytes((long)N, st);
+    CU(h, tmp.alloc(bytes));
+    if (n > 0) {
+        CU(h, cudaMemcpyAsync(d_pred, pred_h, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, st));
+        CU(h, cudaMemcpyAsync(d_y, y_h, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, st));
+    }
+    cudaError_t e = cudaSuccess;
+    RET(launch(h, "auc_dist_rle", [&] { e = auc_dist_local(d_pred, d_y, n, k0, c0, ks, cs, uk, uc, d_u, tmp, bytes, st); }));
+    CU(h, e);
+    d_pred.reset(); d_y.reset(); k0.reset(); c0.reset(); ks.reset(); cs.reset();
+    std::vector<int64_t> scnt, soff, rcnt, roff;
+    int64_t M = 0;
+    RET(dist_plan(h, "auc_dist_part", uk, false, d_u, smp, spl, off, scnt, soff, rcnt, roff, &M));
+    const size_t MM = (size_t)std::max<int64_t>(M, 1);
+    DevBuf<unsigned> rk, mk; DevBuf<unsigned long long> rc, mc, inc;
+    CU(h, rk.alloc(MM)); CU(h, rc.alloc(MM));
+    int rcode = CTR_OK;
+    RET(launch(h, "auc_dist_ranks", [&] {
+        rcode = comm_route(h, uk, scnt.data(), soff.data(), rk, rcnt.data(), roff.data(), sizeof(unsigned));
+        if (rcode == CTR_OK) rcode = comm_route(h, uc, scnt.data(), soff.data(), rc, rcnt.data(), roff.data(), sizeof(unsigned long long)); }));
+    RET(rcode);
+    CU(h, ks.alloc(MM)); CU(h, cs.alloc(MM)); CU(h, mk.alloc(MM)); CU(h, mc.alloc(MM)); CU(h, inc.alloc(MM));
+    if ((size_t)M > N) { bytes = auc_dist_rle_bytes((long)M, st); CU(h, tmp.alloc(bytes)); }
+    RET(launch(h, "auc_dist_merge", [&] { e = auc_dist_rle(rk, rc, (long)M, ks, cs, mk, mc, d_u, tmp, bytes, st); }));
+    CU(h, e);
+    int m = 0;
+    CU(h, cudaMemcpyAsync(&m, d_u, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    unsigned long long pn[2];
+    RET(launch(h, "auc_dist_area", [&] { e = auc_dist_totals(mc, m, inc, tmp, bytes, &pn[0], &pn[1], st); }));
+    CU(h, e);
+    int64_t mine[2] = {(int64_t)pn[0], (int64_t)pn[1]}, all[2 * kMaxPeers];
+    RET(comm_gather_i64(h, mine, 2, all));
+    unsigned long long base = 0, P = 0, Nn = 0;
+    for (int j = 0; j < W; j++) {
+        if (j < h->comm.rank) base += (unsigned long long)all[2 * j];
+        P += (unsigned long long)all[2 * j]; Nn += (unsigned long long)all[2 * j + 1];
+    }
+    RET(launch(h, "auc_dist_area", [&] { e = auc_dist_area(mc, inc, m, base, acc, st); }));
+    CU(h, e);
+    RET(launch(h, "auc_dist_ranks", [&] { rcode = comm_sum_u64(h, acc, 1); }));
+    RET(rcode);
+    unsigned long long area2 = 0;
+    CU(h, cudaMemcpyAsync(&area2, acc, sizeof area2, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *auc = auc_dist_value(area2, P, Nn);
+    return CTR_OK;
+}
+
+// ctr_group_auc_dist on world > 1 after the agreement: records sorted by group, range partition, records to their
+// owners, the grouped driver on each rank's groups, the groups' terms concatenated in rank order (ascending groups) and
+// folded on every rank as ctr_group_auc folds them
+int gauc_dist_ranks(ctr_handle* h, const float* pred_h, const float* y_h, const int64_t* group_h, long n, double* gauc, int64_t* n_groups,
+                    int64_t* n_used, int64_t cap, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+    cudaStream_t st = h->stream;
+    const int W = h->comm.world, me = h->comm.rank;
+    const size_t N = (size_t)std::max<long>(n, 1);
+    DevBuf<float> d_pred, d_y; DevBuf<long long> d_group, smp, off;
+    DevBuf<unsigned long long> g0, v0, g1, v1, spl; DevBuf<int> d_u; DevBuf<unsigned char> tmp;
+    CU(h, d_pred.alloc(N)); CU(h, d_y.alloc(N)); CU(h, d_group.alloc(N));
+    CU(h, g0.alloc(N)); CU(h, v0.alloc(N)); CU(h, g1.alloc(N)); CU(h, v1.alloc(N));
+    CU(h, spl.alloc(kMaxPeers)); CU(h, smp.alloc(kDistSamples + 1)); CU(h, off.alloc(kMaxPeers + 1)); CU(h, d_u.alloc(1));
+    size_t bytes = gauc_dist_bytes((long)N, st);
+    CU(h, tmp.alloc(bytes));
+    const int un = (int)n;
+    CU(h, cudaMemcpyAsync(d_u, &un, sizeof(int), cudaMemcpyHostToDevice, st));
+    cudaError_t e = cudaSuccess;
+    if (n > 0) {
+        CU(h, cudaMemcpyAsync(d_pred, pred_h, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, st));
+        CU(h, cudaMemcpyAsync(d_y, y_h, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, st));
+        CU(h, cudaMemcpyAsync(d_group, group_h, (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+        RET(launch(h, "gauc_dist_sort", [&] { e = gauc_dist_sort(d_pred, d_y, d_group, n, g0, v0, g1, v1, tmp, bytes, st); }));
+        CU(h, e);
+    }
+    CU(h, cudaStreamSynchronize(st));          // the pageable copies have read the caller's arrays
+    d_pred.reset(); d_y.reset(); d_group.reset(); g0.reset(); v0.reset();
+    std::vector<int64_t> scnt, soff, rcnt, roff;
+    int64_t M = 0;
+    RET(dist_plan(h, "gauc_dist_part", g1, true, d_u, smp, spl, off, scnt, soff, rcnt, roff, &M));
+    const size_t MM = (size_t)std::max<int64_t>(M, 1);
+    DevBuf<unsigned long long> rg, rv;
+    CU(h, rg.alloc(MM)); CU(h, rv.alloc(MM));
+    int rcode = CTR_OK;
+    RET(launch(h, "gauc_dist_ranks", [&] {
+        rcode = comm_route(h, g1, scnt.data(), soff.data(), rg, rcnt.data(), roff.data(), sizeof(unsigned long long));
+        if (rcode == CTR_OK) rcode = comm_route(h, v1, scnt.data(), soff.data(), rv, rcnt.data(), roff.data(), sizeof(unsigned long long)); }));
+    RET(rcode);
+    CU(h, cudaStreamSynchronize(st));
+    g1.reset(); v1.reset();
+    DevBuf<unsigned long long> uniq; DevBuf<GaucAgg> agg;
+    int R = 0;
+    if (M > 0) {
+        DevBuf<GaucScan> scan; DevBuf<GaucAgg> val;
+        CU(h, g0.alloc(MM)); CU(h, v0.alloc(MM)); CU(h, g1.alloc(MM)); CU(h, v1.alloc(MM));
+        CU(h, scan.alloc(MM)); CU(h, val.alloc(MM)); CU(h, uniq.alloc(MM)); CU(h, agg.alloc(MM));
+        if ((size_t)M > N) { bytes = gauc_dist_bytes((long)M, st); CU(h, tmp.alloc(bytes)); }
+        RET(launch(h, "gauc_dist_order", [&] { e = gauc_dist_order(rg, rv, (long)M, g0, v0, g1, v1, tmp, bytes, st); }));
+        CU(h, e);
+        rg.reset(); rv.reset();
+        RET(gauc_group_terms(profiled(h), g1, v1, (long)M, scan, val, uniq, agg, d_u, tmp, bytes, dist_grid((long)M), st));
+        CU(h, cudaMemcpyAsync(&R, d_u, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+    }
+    int64_t mine = R, cnt[kMaxPeers], goff[kMaxPeers];
+    RET(comm_gather_i64(h, &mine, 1, cnt));
+    int64_t G = 0;
+    for (int j = 0; j < W; j++) { goff[j] = G; G += cnt[j]; }
+    if (G > 0x7fffffffll) return set_err(h, CTR_EINVAL, "group auc: %lld groups; at most 2^31 - 1", (long long)G);
+    if ((out_group || out_n || out_pos || out_auc) && G > cap)
+        return set_err(h, CTR_EINVAL, "group auc: %lld groups do not fit the per-group arrays (cap %lld)", (long long)G, (long long)cap);
+    DevBuf<unsigned long long> all_uniq; DevBuf<GaucAgg> all_agg;
+    CU(h, all_uniq.alloc((size_t)G)); CU(h, all_agg.alloc((size_t)G));
+    if (R > 0) {
+        CU(h, cudaMemcpyAsync(all_uniq.get() + goff[me], uniq, sizeof(unsigned long long) * (size_t)R, cudaMemcpyDeviceToDevice, st));
+        CU(h, cudaMemcpyAsync(all_agg.get() + goff[me], agg, sizeof(GaucAgg) * (size_t)R, cudaMemcpyDeviceToDevice, st));
+    }
+    RET(launch(h, "gauc_dist_ranks", [&] {
+        rcode = comm_concat(h, all_uniq, sizeof(unsigned long long), cnt, goff);
+        if (rcode == CTR_OK) rcode = comm_concat(h, all_agg, sizeof(GaucAgg), cnt, goff); }));
+    RET(rcode);
+    const int g32 = (int)G;
+    CU(h, cudaMemcpyAsync(d_u, &g32, sizeof(int), cudaMemcpyHostToDevice, st));
+    return gauc_fold(h, all_uniq, all_agg, d_u, (size_t)G, cap, gauc, n_groups, n_used, out_group, out_n, out_pos, out_auc);
+}
+
+}  // namespace
+
+// On world > 1 a rank whose arguments are bad still takes part in the agreement with its refusal, so that no rank is
+// left waiting; a null handle is refused before anything else.
+int ctr_roc_auc_dist(ctr_handle* h, const float* pred, const float* y, int64_t n, double* auc) {
+    if (!h) return set_err(h, CTR_EINVAL, "bad auc arguments (null handle)");
+    if (h->comm.world == 1) return ctr_roc_auc(h, pred, y, n, auc);
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    h->err.clear();
+    const bool ok = auc && n >= 0 && n <= 0x7fffffff && (n == 0 || (pred && y));
+    const int verdict = ok ? CTR_OK : set_err(h, CTR_EINVAL, "bad auc_dist arguments (n in [0, 2^31), pred and y non-null when n > 0, auc non-null)");
+    int64_t shares[kMaxPeers], total = 0;
+    RET(eval_agree(h, 1, verdict, n, shares, &total));
+    return auc_dist_ranks(h, pred, y, (long)n, auc);
+}
+
+int ctr_group_auc_dist(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n, double* gauc, int64_t* n_groups,
+                       int64_t* n_used, int64_t cap, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc) {
+    if (!h) return set_err(h, CTR_EINVAL, "bad group auc arguments (null handle)");
+    const bool outs = out_group || out_n || out_pos || out_auc;
+    if (h->comm.world == 1) {
+        if (!pred || !y || !group || !gauc || n < 1 || n > 0x7fffffff)
+            return set_err(h, CTR_EINVAL, "bad group auc arguments (n must be in [1, 2^31); pred, y, group and gauc non-null)");
+        if (outs && cap < 0) return set_err(h, CTR_EINVAL, "bad group auc arguments (cap %lld < 0)", (long long)cap);
+        std::lock_guard<std::mutex> lk(h->mu);
+        CU(h, cudaSetDevice(h->dev));
+        return gauc_run(h, pred, y, group, (long)n, gauc, n_groups, n_used, cap, out_group, out_n, out_pos, out_auc);
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    CU(h, cudaSetDevice(h->dev));
+    h->err.clear();
+    const bool ok = gauc && n >= 0 && n <= 0x7fffffff && (n == 0 || (pred && y && group)) && (!outs || cap >= 0);
+    const int verdict = ok ? CTR_OK : set_err(h, CTR_EINVAL, "bad group_auc_dist arguments (n in [0, 2^31), pred, y and group non-null when n > 0, "
+                                                             "gauc non-null, cap >= 0 with per-group arrays)");
+    int64_t shares[kMaxPeers], total = 0;
+    RET(eval_agree(h, 2, verdict, n, shares, &total));
+    return gauc_dist_ranks(h, pred, y, group, (long)n, gauc, n_groups, n_used, cap, out_group, out_n, out_pos, out_auc);
+}
 namespace {
 
 // binaryClfCurve on the engine stream (auc.cuh): with check_labels the labels' range and binariness first, then

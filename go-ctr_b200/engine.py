@@ -33,7 +33,7 @@ EXPORTS = ["ctr_abi_version", "ctr_config_default", "ctr_create", "ctr_destroy",
            "ctr_set_stream", "ctr_launch_count", "ctr_profile_enable", "ctr_profile_get", "ctr_profile_reset",
            "ctr_profile_dump", "ctr_debug_grads_idx", "ctr_ubcache_upload", "ctr_ubcache_window", "ctr_ubcache_window_dev", "ctr_ubcache_append", "ctr_ubcache_set", "ctr_ubcache_download", "ctr_idmap_build", "ctr_idmap_lookup", "ctr_idmap_lookup_dev",
            "ctr_idmap_insert", "ctr_idmap_download", "ctr_table_write_rows",
-           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_item_emb_vocab", "ctr_comm_unique_id", "ctr_comm_init",
+           "ctr_batch_predict_keys", "ctr_checkpoint_save", "ctr_checkpoint_load", "ctr_roc_auc", "ctr_group_auc", "ctr_roc_auc_dist", "ctr_group_auc_dist", "ctr_roc_curve", "ctr_pr_curve", "ctr_average_precision", "ctr_group_average_precision", "ctr_accuracy_score", "ctr_confusion_matrix", "ctr_precision_recall_fscore", "ctr_r2_score", "ctr_mean_error", "ctr_knn_search", "ctr_recommend_topk", "ctr_rank_items", "ctr_recommend_topk_ex", "ctr_rank_items_ex", "ctr_rank_metrics", "ctr_i2v_config_default", "ctr_i2v_paths", "ctr_i2v_train", "ctr_i2v_train_dist", "ctr_item_emb_train", "ctr_item_emb_vocab", "ctr_comm_unique_id", "ctr_comm_init",
            "ctr_mlp_config_default", "ctr_mlp_options_default", "ctr_mlp_create", "ctr_mlp_create_ex", "ctr_mlp_destroy", "ctr_mlp_last_error", "ctr_mlp_fit", "ctr_mlp_predict",
            "ctr_mlp_get_params", "ctr_mlp_set_params", "ctr_mlp_fit_keys", "ctr_mlp_fit_keys_dist", "ctr_mlp_predict_keys",
            "ctr_mlp_recommend_topk", "ctr_mlp_rank_items", "ctr_mlp_recommend_topk_ex", "ctr_mlp_rank_items_ex", "ctr_mlp_get_classes", "ctr_mlp_set_classes", "ctr_mlp_regressor_create", "ctr_mlp_predict_f64",
@@ -542,6 +542,40 @@ class Engine:
         if outs is None:
             return gauc.value, ng.value, nu.value
         return gauc.value, ng.value, nu.value, {k: v[:ng.value].copy() for k, v in outs.items()}
+
+    def roc_auc_dist(self, pred, y):
+        """ROC AUC over every rank's samples (ctr_roc_auc_dist): collective on a multi-GPU handle, each rank passing its
+        own samples (possibly none); every rank gets roc_auc of all ranks' samples concatenated in rank order."""
+        p, pp = _f(pred); t, tp = _f(y)
+        if p.size != t.size:
+            raise ValueError("pred and y differ in length: %d, %d" % (p.size, t.size))
+        auc = C.c_double(0)
+        self._ck(self.L.ctr_roc_auc_dist(self.h, pp, tp, C.c_int64(p.size), C.byref(auc)))
+        return auc.value
+
+    def group_auc_dist(self, pred, y, group, per_group=False):
+        """group_auc over every rank's samples (ctr_group_auc_dist): collective on a multi-GPU handle, each rank passing
+        its own samples (possibly none).  Returns what group_auc returns on all ranks' samples concatenated in rank
+        order, on every rank.  With per_group=True the call runs twice: once for the group count, once for the arrays."""
+        p, pp = _f(pred); t, tp = _f(y)
+        gr = np.ascontiguousarray(group, np.int64)
+        if not p.size == t.size == gr.size:
+            raise ValueError("pred, y and group differ in length: %d, %d, %d" % (p.size, t.size, gr.size))
+        gauc = C.c_double(0); ng = C.c_int64(0); nu = C.c_int64(0)
+
+        def call(outs):
+            ptr = (lambda k, ty: outs[k].ctypes.data_as(C.POINTER(ty))) if outs else (lambda k, ty: None)
+            cap = outs["group"].size if outs else 0
+            self._ck(self.L.ctr_group_auc_dist(self.h, pp, tp, gr.ctypes.data_as(_lp), C.c_int64(p.size), C.byref(gauc), C.byref(ng),
+                                               C.byref(nu), C.c_int64(cap), ptr("group", C.c_int64), ptr("n", C.c_int32),
+                                               ptr("pos", C.c_int32), ptr("auc", C.c_double)))
+        call(None)
+        if not per_group:
+            return gauc.value, ng.value, nu.value
+        k = ng.value
+        outs = dict(group=np.empty(k, np.int64), n=np.empty(k, np.int32), pos=np.empty(k, np.int32), auc=np.empty(k, np.float64))
+        call(outs)
+        return gauc.value, ng.value, nu.value, outs
 
     def _curve(self, fn, pred, y, pos_label):
         p, pp = _f(pred); t, tp = _f(y)

@@ -279,6 +279,57 @@ func (e *Engine) GroupAUC(pred, y []float32, group []int64, perGroup bool) (gauc
 	return float64(g), int64(nu), groups, n, pos, auc, nil
 }
 
+func f32n(p []float32) *C.float {
+	if len(p) == 0 {
+		return nil
+	}
+	return f32(p)
+}
+
+// RocAUCDist is utils.RocAuc32 over every rank's samples of a multi-GPU engine (ctr_roc_auc_dist): collective, each
+// rank passing its own samples (possibly none); every rank gets the AUC of all ranks' samples concatenated in rank
+// order, bit for bit what one GPU computes on them.  On a single-GPU engine it is ctr_roc_auc.
+func (e *Engine) RocAUCDist(pred, y []float32) (float64, error) {
+	if len(y) != len(pred) {
+		return 0, fmt.Errorf("ctrb200: RocAUCDist needs equally long pred and y")
+	}
+	var a C.double
+	err := e.err(C.ctr_roc_auc_dist(e.h, f32n(pred), f32n(y), C.int64_t(len(pred)), &a))
+	return float64(a), err
+}
+
+// GroupAUCDist is GroupAUC over every rank's samples of a multi-GPU engine (ctr_group_auc_dist), with GroupAUC's
+// results on every rank: those of one GPU over all ranks' samples concatenated in rank order.  Collective; a rank may
+// pass no samples.  With perGroup the call runs twice, once for the group count and once for the arrays.
+func (e *Engine) GroupAUCDist(pred, y []float32, group []int64, perGroup bool) (gauc float64, usedGroups int64, groups []int64, n, pos []int32, auc []float64, err error) {
+	m := len(pred)
+	if len(y) != m || len(group) != m {
+		return 0, 0, nil, nil, nil, nil, fmt.Errorf("ctrb200: GroupAUCDist needs equally long pred, y and group")
+	}
+	var g C.double
+	var ng, nu C.int64_t
+	call := func(k int) error {
+		var gp *C.int64_t
+		var np, pp *C.int32_t
+		var ap *C.double
+		if k > 0 {
+			gp, np, pp, ap = i64(groups), i32(n), i32(pos), (*C.double)(unsafe.Pointer(&auc[0]))
+		}
+		return e.err(C.ctr_group_auc_dist(e.h, f32n(pred), f32n(y), i64n(group), C.int64_t(m), &g, &ng, &nu, C.int64_t(k), gp, np, pp, ap))
+	}
+	if err = call(0); err != nil {
+		return 0, 0, nil, nil, nil, nil, err
+	}
+	if perGroup && ng > 0 {
+		k := int(ng)
+		groups, n, pos, auc = make([]int64, k), make([]int32, k), make([]int32, k), make([]float64, k)
+		if err = call(k); err != nil {
+			return 0, 0, nil, nil, nil, nil, err
+		}
+	}
+	return float64(g), int64(nu), groups, n, pos, auc, nil
+}
+
 func f64(p []float64) *C.double { return (*C.double)(unsafe.Pointer(&p[0])) }
 
 // curve runs ctr_roc_curve (roc) or ctr_pr_curve with room for n + 1 points and trims the three arrays; the PR curve's

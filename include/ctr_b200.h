@@ -320,7 +320,8 @@ int ctr_checkpoint_save(ctr_handle* h, const char* path);
 int ctr_checkpoint_load(ctr_handle* h, const char* path);
 
 /* utils.RocAuc32 (util.go:131-148 → nn/metrics/ranking.go:144): labels binarised at 0.5, tied
- * scores grouped, trapezoid. Sorted on the device. */
+ * scores grouped, trapezoid. Sorted on the device.  Each rank evaluates the samples it passes (ctr_roc_auc_dist evaluates
+ * every rank's). */
 int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, double* auc);
 
 /* Grouped AUC (GAUC: the metric of the DIN paper and of go-ctr's README.md:17/25/33): samples are grouped by
@@ -336,10 +337,52 @@ int ctr_roc_auc(ctr_handle* h, const float* pred, const float* y, int64_t n, dou
  * groups), n_used (used groups) and the out_* arrays may each be NULL.  A non-NULL out_* array has room for n entries;
  * its first *n_groups entries are written in ascending group order: the group id, n_g, P_g and AUC_g (NaN when unused).
  * Host buffers; needs no tables (a handle created with batch = pred_batch = 1 is enough).  Runs on the engine stream
- * under the handle's mutex.  Not collective under world > 1: each rank evaluates the samples it passes. */
+ * under the handle's mutex.  Not collective under world > 1: each rank evaluates the samples it passes (ctr_group_auc_dist
+ * evaluates every rank's). */
 int ctr_group_auc(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n,
                   double* gauc, int64_t* n_groups, int64_t* n_used,
                   int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc);
+
+/* ctr_roc_auc and ctr_group_auc over every rank's samples of a multi-GPU handle (a held-out set each rank scored for
+ * its own keys).  Neither needs tables; both run on the engine stream under the handle's mutex and use its
+ * communicator.  h NULL is CTR_EINVAL before any collective work.
+ * World == 1: the calls are ctr_roc_auc and ctr_group_auc, with their results, refusals and messages; the per-group
+ *   arrays are written as ctr_group_auc writes them, and cap bounds them (see below).
+ * World > 1: collective; every rank calls with its own samples.  n in [0, 2^31) per rank (n = 0 allows NULL arrays)
+ *   and the total in [1, 2^32).  Every rank receives what the single-GPU call returns on all ranks' samples concatenated
+ *   in rank order, bit for bit, by its rules (labels binarised at 0.5, -0 read as +0, the NaN key order, ascending
+ *   signed group order).  Every rank checks its arguments, then the ranks exchange verdicts as the live-table calls do:
+ *   if any rank fails, every rank returns the lowest failing rank's code, and nothing is written on any rank.  A CUDA
+ *   or NCCL failure after the agreement follows the rule of ctr_idmap_insert: that rank returns the error and the
+ *   others may wait in the exchange.
+ *
+ * ctr_roc_auc_dist: equal to ctr_roc_auc on the concatenation whenever that call is exact there (2 P N < 2^53; its
+ *   trapezoid terms are half-integers summed in double).  Each rank sorts its score keys and sums the counts of equal
+ *   keys into runs (key, positives, negatives); splitters from regular samples of the ranks' runs cut the key range
+ *   into one range per rank, so equal scores always meet on one rank; each owner merges the runs it receives, learns
+ *   the positives of the lower ranks, and sums its part of area2 = sum (fp_j - fp_{j-1}) (tp_j + tp_{j-1}) in uint64;
+ *   one all-reduce completes it, and *auc = ((double)area2 * 0.5) / ((double)P * (double)N), NaN when P or N is 0.
+ *   NVLink traffic: 12 bytes per run a rank sends (a tie group of scores on a rank is one run), plus four all-gathers
+ *   of at most 256 bytes per rank (the agreement's included) and one 8-byte all-reduce.  Device scratch per rank: about 40 bytes per sample while the
+ *   runs are built, then 40 bytes per received run.
+ *
+ * ctr_group_auc_dist: *gauc, *n_groups, *n_used and the per-group outputs equal ctr_group_auc on the concatenation bit
+ *   for bit, the compensated sum included.  Each rank sorts records (group, score key and label; 16 bytes) by group,
+ *   the records of each group range go to one rank, so every group lives whole on one rank, and each rank runs
+ *   ctr_group_auc's grouped driver on its groups.  The groups' terms (group id, n_g, P_g, area2_g; 24 bytes a group) are
+ *   all-gathered in rank order, which is ascending group order, and every rank folds them as ctr_group_auc does.
+ *   NVLink traffic: 16 bytes per sample that changes rank, 24 bytes per group to every rank, and four all-gathers of
+ *   at most 256 bytes per rank.  Device scratch: about
+ *   56 bytes per own sample while sorting, then ctr_group_auc's 100 bytes per received sample, then 24 bytes per group
+ *   of all ranks.  A group is never split, so one group holding most samples puts them all on one rank; more than
+ *   2^31 - 1 samples on one rank, or more than 2^31 - 1 groups in all, is CTR_EINVAL on every rank.
+ *   out_group, out_n, out_pos and out_auc may each be NULL and receive the first *n_groups groups in ascending group
+ *   order; a non-NULL array with cap < *n_groups is CTR_EINVAL, decided once the group count is known and before
+ *   anything is written. */
+int ctr_roc_auc_dist(ctr_handle* h, const float* pred, const float* y, int64_t n, double* auc);
+int ctr_group_auc_dist(ctr_handle* h, const float* pred, const float* y, const int64_t* group, int64_t n,
+                       double* gauc, int64_t* n_groups, int64_t* n_used,
+                       int64_t cap, int64_t* out_group, int32_t* out_n, int32_t* out_pos, double* out_auc);
 
 /* The curves and average precision of nn/metrics/ranking.go, on the device.  All four follow binaryClfCurve
  * (ranking.go:13-57): scores ordered as ctr_roc_auc orders them (descending; -0 and +0 one threshold group; every NaN
